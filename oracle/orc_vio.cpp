@@ -204,7 +204,9 @@ void VIOManager::warpAffine(const M2 &A_cur_ref, const Image &img_ref, const V2 
       pp0 *= (1 << pyramid_level), pp1 *= (1 << pyramid_level);
       const float px0 = (A00 * pp0 + A01 * pp1) + pxr0;
       const float px1 = (A10 * pp0 + A11 * pp1) + pxr1;
-      if (px0 < 0 || px1 < 0 || px0 >= img_ref.cols - 1 || px1 >= img_ref.rows - 1)
+      // the reference's in-frame test (:312) written so that a NaN position (singular A with non-zero entries: inf * 0 or
+      // inf - inf) counts as outside; the reference would hand NaN to vk::interpolateMat_8u and read out of bounds
+      if (!(px0 >= 0 && px1 >= 0 && px0 < img_ref.cols - 1 && px1 < img_ref.rows - 1))
         patch_ptr[patch_size_total * pyramid_level + y * patch_size + x] = 0;
       else
         patch_ptr[patch_size_total * pyramid_level + y * patch_size + x] = (float)interpolateMat_8u(img_ref, px0, px1);

@@ -342,3 +342,45 @@ def test_numpy_restatement_of_the_inverse_compositional_variant(small_vio_frame)
     vio.set_inverse(False)
     fwd = vio.update(fr["img"], pos, wp, np.zeros(n, np.int32), np.ones(n), fr["state_prior"], fr["state_prior"])
     assert fwd["HTH"][level][0][6, 6] > 0  # the forward variant is untouched by the switch
+
+
+def _numpy_image_patch(img, pc, level):
+    """getImagePatch (vio.cpp:203-225) restated in numpy float32 scalars: linear addressing img.data + offset, with the
+    documented border rule that a read outside [0, w·h) is 0 (DESIGN §4)."""
+    flat = np.ascontiguousarray(img).ravel()
+    npix, w = flat.size, img.shape[1]
+    s = 1 << level
+    u, v = f32(pc[0]), f32(pc[1])
+    ui, vi = int(np.floor(f32(pc[0] / s)) * f32(s)), int(np.floor(f32(pc[1] / s)) * f32(s))
+    su, sv = f32(u - f32(ui)) / f32(s), f32(v - f32(vi)) / f32(s)
+    w_tl, w_tr = f32((1.0 - float(su)) * (1.0 - float(sv))), f32(float(su) * (1.0 - float(sv)))
+    w_bl, w_br = f32((1.0 - float(su)) * float(sv)), su * sv
+
+    def tap(i):
+        return f32(flat[i]) if 0 <= i < npix else f32(0)
+
+    out = np.zeros(64, f32)
+    for x in range(8):
+        for y in range(8):
+            b = (vi - 4 * s + x * s) * w + (ui - 4 * s) + y * s
+            out[8 * x + y] = w_tl * tap(b) + w_tr * tap(b + s) + w_bl * tap(b + s * w) + w_br * tap(b + s * w + s)
+    return out
+
+
+def test_numpy_image_patch_with_the_tap_rule_agrees_with_cpp_oracle_at_the_border(small_vio_frame):
+    """Edge, corner and just-outside pixels at levels 0..3, including reads beyond the image buffer (where the reference
+    itself is undefined and the zero rule is the oracle's own): bit for bit."""
+    import vio_border as VB
+
+    fr = small_vio_frame
+    cam, L = fr["cam_cfg"], fr["vio_cfg"].levels
+    ins, outs = VB.edge_pixels(cam.width, cam.height, L, np.random.default_rng(7), n_mid=1)
+    pcs = np.concatenate([ins, outs])
+    vio = O.OracleVIO(cam, fr["ext"], fr["vio_cfg"])
+    beyond = 0
+    for pc in pcs:
+        for lvl in range(L):
+            np.testing.assert_array_equal(vio.get_image_patch(fr["img"], pc, lvl), _numpy_image_patch(fr["img"], pc, lvl), err_msg=f"{pc} level {lvl}")
+            _, _, y0, y1 = VB.footprint_box(pc[None], 1 << lvl)  # getImagePatch reads one stride less: rows y0 + s .. y1 - s
+            beyond += bool(y0[0] + (1 << lvl) < 0 or y1[0] - (1 << lvl) > cam.height - 1)
+    assert beyond >= 50, beyond  # patches with reads outside [0, w·h)

@@ -18,6 +18,7 @@ import numpy as np
 import pytest
 
 import oracle_bind as O
+import vio_border as VB
 from conftest import get_frame
 from fast_livo2_b200 import synthetic as S
 from parity_util import assert_state_close
@@ -168,3 +169,90 @@ def test_oracle_reproduces_the_reference_source_on_the_baseline_configs(name):
     assert want_vio < 0 or ov["total_iters"] == want_vio
     assert_state_close(ov["state"], rv["state"], rot_tol=1e-11, pos_tol=1e-11, cov_tol=1e-9, rest_tol=1e-11)
     np.testing.assert_allclose(ov["errors"], rv["errors"], rtol=1e-6, atol=1e-4)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# The border rule (DESIGN §4): taps use the reference's linear addressing and read 0 outside [0, w·h). Where the reference is
+# well defined — a footprint that wraps to the neighbouring row but stays inside the buffer, and warpAffine's explicit
+# in-frame test — the oracle must reproduce it bit for bit. Beyond the buffer the reference reads outside img.data
+# (undefined), so those cases are checked against the oracle only (tests/test_oracle_numpy_crosscheck.py, tests/test_gpu_vio_border.py).
+BORDER_FRAME = dict(seed=2, n_pts=2000, n_map=120_000, n_patches=250, scene_scale=0.5)
+
+
+def warp_affine_border_cases(cols, rows):
+    """(A_cur_ref, px_ref, search_level) whose warpAffine samples fall on both sides of 0 / cols-1 / rows-1 and exactly on
+    them: dyadic matrices (exact inverses and determinants, so the sample positions are exact) around reference pixels at
+    integer and half-integer distances from the edges, plus a zero matrix (NaN inverse: the patch is left untouched)."""
+    mats = [np.eye(2), 2.0 * np.eye(2), 0.5 * np.eye(2), np.array([[1.25, -0.5], [0.5, 1.25]]), np.array([[1.0, 0.5], [0.25, 1.0]])]
+    pxs = [(cols - 4.0, 200.0), (cols - 3.5, 300.5), (cols - 1.0, 250.25), (cols - 1.5, 260.0), (0.0, 220.0), (3.0, 230.5), (0.5, 240.0),
+           (320.0, rows - 4.0), (321.5, rows - 2.5), (300.25, rows - 1.0), (310.0, 0.0), (305.5, 2.0), (cols - 3.0, rows - 3.0), (2.0, 1.0),
+           (cols - 1.0, rows - 1.0), (0.0, 0.0)]
+    cases = [(A, np.array(px), sl) for sl in range(3) for A in mats for px in pxs]
+    cases.append((np.zeros((2, 2)), np.array([cols - 4.0, 200.0]), 0))
+    return cases
+
+
+def _border_inputs(in_buffer_only):
+    fr = get_frame(**BORDER_FRAME)
+    prior = _prior(fr)
+    return fr, prior, VB.border_patch_set(fr, prior, in_buffer_only=in_buffer_only)
+
+
+@needs_ref
+def test_oracle_image_patch_at_the_border_reproduces_the_reference_source():
+    """getImagePatch (vio.cpp:203-225) at left / right edge pixels, levels 0..3: reads that wrap to the neighbouring row."""
+    fr = get_frame(**BORDER_FRAME)
+    cam, L = fr["cam_cfg"], fr["vio_cfg"].levels
+    pcs, _ = VB.edge_pixels(cam.width, cam.height, L, np.random.default_rng(4))
+    # getImagePatch reads columns x0 + s .. x1 - s of updateState's footprint box
+    wraps = sum(int(((x0 + (1 << l) < 0) | (x1 - (1 << l) > cam.width - 1)).sum()) for l in range(L)
+                for x0, x1, _, _ in [VB.footprint_box(pcs, 1 << l)])
+    assert wraps >= 60, wraps  # patch reads that leave the image row (counted here, independently of both sides)
+
+    def ref():
+        r = O.RefVIO(cam, fr["ext"], fr["vio_cfg"])
+        return dict(patch=np.array([[r.get_image_patch(fr["img"], pc, lvl) for lvl in range(L)] for pc in pcs]))
+
+    r = PIN.get("border/image_patch", ref, exact=("patch",))
+    orc = O.OracleVIO(cam, fr["ext"], fr["vio_cfg"])
+    assert O.same(np.array([[orc.get_image_patch(fr["img"], pc, lvl) for lvl in range(L)] for pc in pcs]), r, "patch")
+
+
+@needs_ref
+def test_oracle_warp_affine_at_the_border_reproduces_the_reference_source():
+    """warpAffine (vio.cpp:292-318): samples across and exactly on 0 / cols-1 / rows-1, search levels 0..2, all levels."""
+    fr = get_frame(**BORDER_FRAME)
+    cam = fr["cam_cfg"]
+    cases = warp_affine_border_cases(cam.width, cam.height)
+
+    def ref():
+        r = O.RefVIO(cam, fr["ext"], fr["vio_cfg"])
+        return dict(warp=np.array([r.warp_affine(fr["img_ref"], A, px, sl) for A, px, sl in cases]))
+
+    r = PIN.get("border/warp_affine", ref, exact=("warp",))
+    orc = O.OracleVIO(cam, fr["ext"], fr["vio_cfg"])
+    got = np.array([orc.warp_affine(fr["img_ref"], A, px, sl) for A, px, sl in cases])
+    assert O.same(got, r, "warp")
+    assert not got[-1].any()  # singular: untouched
+    # both sides of the limits are really sampled: zeros from the in-frame test next to interpolated values in one patch
+    mixed = sum(bool((g == 0).any() and (g != 0).any()) for g in got)
+    assert mixed >= len(cases) // 3, mixed
+
+
+@needs_ref
+def test_oracle_vio_update_with_border_footprints_reproduces_the_reference_source():
+    """computeJacobianAndUpdateEKF on interior patches plus left / right edge patches whose footprints wrap to the neighbouring
+    row at every stride 1..32 (search levels forced across 0..2), inside the buffer: the tolerances of
+    test_oracle_vio_update_reproduces_the_reference_source."""
+    fr, prior, bs = _border_inputs(in_buffer_only=True)
+    assert bs["n_leave"] >= 30, bs["n_leave"]
+    args = (fr["img"], bs["vis_pos"], bs["warp_patch"], bs["search_levels"], bs["inv_ref_expo"], prior, prior)
+    ref = PIN.get("border/update", lambda: {k: v for k, v in O.RefVIO(fr["cam_cfg"], fr["ext"], fr["vio_cfg"]).update(*args).items() if k in ("state", "errors", "H_T_H")})
+    orc = O.OracleVIO(fr["cam_cfg"], fr["ext"], fr["vio_cfg"]).update(*args)
+    assert orc["total_iters"] >= 4 and (orc["accepted_per_level"] < orc["iters_per_level"]).any()  # real accept / rollback decisions
+    assert_state_close(orc["state"], ref["state"], rot_tol=1e-11, pos_tol=1e-11, cov_tol=1e-9, rest_tol=1e-11)
+    np.testing.assert_allclose(orc["errors"], ref["errors"], rtol=1e-6, atol=1e-4)
+    blocks = orc["HTH"].reshape(-1, 7, 7)
+    blocks = blocks[np.abs(blocks).max(axis=(1, 2)) > 0]
+    want = ref["H_T_H"][:7, :7]
+    assert min(np.abs(b - want).max() / np.abs(want).max() for b in blocks) < 1e-10
