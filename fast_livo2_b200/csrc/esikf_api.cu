@@ -776,6 +776,7 @@ static int lio_fill_args(esikf_ctx *ctx, LioKernelArgs &ka, double *state_ptr) {
   }
   ka.voxel_size_f = (float)ctx->lio_cfg.voxel_size;
   ka.sigma_num = ctx->lio_cfg.sigma_num;
+  ka.prob_sure_sigma = prob_sure_sigma_of(ka.sigma_num);
   ka.match_plane = ctx->match_plane.p, ka.normal_plane = ctx->normal_plane.p, ka.dis_to_plane = ctx->dis.p;
   ka.partials = ctx->partials.p, ka.info = ctx->info.p, ka.ctrl = ctx->ctrl.p;
   return 0;

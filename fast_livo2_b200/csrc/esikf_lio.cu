@@ -53,6 +53,7 @@ struct LioKernelArgs {
   int inv_voxel_exact;
   float voxel_size_f;        // float voxel size that positioned the roots (voxel_map.cpp:534,578-581)
   double sigma_num;
+  double prob_sure_sigma;    // sigma_l up to which a passing candidate's this_prob is known to be > 0 (-1: never, see prob_sure_sigma_of)
   int32_t *match_plane;      // [n_total]
   int32_t *normal_plane;     // [n_total] sticky
   float *dis_to_plane;       // [n_total]
@@ -70,7 +71,7 @@ struct LioCold {
   const HashSlot *slots;
   uint32_t hash_mask;
   float voxel_size_f;
-  double sigma_num;
+  double sigma_num, prob_sure_sigma;
   double voxel_size, inv_voxel_size;
   int inv_voxel_exact, stage_mode;
   double extR[9], extT[3];
@@ -293,10 +294,15 @@ __device__ __forceinline__ double spp_of(const RecHead &h, double cx, double cy,
 __device__ __forceinline__ void rot_t_n(const double *R, const RecHead &h, double &m0, double &m1, double &m2) {
   m0 = R[0] * h.n0 + R[3] * h.n1 + R[6] * h.n2, m1 = R[1] * h.n0 + R[4] * h.n1 + R[7] * h.n2, m2 = R[2] * h.n0 + R[5] * h.n1 + R[8] * h.n2;
 }
-// this_prob of :740 — only needed to arbitrate between several candidates that pass both gates
+// this_prob of :740 — needed to arbitrate between several candidates that pass both gates, and where a lone passing
+// candidate's probability may be 0: the reference chooses a plane only on this_prob > 0 (strict '>' from prob = 0).
 __device__ __forceinline__ double prob_of(double sigma_l, float dis_to_plane) {
   return 1.0 / sqrt(sigma_l) * exp(-0.5 * (double)dis_to_plane * (double)dis_to_plane / sigma_l);
 }
+// A candidate that passes the sigma gate has dis^2 / sigma_l < sigma_num^2. With sigma_num <= 30 and sigma_l <= 1e200 that
+// makes exp(-dis^2 / (2 sigma_l)) > e^-451 and 1 / sqrt(sigma_l) >= 1e-100, so this_prob > 1e-296 > 0: a lone passing
+// candidate wins without evaluating it. Above that (sigma_num ~ 38.6 and more, a legal lio/sigma_num) exp underflows to 0.
+__host__ __device__ inline double prob_sure_sigma_of(double sigma_num) { return sigma_num <= 30.0 ? 1e200 : -1.0; }
 
 // build_single_residual's plane branch (:721-768) for a candidate that is NOT the lane's resident record (extra candidates
 // of sub-divided voxels, neighbour voxels): everything from scratch. bc: body covariance (6), c*: cross-matrix vector.
@@ -377,11 +383,13 @@ __device__ __forceinline__ void pair_of(const PairLayout &L, int k, int &owner, 
 
 // Pass 1 over the extra candidates (sub-divided root voxels) of ALL pending lanes of the warp: which of them pass both
 // gates. Per pending lane: npass = number of passing extras, (fidx, fdis) = the first of them in DFS order. No
-// probabilities: a point whose candidates pass at most once in total needs none (any passing candidate has this_prob > 0
-// and wins, :741-768); only points with two or more passing candidates go through warp_eval_extras_prob.
+// probabilities: a point whose candidates pass at most once in total needs none as long as that candidate's this_prob is
+// sure to be > 0 (prob_sure_sigma_of; it then wins, :741-768). unsure: some passing extra of the warp is not sure of it.
+// Points with two or more passing candidates, or an unsure one, go through warp_eval_extras_prob.
 __device__ __forceinline__ void warp_eval_extras_count(const LioCold &a, const LioSmem &sm, const double (*wslots)[SLOT_D], bool pending, const double pw[3],
-                                                       double cx, double cy, double cz, uint32_t first, uint32_t count, int lane, int &npass, int &fidx, float &fdis) {
-  npass = 0, fidx = -1, fdis = 0.f;
+                                                       double cx, double cy, double cz, uint32_t first, uint32_t count, int lane, int &npass, int &fidx, float &fdis,
+                                                       bool &unsure) {
+  npass = 0, fidx = -1, fdis = 0.f, unsure = false;
   const PairLayout L = pair_layout(pending, count, lane);
   if (!L.mask) return;
   for (int base = 0; base < L.total; base += 32) {
@@ -394,12 +402,13 @@ __device__ __forceinline__ void warp_eval_extras_count(const LioCold &a, const L
     for (int c = 0; c < 3; c++) opw[c] = __shfl_sync(0xffffffffu, pw[c], owner);
     const double ocx = __shfl_sync(0xffffffffu, cx, owner), ocy = __shfl_sync(0xffffffffu, cy, owner), ocz = __shfl_sync(0xffffffffu, cz, owner);
     const uint32_t ofirst = __shfl_sync(0xffffffffu, first, owner);
-    bool pass = false;
+    bool pass = false, sure = true;
     float dis = 0.f;
     if (have) {
       const EvalOut e = eval_cold(reinterpret_cast<const double *>(a.recs + ofirst + cand), opw, &wslots[owner][SL_BC], ocx, ocy, ocz, sm, a.sigma_num);
-      pass = e.pass, dis = e.dis;
+      pass = e.pass, dis = e.dis, sure = e.sigma_l <= a.prob_sure_sigma;
     }
+    if (__any_sync(0xffffffffu, pass && !sure)) unsure = true;
     const int myidx = (int)(ofirst + cand);
     for (unsigned m = L.mask; m; m &= m - 1) {
       const int jl = __ffs(m) - 1;
@@ -462,26 +471,33 @@ __device__ __forceinline__ void warp_eval_extras_prob(const LioCold &a, const Li
 
 // All candidates of one root voxel for the lanes that have one (`act`): the first candidate's result is (pass0, sigma0,
 // sd0, dtp0) — evaluated by the caller, from the slot or cold —, the extras are counted lane-parallel; probabilities are
-// evaluated only where two or more candidates pass. On return best_idx / best_dis hold the winner (or -1).
+// evaluated only where two or more candidates pass or a passing one may have this_prob == 0. On return best_idx / best_dis
+// hold the winner (or -1: none passed, or none with this_prob > 0), passed whether any candidate passed (is_sucess).
 __device__ LIO_COLD void resolve_voxel(const LioCold &a, const LioSmem &sm, const double (*wslots)[SLOT_D], bool act, const double pw[3], double cx, double cy,
                                               double cz, uint32_t first, uint32_t count, bool pass0, double sigma0, float dis0, float dtp0, int lane, int &best_idx,
-                                              float &best_dis) {
+                                              float &best_dis, bool &passed) {
   const bool pend = act && count > 1;
   int npass, fidx;
   float fdis;
-  warp_eval_extras_count(a, sm, wslots, pend, pw, cx, cy, cz, first, count, lane, npass, fidx, fdis);
+  bool unsure;
+  warp_eval_extras_count(a, sm, wslots, pend, pw, cx, cy, cz, first, count, lane, npass, fidx, fdis, unsure);
   const int total = (act && pass0 ? 1 : 0) + npass;
   if (act) {
+    passed = total >= 1;
     if (pass0) best_idx = (int)first, best_dis = dis0;
     else if (total >= 1) best_idx = fidx, best_dis = fdis;
   }
-  const bool slow = pend && total >= 2;
+  unsure = unsure || (pass0 && !(sigma0 <= a.prob_sure_sigma));
+  const bool slow = act && (total >= 2 || (total == 1 && unsure));
   if (__any_sync(0xffffffffu, slow)) {
     Cand best;
     best.prob = 0.0, best.idx = -1, best.dis = 0.f;
-    if (slow && pass0) best.prob = prob_of(sigma0, dtp0), best.idx = (int)first, best.dis = dis0;
+    if (slow && pass0) {
+      const double p0 = prob_of(sigma0, dtp0);
+      if (p0 > best.prob) best.prob = p0, best.idx = (int)first, best.dis = dis0;  // this_prob > prob, prob starting at 0 (:741)
+    }
     warp_eval_extras_prob(a, sm, wslots, slow, pw, cx, cy, cz, first, count, lane, best);
-    if (slow) best_idx = best.idx, best_dis = best.dis;
+    if (slow) best_idx = best.idx, best_dis = best.idx >= 0 ? best.dis : 0.f;
   }
 }
 
@@ -517,7 +533,8 @@ struct AssocOut {
 };
 // Cold part of the association: the extras of sub-divided home voxels, then one neighbour voxel for the lanes whose home
 // voxel gave nothing (voxel_map.cpp:680-691). loc is in voxel units, centre / quarter length in metres: reproduced
-// literally. Called by the whole warp. flags: 1 = extras pending, 2 = home voxel exists, 4 = its first candidate passed.
+// literally. Called by the whole warp. flags: 1 = extras pending, 2 = home voxel exists, 4 = its first candidate passed,
+// 8 = the lane matched its single-candidate home voxel on the hot path.
 __device__ LIO_COLD AssocOut lio_cold_assoc(const LioSmem &sm, int warp, int lane, unsigned flags, float pwx, float pwy, float pwz, uint32_t first, uint32_t count,
                                             double sigma0, float dis0, float dtp0) {
   const LioCold &a = sm.cold;
@@ -528,14 +545,15 @@ __device__ LIO_COLD AssocOut lio_cold_assoc(const LioSmem &sm, int warp, int lan
   const double pw[3] = {(double)pwx, (double)pwy, (double)pwz};
   double cx, cy, cz;
   cross_vec(a.extR, a.extT, px, py, pz, cx, cy, cz);
-  int bi = (pass0 && count == 1) ? (int)first : -1;
-  float bd = (pass0 && count == 1) ? dis0 : 0.f;
-  resolve_voxel(a, sm, sm.rec[warp], pend1, pw, cx, cy, cz, first, count, pass0, sigma0, dis0, dtp0, lane, bi, bd);
+  int bi = (flags & 8u) ? (int)first : -1;
+  float bd = (flags & 8u) ? dis0 : 0.f;
+  bool passed = pass0;  // is_sucess of the home voxel
+  resolve_voxel(a, sm, sm.rec[warp], pend1, pw, cx, cy, cz, first, count, pass0, sigma0, dis0, dtp0, lane, bi, bd, passed);
   uint32_t f2 = 0, c2 = 0;
   bool found2 = false;
   EvalOut e2;
   e2.pass = false, e2.sigma_l = 0.0, e2.dis = 0.f, e2.dis_to_plane = 0.f;
-  if (found_home && bi < 0) {
+  if (found_home && !passed) {  // the neighbour only when no home candidate passed (:674), chosen or not
     const double vsf = (double)a.voxel_size_f;
     const double ql = (double)(a.voxel_size_f / 4.0f);
     long long key[3], nk[3];
@@ -550,7 +568,8 @@ __device__ LIO_COLD AssocOut lio_cold_assoc(const LioSmem &sm, int warp, int lan
     found2 = probe(a.slots, a.hash_mask, nk[0], nk[1], nk[2], f2, c2) && c2 > 0;
     if (found2) e2 = eval_cold(reinterpret_cast<const double *>(a.recs + f2), pw, slot + SL_BC, cx, cy, cz, sm, a.sigma_num);
   }
-  if (__any_sync(0xffffffffu, found2)) resolve_voxel(a, sm, sm.rec[warp], found2, pw, cx, cy, cz, f2, c2, e2.pass, e2.sigma_l, e2.dis, e2.dis_to_plane, lane, bi, bd);
+  if (__any_sync(0xffffffffu, found2))
+    resolve_voxel(a, sm, sm.rec[warp], found2, pw, cx, cy, cz, f2, c2, e2.pass, e2.sigma_l, e2.dis, e2.dis_to_plane, lane, bi, bd, passed);
   AssocOut o;
   o.idx = bi, o.dis = bd;
   return o;
@@ -637,7 +656,7 @@ __device__ LIO_COLD double lio_cold_wgt(LioSmem &sm, int warp, int lane, const d
 __device__ __forceinline__ void lio_init_cold(LioSmem &sm, const LioKernelArgs &a) {
   if (threadIdx.x == 0) {
     LioCold &c = sm.cold;
-    c.recs = a.recs, c.slots = a.slots, c.hash_mask = a.hash_mask, c.voxel_size_f = a.voxel_size_f, c.sigma_num = a.sigma_num;
+    c.recs = a.recs, c.slots = a.slots, c.hash_mask = a.hash_mask, c.voxel_size_f = a.voxel_size_f, c.sigma_num = a.sigma_num, c.prob_sure_sigma = a.prob_sure_sigma;
     c.voxel_size = a.voxel_size, c.inv_voxel_size = a.inv_voxel_size, c.inv_voxel_exact = a.inv_voxel_exact, c.stage_mode = a.stage_mode;
     for (int k = 0; k < 9; k++) c.extR[k] = a.extR[k];
     for (int k = 0; k < 3; k++) c.extT[k] = a.extT[k];
@@ -738,13 +757,14 @@ __device__ __forceinline__ void lio_process_range(const LioKernelArgs &a, LioSme
         sigma0 = sigma_plane(slot, g.e0, g.e1, g.e2) + quad_bc(slot + SL_BC, m0, m1, m2) + sw.x;
         if ((double)g.dis_to_plane < a.sigma_num * sqrt(sigma0)) pass0 = true, dis0 = (float)g.sd, dtp0 = g.dis_to_plane;
       }
-      if (pass0 && count == 1) best_idx = (int)first, best_dis = dis0;
+      // a lone passing candidate wins unless its this_prob is 0 (only possible for a large sigma_num, prob_sure_sigma_of)
+      if (pass0 && count == 1 && (sigma0 <= a.prob_sure_sigma || prob_of(sigma0, dtp0) > 0.0)) best_idx = (int)first, best_dis = dis0;
     }
     const bool pend1 = have0 && count > 1;
-    const bool need_nb = valid && found && !pend1 && best_idx < 0;  // for pend1 lanes: decided after their extras
+    const bool need_nb = valid && found && !pend1 && !pass0;  // for pend1 lanes: decided after their extras
     if (__any_sync(0xffffffffu, pend1 || need_nb)) {  // cold: narrow arguments, everything else comes from shared memory
-      const AssocOut ao = lio_cold_assoc(sm, warp, lane, (pend1 ? 1u : 0u) | ((valid && found) ? 2u : 0u) | (pass0 ? 4u : 0u), (float)pw[0], (float)pw[1], (float)pw[2],
-                                         first, count, sigma0, dis0, dtp0);
+      const AssocOut ao = lio_cold_assoc(sm, warp, lane, (pend1 ? 1u : 0u) | ((valid && found) ? 2u : 0u) | (pass0 ? 4u : 0u) | (best_idx >= 0 ? 8u : 0u),
+                                         (float)pw[0], (float)pw[1], (float)pw[2], first, count, sigma0, dis0, dtp0);
       best_idx = ao.idx, best_dis = ao.dis;
     }
     LIO_PHASE_FENCE();

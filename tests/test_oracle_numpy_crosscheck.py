@@ -3,7 +3,9 @@ iteration: TransformLidar + per-point covariance (voxel_map.cpp:376-390), voxel 
 and max-probability choice (:721-754), Jacobian / R^-1 (:414-458) and the information sums (:464-466). The C++ oracle must
 agree with it point by point — this is what stands in for the golden vectors the reference does not ship."""
 import numpy as np
+import pytest
 
+import lio_assoc
 import oracle_bind as O
 from fast_livo2_b200 import synthetic as S
 
@@ -26,43 +28,12 @@ def _body_cov(p, dept, beam):
     return np.outer(d, d) * float(rv) + A @ (np.eye(2) * dv) @ A.T
 
 
-def _key(pw, vs):
-    loc = np.zeros(3, f32)
-    for j in range(3):
-        loc[j] = f32(pw[j] / vs)
-        if loc[j] < 0:
-            loc[j] = f32(float(loc[j]) - 1.0)
-    return loc, tuple(int(np.trunc(float(x))) for x in loc)
-
-
-def _eval(pl, pw, var, sigma_num):
-    n, c = pl["normal"], pl["center"]
-    pv = np.zeros((6, 6))
-    iu = np.triu_indices(6)
-    pv[iu] = pl["plane_var"]
-    pv = pv + pv.T - np.diag(np.diag(pv))
-    sd = n @ pw + float(pl["d"])
-    dtp = f32(abs(sd))
-    dtc = f32(((c - pw) ** 2).sum())
-    with np.errstate(invalid="ignore"):
-        rd = np.sqrt(f32(dtc - f32(dtp * dtp)))
-    if not (float(rd) <= 3.0 * float(pl["radius"])):
-        return None
-    J = np.concatenate([pw - c, -n])
-    sig = J @ pv @ J + n @ var @ n
-    if not (float(dtp) < sigma_num * np.sqrt(sig)):
-        return None
-    return 1.0 / np.sqrt(sig) * np.exp(-0.5 * float(dtp) * float(dtp) / sig), f32(sd)
-
-
 def _check_one_lio_iteration(fr, pts, state):
     """One LIO pass of the C++ oracle against the numpy restatement, point by point; returns (matched, via neighbour, multi-plane)."""
     cfg, ext, vm = fr["lio_cfg"], fr["ext"], fr["map"]
     st = S.unpack_state(state)
     R, t, P = st["R"], st["p"], st["cov"]
-    roots = {tuple(k): (f, c) for k, f, c in zip(vm["keys"].tolist(), vm["first"], vm["count"])}
-    vsf = float(f32(cfg.voxel_size))
-    ql = float(f32(f32(cfg.voxel_size) / f32(4)))
+    roots = {tuple(k): (int(f), int(c)) for k, f, c in zip(vm["keys"].tolist(), vm["first"], vm["count"])}
     lio = O.OracleLIO(cfg, ext)
     lio.set_map(vm)
     sp = lio.single_pass(pts, state, state)
@@ -78,36 +49,17 @@ def _check_one_lio_iteration(fr, pts, state):
         var = R @ bc @ R.T + (-cm) @ P[0:3, 0:3] @ (-cm).T + P[3:6, 3:6]
         np.testing.assert_allclose(sp["point_w"][i], pw, rtol=0, atol=0)
         np.testing.assert_allclose(sp["var"][i], var, rtol=1e-11, atol=1e-18)
-        loc, key = _key(pw, cfg.voxel_size)
-        best = None
-        if key in roots:
-            f, c = roots[key]
-            n_multi += c > 1
-            for j in range(f, f + c):
-                e = _eval(vm["planes"][j], pw, var, cfg.sigma_num)
-                if e is not None and (best is None or e[0] > best[0]):
-                    best = (e[0], j, e[1])
-            if best is None:
-                nk = list(key)
-                for a in range(3):
-                    center = (0.5 + key[a]) * vsf
-                    if float(loc[a]) > center + ql:
-                        nk[a] += 1
-                    elif float(loc[a]) < center - ql:
-                        nk[a] -= 1
-                if tuple(nk) in roots:
-                    f, c = roots[tuple(nk)]
-                    for j in range(f, f + c):
-                        e = _eval(vm["planes"][j], pw, var, cfg.sigma_num)
-                        if e is not None and (best is None or e[0] > best[0]):
-                            best = (e[0], j, e[1])
-                    n_neigh += best is not None
-        if best is None:
+        # voxel key, gates and the max-probability choice with the neighbour rule (lio_assoc.associate: is_sucess is kept
+        # apart from the chosen plane, the first of equal probabilities wins, a probability of 0 is never chosen)
+        a = lio_assoc.associate(vm, roots, pw, var, cfg.sigma_num, cfg.voxel_size)
+        n_multi += a["home"] and roots[a["key"]][1] > 1
+        n_neigh += a["via"] == "nb"
+        if a["plane"] < 0:
             assert sp["plane"][i] == -1
             continue
         n_match += 1
-        assert sp["plane"][i] == best[1] and sp["dis"][i] == best[2]
-        pl = vm["planes"][best[1]]
+        assert sp["plane"][i] == a["plane"] and sp["dis"][i] == a["dis"]
+        pl = vm["planes"][a["plane"]]
         n, c = pl["normal"], pl["center"]
         pv = np.zeros((6, 6))
         iu = np.triu_indices(6)
@@ -121,7 +73,7 @@ def _check_one_lio_iteration(fr, pts, state):
         np.testing.assert_allclose(sp["H"][i], H, rtol=1e-12, atol=1e-15)
         np.testing.assert_allclose(sp["R_inv"][i], rinv, rtol=1e-11)
         HTH += rinv * np.outer(H, H)
-        HTz += rinv * H * (-float(best[2]))
+        HTz += rinv * H * (-float(a["dis"]))
     # the full oracle's first-iteration information matrix over the same points
     r = lio.state_estimation(pts, state, state)
     assert r["M"][0] == n_match
@@ -162,6 +114,22 @@ def test_numpy_restatement_agrees_on_voxel_boundaries_and_negative_keys(small_fr
     assert (pts < 0).any() and (pts > 0).any()
     n_match, n_neigh, _ = _check_one_lio_iteration(fr, pts, state)
     assert n_match > 20
+
+
+@pytest.mark.parametrize("name", lio_assoc.CASES)
+def test_numpy_restatement_agrees_on_hand_built_association_maps(name):
+    """The hand-built maps of tests/lio_assoc.py (wide and deep octrees, exact ties, neighbour voxels with one to 130 candidates,
+    range-gate boundaries; sigma_num = 40 with passing candidates of probability 0): the oracle's first iteration against
+    the restatement above, point by point; every neighbour-root kind is reached. The reference source is undefined for the zero-probability case (it pushes an
+    uninitialised PointToPlane), so there this restatement and the oracle's documented rule are the references."""
+    fr = lio_assoc.case(name)
+    n_match, n_neigh, n_multi = _check_one_lio_iteration(fr, fr["pts"], fr["state_prior"])
+    assert n_match > 50 and n_multi >= 10
+    if name == "zero_prob":
+        z = np.array([t.startswith("zero_prob") and "ok" not in t for t in fr["tags"]])
+        assert n_match <= len(fr["pts"]) - z.sum()
+    else:
+        assert n_neigh >= 20
 
 
 def test_numpy_restatement_of_one_vio_iteration(small_vio_frame):

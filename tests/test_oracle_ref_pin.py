@@ -123,6 +123,24 @@ def test_edge_scan_oracle_reproduces_the_reference_source(kind):
 
 
 @needs_ref
+@pytest.mark.parametrize("name", ["main", "displaced"])
+def test_hand_built_association_oracle_reproduces_the_reference_source(name):
+    """The hand-built maps of tests/lio_assoc.py: roots with up to 131 candidates in layer-2 / layer-3 leaves, byte-identical
+    planes (exact probability ties, the first in DFS order wins), range-gate failures and one-ulp radius boundaries,
+    neighbour voxels from one to 130 candidates, with ties, without a plane or absent; at the pose the scan was placed at and at a displaced prior. The sigma_num = 40 case of
+    the same file is not pinned here: where a candidate passes with this_prob == 0 the reference pushes an uninitialised
+    PointToPlane, so its output is undefined; the oracle's documented rule (DESIGN §4) and the numpy restatement
+    (test_oracle_numpy_crosscheck.py) are the references there."""
+    import lio_assoc
+
+    fr = lio_assoc.case(name)
+    o = _oracle(fr, fr["lio_cfg"])
+    r = PIN.get(f"assoc/{name}", lambda: _ref_lio(fr, cfg=fr["lio_cfg"]), exact=EXACT)
+    assert r["iters"] == 5
+    _check(o, r, fr["map"]["planes"])
+
+
+@needs_ref
 def test_calc_body_cov_matches_the_reference_source():
     import ctypes as C
 
