@@ -165,7 +165,32 @@ int orc_lio_clear_out_of_map(void *h, int x_max, int x_min, int y_max, int y_min
       ++it;
     }
   }
+  refresh_flat_ids(m);  // StateEstimation on the pruned map reports flat ids of what is left
   return deleted;
+}
+// lio/layer_init_num (include/voxel_map.h:40): points a node of layer k collects before its first fit. n entries; a node of
+// layer k reads entry k, so a map of max_layer L needs L + 1 of them.
+void orc_lio_set_layer_init_num(void *h, const int32_t *lin, int n) {
+  ((VoxelMapManager *)h)->config_setting_.layer_init_num_.assign(lin, lin + n);
+}
+// Every node of every root (DFS pre-order, leaves 0..7), 12 int64 a row: key x y z | layer path | init_octo octo_state
+// update_enable is_plane | new_points temp_points_.size() points_size. Returns the number of nodes; rows beyond cap are not written.
+static void dump_node(const VoxelOctoTree *nd, int64_t path, const VOXEL_LOCATION &key, int64_t *out, int cap, int *n) {
+  if (*n < cap) {
+    int64_t *r = out + (size_t)(*n) * 12;
+    r[0] = key.x, r[1] = key.y, r[2] = key.z, r[3] = nd->layer_, r[4] = path;
+    r[5] = nd->init_octo_, r[6] = nd->octo_state_, r[7] = nd->update_enable_, r[8] = nd->plane_ptr_->is_plane_;
+    r[9] = nd->new_points_, r[10] = (int64_t)nd->temp_points_.size(), r[11] = nd->plane_ptr_->points_size_;
+  }
+  (*n)++;
+  for (int l = 0; l < 8; l++)
+    if (nd->leaves_[l]) dump_node(nd->leaves_[l], path | ((int64_t)l << (3 * nd->layer_)), key, out, cap, n);
+}
+int orc_lio_dump_nodes(void *h, int64_t *out, int cap) {
+  VoxelMapManager *m = (VoxelMapManager *)h;
+  int n = 0;
+  for (auto &kv : m->voxel_map_) dump_node(kv.second, 0, kv.first, out, cap, &n);
+  return n;
 }
 // Two-call flatten: sizes first (planes == NULL), then fill.
 void orc_lio_flatten(void *h, int *n_roots, int *n_planes, int64_t *keys, int32_t *first, int32_t *count, void *planes) {

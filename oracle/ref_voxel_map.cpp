@@ -47,6 +47,10 @@ void pack_state(const StatesGroup &st, double *s) {
 
 extern "C" {
 
+// Version of this driver's C API. tests/oracle_bind.py uses the library live only at this version (an older build, whatever
+// its timestamp, lacks entry points the tests call); the Makefile rebuilds a library that does not export it.
+int ref_lio_driver_version_2(void) { return 2; }
+
 // cfg: voxel_size, max_layer, max_iterations, sigma_num, dept_err, beam_err.
 // Outputs: state_out (386), M_out[8] (effective feature num per iteration, parsed from the reference's own console line,
 // voxel_map.cpp:404-405), iters_out, normals_out (n x 3: pv_list_[i].normal), and the final ptpl_list_ as
@@ -160,12 +164,14 @@ struct RefMap {
     delete mgr;
   }
 };
-// cfg: voxel_size, max_layer, min_eigen_value (planner_threshold_), max_points_num, layer_init_num[0..4]
+// cfg: voxel_size, max_layer, min_eigen_value (planner_threshold_), max_points_num, layer_init_num[0..7] (a node of layer k
+// reads entry k: max_layer up to 7)
 void *ref_map_create(const double *cfg) {
   RefMap *r = new RefMap;
   VoxelMapConfig &c = r->config;
   c.max_voxel_size_ = cfg[0], c.max_layer_ = (int)cfg[1], c.planner_threshold_ = cfg[2], c.max_points_num_ = (int)cfg[3];
-  c.layer_init_num_ = std::vector<int>{(int)cfg[4], (int)cfg[5], (int)cfg[6], (int)cfg[7], (int)cfg[8]};
+  c.layer_init_num_.clear();
+  for (int k = 0; k < 8; k++) c.layer_init_num_.push_back((int)cfg[4 + k]);
   c.max_iterations_ = 5, c.sigma_num_ = 3, c.dept_err_ = 0.02, c.beam_err_ = 0.05, c.is_pub_plane_map_ = false;
   c.sliding_thresh = 8, c.map_sliding_en = false, c.half_map_size = 100;
   r->mgr = new VoxelMapManager(c, r->map);
@@ -251,6 +257,26 @@ void ref_map_flatten(void *h, int *n_roots, int *n_planes, int64_t *keys, int32_
   }
   *n_roots = nr, *n_planes = np;
   if (planes_v) memcpy(planes_v, planes.data(), planes.size() * sizeof(FlatPlane));
+}
+
+// Every node of every root (DFS pre-order, leaves 0..7), 12 int64 a row: key x y z | layer path | init_octo octo_state
+// update_enable is_plane | new_points temp_points_.size() points_size. Returns the number of nodes; rows beyond cap are not written.
+static void ref_dump_node(const VoxelOctoTree *nd, int64_t path, const VOXEL_LOCATION &key, int64_t *out, int cap, int *n) {
+  if (*n < cap) {
+    int64_t *r = out + (size_t)(*n) * 12;
+    r[0] = key.x, r[1] = key.y, r[2] = key.z, r[3] = nd->layer_, r[4] = path;
+    r[5] = nd->init_octo_, r[6] = nd->octo_state_, r[7] = nd->update_enable_, r[8] = nd->plane_ptr_->is_plane_;
+    r[9] = nd->new_points_, r[10] = (int64_t)nd->temp_points_.size(), r[11] = nd->plane_ptr_->points_size_;
+  }
+  (*n)++;
+  for (int l = 0; l < 8; l++)
+    if (nd->leaves_[l]) ref_dump_node(nd->leaves_[l], path | ((int64_t)l << (3 * nd->layer_)), key, out, cap, n);
+}
+int ref_map_dump_nodes(void *h, int64_t *out, int cap) {
+  RefMap *r = static_cast<RefMap *>(h);
+  int n = 0;
+  for (const auto &kv : r->mgr->voxel_map_) ref_dump_node(kv.second, 0, kv.first, out, cap, &n);
+  return n;
 }
 
 // calcBodyCov of the reference (voxel_map.cpp:15-34) for one point.

@@ -5,6 +5,7 @@ import ctypes as C
 import numpy as np
 
 import __graft_entry__
+import oracle_bind as O
 from fast_livo2_b200.synthetic import PLANE_DTYPE
 
 SO = __graft_entry__.MAP_HARNESS_LIB
@@ -25,9 +26,9 @@ class HostMap:
         self.lib.maph_usage.argtypes = [C.c_void_p, C.c_void_p]
         self.lib.maph_destroy.argtypes = [C.c_void_p]
         self.lib.maph_slide.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-        lin = np.zeros(8, np.int32)
-        lin[:len(cfg.layer_init_num)] = cfg.layer_init_num
-        lin[len(cfg.layer_init_num):] = cfg.layer_init_num[-1]
+        self.lib.maph_dump_nodes.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+        self.lib.maph_slots_used.argtypes = [C.c_void_p]
+        lin = O.layer_init_num8(cfg)
         self.h = self.lib.maph_create(cfg.voxel_size, cfg.min_eigen_value, cfg.max_layer, cfg.max_points_num, lin.ctypes.data, hash_cap, node_cap, pool_cap, rec_cap)
 
     def __del__(self):
@@ -53,6 +54,13 @@ class HostMap:
         lo, hi = np.ascontiguousarray(lo, np.int64), np.ascontiguousarray(hi, np.int64)
         return self.lib.maph_slide(self.h, lo.ctypes.data, hi.ctypes.data)
 
+    def dump_nodes(self):
+        """Every octree node (oracle_bind.NODE_COLS), roots in key order, nodes in DFS pre-order."""
+        return O._dump_nodes(lambda out, cap: self.lib.maph_dump_nodes(self.h, out.ctypes.data, cap))
+
+    def slots_used(self):
+        return self.lib.maph_slots_used(self.h)
+
     def usage(self):
         u = np.zeros(4, np.int64)
         self.lib.maph_usage(self.h, u.ctypes.data)
@@ -71,12 +79,20 @@ def compare_flat_maps(a, b, rtol=1e-9, what=("a", "b"), exact=False):
     assert np.array_equal(a["count"][ia], b["count"][ib]), "candidate counts per root differ"
     sel_a = np.concatenate([np.arange(f, f + c) for f, c in zip(a["first"][ia], a["count"][ia])] or [np.zeros(0, np.int64)]).astype(np.int64)
     sel_b = np.concatenate([np.arange(f, f + c) for f, c in zip(b["first"][ib], b["count"][ib])] or [np.zeros(0, np.int64)]).astype(np.int64)
-    pa, pb = a["planes"][sel_a], b["planes"][sel_b]
+    pa, pb = a["planes"][sel_a].copy(), b["planes"][sel_b].copy()
+    # NaN (a plane fitted with two equal smallest eigenvalues keeps 0 / 0 terms in plane_var) must sit in the same fields on
+    # both sides; it then compares equal whatever its payload: the CPU and the GPU need not produce the same NaN bits
+    for f in ("center", "normal", "plane_var", "d", "radius"):
+        na, nb = np.isnan(pa[f]), np.isnan(pb[f])
+        assert np.array_equal(na, nb), f"NaN in different {f} fields of {what[0]} and {what[1]}"
+        pa[f][na], pb[f][nb] = 0, 0
     if exact:  # every byte of every candidate record (centre, normal incl. its sign, plane_var, d, radius, layer, path)
-        bad = np.nonzero(pa.view(np.uint8).reshape(len(pa), -1) != pb.view(np.uint8).reshape(len(pb), -1))[0]
+        bad = np.nonzero(pa.view(np.uint8).reshape(len(pa), pa.dtype.itemsize) != pb.view(np.uint8).reshape(len(pb), pb.dtype.itemsize))[0]
         assert len(bad) == 0, f"{len(np.unique(bad))} of {len(pa)} plane records differ between {what[0]} and {what[1]}"
         return len(pa)
     assert np.array_equal(pa["layer"], pb["layer"]) and np.array_equal(pa["path"], pb["path"]), "candidate order (layer / path) differs"
+    if len(pa) == 0:
+        return 0
     np.testing.assert_allclose(pa["center"], pb["center"], rtol=rtol, atol=1e-12)
     sign = np.sign((pa["normal"] * pb["normal"]).sum(1))
     assert np.all(sign != 0)
@@ -91,3 +107,24 @@ def compare_flat_maps(a, b, rtol=1e-9, what=("a", "b"), exact=False):
     # the refit sums are ill-conditioned where two eigenvalues nearly coincide (1 / (l_min - l_m)): relative to the plane's largest entry
     assert np.max(np.abs(va - vb) / scale) < max(rtol, 1e-7), f"plane_var differs by {np.max(np.abs(va - vb) / scale):.3e} (relative to the largest entry)"
     return len(pa)
+
+
+def compare_node_dumps(a, b, what=("a", "b"), a_releases_cut_lists=False):
+    """Node dumps (oracle_bind.NODE_COLS, roots in key order, DFS pre-order) equal row by row. With a_releases_cut_lists, `a`
+    is the device state machine: it frees the temp_points_ of a node it cut (octo_state 1: a non-plane node above the last
+    layer, which only forwards points and is never fitted again), where the reference keeps the list it distributed. There
+    the list size of `a` must be 0 and the other side's is not compared. Returns the number of nodes."""
+    assert a.shape == b.shape, f"{len(a)} nodes in {what[0]}, {len(b)} in {what[1]}"
+    a, b = a.copy(), b.copy()
+    if a_releases_cut_lists:
+        cut = a[:, 6] == 1
+        assert np.all(a[cut, 10] == 0), f"{what[0]} keeps the list of a cut node"
+        b[cut, 10] = 0
+    bad = np.nonzero(np.any(a != b, axis=1))[0]
+    if len(bad):
+        import oracle_bind as O
+
+        i = bad[0]
+        raise AssertionError(f"{len(bad)} of {len(a)} nodes differ between {what[0]} and {what[1]}; first: " +
+                             ", ".join(f"{c} {x}/{y}" for c, x, y in zip(O.NODE_COLS, a[i], b[i])))
+    return len(a)

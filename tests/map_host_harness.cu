@@ -114,4 +114,39 @@ void maph_usage(void *h, long long *out4) {
   HostMap *m = (HostMap *)h;
   out4[0] = m->counters[0], out4[1] = m->counters[1], out4[2] = (long long)m->counters64[0], out4[3] = m->counters[3];
 }
+// Every node of every root (roots in slot order, nodes in DFS pre-order, leaves 0..7), MAP_DUMP_COLS int64 a row:
+// key x y z | layer path | init_octo octo_state update_enable is_plane | new_points temp_points_.size() points_size.
+// Returns the number of nodes; rows beyond cap are counted, not written.
+#define MAP_DUMP_COLS 12
+static void dump_node(const MapArena &A, int id, long long path, const long long *key, long long *out, int cap, int *n) {
+  const MapNode &nd = A.nodes[id];
+  if (*n < cap) {
+    long long *r = out + (size_t)(*n) * MAP_DUMP_COLS;
+    r[0] = key[0], r[1] = key[1], r[2] = key[2], r[3] = nd.layer, r[4] = path;
+    r[5] = nd.init_octo, r[6] = nd.octo_state, r[7] = nd.update_enable, r[8] = nd.is_plane;
+    r[9] = nd.new_points, r[10] = nd.list_size, r[11] = nd.points_size;
+  }
+  (*n)++;
+  for (int l = 0; l < 8; l++)
+    if (nd.children[l] >= 0) dump_node(A, nd.children[l], path | ((long long)l << (3 * nd.layer)), key, out, cap, n);
+}
+int maph_dump_nodes(void *h, long long *out, int cap) {
+  HostMap *m = (HostMap *)h;
+  int n = 0;
+  for (size_t s = 0; s < m->slots.size(); s++) {
+    if (m->slots[s].key == ESIKF_KEY_EMPTY || m->slot_root[s] < 0) continue;
+    const unsigned long long k = m->slots[s].key;
+    const long long key[3] = {(long long)(k >> 42) - ESIKF_KEY_BIAS, (long long)((k >> 21) & (ESIKF_KEY_RANGE - 1)) - ESIKF_KEY_BIAS,
+                              (long long)(k & (ESIKF_KEY_RANGE - 1)) - ESIKF_KEY_BIAS};
+    dump_node(m->A, m->slot_root[s], 0, key, out, cap, &n);
+  }
+  return n;
+}
+// slots in use (occupied keys, whether or not their root was created)
+int maph_slots_used(void *h) {
+  HostMap *m = (HostMap *)h;
+  int n = 0;
+  for (auto &s : m->slots) n += s.key != ESIKF_KEY_EMPTY;
+  return n;
+}
 }

@@ -39,6 +39,9 @@ def load(kind="parity"):
     lib.orc_lio_tick_build_map.argtypes = [vp, fp, C.c_int, dp]
     lib.orc_lio_tick_update_map.argtypes = [vp, dp, dp]
     lib.orc_lio_flatten.argtypes = [vp, C.POINTER(C.c_int), C.POINTER(C.c_int), i64p, ip, ip, vp]
+    lib.orc_lio_set_layer_init_num.argtypes = [vp, ip, C.c_int]
+    lib.orc_lio_dump_nodes.restype = C.c_int
+    lib.orc_lio_dump_nodes.argtypes = [vp, i64p, C.c_int]
     lib.orc_lio_state_estimation.restype = C.c_double
     lib.orc_lio_state_estimation.argtypes = [vp, fp, C.c_int, dp, dp, dp, ip, ip, fp, dp, dp, dp]
     lib.orc_lio_single_pass.argtypes = [vp, fp, C.c_int, dp, dp, ip, fp, dp, dp, dp, dp]
@@ -90,11 +93,32 @@ def c64(a):
     return np.ascontiguousarray(a, dtype=np.float64)
 
 
+def layer_init_num8(cfg):
+    """lio/layer_init_num as the 8 entries (one per possible layer) every side of the map tests is given: padded with its last."""
+    lin = list(cfg.layer_init_num)
+    return np.array((lin + [lin[-1]] * 8)[:8], np.int32)
+
+
+# one row of a node dump (oracle, reference source, host harness): the state of a VoxelOctoTree node
+NODE_COLS = ("kx", "ky", "kz", "layer", "path", "init_octo", "octo_state", "update_enable", "is_plane", "new_points", "temp_points", "points_size")
+
+
+def _dump_nodes(fill):
+    n = fill(np.zeros((1, 12), np.int64), 0)
+    out = np.zeros((max(n, 1), 12), np.int64)
+    assert fill(out, n) == n
+    out = out[:n]
+    # roots in key order (a stable sort keeps every root's DFS order)
+    return out[np.lexsort((out[:, 2], out[:, 1], out[:, 0]))] if n else out
+
+
 class OracleLIO:
     def __init__(self, lio_cfg, ext, threads=1, kind="parity"):
         self.lib = load(kind)
         self.cfg = lio_cfg
         self.h = self.lib.orc_lio_create(dptr(lio_cfg.as_array()), dptr(c64(ext.extR)), dptr(c64(ext.extT)), threads)
+        lin = layer_init_num8(lio_cfg)
+        self.lib.orc_lio_set_layer_init_num(self.h, iptr(lin), len(lin))
 
     def __del__(self):
         try:
@@ -138,6 +162,10 @@ class OracleLIO:
         planes = np.zeros(npl.value, PLANE_DTYPE)
         self.lib.orc_lio_flatten(self.h, C.byref(nr), C.byref(npl), _p(keys, C.c_int64), iptr(first), iptr(count), planes.ctypes.data)
         return dict(keys=keys, first=first, count=count, planes=planes)
+
+    def dump_nodes(self):
+        """Every octree node (see NODE_COLS), roots in key order, nodes in DFS pre-order."""
+        return _dump_nodes(lambda out, cap: self.lib.orc_lio_dump_nodes(self.h, _p(out, C.c_int64), cap))
 
     def state_estimation(self, pts, state_in, state_prop):
         pts = np.ascontiguousarray(pts, dtype=np.float32)
@@ -294,8 +322,17 @@ def inverse_refs_from_frame(fr):
 REF_LIO_SO = os.path.join(ORACLE_DIR, "_ref", "libfl2_ref_lio.so")
 
 
+REF_LIO_DRIVER = "ref_lio_driver_version_2"  # oracle/ref_voxel_map.cpp's C API version the tests are written against
+_ref_lio_ok = None
+
+
 def ref_lio_available():
-    return os.path.exists(REF_LIO_SO)
+    """The reference-source library exists and was built from the current driver. A library built from an older driver (one
+    that lacks the node dump, say) is not used live: the tests then compare with the stored outputs instead."""
+    global _ref_lio_ok
+    if _ref_lio_ok is None:
+        _ref_lio_ok = os.path.exists(REF_LIO_SO) and hasattr(C.CDLL(REF_LIO_SO), REF_LIO_DRIVER)
+    return _ref_lio_ok
 
 
 def ref_lio_state_estimation(fr, state_in=None, state_prop=None, cfg=None, pts=None, so=None):
@@ -337,8 +374,9 @@ class RefMap:
         self.lib.ref_map_destroy.argtypes = [C.c_void_p]
         self.lib.ref_map_update.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
         self.lib.ref_map_flatten.argtypes = [C.c_void_p] * 7
-        lin = list(cfg.layer_init_num) + [cfg.layer_init_num[-1]] * 5
-        a = c64([cfg.voxel_size, cfg.max_layer, cfg.min_eigen_value, cfg.max_points_num] + lin[:5])
+        self.lib.ref_map_dump_nodes.restype = C.c_int
+        self.lib.ref_map_dump_nodes.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+        a = c64([cfg.voxel_size, cfg.max_layer, cfg.min_eigen_value, cfg.max_points_num] + layer_init_num8(cfg).tolist())
         self.h = self.lib.ref_map_create(a.ctypes.data)
 
     def __del__(self):
@@ -366,6 +404,12 @@ class RefMap:
         planes = np.zeros(npl.value, PLANE_DTYPE)
         self.lib.ref_map_flatten(self.h, C.addressof(nr), C.addressof(npl), keys.ctypes.data, first.ctypes.data, count.ctypes.data, planes.ctypes.data)
         return dict(keys=keys, first=first, count=count, planes=planes)
+
+    def dump_nodes(self):
+        return _dump_nodes(lambda out, cap: self.lib.ref_map_dump_nodes(self.h, out.ctypes.data, cap))
+
+    def clear_out_of_map(self, lo, hi):
+        self.lib.ref_map_clear_out_of_map(C.c_void_p(self.h), int(hi[0]), int(lo[0]), int(hi[1]), int(lo[1]), int(hi[2]), int(lo[2]))
 
 
 # ---------------------------------------------------------------------------------------------------------------------

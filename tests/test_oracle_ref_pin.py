@@ -240,3 +240,28 @@ def test_oracle_build_voxel_map_reproduces_the_reference_source():
         ref.build(scan, st0, ext, cfg)
     n = _compare_map(MB, orc.flatten(), ref, "build_map", ("oracle BuildVoxelMap", "reference source"))
     assert n > 1500
+
+
+@needs_ref
+@pytest.mark.parametrize("name", ["deep_blob_L3", "deep_blob_L7", "deep_cut", "candidates_growth", "candidates_layer3", "layer_init_update", "layer_init_cut",
+                                  "max_points_last_layer", "max_points_cut", "refit_flip", "on_centre", "box_corners", "big_list", "key_edges", "slide"])
+def test_oracle_map_streams_reproduce_the_reference_source(name):
+    """The hand-built streams of tests/map_streams.py (deep octrees, 64 / 72 candidates, per-layer layer_init_num, every
+    max_points_num boundary, refits that flip plane / non-plane, points on split planes, box-corner eigenvalues at the
+    threshold and equal smallest eigenvalues, slides): the oracle's UpdateVoxelMap / clearMemOutOfMap against the REFERENCE
+    SOURCE's after every tick, node by node (every field of the node dump equal) and plane by plane (1e-9; NaN in the same
+    fields). The whole maps are stored: they are small."""
+    import map_bind as MB
+    import map_streams as MS
+
+    c = MS.case(name)
+    o = MS.replay(c, {"orc": MS.OracleSide(c["cfg"])})["orc"]
+    r = MS.replay(c, {"ref": MS.RefSide(c["cfg"])})["ref"] if PIN.live else None
+    for t, x in enumerate(o):
+        for stage in ("", "slid") if "slid" in x else ("",):
+            flat, dump = (x["slid"], x["slid_dump"]) if stage else (x["flat"], x["dump"])
+            key = f"map/{name}/tick{t}{'/' + stage if stage else ''}"
+            y = PIN.get(key, lambda: {**(r[t]["slid"] if stage else r[t]["flat"]), "dump": r[t]["slid_dump"] if stage else r[t]["dump"]})
+            what = (f"oracle, tick {t} {stage}", "reference source")
+            MB.compare_node_dumps(dump, y["dump"], what)
+            MB.compare_flat_maps(flat, {k: y[k] for k in ("keys", "first", "count", "planes")}, rtol=1e-9, what=what)
