@@ -57,9 +57,16 @@ struct SolveLiteralScratch {
   double K[19 * 19];
 };
 
+// |v| as the reference evaluates it, (v0 v0 + v1 v1) + v2 v2 with every product rounded: a contracted (FMA) sum can land on
+// the other side of a threshold (Exp's 1e-5, the convergence rules) than the reference's, which changes the branch taken
+// or the iteration count.
+__device__ __forceinline__ double norm3_rn(const double *v) {
+  return sqrt(__dadd_rn(__dadd_rn(__dmul_rn(v[0], v[0]), __dmul_rn(v[1], v[1])), __dmul_rn(v[2], v[2])));
+}
+
 // Exp(v) of include/utils/so3_math.h:44-58 (identity when |v| <= 1e-5)
 __device__ inline void so3_exp(const double v[3], double E[9]) {
-  double nrm = sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+  const double nrm = norm3_rn(v);
   for (int i = 0; i < 9; i++) E[i] = (i % 4 == 0) ? 1.0 : 0.0;
   if (nrm > 0.00001) {
     double r[3] = {v[0] / nrm, v[1] / nrm, v[2] / nrm};
@@ -234,7 +241,7 @@ __device__ inline void gain_rows(SolveSmem &sm, double pscale, int solve_mode, i
   for (int i = 0; i < m; i++) x[i] = __shfl_sync(0xffffffffu, col[i], (lane + m) & 31);
 }
 
-__device__ inline double warp_norm3(const double *v) { return sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]); }
+__device__ inline double warp_norm3(const double *v) { return norm3_rn(v); }
 
 #define SOLVE_THREADS 512
 
