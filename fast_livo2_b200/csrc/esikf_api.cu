@@ -8,6 +8,8 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <algorithm>
+#include <initializer_list>
 #include <string>
 #include <utility>
 #include <vector>
@@ -60,9 +62,22 @@ static NcclApi g_nccl;
 enum { NCCL_FLOAT64 = 8, NCCL_SUM = 0 };
 
 // ---------------------------------------------------------------------------------------------------------------------
+// Device allocation owned by its holder: freed on destruction, moved but never copied.
 template <typename T> struct DevBuf {
   T *p = nullptr;
   size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf &) = delete;
+  DevBuf &operator=(const DevBuf &) = delete;
+  DevBuf(DevBuf &&o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr, o.cap = 0; }
+  DevBuf &operator=(DevBuf &&o) noexcept {
+    std::swap(p, o.p), std::swap(cap, o.cap);  // the old allocation leaves with `o`
+    return *this;
+  }
+  ~DevBuf() {
+    if (p) cudaFree(p);
+  }
+  // grow to at least n elements (with headroom); the old contents are discarded
   cudaError_t reserve(size_t n) {
     if (n <= cap) return cudaSuccess;
     if (p) cudaFree(p);
@@ -72,9 +87,38 @@ template <typename T> struct DevBuf {
     if (e == cudaSuccess) cap = want;
     return e;
   }
-  void release() {
-    if (p) cudaFree(p);
-    p = nullptr, cap = 0;
+};
+
+// The buffers of one device-map arena (MapArena, esikf_map.cuh) and the capacities they were reserved for. The slots,
+// planes and recs buffers of the live arena also hold a host-uploaded map (esikf_map_upload).
+struct MapArenaBufs {
+  DevBuf<HashSlot> slots;
+  DevBuf<int> slot_root, slot_cap;
+  DevBuf<MapNode> nodes;
+  DevBuf<double> pool;
+  DevBuf<PlaneRec> recs;
+  DevBuf<esikf_plane> planes;
+  DevBuf<int> rec_node, counters;
+  DevBuf<unsigned long long> counters64;
+  uint32_t hash_cap = 0;
+  int node_cap = 0, rec_cap = 0;
+  long long pool_cap = 0;  // points
+  cudaError_t reserve(uint32_t hash_cap_, int node_cap_, int rec_cap_, long long pool_cap_) {
+    cudaError_t e;
+    if ((e = slots.reserve(hash_cap_)) || (e = slot_root.reserve(hash_cap_)) || (e = slot_cap.reserve(hash_cap_)) || (e = nodes.reserve((size_t)node_cap_)) ||
+        (e = pool.reserve((size_t)pool_cap_ * MAP_PT_D)) || (e = recs.reserve((size_t)rec_cap_)) || (e = planes.reserve((size_t)rec_cap_)) ||
+        (e = rec_node.reserve((size_t)rec_cap_)) || (e = counters.reserve(8)) || (e = counters64.reserve(2)))
+      return e;
+    hash_cap = hash_cap_, node_cap = node_cap_, rec_cap = rec_cap_, pool_cap = pool_cap_;
+    return cudaSuccess;
+  }
+  MapArena view(const MapCfg &cfg) const {
+    MapArena A;
+    A.slots = slots.p, A.hash_mask = hash_cap - 1, A.slot_root = slot_root.p, A.slot_cap = slot_cap.p;
+    A.nodes = nodes.p, A.node_cap = node_cap, A.pool = pool.p, A.pool_cap = pool_cap;
+    A.recs = recs.p, A.planes = planes.p, A.rec_node = rec_node.p, A.rec_cap = rec_cap;
+    A.counters = counters.p, A.counters64 = counters64.p, A.cfg = cfg;
+    return A;
   }
 };
 
@@ -100,11 +144,10 @@ struct esikf_ctx {
   bool have_ext = false, have_ext_dev = false;
   double ext_host[12] = {};
 
-  // map
-  DevBuf<HashSlot> slots;
+  // map: map.slots / map.planes (the map as uploaded, 256-byte records) / map.recs (what the residual kernel reads, 144-byte
+  // records derived on the device) serve both the host-uploaded and the device-resident map
+  MapArenaBufs map;
   uint32_t hash_mask = 0;
-  DevBuf<esikf_plane> planes;   // the map as uploaded (256-byte records)
-  DevBuf<PlaneRec> recs;        // what the residual kernel reads (144-byte records derived on the device)
   DevBuf<int32_t> patch_ids;
   int n_planes = 0, n_roots = 0;
   double voxel_size = 0.5;
@@ -113,22 +156,13 @@ struct esikf_ctx {
   // device-resident map (esikf_map_device_*): octree nodes, point lists and refits stay on the GPU
   bool dev_map = false;
   esikf_map_cfg map_cfg{};
-  MapArena arena{};
-  DevBuf<int> map_slot_root, map_slot_cap, map_rec_node, map_counters, map_work;
-  DevBuf<unsigned long long> map_counters64;
-  DevBuf<MapNode> map_nodes;
-  DevBuf<double> map_pool, map_pt, map_pt_normal;
+  MapCfg arena_cfg{};
+  MapArenaBufs spare;  // esikf_map_device_slide copies the surviving roots into it, then it and `map` change roles
+  DevBuf<int> map_work, map_survivors;
+  DevBuf<double> map_pt, map_pt_normal;
   DevBuf<unsigned int> map_key_in, map_key_out, map_idx_in, map_idx_out;
   DevBuf<MapTouched> map_touched;
   DevBuf<unsigned char> map_sort_tmp;
-  // second arena: esikf_map_device_slide copies the surviving roots into it, then the two change roles
-  DevBuf<HashSlot> slots2;
-  DevBuf<esikf_plane> planes2;
-  DevBuf<PlaneRec> recs2;
-  DevBuf<int> map_slot_root2, map_slot_cap2, map_rec_node2, map_counters2, map_survivors;
-  DevBuf<unsigned long long> map_counters64_2;
-  DevBuf<MapNode> map_nodes2;
-  DevBuf<double> map_pool2;
   int map_pt_n = 0;            // points the normal snapshot / last map step covers
   bool map_normals_valid = false;
   int map_hash_bits = 0;
@@ -147,7 +181,7 @@ struct esikf_ctx {
 
   // shared update state
   DevBuf<double> state_prop;             // [state 386 | prop 386] contiguous: one H2D copy per update
-  struct { double *p; } state, prop;
+  double *state = nullptr, *prop = nullptr;
   DevBuf<double> info, partials, old_state, G;
   // pinned staging ring for the two packed states of an update (slot reuse guarded by an event)
   enum { STAGE_SLOTS = 16 };
@@ -158,9 +192,9 @@ struct esikf_ctx {
   unsigned launch_parity = 0;            // the persistent kernels alternate between two grid-barrier counters
   DevBuf<unsigned char> ctl_block;  // [esikf_lio_stats | Ctrl | 64 B pad | esikf_vio_stats]; initialised by CTA 0 of the persistent kernels,
                                     // by a memset on the per-iteration launch path
-  struct { Ctrl *p; } ctrl;
-  struct { esikf_lio_stats *p; } lio_stats;
-  struct { esikf_vio_stats *p; } vio_stats;
+  esikf_lio_stats *lio_stats = nullptr;
+  Ctrl *ctrl = nullptr;
+  esikf_vio_stats *vio_stats = nullptr;
   int partial_blocks = 0;
 
   // VIO
@@ -182,7 +216,7 @@ struct esikf_ctx {
   DevBuf<int32_t> warp_levels;
   int n_patches = 0;
   // warp producers
-  std::vector<uint8_t *> ref_imgs;
+  std::vector<DevBuf<uint8_t>> ref_imgs;
   DevBuf<const uint8_t *> ref_img_ptrs;
   int ref_w = 0, ref_h = 0;
   DevBuf<int32_t> ref_idx;
@@ -206,6 +240,24 @@ struct esikf_ctx {
   bool lio_timed = false, vio_timed = false;
   DevBuf<uint8_t> flush;
   DevBuf<double> scratch_state, point_cov_tmp;
+
+  MapArena arena() const { return map.view(arena_cfg); }  // the live device map as the kernels see it
+
+  // Runs before the members are destroyed: the stream is drained first, then what is not a DevBuf is released here.
+  ~esikf_ctx() {
+    cudaSetDevice(device);
+    if (stream) cudaStreamSynchronize(stream);
+    if (comm && g_nccl.CommDestroy) g_nccl.CommDestroy(comm);
+    for (size_t r = 0; r < peer_ptrs.size(); r++)
+      if ((int)r != rank && peer_ptrs[r]) cudaIpcCloseMemHandle(peer_ptrs[r]);
+    if (mailbox) cudaFree(mailbox);
+    if (stage) cudaFreeHost(stage);
+    if (stage_ctrl) cudaFreeHost(stage_ctrl);
+    for (cudaEvent_t e : stage_ev)
+      if (e) cudaEventDestroy(e);
+    for (cudaEvent_t e : ev) cudaEventDestroy(e);
+    if (stream) cudaStreamDestroy(stream);
+  }
 };
 
 static int fail(esikf_ctx *c, int code, const char *fmt, ...) {
@@ -269,19 +321,19 @@ int esikf_create(esikf_ctx **out, int device) {
        ctx->barrier.reserve(128) == cudaSuccess;
   if (ok) cudaMemsetAsync(ctx->barrier.p, 0, 128 * sizeof(unsigned int), ctx->stream);
   if (ok) {
-    ctx->state.p = ctx->state_prop.p, ctx->prop.p = ctx->state_prop.p + S_N;
+    ctx->state = ctx->state_prop.p, ctx->prop = ctx->state_prop.p + S_N;
     for (int i = 0; i < esikf_ctx::STAGE_SLOTS; i++) ok = ok && cudaEventCreateWithFlags(&ctx->stage_ev[i], cudaEventDisableTiming) == cudaSuccess;
   }
   if (ok) {
     unsigned char *b = ctx->ctl_block.p;
-    ctx->lio_stats.p = reinterpret_cast<esikf_lio_stats *>(b);
-    ctx->ctrl.p = reinterpret_cast<Ctrl *>(b + sizeof(esikf_lio_stats));
-    ctx->vio_stats.p = reinterpret_cast<esikf_vio_stats *>(b + sizeof(esikf_lio_stats) + sizeof(Ctrl) + 64);
+    ctx->lio_stats = reinterpret_cast<esikf_lio_stats *>(b);
+    ctx->ctrl = reinterpret_cast<Ctrl *>(b + sizeof(esikf_lio_stats));
+    ctx->vio_stats = reinterpret_cast<esikf_vio_stats *>(b + sizeof(esikf_lio_stats) + sizeof(Ctrl) + 64);
     cudaMemsetAsync(b, 0, ctx->ctl_block.cap, ctx->stream);
   }
   cudaDeviceGetAttribute(&ctx->coop_ok, cudaDevAttrCooperativeLaunch, device);
   if (!ok) {
-    esikf_destroy(ctx);
+    delete ctx;
     return ESIKF_ERR_CUDA;
   }
   cudaFuncSetAttribute(lio_residual_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(LioSmem));
@@ -317,38 +369,7 @@ int esikf_create(esikf_ctx **out, int device) {
   return ESIKF_OK;
 }
 
-void esikf_destroy(esikf_ctx *ctx) {
-  if (!ctx) return;
-  cudaSetDevice(ctx->device);
-  if (ctx->stream) cudaStreamSynchronize(ctx->stream);
-  if (ctx->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(ctx->comm);
-  for (size_t r = 0; r < ctx->peer_ptrs.size(); r++)
-    if ((int)r != ctx->rank && ctx->peer_ptrs[r]) cudaIpcCloseMemHandle(ctx->peer_ptrs[r]);
-  if (ctx->mailbox) cudaFree(ctx->mailbox);
-  ctx->peer_ptrs_dev.release();
-  ctx->slots.release(), ctx->planes.release(), ctx->recs.release(), ctx->patch_ids.release(), ctx->pts.release(), ctx->pre.release(), ctx->match_plane.release();
-  ctx->normal_plane.release(), ctx->dis.release(), ctx->ext_dev.release(), ctx->state_prop.release();
-  ctx->map_slot_root.release(), ctx->map_slot_cap.release(), ctx->map_rec_node.release(), ctx->map_counters.release(), ctx->map_work.release(), ctx->map_counters64.release();
-  ctx->map_nodes.release(), ctx->map_pool.release(), ctx->map_pt.release(), ctx->map_pt_normal.release(), ctx->map_key_in.release(), ctx->map_key_out.release();
-  ctx->map_idx_in.release(), ctx->map_idx_out.release(), ctx->map_touched.release(), ctx->map_sort_tmp.release();
-  ctx->slots2.release(), ctx->planes2.release(), ctx->recs2.release(), ctx->map_slot_root2.release(), ctx->map_slot_cap2.release(), ctx->map_rec_node2.release();
-  ctx->map_counters2.release(), ctx->map_survivors.release(), ctx->map_counters64_2.release(), ctx->map_nodes2.release(), ctx->map_pool2.release();
-  if (ctx->stage) cudaFreeHost(ctx->stage);
-  if (ctx->stage_ctrl) cudaFreeHost(ctx->stage_ctrl);
-  for (int i = 0; i < esikf_ctx::STAGE_SLOTS; i++)
-    if (ctx->stage_ev[i]) cudaEventDestroy(ctx->stage_ev[i]);
-  ctx->info.release(), ctx->partials.release(), ctx->old_state.release(), ctx->G.release(), ctx->ctl_block.release();
-  ctx->stamps.release(), ctx->barrier.release(), ctx->img.release(), ctx->vis_pos.release(), ctx->inv_expo.release();
-  ctx->warp_patch.release(), ctx->errors.release(), ctx->search_levels.release(), ctx->ref_img_ptrs.release(), ctx->ref_idx.release();
-  ctx->px_ref.release(), ctx->pos_w.release(), ctx->normal_w.release(), ctx->T_ref.release(), ctx->T_cur.release();
-  ctx->warp_out.release(), ctx->warp_levels.release();
-  ctx->inv_ref_px.release(), ctx->inv_ref_f.release(), ctx->inv_ref_R.release(), ctx->inv_ref_pos.release(), ctx->H_sub_inv.release(), ctx->inv_ref_idx.release();
-  ctx->A_cur_ref.release(), ctx->pc_buf.release(), ctx->patch_buf.release(), ctx->flush.release(), ctx->scratch_state.release(), ctx->point_cov_tmp.release();
-  for (uint8_t *p : ctx->ref_imgs) cudaFree(p);
-  for (cudaEvent_t e : ctx->ev) cudaEventDestroy(e);
-  if (ctx->stream) cudaStreamDestroy(ctx->stream);
-  delete ctx;
-}
+void esikf_destroy(esikf_ctx *ctx) { delete ctx; }
 
 const char *esikf_last_error(const esikf_ctx *ctx) { return ctx ? ctx->err.c_str() : "null context"; }
 void *esikf_stream(esikf_ctx *ctx) { return ctx ? (void *)ctx->stream : nullptr; }
@@ -436,13 +457,13 @@ int esikf_map_upload(esikf_ctx *ctx, const int64_t *keys, const int32_t *first, 
     }
     table[s].key = k, table[s].first = (uint32_t)first[r], table[s].count = (uint32_t)count[r];
   }
-  CK(ctx->slots.reserve(cap));
-  CK(ctx->planes.reserve((size_t)n_planes + 1));
-  CK(ctx->recs.reserve((size_t)n_planes + 1));
-  CK(cudaMemcpyAsync(ctx->slots.p, table.data(), cap * sizeof(HashSlot), cudaMemcpyHostToDevice, ctx->stream));
+  CK(ctx->map.slots.reserve(cap));
+  CK(ctx->map.planes.reserve((size_t)n_planes + 1));
+  CK(ctx->map.recs.reserve((size_t)n_planes + 1));
+  CK(cudaMemcpyAsync(ctx->map.slots.p, table.data(), cap * sizeof(HashSlot), cudaMemcpyHostToDevice, ctx->stream));
   if (n_planes) {
-    CK(cudaMemcpyAsync(ctx->planes.p, planes, (size_t)n_planes * sizeof(esikf_plane), cudaMemcpyHostToDevice, ctx->stream));
-    plane_compact_kernel<<<(n_planes + 127) / 128, 128, 0, ctx->stream>>>(ctx->planes.p, nullptr, n_planes, ctx->recs.p);
+    CK(cudaMemcpyAsync(ctx->map.planes.p, planes, (size_t)n_planes * sizeof(esikf_plane), cudaMemcpyHostToDevice, ctx->stream));
+    plane_compact_kernel<<<(n_planes + 127) / 128, 128, 0, ctx->stream>>>(ctx->map.planes.p, nullptr, n_planes, ctx->map.recs.p);
     ctx->launches++;
   }
   CK(cudaStreamSynchronize(ctx->stream));
@@ -464,13 +485,13 @@ int esikf_map_patch(esikf_ctx *ctx, const int32_t *plane_ids, const esikf_plane 
   for (int i = 0; i < n;) {
     int j = i + 1;
     while (j < n && plane_ids[j] == plane_ids[j - 1] + 1) j++;  // a run of consecutive ids travels as one copy
-    CK(cudaMemcpyAsync(ctx->planes.p + plane_ids[i], planes + i, (size_t)(j - i) * sizeof(esikf_plane), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->map.planes.p + plane_ids[i], planes + i, (size_t)(j - i) * sizeof(esikf_plane), cudaMemcpyHostToDevice, ctx->stream));
     i = j;
   }
   if (n > 0) {
     CK(ctx->patch_ids.reserve(n));
     CK(cudaMemcpyAsync(ctx->patch_ids.p, plane_ids, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
-    plane_compact_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(ctx->planes.p, ctx->patch_ids.p, n, ctx->recs.p);
+    plane_compact_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(ctx->map.planes.p, ctx->patch_ids.p, n, ctx->map.recs.p);
     ctx->launches++;
   }
   CK(cudaStreamSynchronize(ctx->stream));
@@ -481,14 +502,14 @@ int esikf_map_patch(esikf_ctx *ctx, const int32_t *plane_ids, const esikf_plane 
 static int map_check_errors(esikf_ctx *ctx, const char *what) {
   int c[4];
   unsigned long long pool_used = 0;
-  CK(cudaMemcpyAsync(c, ctx->map_counters.p, sizeof(c), cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(&pool_used, ctx->map_counters64.p, sizeof(pool_used), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(c, ctx->map.counters.p, sizeof(c), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(&pool_used, ctx->map.counters64.p, sizeof(pool_used), cudaMemcpyDeviceToHost, ctx->stream));
   int work[2];
   CK(cudaMemcpyAsync(work, ctx->map_work.p, sizeof(work), cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   ctx->map_last.nodes = c[0], ctx->map_last.records = c[1], ctx->map_last.errors = c[2], ctx->map_last.roots = c[3];
   ctx->map_last.pool_points = (int64_t)pool_used, ctx->map_last.touched_roots = work[0];
-  ctx->n_planes = c[1] < (int)ctx->arena.rec_cap ? c[1] : (int)ctx->arena.rec_cap;
+  ctx->n_planes = c[1] < ctx->map.rec_cap ? c[1] : ctx->map.rec_cap;
   ctx->n_roots = c[3];
   if (c[2]) {
     ctx->have_map = false;  // the map is not trustworthy any more: the next lio_run must not use it
@@ -513,26 +534,13 @@ int esikf_map_device_init(esikf_ctx *ctx, const esikf_map_cfg *cfg) {
   const int64_t rec_cap = cfg->record_capacity > 0 ? cfg->record_capacity : 4 * roots;
   const int64_t pool_cap = cfg->point_capacity > 0 ? cfg->point_capacity : 64 * roots;
   if (node_cap > 0x7fffffff || rec_cap > 0x7fffffff || pool_cap > 0x7fffffff) return fail(ctx, ESIKF_ERR_ARG, "map_device_init: capacity above 2^31");
-  CK(ctx->slots.reserve(cap));
-  CK(ctx->map_slot_root.reserve(cap));
-  CK(ctx->map_slot_cap.reserve(cap));
-  CK(ctx->map_nodes.reserve((size_t)node_cap));
-  CK(ctx->map_pool.reserve((size_t)pool_cap * MAP_PT_D));
-  CK(ctx->recs.reserve((size_t)rec_cap));
-  CK(ctx->planes.reserve((size_t)rec_cap));
-  CK(ctx->map_rec_node.reserve((size_t)rec_cap));
-  CK(ctx->map_counters.reserve(8));
-  CK(ctx->map_counters64.reserve(2));
+  CK(ctx->map.reserve(cap, (int)node_cap, (int)rec_cap, pool_cap));
   CK(ctx->map_work.reserve(4));
-  MapArena &A = ctx->arena;
-  A.slots = ctx->slots.p, A.hash_mask = cap - 1, A.slot_root = ctx->map_slot_root.p, A.slot_cap = ctx->map_slot_cap.p;
-  A.nodes = ctx->map_nodes.p, A.node_cap = (int)node_cap, A.pool = ctx->map_pool.p, A.pool_cap = pool_cap;
-  A.recs = ctx->recs.p, A.planes = ctx->planes.p, A.rec_node = ctx->map_rec_node.p, A.rec_cap = (int)rec_cap;
-  A.counters = ctx->map_counters.p, A.counters64 = ctx->map_counters64.p;
-  A.cfg.voxel_size = (float)cfg->voxel_size, A.cfg.planer_threshold = (float)cfg->min_eigen_value;
-  A.cfg.max_layer = cfg->max_layer, A.cfg.max_points_num = cfg->max_points_num;
-  for (int k = 0; k < MAP_MAX_LAYERS; k++) A.cfg.layer_init_num[k] = cfg->layer_init_num[k <= cfg->max_layer ? k : cfg->max_layer];
-  map_reset_kernel<<<(cap + 255) / 256, 256, 0, ctx->stream>>>(A);
+  MapCfg &mc = ctx->arena_cfg;
+  mc.voxel_size = (float)cfg->voxel_size, mc.planer_threshold = (float)cfg->min_eigen_value;
+  mc.max_layer = cfg->max_layer, mc.max_points_num = cfg->max_points_num;
+  for (int k = 0; k < MAP_MAX_LAYERS; k++) mc.layer_init_num[k] = cfg->layer_init_num[k <= cfg->max_layer ? k : cfg->max_layer];
+  map_reset_kernel<<<(cap + 255) / 256, 256, 0, ctx->stream>>>(ctx->arena());
   CK(cudaMemsetAsync(ctx->map_work.p, 0, 4 * sizeof(int), ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   ctx->launches++;
@@ -550,7 +558,7 @@ int esikf_map_device_init(esikf_ctx *ctx, const esikf_map_cfg *cfg) {
 // sort by slot, list the touched roots, replay them
 static int map_apply_points(esikf_ctx *ctx, int n, bool build) {
   cudaStream_t st = ctx->stream;
-  const unsigned int invalid = ctx->arena.hash_mask + 1u;
+  const unsigned int invalid = ctx->map.hash_cap;
   size_t tmp_bytes = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, ctx->map_key_in.p, ctx->map_key_out.p, ctx->map_idx_in.p, ctx->map_idx_out.p, n, 0, ctx->map_hash_bits + 1, st);
   CK(ctx->map_sort_tmp.reserve(tmp_bytes + 16));
@@ -558,7 +566,7 @@ static int map_apply_points(esikf_ctx *ctx, int n, bool build) {
                                      ctx->map_hash_bits + 1, st));
   CK(cudaMemsetAsync(ctx->map_work.p, 0, 2 * sizeof(int), st));
   map_heads_kernel<<<(n + 255) / 256, 256, 0, st>>>(ctx->map_key_out.p, n, invalid, ctx->map_touched.p, ctx->map_work.p);
-  map_replay_kernel<<<ctx->sm_count * 4, 128, 0, st>>>(ctx->arena, ctx->map_touched.p, ctx->map_work.p, ctx->map_idx_out.p, ctx->map_pt.p, build ? 1 : 0);
+  map_replay_kernel<<<ctx->sm_count * 4, 128, 0, st>>>(ctx->arena(), ctx->map_touched.p, ctx->map_work.p, ctx->map_idx_out.p, ctx->map_pt.p, build ? 1 : 0);
   ctx->launches += 4;
   CK(cudaGetLastError());
   return map_check_errors(ctx, build ? "map_device_build" : "map_device_update");
@@ -587,7 +595,7 @@ static int map_from_scan(esikf_ctx *ctx, const double *state, bool build) {
   int rc = map_reserve_tick(ctx, n);
   if (rc) return rc;
   cudaStream_t st = ctx->stream;
-  const double *dev_state = ctx->state.p;  // the posterior the last update left on the device
+  const double *dev_state = ctx->state;  // the posterior the last update left on the device
   if (state) {
     CK(ctx->scratch_state.reserve(S_N));
     CK(cudaMemcpyAsync(ctx->scratch_state.p, state, S_N * sizeof(double), cudaMemcpyHostToDevice, st));
@@ -598,9 +606,9 @@ static int map_from_scan(esikf_ctx *ctx, const double *state, bool build) {
   a.pts = ctx->pts.p, a.pre = ctx->pre.p, a.pre_stride = ctx->pre_stride, a.n = n, a.state = dev_state;
   memcpy(a.extR, ctx->ext.extR, 72), memcpy(a.extT, ctx->ext.extT, 24);
   a.build = build ? 1 : 0, a.dept_err = (float)ctx->map_cfg.dept_err, a.beam_err = (float)ctx->map_cfg.beam_err;
-  a.match_plane = build ? nullptr : ctx->normal_plane.p, a.recs = ctx->recs.p, a.pt_normal = ctx->map_pt_normal.p;
-  a.pt = ctx->map_pt.p, a.pt_slot = ctx->map_key_in.p, a.pt_idx = ctx->map_idx_in.p, a.invalid_slot = ctx->arena.hash_mask + 1u;
-  map_points_kernel<<<(n + 255) / 256, 256, 0, st>>>(ctx->arena, a);
+  a.match_plane = build ? nullptr : ctx->normal_plane.p, a.recs = ctx->map.recs.p, a.pt_normal = ctx->map_pt_normal.p;
+  a.pt = ctx->map_pt.p, a.pt_slot = ctx->map_key_in.p, a.pt_idx = ctx->map_idx_in.p, a.invalid_slot = ctx->map.hash_cap;
+  map_points_kernel<<<(n + 255) / 256, 256, 0, st>>>(ctx->arena(), a);
   ctx->map_pt_n = n, ctx->map_normals_valid = !build;
   return map_apply_points(ctx, n, build);
 }
@@ -622,7 +630,7 @@ int esikf_map_device_update_points(esikf_ctx *ctx, const double *point_w, const 
   // [n][12] = point_w | var: two strided copies
   CK(cudaMemcpy2DAsync(ctx->map_pt.p, MAP_PT_D * sizeof(double), point_w, 3 * sizeof(double), 3 * sizeof(double), n, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpy2DAsync(ctx->map_pt.p + 3, MAP_PT_D * sizeof(double), var, 9 * sizeof(double), 9 * sizeof(double), n, cudaMemcpyHostToDevice, st));
-  map_keys_kernel<<<(n + 255) / 256, 256, 0, st>>>(ctx->arena, ctx->map_pt.p, n, ctx->map_key_in.p, ctx->map_idx_in.p, ctx->arena.hash_mask + 1u);
+  map_keys_kernel<<<(n + 255) / 256, 256, 0, st>>>(ctx->arena(), ctx->map_pt.p, n, ctx->map_key_in.p, ctx->map_idx_in.p, ctx->map.hash_cap);
   ctx->launches++;
   ctx->map_normals_valid = false;
   return map_apply_points(ctx, n, false);
@@ -634,22 +642,11 @@ int esikf_map_device_slide(esikf_ctx *ctx, const int64_t key_min[3], const int64
   if (!ctx->dev_map) return fail(ctx, ESIKF_ERR_STATE, "map_device_slide before esikf_map_device_init");
   CK(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
-  const MapArena S = ctx->arena;
-  const unsigned cap = S.hash_mask + 1u;
-  CK(ctx->slots2.reserve(cap));
-  CK(ctx->map_slot_root2.reserve(cap));
-  CK(ctx->map_slot_cap2.reserve(cap));
-  CK(ctx->map_nodes2.reserve((size_t)S.node_cap));
-  CK(ctx->map_pool2.reserve((size_t)S.pool_cap * MAP_PT_D));
-  CK(ctx->recs2.reserve((size_t)S.rec_cap));
-  CK(ctx->planes2.reserve((size_t)S.rec_cap));
-  CK(ctx->map_rec_node2.reserve((size_t)S.rec_cap));
-  CK(ctx->map_counters2.reserve(8));
-  CK(ctx->map_counters64_2.reserve(2));
+  const MapArenaBufs &live = ctx->map;
+  const unsigned cap = live.hash_cap;
+  CK(ctx->spare.reserve(cap, live.node_cap, live.rec_cap, live.pool_cap));
   CK(ctx->map_survivors.reserve((size_t)(ctx->map_last.roots > 0 ? ctx->map_last.roots : 1) + 1));
-  MapArena D = S;
-  D.slots = ctx->slots2.p, D.slot_root = ctx->map_slot_root2.p, D.slot_cap = ctx->map_slot_cap2.p, D.nodes = ctx->map_nodes2.p, D.pool = ctx->map_pool2.p;
-  D.recs = ctx->recs2.p, D.planes = ctx->planes2.p, D.rec_node = ctx->map_rec_node2.p, D.counters = ctx->map_counters2.p, D.counters64 = ctx->map_counters64_2.p;
+  const MapArena S = ctx->arena(), D = ctx->spare.view(ctx->arena_cfg);
   const long long big = 1ll << 40;
   const long long lo[3] = {key_min ? key_min[0] : -big, key_min ? key_min[1] : -big, key_min ? key_min[2] : -big};
   const long long hi[3] = {key_max ? key_max[0] : big, key_max ? key_max[1] : big, key_max ? key_max[2] : big};
@@ -660,10 +657,7 @@ int esikf_map_device_slide(esikf_ctx *ctx, const int64_t key_min[3], const int64
   ctx->launches += 3;
   CK(cudaGetLastError());
   // the fresh arena becomes the map (also when the copy reports an error: the status says so and the map is invalidated)
-  std::swap(ctx->slots, ctx->slots2), std::swap(ctx->map_slot_root, ctx->map_slot_root2), std::swap(ctx->map_slot_cap, ctx->map_slot_cap2);
-  std::swap(ctx->map_nodes, ctx->map_nodes2), std::swap(ctx->map_pool, ctx->map_pool2), std::swap(ctx->recs, ctx->recs2), std::swap(ctx->planes, ctx->planes2);
-  std::swap(ctx->map_rec_node, ctx->map_rec_node2), std::swap(ctx->map_counters, ctx->map_counters2), std::swap(ctx->map_counters64, ctx->map_counters64_2);
-  ctx->arena = D;
+  std::swap(ctx->map, ctx->spare);
   ctx->map_normals_valid = false;  // record positions of the last update are gone
   return map_check_errors(ctx, "map_device_slide");
 }
@@ -694,26 +688,21 @@ int esikf_map_device_download(esikf_ctx *ctx, int64_t *keys, int32_t *first, int
     CK(d_count.reserve(roots_cap));
     CK(d_planes.reserve(planes_cap > 0 ? planes_cap : 1));
   }
-  const unsigned cap = ctx->arena.hash_mask + 1u;
-  map_download_kernel<<<(cap + 255) / 256, 256, 0, st>>>(ctx->arena, fill ? d_keys.p : nullptr, d_first.p, d_count.p, d_planes.p, fill ? roots_cap : 0, fill ? planes_cap : 0, d_out.p);
+  const unsigned cap = ctx->map.hash_cap;
+  map_download_kernel<<<(cap + 255) / 256, 256, 0, st>>>(ctx->arena(), fill ? d_keys.p : nullptr, d_first.p, d_count.p, d_planes.p, fill ? roots_cap : 0, fill ? planes_cap : 0, d_out.p);
   ctx->launches++;
   int out[2];
   CK(cudaMemcpyAsync(out, d_out.p, sizeof(out), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   *n_roots = out[0], *n_planes = out[1];
-  int rc = ESIKF_OK;
-  if (fill) {
-    if (out[0] > roots_cap || out[1] > planes_cap)
-      rc = fail(ctx, ESIKF_ERR_ARG, "map_device_download: %d roots / %d planes do not fit the buffers (%d / %d)", out[0], out[1], roots_cap, planes_cap);
-    else {
-      CK(cudaMemcpy(keys, d_keys.p, (size_t)out[0] * 3 * sizeof(int64_t), cudaMemcpyDeviceToHost));
-      CK(cudaMemcpy(first, d_first.p, (size_t)out[0] * sizeof(int32_t), cudaMemcpyDeviceToHost));
-      CK(cudaMemcpy(count, d_count.p, (size_t)out[0] * sizeof(int32_t), cudaMemcpyDeviceToHost));
-      if (out[1]) CK(cudaMemcpy(planes, d_planes.p, (size_t)out[1] * sizeof(esikf_plane), cudaMemcpyDeviceToHost));
-    }
-  }
-  d_keys.release(), d_first.release(), d_count.release(), d_planes.release(), d_out.release();
-  return rc;
+  if (!fill) return ESIKF_OK;
+  if (out[0] > roots_cap || out[1] > planes_cap)
+    return fail(ctx, ESIKF_ERR_ARG, "map_device_download: %d roots / %d planes do not fit the buffers (%d / %d)", out[0], out[1], roots_cap, planes_cap);
+  CK(cudaMemcpy(keys, d_keys.p, (size_t)out[0] * 3 * sizeof(int64_t), cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(first, d_first.p, (size_t)out[0] * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(count, d_count.p, (size_t)out[0] * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  if (out[1]) CK(cudaMemcpy(planes, d_planes.p, (size_t)out[1] * sizeof(esikf_plane), cudaMemcpyDeviceToHost));
+  return ESIKF_OK;
 }
 
 // pv.normal of every point of the last update (voxel_map.cpp:744: the plane that last became the point's best candidate in any
@@ -733,7 +722,7 @@ int esikf_lio_fetch_normals(esikf_ctx *ctx, double *normals) {
   if (n == 0) return ESIKF_OK;
   if (!(ctx->dev_map && ctx->map_normals_valid && ctx->map_pt_n == n)) {
     CK(ctx->map_pt_normal.reserve((size_t)n * 3 + 4));
-    gather_normals_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(ctx->normal_plane.p, ctx->recs.p, n, ctx->map_pt_normal.p);
+    gather_normals_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(ctx->normal_plane.p, ctx->map.recs.p, n, ctx->map_pt_normal.p);
     ctx->launches++;
   }
   CK(cudaMemcpyAsync(normals, ctx->map_pt_normal.p, (size_t)n * 3 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
@@ -763,8 +752,8 @@ static int lio_fill_args(esikf_ctx *ctx, LioKernelArgs &ka, double *state_ptr) {
   ka.pre_stride = ctx->pre_stride;
   ka.partial_stride = ctx->partial_blocks;
   shard_of(ctx->n_pts, ctx->rank, ctx->nranks, ka.begin, ka.count);
-  ka.state = state_ptr, ka.prop = ctx->prop.p;
-  ka.slots = ctx->slots.p, ka.hash_mask = ctx->hash_mask, ka.recs = ctx->recs.p;
+  ka.state = state_ptr, ka.prop = ctx->prop;
+  ka.slots = ctx->map.slots.p, ka.hash_mask = ctx->hash_mask, ka.recs = ctx->map.recs.p;
   ka.stage_mode = (ctx->tuning & ESIKF_TUNE_STAGE_LDG) ? 1 : 0;
   memcpy(ka.extR, ctx->ext.extR, sizeof(ka.extR));
   memcpy(ka.extT, ctx->ext.extT, sizeof(ka.extT));
@@ -778,7 +767,7 @@ static int lio_fill_args(esikf_ctx *ctx, LioKernelArgs &ka, double *state_ptr) {
   ka.sigma_num = ctx->lio_cfg.sigma_num;
   ka.prob_sure_sigma = prob_sure_sigma_of(ka.sigma_num);
   ka.match_plane = ctx->match_plane.p, ka.normal_plane = ctx->normal_plane.p, ka.dis_to_plane = ctx->dis.p;
-  ka.partials = ctx->partials.p, ka.info = ctx->info.p, ka.ctrl = ctx->ctrl.p;
+  ka.partials = ctx->partials.p, ka.info = ctx->info.p, ka.ctrl = ctx->ctrl;
   return 0;
 }
 static int lio_grid(const esikf_ctx *ctx, int count) {
@@ -797,18 +786,50 @@ static int upload_states(esikf_ctx *ctx, const double *state_in, const double *s
   CK(cudaEventRecord(ctx->stage_ev[slot], ctx->stream));
   return ESIKF_OK;
 }
-static PeerArgs peer_args(esikf_ctx *ctx) {
-  PeerArgs p;
-  p.mbox = ctx->p2p ? ctx->peer_ptrs_dev.p : nullptr;
-  p.seq = ctx->peer_seq_dev;
-  p.rank = ctx->rank, p.nranks = ctx->p2p ? ctx->nranks : 1;
-  return p;
-}
 static int allreduce_info(esikf_ctx *ctx) {
   if (ctx->nranks <= 1) return ESIKF_OK;
   if (!ctx->comm) return fail(ctx, ESIKF_ERR_STATE, "per-iteration launches with %d ranks need esikf_comm_init (NCCL)", ctx->nranks);
   int r = g_nccl.AllReduce(ctx->info.p, ctx->info.p, NE_MAX, NCCL_FLOAT64, NCCL_SUM, ctx->comm, ctx->stream);
   if (r != 0) return fail(ctx, ESIKF_ERR_COMM, "ncclAllReduce failed: %s", g_nccl.GetErrorString ? g_nccl.GetErrorString(r) : "?");
+  return ESIKF_OK;
+}
+
+// The SolveArgs fields every solve reads; the LIO / VIO callers add their own.
+static SolveArgs solve_args(const esikf_ctx *ctx, double *state, int max_iterations) {
+  SolveArgs sa;
+  memset(&sa, 0, sizeof(sa));
+  sa.state = state, sa.prop = ctx->prop, sa.info = ctx->info.p, sa.ctrl = ctx->ctrl;
+  sa.max_iterations = max_iterations, sa.solve_mode = ctx->solve_mode;
+  return sa;
+}
+
+// One persistent cooperative kernel per update (coop_blocks: co-resident CTAs per SM of that kernel); otherwise one
+// residual + one solve launch per iteration.
+static bool persistent_update(const esikf_ctx *ctx, int coop_blocks) {
+  return ctx->loop_mode >= 1 && (ctx->nranks == 1 || ctx->p2p) && ctx->coop_ok && coop_blocks > 0 && !ctx->timing;
+}
+
+// Cooperative launch of lio_update_kernel<PEER> / vio_update_kernel<PEER, INVERSE>. Their arguments are
+// (ka, sa, barrier, barrier_next, stamps, parity_stride, peer, tail...): `ka` is the kernel's LioKernelArgs /
+// VioKernelArgs, `tail` the VIO-only arguments. Both instantiations get the same argument list, so the single-GPU
+// launch passes exactly what the peer launch does. `stamp_off` / `stamp_words`: this kernel's slice of the phase stamps.
+static int launch_persistent(esikf_ctx *ctx, const void *fn, const void *fn_peer, const char *name, int grid, int threads, size_t smem, void *ka, SolveArgs &sa,
+                             size_t stamp_off, size_t stamp_words, bool &timed, std::initializer_list<void *> tail) {
+  const unsigned par = ctx->launch_parity & 1;
+  unsigned int *bar = ctx->barrier.p + 64 * par, *bar_next = ctx->barrier.p + 64 * (par ^ 1);  // this launch's barrier / the next launch's (zeroed by the kernel)
+  unsigned long long *stamps = ctx->want_stamps ? ctx->stamps.p + stamp_off : nullptr;
+  if (stamps) CK(cudaMemsetAsync(stamps, 0, stamp_words * sizeof(unsigned long long), ctx->stream));
+  size_t parity_stride = (size_t)ctx->partial_blocks * NE_MAX;
+  PeerArgs peer;
+  peer.mbox = ctx->p2p ? ctx->peer_ptrs_dev.p : nullptr, peer.seq = ctx->peer_seq_dev;
+  peer.rank = ctx->rank, peer.nranks = ctx->p2p ? ctx->nranks : 1;
+  void *kargs[9] = {ka, (void *)&sa, (void *)&bar, (void *)&bar_next, (void *)&stamps, (void *)&parity_stride, (void *)&peer};
+  std::copy(tail.begin(), tail.end(), kargs + 7);
+  cudaError_t le = cudaLaunchCooperativeKernel(ctx->p2p && ctx->nranks > 1 ? fn_peer : fn, dim3(grid), dim3(threads), kargs, smem, ctx->stream);
+  if (le != cudaSuccess) return fail(ctx, ESIKF_ERR_CUDA, "cooperative launch of %s failed: %s", name, cudaGetErrorString(le));
+  ctx->launch_parity++;  // only a launch that happened consumes its barrier counter (the kernel zeroes the other one)
+  ctx->launches += 1;
+  timed = false;
   return ESIKF_OK;
 }
 
@@ -825,9 +846,9 @@ int esikf_lio_run(esikf_ctx *ctx, const double *state_in, const double *state_pr
     int rc = upload_states(ctx, state_in, state_prop);
     if (rc) return rc;
   }
-  const bool fused_lio = ctx->loop_mode >= 1 && (ctx->nranks == 1 || ctx->p2p) && ctx->coop_ok && ctx->coop_lio > 0 && !ctx->timing;
+  const bool fused_lio = persistent_update(ctx, ctx->coop_lio);
   // the persistent kernel initialises its own loop control / stats / barrier; the per-iteration path needs them zeroed
-  if (!fused_lio) CK(cudaMemsetAsync(ctx->lio_stats.p, 0, sizeof(esikf_lio_stats) + sizeof(Ctrl) + 64, st));
+  if (!fused_lio) CK(cudaMemsetAsync(ctx->lio_stats, 0, sizeof(esikf_lio_stats) + sizeof(Ctrl) + 64, st));
   const int n = ctx->n_pts;
   if (ctx->scan_fresh) {
     if (n > 0) {
@@ -837,28 +858,13 @@ int esikf_lio_run(esikf_ctx *ctx, const double *state_in, const double *state_pr
     ctx->scan_fresh = false;
   }
   LioKernelArgs ka;
-  lio_fill_args(ctx, ka, ctx->state.p);
-  SolveArgs sa;
-  memset(&sa, 0, sizeof(sa));
-  sa.state = ctx->state.p, sa.prop = ctx->prop.p, sa.info = ctx->info.p, sa.ctrl = ctx->ctrl.p;
-  sa.max_iterations = cfg->max_iterations, sa.solve_mode = ctx->solve_mode, sa.lio_stats = ctx->lio_stats.p;
+  lio_fill_args(ctx, ka, ctx->state);
+  SolveArgs sa = solve_args(ctx, ctx->state, cfg->max_iterations);
+  sa.lio_stats = ctx->lio_stats;
   const int grid = lio_grid(ctx, ka.count);
-  if (fused_lio) {
-    const unsigned par = ctx->launch_parity & 1;
-    unsigned int *bar = ctx->barrier.p + 64 * par, *bar_next = ctx->barrier.p + 64 * (par ^ 1);  // this launch's barrier / the next launch's (zeroed by the kernel)
-    unsigned long long *stamps = ctx->want_stamps ? ctx->stamps.p : nullptr;
-    if (stamps) CK(cudaMemsetAsync(stamps, 0, 64 * sizeof(unsigned long long), st));
-    size_t parity_stride = (size_t)ctx->partial_blocks * NE_MAX;
-    PeerArgs peer = peer_args(ctx);
-    void *kargs[] = {(void *)&ka, (void *)&sa, (void *)&bar, (void *)&bar_next, (void *)&stamps, (void *)&parity_stride, (void *)&peer};
-    const void *fn = (ctx->p2p && ctx->nranks > 1) ? (const void *)lio_update_kernel<true> : (const void *)lio_update_kernel<false>;
-    cudaError_t le = cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(LIO_THREADS), kargs, sizeof(LioSmem), st);
-    if (le != cudaSuccess) return fail(ctx, ESIKF_ERR_CUDA, "cooperative launch of lio_update_kernel failed: %s", cudaGetErrorString(le));
-    ctx->launch_parity++;  // only a launch that happened consumes its barrier counter (the kernel zeroes the other one)
-    ctx->launches += 1;
-    ctx->lio_timed = false;
-    return ESIKF_OK;
-  }
+  if (fused_lio)
+    return launch_persistent(ctx, (const void *)lio_update_kernel<false>, (const void *)lio_update_kernel<true>, "lio_update_kernel", grid, LIO_THREADS,
+                             sizeof(LioSmem), &ka, sa, 0, 64, ctx->lio_timed, {});
   ctx->lio_timed = ctx->timing;
   ctx->lio_slots = cfg->max_iterations;
   for (int it = 0; it < cfg->max_iterations; it++) {
@@ -881,10 +887,10 @@ int esikf_lio_run(esikf_ctx *ctx, const double *state_in, const double *state_pr
 // (Ctrl::comm_error, sticky on the device) into ESIKF_ERR_COMM once.
 static int finish_fetch(esikf_ctx *ctx) {
   Ctrl *h = reinterpret_cast<Ctrl *>(ctx->stage_ctrl);
-  CK(cudaMemcpyAsync(h, ctx->ctrl.p, sizeof(Ctrl), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(h, ctx->ctrl, sizeof(Ctrl), cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   if (h->comm_error) {
-    cudaMemsetAsync(&ctx->ctrl.p->comm_error, 0, sizeof(int), ctx->stream);
+    cudaMemsetAsync(&ctx->ctrl->comm_error, 0, sizeof(int), ctx->stream);
     return fail(ctx, ESIKF_ERR_COMM, "a bounded in-kernel wait expired (grid barrier or peer mailbox): a rank did not take part in the update");
   }
   return ESIKF_OK;
@@ -895,8 +901,8 @@ int esikf_lio_fetch(esikf_ctx *ctx, double *state_out, esikf_lio_stats *stats, i
   CK(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
   const size_t n = (size_t)ctx->n_pts;
-  if (state_out) CK(cudaMemcpyAsync(state_out, ctx->state.p, S_N * sizeof(double), cudaMemcpyDeviceToHost, st));
-  if (stats) CK(cudaMemcpyAsync(stats, ctx->lio_stats.p, sizeof(esikf_lio_stats), cudaMemcpyDeviceToHost, st));
+  if (state_out) CK(cudaMemcpyAsync(state_out, ctx->state, S_N * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (stats) CK(cudaMemcpyAsync(stats, ctx->lio_stats, sizeof(esikf_lio_stats), cudaMemcpyDeviceToHost, st));
   if (match_plane && n) CK(cudaMemcpyAsync(match_plane, ctx->match_plane.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   if (normal_plane && n) CK(cudaMemcpyAsync(normal_plane, ctx->normal_plane.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   if (dis_to_plane && n) CK(cudaMemcpyAsync(dis_to_plane, ctx->dis.p, n * sizeof(float), cudaMemcpyDeviceToHost, st));
@@ -1018,7 +1024,7 @@ static void vio_fill_args(esikf_ctx *ctx, VioKernelArgs &ka, double *state_ptr) 
   ka.exposure_en = ctx->vio_cfg.exposure_estimate_en;
   ka.state = state_ptr;
   vio_consts(ctx, ka.Rci, ka.Pci, ka.Jdp_dR);
-  ka.errors = ctx->errors.p, ka.partials = ctx->partials.p, ka.info = ctx->info.p, ka.ctrl = ctx->ctrl.p;
+  ka.errors = ctx->errors.p, ka.partials = ctx->partials.p, ka.info = ctx->info.p, ka.ctrl = ctx->ctrl;
   ka.partial_stride = ctx->partial_blocks;
 }
 static int vio_grid(const esikf_ctx *ctx, int count) {
@@ -1070,19 +1076,16 @@ int esikf_vio_run(esikf_ctx *ctx, const double *state_in, const double *state_pr
     if (ctx->n_inv_refs != ctx->n_patches) return fail(ctx, ESIKF_ERR_STATE, "vio_run: inverse_composition_en needs esikf_vio_set_inverse_refs for the %d patches (have %d)", ctx->n_patches, ctx->n_inv_refs);
     if (ctx->ref_w != ctx->cam.width || ctx->ref_h != ctx->cam.height) return fail(ctx, ESIKF_ERR_STATE, "vio_run: reference images must have the camera's size");
   }
-  const bool fused_vio = ctx->n_patches > 0 && ctx->loop_mode >= 1 && (ctx->nranks == 1 || ctx->p2p) && ctx->coop_ok && ctx->coop_vio > 0 && !ctx->timing;
+  const bool fused_vio = ctx->n_patches > 0 && persistent_update(ctx, ctx->coop_vio);
   if (!fused_vio) {
-    CK(cudaMemsetAsync(ctx->ctrl.p, 0, sizeof(Ctrl), st));
-    CK(cudaMemsetAsync(ctx->vio_stats.p, 0, sizeof(esikf_vio_stats), st));
+    CK(cudaMemsetAsync(ctx->ctrl, 0, sizeof(Ctrl), st));
+    CK(cudaMemsetAsync(ctx->vio_stats, 0, sizeof(esikf_vio_stats), st));
   }
   if (ctx->n_patches == 0) return ESIKF_OK;  // total_points == 0: early return (vio.cpp:786)
   VioKernelArgs ka;
-  vio_fill_args(ctx, ka, ctx->state.p);
-  SolveArgs sa;
-  memset(&sa, 0, sizeof(sa));
-  sa.state = ctx->state.p, sa.prop = ctx->prop.p, sa.info = ctx->info.p, sa.ctrl = ctx->ctrl.p;
-  sa.max_iterations = ctx->vio_cfg.max_iterations, sa.solve_mode = ctx->solve_mode, sa.vio_stats = ctx->vio_stats.p;
-  sa.old_state = ctx->old_state.p, sa.G = ctx->G.p, sa.img_point_cov = ctx->vio_cfg.img_point_cov;
+  vio_fill_args(ctx, ka, ctx->state);
+  SolveArgs sa = solve_args(ctx, ctx->state, ctx->vio_cfg.max_iterations);
+  sa.vio_stats = ctx->vio_stats, sa.old_state = ctx->old_state.p, sa.G = ctx->G.p, sa.img_point_cov = ctx->vio_cfg.img_point_cov;
   const int grid = vio_grid(ctx, ka.count);
   VioInvArgs iv;
   memset(&iv, 0, sizeof(iv));
@@ -1093,12 +1096,6 @@ int esikf_vio_run(esikf_ctx *ctx, const double *state_in, const double *state_pr
     iv.ref_w = ctx->ref_w, iv.ref_h = ctx->ref_h, iv.fx = ctx->cam.fx, iv.fy = ctx->cam.fy;
   }
   if (fused_vio) {
-    const unsigned par = ctx->launch_parity & 1;
-    unsigned int *bar = ctx->barrier.p + 64 * par, *bar_next = ctx->barrier.p + 64 * (par ^ 1);
-    unsigned long long *stamps = ctx->want_stamps ? ctx->stamps.p + 64 : nullptr;
-    if (stamps) CK(cudaMemsetAsync(stamps, 0, 512 * sizeof(unsigned long long), st));
-    size_t parity_stride = (size_t)ctx->partial_blocks * NE_MAX;
-    PeerArgs peer = peer_args(ctx);
     VioTma tma_off;
     tma_off.enabled = 0;
     VioTma *tma = &tma_off;
@@ -1107,16 +1104,9 @@ int esikf_vio_run(esikf_ctx *ctx, const double *state_in, const double *state_pr
       if (rc) return rc;
       tma = &ctx->tma;
     }
-    void *kargs[] = {(void *)&ka, (void *)&sa, (void *)&bar, (void *)&bar_next, (void *)&stamps, (void *)&parity_stride, (void *)&peer, (void *)&iv, (void *)tma};
-    const bool peers = ctx->p2p && ctx->nranks > 1;
-    const void *fn = inverse ? (peers ? (const void *)vio_update_kernel<true, true> : (const void *)vio_update_kernel<false, true>)
-                             : (peers ? (const void *)vio_update_kernel<true, false> : (const void *)vio_update_kernel<false, false>);
-    cudaError_t le = cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(VIO_THREADS), kargs, VIO_PERSIST_SMEM, st);
-    if (le != cudaSuccess) return fail(ctx, ESIKF_ERR_CUDA, "cooperative launch of vio_update_kernel failed: %s", cudaGetErrorString(le));
-    ctx->launch_parity++;
-    ctx->launches += 1;
-    ctx->vio_timed = false;
-    return ESIKF_OK;
+    const void *fn = inverse ? (const void *)vio_update_kernel<false, true> : (const void *)vio_update_kernel<false, false>;
+    const void *fn_peer = inverse ? (const void *)vio_update_kernel<true, true> : (const void *)vio_update_kernel<true, false>;
+    return launch_persistent(ctx, fn, fn_peer, "vio_update_kernel", grid, VIO_THREADS, VIO_PERSIST_SMEM, &ka, sa, 64, 512, ctx->vio_timed, {&iv, tma});
   }
   ctx->vio_timed = ctx->timing;
   ctx->vio_slots = ctx->vio_cfg.patch_pyrimid_level * ctx->vio_cfg.max_iterations;
@@ -1151,8 +1141,8 @@ int esikf_vio_fetch(esikf_ctx *ctx, double *state_out, esikf_vio_stats *stats, f
   if (!ctx) return ESIKF_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
-  if (state_out) CK(cudaMemcpyAsync(state_out, ctx->state.p, S_N * sizeof(double), cudaMemcpyDeviceToHost, st));
-  if (stats) CK(cudaMemcpyAsync(stats, ctx->vio_stats.p, sizeof(esikf_vio_stats), cudaMemcpyDeviceToHost, st));
+  if (state_out) CK(cudaMemcpyAsync(state_out, ctx->state, S_N * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (stats) CK(cudaMemcpyAsync(stats, ctx->vio_stats, sizeof(esikf_vio_stats), cudaMemcpyDeviceToHost, st));
   if (errors && ctx->n_patches) CK(cudaMemcpyAsync(errors, ctx->errors.p, (size_t)ctx->n_patches * sizeof(float), cudaMemcpyDeviceToHost, st));
   return finish_fetch(ctx);
 }
@@ -1190,17 +1180,19 @@ int esikf_vio_set_ref_images(esikf_ctx *ctx, const uint8_t *const *imgs, int32_t
   if (!ctx || n_imgs < 0 || width <= 0 || height <= 0 || (n_imgs > 0 && !imgs)) return fail(ctx, ESIKF_ERR_ARG, "set_ref_images: bad argument");
   CK(cudaSetDevice(ctx->device));
   CK(cudaStreamSynchronize(ctx->stream));
-  for (uint8_t *p : ctx->ref_imgs) cudaFree(p);
   ctx->ref_imgs.clear();
   ctx->n_inv_refs = 0;  // the inverse-compositional reference indices pointed into the images just released
+  std::vector<const uint8_t *> ptrs;
   for (int i = 0; i < n_imgs; i++) {
-    uint8_t *d = nullptr;
-    CK(cudaMalloc(&d, (size_t)width * height + 64));
-    ctx->ref_imgs.push_back(d);
-    CK(cudaMemcpyAsync(d, imgs[i], (size_t)width * height, cudaMemcpyHostToDevice, ctx->stream));
+    DevBuf<uint8_t> d;
+    CK(cudaMalloc(&d.p, (size_t)width * height + 64));  // exact size: the images are replaced as a whole, never grown
+    d.cap = (size_t)width * height + 64;
+    ptrs.push_back(d.p);
+    ctx->ref_imgs.push_back(std::move(d));
+    CK(cudaMemcpyAsync(ctx->ref_imgs.back().p, imgs[i], (size_t)width * height, cudaMemcpyHostToDevice, ctx->stream));
   }
   CK(ctx->ref_img_ptrs.reserve(n_imgs + 1));
-  if (n_imgs) CK(cudaMemcpyAsync(ctx->ref_img_ptrs.p, ctx->ref_imgs.data(), n_imgs * sizeof(uint8_t *), cudaMemcpyHostToDevice, ctx->stream));
+  if (n_imgs) CK(cudaMemcpyAsync(ctx->ref_img_ptrs.p, ptrs.data(), n_imgs * sizeof(uint8_t *), cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   ctx->ref_w = width, ctx->ref_h = height;
   return ESIKF_OK;
@@ -1403,12 +1395,8 @@ int esikf_profile_kernel(esikf_ctx *ctx, int32_t which, int32_t arg, int32_t rep
   const size_t flush_bytes = 256u << 20;
   if (flush_l2) CK(ctx->flush.reserve(flush_bytes));
   // work on a scratch copy of the resident state so the measured launches never disturb an update in flight
-  CK(cudaMemcpyAsync(ctx->scratch_state.p, ctx->state.p, S_N * sizeof(double), cudaMemcpyDeviceToDevice, st));
-  CK(cudaMemsetAsync(ctx->ctrl.p, 0, sizeof(Ctrl), st));
-  cudaEvent_t e0, e1;
-  CK(cudaEventCreate(&e0));
-  CK(cudaEventCreate(&e1));
-  double total = 0.0;
+  CK(cudaMemcpyAsync(ctx->scratch_state.p, ctx->state, S_N * sizeof(double), cudaMemcpyDeviceToDevice, st));
+  CK(cudaMemsetAsync(ctx->ctrl, 0, sizeof(Ctrl), st));
   LioKernelArgs la;
   VioKernelArgs va;
   SolveArgs sa;
@@ -1418,8 +1406,7 @@ int esikf_profile_kernel(esikf_ctx *ctx, int32_t which, int32_t arg, int32_t rep
     if (!ctx->have_map || ctx->n_pts == 0 || ctx->scan_fresh) return fail(ctx, ESIKF_ERR_STATE, "profile_kernel: no resident LIO frame (run lio once)");
     lio_fill_args(ctx, la, ctx->scratch_state.p);
     grid = lio_grid(ctx, la.count);
-    sa.state = ctx->scratch_state.p, sa.prop = ctx->prop.p, sa.info = ctx->info.p, sa.ctrl = ctx->ctrl.p;
-    sa.max_iterations = 1 << 20, sa.solve_mode = ctx->solve_mode;
+    sa = solve_args(ctx, ctx->scratch_state.p, 1 << 20);
   } else if (which == 2) {
     if (ctx->n_patches == 0 || ctx->img_w == 0) return fail(ctx, ESIKF_ERR_STATE, "profile_kernel: no resident VIO frame");
     vio_fill_args(ctx, va, ctx->scratch_state.p);
@@ -1428,11 +1415,22 @@ int esikf_profile_kernel(esikf_ctx *ctx, int32_t which, int32_t arg, int32_t rep
   } else {
     return fail(ctx, ESIKF_ERR_ARG, "profile_kernel: which=%d", which);
   }
+  struct Events {  // destroyed on every return
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    ~Events() {
+      if (e0) cudaEventDestroy(e0);
+      if (e1) cudaEventDestroy(e1);
+    }
+  } ev;
+  cudaEvent_t &e0 = ev.e0, &e1 = ev.e1;
+  CK(cudaEventCreate(&e0));
+  CK(cudaEventCreate(&e1));
+  double total = 0.0;
   for (int r = 0; r < reps + 3; r++) {  // 3 warm-up launches
     if (flush_l2) CK(cudaMemsetAsync(ctx->flush.p, r & 0xff, flush_bytes, st));
     if (which == 1) {
-      CK(cudaMemcpyAsync(ctx->scratch_state.p, ctx->state.p, S_N * sizeof(double), cudaMemcpyDeviceToDevice, st));
-      CK(cudaMemsetAsync(ctx->ctrl.p, 0, sizeof(Ctrl), st));
+      CK(cudaMemcpyAsync(ctx->scratch_state.p, ctx->state, S_N * sizeof(double), cudaMemcpyDeviceToDevice, st));
+      CK(cudaMemsetAsync(ctx->ctrl, 0, sizeof(Ctrl), st));
     }
     CK(cudaEventRecord(e0, st));
     if (which == 0) lio_residual_kernel<<<grid, LIO_THREADS, sizeof(LioSmem), st>>>(la);
@@ -1447,8 +1445,6 @@ int esikf_profile_kernel(esikf_ctx *ctx, int32_t which, int32_t arg, int32_t rep
     CK(cudaEventElapsedTime(&ms, e0, e1));
     if (r >= 3) total += ms;
   }
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
   CK(cudaGetLastError());
   *avg_ms = (float)(total / reps);
   return ESIKF_OK;
