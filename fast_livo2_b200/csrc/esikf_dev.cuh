@@ -78,6 +78,11 @@ __host__ __device__ __forceinline__ double m_sub(double a, double b) {
 }
 __host__ __device__ __forceinline__ double m_dot3(double a0, double b0, double a1, double b1, double a2, double b2) { return m_add(m_add(m_mul(a0, b0), m_mul(a1, b1)), m_mul(a2, b2)); }
 
+// a00 a11 - a01 a10 with both products rounded, as the reference's 2 x 2 determinant (getBestSearchLevel, warpAffine's
+// inverse). Contracted into an FMA it can land on the other side of getBestSearchLevel's thresholds 3 / 12 when it lies
+// within an ulp of one, and it gives a different float inverse when the products cancel.
+__device__ __forceinline__ double det2_rn(double a00, double a11, double a01, double a10) { return __dsub_rn(__dmul_rn(a00, a11), __dmul_rn(a01, a10)); }
+
 // 256-byte map plane -> the 144-byte record (one definition for the upload / patch kernel and the device-resident map, evaluated
 // without FMA contraction: both paths hand the residual kernel bit-identical records for the same plane)
 __host__ __device__ constexpr int tri6u(int i, int j) { return i * 6 - (i * (i - 1)) / 2 + (j - i); }  // i <= j

@@ -446,7 +446,7 @@ __global__ void warp_matrix_kernel(CamDev cam, int n, const double *__restrict__
   A_out[4 * i] = A00, A_out[4 * i + 1] = A01, A_out[4 * i + 2] = A10, A_out[4 * i + 3] = A11;
   // getBestSearchLevel(A, 2)   (:320-331)
   int sl = 0;
-  double Dt = A00 * A11 - A01 * A10;
+  double Dt = det2_rn(A00, A11, A01, A10);
   while (Dt > 3.0 && sl < 2) {
     sl += 1;
     Dt *= 0.25;
@@ -462,7 +462,7 @@ __global__ void warp_affine_kernel(const uint8_t *const *__restrict__ ref_imgs, 
   if (gid >= n * levels * 64) return;
   const int i = gid / (levels * 64), rem = gid % (levels * 64), pyramid_level = rem >> 6, pix = rem & 63, y = pix >> 3, x = pix & 7;
   const double a00 = A_cur_ref[4 * i], a01 = A_cur_ref[4 * i + 1], a10 = A_cur_ref[4 * i + 2], a11 = A_cur_ref[4 * i + 3];
-  const double det = a00 * a11 - a01 * a10;
+  const double det = det2_rn(a00, a11, a01, a10);
   const double id = 1.0 / det;
   const float A00 = (float)(a11 * id), A01 = (float)(-a01 * id), A10 = (float)(-a10 * id), A11 = (float)(a00 * id);
   if (isnan(A00)) return;  // :297-301 (patch left untouched)

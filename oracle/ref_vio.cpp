@@ -53,6 +53,11 @@ struct RefVio {
 
 extern "C" {
 
+// Version of this library: 2 = the stand-in matrix library inverts a fixed 2 x 2 by Eigen's closed form (warpAffine's
+// A_cur_ref.inverse()); an older build inverted it by LU, which differs in the last bits when the determinant cancels.
+// tests/oracle_bind.py uses the library live only at this version; the Makefile rebuilds a library that does not export it.
+int ref_vio_driver_version_2(void) { return 2; }
+
 // cam = [model (0 pinhole / radtan, 1 equidistant), width, height, fx, fy, cx, cy, d0..d4]; cfg = [patch_pyrimid_level, max_iterations, img_point_cov, exposure_estimate_en]
 void *ref_vio_create(const double *cam, const double *extR, const double *extT, const double *Rcl, const double *Pcl, const double *cfg) {
   if ((int)cam[0] != 0 && (int)cam[0] != 1) return nullptr;

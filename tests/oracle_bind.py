@@ -418,8 +418,17 @@ class RefMap:
 REF_VIO_SO = os.path.join(ORACLE_DIR, "_ref", "libfl2_ref_vio.so")
 
 
+REF_VIO_DRIVER = "ref_vio_driver_version_2"  # oracle/ref_vio.cpp + stand-in headers the tests are written against
+_ref_vio_ok = None
+
+
 def ref_vio_available():
-    return os.path.exists(REF_VIO_SO)
+    """The reference-source VIO library exists and was built at the current version. An older build (whose stand-in inverted
+    2 x 2 matrices by LU, not by Eigen's closed form) is not used live: the tests then compare with the stored outputs."""
+    global _ref_vio_ok
+    if _ref_vio_ok is None:
+        _ref_vio_ok = os.path.exists(REF_VIO_SO) and hasattr(C.CDLL(REF_VIO_SO), REF_VIO_DRIVER)
+    return _ref_vio_ok
 
 
 class RefVIO:

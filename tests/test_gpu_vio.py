@@ -70,14 +70,12 @@ def test_warp_matrix_and_warp_affine(gpu_ctx, small_vio_frame):
     o = O.oracle_warp_patches(fr, prior)
     np.testing.assert_allclose(g["A_cur_ref"], o["A_cur_ref"], rtol=1e-10, atol=1e-12)
     assert np.array_equal(g["search_levels"], o["search_levels"])
-    # the warp itself is float arithmetic without contraction: bit-exact given the same A (feed the oracle the GPU's A)
+    # the warp itself (the inverse through the rounded-products determinant, then float arithmetic without contraction) is
+    # bit-exact given the same A: feed the oracle the GPU's A
     vio = O.OracleVIO(fr["cam_cfg"], fr["ext"], fr["vio_cfg"])
-    n_exact = 0
     for i in range(len(fr["vis_pos"])):
         ref = vio.warp_affine(fr["img_ref"], g["A_cur_ref"][i], fr["px_ref"][i], g["search_levels"][i])
-        n_exact += np.array_equal(ref, g["warp_patch"][i])
-        np.testing.assert_allclose(g["warp_patch"][i], ref, atol=2e-3)
-    assert n_exact >= 0.98 * len(fr["vis_pos"])
+        assert np.array_equal(ref, g["warp_patch"][i]), i
 
 
 @pytest.mark.parametrize("seed", [2, 6])
