@@ -117,15 +117,13 @@ struct Ctrl {
   int iter;         // LIO: iterations executed so far ; VIO: total iterations
   int rematch_num;  // LIO (voxel_map.cpp:365,482)
   int level_done;   // VIO: EKF_end of the current level
-  int level;        // VIO: level being processed
-  int level_iter;   // VIO: iteration counter inside the level
   float last_error; // VIO (vio.cpp:1528)
   int has_G;        // VIO: G valid (at least one accepted update)
   unsigned int block_counter;  // last-block-done counter of the per-iteration residual kernels
-  int accepted_in_level;       // VIO: accepted updates of the current level (diagnostics)
   int comm_error;              // a bounded wait (grid barrier / peer mailbox) expired: results of this update are invalid
-  int pad[5];
+  int pad[8];
 };
+static_assert(sizeof(Ctrl) == 64, "the VIO stats follow the control block in one allocation: keep its size (and their alignment)");
 
 #ifdef __CUDACC__
 __device__ __forceinline__ unsigned long long globaltimer_ns() {
@@ -133,6 +131,10 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
 }
+
+// A value of the update state: in global memory, written by an earlier launch (global), or the CTA's resident copy in shared
+// memory (persistent kernels).
+__device__ __forceinline__ double ld_state(const double *p, bool global) { return global ? __ldcg(p) : *p; }
 
 // fp64 tensor-core contraction step: D(8x8) += A(8x4) * B(4x8), mma.sync.m8n8k4.f64 (SASS DMMA).
 // Lane l holds A[l/4][l%4], B[l%4][l/4] and D[l/4][2*(l%4) + {0,1}].

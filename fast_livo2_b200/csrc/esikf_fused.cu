@@ -133,14 +133,65 @@ struct FusedSolveSmem {
 };
 static_assert(sizeof(FusedSolveSmem) % 8 == 0, "what follows it in shared memory holds doubles");
 
-__device__ __forceinline__ void lio_consts_from_resident(LioSmem &sm, const FusedSolveSmem &fs) {
-  const int tid = threadIdx.x;
-  if (tid < 9) {
-    sm.R[tid] = fs.io.st[S_R + tid];
-  } else if (tid < 12) {
-    sm.t[tid - 9] = fs.io.st[S_P + tid - 9];
+// Prologue of both persistent kernels: the CTA's loop control, wait guard and literal-mode workspace (solve_mode 1 borrows
+// `lit`), the next launch's barrier counter (no host memset per update), zeroed stats, P and the poses staged once for the
+// whole update, and the gain's loop invariants on the last warp. `setup` is the kernel's own set-up and ends with a CTA
+// barrier (fs.sm.P is in place after it). Returns the peer exchange counter.
+template <int M, int WARPS, bool PEER, class F>
+__device__ __forceinline__ unsigned int persist_prologue(FusedSolveSmem &fs, SolveLiteralScratch &lit, SolveArgs &sa, unsigned int *barrier_next, const PeerArgs &peer,
+                                                         double pscale, F setup) {
+  const bool publisher = (blockIdx.x == gridDim.x - 1);
+  sa.no_publish = !publisher;
+  if (threadIdx.x == 0) {
+    Ctrl z;
+    memset(&z, 0, sizeof(z));
+    fs.ctrl = z;
+    fs.wg.error_flag = &sa.ctrl->comm_error, fs.wg.dead = false;
+    fs.sm.W = lit.W, fs.sm.K = lit.K;
+    if (blockIdx.x == 0) barrier_next[0] = 0u, barrier_next[32] = 0u;
+  }
+  int *const stats = (M == 6) ? reinterpret_cast<int *>(sa.lio_stats) : reinterpret_cast<int *>(sa.vio_stats);
+  const int stats_words = (int)((M == 6) ? sizeof(esikf_lio_stats) : sizeof(esikf_vio_stats)) / 4;
+  if (publisher && stats)
+    for (int t = threadIdx.x; t < stats_words; t += blockDim.x) stats[t] = 0;
+  solve_load(fs.sm, fs.io, sa, false);
+  const unsigned int seq = PEER ? __ldcg(peer.seq) : 0u;
+  setup();
+  if ((threadIdx.x >> 5) == WARPS - 1 && sa.solve_mode == 0) gain_setup<M>(fs.sm, pscale, threadIdx.x & 31);  // first used after two CTA barriers
+  return seq;
+}
+
+// Exchange step of one iteration: the CTA's partial vector, ONE grid barrier (warp 1 evaluates vec = state_propagat (-)
+// state meanwhile, voxel_map.cpp:470 / vio.cpp:1664), the fixed-order sum into fs.io.info and, with peers, the rank-ordered
+// sum over the mailboxes. Ends with a CTA barrier. Phase stamp: all CTAs arrived.
+template <int WARPS, int M, bool PEER>
+__device__ __forceinline__ void persist_exchange(FusedSolveSmem &fs, ReduceSmem<WARPS> &red, double D0, double D1, double cnt, double *part, int partial_stride,
+                                                 unsigned int *barrier, unsigned int &epoch, const PeerArgs &peer, unsigned int &seq, unsigned long long *stamps, int &sk) {
+  store_partials<WARPS, M>(red, D0, D1, cnt, part, partial_stride);
+  grid_barrier_overlap(barrier, epoch, fs.wg, [&]() {
+    if ((threadIdx.x >> 5) == 1) boxminus_warp(fs.io.pr, fs.io.st, fs.sm.vec, threadIdx.x & 31);
+  });
+  stamp(stamps, sk);
+  sum_partials<M>(part, partial_stride, gridDim.x, fs.io.info, WARPS);
+  if (PEER) {
+    __syncthreads();
+    if (blockIdx.x == 0) peer_push(fs.io.info, peer, seq);
+    peer_pull(fs.io.info, peer, seq, fs.wg);
+    seq++;
   }
   __syncthreads();
+}
+
+// Epilogue, publisher only: the loop-control block and the exchange counter back to global memory. An expired wait stays
+// raised, whether this CTA or another one saw it.
+template <bool PEER> __device__ __forceinline__ void persist_epilogue(FusedSolveSmem &fs, Ctrl *ctrl, const PeerArgs &peer, unsigned int seq) {
+  if (threadIdx.x == 0) {
+    fs.ctrl.comm_error = fs.wg.dead ? 1 : 0;
+    const int err = *reinterpret_cast<volatile int *>(&ctrl->comm_error);
+    *ctrl = fs.ctrl;
+    if (err) ctrl->comm_error = 1;
+    if (PEER) *peer.seq = seq;
+  }
 }
 
 template <bool PEER>
@@ -151,54 +202,23 @@ __global__ void __launch_bounds__(LIO_THREADS, 1) lio_update_kernel(const LioKer
   static_assert(sizeof(FusedSolveSmem) <= sizeof(sm.fs_raw), "solve state must fit");
   static_assert(sizeof(SolveLiteralScratch) <= sizeof(sm.rec), "literal scratch must fit in the record slots");
   FusedSolveSmem &fs = *reinterpret_cast<FusedSolveSmem *>(sm.fs_raw);
+  SolveLiteralScratch &lit = *reinterpret_cast<SolveLiteralScratch *>(&sm.rec[0][0][0]);
   SolveArgs sa = sa_in;
-  const bool publisher = (blockIdx.x == gridDim.x - 1);
-  sa.no_publish = !publisher;
   unsigned int epoch = 0;
   int lo, hi;
   lio_block_range(a.count, lo, hi);
-  if (threadIdx.x == 0) {
-    Ctrl z;
-    memset(&z, 0, sizeof(z));
-    fs.ctrl = z;
-    fs.wg.error_flag = &a.ctrl->comm_error, fs.wg.dead = false;
-    // the literal-mode workspace (solve_mode 1, parity checks) borrows the record slots and forces a re-stage
-    SolveLiteralScratch *lit = reinterpret_cast<SolveLiteralScratch *>(&sm.rec[0][0][0]);
-    fs.sm.W = lit->W, fs.sm.K = lit->K;
-    if (blockIdx.x == 0) barrier_next[0] = 0u, barrier_next[32] = 0u;  // the NEXT launch's barrier counter (no host memset per update)
-  }
-  if (publisher && sa.lio_stats)
-    for (int t = threadIdx.x; t < (int)(sizeof(esikf_lio_stats) / 4); t += blockDim.x) reinterpret_cast<int *>(sa.lio_stats)[t] = 0;
-  solve_load(fs.sm, fs.io, sa, false);  // P, current and prior pose: staged once per CTA, resident for the whole update
-  {
-    // prior-pose constants (voxel_map.cpp:425-428, 445) never change inside the loop
-    const int tid = threadIdx.x;
-    if (tid < 9) {
-      const int r = tid / 3, c = tid % 3;
-      sm.Rp[tid] = a.prop[S_R + tid];
-      double s = 0;
-      for (int k = 0; k < 3; k++) s += a.prop[S_R + r * 3 + k] * a.extR[k * 3 + c];
-      sm.Mp[tid] = s;
-    } else if (tid < 12) {
-      sm.tp[tid - 9] = a.prop[S_P + tid - 9];
-    }
-  }
-  unsigned int seq = PEER ? __ldcg(peer.seq) : 0u;
-  lio_init_cold(sm, a);
-  lio_init_barriers(sm);  // ends with a CTA barrier: fs.sm.P is in place
-  if ((threadIdx.x >> 5) == LIO_WARPS - 1 && sa.solve_mode == 0) gain_setup<6>(fs.sm, 1.0, threadIdx.x & 31);  // loop invariants of the gain; first used after two CTA barriers
-  if (threadIdx.x < 9) {
-    // state_.cov is only written after the loop (:489): the covariance blocks of pv.var (:377-378) are loop constants
-    const int r = threadIdx.x / 3, c = threadIdx.x % 3;
-    sm.Ptt[threadIdx.x] = fs.sm.P[r * 19 + c];
-    sm.Ppp[threadIdx.x] = fs.sm.P[(3 + r) * 19 + (3 + c)];
-  }
+  unsigned int seq = persist_prologue<6, LIO_WARPS, PEER>(fs, lit, sa, barrier_next, peer, 1.0, [&]() {
+    lio_prior_consts(sm, a);  // never change inside the loop
+    lio_init_cold(sm, a);
+    lio_init_barriers(sm);    // fs.sm.P is in place
+    lio_pose_consts(sm, fs.io.st, fs.sm.P, false);  // Ptt / Ppp for the whole update
+  });
   int sk = 0;
   LaneCache lc;
   lane_cache_init(lc);
   for (int it = 0; it < sa.max_iterations; it++) {
     stamp(stamps, sk);  // 0: iteration start
-    lio_consts_from_resident(sm, fs);
+    lio_pose_consts(sm, fs.io.st, nullptr, false);
     stamp(stamps, sk);  // 1: constants in place
     double D0 = 0.0, D1 = 0.0;
     int cnt = 0;
@@ -209,56 +229,18 @@ __global__ void __launch_bounds__(LIO_THREADS, 1) lio_update_kernel(const LioKer
       if (threadIdx.x == 0) stamps[640 + blockIdx.x] = globaltimer_ns();
     }
     stamp(stamps, sk);  // 2: this CTA's warps issued their slice (CTA 0 / thread 0)
-    double *const part = a.partials + (size_t)(it & 1) * partial_parity_stride;
-    store_partials<LIO_WARPS, 6>(sm.red, D0, D1, (double)cnt, part, a.partial_stride);
-    grid_barrier_overlap(barrier, epoch, fs.wg, [&]() {
-      if ((threadIdx.x >> 5) == 1) boxminus_warp(fs.io.pr, fs.io.st, fs.sm.vec, threadIdx.x & 31);  // vec = state_propagat (-) state_ (:470)
-    });
-    stamp(stamps, sk);  // 3: all CTAs arrived
-    sum_partials<6>(part, a.partial_stride, gridDim.x, fs.io.info, LIO_WARPS);
-    if (PEER) {
-      __syncthreads();
-      if (blockIdx.x == 0) peer_push(fs.io.info, peer, seq);
-      peer_pull(fs.io.info, peer, seq, fs.wg);
-      seq++;
-    }
-    __syncthreads();
+    persist_exchange<LIO_WARPS, 6, PEER>(fs, sm.red, D0, D1, (double)cnt, a.partials + (size_t)(it & 1) * partial_parity_stride, a.partial_stride, barrier, epoch, peer,
+                                         seq, stamps, sk);  // 3: all CTAs arrived
     stamp(stamps, sk);  // 4: information vector complete
     sa.dbg = (stamps && blockIdx.x == 0) ? stamps + sk + 1 : nullptr;  // 6: gain rows done, 7: boxplus done
-    lio_solve_block(sa, fs.sm, fs.io, fs.ctrl, true, true);
+    lio_solve_block(sa, fs.sm, fs.io, fs.ctrl);
     if (sa.solve_mode == 1) lane_cache_reset(lc);  // the literal workspace borrowed the record slots
     stamp(stamps, sk);  // 5: solved (state, loop control current in every CTA)
     sk += 2;            // 6, 7: spare
     if (fs.ctrl.stop) break;  // EKF_stop_flg (voxel_map.cpp:499)
   }
   if (sa.solve_mode != 1) lio_write_outputs(a, sm, lo, hi, lc);
-  if (publisher && threadIdx.x == 0) {
-    fs.ctrl.comm_error = fs.wg.dead ? 1 : 0;
-    const int err = *reinterpret_cast<volatile int *>(&a.ctrl->comm_error);
-    *a.ctrl = fs.ctrl;
-    if (err) a.ctrl->comm_error = 1;
-    if (PEER) *peer.seq = seq;
-  }
-}
-
-__device__ __forceinline__ void vio_consts_from_resident(VioSmem &sm, const VioKernelArgs &a, const FusedSolveSmem &fs) {
-  const int tid = threadIdx.x;
-  if (tid < 9) {
-    // Rcw = Rci * Rwi^T  (vio.cpp:1542)
-    const int r = tid / 3, c = tid % 3;
-    double s = 0;
-    for (int k = 0; k < 3; k++) s += a.Rci[r * 3 + k] * fs.io.st[S_R + c * 3 + k];
-    sm.Rcw[tid] = s;
-  }
-  if (tid == 0) sm.inv_expo = fs.io.st[S_EXPO];
-  __syncthreads();
-  if (tid < 3) {
-    // Pcw = -Rci Rwi^T Pwi + Pci  (:1543)
-    double s = 0;
-    for (int k = 0; k < 3; k++) s += sm.Rcw[tid * 3 + k] * fs.io.st[S_P + k];
-    sm.Pcw[tid] = -s + a.Pci[tid];
-  }
-  __syncthreads();
+  if (!sa.no_publish) persist_epilogue<PEER>(fs, a.ctrl, peer, seq);
 }
 
 // INVERSE: the inverse-compositional variant (vio/inverse_composition_en, src/vio.cpp:792-795, 1327-1518) in the same loop:
@@ -273,37 +255,24 @@ __global__ void __launch_bounds__(VIO_THREADS, 1) vio_update_kernel(const VioKer
   FusedSolveSmem &fs = *reinterpret_cast<FusedSolveSmem *>(smem_raw + sizeof(VioSmem));
   SolveLiteralScratch &lit = *reinterpret_cast<SolveLiteralScratch *>(&sm.rows[0][0][0]);
   static_assert(sizeof(SolveLiteralScratch) <= sizeof(sm.rows), "literal scratch must fit in the row staging area");
-  const bool publisher = (blockIdx.x == gridDim.x - 1);
-  sa.no_publish = !publisher;
   unsigned int epoch = 0;
   int lo, hi;
   vio_block_range(a.count, lo, hi);
   const bool cached = (hi - lo) <= VIO_WARPS * VIO_KMAX;
-  if (threadIdx.x == 0) {
-    Ctrl z;
-    memset(&z, 0, sizeof(z));
-    fs.ctrl = z;
-    fs.wg.error_flag = &a.ctrl->comm_error, fs.wg.dead = false;
-    fs.sm.W = lit.W, fs.sm.K = lit.K;
-    if (blockIdx.x == 0) barrier_next[0] = 0u, barrier_next[32] = 0u;
-  }
-  if (publisher && sa.vio_stats)
-    for (int t = threadIdx.x; t < (int)(sizeof(esikf_vio_stats) / 4); t += blockDim.x) reinterpret_cast<int *>(sa.vio_stats)[t] = 0;
-  solve_load(fs.sm, fs.io, sa, false);
-  vio_cache_reset(sm);
-  unsigned int seq = PEER ? __ldcg(peer.seq) : 0u;
   unsigned tma_phase = 0;  // parity of this warp's TMA barrier
-  if (threadIdx.x < VIO_WARPS) mbar_init(&sm.tma_bar[threadIdx.x], 1);
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  __syncthreads();
-  if ((threadIdx.x >> 5) == VIO_WARPS - 1 && sa.solve_mode == 0) gain_setup<7>(fs.sm, 1.0 / sa.img_point_cov, threadIdx.x & 31);  // loop invariants of the gain
+  unsigned int seq = persist_prologue<7, VIO_WARPS, PEER>(fs, lit, sa, barrier_next, peer, 1.0 / sa.img_point_cov, [&]() {
+    vio_cache_reset(sm);
+    if (threadIdx.x < VIO_WARPS) mbar_init(&sm.tma_bar[threadIdx.x], 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    __syncthreads();
+  });
   int slot = 0;
   for (int level = a.levels - 1; level >= 0; level--) {      // vio.cpp:790
     for (int it = 0; it < sa.max_iterations; it++) {          // :1536
       const int cur = slot++;  // counts executed iterations (a level may end early): the partial-buffer parity follows it
       int sk = 8 * ((a.levels - 1 - level) * sa.max_iterations + it);
       stamp(stamps, sk);
-      vio_consts_from_resident(sm, a, fs);
+      vio_load_consts(sm, a, fs.io.st, false);
       stamp(stamps, sk);
       double D0 = 0.0, D1 = 0.0, n_meas = 0.0;
       if (INVERSE) {
@@ -314,24 +283,12 @@ __global__ void __launch_bounds__(VIO_THREADS, 1) vio_update_kernel(const VioKer
         vio_process_range(a, sm, level, lo, hi, D0, D1, n_meas, cached, tma.enabled ? &tma : nullptr, &tma_phase);
       }
       stamp(stamps, sk);
-      double *const part = a.partials + (size_t)(cur & 1) * partial_parity_stride;
-      store_partials<VIO_WARPS, 7>(sm.red, D0, D1, n_meas, part, a.partial_stride);
-      grid_barrier_overlap(barrier, epoch, fs.wg, [&]() {
-        if ((threadIdx.x >> 5) == 1) boxminus_warp(fs.io.pr, fs.io.st, fs.sm.vec, threadIdx.x & 31);  // vec = state_propagat (-) state (:1664)
-      });
+      persist_exchange<VIO_WARPS, 7, PEER>(fs, sm.red, D0, D1, n_meas, a.partials + (size_t)(cur & 1) * partial_parity_stride, a.partial_stride, barrier, epoch, peer,
+                                           seq, stamps, sk);
       stamp(stamps, sk);
-      sum_partials<7>(part, a.partial_stride, gridDim.x, fs.io.info, VIO_WARPS);
-      if (PEER) {
-        __syncthreads();
-        if (blockIdx.x == 0) peer_push(fs.io.info, peer, seq);
-        peer_pull(fs.io.info, peer, seq, fs.wg);
-        seq++;
-      }
-      __syncthreads();
-      stamp(stamps, sk);
-      sa.level = level, sa.slot_iter = it, sa.last_slot = 0;
+      sa.level = level, sa.slot_iter = it;
       sa.dbg = (stamps && blockIdx.x == 0) ? stamps + sk + 1 : nullptr;  // 6: gain rows done, 7: boxplus done
-      vio_solve_block(sa, fs.sm, fs.io, fs.ctrl, true, true);
+      vio_solve_block(sa, fs.sm, fs.io, fs.ctrl);
       if (sa.solve_mode == 1) {  // the literal workspace borrowed the row area; nothing cached lives there
         __syncthreads();
       }
@@ -339,21 +296,10 @@ __global__ void __launch_bounds__(VIO_THREADS, 1) vio_update_kernel(const VioKer
       if (fs.ctrl.level_done) break;  // EKF_end (:1685)
     }
   }
-  // state->cov -= G * state->cov (vio.cpp:800): a last-slot pass of the solve routine with the level already finished
-  if (publisher) {
-    __syncthreads();
-    sa.level = 0, sa.slot_iter = 1, sa.last_slot = 1, sa.dbg = nullptr;
-    if (threadIdx.x == 0) fs.ctrl.level_done = 1;
-    __syncthreads();
-    vio_solve_block(sa, fs.sm, fs.io, fs.ctrl, true, true);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      fs.ctrl.comm_error = fs.wg.dead ? 1 : 0;
-      const int err = *reinterpret_cast<volatile int *>(&a.ctrl->comm_error);
-      *a.ctrl = fs.ctrl;
-      if (err) a.ctrl->comm_error = 1;
-      if (PEER) *peer.seq = seq;
-    }
+  if (!sa.no_publish) {
+    __syncthreads();  // this CTA's threads stored every accepted G
+    if (fs.ctrl.has_G) vio_final_cov(sa, fs.sm, fs.io, false);
+    persist_epilogue<PEER>(fs, a.ctrl, peer, seq);
   }
 }
 

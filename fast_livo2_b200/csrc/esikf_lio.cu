@@ -198,22 +198,35 @@ __device__ __forceinline__ void lane_cache_init(LaneCache &lc) {
   lc.out_valid = false;
 }
 
-// Load the per-iteration constants (current pose / covariance blocks, prior pose) into shared memory.
-__device__ __forceinline__ void lio_load_consts(LioSmem &sm, const LioKernelArgs &a) {
+// Prior-pose constants (voxel_map.cpp:425-428): Rp, tp and Mp = Rp * extR (state_propagat.rot_end * extR_, :445).
+// No barrier: the caller's next one publishes them.
+__device__ __forceinline__ void lio_prior_consts(LioSmem &sm, const LioKernelArgs &a) {
   const int tid = threadIdx.x;
   if (tid < 9) {
-    sm.R[tid] = __ldcg(a.state + S_R + tid);
+    const int r = tid / 3, c = tid % 3;
     sm.Rp[tid] = a.prop[S_R + tid];
-    int r = tid / 3, c = tid % 3;
-    sm.Ptt[tid] = __ldcg(a.state + S_COV + r * 19 + c);
-    sm.Ppp[tid] = __ldcg(a.state + S_COV + (3 + r) * 19 + (3 + c));
-    // Mp = Rp * extR  (state_propagat.rot_end * extR_, voxel_map.cpp:445)
     double s = 0;
     for (int k = 0; k < 3; k++) s += a.prop[S_R + r * 3 + k] * a.extR[k * 3 + c];
     sm.Mp[tid] = s;
   } else if (tid < 12) {
-    sm.t[tid - 9] = __ldcg(a.state + S_P + tid - 9);
     sm.tp[tid - 9] = a.prop[S_P + tid - 9];
+  }
+}
+
+// Current-pose constants: R, t of the packed state `st`, and the covariance blocks Ptt / Ppp of P (19 x 19) that pv.var
+// uses (:377-378; state_.cov only changes after the loop, :489: P == nullptr keeps the blocks already in place). global: st
+// and P are the update's state in global memory, else the CTA's resident copies. Ends with a CTA barrier.
+__device__ __forceinline__ void lio_pose_consts(LioSmem &sm, const double *st, const double *P, bool global) {
+  const int tid = threadIdx.x;
+  if (tid < 9) {
+    const int r = tid / 3, c = tid % 3;
+    sm.R[tid] = ld_state(st + S_R + tid, global);
+    if (P) {
+      sm.Ptt[tid] = ld_state(P + r * 19 + c, global);
+      sm.Ppp[tid] = ld_state(P + (3 + r) * 19 + (3 + c), global);
+    }
+  } else if (tid < 12) {
+    sm.t[tid - 9] = ld_state(st + S_P + tid - 9, global);
   }
   __syncthreads();
 }
@@ -876,7 +889,8 @@ __global__ void __launch_bounds__(LIO_THREADS, 1) lio_residual_kernel(const LioK
   LioSmem &sm = *reinterpret_cast<LioSmem *>(smem_raw);
   lio_init_cold(sm, a);
   lio_init_barriers(sm);
-  lio_load_consts(sm, a);
+  lio_prior_consts(sm, a);
+  lio_pose_consts(sm, a.state, a.state + S_COV, true);
   double D0 = 0.0, D1 = 0.0;  // this lane's two entries of the warp's 8x8 block
   int cnt = 0;
   int lo, hi;

@@ -3,8 +3,8 @@
 //
 //   lio_solve_block / lio_solve_kernel : src/voxel_map.cpp:462-499  (K_1, G, solution, state_ += solution, convergence /
 //                                        rematch / (I-G)P)
-//   vio_solve_block / vio_solve_kernel : src/vio.cpp:1636-1685 + :800 (error-gated accept / rollback, K_1, G, solution, final
-//                                        cov -= G cov)
+//   vio_solve_block / vio_solve_kernel : src/vio.cpp:1636-1685 (error-gated accept / rollback, K_1, G, solution)
+//   vio_final_cov                      : src/vio.cpp:800 (cov -= G cov after the last level)
 //
 // Gain: the reference computes K_1 = (H^T H + P^-1)^-1 with two 19x19 partial-pivot inversions and then only uses the
 // first m (6 or 7) columns of K_1. Because H^T H is zero outside its leading m x m block A, the push-through identity gives
@@ -241,8 +241,6 @@ __device__ inline void gain_rows(SolveSmem &sm, double pscale, int solve_mode, i
   for (int i = 0; i < m; i++) x[i] = __shfl_sync(0xffffffffu, col[i], (lane + m) & 31);
 }
 
-__device__ inline double warp_norm3(const double *v) { return norm3_rn(v); }
-
 #define SOLVE_THREADS 512
 
 // Staging shared by both solve routines: one global round trip brings P, info, the pose parts of state / prior / old_state.
@@ -273,6 +271,17 @@ __device__ __forceinline__ void solve_load(SolveSmem &sm, SolveIO &io, const Sol
     io.pr[t] = r0;
     if (want_old) io.old[t] = o0;
   }
+}
+
+// What a persistent kernel keeps resident or prepares in its prologue and grid-barrier wait, staged by a per-iteration solve
+// launch: the inputs, vec = state_propagat (-) state on warp 1 and the loop invariants of the gain on warp 2.
+template <int m> __device__ __forceinline__ void solve_stage(SolveSmem &sm, SolveIO &io, const SolveArgs &a, double pscale, bool want_old) {
+  const int tid = threadIdx.x, lane = tid & 31;
+  solve_load(sm, io, a, want_old);
+  __syncthreads();
+  if (tid >= 32 && tid < 64) boxminus_warp(io.pr, io.st, sm.vec, lane);
+  if (tid >= 64 && tid < 96 && a.solve_mode == 0) gain_setup<m>(sm, pscale, lane);
+  __syncthreads();
 }
 
 // m x m information block and H^T z out of the compact vector (mirrored), by one warp.
@@ -308,21 +317,12 @@ __device__ __forceinline__ void lio_write_stats(const SolveArgs &a, SolveSmem &s
 
 // One LIO gain solve + state update (src/voxel_map.cpp:462-499) by the calling block. Returns EKF_stop_flg.
 // `ctrl` is the loop-control block the routine reads and updates (global memory for the per-iteration kernels, the CTA's
-// shared-memory copy inside the persistent kernel). resident: P / poses / info are already staged in sm / io.
-// vec_ready: state_propagat (-) state_ is already in sm.vec (the persistent kernel evaluates it inside the barrier wait).
-__device__ __noinline__ bool lio_solve_block(const SolveArgs &a, SolveSmem &sm, SolveIO &io, Ctrl &ctrl, bool resident, bool vec_ready) {
+// shared-memory copy inside the persistent kernel). Expects P, the poses and info in sm / io, vec = state_propagat (-) state_
+// (:470) in sm.vec and, in solve_mode 0, gain_setup<6> done: solve_stage or the persistent kernel's prologue and barrier wait.
+__device__ __noinline__ bool lio_solve_block(const SolveArgs &a, SolveSmem &sm, SolveIO &io, Ctrl &ctrl) {
   const int tid = threadIdx.x, lane = tid & 31;
   const int iterCount = ctrl.iter;
   const int rematch0 = ctrl.rematch_num;
-  if (!resident) {
-    solve_load(sm, io, a, false);
-    __syncthreads();
-  }
-  if (!vec_ready) {
-    if (tid >= 32 && tid < 64) boxminus_warp(io.pr, io.st, sm.vec, lane);  // vec = state_propagat (-) state_ (:470)
-    if (!resident && tid >= 64 && tid < 96 && a.solve_mode == 0) gain_setup<6>(sm, 1.0, lane);  // per-iteration launches: nothing is kept
-    __syncthreads();
-  }
   if (tid < 32) {
     unpack_info<6>(sm, io, lane);  // H^T R^-1 H, H^T R^-1 z
     double x[6], g[6];
@@ -349,7 +349,7 @@ __device__ __noinline__ bool lio_solve_block(const SolveArgs &a, SolveSmem &sm, 
     boxplus_warp(io.st, sm.sol, lane);  // state_ += solution (:474)
     if (a.dbg && tid == 0) a.dbg[1] = globaltimer_ns();
     if (lane == 0) {
-      const bool converged = (warp_norm3(sm.sol) * 57.3 < 0.01) && (warp_norm3(sm.sol + 3) * 100 < 0.015);  // :477
+      const bool converged = (norm3_rn(sm.sol) * 57.3 < 0.01) && (norm3_rn(sm.sol + 3) * 100 < 0.015);  // :477
       int rematch = rematch0;
       if (converged || ((rematch == 0) && (iterCount == (a.max_iterations - 2)))) rematch++;  // :482
       const bool stop = (rematch >= 2) || (iterCount == a.max_iterations - 1);                // :485
@@ -386,15 +386,16 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 1) lio_solve_kernel(const Solve
   __shared__ Ctrl ctrl;
   if (threadIdx.x == 0) sm.W = lit.W, sm.K = lit.K, ctrl = *a.ctrl;
   __syncthreads();
-  lio_solve_block(a, sm, io, ctrl, false, false);
+  solve_stage<6>(sm, io, a, 1.0, false);
+  lio_solve_block(a, sm, io, ctrl);
   __syncthreads();
   if (threadIdx.x == 0) a.ctrl->iter = ctrl.iter, a.ctrl->rematch_num = ctrl.rematch_num, a.ctrl->stop = ctrl.stop;
 }
 
 __device__ __forceinline__ void vio_write_stats(const SolveArgs &a, SolveSmem &sm, SolveIO &io) {
   const int tid = threadIdx.x, level = a.level, iteration = a.slot_iter;
-  const bool accepted = io.flags[0] != 0, ran = io.flags[2] != 0;
-  if (ran && a.vio_stats && level < 8) {
+  const bool accepted = io.flags[0] != 0;
+  if (a.vio_stats && level < 8) {
     esikf_vio_stats &S = *a.vio_stats;
     if (accepted && iteration < 8) {
       for (int t = tid; t < 49; t += blockDim.x) S.HTH[level][iteration][t] = sm.A[t];
@@ -410,107 +411,88 @@ __device__ __forceinline__ void vio_write_stats(const SolveArgs &a, SolveSmem &s
   }
 }
 
-// One VIO accept/rollback + gain solve (src/vio.cpp:1636-1685) by the calling block; on the last slot also the final
-// covariance update (:800). Returns EKF_end of the level. vec_ready as for lio_solve_block.
-__device__ __noinline__ bool vio_solve_block(const SolveArgs &a, SolveSmem &sm, SolveIO &io, Ctrl &ctrl, bool resident, bool vec_ready) {
+// One VIO accept/rollback + gain solve (src/vio.cpp:1636-1685) by the calling block, for an iteration of a level that has
+// not ended (EKF_end). Returns EKF_end. Expects the same staging as lio_solve_block, with gain_setup<7>.
+__device__ __noinline__ bool vio_solve_block(const SolveArgs &a, SolveSmem &sm, SolveIO &io, Ctrl &ctrl) {
   const int tid = threadIdx.x, lane = tid & 31;
-  const bool level_done_in = (a.slot_iter == 0) ? false : (ctrl.level_done != 0);   // entering a level: EKF_end = false (vio.cpp:1527)
-  const float last_error_in = (a.slot_iter == 0) ? FLT_MAX : ctrl.last_error;       // :1528
-  const int has_G_in = ctrl.has_G;
-  if (level_done_in && !a.last_slot) return true;
-  if (!resident) {
-    solve_load(sm, io, a, a.slot_iter != 0);
-    __syncthreads();
-  }
-  if (!vec_ready && !level_done_in) {
-    // vec = state_propagat (-) state (:1664) on warp 1
-    if (tid >= 32 && tid < 64) boxminus_warp(io.pr, io.st, sm.vec, lane);
-    if (!resident && tid >= 64 && tid < 96 && a.solve_mode == 0) gain_setup<7>(sm, 1.0 / a.img_point_cov, lane);  // per-iteration launches: nothing is kept
-    __syncthreads();
-  }
+  const float last_error_in = (a.slot_iter == 0) ? FLT_MAX : ctrl.last_error;  // entering a level (vio.cpp:1527-1528)
   if (tid < 32) {
-    bool accepted = false, ekf_end = level_done_in;
-    float error = 0.f, last_error = last_error_in;
-    if (!level_done_in) {
-      if (a.slot_iter == 0 && lane < 25) io.old[lane] = io.st[lane];  // old_state = *state at level entry (:1523)
-      // error = sum(res^2) / n_meas as float (vio.cpp:1636)
-      const double sum_sq = io.info[INFO_EXTRA(7)];
-      const int n_meas = (int)io.info[INFO_COUNTM(7)];
-      error = __fdiv_rn((float)sum_sq, (float)n_meas);
-      if (error <= last_error) {  // :1648
-        accepted = true;
-        if (lane < 25) io.old[lane] = io.st[lane];  // old_state = *state
-        last_error = error;
-        unpack_info<7>(sm, io, lane);  // H^T H 7x7, H^T z
-        double x[7];
-        gain_rows<7>(sm, 1.0 / a.img_point_cov, a.solve_mode, lane, x);
-        if (a.dbg && tid == 0) a.dbg[0] = globaltimer_ns();
-        double g[7];
+    bool accepted = false, ekf_end;
+    float last_error = last_error_in;
+    if (a.slot_iter == 0 && lane < 25) io.old[lane] = io.st[lane];  // old_state = *state at level entry (:1523)
+    // error = sum(res^2) / n_meas as float (vio.cpp:1636)
+    const double sum_sq = io.info[INFO_EXTRA(7)];
+    const int n_meas = (int)io.info[INFO_COUNTM(7)];
+    const float error = __fdiv_rn((float)sum_sq, (float)n_meas);
+    if (error <= last_error) {  // :1648
+      accepted = true;
+      if (lane < 25) io.old[lane] = io.st[lane];  // old_state = *state
+      last_error = error;
+      unpack_info<7>(sm, io, lane);  // H^T H 7x7, H^T z
+      double x[7];
+      gain_rows<7>(sm, 1.0 / a.img_point_cov, a.solve_mode, lane, x);
+      if (a.dbg && tid == 0) a.dbg[0] = globaltimer_ns();
+      double g[7];
 #pragma unroll
-        for (int j = 0; j < 7; j++) {
-          double s = 0.0;
+      for (int j = 0; j < 7; j++) {
+        double s = 0.0;
 #pragma unroll
-          for (int k = 0; k < 7; k++) s += x[k] * sm.A[k * 7 + j];
-          g[j] = s;
-        }
-        if (lane < 19) {
-          double s1 = 0.0, s2 = 0.0;
-#pragma unroll
-          for (int k = 0; k < 7; k++) s1 += x[k] * sm.HTz[k], s2 += g[k] * sm.vec[k];
-          sm.sol[lane] = -s1 + sm.vec[lane] - s2;  // :1667
-#pragma unroll
-          for (int j = 0; j < 7; j++) io.g[lane][j] = g[j];  // G.block<19,7>  (:1665)
-        }
-        __syncwarp();
-        boxplus_warp(io.st, sm.sol, lane);
-        if (a.dbg && tid == 0) a.dbg[1] = globaltimer_ns();
-        // :1675 (float constants 57.3f / 100.0f / 0.001f promote to double against the double norm)
-        ekf_end = (warp_norm3(sm.sol) * (double)57.3f < (double)0.001f) && (warp_norm3(sm.sol + 3) * (double)100.0f < (double)0.001f);
-      } else {
-        __syncwarp();
-        if (lane < 25) io.st[lane] = io.old[lane];  // *state = old_state  (:1679)
-        ekf_end = true;
+        for (int k = 0; k < 7; k++) s += x[k] * sm.A[k * 7 + j];
+        g[j] = s;
       }
+      if (lane < 19) {
+        double s1 = 0.0, s2 = 0.0;
+#pragma unroll
+        for (int k = 0; k < 7; k++) s1 += x[k] * sm.HTz[k], s2 += g[k] * sm.vec[k];
+        sm.sol[lane] = -s1 + sm.vec[lane] - s2;  // :1667
+#pragma unroll
+        for (int j = 0; j < 7; j++) io.g[lane][j] = g[j];  // G.block<19,7>  (:1665)
+      }
+      __syncwarp();
+      boxplus_warp(io.st, sm.sol, lane);
+      if (a.dbg && tid == 0) a.dbg[1] = globaltimer_ns();
+      // :1675 (float constants 57.3f / 100.0f / 0.001f promote to double against the double norm)
+      ekf_end = (norm3_rn(sm.sol) * (double)57.3f < (double)0.001f) && (norm3_rn(sm.sol + 3) * (double)100.0f < (double)0.001f);
+    } else {
+      __syncwarp();
+      if (lane < 25) io.st[lane] = io.old[lane];  // *state = old_state  (:1679)
+      ekf_end = true;
     }
     if (lane == 0) {
-      io.flags[0] = accepted, io.flags[1] = ekf_end, io.flags[2] = !level_done_in;
+      io.flags[0] = accepted, io.flags[1] = ekf_end;
       reinterpret_cast<float *>(io.flags)[3] = last_error;
       reinterpret_cast<float *>(io.flags)[4] = error;
-      if (!level_done_in) {
-        ctrl.iter += 1;
-        ctrl.last_error = last_error;
-        if (a.slot_iter == 0) ctrl.accepted_in_level = 0;
-        if (accepted) ctrl.has_G = 1, ctrl.accepted_in_level += 1;
-      }
+      ctrl.iter += 1;
+      ctrl.last_error = last_error;
+      if (accepted) ctrl.has_G = 1;
       ctrl.level_done = ekf_end;
-      if (a.last_slot) ctrl.stop = 1;
     }
   }
   __syncthreads();
-  const bool accepted = io.flags[0] != 0, ran = io.flags[2] != 0;
-  if (ran && !a.no_publish) {
+  if (!a.no_publish) {
     for (int t = tid; t < 25; t += blockDim.x) {
       a.state[t] = io.st[t];
       a.old_state[t] = io.old[t];
     }
-    if (accepted)
+    if (io.flags[0])
       for (int t = tid; t < 133; t += blockDim.x) a.G[t] = io.g[t / 7][t % 7];
     vio_write_stats(a, sm, io);
-  }
-  if (a.last_slot && !a.no_publish) {
-    // state->cov -= G * state->cov   (vio.cpp:800) with the last accepted G (this slot's if accepted, else the stored one)
-    const bool haveG = accepted || has_G_in;
-    if (haveG)
-      for (int t = tid; t < 361; t += blockDim.x) {
-        const int r = t / 19, c = t - 19 * r;
-        double s = 0.0;
-        for (int j = 0; j < 7; j++) s += (accepted ? io.g[r][j] : __ldcg(a.G + r * 7 + j)) * sm.P[j * 19 + c];
-        a.state[S_COV + t] = sm.P[t] - s;
-      }
   }
   return io.flags[1] != 0;
 }
 
+// state->cov -= G * state->cov (vio.cpp:800), once after the last level, by the whole block; the caller checks that some
+// update was accepted (Ctrl::has_G). G is the last accepted gain block: io.g when `fresh`, else the stored a.G.
+__device__ __forceinline__ void vio_final_cov(const SolveArgs &a, const SolveSmem &sm, const SolveIO &io, bool fresh) {
+  for (int t = threadIdx.x; t < 361; t += blockDim.x) {
+    const int r = t / 19, c = t - 19 * r;
+    double s = 0.0;
+    for (int j = 0; j < 7; j++) s += (fresh ? io.g[r][j] : __ldcg(a.G + r * 7 + j)) * sm.P[j * 19 + c];
+    a.state[S_COV + t] = sm.P[t] - s;
+  }
+}
+
+// One (level, iteration) slot of the per-iteration VIO path; the last slot also applies the final covariance update.
 __global__ void __launch_bounds__(SOLVE_THREADS, 1) vio_solve_kernel(const SolveArgs a) {
   __shared__ SolveSmem sm;
   __shared__ SolveIO io;
@@ -518,7 +500,18 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 1) vio_solve_kernel(const Solve
   __shared__ Ctrl ctrl;
   if (threadIdx.x == 0) sm.W = lit.W, sm.K = lit.K, ctrl = *a.ctrl;
   __syncthreads();
-  vio_solve_block(a, sm, io, ctrl, false, false);
+  const bool run = a.slot_iter == 0 || !ctrl.level_done;  // EKF_end: the remaining slots of the level do nothing (vio.cpp:1685)
+  if (!run && !a.last_slot) return;
+  bool fresh = false;
+  if (run) {
+    solve_stage<7>(sm, io, a, 1.0 / a.img_point_cov, a.slot_iter != 0);
+    vio_solve_block(a, sm, io, ctrl);
+    fresh = io.flags[0] != 0;
+  } else {
+    solve_load(sm, io, a, false);  // P for the covariance update
+    __syncthreads();
+  }
+  if (a.last_slot && ctrl.has_G) vio_final_cov(a, sm, io, fresh);
   __syncthreads();
   if (threadIdx.x == 0) {
     const unsigned bc = a.ctrl->block_counter;

@@ -148,25 +148,50 @@ struct __align__(128) VioSmem {
   ReduceSmem<VIO_WARPS> red;
 };
 
-// Per-iteration constants of updateState (vio.cpp:1540-1544): Rcw, Pcw, inv_expo_time.
-__device__ __forceinline__ void vio_load_consts(VioSmem &sm, const VioKernelArgs &a) {
+// Per-iteration constants of updateState (vio.cpp:1540-1544): Rcw, Pcw, inv_expo_time of the packed state `st` (global: the
+// update's state in global memory, else the CTA's resident copy).
+__device__ __forceinline__ void vio_load_consts(VioSmem &sm, const VioKernelArgs &a, const double *st, bool global) {
   const int tid = threadIdx.x;
   if (tid < 9) {
     // Rcw = Rci * Rwi^T  (vio.cpp:1542)
-    int r = tid / 3, c = tid % 3;
+    const int r = tid / 3, c = tid % 3;
     double s = 0;
-    for (int k = 0; k < 3; k++) s += a.Rci[r * 3 + k] * __ldcg(a.state + S_R + c * 3 + k);
+    for (int k = 0; k < 3; k++) s += a.Rci[r * 3 + k] * ld_state(st + S_R + c * 3 + k, global);
     sm.Rcw[tid] = s;
   }
-  if (tid == 0) sm.inv_expo = __ldcg(a.state + S_EXPO);
+  if (tid == 0) sm.inv_expo = ld_state(st + S_EXPO, global);
   __syncthreads();
   if (tid < 3) {
     // Pcw = -Rci Rwi^T Pwi + Pci  (:1543)
     double s = 0;
-    for (int k = 0; k < 3; k++) s += sm.Rcw[tid * 3 + k] * __ldcg(a.state + S_P + k);
+    for (int k = 0; k < 3; k++) s += sm.Rcw[tid * 3 + k] * ld_state(st + S_P + k, global);
     sm.Pcw[tid] = -s + a.Pci[tid];
   }
   __syncthreads();
+}
+
+// Bilinear tap geometry of a patch centred at (pcu, pcv) on pyramid level `level` (vio.cpp:1580-1589, 203-225): the integer
+// tap base (u, v) and the four weights, float via double (1.0 - subpix). The reference divides by scale = 2^level; this
+// multiplies by 2^-level, assembled from its exponent bits. x / 2^level and x * 2^-level are both the correctly rounded value
+// of the same real number, in float and in double, so the results are bit-identical.
+struct TapGeom {
+  int u, v;
+  float w_tl, w_tr, w_bl, w_br;
+};
+__device__ __forceinline__ TapGeom tap_geometry(double pcu, double pcv, int level) {
+  const int scale = 1 << level;
+  const float inv_scale = __int_as_float((127 - level) << 23);
+  const double inv_scale_d = __longlong_as_double((long long)(1023 - level) << 52);
+  TapGeom g;
+  g.u = (int)(floorf((float)(pcu * inv_scale_d)) * scale);
+  g.v = (int)(floorf((float)(pcv * inv_scale_d)) * scale);
+  const float subpix_u = __fmul_rn((float)pcu - (float)g.u, inv_scale);
+  const float subpix_v = __fmul_rn((float)pcv - (float)g.v, inv_scale);
+  g.w_tl = (float)((1.0 - subpix_u) * (1.0 - subpix_v));
+  g.w_tr = (float)(subpix_u * (1.0 - subpix_v));
+  g.w_bl = (float)((1.0 - subpix_u) * subpix_v);
+  g.w_br = subpix_u * subpix_v;
+  return g;
 }
 
 __device__ __forceinline__ void vio_cache_reset(VioSmem &sm) {
@@ -206,24 +231,13 @@ __device__ __forceinline__ void vio_process_range(const VioKernelArgs &a, VioSme
     const double X = c.X, Y = c.Y, Z = c.Z, inv_ref_expo = c.inv_ref_expo;
     const int pyramid_level = level + search_level;
     const int scale = 1 << pyramid_level;
-    // 2^-pyramid_level assembled from its exponent bits — the value 1.0f / (float)scale has; x / 2^k == x * 2^-k exactly
-    const float inv_scale = __int_as_float((127 - pyramid_level) << 23);
-    const double inv_scale_d = __longlong_as_double((long long)(1023 - pyramid_level) << 52);
+    const float inv_scale = __int_as_float((127 - pyramid_level) << 23);  // 1.0f / scale
     const double pf0 = sm.Rcw[0] * X + sm.Rcw[1] * Y + sm.Rcw[2] * Z + sm.Pcw[0];
     const double pf1 = sm.Rcw[3] * X + sm.Rcw[4] * Y + sm.Rcw[5] * Z + sm.Pcw[1];
     const double pf2 = sm.Rcw[6] * X + sm.Rcw[7] * Y + sm.Rcw[8] * Z + sm.Pcw[2];
     double pcu, pcv;
     world2cam(a.cam, pf0, pf1, pf2, pcu, pcv);
-    // bilinear weights (:1580-1589) — float, via double (1.0 - subpix)
-    const float u_ref = (float)pcu, v_ref = (float)pcv;
-    const int u_ref_i = (int)(floorf((float)(pcu * inv_scale_d)) * scale);
-    const int v_ref_i = (int)(floorf((float)(pcv * inv_scale_d)) * scale);
-    const float subpix_u = __fmul_rn(u_ref - (float)u_ref_i, inv_scale);
-    const float subpix_v = __fmul_rn(v_ref - (float)v_ref_i, inv_scale);
-    const float w_tl = (float)((1.0 - subpix_u) * (1.0 - subpix_v));
-    const float w_tr = (float)(subpix_u * (1.0 - subpix_v));
-    const float w_bl = (float)((1.0 - subpix_u) * subpix_v);
-    const float w_br = subpix_u * subpix_v;
+    const TapGeom tg = tap_geometry(pcu, pcv, pyramid_level);
 
     // the 11 x 11 tap footprint: tile (r, c) <-> image linear index base0 + r*scale*width + c*scale, where tile (1,1) is the
     // top-left tap of patch pixel (0,0) (:1597). Staged only when the footprint moved.
@@ -231,12 +245,12 @@ __device__ __forceinline__ void vio_process_range(const VioKernelArgs &a, VioSme
     float tv[4] = {0.f, 0.f, 0.f, 0.f};
     bool restage, by_tma = false;
     {
-      const long long base0 = (long long)(v_ref_i - 5 * scale) * width + (u_ref_i - 5 * scale);
+      const long long base0 = (long long)(tg.v - 5 * scale) * width + (tg.u - 5 * scale);
       const bool repv = (c.pv_level != level);
       restage = (c.tile_scale != scale || c.tile_base0 != base0);
       __syncwarp();
       if (restage) {
-        const int x0 = u_ref_i - 5 * scale, y0 = v_ref_i - 5 * scale;
+        const int x0 = tg.u - 5 * scale, y0 = tg.v - 5 * scale;
         by_tma = tma && pyramid_level <= VIO_TMA_MAXLVL && x0 >= 0 && y0 >= 0 && x0 + 10 * scale < width && y0 + 10 * scale < a.cam.height;
         if (by_tma) {
           if (lane == 0) {
@@ -283,7 +297,7 @@ __device__ __forceinline__ void vio_process_range(const VioKernelArgs &a, VioSme
         mbar_wait(&sm.tma_bar[warp], *tma_phase & 1u);
         *tma_phase ^= 1u;
         const unsigned inner = VIO_TMA_INNER(pyramid_level);
-        const unsigned char *raw = sm.tile[warp] + ((u_ref_i - 5 * scale) & 15);  // the box starts at the 16-byte boundary below the first tap
+        const unsigned char *raw = sm.tile[warp] + ((tg.u - 5 * scale) & 15);  // the box starts at the 16-byte boundary below the first tap
 #pragma unroll
         for (int q = 0; q < 4; q++) {
           const int t = lane + 32 * q;
@@ -307,7 +321,7 @@ __device__ __forceinline__ void vio_process_range(const VioKernelArgs &a, VioSme
       if (g < 100) {
         const int ga = g / 10, gb = g - 10 * ga;
         const float *t0 = sT + ga * 11 + gb;
-        sG[g] = bil(w_tl, w_tr, w_bl, w_br, t0[0], t0[1], t0[11], t0[12]);
+        sG[g] = bil(tg.w_tl, tg.w_tr, tg.w_bl, tg.w_br, t0[0], t0[1], t0[11], t0[12]);
       }
     }
     __syncwarp();
@@ -363,7 +377,7 @@ __global__ void __launch_bounds__(VIO_THREADS, 1) vio_patch_kernel(const VioKern
   if (a.slot_iter > 0 && a.ctrl->level_done) return;  // EKF_end of this level: remaining slots do nothing
   extern __shared__ __align__(128) unsigned char smem_raw[];
   VioSmem &sm = *reinterpret_cast<VioSmem *>(smem_raw);
-  vio_load_consts(sm, a);
+  vio_load_consts(sm, a, a.state, true);
   double D0 = 0.0, D1 = 0.0, n_meas = 0.0;
   int lo, hi;
   vio_block_range(a.count, lo, hi);
@@ -379,21 +393,12 @@ __global__ void image_patch_kernel(const uint8_t *__restrict__ img, int width, i
   int gid = blockIdx.x * blockDim.x + threadIdx.x;
   if (gid >= n * 64) return;
   int i = gid >> 6, pix = gid & 63, x = pix >> 3, y = pix & 7;
-  const double pcu = pc[2 * i], pcv = pc[2 * i + 1];
   const int scale = 1 << level;
-  const float u_ref = (float)pcu, v_ref = (float)pcv;
-  const int u_ref_i = (int)(floorf((float)(pcu / scale)) * scale);
-  const int v_ref_i = (int)(floorf((float)(pcv / scale)) * scale);
-  const float subpix_u = (u_ref - (float)u_ref_i) / (float)scale;
-  const float subpix_v = (v_ref - (float)v_ref_i) / (float)scale;
-  const float w_tl = (float)((1.0 - subpix_u) * (1.0 - subpix_v));
-  const float w_tr = (float)(subpix_u * (1.0 - subpix_v));
-  const float w_bl = (float)((1.0 - subpix_u) * subpix_v);
-  const float w_br = subpix_u * subpix_v;
+  const TapGeom tg = tap_geometry(pc[2 * i], pc[2 * i + 1], level);
   const long npix = (long)width * height;
-  const long b = (long)(v_ref_i - 4 * scale + x * scale) * width + (u_ref_i - 4 * scale) + (long)y * scale;
+  const long b = (long)(tg.v - 4 * scale + x * scale) * width + (tg.u - 4 * scale) + (long)y * scale;
   const long sw = (long)scale * width;
-  out[gid] = bil(w_tl, w_tr, w_bl, w_br, tap(img, b, npix), tap(img, b + scale, npix), tap(img, b + sw, npix), tap(img, b + sw + scale, npix));
+  out[gid] = bil(tg.w_tl, tg.w_tr, tg.w_bl, tg.w_br, tap(img, b, npix), tap(img, b + scale, npix), tap(img, b + sw, npix), tap(img, b + sw + scale, npix));
 }
 
 // getWarpMatrixAffineHomography + getBestSearchLevel for the normal_en branch of retrieveFromVisualSparseMap (vio.cpp:699-715).
@@ -534,22 +539,14 @@ __device__ __forceinline__ void vio_inverse_precompute_patch(const VioKernelArgs
     Cm[r][1] = -B[r][0] * Z + B[r][2] * X;
     Cm[r][2] = B[r][0] * Y - B[r][1] * X;
   }
-  const double pcu = v.ref_px[2 * (size_t)i], pcv = v.ref_px[2 * (size_t)i + 1];
-  const float u_ref = (float)pcu, v_ref = (float)pcv;
-  const int u_ref_i = (int)(floorf((float)(pcu / scale)) * scale);
-  const int v_ref_i = (int)(floorf((float)(pcv / scale)) * scale);
-  const float subpix_u = (u_ref - (float)u_ref_i) / (float)scale;
-  const float subpix_v = (v_ref - (float)v_ref_i) / (float)scale;
-  const float w_tl = (float)((1.0 - subpix_u) * (1.0 - subpix_v));
-  const float w_tr = (float)(subpix_u * (1.0 - subpix_v));
-  const float w_bl = (float)((1.0 - subpix_u) * subpix_v);
-  const float w_br = subpix_u * subpix_v;
+  const TapGeom tg = tap_geometry(v.ref_px[2 * (size_t)i], v.ref_px[2 * (size_t)i + 1], level);
+  const float w_tl = tg.w_tl, w_tr = tg.w_tr, w_bl = tg.w_bl, w_br = tg.w_br;
   const double inv_scale = 1.0 / scale;
   const long sw = (long)scale * width;
 #pragma unroll
   for (int k = 0; k < 2; k++) {
     const int pix = 2 * lane + k, x = pix >> 3, y = pix & 7;
-    const long b = (long)(v_ref_i + x * scale - 4 * scale) * width + (u_ref_i - 4 * scale) + (long)y * scale;
+    const long b = (long)(tg.v + x * scale - 4 * scale) * width + (tg.u - 4 * scale) + (long)y * scale;
     const float du = __fmul_rn(0.5f, __fsub_rn(bil(w_tl, w_tr, w_bl, w_br, tap(img, b + scale, npix), tap(img, b + 2 * scale, npix), tap(img, b + sw + scale, npix),
                                                  tap(img, b + sw + 2 * scale, npix)),
                                              bil(w_tl, w_tr, w_bl, w_br, tap(img, b - scale, npix), tap(img, b, npix), tap(img, b + sw - scale, npix), tap(img, b + sw, npix))));
@@ -591,23 +588,15 @@ __device__ __forceinline__ void vio_inverse_process_range(const VioKernelArgs &a
     const double pf2 = sm.Rcw[6] * X + sm.Rcw[7] * Y + sm.Rcw[8] * Z + sm.Pcw[2];
     double pcu, pcv;
     world2cam(a.cam, pf0, pf1, pf2, pcu, pcv);
-    const float u_ref = (float)pcu, v_ref = (float)pcv;
-    const int u_ref_i = (int)(floorf((float)(pcu / scale)) * scale);
-    const int v_ref_i = (int)(floorf((float)(pcv / scale)) * scale);
-    const float subpix_u = (u_ref - (float)u_ref_i) / (float)scale;
-    const float subpix_v = (v_ref - (float)v_ref_i) / (float)scale;
-    const float w_tl = (float)((1.0 - subpix_u) * (1.0 - subpix_v));
-    const float w_tr = (float)(subpix_u * (1.0 - subpix_v));
-    const float w_bl = (float)((1.0 - subpix_u) * subpix_v);
-    const float w_br = subpix_u * subpix_v;
+    const TapGeom tg = tap_geometry(pcu, pcv, level);
     const float2 Pv = *reinterpret_cast<const float2 *>(a.warp_patch + (size_t)i * 64 * a.levels + 64 * level + 2 * lane);
     const long sw = (long)scale * width;
     double sq = 0.0;
 #pragma unroll
     for (int k = 0; k < 2; k++) {
       const int pix = 2 * lane + k, x = pix >> 3, y = pix & 7;
-      const long b = (long)(v_ref_i + x * scale - 4 * scale) * width + (u_ref_i - 4 * scale) + (long)y * scale;
-      const float cur = bil(w_tl, w_tr, w_bl, w_br, tap(a.img, b, npix), tap(a.img, b + scale, npix), tap(a.img, b + sw, npix), tap(a.img, b + sw + scale, npix));
+      const long b = (long)(tg.v + x * scale - 4 * scale) * width + (tg.u - 4 * scale) + (long)y * scale;
+      const float cur = bil(tg.w_tl, tg.w_tr, tg.w_bl, tg.w_br, tap(a.img, b, npix), tap(a.img, b + scale, npix), tap(a.img, b + sw, npix), tap(a.img, b + sw + scale, npix));
       const double res = (double)__fsub_rn(cur, k == 0 ? Pv.x : Pv.y);  // float residual, then widened (:1466-1468)
       const double *hi6 = v.H_sub_inv + ((size_t)lp * 64 + pix) * 6;
       const double r0 = hi6[0], r1 = hi6[1], r2 = hi6[2], t0 = hi6[3], t1 = hi6[4], t2 = hi6[5];
@@ -650,7 +639,7 @@ __global__ void __launch_bounds__(VIO_THREADS, 1) vio_inverse_patch_kernel(const
   extern __shared__ __align__(128) unsigned char smem_raw[];
   VioSmem &sm = *reinterpret_cast<VioSmem *>(smem_raw);
   __shared__ double Rwi[9], Pwi[3];
-  vio_load_consts(sm, a);
+  vio_load_consts(sm, a, a.state, true);
   if (threadIdx.x < 9) Rwi[threadIdx.x] = __ldcg(a.state + S_R + threadIdx.x);
   if (threadIdx.x < 3) Pwi[threadIdx.x] = __ldcg(a.state + S_P + threadIdx.x);
   __syncthreads();
