@@ -10,12 +10,12 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
 import oracle_bind as O  # noqa: E402
-from test_oracle_ref_pin import _case  # noqa: E402
+from ref_pin_cases import lio_case, vio_inputs  # noqa: E402
 
 assert O.ref_lio_available(), "build oracle/_ref first (make -C oracle)"
 out = {}
 for name in ("small", "hilti_voxel_04_non_identity_extrinsics"):
-    fr, cfg = _case(name)
+    fr, cfg = lio_case(name)
     r = O.ref_lio_state_estimation(fr, cfg=cfg)
     out[f"{name}_iters"] = np.int32(r["iters"])
     for k in ("M", "ptpl_center", "ptpl_dis", "normals", "state"):
@@ -25,11 +25,9 @@ print("wrote", os.path.join(HERE, "ref_lio_golden.npz"), {k: np.asarray(v).shape
 
 # ---- VIO half: oracle/_ref/libfl2_ref_vio.so = /root/reference/src/vio.cpp (+ frame.cpp, visual_point.cpp, voxel_map.cpp)
 if O.ref_vio_available():
-    from test_oracle_ref_pin_vio import _inputs  # noqa: E402
-
     vout = {}
     for name in ("small", "exposure"):
-        fr, prior, w = _inputs(name)
+        fr, prior, w = vio_inputs(name)
         r = O.RefVIO(fr["cam_cfg"], fr["ext"], fr["vio_cfg"]).update(fr["img"], fr["vis_pos"], w["warp_patch"], w["search_levels"], fr["inv_ref_expo"], prior, prior)
         vout[f"{name}_state"], vout[f"{name}_errors"], vout[f"{name}_warp_patch"] = r["state"], r["errors"], w["warp_patch"]
         vout[f"{name}_search_levels"], vout[f"{name}_prior"] = w["search_levels"], prior

@@ -1,14 +1,40 @@
-"""ctypes binding of tests/map_host_harness.cu (the device voxel-map state machine compiled for the host) + the comparison of
-two flattened maps (keys / candidate lists / plane records) used by the CPU and GPU map tests."""
+"""ctypes binding of tests/map_host_harness.cu (the device voxel-map state machine compiled for the host), the comparison of
+two flattened maps (keys / candidate lists / plane records) and the point streams and oracle map updates used by the CPU and
+GPU map tests."""
 import ctypes as C
 
 import numpy as np
 
 import __graft_entry__
 import oracle_bind as O
+from fast_livo2_b200 import synthetic as S
 from fast_livo2_b200.synthetic import PLANE_DTYPE
 
 SO = __graft_entry__.MAP_HARNESS_LIB
+
+
+def tick_points(rng, rects, n, lo, hi, noise=0.01):
+    """n noisy points on the scene's planes inside the axis-aligned window [lo, hi] (the sensor's footprint of this tick),
+    float32-rounded like TransformLidar's output (src/voxel_map.cpp:524-526), each with a small SPD covariance."""
+    pw, _ = S.sample_on_rects(rects, 6 * n, rng)
+    pw = pw[np.all((pw >= lo) & (pw <= hi), axis=1)][:n]
+    pw = pw + rng.normal(0, noise, pw.shape)
+    pw = pw.astype(np.float32).astype(np.float64)
+    A = rng.normal(0, 0.01, (len(pw), 3, 3))
+    var = A @ A.transpose(0, 2, 1) + np.eye(3) * 1e-5
+    return pw, var
+
+
+def oracle_map(cfg):
+    """An oracle LIO instance whose map the tests grow with oracle_update_map."""
+    return O.OracleLIO(cfg, S.avia_extrinsics())
+
+
+def oracle_update_map(orc, pw, var):
+    """The oracle's UpdateVoxelMap on world points and their covariances."""
+    pw = np.ascontiguousarray(pw, np.float64)
+    var = np.ascontiguousarray(var.reshape(-1, 9), np.float64)
+    orc.lib.orc_lio_update_map(orc.h, O.dptr(pw), O.dptr(var), len(pw))
 
 
 def build():

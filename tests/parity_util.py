@@ -1,4 +1,6 @@
-"""Shared comparison helpers for the GPU-vs-oracle parity tests."""
+"""Shared comparison helpers for the GPU-vs-oracle parity tests, and the golden vectors they run on."""
+import os
+
 import numpy as np
 
 import oracle_bind as O
@@ -73,3 +75,19 @@ def edge_scan(fr, seed=4):
     pts = np.ascontiguousarray(np.concatenate([on_corner, on_face, np.nextafter(on_corner, np.float32(-np.inf)), np.nextafter(on_corner, np.float32(np.inf)),
                                                inside, zero_z, off_plane]))
     return pts, ext, state
+
+
+GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+
+
+def load_golden():
+    """tests/golden/esikf_golden.npz (made by tests/golden/make_golden.py): (arrays, LIO config, VIO config, camera, extrinsics, map)."""
+    g = np.load(os.path.join(GOLDEN_DIR, "esikf_golden.npz"))
+    lc, vc, cc = g["lio_cfg"], g["vio_cfg"], g["cam_cfg"]
+    lio = S.LioCfg(voxel_size=float(lc[0]), max_layer=int(lc[1]), max_iterations=int(lc[2]), sigma_num=float(lc[3]), dept_err=float(lc[4]),
+                   beam_err=float(lc[5]), min_eigen_value=float(lc[6]), max_points_num=int(lc[7]))
+    vio = S.VioCfg(levels=int(vc[0]), max_iterations=int(vc[1]), img_point_cov=float(vc[2]), exposure_estimate_en=bool(vc[3]))
+    cam = S.CamCfg(model=int(cc[0]), width=int(cc[1]), height=int(cc[2]), fx=float(cc[3]), fy=float(cc[4]), cx=float(cc[5]), cy=float(cc[6]), d=tuple(cc[7:12]))
+    ext = S.Extrinsics(g["extR"], g["extT"], g["Rcl"], g["Pcl"])
+    vmap = dict(keys=g["map_keys"], first=g["map_first"], count=g["map_count"], planes=np.ascontiguousarray(g["map_planes"]).view(S.PLANE_DTYPE).reshape(-1))
+    return g, lio, vio, cam, ext, vmap

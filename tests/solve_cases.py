@@ -23,6 +23,8 @@ from fractions import Fraction
 import mpmath
 import numpy as np
 
+import oracle_bind as O
+from conftest import get_frame
 from fast_livo2_b200 import synthetic as S
 
 F57 = float(np.float32(57.3))  # the float constants of vio.cpp:1675, promoted to double against the double norm
@@ -393,3 +395,108 @@ def emulate_device_solution(P, A, HTz, vec, pscale, m, sign):
             s2 = fma(G[r, k], float(vec[k]), s2)
         sol[r] = ((s1 if sign > 0 else -s1) + float(vec[r])) - s2
     return sol, G
+
+
+# ----------------------------------------------------------------------------------------------- the cases on the oracle
+LIO_CASES = lio_zero_info_cases()
+VIO_CASES = vio_zero_info_cases()
+EMPTY_MAP = dict(keys=np.zeros((0, 3), np.int64), first=np.zeros(0, np.int32), count=np.zeros(0, np.int32), planes=np.zeros(0, S.PLANE_DTYPE))
+
+
+def lio_cfg(case):
+    return S.LioCfg(max_iterations=case["max_iterations"])
+
+
+def oracle_lio_zero(case):
+    lio = O.OracleLIO(lio_cfg(case), S.avia_extrinsics())
+    lio.set_map(EMPTY_MAP)
+    return lio.state_estimation(lio_zero_info_scan(), case["state_in"], case["state_prop"])
+
+
+def oracle_vio_zero(case):
+    cam, vcfg, ext = S.CamCfg(), vio_zero_info_cfg(), S.avia_extrinsics()
+    d = vio_zero_info_inputs(cam, ext, vcfg.levels)
+    vio = O.OracleVIO(cam, ext, vcfg)
+    return vio.update(d["img"], d["pos"], d["warp_patch"], d["search_levels"], d["inv_expo"], case["state_in"], case["state_prop"])
+
+
+def check_lio_rule(r, m):
+    """converged[it] is the rule on solution[it], and the iteration count follows the rematch / stop rule."""
+    for it in range(r["iters"]):
+        assert bool(r["converged"][it]) == lio_converged(r["solution"][it]), f"iteration {it}"
+    assert r["iters"] == expected_lio_iters([bool(c) for c in r["converged"]], m)
+
+
+def check_vio_rule(r, levels):
+    """Each level ends after its first accepted iteration whose solution meets the rule (or at max_iterations); with the
+    zero-information tie every iteration is accepted."""
+    for lvl in range(levels):
+        n_it, n_acc = int(r["iters_per_level"][lvl]), int(r["accepted_per_level"][lvl])
+        assert n_acc == n_it
+        ends = [vio_end(r["solution"][lvl][it]) for it in range(n_acc)]
+        assert not any(ends[:-1])
+        assert ends[-1] or n_it == vio_zero_info_cfg().max_iterations
+
+
+def gain_frames():
+    return dict(small=dict(seed=1, n_pts=4000, n_map=150_000, scene_scale=0.5),
+                corridor=dict(seed=5, n_pts=6000, n_map=400_000, lio=S.LioCfg(voxel_size=0.4, min_eigen_value=1e-4, max_points_num=100),
+                              ext=S.hilti_extrinsics(), scene="corridor", scene_scale=0.25),
+                vio=dict(seed=2, n_pts=2000, n_map=120_000, n_patches=150, scene_scale=0.5),
+                vio_expo_off=dict(seed=8, n_pts=1000, n_map=100_000, n_patches=120, scene_scale=0.5, vio=S.VioCfg(levels=3, exposure_estimate_en=False)))
+
+
+def gain_inputs(frame_name, cov_name):
+    """(frame, state_in, state_prop): the frame's prior with the family's covariance, the iterate displaced from it so that
+    state_propagat (-) state is not zero."""
+    fr = get_frame(**gain_frames()[frame_name])
+    P = stress_covs()[cov_name]
+    prop = fr["state_prior"].copy()
+    prop[25:] = P.reshape(-1)
+    st = prop.copy()
+    st[0:9] = (prop[0:9].reshape(3, 3) @ S.so3_exp(np.array([2e-4, -1e-4, 3e-4]))).reshape(9)
+    st[9:12] += np.array([3e-3, -2e-3, 1e-3])
+    return fr, st, prop
+
+
+def oracle_vio_warp(fr, state):
+    w = O.oracle_warp_patches(fr, state)
+    return w["warp_patch"], w["search_levels"]
+
+
+def gain_truth(kind, P, HTH, HTz, vec, img_point_cov=None):
+    """(mpmath solution, mpmath G, emulated device solution) of one iteration."""
+    m, sign, ps = (6, 1, 1.0) if kind == "lio" else (7, -1, 1.0 / img_point_cov)
+    sol, G = mp_solution(P, HTH, HTz, vec, ps, m, sign)
+    emu, _ = emulate_device_solution(P, HTH, HTz, vec, ps, m, sign)
+    return to_np(sol).reshape(19), G, emu
+
+
+def boxminus(prop, st):
+    v = np.zeros(19)
+    O.load().orc_boxminus(O.dptr(O.c64(prop)), O.dptr(O.c64(st)), O.dptr(v))
+    return v
+
+
+def oracle_gain_run(frame_name, cov_name):
+    fr, st, prop = gain_inputs(frame_name, cov_name)
+    if frame_name.startswith("vio"):
+        wp, sl = oracle_vio_warp(fr, prop)
+        vio = O.OracleVIO(fr["cam_cfg"], fr["ext"], fr["vio_cfg"])
+        r = vio.update(fr["img"], fr["vis_pos"], wp, sl, fr["inv_ref_expo"], st, prop)
+        L = fr["vio_cfg"].levels
+        return fr, st, prop, r, r["HTH"][L - 1][0], r["HTz"][L - 1][0], r["solution"][L - 1][0]
+    lio = O.OracleLIO(fr["lio_cfg"], fr["ext"])
+    lio.set_map(fr["map"])
+    r = lio.state_estimation(fr["pts"], st, prop)
+    return fr, st, prop, r, r["HTH"][0], r["HTz"][0], r["solution"][0]
+
+
+def gain_bound(frame_name, cov_name):
+    """The device bound of a gain case, fixed on the CPU: 4 max(oracle error, emulated device error) + 1e-14, relative to the
+    40-digit solution of the first iteration."""
+    fr, st, prop, r, HTH, HTz, sol0 = oracle_gain_run(frame_name, cov_name)
+    kind = "vio" if frame_name.startswith("vio") else "lio"
+    truth, _, emu = gain_truth(kind, prop[25:].reshape(19, 19), HTH, HTz, boxminus(prop, st), fr["vio_cfg"].img_point_cov)
+    e_orc, e_emu = rel_err(sol0, truth), rel_err(emu, truth)
+    return dict(oracle=e_orc, emulation=e_emu, bound=4 * max(e_orc, e_emu) + 1e-14, run=r)

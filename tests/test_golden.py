@@ -6,26 +6,12 @@ import numpy as np
 import pytest
 
 from fast_livo2_b200 import synthetic as S
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-
-
-def _load():
-    g = np.load(os.path.join(HERE, "golden", "esikf_golden.npz"))
-    lc, vc, cc = g["lio_cfg"], g["vio_cfg"], g["cam_cfg"]
-    lio = S.LioCfg(voxel_size=float(lc[0]), max_layer=int(lc[1]), max_iterations=int(lc[2]), sigma_num=float(lc[3]), dept_err=float(lc[4]),
-                   beam_err=float(lc[5]), min_eigen_value=float(lc[6]), max_points_num=int(lc[7]))
-    vio = S.VioCfg(levels=int(vc[0]), max_iterations=int(vc[1]), img_point_cov=float(vc[2]), exposure_estimate_en=bool(vc[3]))
-    cam = S.CamCfg(model=int(cc[0]), width=int(cc[1]), height=int(cc[2]), fx=float(cc[3]), fy=float(cc[4]), cx=float(cc[5]), cy=float(cc[6]), d=tuple(cc[7:12]))
-    ext = S.Extrinsics(g["extR"], g["extT"], g["Rcl"], g["Pcl"])
-    vmap = dict(keys=g["map_keys"], first=g["map_first"], count=g["map_count"], planes=np.ascontiguousarray(g["map_planes"]).view(S.PLANE_DTYPE).reshape(-1))
-    return g, lio, vio, cam, ext, vmap
-
+from parity_util import GOLDEN_DIR, load_golden
 
 def test_oracle_reproduces_golden_vectors():
     import oracle_bind as O
 
-    g, lio_cfg, vio_cfg, cam, ext, vmap = _load()
+    g, lio_cfg, vio_cfg, cam, ext, vmap = load_golden()
     lio = O.OracleLIO(lio_cfg, ext)
     lio.set_map(vmap)
     o = lio.state_estimation(g["pts"], g["state_prior"], g["state_prior"])
@@ -43,8 +29,8 @@ def test_oracle_reproduces_inverse_variant_golden_vectors():
     """Same inputs, vio/inverse_composition_en on (tests/golden/esikf_golden_inverse.npz)."""
     import oracle_bind as O
 
-    g, lio_cfg, vio_cfg, cam, ext, vmap = _load()
-    gi = np.load(os.path.join(HERE, "golden", "esikf_golden_inverse.npz"))
+    g, lio_cfg, vio_cfg, cam, ext, vmap = load_golden()
+    gi = np.load(os.path.join(GOLDEN_DIR, "esikf_golden_inverse.npz"))
     vio = O.OracleVIO(cam, ext, vio_cfg)
     vio.set_inverse_refs([g["img_ref"]], gi["ref_img_index"], gi["ref_px"], gi["ref_f"], gi["ref_R"], gi["ref_pos"])
     vio.set_inverse(True)
@@ -62,7 +48,7 @@ def test_cuda_path_matches_golden_vectors(gpu_ctx):
     from fast_livo2_b200 import api
     from parity_util import assert_state_close
 
-    g, lio_cfg, vio_cfg, cam, ext, vmap = _load()
+    g, lio_cfg, vio_cfg, cam, ext, vmap = load_golden()
     ctx = gpu_ctx
     ctx.set_extrinsics(ext)
     ctx.map_upload(vmap, lio_cfg.voxel_size)

@@ -7,9 +7,8 @@ import pytest
 import oracle_bind as O
 from fast_livo2_b200 import api
 from fast_livo2_b200 import synthetic as S
-from parity_util import assert_state_close
-from test_gpu_vio import _compare_vio, _gpu_warp, _setup, _vio_prior
-from test_map_host import _tick_points
+from harness import compare_lio, compare_vio, lio_gpu, lio_oracle, vio_prior, vio_setup, vio_warp
+from map_bind import tick_points
 
 pytestmark = pytest.mark.gpu
 
@@ -33,27 +32,14 @@ def new_context():
         ctx.close()
 
 
-def _lio_equals_oracle(ctx, fr):
-    ctx.set_extrinsics(fr["ext"])
-    ctx.map_upload(fr["map"], fr["lio_cfg"].voxel_size)
-    g = ctx.lio_update(fr["pts"], fr["state_prior"], fr["state_prior"], fr["lio_cfg"])
-    lio = O.OracleLIO(fr["lio_cfg"], fr["ext"])
-    lio.set_map(fr["map"])
-    o = lio.state_estimation(fr["pts"], fr["state_prior"], fr["state_prior"])
-    assert g["iters"] == o["iters"] and np.array_equal(g["M"], o["M"])
-    assert np.array_equal(g["match_plane"], o["match_plane"]) and np.array_equal(g["normal_plane"], o["normal_plane"])
-    assert_state_close(g["state"], o["state"])
-    return g
-
-
 def _vio_equals_oracle(ctx, fr):
-    _setup(ctx, fr)
-    prior = _vio_prior(fr)
-    w = _gpu_warp(ctx, fr, prior)
+    vio_setup(ctx, fr)
+    prior = vio_prior(fr)
+    w = vio_warp(ctx, fr, prior)
     args = (fr["img"], fr["vis_pos"], w["warp_patch"], w["search_levels"], fr["inv_ref_expo"], prior, prior)
     g = ctx.vio_update(*args)
     o = O.OracleVIO(fr["cam_cfg"], fr["ext"], fr["vio_cfg"]).update(*args)
-    _compare_vio(g, o, fr["vio_cfg"].levels)
+    compare_vio(g, o, fr["vio_cfg"].levels)
 
 
 def _status(excinfo):
@@ -72,7 +58,7 @@ def test_profile_kernel_errors_repeat_and_leave_the_context_usable(new_context, 
     for i in range(1000):
         with pytest.raises(api.EsikfError):
             ctx.profile_kernel(7 if i % 2 else 0, reps=1, flush_l2=False)
-    _lio_equals_oracle(ctx, small_frame)
+    compare_lio(lio_gpu(ctx, small_frame), lio_oracle(small_frame))
     # a resident LIO frame is measurable now; VIO still is not, and an unknown id is still refused
     assert ctx.profile_kernel(0, reps=2, flush_l2=False) > 0
     for which, msg in ((2, "no resident VIO frame"), (9, "which=9")):
@@ -101,7 +87,7 @@ def _walk_allocating_entry_points(ctx, fr):
     ctx.lio_fetch_normals()
     ctx.map_device_update()
     ctx.lio_fetch_normals()
-    pw, var = _tick_points(rng, rects, 4000, np.array([-12.0, -9.0, -3.0]), np.array([12.0, 9.0, 5.0]))
+    pw, var = tick_points(rng, rects, 4000, np.array([-12.0, -9.0, -3.0]), np.array([12.0, 9.0, 5.0]))
     ctx.map_device_update_points(pw, var)
     ctx.map_device_slide(np.array([-8, -8, -4]), np.array([8, 8, 6]))
     ctx.map_device_slide()
@@ -120,10 +106,10 @@ def _walk_allocating_entry_points(ctx, fr):
     assert ctx.profile_kernel(0, reps=2) > 0  # L2 flush buffer + measurement events
 
     # VIO: reference images twice, warp producers, inverse-compositional references, an update with timing
-    _setup(ctx, fr)
+    vio_setup(ctx, fr)
     ctx.vio_set_ref_images([fr["img_ref"], fr["img"]])
     n = len(fr["vis_pos"])
-    prior = _vio_prior(fr)
+    prior = vio_prior(fr)
     st = S.unpack_state(prior)
     T_cur = api.pack_T(*S.camera_pose(fr["ext"], st["R"], st["p"]))
     T_ref = np.tile(api.pack_T(*fr["T_ref"]), (n, 1))
@@ -156,5 +142,5 @@ def test_contexts_release_everything_they_allocate(new_context, small_vio_frame)
         finally:
             ctx.close()
     ctx = new_context()
-    _lio_equals_oracle(ctx, fr)
+    compare_lio(lio_gpu(ctx, fr), lio_oracle(fr))
     _vio_equals_oracle(ctx, fr)

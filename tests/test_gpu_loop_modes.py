@@ -8,40 +8,22 @@ import pytest
 
 from conftest import get_frame
 from fast_livo2_b200 import api
-from test_gpu_vio import _gpu_warp, _setup, _vio_prior
+from harness import LIO_KEYS, VIO_KEYS, bits_equal, sweep, vio_prior, vio_setup, vio_warp
 
 pytestmark = pytest.mark.gpu
-
-LIO_KEYS = ("state", "match_plane", "normal_plane", "dis_to_plane", "M", "HTH", "HTz", "solution", "total_residual", "converged")
-VIO_KEYS = ("state", "errors", "iters_per_level", "accepted_per_level", "error_trace", "HTH", "HTz", "solution")
-
-
-def _bits_equal(a, b, keys):
-    for k in keys:
-        x, y = np.ascontiguousarray(a[k]), np.ascontiguousarray(b[k])
-        assert x.shape == y.shape and x.tobytes() == y.tobytes(), k
-
 
 @pytest.mark.parametrize("solve_mode", [0, 1])
 def test_lio_persistent_kernel_is_bit_identical_to_per_iteration_launches(gpu_ctx, solve_mode):
     fr = get_frame(seed=4, n_pts=20000, n_map=150_000, scene_scale=0.5)
     gpu_ctx.set_extrinsics(fr["ext"])
     gpu_ctx.map_upload(fr["map"], fr["lio_cfg"].voxel_size)
-    gpu_ctx.set_solve_mode(solve_mode)
-    try:
-        out = {}
-        for mode in (0, 2, 2, 0, 2):
-            gpu_ctx.set_loop_mode(mode)
-            r = gpu_ctx.lio_update(fr["pts"], fr["state_prior"], fr["state_prior"], fr["lio_cfg"])
-            out.setdefault(mode, []).append(r)
-    finally:
-        gpu_ctx.set_loop_mode(api.DEFAULT_LOOP_MODE)
-        gpu_ctx.set_solve_mode(0)
-    ref = out[0][0]
+    runs = sweep(gpu_ctx, lambda: gpu_ctx.lio_update(fr["pts"], fr["state_prior"], fr["state_prior"], fr["lio_cfg"]),
+                 [dict(loop_mode=m, solve_mode=solve_mode) for m in (0, 2, 2, 0, 2)])
+    ref = runs[0]
     assert ref["iters"] >= 3
-    for r in out[2] + out[0][1:]:
+    for r in runs[1:]:
         assert r["iters"] == ref["iters"]
-        _bits_equal(ref, r, LIO_KEYS)
+        bits_equal(ref, r, LIO_KEYS)
 
 
 @pytest.mark.parametrize("n_pts,n_map,kw", [(100_000, 1_000_000, {}), (260_000, 1_000_000, dict(beam_err=0.01))])
@@ -53,42 +35,26 @@ def test_lio_full_size_frames_resident_and_several_tiles_per_cta(gpu_ctx, n_pts,
     fr = get_frame(seed=12 if n_pts > 100_000 else 0, n_pts=n_pts, n_map=n_map, **(dict(lio=S.LioCfg(**kw)) if kw else dict(n_patches=2000)))
     gpu_ctx.set_extrinsics(fr["ext"])
     gpu_ctx.map_upload(fr["map"], fr["lio_cfg"].voxel_size)
-    try:
-        gpu_ctx.set_loop_mode(0)
-        a = gpu_ctx.lio_update(fr["pts"], fr["state_prior"], fr["state_prior"], fr["lio_cfg"])
-        gpu_ctx.set_loop_mode(2)
-        b = gpu_ctx.lio_update(fr["pts"], fr["state_prior"], fr["state_prior"], fr["lio_cfg"])
-        gpu_ctx.set_tuning(api.TUNE_STAGE_LDG)
-        c = gpu_ctx.lio_update(fr["pts"], fr["state_prior"], fr["state_prior"], fr["lio_cfg"])
-    finally:
-        gpu_ctx.set_tuning(0)
-        gpu_ctx.set_loop_mode(api.DEFAULT_LOOP_MODE)
+    a, b, c = sweep(gpu_ctx, lambda: gpu_ctx.lio_update(fr["pts"], fr["state_prior"], fr["state_prior"], fr["lio_cfg"]),
+                    [dict(loop_mode=0), dict(loop_mode=2), dict(loop_mode=2, tuning=api.TUNE_STAGE_LDG)])
     assert a["iters"] == b["iters"] == c["iters"]
-    _bits_equal(a, b, LIO_KEYS)
-    _bits_equal(a, c, LIO_KEYS)
+    bits_equal(a, b, LIO_KEYS)
+    bits_equal(a, c, LIO_KEYS)
 
 
 @pytest.mark.parametrize("solve_mode", [0, 1])
 def test_vio_persistent_kernel_is_bit_identical_to_per_iteration_launches(gpu_ctx, small_vio_frame, solve_mode):
     fr = small_vio_frame
-    _setup(gpu_ctx, fr)
-    prior = _vio_prior(fr)
-    w = _gpu_warp(gpu_ctx, fr, prior)
+    vio_setup(gpu_ctx, fr)
+    prior = vio_prior(fr)
+    w = vio_warp(gpu_ctx, fr, prior)
     args = (fr["img"], fr["vis_pos"], w["warp_patch"], w["search_levels"], fr["inv_ref_expo"], prior, prior)
-    gpu_ctx.set_solve_mode(solve_mode)
-    try:
-        out = {}
-        for mode in (0, 2, 2, 0, 2):
-            gpu_ctx.set_loop_mode(mode)
-            out.setdefault(mode, []).append(gpu_ctx.vio_update(*args))
-    finally:
-        gpu_ctx.set_loop_mode(api.DEFAULT_LOOP_MODE)
-        gpu_ctx.set_solve_mode(0)
-    ref = out[0][0]
+    runs = sweep(gpu_ctx, lambda: gpu_ctx.vio_update(*args), [dict(loop_mode=m, solve_mode=solve_mode) for m in (0, 2, 2, 0, 2)])
+    ref = runs[0]
     assert ref["total_iters"] >= 4
-    for r in out[2] + out[0][1:]:
+    for r in runs[1:]:
         assert r["total_iters"] == ref["total_iters"]
-        _bits_equal(ref, r, VIO_KEYS)
+        bits_equal(ref, r, VIO_KEYS)
 
 
 @pytest.mark.parametrize("n_patches", [4000, 6000])
@@ -100,24 +66,17 @@ def test_vio_patch_cache_with_two_and_more_patches_per_warp_and_search_levels(gp
     cam = S.CamCfg(width=612, height=512, fx=612.0 * 0.72, fy=612.0 * 0.72, cx=306.0, cy=256.0)
     vcfg = S.VioCfg(levels=5, img_point_cov=1000.0)
     fr = get_frame(seed=13, n_pts=1000, n_map=300_000, n_patches=4000, scene_scale=0.7, cam=cam, vio=vcfg)
-    _setup(gpu_ctx, fr)
-    prior = _vio_prior(fr, 13)
-    w = _gpu_warp(gpu_ctx, fr, prior)
+    vio_setup(gpu_ctx, fr)
+    prior = vio_prior(fr, 13)
+    w = vio_warp(gpu_ctx, fr, prior)
     n = len(fr["vis_pos"])
     rep = (np.arange(n_patches) % n)
     sl = (np.arange(n_patches) % 2).astype(np.int32)  # exercise search_level 1 as well
     args = (fr["img"], fr["vis_pos"][rep], w["warp_patch"][rep], sl, fr["inv_ref_expo"][rep], prior, prior)
-    try:
-        gpu_ctx.set_loop_mode(0)
-        a = gpu_ctx.vio_update(*args)
-        gpu_ctx.set_loop_mode(2)
-        b = gpu_ctx.vio_update(*args)
-        b2 = gpu_ctx.vio_update(*args)
-    finally:
-        gpu_ctx.set_loop_mode(api.DEFAULT_LOOP_MODE)
+    a, b, b2 = sweep(gpu_ctx, lambda: gpu_ctx.vio_update(*args), [dict(loop_mode=0), dict(loop_mode=2), dict(loop_mode=2)])
     assert a["total_iters"] == b["total_iters"] == b2["total_iters"]
-    _bits_equal(a, b, VIO_KEYS)
-    _bits_equal(a, b2, VIO_KEYS)
+    bits_equal(a, b, VIO_KEYS)
+    bits_equal(a, b2, VIO_KEYS)
 
 
 def test_vio_tap_footprints_through_tma_are_bit_identical(gpu_ctx):
@@ -125,23 +84,15 @@ def test_vio_tap_footprints_through_tma_are_bit_identical(gpu_ctx):
     {1, s}) instead of per-lane byte loads. BASELINE config-2 image (640 x 512, pitch a multiple of 16) with search levels
     0 / 1 / 2 so that every tap stride up to 8 goes through the tensor maps and strides 16 / 32 fall back."""
     fr = get_frame(seed=0, n_pts=100_000, n_map=1_000_000, n_patches=2000)
-    _setup(gpu_ctx, fr)
-    prior = _vio_prior(fr)
-    w = _gpu_warp(gpu_ctx, fr, prior)
+    vio_setup(gpu_ctx, fr)
+    prior = vio_prior(fr)
+    w = vio_warp(gpu_ctx, fr, prior)
     n = len(fr["vis_pos"])
     out = []
-    try:
-        for sl in (w["search_levels"], (np.arange(n) % 3).astype(np.int32)):
-            args = (fr["img"], fr["vis_pos"], w["warp_patch"], sl, fr["inv_ref_expo"], prior, prior)
-            gpu_ctx.set_tuning(0)
-            a = gpu_ctx.vio_update(*args)
-            gpu_ctx.set_tuning(api.TUNE_VIO_TMA)
-            b = gpu_ctx.vio_update(*args)
-            b2 = gpu_ctx.vio_update(*args)
-            out.append((a, b, b2))
-    finally:
-        gpu_ctx.set_tuning(0)
+    for sl in (w["search_levels"], (np.arange(n) % 3).astype(np.int32)):
+        args = (fr["img"], fr["vis_pos"], w["warp_patch"], sl, fr["inv_ref_expo"], prior, prior)
+        out.append(sweep(gpu_ctx, lambda: gpu_ctx.vio_update(*args), [dict(), dict(tuning=api.TUNE_VIO_TMA), dict(tuning=api.TUNE_VIO_TMA)]))
     for a, b, b2 in out:
         assert a["total_iters"] == b["total_iters"] == b2["total_iters"] and a["total_iters"] >= 4
-        _bits_equal(a, b, VIO_KEYS)
-        _bits_equal(a, b2, VIO_KEYS)
+        bits_equal(a, b, VIO_KEYS)
+        bits_equal(a, b2, VIO_KEYS)

@@ -14,8 +14,8 @@ import map_bind as MB
 import oracle_bind as O
 from fast_livo2_b200 import api
 from fast_livo2_b200 import synthetic as S
+from map_bind import oracle_map, oracle_update_map, tick_points
 from parity_util import assert_state_close
-from test_map_host import _oracle, _oracle_update, _tick_points
 
 pytestmark = pytest.mark.gpu
 
@@ -24,12 +24,12 @@ pytestmark = pytest.mark.gpu
 def test_device_update_voxel_map_matches_the_oracle_for_ten_ticks(gpu_ctx, cfg):
     rng = np.random.default_rng(5)
     rects = S.make_scene("room", 0.5)
-    orc = _oracle(cfg)
+    orc = oracle_map(cfg)
     gpu_ctx.map_device_init(cfg, root_capacity=1 << 16)
     for tick in range(10):
         lo = np.array([-10.0 + 1.5 * tick, -8.0, -2.0])
-        pw, var = _tick_points(rng, rects, 6000, lo, lo + np.array([8.0, 16.0, 6.0]))
-        _oracle_update(orc, pw, var)
+        pw, var = tick_points(rng, rects, 6000, lo, lo + np.array([8.0, 16.0, 6.0]))
+        oracle_update_map(orc, pw, var)
         gpu_ctx.map_device_update_points(pw, var)
         # refits add the per-point terms in point order without FMA contraction: bit-identical to the serial evaluation
         n = MB.compare_flat_maps(gpu_ctx.map_device_download(), orc.flatten(), what=("device map", "oracle"), exact=True)
@@ -102,12 +102,12 @@ def test_device_map_sliding_matches_clear_mem_out_of_map_and_keeps_tracking(gpu_
     cfg = S.LioCfg()
     rng = np.random.default_rng(17)
     rects = S.make_scene("room", 0.5)
-    orc = _oracle(cfg)
+    orc = oracle_map(cfg)
     gpu_ctx.map_device_init(cfg, root_capacity=1 << 16)
     lo_w, hi_w = np.array([-12.0, -9.0, -3.0]), np.array([12.0, 9.0, 5.0])
     for tick in range(6):
-        pw, var = _tick_points(rng, rects, 6000, lo_w, hi_w)
-        _oracle_update(orc, pw, var)
+        pw, var = tick_points(rng, rects, 6000, lo_w, hi_w)
+        oracle_update_map(orc, pw, var)
         gpu_ctx.map_device_update_points(pw, var)
     before = gpu_ctx.map_device_stats()
     c, half = np.array([4, -2, 1]), 12
@@ -117,8 +117,8 @@ def test_device_map_sliding_matches_clear_mem_out_of_map_and_keeps_tracking(gpu_
     assert deleted > 0 and after["roots"] == before["roots"] - deleted and after["pool_points"] < before["pool_points"] and after["errors"] == 0
     MB.compare_flat_maps(gpu_ctx.map_device_download(), orc.flatten())
     for tick in range(4):
-        pw, var = _tick_points(rng, rects, 6000, lo_w, hi_w)
-        _oracle_update(orc, pw, var)
+        pw, var = tick_points(rng, rects, 6000, lo_w, hi_w)
+        oracle_update_map(orc, pw, var)
         gpu_ctx.map_device_update_points(pw, var)
         MB.compare_flat_maps(gpu_ctx.map_device_download(), orc.flatten())
     # compaction only
@@ -130,7 +130,7 @@ def test_device_map_capacity_errors_are_statuses(gpu_ctx):
     cfg = S.LioCfg()
     rng = np.random.default_rng(2)
     rects = S.make_scene("room", 0.5)
-    pw, var = _tick_points(rng, rects, 5000, np.array([-12.0, -9.0, -3.0]), np.array([12.0, 9.0, 5.0]))
+    pw, var = tick_points(rng, rects, 5000, np.array([-12.0, -9.0, -3.0]), np.array([12.0, 9.0, 5.0]))
     for kw, flag in ((dict(root_capacity=1 << 12, node_capacity=16), 1), (dict(root_capacity=1 << 12, point_capacity=64), 2), (dict(root_capacity=1 << 12, record_capacity=4), 4),
                      (dict(root_capacity=128), 8)):
         gpu_ctx.map_device_init(cfg, **kw)

@@ -10,25 +10,20 @@ import map_bind as MB
 import map_streams as MS
 from fast_livo2_b200 import api
 from fast_livo2_b200 import synthetic as S
-from parity_util import assert_state_close
+from harness import compare_lio
 
 pytestmark = pytest.mark.gpu
 
 
-def _lio_compare(g, o):
-    assert g["iters"] == o["iters"] and np.array_equal(np.asarray(g["M"])[:g["iters"]], o["M"]), (g["M"], o["M"])
-    # association bit for bit: which points matched and their point-to-plane distances (plane ids differ by construction:
-    # record slots on the device, flat ids in the oracle)
-    assert np.array_equal(g["match_plane"] >= 0, o["match_plane"] >= 0)
-    assert np.array_equal(g["dis_to_plane"], o["dis_to_plane"])
-    assert_state_close(g["state"], o["state"], rot_tol=1e-9, pos_tol=2e-9, cov_tol=1e-7, rest_tol=1e-9)
+# plane ids differ by construction (record slots on the device, flat ids in the oracle): compared as matched / unmatched
+ON_DEVICE_MAP = dict(same_plane_ids=False, rot_tol=1e-9, pos_tol=2e-9, cov_tol=1e-7, rest_tol=1e-9)
 
 
 def _lio(ctx, orc, c, seed=0, n=3000):
     pts, prior = MS.lio_scan(c, np.random.default_rng(seed), n)
     g = ctx.lio_update(pts, prior, prior, c["cfg"])
     o = orc.o.state_estimation(pts, prior, prior)
-    _lio_compare(g, o)
+    compare_lio(g, o, **ON_DEVICE_MAP)
     return g, o, pts
 
 
@@ -50,7 +45,7 @@ def test_device_streams_match_the_oracle_every_tick(gpu_ctx, name):
         # a scan on the mid-planes of the boxes: the equal-eigenvalue plane (NaN plane_var) never matches, the valid one does
         pts, prior = MS.box_scan()
         g = gpu_ctx.lio_update(pts, prior, prior, c["cfg"])
-        _lio_compare(g, sides["orc"].o.state_estimation(pts, prior, prior))
+        compare_lio(g, sides["orc"].o.state_estimation(pts, prior, prior), **ON_DEVICE_MAP)
         k = MS.voxel_keys(pts, c["cfg"])
         at = lambda name: np.all(k == np.array(MS.BOX_KEYS[name]), axis=1)
         assert at("equal_min").sum() > 0 and not (g["match_plane"][at("equal_min")] >= 0).any()
@@ -81,12 +76,12 @@ def test_device_slides_twice_and_lio_reads_the_swapped_arena(gpu_ctx):
             if after["roots"]:
                 pts, prior = MS.lio_scan(c, rng, 4000)
                 o = orc.o.state_estimation(pts, prior, prior)
-                _lio_compare(gpu_ctx.lio_update(pts, prior, prior, c["cfg"]), o)
+                compare_lio(gpu_ctx.lio_update(pts, prior, prior, c["cfg"]), o, **ON_DEVICE_MAP)
                 assert o["M"][0] > 100
                 lio_runs += 1
     assert lio_runs == 2
     pts, prior = MS.lio_scan(c, rng, 4000)  # after the empty box and the rebuild
-    _lio_compare(gpu_ctx.lio_update(pts, prior, prior, c["cfg"]), orc.o.state_estimation(pts, prior, prior))
+    compare_lio(gpu_ctx.lio_update(pts, prior, prior, c["cfg"]), orc.o.state_estimation(pts, prior, prior), **ON_DEVICE_MAP)
 
 
 @pytest.mark.parametrize("name", ["deep_blob_L7", "candidates_layer3"])

@@ -17,9 +17,8 @@ import vio_border as VB
 from conftest import get_frame
 from fast_livo2_b200 import api
 from fast_livo2_b200 import synthetic as S
-from test_gpu_loop_modes import VIO_KEYS, _bits_equal
-from test_gpu_vio import _compare_vio, _setup, _vio_prior
-from test_oracle_ref_pin_vio import BORDER_FRAME, warp_affine_border_cases
+from harness import VIO_KEYS, bits_equal, compare_vio, sm_count, sweep, vio_prior, vio_setup
+from ref_pin_cases import BORDER_FRAME, warp_affine_border_cases
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -31,7 +30,7 @@ FISHEYE = dict(seed=9, n_pts=1000, n_map=100_000, n_patches=100, scene_scale=0.5
 @pytest.fixture(scope="module")
 def border():
     fr = get_frame(**BORDER_FRAME)
-    prior = _vio_prior(fr)
+    prior = vio_prior(fr)
     return fr, prior, VB.border_patch_set(fr, prior)
 
 
@@ -40,31 +39,12 @@ def _args(fr, bs, prior, idx=None):
     return (fr["img"], bs["vis_pos"][idx], bs["warp_patch"][idx], bs["search_levels"][idx], bs["inv_ref_expo"][idx], prior, prior)
 
 
-def _modes(ctx, args, modes=(0, 2), tuning=0):
-    out = []
-    try:
-        ctx.set_tuning(tuning)
-        for m in modes:
-            ctx.set_loop_mode(m)
-            out.append(ctx.vio_update(*args))
-    finally:
-        ctx.set_loop_mode(api.DEFAULT_LOOP_MODE)
-        ctx.set_tuning(0)
-    return out
-
-
-def _sm_count():
-    import torch
-
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
 # --------------------------------------------------------------------------------------------------------- a. getImagePatch
 def test_image_patch_at_the_border_is_bit_exact(gpu_ctx, border):
     """image_patch_kernel at edge, corner and just-outside pixels, levels 0..3: reads that wrap to the neighbouring row and
     reads outside the buffer (0)."""
     fr, _, _ = border
-    _setup(gpu_ctx, fr)
+    vio_setup(gpu_ctx, fr)
     cam, L = fr["cam_cfg"], fr["vio_cfg"].levels
     ins, outs = VB.edge_pixels(cam.width, cam.height, L, np.random.default_rng(4))
     pcs = np.concatenate([ins, outs])
@@ -116,7 +96,7 @@ def test_warp_affine_across_and_on_the_in_frame_limits(gpu_ctx, border):
     0..2, plus singular matrices (zero: NaN inverse, patch untouched; non-zero: inf entries, NaN and inf sample positions
     count as outside): bit for bit against the oracle."""
     fr, _, _ = border
-    _setup(gpu_ctx, fr)
+    vio_setup(gpu_ctx, fr)
     cam = fr["cam_cfg"]
     cases = warp_affine_border_cases(cam.width, cam.height)
     for sl in range(3):
@@ -137,7 +117,7 @@ def test_warp_patches_with_px_ref_near_the_border(gpu_ctx, border):
     """warp_matrix_kernel + warp_affine_kernel on the border set (reference pixels near and beyond the reference image's
     edges): A to 1e-10, identical search levels, warp samples as in test_gpu_vio."""
     fr, prior, bs = border
-    _setup(gpu_ctx, fr)
+    vio_setup(gpu_ctx, fr)
     n = len(bs["vis_pos"])
     st = S.unpack_state(prior)
     T_cur = S.camera_pose(fr["ext"], st["R"], st["p"])
@@ -158,29 +138,25 @@ def test_warp_patches_with_px_ref_near_the_border(gpu_ctx, border):
 def test_vio_update_on_the_border_set_matches_oracle(gpu_ctx, border):
     fr, prior, bs = border
     assert bs["n_leave"] >= 60 and 0.2 <= bs["border"].mean() <= 0.3, (bs["n_leave"], bs["border"].mean())
-    _setup(gpu_ctx, fr)
+    vio_setup(gpu_ctx, fr)
     args = _args(fr, bs, prior)
     g = gpu_ctx.vio_update(*args)
     o = O.OracleVIO(fr["cam_cfg"], fr["ext"], fr["vio_cfg"]).update(*args)
     assert o["total_iters"] >= 4 and (o["accepted_per_level"] < o["iters_per_level"]).any()  # real accept / rollback decisions
-    _compare_vio(g, o, fr["vio_cfg"].levels)
+    compare_vio(g, o, fr["vio_cfg"].levels)
 
 
 @pytest.mark.parametrize("solve_mode", [0, 1])
 def test_vio_update_on_the_border_set_loop_modes_are_bit_identical(gpu_ctx, border, solve_mode):
     fr, prior, bs = border
-    _setup(gpu_ctx, fr)
+    vio_setup(gpu_ctx, fr)
     args = _args(fr, bs, prior)
-    gpu_ctx.set_solve_mode(solve_mode)
-    try:
-        a, b, b2 = _modes(gpu_ctx, args, (0, 2, 2))
-    finally:
-        gpu_ctx.set_solve_mode(0)
+    a, b, b2 = sweep(gpu_ctx, lambda: gpu_ctx.vio_update(*args), [dict(loop_mode=m, solve_mode=solve_mode) for m in (0, 2, 2)])
     assert a["total_iters"] >= 4
-    _bits_equal(a, b, VIO_KEYS)
-    _bits_equal(a, b2, VIO_KEYS)
+    bits_equal(a, b, VIO_KEYS)
+    bits_equal(a, b2, VIO_KEYS)
     if solve_mode == 1:
-        _compare_vio(b, O.OracleVIO(fr["cam_cfg"], fr["ext"], fr["vio_cfg"]).update(*args), fr["vio_cfg"].levels)
+        compare_vio(b, O.OracleVIO(fr["cam_cfg"], fr["ext"], fr["vio_cfg"]).update(*args), fr["vio_cfg"].levels)
 
 
 @pytest.mark.parametrize("regime", ["all_cached", "at_limit", "over_limit"])
@@ -189,8 +165,8 @@ def test_vio_patch_cache_regimes_with_border_footprints(gpu_ctx, border, regime)
     grid = min(ceil(n / 16), min(SMs, 160)) CTAs of per = ceil(n / grid) patches: per <= 32 (every CTA cached), = 32 (the
     limit) and = 33 (slot 0 refilled for every patch). Against the cold per-iteration launches, bit for bit."""
     fr, prior, bs = border
-    _setup(gpu_ctx, fr)
-    G = min(_sm_count(), 160)
+    vio_setup(gpu_ctx, fr)
+    G = min(sm_count(), 160)
     n = {"all_cached": len(bs["vis_pos"]), "at_limit": 32 * G, "over_limit": 32 * G + 1}[regime]
     grid = min(-(-n // 16), G)
     per = -(-n // grid)
@@ -198,9 +174,10 @@ def test_vio_patch_cache_regimes_with_border_footprints(gpu_ctx, border, regime)
     # the border patches first so that every CTA holds some
     order = np.concatenate([np.nonzero(bs["border"])[0], np.nonzero(~bs["border"])[0]])
     idx = order[np.arange(n) % len(order)]
-    a, b = _modes(gpu_ctx, _args(fr, bs, prior, idx))
+    args = _args(fr, bs, prior, idx)
+    a, b = sweep(gpu_ctx, lambda: gpu_ctx.vio_update(*args), [dict(loop_mode=0), dict(loop_mode=2)])
     assert a["total_iters"] >= 4
-    _bits_equal(a, b, VIO_KEYS)
+    bits_equal(a, b, VIO_KEYS)
 
 
 # --------------------------------------------------------------------------------------------------------- d. TMA guard
@@ -236,16 +213,15 @@ def test_tma_footprints_at_the_guard_are_bit_identical_to_per_lane_loads(gpu_ctx
         assert ys[i] is None or y0[i] == ys[i], (i, y0[i], ys[i])
     assert (x0 + 10 * stride == cam.width).sum() == 1 and (x0 + 10 * stride == cam.width - stride).sum() == 1
     try:
-        _setup(gpu_ctx, fr)
+        vio_setup(gpu_ctx, fr)
         gpu_ctx.vio_set_camera(cam, vcfg)
         args = _args(fr, bs, prior)
-        a, = _modes(gpu_ctx, args, (2,))
-        b, b2 = _modes(gpu_ctx, args, (2, 2), tuning=api.TUNE_VIO_TMA)
+        a, b, b2 = sweep(gpu_ctx, lambda: gpu_ctx.vio_update(*args), [dict(), dict(tuning=api.TUNE_VIO_TMA), dict(tuning=api.TUNE_VIO_TMA)])
     finally:
         gpu_ctx.vio_set_camera(cam, fr["vio_cfg"])
     assert a["total_iters"] >= 2
-    _bits_equal(a, b, VIO_KEYS)
-    _bits_equal(a, b2, VIO_KEYS)
+    bits_equal(a, b, VIO_KEYS)
+    bits_equal(a, b2, VIO_KEYS)
 
 
 # --------------------------------------------------------------------------------------------------------- e. drift across the edge
@@ -255,7 +231,7 @@ def test_footprint_restaged_across_the_edge_between_iterations(gpu_ctx, border):
     per-iteration launches (with and without TMA) bit for bit, and against the oracle."""
     fr, _, _ = border
     cam = fr["cam_cfg"]
-    prior = _vio_prior(fr, seed=11, rot_deg=0.5, pos=0.02)
+    prior = vio_prior(fr, seed=11, rot_deg=0.5, pos=0.02)
     vcfg = dataclasses.replace(fr["vio_cfg"], levels=1, max_iterations=8)
     v, u = 0.5 * cam.height + 17.3, 0.5 * cam.width - 23.7
     # anchor exactly 5 px (stride 1) from each edge at the prior: the footprint touches column / row 0 or the last one
@@ -266,17 +242,16 @@ def test_footprint_restaged_across_the_edge_between_iterations(gpu_ctx, border):
     assert not VB.leaves_image(px, np.zeros(4, np.int32), 1, cam.width, cam.height).any()
     fr1 = dict(fr, vio_cfg=vcfg)
     try:
-        _setup(gpu_ctx, fr)
+        vio_setup(gpu_ctx, fr)
         gpu_ctx.vio_set_camera(cam, vcfg)
         args = _args(fr, bs, prior)
-        a, b = _modes(gpu_ctx, args)
-        c, = _modes(gpu_ctx, args, (2,), tuning=api.TUNE_VIO_TMA)
+        a, b, c = sweep(gpu_ctx, lambda: gpu_ctx.vio_update(*args), [dict(loop_mode=0), dict(loop_mode=2), dict(loop_mode=2, tuning=api.TUNE_VIO_TMA)])
     finally:
         gpu_ctx.vio_set_camera(cam, fr["vio_cfg"])
     assert a["total_iters"] >= 2
-    _bits_equal(a, b, VIO_KEYS)
-    _bits_equal(a, c, VIO_KEYS)
-    _compare_vio(b, O.OracleVIO(cam, fr["ext"], vcfg).update(*args), 1)
+    bits_equal(a, b, VIO_KEYS)
+    bits_equal(a, c, VIO_KEYS)
+    compare_vio(b, O.OracleVIO(cam, fr["ext"], vcfg).update(*args), 1)
     # where the posterior projects them: at least one footprint now leaves the image
     st = S.unpack_state(b["state"])
     Rcw, Pcw = S.camera_pose(fr1["ext"], st["R"], st["p"])
@@ -300,29 +275,29 @@ def test_inverse_variant_with_reference_pixels_near_the_border(gpu_ctx, border):
     n = len(bs["vis_pos"])
     args = (fr["img"], bs["vis_pos"], bs["warp_patch"], bs["search_levels"], np.ones(n), prior, prior)
     try:
-        _setup(gpu_ctx, fr)
+        vio_setup(gpu_ctx, fr)
         gpu_ctx.vio_set_camera(cam, inv_cfg)
         gpu_ctx.vio_set_inverse_refs(refs["ref_img_index"], refs["ref_px"], refs["ref_f"], refs["ref_R"], refs["ref_pos"])
-        a, b = _modes(gpu_ctx, args)
+        a, b = sweep(gpu_ctx, lambda: gpu_ctx.vio_update(*args), [dict(loop_mode=0), dict(loop_mode=2)])
     finally:
         gpu_ctx.vio_set_camera(cam, fr["vio_cfg"])
     assert a["total_iters"] >= 3
-    _bits_equal(a, b, VIO_KEYS)
+    bits_equal(a, b, VIO_KEYS)
     vio = O.OracleVIO(cam, fr["ext"], fr["vio_cfg"])
     vio.set_inverse_refs(**refs)
     vio.set_inverse(True)
-    _compare_vio(b, vio.update(*args), L)
+    compare_vio(b, vio.update(*args), L)
 
 
 # --------------------------------------------------------------------------------------------------------- g. fisheye
 def test_fisheye_camera_with_border_patches(gpu_ctx):
     """Config 3's equidistant camera, where distortion is largest at the edge: a few border patches among the interior ones."""
     fr = get_frame(**FISHEYE)
-    prior = _vio_prior(fr, 9)
+    prior = vio_prior(fr, 9)
     bs = VB.border_patch_set(fr, prior, every=4)
     assert bs["n_leave"] >= 10, bs["n_leave"]
-    _setup(gpu_ctx, fr)
+    vio_setup(gpu_ctx, fr)
     args = _args(fr, bs, prior)
-    a, b = _modes(gpu_ctx, args)
-    _bits_equal(a, b, VIO_KEYS)
-    _compare_vio(b, O.OracleVIO(fr["cam_cfg"], fr["ext"], fr["vio_cfg"]).update(*args), fr["vio_cfg"].levels)
+    a, b = sweep(gpu_ctx, lambda: gpu_ctx.vio_update(*args), [dict(loop_mode=0), dict(loop_mode=2)])
+    bits_equal(a, b, VIO_KEYS)
+    compare_vio(b, O.OracleVIO(fr["cam_cfg"], fr["ext"], fr["vio_cfg"]).update(*args), fr["vio_cfg"].levels)

@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 
 import oracle_bind as O
-from test_gpu_vio import _compare_vio, _gpu_warp, _setup, _vio_prior
+from harness import VIO_KEYS, bits_equal, compare_vio, sweep, vio_prior, vio_setup, vio_warp
 
 pytestmark = pytest.mark.gpu
 
@@ -16,10 +16,10 @@ def test_inverse_variant_matches_oracle(gpu_ctx, small_vio_frame):
     fr = small_vio_frame
     inv_cfg = dataclasses.replace(fr["vio_cfg"], inverse_composition_en=True)
     refs = O.inverse_refs_from_frame(fr)
-    prior = _vio_prior(fr)
+    prior = vio_prior(fr)
     try:
-        _setup(gpu_ctx, fr)
-        w = _gpu_warp(gpu_ctx, fr, prior)
+        vio_setup(gpu_ctx, fr)
+        w = vio_warp(gpu_ctx, fr, prior)
         gpu_ctx.vio_set_camera(fr["cam_cfg"], inv_cfg)
         gpu_ctx.vio_set_inverse_refs(refs["ref_img_index"], refs["ref_px"], refs["ref_f"], refs["ref_R"], refs["ref_pos"])
         n = len(fr["vis_pos"])
@@ -33,11 +33,11 @@ def test_inverse_variant_matches_oracle(gpu_ctx, small_vio_frame):
     vio.set_inverse(True)
     o = vio.update(*args)
     assert np.array_equal(g["state"], g2["state"])  # deterministic
-    _compare_vio(g, o, fr["vio_cfg"].levels)
+    compare_vio(g, o, fr["vio_cfg"].levels)
     # the forward variant is back after restoring the configuration
     f = gpu_ctx.vio_update(*args)
     vio.set_inverse(False)
-    _compare_vio(f, vio.update(*args), fr["vio_cfg"].levels)
+    compare_vio(f, vio.update(*args), fr["vio_cfg"].levels)
 
 
 def test_inverse_variant_needs_its_reference_data(gpu_ctx, small_vio_frame):
@@ -45,10 +45,10 @@ def test_inverse_variant_needs_its_reference_data(gpu_ctx, small_vio_frame):
 
     fr = small_vio_frame
     inv_cfg = dataclasses.replace(fr["vio_cfg"], inverse_composition_en=True)
-    prior = _vio_prior(fr)
+    prior = vio_prior(fr)
     try:
-        _setup(gpu_ctx, fr)
-        w = _gpu_warp(gpu_ctx, fr, prior)
+        vio_setup(gpu_ctx, fr)
+        w = vio_warp(gpu_ctx, fr, prior)
         gpu_ctx.vio_set_camera(fr["cam_cfg"], inv_cfg)
         gpu_ctx.vio_set_inverse_refs(np.zeros(3, np.int32), np.zeros((3, 2)), np.zeros((3, 3)), np.zeros((3, 9)), np.zeros((3, 3)))
         with pytest.raises(api.EsikfError):
@@ -59,11 +59,10 @@ def test_inverse_variant_needs_its_reference_data(gpu_ctx, small_vio_frame):
 
 def test_inverse_variant_matches_golden_vectors(gpu_ctx):
     """tests/golden/esikf_golden_inverse.npz: the CUDA path without the oracle in the loop."""
-    from parity_util import assert_state_close
-    from test_golden import HERE, _load
+    from parity_util import GOLDEN_DIR, assert_state_close, load_golden
 
-    g, lio_cfg, vio_cfg, cam, ext, vmap = _load()
-    gi = np.load(os.path.join(HERE, "golden", "esikf_golden_inverse.npz"))
+    g, lio_cfg, vio_cfg, cam, ext, vmap = load_golden()
+    gi = np.load(os.path.join(GOLDEN_DIR, "esikf_golden_inverse.npz"))
     n = len(g["vis_pos"])
     try:
         gpu_ctx.set_extrinsics(ext)
@@ -83,29 +82,22 @@ def test_inverse_variant_persistent_kernel_is_bit_identical_to_per_iteration_lau
     """loop_mode 2 runs the inverse-compositional loop inside the same persistent kernel as the forward variant
     (vio_update_kernel<.., INVERSE>: H_sub_inv of a level precomputed by the warp that later reads it); it must reproduce
     the per-iteration launches (loop_mode 0: precompute kernel + patch kernel + solve kernel) bit for bit."""
-    from fast_livo2_b200 import api
-    from test_gpu_loop_modes import VIO_KEYS, _bits_equal
-
     fr = small_vio_frame
     inv_cfg = dataclasses.replace(fr["vio_cfg"], inverse_composition_en=True)
     refs = O.inverse_refs_from_frame(fr)
-    prior = _vio_prior(fr)
-    out = {}
+    prior = vio_prior(fr)
     try:
-        _setup(gpu_ctx, fr)
-        w = _gpu_warp(gpu_ctx, fr, prior)
+        vio_setup(gpu_ctx, fr)
+        w = vio_warp(gpu_ctx, fr, prior)
         gpu_ctx.vio_set_camera(fr["cam_cfg"], inv_cfg)
         gpu_ctx.vio_set_inverse_refs(refs["ref_img_index"], refs["ref_px"], refs["ref_f"], refs["ref_R"], refs["ref_pos"])
         n = len(fr["vis_pos"])
         args = (fr["img"], fr["vis_pos"], w["warp_patch"], w["search_levels"], np.ones(n), prior, prior)
-        for mode in (0, 2, 2, 0):
-            gpu_ctx.set_loop_mode(mode)
-            out.setdefault(mode, []).append(gpu_ctx.vio_update(*args))
+        runs = sweep(gpu_ctx, lambda: gpu_ctx.vio_update(*args), [dict(loop_mode=m) for m in (0, 2, 2, 0)])
     finally:
-        gpu_ctx.set_loop_mode(api.DEFAULT_LOOP_MODE)
         gpu_ctx.vio_set_camera(fr["cam_cfg"], fr["vio_cfg"])
-    ref = out[0][0]
+    ref = runs[0]
     assert ref["total_iters"] >= 3
-    for r in out[2] + out[0][1:]:
+    for r in runs[1:]:
         assert r["total_iters"] == ref["total_iters"]
-        _bits_equal(ref, r, VIO_KEYS)
+        bits_equal(ref, r, VIO_KEYS)

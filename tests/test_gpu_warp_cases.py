@@ -11,10 +11,7 @@ import oracle_bind as O
 import warp_cases as W
 from fast_livo2_b200 import api
 from fast_livo2_b200 import synthetic as S
-from test_gpu_loop_modes import VIO_KEYS, _bits_equal
-from test_gpu_vio import _compare_vio, _setup
-from test_gpu_vio_border import _modes
-from test_warp_cases import EXT, oracle_warp_matrix
+from harness import VIO_KEYS, bits_equal, compare_vio, sweep, variant, vio_setup
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -29,7 +26,7 @@ def _ref_image(cam, seed=0):
 def _device_warp(ctx, camera, case, levels=4, keep_on_device=False):
     cam = W.CAMERAS[camera]
     img = _ref_image(cam)
-    ctx.set_extrinsics(EXT)
+    ctx.set_extrinsics(W.EXT)
     ctx.vio_set_camera(cam, S.VioCfg(levels=levels))
     ctx.vio_set_ref_images([img])
     n = len(case["px_ref"])
@@ -40,7 +37,7 @@ def _device_warp(ctx, camera, case, levels=4, keep_on_device=False):
 
 def _assert_warp_is_oracle_warp_affine(camera, g, img, px_ref, levels=4):
     """warp_patch = the oracle's warpAffine given the device's own A and level, bit for bit, for every patch."""
-    vio = O.OracleVIO(W.CAMERAS[camera], EXT, S.VioCfg(levels=levels))
+    vio = O.OracleVIO(W.CAMERAS[camera], W.EXT, S.VioCfg(levels=levels))
     want = np.array([vio.warp_affine(img, g["A_cur_ref"][i], px_ref[i], int(g["search_levels"][i])) for i in range(len(px_ref))])
     bad = np.nonzero((want != g["warp_patch"]).any(1))[0]
     assert len(bad) == 0, (len(bad), bad[:10])
@@ -60,7 +57,7 @@ def test_search_level_at_the_thresholds(gpu_ctx, camera, thr):
     assert np.array_equal(g["search_levels"], W.search_level(W.det_rounded(Ag)))
     near, split = W.reach(Ag, thr)
     assert near.sum() >= 50 and split.sum() >= 5, (near.sum(), split.sum())
-    Ao, slo = oracle_warp_matrix(camera, case)
+    Ao, slo = W.oracle_warp_matrix(camera, case)
     np.testing.assert_allclose(Ag, Ao, rtol=0, atol=1e-10)
     # |dD| <= |a00| |da11| + |a11| |da00| + |a01| |da10| + |a10| |da01| + rounding, with |da| <= 1e-10
     bound = 1e-10 * np.abs(Ao).reshape(-1, 4).sum(1) * 2 + 8 * np.spacing(thr)
@@ -83,7 +80,7 @@ def test_edge_geometries(gpu_ctx, camera):
     h0 = np.array([nm.startswith("h_zero") for nm in e["name"]])
     assert np.isnan(Ag[h0]).all() and not np.isnan(Ag[~h0]).any()
     assert not g["warp_patch"][h0].any() and g["warp_patch"][~h0].any(1).all()
-    Ao, slo = oracle_warp_matrix(camera, e)
+    Ao, slo = W.oracle_warp_matrix(camera, e)
     np.testing.assert_allclose(Ag[~h0], Ao[~h0], rtol=0, atol=1e-10)
     assert np.array_equal(sl, slo)
     _assert_warp_is_oracle_warp_affine(camera, g, img, e["px_ref"])
@@ -95,7 +92,7 @@ def test_edge_geometries(gpu_ctx, camera):
     gpu_ctx.vio_run(prior, prior)
     a = gpu_ctx.vio_fetch()
     b = gpu_ctx.vio_update(cur, e["pos_w"], g["warp_patch"], sl, np.ones(n), prior, prior)
-    _bits_equal(a, b, VIO_KEYS)
+    bits_equal(a, b, VIO_KEYS)
 
 
 # --------------------------------------------------------------------------------------------------------- c. caller matrices
@@ -112,11 +109,11 @@ def test_warp_affine_on_cancelling_matrices(gpu_ctx):
     inside = 0
     for L in range(1, 9):
         vcfg = S.VioCfg(levels=L)
-        gpu_ctx.set_extrinsics(EXT)
+        gpu_ctx.set_extrinsics(W.EXT)
         gpu_ctx.vio_set_camera(cam, vcfg)
         gpu_ctx.vio_set_ref_images([img])
         out = gpu_ctx.vio_warp_affine(np.zeros(n, np.int32), px, A, sl)
-        vio = O.OracleVIO(cam, EXT, vcfg)
+        vio = O.OracleVIO(cam, W.EXT, vcfg)
         want = np.array([vio.warp_affine(img, A[i], px[i], int(sl[i])) for i in range(n)])
         assert np.array_equal(out, want), L
         inside += int((want != 0).sum())
@@ -149,27 +146,23 @@ def test_deep_update_matches_oracle(gpu_ctx, deep, solve_mode):
     fr, prior, pt = deep
     L = fr["vio_cfg"].levels
     assert set(pt["search_levels"].tolist()) == {0, 1, 2} and (L < 7 or (~pt["in_buffer"]).any())  # taps beyond the buffer read 0
-    _setup(gpu_ctx, fr)
+    vio_setup(gpu_ctx, fr)
     args = _deep_args(fr, prior, pt)
-    gpu_ctx.set_solve_mode(solve_mode)
-    try:
+    with variant(gpu_ctx, solve_mode=solve_mode):
         g = gpu_ctx.vio_update(*args)
-    finally:
-        gpu_ctx.set_solve_mode(0)
     o = O.OracleVIO(fr["cam_cfg"], fr["ext"], fr["vio_cfg"]).update(*args)
     assert (o["iters_per_level"][:L] > 0).all() and o["total_iters"] > L
-    _compare_vio(g, o, L)
+    compare_vio(g, o, L)
 
 
 def test_deep_update_loop_modes_and_tma_are_bit_identical(gpu_ctx, deep):
     fr, prior, pt = deep
-    _setup(gpu_ctx, fr)
+    vio_setup(gpu_ctx, fr)
     args = _deep_args(fr, prior, pt)
-    a, b = _modes(gpu_ctx, args, (2, 0))
-    c, = _modes(gpu_ctx, args, (2,), tuning=api.TUNE_VIO_TMA)
+    a, b, c = sweep(gpu_ctx, lambda: gpu_ctx.vio_update(*args), [dict(loop_mode=2), dict(loop_mode=0), dict(loop_mode=2, tuning=api.TUNE_VIO_TMA)])
     assert a["total_iters"] > fr["vio_cfg"].levels
-    _bits_equal(a, b, VIO_KEYS)
-    _bits_equal(a, c, VIO_KEYS)
+    bits_equal(a, b, VIO_KEYS)
+    bits_equal(a, c, VIO_KEYS)
 
 
 def test_timing_and_phase_stamps_at_eight_levels_and_eight_iterations(gpu_ctx):
@@ -177,23 +170,22 @@ def test_timing_and_phase_stamps_at_eight_levels_and_eight_iterations(gpu_ctx):
     launches time every (level, iteration) slot; the persistent kernel stamps exactly the iterations it executed (slot
     (levels - 1 - level) * max_iterations + it, as iters_per_level reports them) and leaves the others zero."""
     fr, prior, pt = W.deep_frame(8)
-    _setup(gpu_ctx, fr)
+    vio_setup(gpu_ctx, fr)
     args = _deep_args(fr, prior, pt)
     try:
         gpu_ctx.set_kernel_timing(True)
-        gpu_ctx.set_loop_mode(0)
-        t = gpu_ctx.vio_update(*args)
-        ms = gpu_ctx.get_kernel_timing()
+        with variant(gpu_ctx, loop_mode=0):
+            t = gpu_ctx.vio_update(*args)
+            ms = gpu_ctx.get_kernel_timing()
         gpu_ctx.set_kernel_timing(False)
-        gpu_ctx.set_loop_mode(2)
         gpu_ctx.set_phase_stamps(True)
-        s = gpu_ctx.vio_update(*args)
-        stamps = gpu_ctx.get_phase_stamps()
+        with variant(gpu_ctx, loop_mode=2):
+            s = gpu_ctx.vio_update(*args)
+            stamps = gpu_ctx.get_phase_stamps()
     finally:
         gpu_ctx.set_kernel_timing(False)
         gpu_ctx.set_phase_stamps(False)
-        gpu_ctx.set_loop_mode(api.DEFAULT_LOOP_MODE)
-    _bits_equal(t, s, VIO_KEYS)
+    bits_equal(t, s, VIO_KEYS)
     assert (ms["vio_patch_ms"] > 0).all() and (ms["vio_solve_ms"] > 0).all()
     ipl = s["iters_per_level"]
     executed = np.zeros(64, bool)

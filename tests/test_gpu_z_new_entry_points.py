@@ -8,7 +8,7 @@ import pytest
 
 import oracle_bind as O
 from fast_livo2_b200 import api
-from test_gpu_vio import _gpu_warp, _setup, _vio_prior
+from harness import compare_lio, lio_gpu, lio_oracle, vio_prior, vio_setup, vio_warp
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -19,9 +19,9 @@ def test_warp_affine_alone_with_caller_matrices(gpu_ctx, small_vio_frame):
     identical to the batched producer for its own matrices, and equal to the oracle's warpAffine for arbitrary ones
     (rotation + anisotropic scale, search levels 0 / 1; a zero matrix leaves zeros)."""
     fr = small_vio_frame
-    _setup(gpu_ctx, fr)
-    prior = _vio_prior(fr)
-    g = _gpu_warp(gpu_ctx, fr, prior)
+    vio_setup(gpu_ctx, fr)
+    prior = vio_prior(fr)
+    g = vio_warp(gpu_ctx, fr, prior)
     n = len(fr["vis_pos"])
     again = gpu_ctx.vio_warp_affine(np.zeros(n, np.int32), fr["px_ref"], g["A_cur_ref"], g["search_levels"])
     assert np.array_equal(again, g["warp_patch"])
@@ -157,20 +157,12 @@ def test_lio_association_on_voxel_boundaries_and_negative_keys(gpu_ctx, kind):
     reciprocal: multiply), 0.4 (true fp64 division) and 2.0. The same scans go through the reference source on the CPU in
     tests/test_oracle_ref_pin.py::test_edge_scan_oracle_reproduces_the_reference_source."""
     from conftest import get_frame
-    from fast_livo2_b200 import synthetic as S
-    from parity_util import assert_state_close, edge_scan
-    from test_oracle_ref_pin import EDGE_FRAMES
+    from parity_util import edge_scan
+    from ref_pin_cases import EDGE_FRAMES
 
     fr = get_frame(**EDGE_FRAMES[kind])
     pts, ext, state = edge_scan(fr)
-    vs = fr["lio_cfg"].voxel_size
-    gpu_ctx.set_extrinsics(ext)
-    gpu_ctx.map_upload(fr["map"], vs)
-    g = gpu_ctx.lio_update(pts, state, state, fr["lio_cfg"])
-    lio = O.OracleLIO(fr["lio_cfg"], ext)
-    lio.set_map(fr["map"])
-    o = lio.state_estimation(pts, state, state)
-    assert g["iters"] == o["iters"] and np.array_equal(g["M"], o["M"]) and o["M"][0] > 20
-    assert np.array_equal(g["match_plane"], o["match_plane"]) and np.array_equal(g["normal_plane"], o["normal_plane"])
-    assert np.array_equal(g["dis_to_plane"], o["dis_to_plane"])
-    assert_state_close(g["state"], o["state"])
+    fe = dict(fr, pts=pts, ext=ext, state_prior=state)
+    o = lio_oracle(fe)
+    assert o["M"][0] > 20
+    compare_lio(lio_gpu(gpu_ctx, fe), o)

@@ -7,29 +7,7 @@ import pytest
 import map_bind as MB
 import oracle_bind as O
 from fast_livo2_b200 import synthetic as S
-
-
-def _tick_points(rng, rects, n, lo, hi, noise=0.01):
-    """n noisy points on the scene's planes inside the axis-aligned window [lo, hi] (the sensor's footprint of this tick),
-    float32-rounded like TransformLidar's output (src/voxel_map.cpp:524-526), each with a small SPD covariance."""
-    pw, _ = S.sample_on_rects(rects, 6 * n, rng)
-    pw = pw[np.all((pw >= lo) & (pw <= hi), axis=1)][:n]
-    pw = pw + rng.normal(0, noise, pw.shape)
-    pw = pw.astype(np.float32).astype(np.float64)
-    A = rng.normal(0, 0.01, (len(pw), 3, 3))
-    var = A @ A.transpose(0, 2, 1) + np.eye(3) * 1e-5
-    return pw, var
-
-
-def _oracle(cfg):
-    ext = S.avia_extrinsics()
-    return O.OracleLIO(cfg, ext)
-
-
-def _oracle_update(orc, pw, var):
-    pw = np.ascontiguousarray(pw, np.float64)
-    var = np.ascontiguousarray(var.reshape(-1, 9), np.float64)
-    orc.lib.orc_lio_update_map(orc.h, O.dptr(pw), O.dptr(var), len(pw))
+from map_bind import oracle_map, oracle_update_map, tick_points
 
 
 @pytest.mark.parametrize("cfg", [S.LioCfg(), S.LioCfg(voxel_size=0.4, max_layer=3, max_points_num=20), S.LioCfg(voxel_size=2.0, max_layer=1, min_eigen_value=0.0005)],
@@ -37,15 +15,15 @@ def _oracle_update(orc, pw, var):
 def test_ten_ticks_of_update_voxel_map_match_the_oracle(cfg):
     rng = np.random.default_rng(5)
     rects = S.make_scene("room", 0.5)
-    orc, hm = _oracle(cfg), MB.HostMap(cfg)
+    orc, hm = oracle_map(cfg), MB.HostMap(cfg)
     total = 0
     for tick in range(10):
         # a window that slides through the room: old voxels keep receiving points (refits, max_points_num), new ones appear
         lo = np.array([-10.0 + 1.5 * tick, -8.0, -2.0])
         hi = lo + np.array([8.0, 16.0, 6.0])
-        pw, var = _tick_points(rng, rects, 6000, lo, hi)
+        pw, var = tick_points(rng, rects, 6000, lo, hi)
         total += len(pw)
-        _oracle_update(orc, pw, var)
+        oracle_update_map(orc, pw, var)
         assert hm.apply(pw, var) == 0
         n = MB.compare_flat_maps(hm.flatten(), orc.flatten(), what=("device state machine", "oracle"), exact=True)  # serial policy: bit for bit
         assert n > 0
@@ -62,12 +40,12 @@ def test_build_voxel_map_form_matches_the_oracle():
     cfg = S.LioCfg()
     rng = np.random.default_rng(9)
     rects = S.make_scene("room", 0.5)
-    orc, hm = _oracle(cfg), MB.HostMap(cfg)
-    pw, var = _tick_points(rng, rects, 40000, np.array([-12.0, -9.0, -3.0]), np.array([12.0, 9.0, 5.0]))
+    orc, hm = oracle_map(cfg), MB.HostMap(cfg)
+    pw, var = tick_points(rng, rects, 40000, np.array([-12.0, -9.0, -3.0]), np.array([12.0, 9.0, 5.0]))
     # the oracle's BuildVoxelMap recomputes var from body points; the build FORM (push all, then init) is what is compared:
     # an empty oracle map fed through UpdateVoxelMap differs (it inits at the 6th point) — so build the oracle map by hand
-    orc2 = _oracle(cfg)
-    _oracle_update(orc2, pw[:0], var[:0])
+    orc2 = oracle_map(cfg)
+    oracle_update_map(orc2, pw[:0], var[:0])
     assert hm.apply(pw, var, build=True) == 0
     fb = hm.flatten()
     # reference for the build form: the oracle's own BuildVoxelMap needs (world, body, state); give it an identity pose so that
@@ -89,8 +67,8 @@ def test_build_voxel_map_form_matches_the_oracle():
     assert n > 500 and len(fb["keys"]) > 0
     # then five incremental ticks on both
     for tick in range(5):
-        pw2, var2 = _tick_points(rng, rects, 5000, np.array([-12.0, -9.0, -3.0]), np.array([12.0, 9.0, 5.0]))
-        _oracle_update(orc3, pw2, var2)
+        pw2, var2 = tick_points(rng, rects, 5000, np.array([-12.0, -9.0, -3.0]), np.array([12.0, 9.0, 5.0]))
+        oracle_update_map(orc3, pw2, var2)
         assert hm3.apply(pw2, var2) == 0
         MB.compare_flat_maps(hm3.flatten(), orc3.flatten(), rtol=1e-7)
 
@@ -102,11 +80,11 @@ def test_map_sliding_keeps_the_box_and_later_ticks_still_match():
     cfg = S.LioCfg()
     rng = np.random.default_rng(17)
     rects = S.make_scene("room", 0.5)
-    orc, hm = _oracle(cfg), MB.HostMap(cfg)
+    orc, hm = oracle_map(cfg), MB.HostMap(cfg)
     lo_w, hi_w = np.array([-12.0, -9.0, -3.0]), np.array([12.0, 9.0, 5.0])
     for tick in range(6):
-        pw, var = _tick_points(rng, rects, 6000, lo_w, hi_w)
-        _oracle_update(orc, pw, var)
+        pw, var = tick_points(rng, rects, 6000, lo_w, hi_w)
+        oracle_update_map(orc, pw, var)
         assert hm.apply(pw, var) == 0
     before = hm.usage()
     # sensor at voxel (4, -2, 1), half_map_size 12 voxels
@@ -118,8 +96,8 @@ def test_map_sliding_keeps_the_box_and_later_ticks_still_match():
     assert after["pool_points"] < before["pool_points"] and after["recs"] <= before["recs"]  # compaction
     MB.compare_flat_maps(hm.flatten(), orc.flatten(), exact=True)
     for tick in range(4):
-        pw, var = _tick_points(rng, rects, 6000, lo_w, hi_w)
-        _oracle_update(orc, pw, var)
+        pw, var = tick_points(rng, rects, 6000, lo_w, hi_w)
+        oracle_update_map(orc, pw, var)
         assert hm.apply(pw, var) == 0
         MB.compare_flat_maps(hm.flatten(), orc.flatten(), exact=True)
 
@@ -128,7 +106,7 @@ def test_capacity_errors_are_reported_not_ignored():
     cfg = S.LioCfg()
     rng = np.random.default_rng(2)
     rects = S.make_scene("room", 0.5)
-    pw, var = _tick_points(rng, rects, 5000, np.array([-12.0, -9.0, -3.0]), np.array([12.0, 9.0, 5.0]))
+    pw, var = tick_points(rng, rects, 5000, np.array([-12.0, -9.0, -3.0]), np.array([12.0, 9.0, 5.0]))
     assert MB.HostMap(cfg, node_cap=16).apply(pw, var) & 1       # MAP_ERR_NODES
     assert MB.HostMap(cfg, pool_cap=64).apply(pw, var) & 2       # MAP_ERR_POOL
     assert MB.HostMap(cfg, hash_cap=64).apply(pw, var) & 8       # MAP_ERR_HASH
@@ -148,8 +126,8 @@ def test_root_voxel_keys_on_voxel_faces_and_negative_coordinates(voxel_size):
     vals = np.concatenate([face, np.nextafter(face, np.float32(np.inf)), np.nextafter(face, np.float32(-np.inf)), np.float32([0.0, -0.0, 1e-30, -1e-30])])
     grid = np.stack(np.meshgrid(vals, vals[::5], vals[::7], indexing="ij"), -1).reshape(-1, 3).astype(np.float64)
     var = np.tile(np.eye(3) * 1e-4, (len(grid), 1, 1))
-    orc, hm = _oracle(cfg), MB.HostMap(cfg)
-    _oracle_update(orc, grid, var)
+    orc, hm = oracle_map(cfg), MB.HostMap(cfg)
+    oracle_update_map(orc, grid, var)
     assert hm.apply(grid, var) == 0
     a, b = hm.flatten(), orc.flatten()
     assert len(a["keys"]) == len(b["keys"]) > 50

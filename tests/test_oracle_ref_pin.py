@@ -11,7 +11,6 @@ run with FL2_RECORD_REF_PIN=1 where the library is built; see oracle_bind.RefPin
 holds the reference's full outputs for two of the cases (test_oracle_matches_reference_golden) — tests/golden/make_ref_golden.py
 regenerates it."""
 import ctypes as C
-import os
 
 import numpy as np
 import pytest
@@ -19,45 +18,13 @@ import pytest
 import oracle_bind as O
 from conftest import get_frame
 from fast_livo2_b200 import synthetic as S
+from harness import lio_oracle
+from map_bind import oracle_update_map, tick_points
+from ref_pin_cases import EDGE_FRAMES, LIO_CASES, LIO_GOLDEN, lio_case
 
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_lio_golden.npz")
 PIN = O.RefPin("lio")
 needs_ref = pytest.mark.skipif(not O.RefPin.available("lio"), reason="neither oracle/_ref/libfl2_ref_lio.so nor tests/golden/ref_pin/lio.npz")
 EXACT = ("M", "ptpl_center", "ptpl_dis", "normals")
-
-CASES = {
-    "small": dict(frame=dict(seed=1, n_pts=4000, n_map=150_000, scene_scale=0.5)),
-    "seed3": dict(frame=dict(seed=3, n_pts=5000, n_map=150_000, scene_scale=0.5)),
-    "20k": dict(frame=dict(seed=4, n_pts=20000, n_map=150_000, scene_scale=0.5)),
-    "three_iterations": dict(frame=dict(seed=0, n_pts=5000, n_map=150_000, scene_scale=0.5), cfg=dict(max_iterations=3)),
-    "hilti_voxel_04_non_identity_extrinsics": dict(frame=dict(seed=5, n_pts=6000, n_map=400_000, lio=S.LioCfg(voxel_size=0.4, min_eigen_value=1e-4, max_points_num=100),
-                                                            ext=S.hilti_extrinsics(), scene="corridor", scene_scale=0.25)),
-    "voxel_2m": dict(frame=dict(seed=7, n_pts=6000, n_map=300_000, lio=S.LioCfg(voxel_size=2.0, min_eigen_value=0.005), scene_scale=2.0)),
-}
-
-
-EDGE_FRAMES = {
-    "voxel_0.5": dict(seed=1, n_pts=4000, n_map=150_000, scene_scale=0.5),
-    "voxel_0.4": dict(seed=5, n_pts=6000, n_map=400_000, lio=S.LioCfg(voxel_size=0.4, min_eigen_value=1e-4, max_points_num=100), ext=S.hilti_extrinsics(), scene="corridor",
-                      scene_scale=0.25),
-    "voxel_2.0": dict(seed=7, n_pts=6000, n_map=300_000, lio=S.LioCfg(voxel_size=2.0, min_eigen_value=0.005), scene_scale=2.0),
-}
-
-
-def _case(name):
-    c = CASES[name]
-    fr = get_frame(**c["frame"])
-    cfg = fr["lio_cfg"]
-    if "cfg" in c:
-        cfg = S.LioCfg(**{**cfg.__dict__, **c["cfg"]})
-    return fr, cfg
-
-
-def _oracle(fr, cfg, state_in=None):
-    lio = O.OracleLIO(cfg, fr["ext"])
-    lio.set_map(fr["map"])
-    s = fr["state_prior"] if state_in is None else state_in
-    return lio.state_estimation(fr["pts"], s, fr["state_prior"])
 
 
 def _ref_lio(fr, **kw):
@@ -81,10 +48,10 @@ def _check(o, r, planes):
 
 
 @needs_ref
-@pytest.mark.parametrize("name", list(CASES))
+@pytest.mark.parametrize("name", list(LIO_CASES))
 def test_oracle_reproduces_the_reference_source(name):
-    fr, cfg = _case(name)
-    o = _oracle(fr, cfg)
+    fr, cfg = lio_case(name)
+    o = lio_oracle(fr, cfg)
     r = PIN.get(f"state_estimation/{name}", lambda: _ref_lio(fr, cfg=cfg), exact=EXACT)
     assert r["iters"] >= 2
     _check(o, r, fr["map"]["planes"])
@@ -93,11 +60,11 @@ def test_oracle_reproduces_the_reference_source(name):
 @needs_ref
 def test_oracle_reproduces_the_reference_source_on_early_stop():
     """A tight prior converges twice in a row: the rematch / stop rule (voxel_map.cpp:477-499) ends the loop after 2 iterations."""
-    fr, cfg = _case("small")
-    st = _oracle(fr, cfg)["state"].copy()
+    fr, cfg = lio_case("small")
+    st = lio_oracle(fr, cfg)["state"].copy()
     st[25:] = (np.eye(19) * 1e-12).reshape(-1)
     fr2 = dict(fr, state_prior=st)
-    o = _oracle(fr2, cfg)
+    o = lio_oracle(fr2, cfg)
     r = PIN.get("early_stop", lambda: _ref_lio(fr2, cfg=cfg), exact=EXACT)
     assert r["iters"] == 2
     _check(o, r, fr["map"]["planes"])
@@ -134,7 +101,7 @@ def test_hand_built_association_oracle_reproduces_the_reference_source(name):
     import lio_assoc
 
     fr = lio_assoc.case(name)
-    o = _oracle(fr, fr["lio_cfg"])
+    o = lio_oracle(fr, fr["lio_cfg"])
     r = PIN.get(f"assoc/{name}", lambda: _ref_lio(fr, cfg=fr["lio_cfg"]), exact=EXACT)
     assert r["iters"] == 5
     _check(o, r, fr["map"]["planes"])
@@ -165,9 +132,9 @@ def test_calc_body_cov_matches_the_reference_source():
 @pytest.mark.parametrize("name", ["small", "hilti_voxel_04_non_identity_extrinsics"])
 def test_oracle_matches_reference_golden(name):
     """Same check against the committed outputs of the reference source (generated by tests/golden/make_ref_golden.py)."""
-    g = np.load(GOLDEN)
-    fr, cfg = _case(name)
-    o = _oracle(fr, cfg)
+    g = np.load(LIO_GOLDEN)
+    fr, cfg = lio_case(name)
+    o = lio_oracle(fr, cfg)
     r = dict(iters=int(g[f"{name}_iters"]), M=g[f"{name}_M"], ptpl_center=g[f"{name}_ptpl_center"], ptpl_dis=g[f"{name}_ptpl_dis"], normals=g[f"{name}_normals"],
              state=g[f"{name}_state"])
     _check(o, r, fr["map"]["planes"])
@@ -192,7 +159,6 @@ def test_oracle_update_voxel_map_reproduces_the_reference_source(cfg):
     plane_var, d and radius. Tolerance, not bits: the reference calls Eigen::EigenSolver, which here is the stand-in's Jacobi
     and in the oracle another Jacobi — a genuine Eigen would differ in the last bits just the same."""
     import map_bind as MB
-    from test_map_host import _oracle_update, _tick_points
 
     rng = np.random.default_rng(5)
     rects = S.make_scene("room", 0.5)
@@ -201,8 +167,8 @@ def test_oracle_update_voxel_map_reproduces_the_reference_source(cfg):
     n = 0
     for tick in range(8):
         lo = np.array([-10.0 + 1.5 * tick, -8.0, -2.0])
-        pw, var = _tick_points(rng, rects, 6000, lo, lo + np.array([8.0, 16.0, 6.0]))
-        _oracle_update(orc, pw, var)
+        pw, var = tick_points(rng, rects, 6000, lo, lo + np.array([8.0, 16.0, 6.0]))
+        oracle_update_map(orc, pw, var)
         if ref is not None:
             ref.update(pw, var)
         n = _compare_map(MB, orc.flatten(), ref, f"update_map/{cid}/tick{tick}", ("oracle", "reference source"))

@@ -28,6 +28,7 @@ from fractions import Fraction
 
 import numpy as np
 
+import oracle_bind as O
 from fast_livo2_b200 import synthetic as S
 
 THRESHOLDS = (3.0, 12.0)
@@ -40,6 +41,7 @@ CAMERAS = {
 }
 N_GEOMETRIES = 34_000  # per camera and threshold, before the geometries without a crossing are dropped
 T_CUR = (np.eye(3), np.zeros(3))
+EXT = S.avia_extrinsics()
 
 
 # ----------------------------------------------------------------------------------------------- the rule and the reach flags
@@ -410,3 +412,12 @@ def deep_frame(levels, pinned=False, n=96, seed=0):
     pt["inv_ref_expo"] = np.ones(len(px))
     pt["in_buffer"] = inb
     return fr, prior, pt
+
+
+# ----------------------------------------------------------------------------------------------- on the oracle
+def oracle_warp_matrix(camera, case, idx=None, levels=4):
+    """(A, search level) of the oracle's getWarpMatrixAffineHomography + getBestSearchLevel on the cases idx (all by default)."""
+    vio = O.OracleVIO(CAMERAS[camera], EXT, S.VioCfg(levels=levels))
+    idx = range(len(case["px_ref"])) if idx is None else idx
+    A, sl = zip(*[vio.warp_matrix(case["px_ref"][i], case["pos_w"][i], case["normal_w"][i], (case["T_ref"][0][i], case["T_ref"][1][i]), T_CUR) for i in idx])
+    return np.array(A), np.array(sl, np.int32)
