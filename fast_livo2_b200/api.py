@@ -84,6 +84,7 @@ def load_library():
     lib.esikf_map_device_update.argtypes = [vp, vp]
     lib.esikf_map_device_update_points.argtypes = [vp, vp, vp, C.c_int32]
     lib.esikf_map_device_stats.argtypes = [vp, vp]
+    lib.esikf_map_device_capacity.argtypes = [vp, vp]
     lib.esikf_map_device_slide.argtypes = [vp, vp, vp]
     lib.esikf_map_device_download.argtypes = [vp, vp, vp, vp, C.c_int32, vp, C.c_int32, vp, vp]
     lib.esikf_lio_fetch_normals.argtypes = [vp, vp]
@@ -124,7 +125,7 @@ DEFAULT_LOOP_MODE = 2  # esikf_set_loop_mode: 2 (alias 1) persistent kernel per 
 
 class MapCfgC(C.Structure):
     _fields_ = [("voxel_size", C.c_double), ("min_eigen_value", C.c_double), ("dept_err", C.c_double), ("beam_err", C.c_double), ("max_layer", C.c_int32),
-                ("max_points_num", C.c_int32), ("layer_init_num", C.c_int32 * 8), ("pad", C.c_int32), ("root_capacity", C.c_int64), ("node_capacity", C.c_int64),
+                ("max_points_num", C.c_int32), ("layer_init_num", C.c_int32 * 8), ("grow", C.c_int32), ("root_capacity", C.c_int64), ("node_capacity", C.c_int64),
                 ("record_capacity", C.c_int64), ("point_capacity", C.c_int64)]
 
 
@@ -135,7 +136,7 @@ class MapStatsC(C.Structure):
 
 EXPORTED_SYMBOLS = [
     "esikf_create", "esikf_destroy", "esikf_last_error", "esikf_stream", "esikf_synchronize", "esikf_host_alloc", "esikf_host_free", "esikf_launch_count", "esikf_set_solve_mode", "esikf_set_loop_mode", "esikf_set_tuning",
-    "esikf_set_extrinsics", "esikf_set_lidar_extrinsics", "esikf_map_upload", "esikf_map_patch", "esikf_map_device_init", "esikf_map_device_build", "esikf_map_device_update", "esikf_map_device_update_points", "esikf_map_device_slide", "esikf_map_device_stats", "esikf_map_device_download", "esikf_lio_fetch_normals", "esikf_lio_set_scan", "esikf_lio_run", "esikf_lio_fetch",
+    "esikf_set_extrinsics", "esikf_set_lidar_extrinsics", "esikf_map_upload", "esikf_map_patch", "esikf_map_device_init", "esikf_map_device_build", "esikf_map_device_update", "esikf_map_device_update_points", "esikf_map_device_slide", "esikf_map_device_stats", "esikf_map_device_capacity", "esikf_map_device_download", "esikf_lio_fetch_normals", "esikf_lio_set_scan", "esikf_lio_run", "esikf_lio_fetch",
     "esikf_lio_update", "esikf_lio_fetch_point_cov", "esikf_vio_set_camera", "esikf_vio_set_image", "esikf_vio_set_patches",
     "esikf_vio_run", "esikf_vio_fetch", "esikf_vio_update", "esikf_vio_get_image_patch", "esikf_vio_set_ref_images",
     "esikf_vio_warp_patches", "esikf_vio_warp_affine", "esikf_vio_set_inverse_refs", "esikf_comm_unique_id", "esikf_comm_init", "esikf_comm_rank", "esikf_shard_range", "esikf_peer_export", "esikf_peer_attach", "esikf_profile_kernel", "esikf_set_kernel_timing", "esikf_get_kernel_timing", "esikf_set_phase_stamps", "esikf_get_phase_stamps",
@@ -229,15 +230,24 @@ class Context:
         self._ck(self.lib.esikf_map_patch(self.h, ids.ctypes.data_as(C.POINTER(C.c_int32)), planes.ctypes.data, len(ids)))
 
     # ------------------------------------------------------------------ device-resident map
-    def map_device_init(self, cfg, root_capacity=0, node_capacity=0, record_capacity=0, point_capacity=0):
-        """cfg: synthetic.LioCfg (voxel_size, min_eigen_value, dept_err, beam_err, max_layer, max_points_num, layer_init_num)."""
+    def map_device_init(self, cfg, root_capacity=0, node_capacity=0, record_capacity=0, point_capacity=0, grow=False):
+        """cfg: synthetic.LioCfg (voxel_size, min_eigen_value, dept_err, beam_err, max_layer, max_points_num, layer_init_num).
+        grow: the capacities are starting sizes and the map grows when a tick would exceed one (else they are fixed)."""
         m = MapCfgC()
         m.voxel_size, m.min_eigen_value, m.dept_err, m.beam_err = cfg.voxel_size, cfg.min_eigen_value, cfg.dept_err, cfg.beam_err
         m.max_layer, m.max_points_num = cfg.max_layer, cfg.max_points_num
         for k in range(8):
             m.layer_init_num[k] = cfg.layer_init_num[min(k, len(cfg.layer_init_num) - 1)]
         m.root_capacity, m.node_capacity, m.record_capacity, m.point_capacity = root_capacity, node_capacity, record_capacity, point_capacity
+        m.grow = 1 if grow else 0
         self._ck(self.lib.esikf_map_device_init(self.h, C.byref(m)))
+
+    def map_device_capacity(self):
+        """The device map's current capacities (root_capacity = hash slots / 2) and whether it grows."""
+        m = MapCfgC()
+        self._ck(self.lib.esikf_map_device_capacity(self.h, C.byref(m)))
+        return dict(root_capacity=m.root_capacity, node_capacity=m.node_capacity, record_capacity=m.record_capacity, point_capacity=m.point_capacity,
+                    grow=bool(m.grow))
 
     def map_device_build(self, state):
         self._ck(self.lib.esikf_map_device_build(self.h, _c(state, np.float64).ctypes.data))

@@ -159,6 +159,7 @@ struct esikf_ctx {
   MapCfg arena_cfg{};
   MapArenaBufs spare;  // esikf_map_device_slide copies the surviving roots into it, then it and `map` change roles
   DevBuf<int> map_work, map_survivors;
+  DevBuf<unsigned long long> map_demand;  // map_demand_kernel's sums and defer word (capacity growth)
   DevBuf<double> map_pt, map_pt_normal;
   DevBuf<unsigned int> map_key_in, map_key_out, map_idx_in, map_idx_out;
   DevBuf<MapTouched> map_touched;
@@ -499,6 +500,8 @@ int esikf_map_patch(esikf_ctx *ctx, const int32_t *plane_ids, const esikf_plane 
 }
 
 // ------------------------------------------------------------------------------------------------ device-resident map (f1)
+__global__ void gather_normals_kernel(const int32_t *__restrict__ match_plane, const PlaneRec *__restrict__ recs, int n, double *__restrict__ out);
+
 static int map_check_errors(esikf_ctx *ctx, const char *what) {
   int c[4];
   unsigned long long pool_used = 0;
@@ -521,7 +524,7 @@ static int map_check_errors(esikf_ctx *ctx, const char *what) {
 }
 
 int esikf_map_device_init(esikf_ctx *ctx, const esikf_map_cfg *cfg) {
-  if (!ctx || !cfg || !(cfg->voxel_size > 0) || cfg->max_layer < 0 || cfg->max_layer >= MAP_MAX_LAYERS || cfg->max_points_num < 1)
+  if (!ctx || !cfg || !(cfg->voxel_size > 0) || cfg->max_layer < 0 || cfg->max_layer >= MAP_MAX_LAYERS || cfg->max_points_num < 1 || (cfg->grow != 0 && cfg->grow != 1))
     return fail(ctx, ESIKF_ERR_ARG, "map_device_init: bad argument");
   for (int k = 0; k <= cfg->max_layer; k++)
     if (cfg->layer_init_num[k] < 1) return fail(ctx, ESIKF_ERR_ARG, "map_device_init: layer_init_num[%d] = %d", k, cfg->layer_init_num[k]);
@@ -536,6 +539,7 @@ int esikf_map_device_init(esikf_ctx *ctx, const esikf_map_cfg *cfg) {
   if (node_cap > 0x7fffffff || rec_cap > 0x7fffffff || pool_cap > 0x7fffffff) return fail(ctx, ESIKF_ERR_ARG, "map_device_init: capacity above 2^31");
   CK(ctx->map.reserve(cap, (int)node_cap, (int)rec_cap, pool_cap));
   CK(ctx->map_work.reserve(4));
+  if (cfg->grow) CK(ctx->map_demand.reserve(MAP_DEMAND_WORDS));
   MapCfg &mc = ctx->arena_cfg;
   mc.voxel_size = (float)cfg->voxel_size, mc.planer_threshold = (float)cfg->min_eigen_value;
   mc.max_layer = cfg->max_layer, mc.max_points_num = cfg->max_points_num;
@@ -555,8 +559,8 @@ int esikf_map_device_init(esikf_ctx *ctx, const esikf_map_cfg *cfg) {
   return ESIKF_OK;
 }
 
-// sort by slot, list the touched roots, replay them
-static int map_apply_points(esikf_ctx *ctx, int n, bool build) {
+// sort by slot, list the touched roots, (growth on) bound what they need, replay them unless that does not fit
+static int map_replay_tick(esikf_ctx *ctx, int n, bool build) {
   cudaStream_t st = ctx->stream;
   const unsigned int invalid = ctx->map.hash_cap;
   size_t tmp_bytes = 0;
@@ -566,10 +570,92 @@ static int map_apply_points(esikf_ctx *ctx, int n, bool build) {
                                      ctx->map_hash_bits + 1, st));
   CK(cudaMemsetAsync(ctx->map_work.p, 0, 2 * sizeof(int), st));
   map_heads_kernel<<<(n + 255) / 256, 256, 0, st>>>(ctx->map_key_out.p, n, invalid, ctx->map_touched.p, ctx->map_work.p);
-  map_replay_kernel<<<ctx->sm_count * 4, 128, 0, st>>>(ctx->arena(), ctx->map_touched.p, ctx->map_work.p, ctx->map_idx_out.p, ctx->map_pt.p, build ? 1 : 0);
+  const unsigned long long *defer = nullptr;
+  if (ctx->map_cfg.grow) {
+    CK(cudaMemsetAsync(ctx->map_demand.p, 0, MAP_DEMAND_WORDS * sizeof(unsigned long long), st));
+    map_demand_kernel<<<ctx->sm_count * 4, 128, 0, st>>>(ctx->arena(), ctx->map_touched.p, ctx->map_work.p, ctx->map_demand.p, build ? 1 : 0);
+    defer = ctx->map_demand.p + 5;
+    ctx->launches++;
+  }
+  map_replay_kernel<<<ctx->sm_count * 4, 128, 0, st>>>(ctx->arena(), ctx->map_touched.p, ctx->map_work.p, ctx->map_idx_out.p, ctx->map_pt.p, build ? 1 : 0, defer);
   ctx->launches += 4;
   CK(cudaGetLastError());
-  return map_check_errors(ctx, build ? "map_device_build" : "map_device_update");
+  return ESIKF_OK;
+}
+
+static int map_capacity_error(esikf_ctx *ctx, const char *what, const char *resource, long long need) {
+  ctx->have_map = false;
+  return fail(ctx, ESIKF_ERR_STATE, "%s: the device map cannot grow to %lld %s (the limit is 2^31)", what, need, resource);
+}
+
+// Capacity growth: copy the live arena into one of the given capacities with the slide's machinery and an unbounded box (the
+// copy only compacts, so it fits any arena at least as large), make it the map and free the old one. Roots without a root
+// node (keys inserted by a tick that was deferred) are not copied. When an allocation fails the map is invalidated: a
+// deferred tick may have inserted keys already, and the LIO probe would treat them as present voxels.
+static int map_grow(esikf_ctx *ctx, long long hash_cap, long long node_cap, long long rec_cap, long long pool_cap, const char *what) {
+  if (hash_cap > (1ll << 31)) return map_capacity_error(ctx, what, "hash slots", hash_cap);
+  if (node_cap > 0x7fffffff) return map_capacity_error(ctx, what, "nodes", node_cap);
+  if (rec_cap > 0x7fffffff) return map_capacity_error(ctx, what, "records", rec_cap);
+  if (pool_cap > 0x7fffffff) return map_capacity_error(ctx, what, "stored points", pool_cap);
+  cudaStream_t st = ctx->stream;
+  MapArenaBufs fresh;
+  cudaError_t e = fresh.reserve((uint32_t)hash_cap, (int)node_cap, (int)rec_cap, pool_cap);
+  if (e == cudaSuccess) e = ctx->map_survivors.reserve((size_t)(ctx->map_last.roots > 0 ? ctx->map_last.roots : 1) + 1);
+  if (e != cudaSuccess) {
+    cudaGetLastError();  // a failed allocation is not sticky: later calls must not report it again
+    ctx->have_map = false;
+    return fail(ctx, ESIKF_ERR_CUDA, "%s: growing the device map to %lld hash slots / %lld nodes / %lld records / %lld points failed: %s", what, hash_cap, node_cap,
+                rec_cap, pool_cap, cudaGetErrorString(e));
+  }
+  const MapArena S = ctx->arena(), D = fresh.view(ctx->arena_cfg);
+  const long long big = 1ll << 40;
+  map_reset_kernel<<<(unsigned)((hash_cap + 255) / 256), 256, 0, st>>>(D);
+  CK(cudaMemsetAsync(ctx->map_work.p, 0, 2 * sizeof(int), st));
+  map_survivors_kernel<<<(ctx->map.hash_cap + 255) / 256, 256, 0, st>>>(S, -big, -big, -big, big, big, big, ctx->map_survivors.p, ctx->map_work.p);
+  map_copy_kernel<<<ctx->sm_count * 4, 128, 0, st>>>(S, D, ctx->map_survivors.p, ctx->map_work.p);
+  ctx->launches += 3;
+  CK(cudaGetLastError());
+  std::swap(ctx->map, fresh);
+  int bits = 0;
+  while ((1ll << bits) < hash_cap) bits++;
+  ctx->hash_mask = (uint32_t)(hash_cap - 1), ctx->map_hash_bits = bits;  // what the LIO probe and the key sort read
+  return map_check_errors(ctx, what);  // synchronises: the old arena (now in `fresh`) is no longer read when it is freed
+}
+
+// growth on: room in the hash table for n new roots (at most one per point) before any key of the tick is inserted
+static bool map_hash_short(const esikf_ctx *ctx, int n) { return ctx->map_cfg.grow && (long long)ctx->map_last.roots + n > (long long)ctx->map.hash_cap / 2; }
+static int map_grow_hash(esikf_ctx *ctx, int n, const char *what) {
+  const MapArenaBufs &m = ctx->map;
+  return map_grow(ctx, map_grown_hash(m.hash_cap, ctx->map_last.roots, n), m.node_cap, m.rec_cap, m.pool_cap, what);
+}
+
+// Apply the keyed tick (map_key_in / map_idx_in, points in map_pt). With growth on, a tick the demand bound says might not
+// fit is not replayed: each short resource grows to map_grown_capacity, the points are keyed again into the new arena and
+// the tick is applied there (a tick that fits costs no extra round trip: the defer word rides on the error check's sync).
+static int map_apply_points(esikf_ctx *ctx, int n, bool build) {
+  const char *what = build ? "map_device_build" : "map_device_update";
+  cudaStream_t st = ctx->stream;
+  int rc = map_replay_tick(ctx, n, build);
+  if (rc || !ctx->map_cfg.grow) return rc ? rc : map_check_errors(ctx, what);
+  unsigned long long d[MAP_DEMAND_WORDS];
+  CK(cudaMemcpyAsync(d, ctx->map_demand.p, sizeof(d), cudaMemcpyDeviceToHost, st));
+  if ((rc = map_check_errors(ctx, what)) || !d[5]) return rc;
+  const MapArenaBufs &m = ctx->map;
+  const esikf_map_stats &u = ctx->map_last;  // the counters before the deferred tick
+  const long long node_cap = (d[5] & MAP_ERR_NODES) ? map_grown_capacity(m.node_cap, u.nodes, (long long)d[0]) : m.node_cap;
+  const long long pool_cap = (d[5] & MAP_ERR_POOL) ? map_grown_capacity(m.pool_cap, u.pool_points, (long long)d[1]) : m.pool_cap;
+  const long long rec_cap = (d[5] & MAP_ERR_RECS) ? map_grown_capacity(m.rec_cap, u.records, (long long)d[2]) : m.rec_cap;
+  if ((rc = map_grow(ctx, m.hash_cap, node_cap, rec_cap, pool_cap, what))) return rc;
+  map_keys_kernel<<<(n + 255) / 256, 256, 0, st>>>(ctx->arena(), ctx->map_pt.p, n, ctx->map_key_in.p, ctx->map_idx_in.p, ctx->map.hash_cap);
+  ctx->launches++;
+  if ((rc = map_replay_tick(ctx, n, build))) return rc;
+  CK(cudaMemcpyAsync(d, ctx->map_demand.p, sizeof(d), cudaMemcpyDeviceToHost, st));
+  if ((rc = map_check_errors(ctx, what))) return rc;
+  if (d[5]) {  // the grown arena holds used + demand of every short resource: the bound itself would be broken
+    ctx->have_map = false;
+    return fail(ctx, ESIKF_ERR_STATE, "%s: the tick was deferred again after the map grew (flags 0x%x)", what, (unsigned)d[5]);
+  }
+  return ESIKF_OK;
 }
 
 static int map_reserve_tick(esikf_ctx *ctx, int n) {
@@ -601,12 +687,22 @@ static int map_from_scan(esikf_ctx *ctx, const double *state, bool build) {
     CK(cudaMemcpyAsync(ctx->scratch_state.p, state, S_N * sizeof(double), cudaMemcpyHostToDevice, st));
     dev_state = ctx->scratch_state.p;
   }
+  const int32_t *match_plane = build ? nullptr : ctx->normal_plane.p;
+  if (map_hash_short(ctx, n)) {
+    // pv.normal refers to the records of the last LIO run: snapshot it before the copy moves them
+    if (match_plane) {
+      gather_normals_kernel<<<(n + 255) / 256, 256, 0, st>>>(match_plane, ctx->map.recs.p, n, ctx->map_pt_normal.p);
+      ctx->launches++;
+      match_plane = nullptr;
+    }
+    if ((rc = map_grow_hash(ctx, n, build ? "map_device_build" : "map_device_update"))) return rc;
+  }
   MapPointArgs a;
   memset(&a, 0, sizeof(a));
   a.pts = ctx->pts.p, a.pre = ctx->pre.p, a.pre_stride = ctx->pre_stride, a.n = n, a.state = dev_state;
   memcpy(a.extR, ctx->ext.extR, 72), memcpy(a.extT, ctx->ext.extT, 24);
   a.build = build ? 1 : 0, a.dept_err = (float)ctx->map_cfg.dept_err, a.beam_err = (float)ctx->map_cfg.beam_err;
-  a.match_plane = build ? nullptr : ctx->normal_plane.p, a.recs = ctx->map.recs.p, a.pt_normal = ctx->map_pt_normal.p;
+  a.match_plane = match_plane, a.recs = ctx->map.recs.p, a.pt_normal = ctx->map_pt_normal.p;
   a.pt = ctx->map_pt.p, a.pt_slot = ctx->map_key_in.p, a.pt_idx = ctx->map_idx_in.p, a.invalid_slot = ctx->map.hash_cap;
   map_points_kernel<<<(n + 255) / 256, 256, 0, st>>>(ctx->arena(), a);
   ctx->map_pt_n = n, ctx->map_normals_valid = !build;
@@ -630,6 +726,7 @@ int esikf_map_device_update_points(esikf_ctx *ctx, const double *point_w, const 
   // [n][12] = point_w | var: two strided copies
   CK(cudaMemcpy2DAsync(ctx->map_pt.p, MAP_PT_D * sizeof(double), point_w, 3 * sizeof(double), 3 * sizeof(double), n, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpy2DAsync(ctx->map_pt.p + 3, MAP_PT_D * sizeof(double), var, 9 * sizeof(double), 9 * sizeof(double), n, cudaMemcpyHostToDevice, st));
+  if (map_hash_short(ctx, n) && (rc = map_grow_hash(ctx, n, "map_device_update"))) return rc;
   map_keys_kernel<<<(n + 255) / 256, 256, 0, st>>>(ctx->arena(), ctx->map_pt.p, n, ctx->map_key_in.p, ctx->map_idx_in.p, ctx->map.hash_cap);
   ctx->launches++;
   ctx->map_normals_valid = false;
@@ -660,6 +757,15 @@ int esikf_map_device_slide(esikf_ctx *ctx, const int64_t key_min[3], const int64
   std::swap(ctx->map, ctx->spare);
   ctx->map_normals_valid = false;  // record positions of the last update are gone
   return map_check_errors(ctx, "map_device_slide");
+}
+
+int esikf_map_device_capacity(esikf_ctx *ctx, esikf_map_cfg *out) {
+  if (!ctx || !out) return fail(ctx, ESIKF_ERR_ARG, "map_device_capacity: bad argument");
+  if (!ctx->dev_map) return fail(ctx, ESIKF_ERR_STATE, "map_device_capacity before esikf_map_device_init");
+  out->root_capacity = ctx->map.hash_cap / 2, out->node_capacity = ctx->map.node_cap;
+  out->record_capacity = ctx->map.rec_cap, out->point_capacity = ctx->map.pool_cap;
+  out->grow = ctx->map_cfg.grow;
+  return ESIKF_OK;
 }
 
 int esikf_map_device_stats(esikf_ctx *ctx, esikf_map_stats *out) {

@@ -6,6 +6,8 @@
 //                         also snapshots the normal of every point's matched plane (pv.normal) before records may move
 //   cub radix sort      : (slot, scan index) pairs by slot — stable, so every root sees its points in scan order
 //   map_heads_kernel    : one entry per touched root {slot, first sorted position, count}
+//   map_demand_kernel   : (capacity growth on) one warp per touched root sums map_root_demand and raises the defer word when
+//                         the tick might not fit the arena
 //   map_replay_kernel   : one warp per touched root, work handed out through an atomic counter (roots differ a lot in work)
 //   map_download_kernel : the map in esikf_map_upload's flat form (tests, visualisation, serialisation)
 #include <cub/device/device_radix_sort.cuh>
@@ -166,9 +168,42 @@ __global__ void __launch_bounds__(256) map_heads_kernel(const unsigned int *__re
   touched[t].slot = s, touched[t].start = j, touched[t].count = lo - j;
 }
 
-__global__ void __launch_bounds__(128) map_replay_kernel(const MapArena A, const MapTouched *__restrict__ touched, int *work, const unsigned int *__restrict__ order,
-                                                         const double *__restrict__ pt, int build) {
+// Capacity growth: demand[0..2] the summed map_root_demand (nodes, pool points, records), [3] next root to hand out, [4] warps
+// done, [5] the defer word: the MAP_ERR_NODES / _POOL / _RECS bits of every resource whose free space is short of the sum.
+// The last warp to finish compares, so the replay that follows only reads one word.
+enum { MAP_DEMAND_WORDS = 8 };
+__global__ void __launch_bounds__(128) map_demand_kernel(const MapArena A, const MapTouched *__restrict__ touched, const int *work, unsigned long long *demand, int build) {
   const WarpCoop co;
+  const int n_touched = *reinterpret_cast<const volatile int *>(&work[0]);
+  for (;;) {
+    int t = 0;
+    if (co.lane() == 0) t = (int)atomicAdd(&demand[3], 1ull);
+    t = co.bcast(t);
+    if (t >= n_touched) break;
+    if (co.lane() == 0) {
+      const MapTouched w = touched[t];
+      const MapDemand d = map_root_demand(A, (int)w.slot, w.count, build != 0);
+      atomicAdd(&demand[0], (unsigned long long)d.nodes), atomicAdd(&demand[1], (unsigned long long)d.pool), atomicAdd(&demand[2], (unsigned long long)d.recs);
+    }
+  }
+  if (co.lane() != 0) return;
+  __threadfence();
+  const unsigned long long warps = (unsigned long long)gridDim.x * (blockDim.x / 32);
+  if (atomicAdd(&demand[4], 1ull) != warps - 1) return;
+  __threadfence();
+  const volatile unsigned long long *v = demand;
+  int defer = 0;
+  if ((long long)A.counters[0] + (long long)v[0] > (long long)A.node_cap) defer |= MAP_ERR_NODES;
+  if ((long long)A.counters64[0] + (long long)v[1] > A.pool_cap) defer |= MAP_ERR_POOL;
+  if ((long long)A.counters[1] + (long long)v[2] > (long long)A.rec_cap) defer |= MAP_ERR_RECS;
+  demand[5] = (unsigned long long)defer;
+}
+
+// defer (growth on): the word map_demand_kernel set; when it is non-zero the tick does not fit and nothing is touched
+__global__ void __launch_bounds__(128) map_replay_kernel(const MapArena A, const MapTouched *__restrict__ touched, int *work, const unsigned int *__restrict__ order,
+                                                         const double *__restrict__ pt, int build, const unsigned long long *defer) {
+  const WarpCoop co;
+  if (defer && *reinterpret_cast<const volatile unsigned long long *>(defer)) return;
   const int n_touched = *reinterpret_cast<volatile int *>(&work[0]);
   for (;;) {
     int t = 0;

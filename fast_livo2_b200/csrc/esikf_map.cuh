@@ -604,6 +604,76 @@ MAP_HD void map_replay_root(const MapArena &A, const C &co, int slot, const unsi
   map_emit_root(A, co, slot);
 }
 
+// ---- Capacity growth (esikf_map_cfg.grow): what map_replay_root can consume, known before any root is touched.
+//
+// Upper bounds on the nodes, pool points and record slots one map_replay_root(slot, k points, build) can hand out, from the
+// root's subtree at tick start. The derivation, with ML = cfg.max_layer:
+//  * Point copies. Only map_cut moves stored points, and it runs only on a node with init_octo == 0 (map_init_octo_tree) or
+//    on a child it just filled. An init_octo == 0 node has no children (children are made by a cut, which sets init_octo,
+//    or by a descent, which needs init_octo). So every copy moves a point one layer down into a fresh child, and the list it
+//    left is freed: a point lives in one list at a time and enters each layer at most once. The points that can move are
+//    the k new ones and S, those stored in init_octo == 0 lists at tick start. The build form pushes into the root whatever
+//    its state and may cut every list of the subtree: there S counts every stored point.
+//  * Nodes. A node is made only when a point enters a layer below 0 (map_child_for, by a descent or a copy), plus the root
+//    when it is new: nodes <= [new root] + ML (k + S).
+//  * Pushes. A new point is pushed once at the node it stops at, then copied at most ML times; a stored point only copied:
+//    pushes <= k (ML + 1) + S ML.
+//  * Pool. map_list_push grows a list from capacity c to max(8 or 2c, reserve), only when it is full, and the reserve (a
+//    cut's count for one fresh child + 1, or the build's k + 1) never exceeds the list's peak size P + 1. The capacities a
+//    list takes in one tick double at least, and all but the last equal its size at a later growth (<= P): they sum to
+//    <= 2P, the last is <= max(8, 2P, P + 1). So one list takes <= 4P + 8 points, P <= its size at tick start + its pushes.
+//    Lists that can take a push: the init_octo == 0 nodes, the plane / last-layer nodes still updating (every node in the
+//    build form), and the new ones. Summed: pool <= 4 (U + pushes) + 8 min(pushes, L + new nodes), U / L the stored points
+//    / the number of those pushable lists at tick start.
+//  * Records. Candidates are nodes, so a root ends the tick with at most T = (nodes now) + (new nodes) of them.
+//    map_emit_root relocates at most once per replay, only when the count exceeds the block it has, into the power-of-two
+//    block of the count (1 for one candidate, else 8 or more): records <= 0 if T fits the block, else that block of T.
+// The bound only sizes headroom; it may be loose but is never exceeded (tests/test_map_growth_host.py checks it root by root).
+struct MapDemand {
+  long long nodes, pool, recs;
+};
+MAP_HD MapDemand map_root_demand(const MapArena &A, int slot, int k, bool build) {
+  const long long ML = A.cfg.max_layer;
+  const int root = A.slot_root[slot];
+  long long S = 0, U = 0, L = 0, have = 0;
+  if (root >= 0) {
+    int stack[MAP_STACK];  // every node, 8 children a layer, ML <= 7: at most 8 ML + 1 entries
+    int sp = 0;
+    stack[sp++] = root;
+    while (sp > 0) {
+      const MapNode &n = A.nodes[stack[--sp]];
+      have++;
+      const bool init0 = build || !n.init_octo;
+      const bool pushable = init0 || (n.update_enable && (n.is_plane || n.layer >= A.cfg.max_layer));
+      if (init0) S += n.list_size;
+      if (pushable) U += n.list_size, L++;
+      for (int l = 0; l < 8; l++)
+        if (n.children[l] >= 0 && sp < MAP_STACK) stack[sp++] = n.children[l];
+    }
+  }
+  MapDemand d;
+  d.nodes = (root < 0 ? 1 : 0) + ML * (k + S);
+  const long long pushes = (long long)k * (ML + 1) + S * ML;
+  const long long lists = L + d.nodes;
+  d.pool = 4 * (U + pushes) + 8 * (pushes < lists ? pushes : lists);
+  const long long T = have + d.nodes;
+  long long blk = T <= 1 ? 1 : 8;
+  while (blk < T) blk *= 2;
+  d.recs = (root >= 0 && T <= A.slot_cap[slot]) ? 0 : blk;
+  return d;
+}
+
+// The capacity a short resource grows to: twice the old one, or what the tick needs if that is more. The host API and the
+// test harness both size their arenas with it.
+MAP_HD long long map_grown_capacity(long long cap, long long used, long long demand) { return 2 * cap > used + demand ? 2 * cap : used + demand; }
+// Hash slots for `roots` roots plus up to n new ones at a load of at most 1/2 (esikf_map_device_init's sizing): a power of two.
+MAP_HD long long map_grown_hash(long long cap, long long roots, long long n) {
+  const long long want = map_grown_capacity(cap, 2 * roots, 2 * n);
+  long long c = cap;
+  while (c < want) c *= 2;
+  return c;
+}
+
 // ---- mapSliding / clearMemOutOfMap (:924-971) as a copy into a fresh arena: the roots inside the box are re-inserted with their
 // whole sub-trees, point lists sized to their content and a tight record block — which also reclaims the dead record
 // blocks and the list space earlier growth left behind. S is read-only.

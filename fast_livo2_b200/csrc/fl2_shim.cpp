@@ -169,6 +169,7 @@ void VoxelMapManager::EnableDeviceMap() {
   const std::vector<int> &lin = config_setting_.layer_init_num_;
   for (int k = 0; k < 8; k++) m.layer_init_num[k] = lin.empty() ? 5 : lin[k < (int)lin.size() ? k : (int)lin.size() - 1];
   m.root_capacity = config_setting_.device_root_capacity_;
+  m.grow = config_setting_.device_map_grow_ ? 1 : 0;
   if ((last_status_ = esikf_map_device_init(ctx_, &m)) != 0) {
     last_error_ = esikf_last_error(ctx_);
     return;

@@ -101,7 +101,8 @@ struct VoxelMapConfig {
   double planner_threshold_ = 0.0025;  // lio/min_eigen_value
   int max_points_num_ = 50;            // lio/max_points_num
   std::vector<int> layer_init_num_{5, 5, 5, 5, 5};
-  long long device_root_capacity_ = 0;  // 0: esikf_map_device_init's default (2^20 root voxels)
+  long long device_root_capacity_ = 0;  // 0: esikf_map_device_init's default (2^20 root voxels); the starting size when growing
+  bool device_map_grow_ = false;        // the device map grows when a tick would exceed its capacities (esikf_map_cfg.grow)
   bool map_sliding_en = false;          // local_map/map_sliding_en
   int half_map_size = 100;              // local_map/half_map_size
   double sliding_thresh = 8.0;          // local_map/sliding_thresh

@@ -175,10 +175,14 @@ typedef struct esikf_map_cfg {
   int32_t max_layer;          /* lio/max_layer (<= 7) */
   int32_t max_points_num;     /* lio/max_points_num */
   int32_t layer_init_num[8];  /* lio/layer_init_num, entries 0..max_layer are used */
-  int32_t pad;
-  /* capacities, fixed at init (nothing is allocated per tick); 0 = default derived from root_capacity (default 2^20):
-   * nodes 4 x, plane records 4 x, stored points 64 x the roots. Exceeding one is reported by the update call
-   * (ESIKF_ERR_STATE, flags in esikf_map_stats.errors) and invalidates the map. */
+  /* 0: the capacities below are fixed. 1: they are starting sizes, and a build / update that would exceed one grows the map
+   * instead (the arena is copied into a larger one, then the tick is applied; the map is the same as with large fixed
+   * capacities). A failed allocation there returns ESIKF_ERR_CUDA and invalidates the map. */
+  int32_t grow;
+  /* capacities; 0 = default derived from root_capacity (default 2^20): nodes 4 x, plane records 4 x, stored points 64 x the
+   * roots. With grow == 0 they are fixed at init (nothing is allocated per tick), and exceeding one is reported by the
+   * update call (ESIKF_ERR_STATE, flags in esikf_map_stats.errors) and invalidates the map. With grow == 1 they are where
+   * the map starts; esikf_map_device_capacity reports where it is. Key-range and octree-depth errors are errors either way. */
   int64_t root_capacity, node_capacity, record_capacity, point_capacity;
 } esikf_map_cfg;
 typedef struct esikf_map_stats {
@@ -205,6 +209,9 @@ int esikf_map_device_update_points(esikf_ctx *ctx, const double *point_w, const 
  * update are void afterwards (esikf_lio_fetch normals / ids refer to the old records): call it between ticks. */
 int esikf_map_device_slide(esikf_ctx *ctx, const int64_t key_min[3], const int64_t key_max[3]);
 int esikf_map_device_stats(esikf_ctx *ctx, esikf_map_stats *out);
+/* The current capacities and grow flag of the device map in esikf_map_cfg's terms (root_capacity = hash slots / 2, the
+ * inverse of init's sizing); the other fields of `out` are left as they are. */
+int esikf_map_device_capacity(esikf_ctx *ctx, esikf_map_cfg *out);
 /* The map in esikf_map_upload's flat form (roots in no particular order). keys == NULL: sizes only. */
 int esikf_map_device_download(esikf_ctx *ctx, int64_t *keys, int32_t *first, int32_t *count, int32_t roots_cap, esikf_plane *planes, int32_t planes_cap,
                               int32_t *n_roots, int32_t *n_planes);
