@@ -87,6 +87,7 @@ def load_library():
     lib.esikf_map_device_capacity.argtypes = [vp, vp]
     lib.esikf_map_device_slide.argtypes = [vp, vp, vp]
     lib.esikf_map_device_download.argtypes = [vp, vp, vp, vp, C.c_int32, vp, C.c_int32, vp, vp]
+    lib.esikf_map_device_export.argtypes = [vp, vp, vp, vp, C.c_int32, vp, C.c_int32, vp, vp]
     lib.esikf_lio_fetch_normals.argtypes = [vp, vp]
     lib.esikf_lio_set_scan.argtypes = [vp, vp, C.c_int32]
     lib.esikf_lio_run.argtypes = [vp, vp, vp, C.POINTER(LioCfgC)]
@@ -136,7 +137,7 @@ class MapStatsC(C.Structure):
 
 EXPORTED_SYMBOLS = [
     "esikf_create", "esikf_destroy", "esikf_last_error", "esikf_stream", "esikf_synchronize", "esikf_host_alloc", "esikf_host_free", "esikf_launch_count", "esikf_set_solve_mode", "esikf_set_loop_mode", "esikf_set_tuning",
-    "esikf_set_extrinsics", "esikf_set_lidar_extrinsics", "esikf_map_upload", "esikf_map_patch", "esikf_map_device_init", "esikf_map_device_build", "esikf_map_device_update", "esikf_map_device_update_points", "esikf_map_device_slide", "esikf_map_device_stats", "esikf_map_device_capacity", "esikf_map_device_download", "esikf_lio_fetch_normals", "esikf_lio_set_scan", "esikf_lio_run", "esikf_lio_fetch",
+    "esikf_set_extrinsics", "esikf_set_lidar_extrinsics", "esikf_map_upload", "esikf_map_patch", "esikf_map_device_init", "esikf_map_device_build", "esikf_map_device_update", "esikf_map_device_update_points", "esikf_map_device_slide", "esikf_map_device_stats", "esikf_map_device_capacity", "esikf_map_device_download", "esikf_map_device_export", "esikf_lio_fetch_normals", "esikf_lio_set_scan", "esikf_lio_run", "esikf_lio_fetch",
     "esikf_lio_update", "esikf_lio_fetch_point_cov", "esikf_vio_set_camera", "esikf_vio_set_image", "esikf_vio_set_patches",
     "esikf_vio_run", "esikf_vio_fetch", "esikf_vio_update", "esikf_vio_get_image_patch", "esikf_vio_set_ref_images",
     "esikf_vio_warp_patches", "esikf_vio_warp_affine", "esikf_vio_set_inverse_refs", "esikf_comm_unique_id", "esikf_comm_init", "esikf_comm_rank", "esikf_shard_range", "esikf_peer_export", "esikf_peer_attach", "esikf_profile_kernel", "esikf_set_kernel_timing", "esikf_get_kernel_timing", "esikf_set_phase_stamps", "esikf_get_phase_stamps",
@@ -279,6 +280,19 @@ class Context:
         self._ck(self.lib.esikf_map_device_download(self.h, keys.ctypes.data, first.ctypes.data, count.ctypes.data, len(first), planes.ctypes.data, len(planes),
                                                     C.byref(nr), C.byref(npl)))
         return dict(keys=keys[:nr.value], first=first[:nr.value], count=count[:nr.value], planes=planes[:npl.value])
+
+    def map_device_export(self):
+        """The subtrees of the roots the last build / update replayed: root r owns nodes[first[r]:first[r] + count[r]]
+        (synthetic.NODE_DTYPE, DFS pre-order, leaves 0..7); roots in hash-slot order."""
+        from .synthetic import NODE_DTYPE
+
+        nr, nn = C.c_int32(0), C.c_int32(0)
+        self._ck(self.lib.esikf_map_device_export(self.h, None, None, None, 0, None, 0, C.byref(nr), C.byref(nn)))
+        keys, first, count = np.zeros((max(nr.value, 1), 3), np.int64), np.zeros(max(nr.value, 1), np.int32), np.zeros(max(nr.value, 1), np.int32)
+        nodes = np.zeros(max(nn.value, 1), NODE_DTYPE)
+        self._ck(self.lib.esikf_map_device_export(self.h, keys.ctypes.data, first.ctypes.data, count.ctypes.data, len(first), nodes.ctypes.data, len(nodes),
+                                                  C.byref(nr), C.byref(nn)))
+        return dict(keys=keys[:nr.value], first=first[:nr.value], count=count[:nr.value], nodes=nodes[:nn.value])
 
     def lio_fetch_normals(self):
         out = np.zeros((self.n_pts, 3), np.float64)

@@ -168,6 +168,13 @@ struct esikf_ctx {
   bool map_normals_valid = false;
   int map_hash_bits = 0;
   esikf_map_stats map_last{};
+  // esikf_map_device_export: points of the last applied tick (its touched list is map_touched, its sorted positions 0..n),
+  // -1 when there is no tick to export (after init, a slide or a failed build / update)
+  int map_export_points = -1;
+  DevBuf<unsigned long long> map_exp_packed;
+  DevBuf<long long> map_exp_keys;
+  DevBuf<int32_t> map_exp_first, map_exp_count, map_exp_rows;
+  DevBuf<esikf_map_node> map_exp_nodes;
 
   // LIO
   DevBuf<float> pts;
@@ -555,6 +562,7 @@ int esikf_map_device_init(esikf_ctx *ctx, const esikf_map_cfg *cfg) {
   ctx->n_planes = 0, ctx->n_roots = 0;
   ctx->dev_map = true, ctx->have_map = true;  // an empty map is a valid map (nothing matches)
   ctx->map_normals_valid = false;
+  ctx->map_export_points = -1;
   memset(&ctx->map_last, 0, sizeof(ctx->map_last));
   return ESIKF_OK;
 }
@@ -669,15 +677,23 @@ static int map_reserve_tick(esikf_ctx *ctx, int n) {
   return ESIKF_OK;
 }
 
+// map_apply_points and, when it succeeded, the tick esikf_map_device_export exports
+static int map_apply_exported(esikf_ctx *ctx, int n, bool build) {
+  const int rc = map_apply_points(ctx, n, build);
+  if (!rc) ctx->map_export_points = n;
+  return rc;
+}
+
 static int map_from_scan(esikf_ctx *ctx, const double *state, bool build) {
   if (!ctx) return ESIKF_ERR_ARG;
+  ctx->map_export_points = -1;
   if (!ctx->dev_map) return fail(ctx, ESIKF_ERR_STATE, "map_device_%s before esikf_map_device_init", build ? "build" : "update");
   if (!ctx->have_ext) return fail(ctx, ESIKF_ERR_STATE, "map_device_%s before set_extrinsics", build ? "build" : "update");
   if (!build && ctx->scan_fresh) return fail(ctx, ESIKF_ERR_STATE, "map_device_update: the resident scan has not been through esikf_lio_run yet");
   if (build && ctx->map_last.roots > 0) return fail(ctx, ESIKF_ERR_STATE, "map_device_build needs an empty map (esikf_map_device_init resets it)");
   CK(cudaSetDevice(ctx->device));
   const int n = ctx->n_pts;
-  if (n == 0) return ESIKF_OK;
+  if (n == 0) return ctx->map_export_points = 0, ESIKF_OK;
   int rc = map_reserve_tick(ctx, n);
   if (rc) return rc;
   cudaStream_t st = ctx->stream;
@@ -706,7 +722,7 @@ static int map_from_scan(esikf_ctx *ctx, const double *state, bool build) {
   a.pt = ctx->map_pt.p, a.pt_slot = ctx->map_key_in.p, a.pt_idx = ctx->map_idx_in.p, a.invalid_slot = ctx->map.hash_cap;
   map_points_kernel<<<(n + 255) / 256, 256, 0, st>>>(ctx->arena(), a);
   ctx->map_pt_n = n, ctx->map_normals_valid = !build;
-  return map_apply_points(ctx, n, build);
+  return map_apply_exported(ctx, n, build);
 }
 
 int esikf_map_device_build(esikf_ctx *ctx, const double *state) {
@@ -716,9 +732,10 @@ int esikf_map_device_build(esikf_ctx *ctx, const double *state) {
 int esikf_map_device_update(esikf_ctx *ctx, const double *state) { return map_from_scan(ctx, state, false); }
 
 int esikf_map_device_update_points(esikf_ctx *ctx, const double *point_w, const double *var, int32_t n) {
+  if (ctx) ctx->map_export_points = -1;
   if (!ctx || n < 0 || (n > 0 && (!point_w || !var))) return fail(ctx, ESIKF_ERR_ARG, "map_device_update_points: bad argument");
   if (!ctx->dev_map) return fail(ctx, ESIKF_ERR_STATE, "map_device_update_points before esikf_map_device_init");
-  if (n == 0) return ESIKF_OK;
+  if (n == 0) return ctx->map_export_points = 0, ESIKF_OK;
   CK(cudaSetDevice(ctx->device));
   int rc = map_reserve_tick(ctx, n);
   if (rc) return rc;
@@ -730,12 +747,13 @@ int esikf_map_device_update_points(esikf_ctx *ctx, const double *point_w, const 
   map_keys_kernel<<<(n + 255) / 256, 256, 0, st>>>(ctx->arena(), ctx->map_pt.p, n, ctx->map_key_in.p, ctx->map_idx_in.p, ctx->map.hash_cap);
   ctx->launches++;
   ctx->map_normals_valid = false;
-  return map_apply_points(ctx, n, false);
+  return map_apply_exported(ctx, n, false);
 }
 
 // mapSliding / clearMemOutOfMap (src/voxel_map.cpp:924-971)
 int esikf_map_device_slide(esikf_ctx *ctx, const int64_t key_min[3], const int64_t key_max[3]) {
   if (!ctx) return ESIKF_ERR_ARG;
+  ctx->map_export_points = -1;
   if (!ctx->dev_map) return fail(ctx, ESIKF_ERR_STATE, "map_device_slide before esikf_map_device_init");
   CK(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
@@ -808,6 +826,53 @@ int esikf_map_device_download(esikf_ctx *ctx, int64_t *keys, int32_t *first, int
   CK(cudaMemcpy(first, d_first.p, (size_t)out[0] * sizeof(int32_t), cudaMemcpyDeviceToHost));
   CK(cudaMemcpy(count, d_count.p, (size_t)out[0] * sizeof(int32_t), cudaMemcpyDeviceToHost));
   if (out[1]) CK(cudaMemcpy(planes, d_planes.p, (size_t)out[1] * sizeof(esikf_plane), cudaMemcpyDeviceToHost));
+  return ESIKF_OK;
+}
+
+int esikf_map_device_export(esikf_ctx *ctx, int64_t *keys, int32_t *first, int32_t *count, int32_t roots_cap, esikf_map_node *nodes, int32_t nodes_cap, int32_t *n_roots,
+                            int32_t *n_nodes) {
+  if (!ctx || !n_roots || !n_nodes) return fail(ctx, ESIKF_ERR_ARG, "map_device_export: bad argument");
+  if (!ctx->dev_map) return fail(ctx, ESIKF_ERR_STATE, "map_device_export before esikf_map_device_init");
+  if (ctx->map_export_points < 0)
+    return fail(ctx, ESIKF_ERR_STATE, "map_device_export: no build / update to export (the map was initialised or slid since, or the last one failed)");
+  *n_roots = 0, *n_nodes = 0;
+  const int n = ctx->map_export_points;
+  if (n == 0) return ESIKF_OK;
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const bool fill = keys && first && count && nodes && roots_cap > 0;
+  // position n stays 0: the exclusive scan leaves the totals there
+  CK(ctx->map_exp_packed.reserve(2 * ((size_t)n + 1)));
+  unsigned long long *packed = ctx->map_exp_packed.p, *offs = packed + n + 1;
+  CK(cudaMemsetAsync(packed, 0, ((size_t)n + 1) * sizeof(unsigned long long), st));
+  map_export_count_kernel<<<ctx->sm_count * 4, 128, 0, st>>>(ctx->arena(), ctx->map_touched.p, ctx->map_work.p, packed);
+  size_t tmp_bytes = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, packed, offs, n + 1, st);
+  CK(ctx->map_sort_tmp.reserve(tmp_bytes + 16));
+  CK(cub::DeviceScan::ExclusiveSum(ctx->map_sort_tmp.p, tmp_bytes, packed, offs, n + 1, st));
+  ctx->launches += 2;
+  unsigned long long total = 0;
+  CK(cudaMemcpyAsync(&total, offs + n, sizeof(total), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const int nr = (int)(total >> 32), nn = (int)(total & 0xffffffffull);
+  *n_roots = nr, *n_nodes = nn;
+  if (!fill) return ESIKF_OK;
+  if (nr > roots_cap || nn > nodes_cap)
+    return fail(ctx, ESIKF_ERR_ARG, "map_device_export: %d roots / %d nodes do not fit the buffers (%d / %d)", nr, nn, roots_cap, nodes_cap);
+  CK(ctx->map_exp_keys.reserve((size_t)nr * 3));
+  CK(ctx->map_exp_first.reserve(nr));
+  CK(ctx->map_exp_count.reserve(nr));
+  CK(ctx->map_exp_nodes.reserve(nn));
+  CK(ctx->map_exp_rows.reserve(nn));
+  map_export_kernel<<<ctx->sm_count * 4, 128, 0, st>>>(ctx->arena(), ctx->map_touched.p, ctx->map_work.p, offs, ctx->map_exp_keys.p, ctx->map_exp_first.p, ctx->map_exp_count.p,
+                                                      ctx->map_exp_nodes.p, ctx->map_exp_rows.p);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(keys, ctx->map_exp_keys.p, (size_t)nr * 3 * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(first, ctx->map_exp_first.p, (size_t)nr * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(count, ctx->map_exp_count.p, (size_t)nr * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(nodes, ctx->map_exp_nodes.p, (size_t)nn * sizeof(esikf_map_node), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
   return ESIKF_OK;
 }
 

@@ -10,7 +10,9 @@
 //                         the tick might not fit the arena
 //   map_replay_kernel   : one warp per touched root, work handed out through an atomic counter (roots differ a lot in work)
 //   map_download_kernel : the map in esikf_map_upload's flat form (tests, visualisation, serialisation)
+//   map_export_*_kernel : the subtrees of the roots the last replay touched, node by node (a host mirror of the map)
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 
 #include "esikf_map.cuh"
 
@@ -230,6 +232,35 @@ __global__ void __launch_bounds__(256) map_download_kernel(const MapArena A, lon
   keys[3 * (size_t)r + 2] = (long long)(k & (ESIKF_KEY_RANGE - 1)) - ESIKF_KEY_BIAS;
   first[r] = off, count[r] = c;
   for (int j = 0; j < c; j++) planes[off + j] = A.planes[A.slots[s].first + j];
+}
+
+// Export of the touched roots (esikf_map_device_export), one warp per root, in two passes over the touched list of the last
+// replay. The count pass writes (1 << 32 | subtree size) at the root's first position in the slot-sorted points (every other
+// position holds 0); an exclusive scan over those positions turns it into (root index << 32 | first row), so the roots come
+// out in slot order whatever order map_heads_kernel listed them in. The write pass lays out the rows.
+__global__ void __launch_bounds__(128) map_export_count_kernel(const MapArena A, const MapTouched *__restrict__ touched, const int *work, unsigned long long *packed) {
+  const WarpCoop co;
+  const int n_touched = work[0], warps = gridDim.x * (blockDim.x / 32);
+  for (int t = (blockIdx.x * blockDim.x + threadIdx.x) / 32; t < n_touched; t += warps) {
+    const MapTouched w = touched[t];
+    const int c = map_export_root(A, co, (int)w.slot, nullptr, nullptr);
+    if (co.lane() == 0) packed[w.start] = (1ull << 32) | (unsigned)c;
+  }
+}
+__global__ void __launch_bounds__(128) map_export_kernel(const MapArena A, const MapTouched *__restrict__ touched, const int *work, const unsigned long long *__restrict__ offs,
+                                                         long long *keys, int32_t *first, int32_t *count, esikf_map_node *nodes, int *rows) {
+  const WarpCoop co;
+  const int n_touched = work[0], warps = gridDim.x * (blockDim.x / 32);
+  for (int t = (blockIdx.x * blockDim.x + threadIdx.x) / 32; t < n_touched; t += warps) {
+    const MapTouched w = touched[t];
+    const unsigned long long o = offs[w.start];
+    const int r = (int)(o >> 32), f = (int)(o & 0xffffffffull);
+    const int c = map_export_root(A, co, (int)w.slot, nodes + f, rows + f);
+    if (co.lane() == 0) {
+      for (int q = 0; q < 3; q++) keys[3 * (size_t)r + q] = nodes[f].key[q];
+      first[r] = f, count[r] = c;
+    }
+  }
 }
 
 // mapSliding: list the occupied slots inside the box, then one warp per surviving root copies it into the fresh arena

@@ -604,6 +604,51 @@ MAP_HD void map_replay_root(const MapArena &A, const C &co, int slot, const unsi
   map_emit_root(A, co, slot);
 }
 
+// ---- Export of one root's subtree for a host mirror (esikf_map_device_export): one esikf_map_node a node, in DFS pre-order
+// with leaves 0..7 (the order of the node dumps). Lane 0 walks the tree and lays out the rows (rows[r] = node of row r), then
+// the lanes fill the records. out == nullptr: the subtree size only. A pure read of the arena.
+MAP_HD void map_export_fields(const MapNode &n, esikf_map_node &o) {
+  for (int k = 0; k < 3; k++) o.voxel_center[k] = n.center[k], o.center[k] = n.pc[k], o.normal[k] = n.pn[k];
+  o.quater_length = n.quarter;
+  o.init_octo = n.init_octo, o.octo_state = n.octo_state, o.update_enable = n.update_enable, o.is_plane = n.is_plane;
+  o.new_points = n.new_points, o.points_size = n.points_size, o.temp_points = n.list_size, o.pad_ = 0;
+  for (int k = 0; k < 21; k++) o.plane_var[k] = n.plane_var[k];
+  o.d = n.d, o.radius = n.radius;
+}
+template <class C>
+MAP_HD int map_export_root(const MapArena &A, const C &co, int slot, esikf_map_node *out, int *rows) {
+  int count = 0;
+  if (co.lane() == 0) {
+    const unsigned long long k = A.slots[slot].key;
+    const long long key[3] = {(long long)(k >> 42) - ESIKF_KEY_BIAS, (long long)((k >> 21) & (ESIKF_KEY_RANGE - 1)) - ESIKF_KEY_BIAS,
+                              (long long)(k & (ESIKF_KEY_RANGE - 1)) - ESIKF_KEY_BIAS};
+    // (node, path, parent row, leaf) entries; a pre-order walk holds at most 7 siblings a layer plus one: < MAP_STACK for ML <= 7
+    int st_node[MAP_STACK], st_path[MAP_STACK], st_parent[MAP_STACK], st_leaf[MAP_STACK];
+    int sp = 0;
+    st_node[sp] = A.slot_root[slot], st_path[sp] = 0, st_parent[sp] = -1, st_leaf[sp] = -1, sp++;
+    while (sp > 0) {
+      --sp;
+      const int id = st_node[sp];
+      const MapNode &n = A.nodes[id];
+      if (out) {
+        esikf_map_node &o = out[count];
+        for (int q = 0; q < 3; q++) o.key[q] = key[q];
+        o.layer = n.layer, o.path = st_path[sp], o.parent = st_parent[sp], o.leaf = st_leaf[sp];
+        rows[count] = id;
+      }
+      const int row = count++, path = st_path[sp];
+      for (int l = 7; l >= 0; l--)  // pushed in reverse: leaf 0 is visited first
+        if (n.children[l] >= 0) st_node[sp] = n.children[l], st_path[sp] = path | (l << (3 * n.layer)), st_parent[sp] = row, st_leaf[sp] = l, sp++;
+    }
+  }
+  count = co.bcast(count);
+  if (out) {
+    co.sync();
+    for (int r = co.lane(); r < count; r += C::N) map_export_fields(A.nodes[rows[r]], out[r]);
+  }
+  return count;
+}
+
 // ---- Capacity growth (esikf_map_cfg.grow): what map_replay_root can consume, known before any root is touched.
 //
 // Upper bounds on the nodes, pool points and record slots one map_replay_root(slot, k points, build) can hand out, from the

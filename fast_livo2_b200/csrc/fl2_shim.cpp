@@ -66,6 +66,80 @@ VoxelOctoTree::~VoxelOctoTree() {
   delete plane_ptr_;
 }
 
+// src/voxel_map.cpp:292-305
+// The node a point falls into: descend while the node is a cut, non-plane node above the last layer and the point's leaf
+// exists. The leaf is chosen by a strict comparison with the node's centre on each axis (x: 4, y: 2, z: 1).
+VoxelOctoTree *VoxelOctoTree::find_correspond(V3D pw) {
+  VoxelOctoTree *node = this;
+  while (node->init_octo_ && !node->plane_ptr_->is_plane_ && node->layer_ < node->max_layer_) {
+    const int leaf = (pw[0] > node->voxel_center_[0]) * 4 + (pw[1] > node->voxel_center_[1]) * 2 + (pw[2] > node->voxel_center_[2]);
+    if (!node->leaves_[leaf]) break;
+    node = node->leaves_[leaf];
+  }
+  return node;
+}
+
+bool ApplyMapExport(VoxelMap &map, const VoxelMapConfig &cfg, const int64_t *keys, const int32_t *first, const int32_t *count, int n_roots, const esikf_map_node *nodes,
+                    int n_nodes, std::string *err) {
+  std::vector<VoxelOctoTree *> at;
+  for (int r = 0; r < n_roots; r++) {
+    const int f = first[r], c = count[r];
+    if (f < 0 || c < 1 || f + c > n_nodes || nodes[f].parent != -1) {
+      if (err) *err = "map export: root " + std::to_string(r) + " has no valid node range";
+      return false;
+    }
+    const VOXEL_LOCATION key(keys[3 * r], keys[3 * r + 1], keys[3 * r + 2]);
+    VoxelOctoTree *&root = map[key];
+    if (!root) root = new VoxelOctoTree, root->plane_ptr_ = new VoxelPlane;
+    at.assign(c, nullptr);
+    for (int j = 0; j < c; j++) {
+      const esikf_map_node &e = nodes[f + j];
+      VoxelOctoTree *t = root;
+      if (j > 0) {
+        if (e.parent < 0 || e.parent >= j || e.leaf < 0 || e.leaf > 7) {
+          if (err) *err = "map export: node " + std::to_string(f + j) + " does not follow its parent in DFS pre-order";
+          return false;
+        }
+        VoxelOctoTree *&leaf = at[e.parent]->leaves_[e.leaf];
+        if (!leaf) leaf = new VoxelOctoTree, leaf->plane_ptr_ = new VoxelPlane;
+        t = leaf;
+      }
+      at[j] = t;
+      t->layer_ = e.layer, t->max_layer_ = cfg.max_layer_;
+      for (int k = 0; k < 3; k++) t->voxel_center_[k] = e.voxel_center[k];
+      t->quater_length_ = e.quater_length;
+      t->init_octo_ = e.init_octo != 0, t->octo_state_ = e.octo_state, t->update_enable_ = e.update_enable != 0;
+      t->new_points_ = e.new_points, t->temp_points_size_ = e.temp_points;
+      VoxelPlane &p = *t->plane_ptr_;
+      for (int k = 0; k < 3; k++) p.center_[k] = e.center[k], p.normal_[k] = e.normal[k];
+      int q = 0;
+      for (int a = 0; a < 6; a++)
+        for (int b = a; b < 6; b++) p.plane_var_[a * 6 + b] = p.plane_var_[b * 6 + a] = e.plane_var[q++];  // symmetric (DESIGN.md §4)
+      p.d_ = e.d, p.radius_ = e.radius, p.points_size_ = e.points_size;
+      p.is_plane_ = e.is_plane != 0, p.is_init_ = e.points_size > 0;
+    }
+  }
+  return true;
+}
+
+void EraseRootsOutside(VoxelMap &map, const int64_t lo[3], const int64_t hi[3]) {
+  for (auto it = map.begin(); it != map.end();) {
+    const VOXEL_LOCATION &loc = it->first;
+    const bool should_remove = loc.x > hi[0] || loc.x < lo[0] || loc.y > hi[1] || loc.y < lo[1] || loc.z > hi[2] || loc.z < lo[2];
+    if (should_remove) {
+      delete it->second;
+      it = map.erase(it);
+    } else {
+      ++it;
+    }
+  }
+}
+
+void ClearVoxelMap(VoxelMap &map) {
+  for (auto &kv : map) delete kv.second;
+  map.clear();
+}
+
 static void flatten_node(const VoxelOctoTree *node, int layer, int max_layer, int path, FlatVoxelMap &out) {
   if (node->plane_ptr_ && node->plane_ptr_->is_plane_) {
     const VoxelPlane &p = *node->plane_ptr_;
@@ -170,11 +244,55 @@ void VoxelMapManager::EnableDeviceMap() {
   for (int k = 0; k < 8; k++) m.layer_init_num[k] = lin.empty() ? 5 : lin[k < (int)lin.size() ? k : (int)lin.size() - 1];
   m.root_capacity = config_setting_.device_root_capacity_;
   m.grow = config_setting_.device_map_grow_ ? 1 : 0;
+  device_map_mirror_ = config_setting_.device_map_mirror_;
+  if (device_map_mirror_) ClearVoxelMap(voxel_map_);  // the mirror starts as empty as the device map
+  mirror_valid_ = false;
   if ((last_status_ = esikf_map_device_init(ctx_, &m)) != 0) {
     last_error_ = esikf_last_error(ctx_);
     return;
   }
   device_map_ = true, map_synced_ = true, device_has_map_ = true;
+  mirror_valid_ = device_map_mirror_;
+}
+
+void VoxelMapManager::InvalidateMirror() {
+  ClearVoxelMap(voxel_map_);
+  mirror_valid_ = false;
+}
+
+// After a device build / update: apply its export to the mirror. An export holds only the roots of one tick, so once a tick
+// is missing (a failed call, export or apply) no later export can complete the mirror: it stays empty and every later call
+// reports so, until EnableDeviceMap() starts a new map that BuildVoxelMap() fills again.
+void VoxelMapManager::UpdateMirror() {
+  if (!device_map_mirror_) return;
+  if (last_status_) return InvalidateMirror();
+  if (!mirror_valid_) {
+    last_status_ = ESIKF_ERR_STATE;
+    last_error_ = "the host mirror of the device map is void since an earlier call failed: EnableDeviceMap() and BuildVoxelMap() rebuild it";
+    return;
+  }
+  // one export call into grow-only pinned buffers sized by the ticks before; a second one only when they are too small
+  int32_t nr = 0, nn = 0;
+  for (int attempt = 0; attempt < 2; attempt++) {
+    int64_t *keys = exp_keys_.get(3 * (size_t)exp_roots_cap_);
+    int32_t *first = exp_first_.get(exp_roots_cap_), *count = exp_count_.get(exp_roots_cap_);
+    esikf_map_node *nodes = exp_nodes_.get(exp_nodes_cap_);
+    if (!keys || !first || !count || !nodes) {
+      last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
+      return InvalidateMirror();
+    }
+    last_status_ = esikf_map_device_export(ctx_, keys, first, count, exp_roots_cap_, nodes, exp_nodes_cap_, &nr, &nn);
+    if (last_status_ == 0 || (nr <= exp_roots_cap_ && nn <= exp_nodes_cap_)) break;
+    exp_roots_cap_ = nr + nr / 4 + 64, exp_nodes_cap_ = nn + nn / 4 + 64;  // too small: grow and export again
+  }
+  if (last_status_) {
+    last_error_ = esikf_last_error(ctx_);
+    return InvalidateMirror();
+  }
+  if (!ApplyMapExport(voxel_map_, config_setting_, exp_keys_.data(), exp_first_.data(), exp_count_.data(), nr, exp_nodes_.data(), nn, &last_error_)) {
+    last_status_ = ESIKF_ERR_STATE;
+    return InvalidateMirror();
+  }
 }
 
 // include/voxel_map.h:231 / src/voxel_map.cpp:532-591 with feats_down_world_ = transformLidar(state_) (LIVMapper.cpp:360)
@@ -195,6 +313,7 @@ void VoxelMapManager::BuildVoxelMap() {
   if ((last_status_ = esikf_set_lidar_extrinsics(ctx_, extR_.m, extT_.v)) == 0 && (last_status_ = esikf_lio_set_scan(ctx_, pts, n)) == 0)
     last_status_ = esikf_map_device_build(ctx_, sbuf);
   if (last_status_) last_error_ = esikf_last_error(ctx_);
+  UpdateMirror();
 }
 
 // LIVMapper.cpp:413-424: pv_list_[i].point_w / .var with the posterior, then UpdateVoxelMap(pv_list_) — on the device
@@ -206,6 +325,7 @@ void VoxelMapManager::UpdateVoxelMap() {
   double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
   state_.pack(sbuf);  // _state == voxelmap_manager->state_ at this point of the tick (LIVMapper.cpp:371); 3 kB
   if ((last_status_ = esikf_map_device_update(ctx_, sbuf)) != 0) last_error_ = esikf_last_error(ctx_);
+  UpdateMirror();
 }
 
 // src/voxel_map.cpp:924-948: nothing until the sensor moved sliding_thresh, then roots further than half_map_size voxels go
@@ -225,6 +345,16 @@ void VoxelMapManager::mapSliding() {
     lo[j] = (int64_t)loc - config_setting_.half_map_size, hi[j] = (int64_t)loc + config_setting_.half_map_size;
   }
   if ((last_status_ = esikf_map_device_slide(ctx_, lo, hi)) != 0) last_error_ = esikf_last_error(ctx_);
+  if (device_map_mirror_) {
+    if (last_status_) {
+      InvalidateMirror();
+    } else if (!mirror_valid_) {
+      last_status_ = ESIKF_ERR_STATE;
+      last_error_ = "the host mirror of the device map is void since an earlier call failed: EnableDeviceMap() and BuildVoxelMap() rebuild it";
+    } else {
+      EraseRootsOutside(voxel_map_, lo, hi);
+    }
+  }
 }
 
 // include/voxel_map.h:232 / src/voxel_map.cpp:609-641
@@ -245,6 +375,7 @@ void VoxelMapManager::UpdateVoxelMap(const std::vector<pointWithVar> &input_poin
     memcpy(var + 9 * i, input_points[i].var.m, 72);
   }
   if ((last_status_ = esikf_map_device_update_points(ctx_, pw, var, (int32_t)n)) != 0) last_error_ = esikf_last_error(ctx_);
+  UpdateMirror();
 }
 
 // include/voxel_map.h:229 / src/voxel_map.cpp:338-511
@@ -854,5 +985,110 @@ long long fl2_shim_session_manager_ns(void *h) {
 }
 
 void fl2_shim_session_destroy(void *h) { delete static_cast<ShimSession *>(h); }
+
+// ---- the host mirror of a device map (VoxelMapConfig::device_map_mirror_). A mirror handle is a session without managers:
+// the apply code runs on the CPU there. The dump / flatten / find hooks take either kind of handle.
+void *fl2_shim_mirror_create(double voxel_size, int max_layer) {
+  ShimSession *s = new ShimSession;
+  s->cfg.max_voxel_size_ = voxel_size, s->cfg.max_layer_ = max_layer;
+  return s;
+}
+int fl2_shim_mirror_apply(void *h, const int64_t *keys, const int32_t *first, const int32_t *count, int n_roots, const esikf_map_node *nodes, int n_nodes) {
+  ShimSession *s = static_cast<ShimSession *>(h);
+  if (!s) return ESIKF_ERR_ARG;
+  return ApplyMapExport(s->map, s->cfg, keys, first, count, n_roots, nodes, n_nodes, nullptr) ? 0 : ESIKF_ERR_ARG;
+}
+void fl2_shim_mirror_erase(void *h, const int64_t *lo, const int64_t *hi) { EraseRootsOutside(static_cast<ShimSession *>(h)->map, lo, hi); }
+// The mirror's nodes as oracle_bind.NODE_COLS rows (DFS pre-order, leaves 0..7, roots in map order). Returns the number of
+// nodes; rows beyond cap are counted, not written.
+static void mirror_dump_node(const VoxelOctoTree *t, int64_t path, const VOXEL_LOCATION &key, int64_t *out, int cap, int *n) {
+  if (*n < cap) {
+    int64_t *r = out + (size_t)(*n) * 12;
+    r[0] = key.x, r[1] = key.y, r[2] = key.z, r[3] = t->layer_, r[4] = path;
+    r[5] = t->init_octo_, r[6] = t->octo_state_, r[7] = t->update_enable_, r[8] = t->plane_ptr_->is_plane_;
+    r[9] = t->new_points_, r[10] = t->temp_points_size_, r[11] = t->plane_ptr_->points_size_;
+  }
+  (*n)++;
+  for (int l = 0; l < 8; l++)
+    if (t->leaves_[l]) mirror_dump_node(t->leaves_[l], path | ((int64_t)l << (3 * t->layer_)), key, out, cap, n);
+}
+int fl2_shim_mirror_dump(void *h, int64_t *out, int cap) {
+  int n = 0;
+  for (const auto &kv : static_cast<ShimSession *>(h)->map) mirror_dump_node(kv.second, 0, kv.first, out, cap, &n);
+  return n;
+}
+// FlattenVoxelMap of the mirror, two calls: planes == NULL returns the sizes
+int fl2_shim_mirror_flatten(void *h, int *n_roots, int *n_planes, int64_t *keys, int32_t *first, int32_t *count, esikf_plane *planes) {
+  ShimSession *s = static_cast<ShimSession *>(h);
+  FlatVoxelMap flat;
+  std::string err;
+  if (!FlattenVoxelMap(s->map, s->cfg, flat, &err)) return ESIKF_ERR_ARG;
+  *n_roots = (int)flat.first.size(), *n_planes = (int)flat.planes.size();
+  if (planes) {
+    memcpy(keys, flat.keys.data(), flat.keys.size() * sizeof(int64_t));
+    memcpy(first, flat.first.data(), flat.first.size() * sizeof(int32_t));
+    memcpy(count, flat.count.data(), flat.count.size() * sizeof(int32_t));
+    memcpy(planes, flat.planes.data(), flat.planes.size() * sizeof(esikf_plane));
+  }
+  return 0;
+}
+// updateReferencePatch's lookup (src/vio.cpp:983-993) per point: the root voxel by the float quotient (with the map's voxel
+// size), then find_correspond. out: n x 4 = found, layer, path, is_plane of the node it returns.
+void fl2_shim_mirror_find(void *h, const double *pts, int n, int64_t *out) {
+  ShimSession *s = static_cast<ShimSession *>(h);
+  for (int i = 0; i < n; i++) {
+    const double *p = pts + 3 * (size_t)i;
+    float loc_xyz[3];
+    for (int j = 0; j < 3; j++) {
+      loc_xyz[j] = p[j] / s->cfg.max_voxel_size_;
+      if (loc_xyz[j] < 0) loc_xyz[j] -= 1.0;
+    }
+    int64_t *o = out + 4 * (size_t)i;
+    o[0] = o[1] = o[2] = o[3] = 0;
+    auto it = s->map.find(VOXEL_LOCATION((int64_t)loc_xyz[0], (int64_t)loc_xyz[1], (int64_t)loc_xyz[2]));
+    if (it == s->map.end()) continue;
+    V3D pw;
+    for (int k = 0; k < 3; k++) pw[k] = p[k];
+    const VoxelOctoTree *t = it->second->find_correspond(pw);
+    int64_t path = 0;  // the leaves find_correspond took (it follows them again)
+    for (const VoxelOctoTree *u = it->second; u != t;) {
+      const int l = 4 * (pw[0] > u->voxel_center_[0]) + 2 * (pw[1] > u->voxel_center_[1]) + (pw[2] > u->voxel_center_[2]);
+      path |= (int64_t)l << (3 * u->layer_);
+      u = u->leaves_[l];
+    }
+    o[0] = 1, o[1] = t->layer_, o[2] = path, o[3] = t->plane_ptr_->is_plane_;
+  }
+}
+// fl2_shim_session_device_map with the growth and mirror switches of VoxelMapConfig
+int fl2_shim_session_device_map_mirror(void *h, const float *pts, int n, const double *state, double min_eigen_value, int max_points_num, long long root_capacity, int grow,
+                                       int mirror) {
+  ShimSession *s = static_cast<ShimSession *>(h);
+  if (!s) return ESIKF_ERR_ARG;
+  s->mgr->config_setting_.device_map_grow_ = grow != 0, s->mgr->config_setting_.device_map_mirror_ = mirror != 0;
+  return fl2_shim_session_device_map(h, pts, n, state, min_eigen_value, max_points_num, root_capacity);
+}
+// UpdateVoxelMap(input_points) (include/voxel_map.h:232) with point_w [n][3] and var [n][9]
+int fl2_shim_session_update_points(void *h, const double *pw, const double *var, int n) {
+  ShimSession *s = static_cast<ShimSession *>(h);
+  if (!s) return ESIKF_ERR_ARG;
+  std::vector<pointWithVar> pts(n);
+  for (int i = 0; i < n; i++) {
+    for (int k = 0; k < 3; k++) pts[i].point_w[k] = pw[3 * i + k];
+    memcpy(pts[i].var.m, var + 9 * (size_t)i, 72);
+  }
+  s->mgr->UpdateVoxelMap(pts);
+  return s->mgr->last_status_;
+}
+// mapSliding (src/voxel_map.cpp:924-948) with the sensor at `position`
+int fl2_shim_session_map_sliding(void *h, const double *position, int half_map_size, double sliding_thresh) {
+  ShimSession *s = static_cast<ShimSession *>(h);
+  if (!s) return ESIKF_ERR_ARG;
+  VoxelMapManager &mgr = *s->mgr;
+  mgr.config_setting_.half_map_size = half_map_size, mgr.config_setting_.sliding_thresh = sliding_thresh;
+  for (int k = 0; k < 3; k++) mgr.position_last_[k] = position[k];
+  mgr.mapSliding();
+  return mgr.last_status_;
+}
+void *fl2_shim_session_context(void *h) { return static_cast<ShimSession *>(h)->mgr->context(); }
 
 }  // extern "C"

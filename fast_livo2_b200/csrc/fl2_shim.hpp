@@ -79,7 +79,8 @@ struct VoxelLocationHash {
   }
 };
 
-// include/voxel_map.h:129-183 (structure only; the map bookkeeping stays with the reference's own code)
+// include/voxel_map.h:129-183 (structure only; the map bookkeeping stays with the reference's own code). The state members below
+// the plane are what the host mirror of a device-resident map carries (VoxelMapConfig::device_map_mirror_).
 struct VoxelOctoTree {
   VoxelPlane *plane_ptr_ = nullptr;
   int layer_ = 0;
@@ -87,7 +88,11 @@ struct VoxelOctoTree {
   double voxel_center_[3] = {0, 0, 0};
   float quater_length_ = 0;
   bool init_octo_ = false;
+  int max_layer_ = 0, octo_state_ = 0, new_points_ = 0;
+  bool update_enable_ = true;
+  int temp_points_size_ = 0;  // temp_points_.size() of the device node; the point list itself is not mirrored
   ~VoxelOctoTree();
+  VoxelOctoTree *find_correspond(V3D pw);  // include/voxel_map.h:181, src/voxel_map.cpp:292-305
 };
 typedef std::unordered_map<VOXEL_LOCATION, VoxelOctoTree *, VoxelLocationHash> VoxelMap;
 
@@ -103,6 +108,11 @@ struct VoxelMapConfig {
   std::vector<int> layer_init_num_{5, 5, 5, 5, 5};
   long long device_root_capacity_ = 0;  // 0: esikf_map_device_init's default (2^20 root voxels); the starting size when growing
   bool device_map_grow_ = false;        // the device map grows when a tick would exceed its capacities (esikf_map_cfg.grow)
+  // device map: keep voxel_map_ as a read-only host mirror of it (the roots every build / update changed are exported and
+  // applied after the call; mapSliding erases what the slide dropped), for the host code that reads the octree, such as
+  // VIOManager::updateReferencePatch's find_correspond. The point lists are not mirrored: the reference's own UpdateVoxelMap
+  // must not run on it. Read by EnableDeviceMap.
+  bool device_map_mirror_ = false;
   bool map_sliding_en = false;          // local_map/map_sliding_en
   int half_map_size = 100;              // local_map/half_map_size
   double sliding_thresh = 8.0;          // local_map/sliding_thresh
@@ -124,6 +134,14 @@ bool FlattenVoxelMap(const VoxelMap &map, const VoxelMapConfig &cfg, FlatVoxelMa
 // list grew or shrank or moved — needs a full upload), true with the ids of the plane records whose content changed
 // (refitted planes: what esikf_map_patch takes). is_update_ is not used: the reference sets it on every fit and never clears it.
 bool DiffFlatVoxelMaps(const FlatVoxelMap &synced, const FlatVoxelMap &now, std::vector<int32_t> &changed_ids);
+// The host mirror of a device map (VoxelMapConfig::device_map_mirror_). ApplyMapExport walks every exported root's rows
+// (esikf_map_device_export) alongside the root's subtree in `map`: nodes that exist are overwritten field by field, missing
+// ones are allocated (between slides a root only grows). False with `err` set on a malformed export. EraseRootsOutside is
+// clearMemOutOfMap's predicate (src/voxel_map.cpp:958) with the bounds the slide was given; ClearVoxelMap deletes every root.
+bool ApplyMapExport(VoxelMap &map, const VoxelMapConfig &cfg, const int64_t *keys, const int32_t *first, const int32_t *count, int n_roots, const esikf_map_node *nodes,
+                    int n_nodes, std::string *err);
+void EraseRootsOutside(VoxelMap &map, const int64_t lo[3], const int64_t hi[3]);
+void ClearVoxelMap(VoxelMap &map);
 
 // Grow-only page-locked host buffer (esikf_host_alloc): the staging areas the shim hands to the C ABI, so that every
 // per-tick copy is a DMA from / into pinned memory instead of a driver-staged pageable copy.
@@ -180,6 +198,7 @@ class VoxelMapManager {
   int last_sync_patched_ = -1;     // planes patched by the last SyncDeviceMap, -1 = it was a full upload
   void StateEstimation(StatesGroup &state_propagat);  // include/voxel_map.h:229
   // ---- device-resident map: the octrees, point lists and refits live on the GPU (esikf_map_device_*); voxel_map_ is not used
+  // unless config_setting_.device_map_mirror_ makes it a read-only host mirror of the device map
   // and SyncDeviceMap is never needed. EnableDeviceMap once after construction, then the reference's own call sequence:
   //   BuildVoxelMap()              first LiDAR frame, from feats_down_body_ and state_      (include/voxel_map.h:231, LIVMapper.cpp:356-366)
   //   UpdateVoxelMap()             LIVMapper.cpp:413-424 in ONE call: world points + covariances with the posterior and the
@@ -187,6 +206,10 @@ class VoxelMapManager {
   //   UpdateVoxelMap(input_points) the reference's signature (include/voxel_map.h:232) with host lists
   void EnableDeviceMap();
   bool device_map_ = false;
+  bool device_map_mirror_ = false;  // voxel_map_ mirrors the device map (config_setting_.device_map_mirror_ at EnableDeviceMap)
+  // false once a build / update / slide, or the export or apply after it, failed: the mirror is then empty and every later
+  // call reports ESIKF_ERR_STATE until EnableDeviceMap() starts a new map (an export holds one tick's roots only)
+  bool mirror_valid_ = false;
   void BuildVoxelMap();
   void UpdateVoxelMap();
   void UpdateVoxelMap(const std::vector<pointWithVar> &input_points);
@@ -203,6 +226,13 @@ class VoxelMapManager {
   PinnedBuf<int32_t> st_match_, st_normal_;
   PinnedBuf<double> st_state_, st_cov_, st_normals_;
   bool lists_pending_ = false;
+  // the host mirror: export of the last device build / update applied to voxel_map_ (cleared when either fails)
+  void UpdateMirror();
+  void InvalidateMirror();
+  PinnedBuf<int64_t> exp_keys_;
+  PinnedBuf<int32_t> exp_first_, exp_count_;
+  PinnedBuf<esikf_map_node> exp_nodes_;
+  int32_t exp_roots_cap_ = 1024, exp_nodes_cap_ = 4096;  // what the export buffers are requested with (grown from the ticks seen)
 };
 
 // include/vio.h:26-57 restated over flat storage

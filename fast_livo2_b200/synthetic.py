@@ -44,6 +44,33 @@ PLANE_DTYPE = np.dtype(
 )
 assert PLANE_DTYPE.itemsize == 256
 
+# esikf_map_node (include/esikf_b200.h): one octree node of the device map as esikf_map_device_export writes it
+NODE_DTYPE = np.dtype(
+    [
+        ("key", "<i8", (3,)),
+        ("layer", "<i4"),
+        ("path", "<i4"),
+        ("parent", "<i4"),
+        ("leaf", "<i4"),
+        ("voxel_center", "<f8", (3,)),
+        ("quater_length", "<f4"),
+        ("init_octo", "u1"),
+        ("octo_state", "u1"),
+        ("update_enable", "u1"),
+        ("is_plane", "u1"),
+        ("new_points", "<i4"),
+        ("points_size", "<i4"),
+        ("temp_points", "<i4"),
+        ("pad_", "<i4"),
+        ("center", "<f8", (3,)),
+        ("normal", "<f8", (3,)),
+        ("plane_var", "<f8", (21,)),
+        ("d", "<f4"),
+        ("radius", "<f4"),
+    ],
+    align=False,
+)
+
 
 # ----------------------------------------------------------------------------- configs
 @dataclasses.dataclass

@@ -215,6 +215,32 @@ int esikf_map_device_capacity(esikf_ctx *ctx, esikf_map_cfg *out);
 /* The map in esikf_map_upload's flat form (roots in no particular order). keys == NULL: sizes only. */
 int esikf_map_device_download(esikf_ctx *ctx, int64_t *keys, int32_t *first, int32_t *count, int32_t roots_cap, esikf_plane *planes, int32_t planes_cap,
                               int32_t *n_roots, int32_t *n_planes);
+/* One octree node of the device map: VoxelOctoTree (include/voxel_map.h:129-183) with its VoxelPlane, everything the device
+ * keeps of a node except its point list. 312 bytes. */
+typedef struct esikf_map_node {
+  int64_t key[3];          /* VOXEL_LOCATION of the root voxel */
+  int32_t layer;           /* layer_ */
+  int32_t path;            /* 3 bits per layer, as esikf_plane.path */
+  int32_t parent;          /* index of the parent node inside its root's range (0 = the root itself), -1 for the root */
+  int32_t leaf;            /* slot of the node in its parent's leaves_, -1 for the root */
+  double voxel_center[3];  /* voxel_center_ */
+  float quater_length;     /* quater_length_ */
+  uint8_t init_octo, octo_state, update_enable, is_plane;  /* init_octo_, octo_state_, update_enable_, plane_ptr_->is_plane_ */
+  int32_t new_points;      /* new_points_ */
+  int32_t points_size;     /* plane_ptr_->points_size_ */
+  int32_t temp_points;     /* temp_points_.size() on the device (a cut node's list is released there, see DESIGN.md K6) */
+  int32_t pad_;
+  double center[3], normal[3];  /* plane_ptr_->center_, normal_ */
+  double plane_var[21];         /* upper triangle (row-major, i <= j) of plane_ptr_->plane_var_ */
+  float d, radius;              /* plane_ptr_->d_, radius_ */
+} esikf_map_node;
+/* The subtrees of the roots the last esikf_map_device_build / _update / _update_points replayed (in the order of their hash
+ * slots), for a host mirror of the map: root r owns nodes [first[r], first[r] + count[r]) in DFS pre-order, leaves 0..7.
+ * A pure read: calling it twice gives the same bytes. keys == NULL: sizes only. ESIKF_ERR_STATE after esikf_map_device_init,
+ * esikf_map_device_slide or a failed build / update (there is no tick to export: the caller drops the roots the slide
+ * removed with the slide's own bounds). */
+int esikf_map_device_export(esikf_ctx *ctx, int64_t *keys, int32_t *first, int32_t *count, int32_t roots_cap, esikf_map_node *nodes, int32_t nodes_cap,
+                            int32_t *n_roots, int32_t *n_nodes);
 
 /* ---------------------------------------------------------------- LIO update (StateEstimation)
  * Staged form (device-resident between calls):
