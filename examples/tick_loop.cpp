@@ -63,18 +63,28 @@ int main() {
     // ---- VIO tick (LIVMapper::handleVIO -> processFrame -> computeJacobianAndUpdateEKF, vio.cpp:1810)
     std::vector<uint8_t> pixels(64 * 48, 128);
     GrayImage img{pixels.data(), 64, 48};
-    SubSparseMap submap;                                 // filled by retrieveFromVisualSparseMap on the host (vio.cpp:352-782)
-    submap.voxel_points_pos.push_back(V3D());
-    submap.voxel_points_pos[0][0] = 0.0, submap.voxel_points_pos[0][1] = 0.0, submap.voxel_points_pos[0][2] = 2.0;
-    submap.warp_patch.push_back(std::vector<float>(64 * vio_manager.patch_pyrimid_level, 128.0f));
-    submap.search_levels.push_back(0);
-    submap.inv_expo_list.push_back(1.0);
+    // retrieveFromVisualSparseMap (vio.cpp:352-782): the map-side part (depth image, feat_map, grid argmin, depth check) and the
+    // choice of each point's reference feature stay on the host; the per-candidate tail runs in SelectSubSparseMap
+    std::vector<uint8_t> ref_pixels(64 * 48, 128);
+    GrayImage ref_img{ref_pixels.data(), 64, 48};        // Feature::img_ of the one reference frame
+    vio_manager.SetReferenceImages(&ref_img, 1);
+    SubMapCandidate cand{};                              // one visual point 2 m ahead, seen from the same pose
+    cand.ref_img_index = 0, cand.ref_level = 0, cand.ref_key = 7;
+    cand.px_ref[0] = 32.0, cand.px_ref[1] = 24.0, cand.ref_f[2] = 1.0, cand.pos_w[2] = 2.0, cand.normal_w[2] = -1.0;
+    cand.T_ref_w[0] = cand.T_ref_w[4] = cand.T_ref_w[8] = 1.0, cand.ref_inv_expo = 1.0;
+    cand.pc[0] = 32.0, cand.pc[1] = 24.0;                // new_frame_->w2c(pos_), :614
+    const double T_cur_w[12] = {1, 0, 0, 0, 1, 0, 0, 0, 1, 0, 0, 0};  // new_frame_->T_f_w_
+    SubSparseMap submap;
     vio_manager.visual_submap = &submap;
-    vio_manager.total_points = 1;
+    vio_manager.SelectSubSparseMap(&cand, 1, img, T_cur_w);  // fills submap and total_points; patches stay on the device
+    std::printf("tick %d retrieval: status %d, %d of 1 candidates kept\n", tick, vio_manager.last_status_, vio_manager.total_points);
     state_propagat = _state;
     vio_manager.computeJacobianAndUpdateEKF(img);
     std::printf("tick %d VIO: status %d, patch error %.3f\n", tick, vio_manager.last_status_, submap.errors.empty() ? -1.0f : submap.errors[0]);
   }
+  // somebody wants the warp patches of the last selection on the host after all
+  vio_manager.MaterializeWarpPatches();
+  std::printf("warp_patch %zu entries\n", vio_manager.visual_submap->warp_patch.size());
   // somebody wants the per-point lists of the last tick after all (e.g. publishing the effective points)
   voxelmap_manager.MaterializePointLists();
   std::printf("pv_list_ %zu entries, ptpl_list_ %zu\n", voxelmap_manager.pv_list_.size(), voxelmap_manager.ptpl_list_.size());

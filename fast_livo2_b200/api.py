@@ -39,6 +39,10 @@ class VioCfgC(C.Structure):
                 ("exposure_estimate_en", C.c_int32), ("inverse_composition_en", C.c_int32)]
 
 
+class VioSelectCfgC(C.Structure):
+    _fields_ = [("normal_en", C.c_int32), ("ncc_en", C.c_int32), ("ncc_thre", C.c_double), ("outlier_threshold", C.c_double)]
+
+
 class LioStatsC(C.Structure):
     _fields_ = [("iters", C.c_int32), ("effct_feat_num", C.c_int32 * 8), ("converged", C.c_int32 * 8), ("pad_", C.c_int32),
                 ("total_residual", C.c_double * 8), ("HTH", C.c_double * (8 * 36)), ("HTz", C.c_double * (8 * 6)),
@@ -105,6 +109,7 @@ def load_library():
     lib.esikf_vio_warp_patches.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_int32]
     lib.esikf_vio_warp_affine.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp]
     lib.esikf_vio_set_inverse_refs.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp]
+    lib.esikf_vio_select_patches.argtypes = [vp, C.c_int32] + [vp] * 12 + [C.c_double, C.POINTER(VioSelectCfgC), ip, vp, vp, vp, vp, vp]
     lib.esikf_comm_unique_id.argtypes = [C.c_char_p]
     lib.esikf_comm_init.argtypes = [vp, C.c_int32, C.c_int32, C.c_char_p]
     lib.esikf_comm_rank.argtypes = [vp, ip, ip]
@@ -140,7 +145,7 @@ EXPORTED_SYMBOLS = [
     "esikf_set_extrinsics", "esikf_set_lidar_extrinsics", "esikf_map_upload", "esikf_map_patch", "esikf_map_device_init", "esikf_map_device_build", "esikf_map_device_update", "esikf_map_device_update_points", "esikf_map_device_slide", "esikf_map_device_stats", "esikf_map_device_capacity", "esikf_map_device_download", "esikf_map_device_export", "esikf_lio_fetch_normals", "esikf_lio_set_scan", "esikf_lio_run", "esikf_lio_fetch",
     "esikf_lio_update", "esikf_lio_fetch_point_cov", "esikf_vio_set_camera", "esikf_vio_set_image", "esikf_vio_set_patches",
     "esikf_vio_run", "esikf_vio_fetch", "esikf_vio_update", "esikf_vio_get_image_patch", "esikf_vio_set_ref_images",
-    "esikf_vio_warp_patches", "esikf_vio_warp_affine", "esikf_vio_set_inverse_refs", "esikf_comm_unique_id", "esikf_comm_init", "esikf_comm_rank", "esikf_shard_range", "esikf_peer_export", "esikf_peer_attach", "esikf_profile_kernel", "esikf_set_kernel_timing", "esikf_get_kernel_timing", "esikf_set_phase_stamps", "esikf_get_phase_stamps",
+    "esikf_vio_warp_patches", "esikf_vio_select_patches", "esikf_vio_warp_affine", "esikf_vio_set_inverse_refs", "esikf_comm_unique_id", "esikf_comm_init", "esikf_comm_rank", "esikf_shard_range", "esikf_peer_export", "esikf_peer_attach", "esikf_profile_kernel", "esikf_set_kernel_timing", "esikf_get_kernel_timing", "esikf_set_phase_stamps", "esikf_get_phase_stamps",
 ]
 
 
@@ -444,6 +449,30 @@ class Context:
         if keep_on_device:
             self.n_patches = n
         return dict(A_cur_ref=A, search_levels=sl, warp_patch=wp)
+
+    def vio_select_patches(self, ref_idx, px_ref, pos_w, T_ref, ref_inv_expo, pc, T_cur, inv_expo_time, normal_w=None, ref_level=None, ref_f=None,
+                           ref_pos=None, ref_key=None, normal_en=True, ncc_en=False, ncc_thre=0.0, outlier_threshold=1000.0, want_patches=False):
+        """The per-candidate tail of the visual sub-map retrieval (esikf_vio_select_patches): warp matrices (homography form
+        from normal_w when normal_en, else the depth form from ref_f / ref_pos / ref_level cached per ref_key), warps, the
+        photometric / NCC gates; the survivors become the sub-map of the next vio_run. Returns kept (candidate indices),
+        errors, search_levels, A_cur_ref (n_kept, 2, 2) and, with want_patches, warp_patch (n_kept, levels*64)."""
+        n = len(px_ref)
+        d = lambda a, shape: None if a is None else _c(a, np.float64).reshape(shape)
+        i32 = lambda a: None if a is None else _c(a, np.int32).reshape(n)
+        args = [i32(ref_idx), d(px_ref, (n, 2)), i32(ref_level), d(ref_f, (n, 3)), d(ref_pos, (n, 3)), d(pos_w, (n, 3)), d(normal_w, (n, 3)),
+                d(T_ref, (n, 12)), d(ref_inv_expo, (n,)), i32(ref_key), d(pc, (n, 2)), d(T_cur, (12,))]
+        cfg = VioSelectCfgC(int(normal_en), int(ncc_en), float(ncc_thre), float(outlier_threshold))
+        nk = C.c_int32(0)
+        kept, err, sl, A = np.zeros(n, np.int32), np.zeros(n, np.float32), np.zeros(n, np.int32), np.zeros((n, 2, 2))
+        wp = np.zeros((n, 64 * self.levels), np.float32) if want_patches else None
+        self._ck(self.lib.esikf_vio_select_patches(self.h, n, *[_addr(a) for a in args], float(inv_expo_time), C.byref(cfg), C.byref(nk), kept.ctypes.data,
+                                                   err.ctypes.data, sl.ctypes.data, A.ctypes.data, _addr(wp)))
+        k = nk.value
+        self.n_patches = k
+        out = dict(kept=kept[:k], errors=err[:k], search_levels=sl[:k], A_cur_ref=A[:k])
+        if want_patches:
+            out["warp_patch"] = wp[:k]
+        return out
 
     # ------------------------------------------------------------------ multi-GPU / measurement
     def vio_set_inverse_refs(self, ref_img_index, ref_px, ref_f, ref_R, ref_pos):

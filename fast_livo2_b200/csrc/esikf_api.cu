@@ -230,6 +230,12 @@ struct esikf_ctx {
   DevBuf<int32_t> ref_idx;
   DevBuf<double> px_ref, pos_w, normal_w, T_ref, T_cur, A_cur_ref, pc_buf;
   DevBuf<float> patch_buf;
+  // esikf_vio_select_patches scratch (the installed sub-map is only written by its final scatter)
+  DevBuf<double> sel_d, sel_A;
+  DevBuf<int32_t> sel_i;
+  DevBuf<float> sel_warp, sel_err;
+  std::vector<double> sel_stage_d;
+  std::vector<int32_t> sel_stage_i;
 
   // multi-GPU
   int rank = 0, nranks = 1;
@@ -1420,6 +1426,104 @@ int esikf_vio_warp_patches(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_ind
     ctx->n_patches = n;
   }
   CK(cudaStreamSynchronize(st));
+  return ESIKF_OK;
+}
+
+int esikf_vio_select_patches(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_index, const double *px_ref, const int32_t *ref_level,
+                             const double *ref_f, const double *ref_pos, const double *pos_w, const double *normal_w,
+                             const double *T_ref_w, const double *ref_inv_expo, const int32_t *ref_key, const double *pc,
+                             const double *T_cur_w, double inv_expo_time, const esikf_vio_select_cfg *cfg, int32_t *n_kept, int32_t *kept_index,
+                             float *error_out, int32_t *search_level_out, double *A_cur_ref_out, float *warp_patch_out) {
+  if (!ctx || n < 0 || !cfg || !n_kept) return fail(ctx, ESIKF_ERR_ARG, "select_patches: bad argument");
+  const bool homography = cfg->normal_en != 0;
+  if (n > 0 && (!ref_img_index || !px_ref || !pos_w || !T_ref_w || !ref_inv_expo || !pc || !T_cur_w || !kept_index ||
+                (homography ? !normal_w : (!ref_f || !ref_pos || !ref_level || !ref_key))))
+    return fail(ctx, ESIKF_ERR_ARG, "select_patches: null argument");
+  if (!ctx->have_cam) return fail(ctx, ESIKF_ERR_STATE, "select_patches before vio_set_camera");
+  if (ctx->img_w == 0) return fail(ctx, ESIKF_ERR_STATE, "select_patches before vio_set_image");
+  if (n > 0 && ctx->ref_imgs.empty()) return fail(ctx, ESIKF_ERR_STATE, "select_patches before set_ref_images");
+  for (int i = 0; i < n; i++) {
+    if (ref_img_index[i] < 0 || ref_img_index[i] >= (int)ctx->ref_imgs.size()) return fail(ctx, ESIKF_ERR_ARG, "select_patches: ref image index %d", ref_img_index[i]);
+    if (!homography && (ref_level[i] < 0 || ref_level[i] > 8)) return fail(ctx, ESIKF_ERR_ARG, "select_patches: ref level %d", ref_level[i]);
+  }
+  CK(cudaSetDevice(ctx->device));
+  const int L = ctx->vio_cfg.patch_pyrimid_level;
+  cudaStream_t st = ctx->stream;
+  // every argument check is above: from here on the call replaces the installed sub-map
+  CK(ctx->vis_pos.reserve((size_t)n * 3 + 4));
+  CK(ctx->warp_patch.reserve((size_t)n * 64 * L + 64));
+  CK(ctx->search_levels.reserve(n + 1));
+  CK(ctx->inv_expo.reserve(n + 1));
+  CK(ctx->errors.reserve(n + 1));
+  *n_kept = 0;
+  if (n == 0) {
+    ctx->n_patches = 0;
+    return ESIKF_OK;
+  }
+  // one staging copy per element type; device layout (doubles): px 2n | ref_f 3n | ref_pos 3n | pos 3n | normal 3n | T_ref 12n |
+  // inv_expo n | pc 2n | T_cur 12, (ints) ref_idx n | ref_level n | ref_key n | search level n | keep n | dst n | n_kept 1 | kept n
+  const size_t N = (size_t)n;
+  const size_t o_px = 0, o_f = 2 * N, o_rp = 5 * N, o_pos = 8 * N, o_nrm = 11 * N, o_T = 14 * N, o_ie = 26 * N, o_pc = 27 * N, o_Tc = 29 * N;
+  std::vector<double> &hd = ctx->sel_stage_d;
+  hd.assign(29 * N + 12, 0.0);
+  auto put = [&](size_t off, const double *src, size_t cnt) {
+    if (src) memcpy(hd.data() + off, src, cnt * sizeof(double));
+  };
+  put(o_px, px_ref, 2 * N), put(o_f, ref_f, 3 * N), put(o_rp, ref_pos, 3 * N), put(o_pos, pos_w, 3 * N), put(o_nrm, normal_w, 3 * N);
+  put(o_T, T_ref_w, 12 * N), put(o_ie, ref_inv_expo, N), put(o_pc, pc, 2 * N), put(o_Tc, T_cur_w, 12);
+  std::vector<int32_t> &hi = ctx->sel_stage_i;
+  hi.assign(3 * N, 0);
+  memcpy(hi.data(), ref_img_index, N * sizeof(int32_t));
+  if (!homography) memcpy(hi.data() + N, ref_level, N * sizeof(int32_t)), memcpy(hi.data() + 2 * N, ref_key, N * sizeof(int32_t));
+  CK(ctx->sel_d.reserve(hd.size()));
+  CK(ctx->sel_i.reserve(7 * N + 1));
+  CK(ctx->sel_A.reserve(8 * N));
+  CK(ctx->sel_warp.reserve(N * 64 * L));
+  CK(ctx->sel_err.reserve(N));
+  CK(cudaMemcpyAsync(ctx->sel_d.p, hd.data(), hd.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(ctx->sel_i.p, hi.data(), hi.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  const double *d = ctx->sel_d.p;
+  int32_t *iv = ctx->sel_i.p;
+  int32_t *d_idx = iv, *d_lvl = iv + N, *d_key = iv + 2 * N, *d_sl = iv + 3 * N, *d_keep = iv + 4 * N, *d_dst = iv + 5 * N, *d_nk = iv + 6 * N,
+          *d_kept = iv + 6 * N + 1;
+  double *d_A = ctx->sel_A.p, *d_Akept = ctx->sel_A.p + 4 * N;
+  CamDev cam;
+  cam_dev(ctx, cam);
+  if (homography)
+    warp_matrix_kernel<<<(n + 127) / 128, 128, 0, st>>>(cam, n, d + o_px, d + o_pos, d + o_nrm, d + o_T, d + o_Tc, d_A, d_sl);
+  else
+    warp_matrix_depth_kernel<<<(n + 127) / 128, 128, 0, st>>>(cam, n, d + o_px, d + o_f, d + o_rp, d + o_pos, d + o_T, d + o_Tc, d_lvl, d_key, d_A, d_sl);
+  // patch_wrap is a fresh zero vector per candidate (:646): a NaN inverse leaves it zero (:297-301)
+  CK(cudaMemsetAsync(ctx->sel_warp.p, 0, N * 64 * L * sizeof(float), st));
+  warp_affine_kernel<<<(n * L * 64 + 255) / 256, 256, 0, st>>>(ctx->ref_img_ptrs.p, d_idx, ctx->ref_w, ctx->ref_h, n, L, d_A, d + o_px, d_sl, ctx->sel_warp.p);
+  SelectGateArgs ga;
+  ga.img = ctx->img.p, ga.width = ctx->img_w, ga.height = ctx->img_h, ga.n = n, ga.levels = L, ga.ncc_en = cfg->ncc_en != 0;
+  ga.pc = d + o_pc, ga.warp = ctx->sel_warp.p, ga.ref_inv_expo = d + o_ie;
+  ga.cur_inv_expo = inv_expo_time, ga.ncc_thre = cfg->ncc_thre, ga.outlier_threshold = cfg->outlier_threshold;
+  ga.error = ctx->sel_err.p, ga.keep = d_keep;
+  select_gate_kernel<<<(n + SELECT_GATE_WARPS - 1) / SELECT_GATE_WARPS, 32 * SELECT_GATE_WARPS, 0, st>>>(ga);
+  select_scan_kernel<<<1, SELECT_SCAN_THREADS, 0, st>>>(d_keep, n, d_dst, d_nk);
+  SelectScatterArgs sa;
+  sa.n = n, sa.levels = L, sa.keep = d_keep, sa.dst = d_dst, sa.search_level = d_sl, sa.pos_w = d + o_pos, sa.ref_inv_expo = d + o_ie, sa.A = d_A;
+  sa.warp = ctx->sel_warp.p, sa.error = ctx->sel_err.p;
+  sa.vis_pos = ctx->vis_pos.p, sa.inv_expo = ctx->inv_expo.p, sa.A_kept = d_Akept, sa.warp_patch = ctx->warp_patch.p, sa.errors = ctx->errors.p;
+  sa.search_levels = ctx->search_levels.p, sa.kept_index = d_kept;
+  select_scatter_kernel<<<(n + 7) / 8, 256, 0, st>>>(sa);
+  ctx->launches += 5;
+  CK(cudaGetLastError());
+  int32_t nk = 0;
+  CK(cudaMemcpyAsync(&nk, d_nk, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  ctx->n_patches = nk;
+  *n_kept = nk;
+  if (nk > 0) {
+    CK(cudaMemcpyAsync(kept_index, d_kept, (size_t)nk * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    if (error_out) CK(cudaMemcpyAsync(error_out, ctx->errors.p, (size_t)nk * sizeof(float), cudaMemcpyDeviceToHost, st));
+    if (search_level_out) CK(cudaMemcpyAsync(search_level_out, ctx->search_levels.p, (size_t)nk * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    if (A_cur_ref_out) CK(cudaMemcpyAsync(A_cur_ref_out, d_Akept, (size_t)nk * 4 * sizeof(double), cudaMemcpyDeviceToHost, st));
+    if (warp_patch_out) CK(cudaMemcpyAsync(warp_patch_out, ctx->warp_patch.p, (size_t)nk * 64 * L * sizeof(float), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+  }
   return ESIKF_OK;
 }
 

@@ -11,6 +11,8 @@
 // Mapping: one warp per visual patch, two pixels per lane. The 64 rows [JdR Jdt cur res] of a patch are staged in shared
 // memory and contracted with 16 fp64 tensor-core steps (mma.sync.m8n8k4.f64); per-warp 8x8 blocks are combined in a fixed
 // order so the error-gated accept / rollback decision is reproducible.
+#include <cub/block/block_scan.cuh>
+
 #include "esikf_dev.cuh"
 
 namespace esikf {
@@ -401,6 +403,17 @@ __global__ void image_patch_kernel(const uint8_t *__restrict__ img, int width, i
   out[gid] = bil(tg.w_tl, tg.w_tr, tg.w_bl, tg.w_br, tap(img, b, npix), tap(img, b + scale, npix), tap(img, b + sw, npix), tap(img, b + sw + scale, npix));
 }
 
+// getBestSearchLevel(A, 2)   (:320-331)
+__device__ __forceinline__ int best_search_level(double A00, double A01, double A10, double A11) {
+  int sl = 0;
+  double Dt = det2_rn(A00, A11, A01, A10);
+  while (Dt > 3.0 && sl < 2) {
+    sl += 1;
+    Dt *= 0.25;
+  }
+  return sl;
+}
+
 // getWarpMatrixAffineHomography + getBestSearchLevel for the normal_en branch of retrieveFromVisualSparseMap (vio.cpp:699-715).
 __global__ void warp_matrix_kernel(CamDev cam, int n, const double *__restrict__ px_ref, const double *__restrict__ pos_w,
                                    const double *__restrict__ normal_w, const double *__restrict__ T_ref_w, const double *__restrict__ T_cur_w,
@@ -449,14 +462,58 @@ __global__ void warp_matrix_kernel(CamDev cam, int n, const double *__restrict__
   world2cam(cam, fv[0], fv[1], fv[2], vu, vv);
   const double A00 = (uu - cu) / 4, A10 = (uv - cv) / 4, A01 = (vu - cu) / 4, A11 = (vv - cv) / 4;
   A_out[4 * i] = A00, A_out[4 * i + 1] = A01, A_out[4 * i + 2] = A10, A_out[4 * i + 3] = A11;
-  // getBestSearchLevel(A, 2)   (:320-331)
-  int sl = 0;
-  double Dt = det2_rn(A00, A11, A01, A10);
-  while (Dt > 3.0 && sl < 2) {
-    sl += 1;
-    Dt *= 0.25;
+  search_level[i] = best_search_level(A00, A01, A10, A11);
+}
+
+// getWarpMatrixAffine + getBestSearchLevel for the depth branch of retrieveFromVisualSparseMap (vio.cpp:275-290, 716-734):
+// xyz_ref = f_ref * |ref_pos - pos|, pyramid_level 0, halfpatch 4. The reference caches (A, level) per reference frame in
+// warp_map for the whole frame, so a candidate uses the result of the FIRST candidate (in candidate order) that carries its
+// ref_key. Each thread finds that owner by a forward scan of the keys and evaluates the owner's inputs itself: the result does
+// not depend on scheduling. The scan stops at the owner, so a thread reads (owner index + 1) keys: the total is bounded by
+// n x (index of the last first occurrence of a key), i.e. by n x (number of distinct reference frames) when the candidates of
+// each frame are spread through the list. Only a set where nearly every candidate has its own reference frame approaches
+// n^2 / 2 reads (8 M for 4 k candidates, about as long as the gate kernel at that size).
+__global__ void warp_matrix_depth_kernel(CamDev cam, int n, const double *__restrict__ px_ref, const double *__restrict__ ref_f,
+                                         const double *__restrict__ ref_pos, const double *__restrict__ pos_w, const double *__restrict__ T_ref_w,
+                                         const double *__restrict__ T_cur_w, const int32_t *__restrict__ level_ref, const int32_t *__restrict__ ref_key,
+                                         double *__restrict__ A_out, int32_t *__restrict__ search_level) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int key = ref_key[i];
+  int o = 0;
+  while (ref_key[o] != key) o++;  // stops at i at the latest
+  const double *Rr = T_ref_w + 12 * (size_t)o, *tr = Rr + 9;
+  const double *Rc = T_cur_w, *tc = T_cur_w + 9;
+  // T_cur_ref = T_cur * T_ref^-1 as Sophus composes it: T_ref^-1 = (Rr^T, -(Rr^T tr)); R = Rc Rr^T, t = Rc (-(Rr^T tr)) + tc
+  double R[9], ti[3], t[3];
+  for (int r = 0; r < 3; r++)
+    for (int c = 0; c < 3; c++) R[3 * r + c] = Rc[3 * r] * Rr[3 * c] + Rc[3 * r + 1] * Rr[3 * c + 1] + Rc[3 * r + 2] * Rr[3 * c + 2];
+  for (int r = 0; r < 3; r++) ti[r] = -(Rr[r] * tr[0] + Rr[3 + r] * tr[1] + Rr[6 + r] * tr[2]);
+  for (int r = 0; r < 3; r++) t[r] = Rc[3 * r] * ti[0] + Rc[3 * r + 1] * ti[1] + Rc[3 * r + 2] * ti[2] + tc[r];
+  const double *rp = ref_pos + 3 * (size_t)o, *pw = pos_w + 3 * (size_t)o, *f = ref_f + 3 * (size_t)o;
+  const double dx = rp[0] - pw[0], dy = rp[1] - pw[1], dz = rp[2] - pw[2];
+  const double depth = sqrt(dx * dx + dy * dy + dz * dz);
+  const double xyz[3] = {f[0] * depth, f[1] * depth, f[2] * depth};
+  const double step = 4.0 * (double)(1 << level_ref[o]);  // halfpatch_size * 2^level_ref * 2^0
+  const double pu = px_ref[2 * (size_t)o], pv = px_ref[2 * (size_t)o + 1];
+  double xdu[3], xdv[3];
+  cam2world(cam, pu + step, pv, xdu);
+  cam2world(cam, pu, pv + step, xdv);
+  const double su = xyz[2] / xdu[2], sv = xyz[2] / xdv[2];
+  for (int r = 0; r < 3; r++) xdu[r] *= su, xdv[r] *= sv;
+  double pc[3], pdu[3], pdv[3];
+  for (int r = 0; r < 3; r++) {
+    pc[r] = R[3 * r] * xyz[0] + R[3 * r + 1] * xyz[1] + R[3 * r + 2] * xyz[2] + t[r];
+    pdu[r] = R[3 * r] * xdu[0] + R[3 * r + 1] * xdu[1] + R[3 * r + 2] * xdu[2] + t[r];
+    pdv[r] = R[3 * r] * xdv[0] + R[3 * r + 1] * xdv[1] + R[3 * r + 2] * xdv[2] + t[r];
   }
-  search_level[i] = sl;
+  double cu, cv, uu, uv, vu, vv;
+  world2cam(cam, pc[0], pc[1], pc[2], cu, cv);
+  world2cam(cam, pdu[0], pdu[1], pdu[2], uu, uv);
+  world2cam(cam, pdv[0], pdv[1], pdv[2], vu, vv);
+  const double A00 = (uu - cu) / 4, A10 = (uv - cv) / 4, A01 = (vu - cu) / 4, A11 = (vv - cv) / 4;
+  A_out[4 * i] = A00, A_out[4 * i + 1] = A01, A_out[4 * i + 2] = A10, A_out[4 * i + 3] = A11;
+  search_level[i] = best_search_level(A00, A01, A10, A11);
 }
 
 // warpAffine for all pyramid levels (vio.cpp:292-318, 739-742). One thread per output value.
@@ -492,6 +549,125 @@ __global__ void warp_affine_kernel(const uint8_t *const *__restrict__ ref_imgs, 
                     __fmul_rn(w11, (float)p[cols + 1]));
   }
   out[gid] = val;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Per-candidate tail of retrieveFromVisualSparseMap (vio.cpp:744-770) after the warps: the current patch, the photometric
+// error, the optional NCC gate, the outlier gate, and the append of the survivors in candidate order.
+struct SelectGateArgs {
+  const uint8_t *img;
+  int width, height, n, levels, ncc_en;
+  const double *pc;            // [n][2] projection of each candidate into the current frame (:614)
+  const float *warp;           // [n][levels*64] warped reference patches
+  const double *ref_inv_expo;  // [n] Feature::inv_expo_time_ of each candidate's reference feature
+  double cur_inv_expo, ncc_thre, outlier_threshold;
+  float *error;                // [n] out
+  int32_t *keep;               // [n] out: 1 = survives both gates
+};
+
+#define SELECT_GATE_WARPS 8
+// One warp per candidate. The sums of the reference are serial and in index order (error: float accumulator of double terms,
+// :746-751; calculateNCC: double sums, :333-350), so each runs on one lane over the staged patches, with the rounding of every
+// step spelled out (no FMA contraction). The chains are independent: the error, the two NCC sums and the three NCC moments
+// run on different lanes.
+__global__ void __launch_bounds__(32 * SELECT_GATE_WARPS) select_gate_kernel(const SelectGateArgs a) {
+  __shared__ float cur_s[SELECT_GATE_WARPS][64], ref_s[SELECT_GATE_WARPS][64];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int i = blockIdx.x * SELECT_GATE_WARPS + w;
+  if (i >= a.n) return;
+  // getImagePatch(img, pc, patch_buffer, 0) (:744), as image_patch_kernel
+  const TapGeom tg = tap_geometry(a.pc[2 * (size_t)i], a.pc[2 * (size_t)i + 1], 0);
+  const long npix = (long)a.width * a.height;
+#pragma unroll
+  for (int q = 0; q < 2; q++) {
+    const int pix = 2 * lane + q, x = pix >> 3, y = pix & 7;
+    const long b = (long)(tg.v - 4 + x) * a.width + (tg.u - 4) + y;
+    cur_s[w][pix] = bil(tg.w_tl, tg.w_tr, tg.w_bl, tg.w_br, tap(a.img, b, npix), tap(a.img, b + 1, npix), tap(a.img, b + a.width, npix),
+                        tap(a.img, b + a.width + 1, npix));
+    ref_s[w][pix] = a.warp[(size_t)i * 64 * a.levels + pix];  // pyramid level 0 of patch_wrap
+  }
+  __syncwarp();
+  const float *cur = cur_s[w], *ref = ref_s[w];
+  double s = 0.0;  // lane 0: error; lanes 1 / 2: sum of the reference / current patch
+  if (lane == 0) {
+    const double ri = a.ref_inv_expo[i], ci = a.cur_inv_expo;
+    float error = 0.0f;
+    for (int k = 0; k < 64; k++) {
+      const double d = __dsub_rn(__dmul_rn(ri, (double)ref[k]), __dmul_rn(ci, (double)cur[k]));
+      error = (float)__dadd_rn((double)error, __dmul_rn(d, d));
+    }
+    s = (double)error;
+  } else if (a.ncc_en && lane <= 2) {
+    const float *p = lane == 1 ? ref : cur;
+    for (int k = 0; k < 64; k++) s = __dadd_rn(s, (double)p[k]);
+  }
+  bool keep = true;
+  if (a.ncc_en) {
+    const double mean_ref = __shfl_sync(0xffffffffu, s, 1) / 64, mean_cur = __shfl_sync(0xffffffffu, s, 2) / 64;
+    double m = 0.0;  // lane 1: numerator, lane 2: demoniator1, lane 3: demoniator2
+    if (lane >= 1 && lane <= 3)
+      for (int k = 0; k < 64; k++) {
+        const double dr = __dsub_rn((double)ref[k], mean_ref), dc = __dsub_rn((double)cur[k], mean_cur);
+        m = __dadd_rn(m, lane == 1 ? __dmul_rn(dr, dc) : lane == 2 ? __dmul_rn(dr, dr) : __dmul_rn(dc, dc));
+      }
+    const double num = __shfl_sync(0xffffffffu, m, 1), d1 = __shfl_sync(0xffffffffu, m, 2), d2 = __shfl_sync(0xffffffffu, m, 3);
+    const double ncc = __ddiv_rn(num, __dsqrt_rn(__dadd_rn(__dmul_rn(d1, d2), 1e-10)));
+    keep = !(ncc < a.ncc_thre);  // :756
+  }
+  if (lane == 0) {
+    a.error[i] = (float)s;
+    a.keep[i] = keep && !(s > a.outlier_threshold * 64);  // :763 (an error equal to the threshold is kept)
+  }
+}
+
+// Exclusive prefix sum of keep[0, n) into dst (one CTA, candidate order) and the survivor count into *n_kept.
+#define SELECT_SCAN_THREADS 1024
+__global__ void __launch_bounds__(SELECT_SCAN_THREADS) select_scan_kernel(const int32_t *__restrict__ keep, int n, int32_t *__restrict__ dst,
+                                                                          int32_t *__restrict__ n_kept) {
+  typedef cub::BlockScan<int, SELECT_SCAN_THREADS> Scan;
+  __shared__ typename Scan::TempStorage tmp;
+  int carry = 0;
+  for (int base = 0; base < n; base += SELECT_SCAN_THREADS) {
+    const int j = base + threadIdx.x;
+    const int f = j < n ? keep[j] : 0;
+    int x, total;
+    Scan(tmp).ExclusiveSum(f, x, total);
+    if (j < n) dst[j] = carry + x;
+    carry += total;
+    __syncthreads();  // tmp is reused by the next chunk
+  }
+  if (threadIdx.x == 0) *n_kept = carry;
+}
+
+// The append of :765-770 for every survivor i at dst[i], one warp per candidate: the visual sub-map the update reads (pos,
+// warp_patch over all levels, search level, the reference feature's inverse exposure time, the gate error) and, per survivor,
+// its candidate index and warp matrix.
+struct SelectScatterArgs {
+  int n, levels;
+  const int32_t *keep, *dst, *search_level;
+  const double *pos_w, *ref_inv_expo, *A;
+  const float *warp, *error;
+  double *vis_pos, *inv_expo, *A_kept;
+  float *warp_patch, *errors;
+  int32_t *search_levels, *kept_index;
+};
+__global__ void select_scatter_kernel(const SelectScatterArgs a) {
+  const int lane = threadIdx.x & 31;
+  const int i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (i >= a.n || !a.keep[i]) return;
+  const int p = a.dst[i];
+  const int len = 64 * a.levels;
+  const float2 *src = reinterpret_cast<const float2 *>(a.warp + (size_t)i * len);
+  float2 *out = reinterpret_cast<float2 *>(a.warp_patch + (size_t)p * len);
+  for (int k = lane; k < len / 2; k += 32) out[k] = src[k];
+  if (lane < 3) a.vis_pos[3 * (size_t)p + lane] = a.pos_w[3 * (size_t)i + lane];
+  if (lane < 4) a.A_kept[4 * (size_t)p + lane] = a.A[4 * (size_t)i + lane];
+  if (lane == 0) {
+    a.search_levels[p] = a.search_level[i];
+    a.inv_expo[p] = a.ref_inv_expo[i];
+    a.errors[p] = a.error[i];
+    a.kept_index[p] = i;
+  }
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

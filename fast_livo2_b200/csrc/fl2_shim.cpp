@@ -510,6 +510,31 @@ void VIOManager::computeJacobianAndUpdateEKF(const GrayImage &img) {
   if (!ctx_ || !state || !state_propagat || !visual_submap) return;
   if (total_points == 0) return;  // src/vio.cpp:786
   const int n = total_points, L = patch_pyrimid_level;
+  if (visual_submap == selected_submap_ && n == selected_count_) {
+    // the sub-map SelectSubSparseMap installed is still on the device: image and states only
+    double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
+    float *err = st_err_.get(n);
+    if (!sbuf || !err) {
+      last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
+      return;
+    }
+    double *sin = sbuf, *sprop = sbuf + ESIKF_STATE_DOUBLES, *sout = sbuf + 2 * ESIKF_STATE_DOUBLES;
+    state->pack(sin);
+    state_propagat->pack(sprop);
+    esikf_vio_stats stats;
+    last_status_ = esikf_vio_set_image(ctx_, img.data, img.cols, img.rows);
+    patch_img_ = nullptr;
+    if (!last_status_) last_status_ = esikf_vio_run(ctx_, sin, sprop);
+    if (!last_status_) last_status_ = esikf_vio_fetch(ctx_, sout, &stats, err);
+    if (last_status_) {
+      last_error_ = esikf_last_error(ctx_);
+      return;
+    }
+    visual_submap->errors.assign(err, err + n);
+    state->unpack(sout);
+    last_total_iters_ = stats.total_iters;
+    return;
+  }
   double *pos = st_pos_.get((size_t)n * 3), *ie = st_ie_.get(n), *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
   float *wp = st_wp_.get((size_t)n * 64 * L), *err = st_err_.get(n);
   int32_t *sl = st_sl_.get(n);
@@ -533,6 +558,8 @@ void VIOManager::computeJacobianAndUpdateEKF(const GrayImage &img) {
   esikf_vio_stats stats;
   patch_img_ = nullptr;  // the update installs its own current image
   last_status_ = esikf_vio_update(ctx_, im, img.cols, img.rows, pos, wp, sl, ie, n, sin, sprop, sout, &stats, err);
+  selected_submap_ = nullptr, selected_count_ = -1;  // the device now holds this upload
+  submap_uploads_++;
   if (last_status_) {
     last_error_ = esikf_last_error(ctx_);
     return;
@@ -575,6 +602,7 @@ void VIOManager::warpAffine(const double A_cur_ref[4], const GrayImage &img_ref,
     const uint8_t *imgs[1] = {img_ref.data};
     last_status_ = esikf_vio_set_ref_images(ctx_, imgs, 1, img_ref.cols, img_ref.rows);
     patch_ref_img_ = last_status_ ? nullptr : img_ref.data, patch_ref_w_ = img_ref.cols, patch_ref_h_ = img_ref.rows;
+    ref_imgs_current_ = false;
   }
   std::vector<float> all((size_t)64 * patch_pyrimid_level);
   const int32_t idx = 0, sl = search_level;
@@ -590,6 +618,81 @@ void VIOManager::warpAffine(const double A_cur_ref[4], const GrayImage &img_ref,
   const float inv00 = (float)(A_cur_ref[3] * inv_det);  // same expression as the kernel's A_ref_cur(0, 0)
   if (inv00 != inv00) return;
   memcpy(patch + 64 * pyramid_level, all.data() + 64 * pyramid_level, sizeof(float) * 64);
+}
+
+void VIOManager::SetReferenceImages(const GrayImage *imgs, int n) {
+  if (!ctx_) return;
+  std::vector<const uint8_t *> ptrs;
+  for (int k = 0; k < n; k++) ptrs.push_back(imgs[k].data);
+  last_status_ = n > 0 ? esikf_vio_set_ref_images(ctx_, ptrs.data(), n, imgs[0].cols, imgs[0].rows) : ESIKF_ERR_ARG;
+  ref_imgs_.assign(imgs, imgs + (n > 0 ? n : 0));
+  ref_imgs_current_ = last_status_ == 0;
+  patch_ref_img_ = nullptr;  // the per-patch warpAffine uploads its own image again
+  if (last_status_) last_error_ = n > 0 ? esikf_last_error(ctx_) : "SetReferenceImages: no image";
+}
+
+void VIOManager::SelectSubSparseMap(const SubMapCandidate *c, int n, const GrayImage &img, const double T_cur_w[12]) {
+  if (!ctx_ || !state || !visual_submap || n < 0 || (n > 0 && !c) || !T_cur_w) return;
+  selected_submap_ = nullptr, selected_count_ = -1;
+  last_status_ = ref_imgs_current_ ? 0 : ESIKF_ERR_STATE;
+  if (last_status_) {
+    last_error_ = "SelectSubSparseMap before SetReferenceImages";
+    return;
+  }
+  last_status_ = esikf_vio_set_image(ctx_, img.data, img.cols, img.rows);
+  patch_img_ = last_status_ ? nullptr : img.data, patch_img_w_ = img.cols, patch_img_h_ = img.rows;
+  const size_t N = (size_t)n;
+  std::vector<int32_t> idx(N), lvl(N), key(N), kept(N), sl(N);
+  std::vector<double> px(2 * N), f(3 * N), rp(3 * N), pw(3 * N), nw(3 * N), T(12 * N), ie(N), pc(2 * N), A(4 * N);
+  std::vector<float> err(N);
+  for (size_t i = 0; i < N; i++) {
+    idx[i] = c[i].ref_img_index, lvl[i] = c[i].ref_level, key[i] = c[i].ref_key, ie[i] = c[i].ref_inv_expo;
+    memcpy(&px[2 * i], c[i].px_ref, 16), memcpy(&pc[2 * i], c[i].pc, 16), memcpy(&T[12 * i], c[i].T_ref_w, 96);
+    memcpy(&f[3 * i], c[i].ref_f, 24), memcpy(&rp[3 * i], c[i].ref_pos, 24), memcpy(&pw[3 * i], c[i].pos_w, 24), memcpy(&nw[3 * i], c[i].normal_w, 24);
+  }
+  esikf_vio_select_cfg cfg;
+  cfg.normal_en = normal_en ? 1 : 0, cfg.ncc_en = ncc_en ? 1 : 0, cfg.ncc_thre = ncc_thre, cfg.outlier_threshold = outlier_threshold;
+  int32_t nk = 0;
+  if (!last_status_)
+    last_status_ = esikf_vio_select_patches(ctx_, n, idx.data(), px.data(), lvl.data(), f.data(), rp.data(), pw.data(), nw.data(), T.data(), ie.data(),
+                                            key.data(), pc.data(), T_cur_w, state->inv_expo_time, &cfg, &nk, kept.data(), err.data(), sl.data(), A.data(),
+                                            nullptr);
+  if (last_status_) {
+    last_error_ = esikf_last_error(ctx_);
+    return;
+  }
+  SubSparseMap &sub = *visual_submap;  // :765-770, in candidate order
+  sub.voxel_points_pos.resize(nk), sub.search_levels.assign(sl.begin(), sl.begin() + nk), sub.errors.assign(err.begin(), err.begin() + nk);
+  sub.inv_expo_list.resize(nk), sub.candidate_index.assign(kept.begin(), kept.begin() + nk), sub.warp_patch.clear();
+  sel_ref_idx_.resize(nk), sel_sl_.assign(sl.begin(), sl.begin() + nk), sel_px_.resize(2 * (size_t)nk), sel_A_.assign(A.begin(), A.begin() + 4 * (size_t)nk);
+  for (int j = 0; j < nk; j++) {
+    const SubMapCandidate &k = c[kept[j]];
+    for (int a = 0; a < 3; a++) sub.voxel_points_pos[j][a] = k.pos_w[a];
+    sub.inv_expo_list[j] = k.ref_inv_expo;
+    sel_ref_idx_[j] = k.ref_img_index, sel_px_[2 * j] = k.px_ref[0], sel_px_[2 * j + 1] = k.px_ref[1];
+  }
+  total_points = nk;
+  selected_submap_ = visual_submap, selected_count_ = nk;
+}
+
+void VIOManager::MaterializeWarpPatches() {
+  if (!ctx_ || !selected_submap_ || selected_submap_ != visual_submap) return;
+  const int nk = selected_count_, L = patch_pyrimid_level;
+  if ((int)visual_submap->warp_patch.size() == nk) return;
+  last_status_ = 0;
+  if (!ref_imgs_current_ && !ref_imgs_.empty()) {  // the per-patch warpAffine replaced them since
+    std::vector<GrayImage> imgs = ref_imgs_;
+    SetReferenceImages(imgs.data(), (int)imgs.size());
+  }
+  // the same kernel on the same matrices, levels and reference pixels as the selection: the patches the device holds
+  std::vector<float> wp((size_t)nk * 64 * L);
+  if (!last_status_) last_status_ = esikf_vio_warp_affine(ctx_, nk, sel_ref_idx_.data(), sel_px_.data(), sel_A_.data(), sel_sl_.data(), wp.data());
+  if (last_status_) {
+    last_error_ = esikf_last_error(ctx_);
+    return;
+  }
+  visual_submap->warp_patch.resize(nk);
+  for (int j = 0; j < nk; j++) visual_submap->warp_patch[j].assign(wp.begin() + (size_t)j * 64 * L, wp.begin() + (size_t)(j + 1) * 64 * L);
 }
 
 }  // namespace fl2b200
@@ -800,6 +903,69 @@ int fl2_shim_resync_run(const int64_t *keys, const int32_t *first, const int32_t
     }
   }
   for (auto &kv : map) delete kv.second;
+  return rc;
+}
+
+// GPU: VIOManager::SelectSubSparseMap + computeJacobianAndUpdateEKF (sub-map left on the device), then the same update from
+// the host-assembled sub-map (MaterializeWarpPatches, a copy of visual_submap, the set_patches path). gate = [normal_en, ncc_en,
+// ncc_thre, outlier_threshold]. counts = [launches of the first update, sub-map uploads after it, launches of the second
+// update, sub-map uploads after it]. Returns 0 or the first failing esikf_status.
+int fl2_shim_select_run(const esikf_camera *cam, const esikf_vio_cfg *vcfg, const esikf_extrinsics *ext, const uint8_t *img, const uint8_t *const *ref_imgs,
+                        int n_imgs, const SubMapCandidate *cands, int n, const double *T_cur_w, const double *state_in, const double *gate, int32_t *n_kept,
+                        int32_t *kept, double *state_sel, float *errors_sel, double *state_host, float *errors_host, float *warp_out, int64_t *counts) {
+  esikf_ctx *ctx = nullptr;
+  int rc = esikf_create(&ctx, 0);
+  if (rc) return rc;
+  {
+    VIOManager vio(ctx);
+    StatesGroup st, stp;
+    st.unpack(state_in), stp.unpack(state_in);
+    SubSparseMap sub;
+    vio.state = &st, vio.state_propagat = &stp, vio.visual_submap = &sub;
+    vio.patch_pyrimid_level = vcfg->patch_pyrimid_level, vio.max_iterations = vcfg->max_iterations, vio.img_point_cov = vcfg->img_point_cov;
+    vio.exposure_estimate_en = vcfg->exposure_estimate_en != 0;
+    vio.cam = *cam;
+    memcpy(vio.Rcl.m, ext->Rcl, 72), memcpy(vio.Pcl.v, ext->Pcl, 24), memcpy(vio.extR.m, ext->extR, 72), memcpy(vio.extT.v, ext->extT, 24);
+    vio.normal_en = gate[0] != 0, vio.ncc_en = gate[1] != 0, vio.ncc_thre = gate[2], vio.outlier_threshold = gate[3];
+    vio.initializeVIO();
+    GrayImage im;
+    im.data = img, im.cols = cam->width, im.rows = cam->height;
+    std::vector<GrayImage> refs(n_imgs);
+    for (int k = 0; k < n_imgs; k++) refs[k].data = ref_imgs[k], refs[k].cols = cam->width, refs[k].rows = cam->height;
+    if (!vio.last_status_) vio.SetReferenceImages(refs.data(), n_imgs);
+    if (!vio.last_status_) vio.SelectSubSparseMap(cands, n, im, T_cur_w);
+    rc = vio.last_status_;
+    if (!rc) {
+      *n_kept = vio.total_points;
+      for (int j = 0; j < vio.total_points; j++) kept[j] = sub.candidate_index[j];
+      int64_t l0 = esikf_launch_count(ctx);
+      vio.computeJacobianAndUpdateEKF(im);
+      counts[0] = esikf_launch_count(ctx) - l0, counts[1] = vio.submap_uploads_;
+      rc = vio.last_status_;
+    }
+    if (!rc) {
+      st.pack(state_sel);
+      for (int j = 0; j < vio.total_points; j++) errors_sel[j] = sub.errors[j];
+      vio.MaterializeWarpPatches();
+      rc = vio.last_status_;
+    }
+    if (!rc) {
+      const int L = vio.patch_pyrimid_level;
+      for (int j = 0; j < vio.total_points; j++) memcpy(warp_out + (size_t)j * 64 * L, sub.warp_patch[j].data(), sizeof(float) * 64 * L);
+      SubSparseMap host = sub;  // the sub-map as a host-side retrieval would have assembled it
+      vio.visual_submap = &host;
+      st.unpack(state_in);
+      int64_t l0 = esikf_launch_count(ctx);
+      vio.computeJacobianAndUpdateEKF(im);
+      counts[2] = esikf_launch_count(ctx) - l0, counts[3] = vio.submap_uploads_;
+      rc = vio.last_status_;
+      if (!rc) {
+        st.pack(state_host);
+        for (int j = 0; j < vio.total_points; j++) errors_host[j] = host.errors[j];
+      }
+    }
+  }
+  esikf_destroy(ctx);
   return rc;
 }
 

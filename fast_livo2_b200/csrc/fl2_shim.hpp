@@ -242,6 +242,24 @@ struct SubSparseMap {
   std::vector<int> search_levels;
   std::vector<V3D> voxel_points_pos;           // voxel_points[i]->pos_
   std::vector<double> inv_expo_list;
+  std::vector<int> candidate_index;            // VIOManager::SelectSubSparseMap: the candidate each entry came from
+};
+
+// One candidate of VIOManager::SelectSubSparseMap: a visual point that passed the retrieval's depth-continuity check
+// (src/vio.cpp:614-640) and the reference feature chosen for it (:645-697). Inputs as esikf_vio_select_patches.
+struct SubMapCandidate {
+  int32_t ref_img_index;  // into VIOManager::SetReferenceImages
+  int32_t ref_level;      // Feature::level_ (depth form)
+  int32_t ref_key;        // Feature::id_, the warp_map key (depth form)
+  int32_t pad_;
+  double px_ref[2];       // Feature::px_
+  double ref_f[3];        // Feature::f_ (depth form)
+  double ref_pos[3];      // Feature::pos() (depth form)
+  double pos_w[3];        // VisualPoint::pos_
+  double normal_w[3];     // VisualPoint::normal_ (homography form)
+  double T_ref_w[12];     // Feature::T_f_w_ as R (row-major) and t
+  double ref_inv_expo;    // Feature::inv_expo_time_
+  double pc[2];           // new_frame_->w2c(pos_), computed by the retrieval at :614
 };
 
 struct GrayImage { const uint8_t *data = nullptr; int cols = 0, rows = 0; };  // cv::Mat CV_8UC1 continuous
@@ -259,8 +277,13 @@ class VIOManager {
   V3D Pcl;
   M3D extR;  // setImuToLidarExtrinsic / setLidarToCameraExtrinsic (src/vio.cpp:29-39)
   V3D extT;
+  // retrieval gate (LIVMapper.cpp:59,70; include/vio.h:101,109). ncc_thre has no default in the reference (the node never
+  // reads it and ncc_en stays false); 0 here, which rejects only anti-correlated patches when ncc_en is set.
+  bool normal_en = true, ncc_en = false;
+  double outlier_threshold = 1000, ncc_thre = 0;
   int last_status_ = 0;
   int last_total_iters_ = 0;  // iterations executed by the last computeJacobianAndUpdateEKF
+  int64_t submap_uploads_ = 0;  // sub-map uploads (esikf_vio_set_patches) made by computeJacobianAndUpdateEKF
   // The per-patch mirrors below are called once per point and level by the reference's retrieval code: the image they are
   // handed is uploaded only when it is not the one of the previous call (same pixel pointer and size). A caller that rewrites
   // the pixels in place calls InvalidatePatchImages().
@@ -270,6 +293,18 @@ class VIOManager {
   explicit VIOManager(esikf_ctx *shared_ctx);  // shares the device context (and stream) of the VoxelMapManager
   void initializeVIO();                         // src/vio.cpp:41-160 (the parts the update needs)
   void computeJacobianAndUpdateEKF(const GrayImage &img);  // include/vio.h:153
+  // Feature::img_ of the reference frames the candidates of SelectSubSparseMap address by ref_img_index.
+  void SetReferenceImages(const GrayImage *imgs, int n);
+  // The per-candidate tail of retrieveFromVisualSparseMap (src/vio.cpp:699-770) on the device for n candidates in grid-cell
+  // order, against the current frame `img` at pose T_cur_w (new_frame_->T_f_w_, R row-major then t) and state->inv_expo_time:
+  // warp form by normal_en, gates by outlier_threshold / ncc_en / ncc_thre. Fills visual_submap (voxel_points_pos,
+  // search_levels, inv_expo_list, errors, candidate_index; warp_patch stays empty, see MaterializeWarpPatches) and
+  // total_points. The warp patches stay on the device: the next computeJacobianAndUpdateEKF on the same visual_submap with
+  // the same total_points uploads only the image and the states.
+  void SelectSubSparseMap(const SubMapCandidate *candidates, int n, const GrayImage &img, const double T_cur_w[12]);
+  // Fills visual_submap->warp_patch of the last SelectSubSparseMap (the same patches the device holds), for callers that read
+  // them on the host. Idempotent per selection.
+  void MaterializeWarpPatches();
   // Per-patch helpers with the reference's signatures (include/vio.h:151, 161-162; V2D / Matrix2d as plain arrays). One
   // launch and one small read-back per call: the frame path should use the batched esikf_vio_get_image_patch /
   // esikf_vio_warp_patches.
@@ -285,6 +320,13 @@ class VIOManager {
   PinnedBuf<float> st_wp_, st_err_;
   PinnedBuf<int32_t> st_sl_;
   PinnedBuf<uint8_t> st_img_;
+  // the sub-map SelectSubSparseMap left on the device, and what MaterializeWarpPatches needs to rebuild its patches
+  const SubSparseMap *selected_submap_ = nullptr;
+  int selected_count_ = -1;
+  std::vector<int32_t> sel_ref_idx_, sel_sl_;
+  std::vector<double> sel_px_, sel_A_;
+  std::vector<GrayImage> ref_imgs_;  // SetReferenceImages (the caller keeps the pixels, as Feature::img_ does)
+  bool ref_imgs_current_ = false;    // false once the per-patch warpAffine replaced the device's reference images
 };
 
 }  // namespace fl2b200

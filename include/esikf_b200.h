@@ -286,7 +286,9 @@ int esikf_vio_update(esikf_ctx *ctx, const uint8_t *img, int32_t width, int32_t 
  *                  pc n x 2 f64 -> patch n x 64 f32 at `level`.
  * warp_patches   : batched getWarpMatrixAffineHomography + getBestSearchLevel + warpAffine over all
  *                  pyramid levels (src/vio.cpp:701-714, 739-742). Reference images are registered
- *                  once (Feature::img_, include/feature.h) and addressed by index. */
+ *                  once (Feature::img_, include/feature.h) and addressed by index. keep_on_device installs every warped
+ *                  patch with inv_expo 1 and gates nothing: callers that need the reference features' exposure times,
+ *                  the depth-form warp or the photometric / NCC gate use esikf_vio_select_patches instead. */
 int esikf_vio_get_image_patch(esikf_ctx *ctx, const double *pc, int32_t n, int32_t level, float *patch_out);
 int esikf_vio_set_ref_images(esikf_ctx *ctx, const uint8_t *const *imgs, int32_t n_imgs, int32_t width, int32_t height);
 int esikf_vio_warp_patches(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_index, const double *px_ref /* n x 2 */,
@@ -295,6 +297,35 @@ int esikf_vio_warp_patches(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_ind
                            const double *T_cur_w /* 12: new_frame_->T_f_w_ */, double *A_cur_ref_out /* n x 4, nullable */,
                            int32_t *search_level_out /* n */, float *warp_patch_out /* n x levels*64 */,
                            int32_t keep_on_device /* 1: also install as the patches of set_patches */);
+/* Gate settings of the sub-map selection (vio/ parameters, LIVMapper.cpp:59,70; include/vio.h:101,109). */
+typedef struct esikf_vio_select_cfg {
+  int32_t normal_en;         /* 1: homography warp (getWarpMatrixAffineHomography); 0: depth warp (getWarpMatrixAffine) */
+  int32_t ncc_en;            /* 1: reject candidates whose calculateNCC is below ncc_thre */
+  double ncc_thre;
+  double outlier_threshold;  /* reject candidates whose photometric error exceeds outlier_threshold * 64 */
+} esikf_vio_select_cfg;
+/* select_patches : the per-candidate tail of retrieveFromVisualSparseMap (src/vio.cpp:699-770) for n candidates in the
+ *                  caller's (grid-cell) order, whose reference feature the caller has chosen (:645-697): the warp matrix and
+ *                  search level (normal_en: homography form from pos_w / normal_w; else the depth form from ref_f /
+ *                  ref_pos / ref_level, cached per ref_key = Feature::id_ like warp_map: a candidate takes the matrix of
+ *                  the first candidate with its key), warpAffine on every pyramid level, the current patch at pc (level 0
+ *                  of the set_image image), the exposure-weighted error, the NCC gate and the outlier gate. The survivors,
+ *                  in candidate order, become the visual sub-map of the next esikf_vio_run (pos_w, warp patch, search level,
+ *                  inv_expo = ref_inv_expo, errors = the gate error); n_kept == 0 installs an empty sub-map.
+ *                  Per candidate: ref_img_index (into set_ref_images), px_ref (2) = Feature::px_, ref_level = Feature::level_,
+ *                  ref_f (3) = Feature::f_, ref_pos (3) = Feature::pos(), pos_w (3), normal_w (3), T_ref_w (12, R(9) t(3) of
+ *                  Feature::T_f_w_), ref_inv_expo = Feature::inv_expo_time_, ref_key, pc (2) = new_frame_->w2c(pos_w).
+ *                  ref_f / ref_pos / ref_level / ref_key may be null when normal_en is set, normal_w when it is not.
+ *                  Outputs hold room for n entries; only the first *n_kept are written: kept_index (candidate indices),
+ *                  error_out, search_level_out, A_cur_ref_out (4 each, row-major) and warp_patch_out (levels*64 each) are
+ *                  nullable. On an error return the installed sub-map is left as it was. */
+int esikf_vio_select_patches(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_index, const double *px_ref, const int32_t *ref_level,
+                             const double *ref_f, const double *ref_pos, const double *pos_w, const double *normal_w,
+                             const double *T_ref_w, const double *ref_inv_expo, const int32_t *ref_key, const double *pc,
+                             const double *T_cur_w /* 12 */, double inv_expo_time /* the current frame's, state->inv_expo_time */,
+                             const esikf_vio_select_cfg *cfg, int32_t *n_kept, int32_t *kept_index, float *error_out /* nullable */,
+                             int32_t *search_level_out /* nullable */, double *A_cur_ref_out /* nullable */,
+                             float *warp_patch_out /* nullable */);
 /* set_inverse_refs: what the inverse-compositional variant (src/vio.cpp:1327-1518) reads of every visual point's reference
  *                  feature (include/feature.h): image (index into set_ref_images), px_, f_ (unit bearing), the rotation
  *                  of T_f_w_ (row-major) and pos() = T_f_w_.inverse().translation(). n must equal the n of set_patches. */

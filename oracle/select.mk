@@ -1,0 +1,20 @@
+# The per-candidate tail of retrieveFromVisualSparseMap (src/vio.cpp:645-770) for the tests of esikf_vio_select_patches —
+# test infrastructure only.
+#   liborc_select.so              : the oracle's restatement (orc_select.cpp) linked with the parity oracle's translation units
+#   _ref/libfl2_ref_select.so     : the reference's own getWarpMatrixAffine / getBestSearchLevel / calculateNCC (ref_select.cpp
+#                                   over the driver ref_vio.cpp), built only where the reference source exists, like the
+#                                   other _ref libraries (see Makefile)
+# make -C oracle -f select.mk
+CXX = /usr/bin/g++
+REF = /root/reference
+REF_SELECT = $(if $(wildcard $(REF)/src/vio.cpp),_ref/libfl2_ref_select.so,)
+ORC = orc_lio.cpp orc_vio.cpp orc_capi.cpp
+
+all: liborc_select.so $(REF_SELECT)
+
+liborc_select.so: orc_select.cpp $(ORC) orc_math.hpp orc_lio.hpp orc_vio.hpp
+	$(CXX) -std=c++17 -fPIC -shared -fopenmp -O2 -ffp-contract=off -Wall -Wno-unused-variable -o $@ orc_select.cpp $(ORC)
+
+_ref/libfl2_ref_select.so: ref_select.cpp ref_vio.cpp $(wildcard ref_shim/*/*) $(wildcard ref_shim/*/*/*) $(REF)/src/vio.cpp $(REF)/src/frame.cpp $(REF)/src/visual_point.cpp $(REF)/src/voxel_map.cpp $(REF)/include/vio.h
+	mkdir -p _ref
+	$(CXX) -std=c++17 -O2 -ffp-contract=off -fPIC -shared -fopenmp -DMP_EN -DMP_PROC_NUM=4 -DROOT_DIR=\"/tmp/\" -w -I ref_shim -I $(REF)/include -o $@ ref_select.cpp
