@@ -186,6 +186,7 @@ struct esikf_ctx {
   bool scan_fresh = false;   // precompute pending
   esikf_lio_cfg lio_cfg{};
   DevBuf<double> ext_dev;    // extR(9) extT(3)
+  DevBuf<double> lio_slot_block;  // lane slots of the LIO kernels' L2-slot warps: [partial_blocks][LIO_L2_WARPS * 32][SLOT_D]
 
   // shared update state
   DevBuf<double> state_prop;             // [state 386 | prop 386] contiguous: one H2D copy per update
@@ -307,6 +308,43 @@ static void shard_of(int n, int rank, int nranks, int &begin, int &count) {
   count = base + (rank < rem ? 1 : 0);
 }
 
+// Dynamic shared memory and occupancy of the LIO kernels of one CTA geometry (L2W L2-slot warps), with their resources
+// under ESIKF_DEBUG. Returns the co-resident CTAs per SM of its persistent kernels.
+template <int L2W> static int lio_kernels_setup(bool debug) {
+  const int smem = (int)sizeof(LioSmem<L2W>), threads = LioSmem<L2W>::THREADS;
+  cudaFuncSetAttribute(lio_residual_kernel<L2W>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  cudaFuncSetAttribute(lio_update_kernel<false, L2W>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  cudaFuncSetAttribute(lio_update_kernel<true, L2W>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  int occ_l = 0, occ_lp = 0, occ_r = 0;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_l, lio_update_kernel<false, L2W>, threads, smem);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_lp, lio_update_kernel<true, L2W>, threads, smem);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_r, lio_residual_kernel<L2W>, threads, smem);
+  if (debug) {
+    cudaFuncAttributes fr, fu;
+    cudaFuncGetAttributes(&fr, lio_residual_kernel<L2W>);
+    cudaFuncGetAttributes(&fu, lio_update_kernel<false, L2W>);
+    fprintf(stderr, "[esikf] LIO %d lanes: smem=%d occupancy lio_update=%d/%d lio_residual=%d; lio_residual regs=%d local=%zu; lio_update regs=%d local=%zu\n", threads,
+            smem, occ_l, occ_lp, occ_r, fr.numRegs, fr.localSizeBytes, fu.numRegs, fu.localSizeBytes);
+  }
+  return occ_l < occ_lp ? occ_l : occ_lp;
+}
+
+// The 768-lane kernel (LIO_L2_WARPS L2-slot warps) runs where its lanes hold every CTA's slice and the 704 lanes of the other
+// one would not: 23 or 24 chunks of 32 points per CTA (config 2's 100 k points on 132 SMs). Smaller slices are resident in
+// 704 lanes too. A larger slice is tiled either way, and the 704-lane kernel tiles faster: its lanes all have shared-memory
+// slots, while the L2-slot lanes would be cold in every tile.
+static bool lio_use_l2_slots(int count, int grid) {
+  const int chunks = (count + 31) / 32, per_cta = (chunks + grid - 1) / grid;
+  return LIO_L2_WARPS > 0 && per_cta > LIO_SMEM_WARPS && per_cta <= LIO_SMEM_WARPS + LIO_L2_WARPS;
+}
+template <int L2W> static void launch_lio_residual(int grid, cudaStream_t st, const LioKernelArgs &ka) {
+  lio_residual_kernel<L2W><<<grid, LioSmem<L2W>::THREADS, sizeof(LioSmem<L2W>), st>>>(ka);
+}
+static void launch_lio_residual(bool l2_slots, int grid, cudaStream_t st, const LioKernelArgs &ka) {
+  if (l2_slots) launch_lio_residual<LIO_L2_WARPS>(grid, st, ka);
+  else launch_lio_residual<0>(grid, st, ka);
+}
+
 extern "C" {
 
 int esikf_create(esikf_ctx **out, int device) {
@@ -332,7 +370,7 @@ int esikf_create(esikf_ctx **out, int device) {
             ctx->scratch_state.reserve(S_N) == cudaSuccess;
   ctx->partial_blocks = ctx->sm_count < 160 ? ctx->sm_count : 160;  // persistent residual kernels: one CTA per SM
   ok = ok && ctx->partials.reserve((size_t)2 * ctx->partial_blocks * NE_MAX) == cudaSuccess && ctx->stamps.reserve(8 * 72 + 64 + 160) == cudaSuccess &&
-       ctx->barrier.reserve(128) == cudaSuccess;
+       ctx->barrier.reserve(128) == cudaSuccess && ctx->lio_slot_block.reserve((size_t)ctx->partial_blocks * LIO_L2_WARPS * 32 * SLOT_D) == cudaSuccess;
   if (ok) cudaMemsetAsync(ctx->barrier.p, 0, 128 * sizeof(unsigned int), ctx->stream);
   if (ok) {
     ctx->state = ctx->state_prop.p, ctx->prop = ctx->state_prop.p + S_N;
@@ -350,31 +388,22 @@ int esikf_create(esikf_ctx **out, int device) {
     delete ctx;
     return ESIKF_ERR_CUDA;
   }
-  cudaFuncSetAttribute(lio_residual_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(LioSmem));
   cudaFuncSetAttribute(vio_patch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(VioSmem));
   cudaFuncSetAttribute(vio_inverse_patch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(VioSmem));
-  cudaError_t ea = cudaFuncSetAttribute(lio_update_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(LioSmem));
-  cudaFuncSetAttribute(lio_update_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(LioSmem));
   cudaError_t eb = cudaFuncSetAttribute(vio_update_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)VIO_PERSIST_SMEM);
   cudaFuncSetAttribute(vio_update_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)VIO_PERSIST_SMEM);
   cudaFuncSetAttribute(vio_update_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)VIO_PERSIST_SMEM);
   cudaFuncSetAttribute(vio_update_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)VIO_PERSIST_SMEM);
   // the persistent kernels need every CTA co-resident: check what the device can hold
-  int occ_l = 0, occ_v = 0, occ_lp = 0, occ_vp = 0, occ_r = 0;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_l, lio_update_kernel<false>, LIO_THREADS, sizeof(LioSmem));
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_lp, lio_update_kernel<true>, LIO_THREADS, sizeof(LioSmem));
+  const bool debug = getenv("ESIKF_DEBUG") != nullptr;
+  const int occ_l0 = lio_kernels_setup<0>(debug), occ_l2 = lio_kernels_setup<LIO_L2_WARPS>(debug);
+  int occ_v = 0, occ_vp = 0;
   cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_v, vio_update_kernel<false, false>, VIO_THREADS, VIO_PERSIST_SMEM);
   cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_vp, vio_update_kernel<true, true>, VIO_THREADS, VIO_PERSIST_SMEM);
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_r, lio_residual_kernel, LIO_THREADS, sizeof(LioSmem));
-  ctx->coop_lio = occ_l < occ_lp ? occ_l : occ_lp, ctx->coop_vio = occ_v < occ_vp ? occ_v : occ_vp;
-  if (getenv("ESIKF_DEBUG")) {
-    fprintf(stderr, "[esikf] SMs=%d smem LIO=%zu VIO=%zu attr=%d/%d occupancy: lio_update=%d vio_update=%d lio_residual=%d coop=%d\n", ctx->sm_count, sizeof(LioSmem),
-            VIO_PERSIST_SMEM, (int)ea, (int)eb, occ_l, occ_v, occ_r, ctx->coop_ok);
+  ctx->coop_lio = occ_l0 < occ_l2 ? occ_l0 : occ_l2, ctx->coop_vio = occ_v < occ_vp ? occ_v : occ_vp;
+  if (debug) {
+    fprintf(stderr, "[esikf] SMs=%d smem VIO=%zu attr=%d occupancy: vio_update=%d coop=%d\n", ctx->sm_count, VIO_PERSIST_SMEM, (int)eb, occ_v, ctx->coop_ok);
     cudaFuncAttributes fa;
-    cudaFuncGetAttributes(&fa, lio_residual_kernel);
-    fprintf(stderr, "[esikf] lio_residual: regs=%d local=%zu\n", fa.numRegs, fa.localSizeBytes);
-    cudaFuncGetAttributes(&fa, lio_update_kernel<false>);
-    fprintf(stderr, "[esikf] lio_update: regs=%d local=%zu\n", fa.numRegs, fa.localSizeBytes);
     cudaFuncGetAttributes(&fa, vio_update_kernel<false, false>);
     fprintf(stderr, "[esikf] vio_update: regs=%d local=%zu\n", fa.numRegs, fa.localSizeBytes);
   }
@@ -945,6 +974,7 @@ static int lio_fill_args(esikf_ctx *ctx, LioKernelArgs &ka, double *state_ptr) {
   ka.prob_sure_sigma = prob_sure_sigma_of(ka.sigma_num);
   ka.match_plane = ctx->match_plane.p, ka.normal_plane = ctx->normal_plane.p, ka.dis_to_plane = ctx->dis.p;
   ka.partials = ctx->partials.p, ka.info = ctx->info.p, ka.ctrl = ctx->ctrl;
+  ka.slot_block = ctx->lio_slot_block.p;
   return 0;
 }
 static int lio_grid(const esikf_ctx *ctx, int count) {
@@ -986,7 +1016,7 @@ static bool persistent_update(const esikf_ctx *ctx, int coop_blocks) {
   return ctx->loop_mode >= 1 && (ctx->nranks == 1 || ctx->p2p) && ctx->coop_ok && coop_blocks > 0 && !ctx->timing;
 }
 
-// Cooperative launch of lio_update_kernel<PEER> / vio_update_kernel<PEER, INVERSE>. Their arguments are
+// Cooperative launch of lio_update_kernel<PEER, L2W> / vio_update_kernel<PEER, INVERSE>. Their arguments are
 // (ka, sa, barrier, barrier_next, stamps, parity_stride, peer, tail...): `ka` is the kernel's LioKernelArgs /
 // VioKernelArgs, `tail` the VIO-only arguments. Both instantiations get the same argument list, so the single-GPU
 // launch passes exactly what the peer launch does. `stamp_off` / `stamp_words`: this kernel's slice of the phase stamps.
@@ -1039,16 +1069,20 @@ int esikf_lio_run(esikf_ctx *ctx, const double *state_in, const double *state_pr
   SolveArgs sa = solve_args(ctx, ctx->state, cfg->max_iterations);
   sa.lio_stats = ctx->lio_stats;
   const int grid = lio_grid(ctx, ka.count);
+  const bool l2_slots = lio_use_l2_slots(ka.count, grid);
+  if (fused_lio && l2_slots)
+    return launch_persistent(ctx, (const void *)lio_update_kernel<false, LIO_L2_WARPS>, (const void *)lio_update_kernel<true, LIO_L2_WARPS>, "lio_update_kernel", grid,
+                             LioSmem<LIO_L2_WARPS>::THREADS, sizeof(LioSmem<LIO_L2_WARPS>), &ka, sa, 0, 64, ctx->lio_timed, {});
   if (fused_lio)
-    return launch_persistent(ctx, (const void *)lio_update_kernel<false>, (const void *)lio_update_kernel<true>, "lio_update_kernel", grid, LIO_THREADS,
-                             sizeof(LioSmem), &ka, sa, 0, 64, ctx->lio_timed, {});
+    return launch_persistent(ctx, (const void *)lio_update_kernel<false, 0>, (const void *)lio_update_kernel<true, 0>, "lio_update_kernel", grid, LioSmem<0>::THREADS,
+                             sizeof(LioSmem<0>), &ka, sa, 0, 64, ctx->lio_timed, {});
   ctx->lio_timed = ctx->timing;
   ctx->lio_slots = cfg->max_iterations;
   for (int it = 0; it < cfg->max_iterations; it++) {
     cudaEvent_t *e = ctx->timing ? timing_events(ctx, EV_LIO_BASE, it) : nullptr;
     if (e) cudaEventRecord(e[0], st);
     ka.init_normal = (it == 0);
-    lio_residual_kernel<<<grid, LIO_THREADS, sizeof(LioSmem), st>>>(ka);
+    launch_lio_residual(l2_slots, grid, st, ka);
     if (e) cudaEventRecord(e[1], st);
     int rc = allreduce_info(ctx);
     if (rc) return rc;
@@ -1708,7 +1742,7 @@ int esikf_profile_kernel(esikf_ctx *ctx, int32_t which, int32_t arg, int32_t rep
       CK(cudaMemsetAsync(ctx->ctrl, 0, sizeof(Ctrl), st));
     }
     CK(cudaEventRecord(e0, st));
-    if (which == 0) lio_residual_kernel<<<grid, LIO_THREADS, sizeof(LioSmem), st>>>(la);
+    if (which == 0) launch_lio_residual(lio_use_l2_slots(la.count, grid), grid, st, la);
     else if (which == 1) lio_solve_kernel<<<1, SOLVE_THREADS, 0, st>>>(sa);
     else if (which == 2) vio_patch_kernel<<<grid, VIO_THREADS, sizeof(VioSmem), st>>>(va);
     else lio_precompute_kernel<<<(ctx->n_pts + 255) / 256, 256, 0, st>>>(ctx->pts.p, ctx->n_pts, ctx->pre.p, ctx->pre_stride, ctx->ext_dev.p, (float)ctx->lio_cfg.dept_err,

@@ -194,11 +194,11 @@ template <bool PEER> __device__ __forceinline__ void persist_epilogue(FusedSolve
   }
 }
 
-template <bool PEER>
-__global__ void __launch_bounds__(LIO_THREADS, 1) lio_update_kernel(const LioKernelArgs a, const SolveArgs sa_in, unsigned int *barrier, unsigned int *barrier_next, unsigned long long *stamps,
+template <bool PEER, int L2W>
+__global__ void __launch_bounds__(LioSmem<L2W>::THREADS, 1) lio_update_kernel(const LioKernelArgs a, const SolveArgs sa_in, unsigned int *barrier, unsigned int *barrier_next, unsigned long long *stamps,
                                                                      size_t partial_parity_stride, const PeerArgs peer) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  LioSmem &sm = *reinterpret_cast<LioSmem *>(smem_raw);
+  LioSmem<L2W> &sm = *reinterpret_cast<LioSmem<L2W> *>(smem_raw);
   static_assert(sizeof(FusedSolveSmem) <= sizeof(sm.fs_raw), "solve state must fit");
   static_assert(sizeof(SolveLiteralScratch) <= sizeof(sm.rec), "literal scratch must fit in the record slots");
   FusedSolveSmem &fs = *reinterpret_cast<FusedSolveSmem *>(sm.fs_raw);
@@ -207,7 +207,7 @@ __global__ void __launch_bounds__(LIO_THREADS, 1) lio_update_kernel(const LioKer
   unsigned int epoch = 0;
   int lo, hi;
   lio_block_range(a.count, lo, hi);
-  unsigned int seq = persist_prologue<6, LIO_WARPS, PEER>(fs, lit, sa, barrier_next, peer, 1.0, [&]() {
+  unsigned int seq = persist_prologue<6, LioSmem<L2W>::WARPS, PEER>(fs, lit, sa, barrier_next, peer, 1.0, [&]() {
     lio_prior_consts(sm, a);  // never change inside the loop
     lio_init_cold(sm, a);
     lio_init_barriers(sm);    // fs.sm.P is in place
@@ -229,7 +229,7 @@ __global__ void __launch_bounds__(LIO_THREADS, 1) lio_update_kernel(const LioKer
       if (threadIdx.x == 0) stamps[640 + blockIdx.x] = globaltimer_ns();
     }
     stamp(stamps, sk);  // 2: this CTA's warps issued their slice (CTA 0 / thread 0)
-    persist_exchange<LIO_WARPS, 6, PEER>(fs, sm.red, D0, D1, (double)cnt, a.partials + (size_t)(it & 1) * partial_parity_stride, a.partial_stride, barrier, epoch, peer,
+    persist_exchange<LioSmem<L2W>::WARPS, 6, PEER>(fs, sm.red, D0, D1, (double)cnt, a.partials + (size_t)(it & 1) * partial_parity_stride, a.partial_stride, barrier, epoch, peer,
                                          seq, stamps, sk);  // 3: all CTAs arrived
     stamp(stamps, sk);  // 4: information vector complete
     sa.dbg = (stamps && blockIdx.x == 0) ? stamps + sk + 1 : nullptr;  // 6: gain rows done, 7: boxplus done

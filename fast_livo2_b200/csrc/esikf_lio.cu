@@ -6,12 +6,15 @@
 //                           covariance, :643-786 voxel probe + plane association, :414-458 Jacobian / R^-1) fused with the
 //                           H^T R^-1 H, H^T R^-1 z reduction (:464-466). No PointToPlane is ever materialised.
 //
-// Mapping: one thread per LiDAR point, 22 warps per CTA, one CTA per SM. A CTA whose slice fits its 704 lanes keeps it
-// resident across iterations; on 132 SMs that holds up to 92.9 k points. Config 2's 100 k points give every CTA 23 or 24
-// chunks of 32, so every CTA streams its slice in two tiles and nothing stays resident (see DESIGN.md §8).
-// Every lane owns a 304-byte shared-memory slot for the whole update: the plane record of its point's voxel (brought in by
-// ONE cp.async.bulk per lane, completion counted on a per-warp mbarrier), the point's body covariance, and everything
-// about the (point, plane) pair that does not change from one iteration to the next:
+// Mapping: one thread per LiDAR point, one CTA per SM, 22 or 24 warps per CTA (chosen per launch). A CTA whose slice fits
+// its lanes keeps it resident across iterations. With 704 lanes that holds up to 92.9 k points on 132 SMs. The 768-lane
+// kernel holds up to 101 k, so config 2's 100 k points (23 or 24 chunks of 32 per CTA) stay resident, and it runs only for
+// such slices. Slices of more than 24 chunks per CTA are streamed by the 704-lane kernel in tiles of 704 (DESIGN.md §8).
+// Every lane owns a 304-byte slot for the whole update: in shared memory for warps 0-21, in an L2-resident per-CTA block of
+// global memory for warps 22-23 (24 shared slots per lane would need 233 KB, more than a block may use). A slot holds the
+// plane record of its point's voxel (brought in by ONE cp.async.bulk per lane, completion counted on a per-warp mbarrier;
+// coalesced __ldg copies into global slots), the point's body covariance, and everything about the (point, plane) pair
+// that does not change from one iteration to the next:
 //   * the voxel key / candidate range (no hash probe while the point stays in its voxel),
 //   * u^T P_rot u + n^T P_pos n, the state-covariance part of n^T var n (state_.cov is constant inside the loop, :377-389),
 //   * R_inv, which the reference evaluates with the PRIOR pose (:425-449) and therefore repeats unchanged every iteration.
@@ -33,8 +36,15 @@ namespace esikf {
 #ifndef LIO_FULL_REC
 #define LIO_FULL_REC 0  // cold candidates: head first, covariance part after the range gate (0, default) or the whole record in one round trip (1). The one-trip form saves an L2 round trip but keeps 18 more registers live
 #endif
-#define LIO_THREADS 704  // 22 warps, one CTA per SM: 132 x 704 = 93k points in a single round
-#define LIO_WARPS (LIO_THREADS / 32)
+// One CTA per SM, in one of two geometries chosen per launch (lio_use_l2_slots in esikf_api.cu). Warps [0, LIO_SMEM_WARPS)
+// keep their lane slots in shared memory; 22 x 32 slots of 304 B is what fits next to the rest of LioSmem. The 768-lane
+// kernel adds LIO_L2_WARPS warps ("L2-slot warps") that keep theirs in a per-CTA block of global memory, which stays in L2
+// for the whole update: 132 x 768 = 101 k points resident on H100. It runs only where it makes a slice resident that the
+// 704-lane kernel (132 x 704 = 92.9 k) would tile. -DLIO_L2_WARPS=0 leaves only the 704-lane kernel (A/B measurements).
+#ifndef LIO_L2_WARPS
+#define LIO_L2_WARPS 2
+#endif
+#define LIO_SMEM_WARPS 22
 
 struct LioKernelArgs {
   const float *pts;          // [n_total][3] body-frame scan
@@ -62,6 +72,7 @@ struct LioKernelArgs {
   Ctrl *ctrl;
   int init_normal;           // first iteration of an update: unmatched points get normal_plane = -1 (pv.normal = 0)
   int stage_mode;            // 0: cp.async.bulk per lane (default), 1: coalesced half-warp __ldg copies (measurement variant)
+  double *slot_block;        // [gridDim.x][LIO_L2_WARPS * 32][SLOT_D]: lane slots of the L2-slot warps
 };
 
 // What the out-of-line cold paths need of the kernel arguments, passed BY VALUE: taking the address of the kernel-parameter
@@ -170,16 +181,34 @@ __device__ __forceinline__ void slot_point(const double *slot, float &px, float 
   px = xy.x, py = xy.y, pz = reinterpret_cast<const float *>(slot + SL_ROW + 8)[1];
 }
 
-// shared-memory layout of the residual kernel
-struct __align__(128) LioSmem {
-  double rec[LIO_WARPS][32][SLOT_D];
+// shared-memory layout of the LIO kernels: the part every CTA geometry shares, then (LioSmem<L2W>) the reduction scratch
+// of its warps, the persistent kernel's solve state and the pointer to the CTA's global slots
+struct LioSmemCore {
+  double rec[LIO_SMEM_WARPS][32][SLOT_D];
   double R[9], t[3], Ptt[9], Ppp[9];      // current state
   double Rp[9], tp[3], Mp[9];             // prior pose, Mp = Rp * extR
   LioCold cold;                           // what the out-of-line cold paths read of the kernel arguments
-  unsigned long long mbar[LIO_WARPS];     // one bulk-copy barrier per warp
-  ReduceSmem<LIO_WARPS> red;
-  unsigned char fs_raw[8704];             // the CTA's resident solve state (FusedSolveSmem) in the persistent kernel
+  unsigned long long mbar[LIO_SMEM_WARPS];  // one bulk-copy barrier per shared-slot warp
 };
+// L2W: number of L2-slot warps of the CTA (0: the 704-lane kernel, LIO_L2_WARPS: the 768-lane one)
+template <int L2W> struct __align__(128) LioSmem : LioSmemCore {
+  static constexpr int L2_WARPS = L2W, WARPS = LIO_SMEM_WARPS + L2W, THREADS = WARPS * 32;
+  ReduceSmem<WARPS> red;
+  unsigned char fs_raw[8704];             // the CTA's resident solve state (FusedSolveSmem) in the persistent kernel
+  double (*l2_slots)[32][SLOT_D];         // this CTA's part of LioKernelArgs::slot_block, one [32][SLOT_D] per L2-slot warp
+};
+static_assert(sizeof(LioSmem<LIO_L2_WARPS>) <= 232448, "LioSmem must fit the 227 KB of shared memory a block may use on sm_90");
+
+// The slots of warp `warp`, in shared memory (L2 = false: LDS / STS on every access) or in the CTA's global slot block
+// (L2 = true). The space is a template parameter, not a run-time choice: a pointer that may point to either would make every
+// slot access of the hot path a generic load / store.
+template <bool L2, class Sm> __device__ __forceinline__ double (*lane_slots(Sm &sm, int warp))[SLOT_D] {
+  if constexpr (L2) return sm.l2_slots[warp - LIO_SMEM_WARPS];
+  else return sm.rec[warp];
+}
+template <bool L2, class Sm> __device__ __forceinline__ const double (*lane_slots(const Sm &sm, int warp))[SLOT_D] {
+  return lane_slots<L2>(const_cast<Sm &>(sm), warp);
+}
 
 // What a lane keeps about ITS point across the iterations of a persistent update (registers); the rest is in its slot.
 struct LaneCache {
@@ -200,7 +229,7 @@ __device__ __forceinline__ void lane_cache_init(LaneCache &lc) {
 
 // Prior-pose constants (voxel_map.cpp:425-428): Rp, tp and Mp = Rp * extR (state_propagat.rot_end * extR_, :445).
 // No barrier: the caller's next one publishes them.
-__device__ __forceinline__ void lio_prior_consts(LioSmem &sm, const LioKernelArgs &a) {
+__device__ __forceinline__ void lio_prior_consts(LioSmemCore &sm, const LioKernelArgs &a) {
   const int tid = threadIdx.x;
   if (tid < 9) {
     const int r = tid / 3, c = tid % 3;
@@ -216,7 +245,7 @@ __device__ __forceinline__ void lio_prior_consts(LioSmem &sm, const LioKernelArg
 // Current-pose constants: R, t of the packed state `st`, and the covariance blocks Ptt / Ppp of P (19 x 19) that pv.var
 // uses (:377-378; state_.cov only changes after the loop, :489: P == nullptr keeps the blocks already in place). global: st
 // and P are the update's state in global memory, else the CTA's resident copies. Ends with a CTA barrier.
-__device__ __forceinline__ void lio_pose_consts(LioSmem &sm, const double *st, const double *P, bool global) {
+__device__ __forceinline__ void lio_pose_consts(LioSmemCore &sm, const double *st, const double *P, bool global) {
   const int tid = threadIdx.x;
   if (tid < 9) {
     const int r = tid / 3, c = tid % 3;
@@ -325,7 +354,7 @@ struct EvalOut {
   float dis, dis_to_plane;
 };
 __device__ __forceinline__ EvalOut eval_cold(const double *__restrict__ q, const double pw[3], const double *bc, double cx, double cy, double cz,
-                                             const LioSmem &sm, double sigma_num) {
+                                             const LioSmemCore &sm, double sigma_num) {
   EvalOut o;
   o.pass = false, o.sigma_l = 0.0, o.dis = 0.f, o.dis_to_plane = 0.f;
 #if !LIO_FULL_REC
@@ -399,7 +428,7 @@ __device__ __forceinline__ void pair_of(const PairLayout &L, int k, int &owner, 
 // probabilities: a point whose candidates pass at most once in total needs none as long as that candidate's this_prob is
 // sure to be > 0 (prob_sure_sigma_of; it then wins, :741-768). unsure: some passing extra of the warp is not sure of it.
 // Points with two or more passing candidates, or an unsure one, go through warp_eval_extras_prob.
-__device__ __forceinline__ void warp_eval_extras_count(const LioCold &a, const LioSmem &sm, const double (*wslots)[SLOT_D], bool pending, const double pw[3],
+__device__ __forceinline__ void warp_eval_extras_count(const LioCold &a, const LioSmemCore &sm, const double (*wslots)[SLOT_D], bool pending, const double pw[3],
                                                        double cx, double cy, double cz, uint32_t first, uint32_t count, int lane, int &npass, int &fidx, float &fdis,
                                                        bool &unsure) {
   npass = 0, fidx = -1, fdis = 0.f, unsure = false;
@@ -440,7 +469,7 @@ __device__ __forceinline__ void warp_eval_extras_count(const LioCold &a, const L
 // Pass 2, only for lanes with two or more passing candidates: winner = arg-max probability with lowest-index tie break,
 // merged with `best` (the first candidate's result) by strict '>' — exactly the order-dependent rule of the recursion
 // (voxel_map.cpp:741: the first of equal probabilities is kept).
-__device__ __forceinline__ void warp_eval_extras_prob(const LioCold &a, const LioSmem &sm, const double (*wslots)[SLOT_D], bool pending, const double pw[3],
+__device__ __forceinline__ void warp_eval_extras_prob(const LioCold &a, const LioSmemCore &sm, const double (*wslots)[SLOT_D], bool pending, const double pw[3],
                                                       double cx, double cy, double cz, uint32_t first, uint32_t count, int lane, Cand &best) {
   const PairLayout L = pair_layout(pending, count, lane);
   if (!L.mask) return;
@@ -486,7 +515,7 @@ __device__ __forceinline__ void warp_eval_extras_prob(const LioCold &a, const Li
 // sd0, dtp0) — evaluated by the caller, from the slot or cold —, the extras are counted lane-parallel; probabilities are
 // evaluated only where two or more candidates pass or a passing one may have this_prob == 0. On return best_idx / best_dis
 // hold the winner (or -1: none passed, or none with this_prob > 0), passed whether any candidate passed (is_sucess).
-__device__ LIO_COLD void resolve_voxel(const LioCold &a, const LioSmem &sm, const double (*wslots)[SLOT_D], bool act, const double pw[3], double cx, double cy,
+__device__ LIO_COLD void resolve_voxel(const LioCold &a, const LioSmemCore &sm, const double (*wslots)[SLOT_D], bool act, const double pw[3], double cx, double cy,
                                               double cz, uint32_t first, uint32_t count, bool pass0, double sigma0, float dis0, float dtp0, int lane, int &best_idx,
                                               float &best_dis, bool &passed) {
   const bool pend = act && count > 1;
@@ -548,10 +577,12 @@ struct AssocOut {
 // voxel gave nothing (voxel_map.cpp:680-691). loc is in voxel units, centre / quarter length in metres: reproduced
 // literally. Called by the whole warp. flags: 1 = extras pending, 2 = home voxel exists, 4 = its first candidate passed,
 // 8 = the lane matched its single-candidate home voxel on the hot path.
-__device__ LIO_COLD AssocOut lio_cold_assoc(const LioSmem &sm, int warp, int lane, unsigned flags, float pwx, float pwy, float pwz, uint32_t first, uint32_t count,
+template <bool L2, class Sm>
+__device__ LIO_COLD AssocOut lio_cold_assoc(const Sm &sm, int warp, int lane, unsigned flags, float pwx, float pwy, float pwz, uint32_t first, uint32_t count,
                                             double sigma0, float dis0, float dtp0) {
   const LioCold &a = sm.cold;
-  const double *slot = &sm.rec[warp][lane][0];
+  const double(*const ws)[SLOT_D] = lane_slots<L2>(sm, warp);
+  const double *slot = &ws[lane][0];
   float px, py, pz;
   slot_point(slot, px, py, pz);
   const bool pend1 = flags & 1u, found_home = flags & 2u, pass0 = flags & 4u;
@@ -561,7 +592,7 @@ __device__ LIO_COLD AssocOut lio_cold_assoc(const LioSmem &sm, int warp, int lan
   int bi = (flags & 8u) ? (int)first : -1;
   float bd = (flags & 8u) ? dis0 : 0.f;
   bool passed = pass0;  // is_sucess of the home voxel
-  resolve_voxel(a, sm, sm.rec[warp], pend1, pw, cx, cy, cz, first, count, pass0, sigma0, dis0, dtp0, lane, bi, bd, passed);
+  resolve_voxel(a, sm, ws, pend1, pw, cx, cy, cz, first, count, pass0, sigma0, dis0, dtp0, lane, bi, bd, passed);
   uint32_t f2 = 0, c2 = 0;
   bool found2 = false;
   EvalOut e2;
@@ -582,19 +613,22 @@ __device__ LIO_COLD AssocOut lio_cold_assoc(const LioSmem &sm, int warp, int lan
     if (found2) e2 = eval_cold(reinterpret_cast<const double *>(a.recs + f2), pw, slot + SL_BC, cx, cy, cz, sm, a.sigma_num);
   }
   if (__any_sync(0xffffffffu, found2))
-    resolve_voxel(a, sm, sm.rec[warp], found2, pw, cx, cy, cz, f2, c2, e2.pass, e2.sigma_l, e2.dis, e2.dis_to_plane, lane, bi, bd, passed);
+    resolve_voxel(a, sm, ws, found2, pw, cx, cy, cz, f2, c2, e2.pass, e2.sigma_l, e2.dis, e2.dis_to_plane, lane, bi, bd, passed);
   AssocOut o;
   o.idx = bi, o.dis = bd;
   return o;
 }
 
 // Cold: bring the first candidate record of the lanes' (new) voxels into their slots and evaluate the record-dependent
-// invariant u^T P_rot u + n^T P_pos n. Called by the whole warp when at least one lane wants a record.
-__device__ LIO_COLD void lio_cold_stage(LioSmem &sm, int warp, int lane, bool want, int cand0, unsigned wmask, unsigned mphase) {
+// invariant u^T P_rot u + n^T P_pos n. Called by the whole warp when at least one lane wants a record. The slots of L2-slot
+// warps take the __ldg copy (a bulk copy needs a shared-memory destination) and use no mbarrier phase.
+template <bool L2, class Sm> __device__ LIO_COLD void lio_cold_stage(Sm &sm, int warp, int lane, bool want, int cand0, unsigned wmask, unsigned mphase) {
   const LioCold &a = sm.cold;
-  double *slot = &sm.rec[warp][lane][0];
+  double(*const ws)[SLOT_D] = lane_slots<L2>(sm, warp);
+  double *slot = &ws[lane][0];
   const double keep_out = slot[SL_OUT];  // the record image covers this word
-  if (a.stage_mode == 0) {
+  if constexpr (L2) __syncwarp();  // global slots: order the read above before the other lanes' copies into this slot
+  if (!L2 && a.stage_mode == 0) {
     // one bulk copy (TMA engine) per lane on the warp's mbarrier; the slot may have been read through the generic proxy before
     unsigned long long *bar = &sm.mbar[warp];
     fence_proxy_async_smem();
@@ -612,7 +646,7 @@ __device__ LIO_COLD void lio_cold_stage(LioSmem &sm, int warp, int lane, bool wa
       const int pidx = __shfl_sync(0xffffffffu, want ? cand0 : -1, src);
       if (pidx >= 0 && sub < 9) {
         const double2 v = __ldg(reinterpret_cast<const double2 *>(a.recs + pidx) + sub);
-        *reinterpret_cast<double2 *>(&sm.rec[warp][src][2 * sub]) = v;
+        *reinterpret_cast<double2 *>(&ws[src][2 * sub]) = v;
       }
     }
     __syncwarp();
@@ -645,8 +679,8 @@ __device__ LIO_COLD void lio_cold_point(const float *__restrict__ pts, const dou
 // Cold (once per point and matched plane): R_inv = 1 / (0.001 + sigma_l + n^T var n) with the PRIOR pose (:425-449):
 // point_world = Rp p_imu + tp, var = (Rp extR) body_cov (Rp extR)^T  =>  n^T var n = m^T body_cov m, m = Mp^T n.
 // Iteration-invariant, cached in the slot together with the plane it belongs to.
-__device__ LIO_COLD double lio_cold_wgt(LioSmem &sm, int warp, int lane, const double *__restrict__ q, int plane_idx) {
-  double *slot = &sm.rec[warp][lane][0];
+template <bool L2, class Sm> __device__ LIO_COLD double lio_cold_wgt(Sm &sm, int warp, int lane, const double *__restrict__ q, int plane_idx) {
+  double *slot = &lane_slots<L2>(sm, warp)[lane][0];
   float px, py, pz;
   slot_point(slot, px, py, pz);
   double pi0, pi1, pi2;
@@ -666,27 +700,31 @@ __device__ LIO_COLD double lio_cold_wgt(LioSmem &sm, int warp, int lane, const d
 #define LIO_PHASE_FENCE() asm volatile("" ::: "memory")  // keeps the next phase's shared-memory loads from being hoisted (register pressure)
 
 // Kernel start: the slice of the kernel arguments the cold paths read, into shared memory.
-__device__ __forceinline__ void lio_init_cold(LioSmem &sm, const LioKernelArgs &a) {
+template <class Sm> __device__ __forceinline__ void lio_init_cold(Sm &sm, const LioKernelArgs &a) {
   if (threadIdx.x == 0) {
     LioCold &c = sm.cold;
     c.recs = a.recs, c.slots = a.slots, c.hash_mask = a.hash_mask, c.voxel_size_f = a.voxel_size_f, c.sigma_num = a.sigma_num, c.prob_sure_sigma = a.prob_sure_sigma;
     c.voxel_size = a.voxel_size, c.inv_voxel_size = a.inv_voxel_size, c.inv_voxel_exact = a.inv_voxel_exact, c.stage_mode = a.stage_mode;
     for (int k = 0; k < 9; k++) c.extR[k] = a.extR[k];
     for (int k = 0; k < 3; k++) c.extT[k] = a.extT[k];
+    if constexpr (Sm::L2_WARPS > 0) sm.l2_slots = reinterpret_cast<double(*)[32][SLOT_D]>(a.slot_block) + (size_t)blockIdx.x * Sm::L2_WARPS;
   }
 }
 
 // Residual / Jacobian build over the points [lo, hi) of this rank's shard (indices local to the shard), accumulated into
 // the calling warp's 8x8 tensor-core block (D0, D1) and matched-point count. The CTA walks its block in tiles of
-// LIO_THREADS points; with a single tile (the resident case) a lane keeps its point, its slot and `lc` for the whole update.
+// Sm::THREADS points; with a single tile (the resident case) a lane keeps its point, its slot and `lc` for the whole update.
 // write_out: store the per-point outputs (match_plane / dis_to_plane / normal_plane) of this pass to global memory; the
 // persistent kernel defers that to its last iteration when the slice is resident (lc.out_* carry the values).
-__device__ __forceinline__ void lio_process_range(const LioKernelArgs &a, LioSmem &sm, int lo, int hi, double &D0, double &D1, int &cnt,
-                                                  LaneCache &lc, bool init_normal, bool write_out) {
+// L2: the calling warp is an L2-slot warp (lane_slots).
+template <bool L2, class Sm>
+__device__ __forceinline__ void lio_process_slots(const LioKernelArgs &a, Sm &sm, int lo, int hi, double &D0, double &D1, int &cnt, LaneCache &lc,
+                                                  bool init_normal, bool write_out) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  double *const slot = &sm.rec[warp][lane][0];
-  const bool resident = (hi - lo <= LIO_THREADS);
-  for (int base = lo; base < hi; base += LIO_THREADS) {
+  double(*const ws)[SLOT_D] = lane_slots<L2>(sm, warp);
+  double *const slot = &ws[lane][0];
+  const bool resident = (hi - lo <= Sm::THREADS);
+  for (int base = lo; base < hi; base += Sm::THREADS) {
     const int li = base + tid;
     const bool valid = li < hi;
     const int i = a.begin + li;
@@ -745,8 +783,8 @@ __device__ __forceinline__ void lio_process_range(const LioKernelArgs &a, LioSme
       const bool want = cand0 >= 0 && cand0 != lc.staged_idx;
       const unsigned wmask = __ballot_sync(0xffffffffu, want);
       if (wmask) {
-        lio_cold_stage(sm, warp, lane, want, cand0, wmask, lc.mphase);
-        if (a.stage_mode == 0) lc.mphase ^= 1u;
+        lio_cold_stage<L2>(sm, warp, lane, want, cand0, wmask, lc.mphase);
+        if (!L2 && a.stage_mode == 0) lc.mphase ^= 1u;
         if (want) lc.staged_idx = cand0;
       }
     }
@@ -776,7 +814,7 @@ __device__ __forceinline__ void lio_process_range(const LioKernelArgs &a, LioSme
     const bool pend1 = have0 && count > 1;
     const bool need_nb = valid && found && !pend1 && !pass0;  // for pend1 lanes: decided after their extras
     if (__any_sync(0xffffffffu, pend1 || need_nb)) {  // cold: narrow arguments, everything else comes from shared memory
-      const AssocOut ao = lio_cold_assoc(sm, warp, lane, (pend1 ? 1u : 0u) | ((valid && found) ? 2u : 0u) | (pass0 ? 4u : 0u) | (best_idx >= 0 ? 8u : 0u),
+      const AssocOut ao = lio_cold_assoc<L2>(sm, warp, lane, (pend1 ? 1u : 0u) | ((valid && found) ? 2u : 0u) | (pass0 ? 4u : 0u) | (best_idx >= 0 ? 8u : 0u),
                                          (float)pw[0], (float)pw[1], (float)pw[2], first, count, sigma0, dis0, dtp0);
       best_idx = ao.idx, best_dis = ao.dis;
     }
@@ -796,7 +834,7 @@ __device__ __forceinline__ void lio_process_range(const LioKernelArgs &a, LioSme
         m0 = sm.R[0] * rn0 + sm.R[3] * rn1 + sm.R[6] * rn2, m1 = sm.R[1] * rn0 + sm.R[4] * rn1 + sm.R[7] * rn2, m2 = sm.R[2] * rn0 + sm.R[5] * rn1 + sm.R[8] * rn2;
       }
       const double2 sw = *reinterpret_cast<const double2 *>(slot + SL_SPP);  // {spp, wgt}
-      wgt = (reinterpret_cast<const int *>(slot + SL_META)[1] == best_idx) ? sw.y : lio_cold_wgt(sm, warp, lane, q, best_idx);
+      wgt = (reinterpret_cast<const int *>(slot + SL_META)[1] == best_idx) ? sw.y : lio_cold_wgt<L2>(sm, warp, lane, q, best_idx);
       float px, py, pz;
       slot_point(slot, px, py, pz);
       double pi0, pi1, pi2;
@@ -839,7 +877,7 @@ __device__ __forceinline__ void lio_process_range(const LioKernelArgs &a, LioSme
       double E0 = 0.0, E1 = 0.0;  // second accumulator pair: two independent DMMA chains per tile
 #pragma unroll
       for (int s = 0; s < 8; s++) {
-        const double *r = &sm.rec[warp][4 * s + t][SL_ROW];
+        const double *r = &ws[4 * s + t][SL_ROW];
         const double wv = r[7];
         const double v = (g == 7) ? ((wv != 0.0) ? 1.0 : 0.0) : r[g];  // a_7 = 1 for matched rows (R_inv > 0), else 0
         const double b = (g == 7) ? (double)fabsf(reinterpret_cast<const float *>(r + 8)[0]) : wv * v;
@@ -851,13 +889,25 @@ __device__ __forceinline__ void lio_process_range(const LioKernelArgs &a, LioSme
     __syncwarp();
   }
 }
+// The warp index is uniform across a warp: each warp runs the instantiation for the space of its slots.
+template <class Sm>
+__device__ __forceinline__ void lio_process_range(const LioKernelArgs &a, Sm &sm, int lo, int hi, double &D0, double &D1, int &cnt, LaneCache &lc,
+                                                  bool init_normal, bool write_out) {
+  if constexpr (Sm::L2_WARPS > 0) {
+    if ((int)(threadIdx.x >> 5) >= LIO_SMEM_WARPS) {
+      lio_process_slots<true>(a, sm, lo, hi, D0, D1, cnt, lc, init_normal, write_out);
+      return;
+    }
+  }
+  lio_process_slots<false>(a, sm, lo, hi, D0, D1, cnt, lc, init_normal, write_out);
+}
 
 // Per-point outputs of a resident slice, written once after the last iteration of the persistent kernel.
-__device__ __forceinline__ void lio_write_outputs(const LioKernelArgs &a, const LioSmem &sm, int lo, int hi, const LaneCache &lc) {
+template <class Sm> __device__ __forceinline__ void lio_write_outputs(const LioKernelArgs &a, const Sm &sm, int lo, int hi, const LaneCache &lc) {
   const int li = lo + threadIdx.x;
-  if (li < hi && hi - lo <= LIO_THREADS && lc.out_valid) {
-    const int i = a.begin + li;
-    const double *slot = &sm.rec[threadIdx.x >> 5][threadIdx.x & 31][0];
+  if (li < hi && hi - lo <= Sm::THREADS && lc.out_valid) {
+    const int i = a.begin + li, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const double *slot = (Sm::L2_WARPS > 0 && warp >= LIO_SMEM_WARPS) ? &lane_slots<true>(sm, warp)[lane][0] : &lane_slots<false>(sm, warp)[lane][0];
     const int2 out = *reinterpret_cast<const int2 *>(slot + SL_OUT);
     a.match_plane[i] = out.x;
     a.dis_to_plane[i] = reinterpret_cast<const float *>(slot + SL_ROW + 8)[0];
@@ -866,7 +916,7 @@ __device__ __forceinline__ void lio_write_outputs(const LioKernelArgs &a, const 
 }
 
 // Contiguous slices of the shard per block in whole warps (32-point chunks), spread as evenly as the chunk count allows:
-// every SM of the grid takes part (100 k points = 3125 chunks: 24 on 89 CTAs and 23 on 43, each more than its 22 warps).
+// every SM of the grid takes part (100 k points = 3125 chunks: 24 on 89 CTAs and 23 on 43, one per warp).
 __device__ __forceinline__ void lio_block_range(int count, int &lo, int &hi) {
   const int chunks = (count + 31) >> 5, g = (int)gridDim.x, b = (int)blockIdx.x;
   const int q = chunks / g, r = chunks % g;
@@ -877,16 +927,16 @@ __device__ __forceinline__ void lio_block_range(int count, int &lo, int &hi) {
   if (hi > count) hi = count;
 }
 
-__device__ __forceinline__ void lio_init_barriers(LioSmem &sm) {
-  if (threadIdx.x < LIO_WARPS) mbar_init(&sm.mbar[threadIdx.x], 1);
+__device__ __forceinline__ void lio_init_barriers(LioSmemCore &sm) {
+  if (threadIdx.x < LIO_SMEM_WARPS) mbar_init(&sm.mbar[threadIdx.x], 1);
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   __syncthreads();
 }
 
-__global__ void __launch_bounds__(LIO_THREADS, 1) lio_residual_kernel(const LioKernelArgs a) {
+template <int L2W> __global__ void __launch_bounds__(LioSmem<L2W>::THREADS, 1) lio_residual_kernel(const LioKernelArgs a) {
   if (a.ctrl->stop) return;  // EKF_stop_flg: remaining iterations of the unrolled loop do nothing
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  LioSmem &sm = *reinterpret_cast<LioSmem *>(smem_raw);
+  LioSmem<L2W> &sm = *reinterpret_cast<LioSmem<L2W> *>(smem_raw);
   lio_init_cold(sm, a);
   lio_init_barriers(sm);
   lio_prior_consts(sm, a);
@@ -898,7 +948,7 @@ __global__ void __launch_bounds__(LIO_THREADS, 1) lio_residual_kernel(const LioK
   LaneCache lc;
   lane_cache_init(lc);
   lio_process_range(a, sm, lo, hi, D0, D1, cnt, lc, a.init_normal != 0, true);
-  reduce_info<LIO_WARPS, 6>(sm.red, D0, D1, (double)cnt, a.partials, a.partial_stride, a.info, a.ctrl);
+  reduce_info<LioSmem<L2W>::WARPS, 6>(sm.red, D0, D1, (double)cnt, a.partials, a.partial_stride, a.info, a.ctrl);
 }
 
 }  // namespace esikf
