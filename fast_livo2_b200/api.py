@@ -81,6 +81,7 @@ def load_library():
     lib.esikf_set_loop_mode.argtypes = [vp, C.c_int]
     lib.esikf_set_tuning.argtypes = [vp, C.c_uint32]
     lib.esikf_set_extrinsics.argtypes = [vp, C.POINTER(ExtrinsicsC)]
+    lib.esikf_set_lidar_extrinsics.argtypes = [vp, dp, dp]
     lib.esikf_map_upload.argtypes = [vp, i64p, ip, ip, C.c_int32, vp, C.c_int32, C.c_double]
     lib.esikf_map_patch.argtypes = [vp, ip, vp, C.c_int32]
     lib.esikf_map_device_init.argtypes = [vp, vp]
@@ -222,6 +223,11 @@ class Context:
         e.Rcl[:] = _c(ext.Rcl, np.float64).reshape(9)
         e.Pcl[:] = _c(ext.Pcl, np.float64)
         self._ck(self.lib.esikf_set_extrinsics(self.h, C.byref(e)))
+
+    def set_lidar_extrinsics(self, extR, extT):
+        """Only the lidar -> IMU part; the camera part set before is kept (Rcl = I, Pcl = 0 if none was)."""
+        R, t = _c(extR, np.float64).reshape(9), _c(extT, np.float64).reshape(3)
+        self._ck(self.lib.esikf_set_lidar_extrinsics(self.h, R.ctypes.data_as(C.POINTER(C.c_double)), t.ctypes.data_as(C.POINTER(C.c_double))))
 
     # ------------------------------------------------------------------ map
     def map_upload(self, vmap, voxel_size):

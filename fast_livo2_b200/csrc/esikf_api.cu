@@ -184,6 +184,8 @@ struct esikf_ctx {
   int n_pts = 0;
   int pre_stride = 0;
   bool scan_fresh = false;   // precompute pending
+  double pre_ext[12] = {};   // the extR extT and dept_err / beam_err the precompute in `pre` was made with
+  float pre_dept_err = 0.f, pre_beam_err = 0.f;
   esikf_lio_cfg lio_cfg{};
   DevBuf<double> ext_dev;    // extR(9) extT(3)
   DevBuf<double> lio_slot_block;  // lane slots of the LIO kernels' L2-slot warps: [partial_blocks][LIO_L2_WARPS * 32][SLOT_D]
@@ -952,6 +954,18 @@ int esikf_lio_set_scan(esikf_ctx *ctx, const float *pts_xyz, int32_t n) {
   return ESIKF_OK;
 }
 
+// calcBodyCov and the cross-matrix vector of every point of the resident scan (voxel_map.cpp:349-360). StateEstimation
+// recomputes both every call; here they are kept with what they were made from and redone only when the scan, the lidar
+// extrinsics or the noise model changed.
+static void lio_precompute(esikf_ctx *ctx, float dept_err, float beam_err) {
+  lio_precompute_kernel<<<(ctx->n_pts + 255) / 256, 256, 0, ctx->stream>>>(ctx->pts.p, ctx->n_pts, ctx->pre.p, ctx->pre_stride, ctx->ext_dev.p, dept_err, beam_err);
+  memcpy(ctx->pre_ext, ctx->ext_host, sizeof(ctx->pre_ext));
+  ctx->pre_dept_err = dept_err, ctx->pre_beam_err = beam_err;
+}
+static bool lio_precompute_current(const esikf_ctx *ctx, float dept_err, float beam_err) {
+  return !ctx->scan_fresh && memcmp(ctx->pre_ext, ctx->ext_host, sizeof(ctx->pre_ext)) == 0 && ctx->pre_dept_err == dept_err && ctx->pre_beam_err == beam_err;
+}
+
 static int lio_fill_args(esikf_ctx *ctx, LioKernelArgs &ka, double *state_ptr) {
   memset(&ka, 0, sizeof(ka));
   ka.pts = ctx->pts.p, ka.pre = ctx->pre.p;
@@ -1057,9 +1071,10 @@ int esikf_lio_run(esikf_ctx *ctx, const double *state_in, const double *state_pr
   // the persistent kernel initialises its own loop control / stats / barrier; the per-iteration path needs them zeroed
   if (!fused_lio) CK(cudaMemsetAsync(ctx->lio_stats, 0, sizeof(esikf_lio_stats) + sizeof(Ctrl) + 64, st));
   const int n = ctx->n_pts;
-  if (ctx->scan_fresh) {
+  const float dept_err = (float)cfg->dept_err, beam_err = (float)cfg->beam_err;
+  if (!lio_precompute_current(ctx, dept_err, beam_err)) {
     if (n > 0) {
-      lio_precompute_kernel<<<(n + 255) / 256, 256, 0, st>>>(ctx->pts.p, n, ctx->pre.p, ctx->pre_stride, ctx->ext_dev.p, (float)cfg->dept_err, (float)cfg->beam_err);
+      lio_precompute(ctx, dept_err, beam_err);
       ctx->launches++;
     }
     ctx->scan_fresh = false;
@@ -1745,8 +1760,7 @@ int esikf_profile_kernel(esikf_ctx *ctx, int32_t which, int32_t arg, int32_t rep
     if (which == 0) launch_lio_residual(lio_use_l2_slots(la.count, grid), grid, st, la);
     else if (which == 1) lio_solve_kernel<<<1, SOLVE_THREADS, 0, st>>>(sa);
     else if (which == 2) vio_patch_kernel<<<grid, VIO_THREADS, sizeof(VioSmem), st>>>(va);
-    else lio_precompute_kernel<<<(ctx->n_pts + 255) / 256, 256, 0, st>>>(ctx->pts.p, ctx->n_pts, ctx->pre.p, ctx->pre_stride, ctx->ext_dev.p, (float)ctx->lio_cfg.dept_err,
-                                                                       (float)ctx->lio_cfg.beam_err);
+    else lio_precompute(ctx, (float)ctx->lio_cfg.dept_err, (float)ctx->lio_cfg.beam_err);
     CK(cudaEventRecord(e1, st));
     CK(cudaEventSynchronize(e1));
     ctx->launches++;

@@ -247,7 +247,9 @@ int esikf_map_device_export(esikf_ctx *ctx, int64_t *keys, int32_t *first, int32
  *   set_scan : feats_down_body_ (xyz float32, n points) -> device + per-frame calcBodyCov/crossmat
  *              (src/voxel_map.cpp:349-360). shard_begin/shard_count select this rank's slice.
  *   run      : the iteration loop (src/voxel_map.cpp:372-500) asynchronously on esikf_stream.
- *   fetch    : state_ / stats / per-point results back to host (synchronises the stream). */
+ *   fetch    : state_ / stats / per-point results back to host (synchronises the stream).
+ * The per-point calcBodyCov / crossmat precompute is made by the first run after set_scan, and redone by a later run on the
+ * same scan whose lidar extrinsics (extR, extT) or dept_err / beam_err differ from the ones it was made with. */
 int esikf_lio_set_scan(esikf_ctx *ctx, const float *pts_xyz, int32_t n);
 int esikf_lio_run(esikf_ctx *ctx, const double *state_in, const double *state_prop, const esikf_lio_cfg *cfg);
 int esikf_lio_fetch(esikf_ctx *ctx, double *state_out, esikf_lio_stats *stats /* nullable */,
