@@ -131,13 +131,15 @@ struct esikf_ctx {
   std::string err;
   int64_t launches = 0;
   int solve_mode = 0;
-  int loop_mode = 2;      // >= 1: one persistent cooperative kernel per update (gain solve replicated in every CTA, one grid
-                          //    barrier per iteration; carries the NVLink peer exchange when peers are attached),
+  int loop_mode = 2;      // >= 1: one persistent cooperative kernel per update (gain solve replicated in every CTA, one
+                          //    grid exchange per iteration; carries the NVLink peer exchange when peers are attached),
                           // 0: one residual + one solve launch per iteration (NCCL communicator, kernel timing)
   int coop_ok = 0;
   int coop_lio = 0, coop_vio = 0;  // co-resident CTAs per SM of the persistent kernels
   uint32_t tuning = 0;             // ESIKF_TUNE_* flags (measurement variants)
-  DevBuf<unsigned int> barrier;       // two grid barriers {counter @ +0, release word @ +128 B}, 256 B apart; launches alternate
+  DevBuf<unsigned int> barrier;          // LIO kernel: two grid barriers {counter @ +0, release word @ +128 B}, 256 B apart; launches alternate
+  DevBuf<unsigned long long> grid_mbox;  // VIO kernel: the grid mailbox (grid_mbox_words), then the exchange counter
+  unsigned int *exchange_seq = nullptr;  // device word: exchanges executed so far (the tag of both mailboxes follows it)
   DevBuf<unsigned long long> stamps;  // 8 per slot: 8 LIO slots then 64 VIO slots
   bool want_stamps = false;
   esikf_extrinsics ext{};
@@ -244,11 +246,10 @@ struct esikf_ctx {
   int rank = 0, nranks = 1;
   ncclComm_t comm = nullptr;
   // NVLink peer-memory all-reduce inside the persistent kernels
-  unsigned long long *mailbox = nullptr;             // own mailbox [2][PEER_MAX_RANKS][PEER_SLOT_WORDS], followed by the exchange counter
+  unsigned long long *mailbox = nullptr;             // own mailbox [2][PEER_MAX_RANKS][PEER_SLOT_WORDS]
   std::vector<unsigned long long *> peer_ptrs;       // mailbox of every rank as mapped into this process
   DevBuf<unsigned long long *> peer_ptrs_dev;
   bool p2p = false;
-  unsigned int *peer_seq_dev = nullptr;              // device word: peer exchanges executed so far
 
   // measurement
   bool timing = false;
@@ -372,8 +373,13 @@ int esikf_create(esikf_ctx **out, int device) {
             ctx->scratch_state.reserve(S_N) == cudaSuccess;
   ctx->partial_blocks = ctx->sm_count < 160 ? ctx->sm_count : 160;  // persistent residual kernels: one CTA per SM
   ok = ok && ctx->partials.reserve((size_t)2 * ctx->partial_blocks * NE_MAX) == cudaSuccess && ctx->stamps.reserve(8 * 72 + 64 + 160) == cudaSuccess &&
-       ctx->barrier.reserve(128) == cudaSuccess && ctx->lio_slot_block.reserve((size_t)ctx->partial_blocks * LIO_L2_WARPS * 32 * SLOT_D) == cudaSuccess;
+       ctx->barrier.reserve(128) == cudaSuccess && ctx->grid_mbox.reserve(grid_mbox_words(ctx->partial_blocks) + 1) == cudaSuccess &&
+       ctx->lio_slot_block.reserve((size_t)ctx->partial_blocks * LIO_L2_WARPS * 32 * SLOT_D) == cudaSuccess;
   if (ok) cudaMemsetAsync(ctx->barrier.p, 0, 128 * sizeof(unsigned int), ctx->stream);
+  if (ok) {  // tag 0 is never sent
+    cudaMemsetAsync(ctx->grid_mbox.p, 0, ctx->grid_mbox.cap * sizeof(unsigned long long), ctx->stream);
+    ctx->exchange_seq = reinterpret_cast<unsigned int *>(ctx->grid_mbox.p + grid_mbox_words(ctx->partial_blocks));
+  }
   if (ok) {
     ctx->state = ctx->state_prop.p, ctx->prop = ctx->state_prop.p + S_N;
     for (int i = 0; i < esikf_ctx::STAGE_SLOTS; i++) ok = ok && cudaEventCreateWithFlags(&ctx->stage_ev[i], cudaEventDisableTiming) == cudaSuccess;
@@ -1031,21 +1037,22 @@ static bool persistent_update(const esikf_ctx *ctx, int coop_blocks) {
 }
 
 // Cooperative launch of lio_update_kernel<PEER, L2W> / vio_update_kernel<PEER, INVERSE>. Their arguments are
-// (ka, sa, barrier, barrier_next, stamps, parity_stride, peer, tail...): `ka` is the kernel's LioKernelArgs /
+// (ka, sa, grid sync, stamps, peer, tail...): `ka` is the kernel's LioKernelArgs /
 // VioKernelArgs, `tail` the VIO-only arguments. Both instantiations get the same argument list, so the single-GPU
 // launch passes exactly what the peer launch does. `stamp_off` / `stamp_words`: this kernel's slice of the phase stamps.
 static int launch_persistent(esikf_ctx *ctx, const void *fn, const void *fn_peer, const char *name, int grid, int threads, size_t smem, void *ka, SolveArgs &sa,
                              size_t stamp_off, size_t stamp_words, bool &timed, std::initializer_list<void *> tail) {
   const unsigned par = ctx->launch_parity & 1;
-  unsigned int *bar = ctx->barrier.p + 64 * par, *bar_next = ctx->barrier.p + 64 * (par ^ 1);  // this launch's barrier / the next launch's (zeroed by the kernel)
+  GridSync gs;
+  gs.barrier = ctx->barrier.p + 64 * par, gs.barrier_next = ctx->barrier.p + 64 * (par ^ 1);  // this launch's barrier / the next launch's (zeroed by the kernel)
+  gs.mbox = ctx->grid_mbox.p;
   unsigned long long *stamps = ctx->want_stamps ? ctx->stamps.p + stamp_off : nullptr;
   if (stamps) CK(cudaMemsetAsync(stamps, 0, stamp_words * sizeof(unsigned long long), ctx->stream));
-  size_t parity_stride = (size_t)ctx->partial_blocks * NE_MAX;
   PeerArgs peer;
-  peer.mbox = ctx->p2p ? ctx->peer_ptrs_dev.p : nullptr, peer.seq = ctx->peer_seq_dev;
+  peer.mbox = ctx->p2p ? ctx->peer_ptrs_dev.p : nullptr, peer.seq = ctx->exchange_seq;
   peer.rank = ctx->rank, peer.nranks = ctx->p2p ? ctx->nranks : 1;
-  void *kargs[9] = {ka, (void *)&sa, (void *)&bar, (void *)&bar_next, (void *)&stamps, (void *)&parity_stride, (void *)&peer};
-  std::copy(tail.begin(), tail.end(), kargs + 7);
+  void *kargs[7] = {ka, (void *)&sa, (void *)&gs, (void *)&stamps, (void *)&peer};
+  std::copy(tail.begin(), tail.end(), kargs + 5);
   cudaError_t le = cudaLaunchCooperativeKernel(ctx->p2p && ctx->nranks > 1 ? fn_peer : fn, dim3(grid), dim3(threads), kargs, smem, ctx->stream);
   if (le != cudaSuccess) return fail(ctx, ESIKF_ERR_CUDA, "cooperative launch of %s failed: %s", name, cudaGetErrorString(le));
   ctx->launch_parity++;  // only a launch that happened consumes its barrier counter (the kernel zeroes the other one)
@@ -1117,7 +1124,7 @@ static int finish_fetch(esikf_ctx *ctx) {
   CK(cudaStreamSynchronize(ctx->stream));
   if (h->comm_error) {
     cudaMemsetAsync(&ctx->ctrl->comm_error, 0, sizeof(int), ctx->stream);
-    return fail(ctx, ESIKF_ERR_COMM, "a bounded in-kernel wait expired (grid barrier or peer mailbox): a rank did not take part in the update");
+    return fail(ctx, ESIKF_ERR_COMM, "a bounded in-kernel wait expired (grid barrier, grid or peer mailbox): a rank did not take part in the update");
   }
   return ESIKF_OK;
 }
@@ -1663,10 +1670,9 @@ int esikf_peer_export(esikf_ctx *ctx, char out[64]) {
   if (!ctx || !out) return ESIKF_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
   if (!ctx->mailbox) {
-    const size_t words = (size_t)2 * PEER_MAX_RANKS * PEER_SLOT_WORDS + 2;  // + the exchange counter
+    const size_t words = (size_t)2 * PEER_MAX_RANKS * PEER_SLOT_WORDS;
     CK(cudaMalloc(&ctx->mailbox, words * sizeof(unsigned long long)));
     CK(cudaMemset(ctx->mailbox, 0, words * sizeof(unsigned long long)));  // tag 0 is never sent
-    ctx->peer_seq_dev = reinterpret_cast<unsigned int *>(ctx->mailbox + (size_t)2 * PEER_MAX_RANKS * PEER_SLOT_WORDS);
   }
   cudaIpcMemHandle_t h;
   CK(cudaIpcGetMemHandle(&h, ctx->mailbox));
@@ -1693,7 +1699,13 @@ int esikf_peer_attach(esikf_ctx *ctx, int32_t rank, int32_t nranks, const char *
   }
   CK(ctx->peer_ptrs_dev.reserve(nranks));
   CK(cudaMemcpy(ctx->peer_ptrs_dev.p, ctx->peer_ptrs.data(), nranks * sizeof(unsigned long long *), cudaMemcpyHostToDevice));
-  // mailbox and exchange counter were zeroed at export time (before the host-side all-gather): a peer may already be writing
+  // the peer mailbox was zeroed at export time (before the host-side all-gather): a peer may already be writing into it. The
+  // exchange counter has to start equal on every rank, so it restarts from 0 when the peers first attach, after this
+  // context's earlier updates; the grid mailbox restarts with it (a word left from before could carry a tag again).
+  if (!ctx->p2p) {
+    CK(cudaMemsetAsync(ctx->grid_mbox.p, 0, ctx->grid_mbox.cap * sizeof(unsigned long long), ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  }
   ctx->rank = rank, ctx->nranks = nranks, ctx->p2p = true;
   return ESIKF_OK;
 }

@@ -120,7 +120,7 @@ struct Ctrl {
   float last_error; // VIO (vio.cpp:1528)
   int has_G;        // VIO: G valid (at least one accepted update)
   unsigned int block_counter;  // last-block-done counter of the per-iteration residual kernels
-  int comm_error;              // a bounded wait (grid barrier / peer mailbox) expired: results of this update are invalid
+  int comm_error;              // a bounded wait (grid barrier / grid or peer mailbox) expired: results of this update are invalid
   int pad[8];
 };
 static_assert(sizeof(Ctrl) == 64, "the VIO stats follow the control block in one allocation: keep its size (and their alignment)");
@@ -160,10 +160,9 @@ template <int WARPS> struct ReduceSmem {
   int is_last;
 };
 
-// warp fragments -> per-CTA compact vector -> global partial column `blockIdx.x` of the entry-major array
-// partials[entry][partial_stride]. Fixed order (warp 0, 1, ...), so the result does not depend on timing.
-template <int WARPS, int M>
-__device__ __forceinline__ void store_partials(ReduceSmem<WARPS> &rs, double D0, double D1, double cnt, double *partials, int partial_stride) {
+// warp fragments -> per-CTA compact vector: thread tid < NE returns entry tid of the CTA's partial (0 elsewhere). Fixed order
+// (warp 0, 1, ...), so the result does not depend on timing.
+template <int WARPS, int M> __device__ __forceinline__ double cta_partial(ReduceSmem<WARPS> &rs, double D0, double D1, double cnt) {
   constexpr int NE = ne_of(M);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   {
@@ -174,18 +173,36 @@ __device__ __forceinline__ void store_partials(ReduceSmem<WARPS> &rs, double D0,
     if (lane == 0) rs.w[warp][NE - 1] = cnt;
   }
   __syncthreads();
+  double s = 0.0;
   if (tid < NE) {
-    double s = rs.w[0][tid];
+    s = rs.w[0][tid];
 #pragma unroll
     for (int w = 1; w < WARPS; w++) s += rs.w[w][tid];
-    partials[(size_t)tid * partial_stride + blockIdx.x] = s;
   }
+  return s;
+}
+
+// The CTA's partial -> global partial column `blockIdx.x` of the entry-major array partials[entry][partial_stride].
+template <int WARPS, int M>
+__device__ __forceinline__ void store_partials(ReduceSmem<WARPS> &rs, double D0, double D1, double cnt, double *partials, int partial_stride) {
+  const double s = cta_partial<WARPS, M>(rs, D0, D1, cnt);
+  if (threadIdx.x < ne_of(M)) partials[(size_t)threadIdx.x * partial_stride + blockIdx.x] = s;
 }
 
 // Fixed-order sum over the per-CTA partial columns by the calling CTA (nb <= 160 columns): warp w owns entries w,
 // w + nwarps, ...; lane l adds columns l, l + 32, ... in order, then a fixed xor-shuffle tree. Every load is issued before
 // the first add, so the whole sum costs ONE L2 round trip. Bit-identical in every CTA that runs it.
 #define SUM_MAXC 5
+// The fixed order of one entry's sum: lane l holds columns l, l + 32, ... (0.0 past the last column) and adds them in order,
+// then the xor-shuffle tree. Every lane returns the total.
+__device__ __forceinline__ double column_sum(const double (&v)[SUM_MAXC]) {
+  double s = v[0];
+#pragma unroll
+  for (int c = 1; c < SUM_MAXC; c++) s += v[c];
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
+  return s;
+}
 template <int M> __device__ __forceinline__ void sum_partials(const double *partials, int partial_stride, int nb, double *out, int nwarps) {
   constexpr int NE = ne_of(M);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -204,11 +221,7 @@ template <int M> __device__ __forceinline__ void sum_partials(const double *part
 #pragma unroll
   for (int k = 0; k < MAXE; k++) {
     const int e = warp + k * nwarps;
-    double s = v[k][0];
-#pragma unroll
-    for (int c = 1; c < SUM_MAXC; c++) s += v[k][c];
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
+    const double s = column_sum(v[k]);
     if (lane == 0 && e < NE) out[e] = s;
   }
 }

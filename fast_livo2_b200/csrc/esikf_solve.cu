@@ -14,7 +14,7 @@
 //
 // Critical path inside the persistent kernels: [all CTAs arrived] -> sum of the partial columns -> gain elimination ->
 // boxplus -> next slice. Everything that does not need the new information vector is hoisted out of it:
-// state_propagat (-) state is evaluated by warp 1 while the CTA waits at the grid barrier, and P never changes inside the
+// state_propagat (-) state is evaluated by warp 1 while the CTA waits in the grid exchange, and P never changes inside the
 // loop. The elimination itself is one warp, one column per lane.
 #include <float.h>
 #include "esikf_dev.cuh"
@@ -273,7 +273,7 @@ __device__ __forceinline__ void solve_load(SolveSmem &sm, SolveIO &io, const Sol
   }
 }
 
-// What a persistent kernel keeps resident or prepares in its prologue and grid-barrier wait, staged by a per-iteration solve
+// What a persistent kernel keeps resident or prepares in its prologue and grid-exchange wait, staged by a per-iteration solve
 // launch: the inputs, vec = state_propagat (-) state on warp 1 and the loop invariants of the gain on warp 2.
 template <int m> __device__ __forceinline__ void solve_stage(SolveSmem &sm, SolveIO &io, const SolveArgs &a, double pscale, bool want_old) {
   const int tid = threadIdx.x, lane = tid & 31;
@@ -318,7 +318,7 @@ __device__ __forceinline__ void lio_write_stats(const SolveArgs &a, SolveSmem &s
 // One LIO gain solve + state update (src/voxel_map.cpp:462-499) by the calling block. Returns EKF_stop_flg.
 // `ctrl` is the loop-control block the routine reads and updates (global memory for the per-iteration kernels, the CTA's
 // shared-memory copy inside the persistent kernel). Expects P, the poses and info in sm / io, vec = state_propagat (-) state_
-// (:470) in sm.vec and, in solve_mode 0, gain_setup<6> done: solve_stage or the persistent kernel's prologue and barrier wait.
+// (:470) in sm.vec and, in solve_mode 0, gain_setup<6> done: solve_stage or the persistent kernel's prologue and exchange wait.
 __device__ __noinline__ bool lio_solve_block(const SolveArgs &a, SolveSmem &sm, SolveIO &io, Ctrl &ctrl) {
   const int tid = threadIdx.x, lane = tid & 31;
   const int iterCount = ctrl.iter;

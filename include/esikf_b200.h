@@ -31,7 +31,7 @@ enum esikf_status {
   ESIKF_ERR_CUDA = -2,        /* a CUDA runtime call failed; see esikf_last_error */
   ESIKF_ERR_ARG = -3,         /* bad argument (null pointer, negative size, key out of range ...) */
   ESIKF_ERR_STATE = -4,       /* call order (e.g. lio_run before map_upload / set_scan) */
-  ESIKF_ERR_COMM = -5         /* NCCL / peer-memory set-up failed, or a bounded in-kernel wait (grid barrier, peer mailbox)
+  ESIKF_ERR_COMM = -5         /* NCCL / peer-memory set-up failed, or a bounded in-kernel wait (grid barrier, grid mailbox, peer mailbox)
                                  expired: the update that reported it is invalid (returned by the fetch calls) */
 };
 
@@ -133,7 +133,7 @@ int64_t esikf_launch_count(const esikf_ctx *ctx);
 int esikf_set_solve_mode(esikf_ctx *ctx, int mode);
 /* loop_mode: how the iteration loop of an update is driven. Results of all modes are bit-identical.
  *   2 (default; 1 is accepted as an alias) = one persistent cooperative kernel per update: every CTA keeps the state on
- *       chip, sums the per-CTA partial vectors after ONE grid barrier per iteration and runs the gain solve itself. With
+ *       chip, sums the per-CTA partial vectors after ONE grid exchange per iteration (LIO: a grid barrier, VIO: a tagged-word mailbox) and runs the gain solve itself. With
  *       peer GPUs attached (esikf_peer_attach) the same kernel also carries the NVLink exchange of the information vector.
  *   0 = one residual + one solve launch per iteration (also used with an NCCL communicator or kernel timing on). */
 int esikf_set_loop_mode(esikf_ctx *ctx, int mode);

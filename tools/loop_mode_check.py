@@ -51,7 +51,7 @@ def check(fr, label, time_it):
     ok = True
     for mode in MODES:
         ctx.set_loop_mode(mode)
-        for rep in range(2):  # twice: the second launch uses the other barrier counter / partial parity history
+        for rep in range(2):  # twice: the second launch uses the other barrier counter and continues the exchange counter
             r, v = run_once(ctx, fr, w)
         if ref is None:
             ref = (r, v)
@@ -143,7 +143,7 @@ def check(fr, label, time_it):
                 ctx.vio_run(post_h, post_h)
             ctx.synchronize()
             s = ctx.get_phase_stamps().astype(np.int64)
-            names = ["consts", "slice", "barrier", "reduce", "solve"]
+            names = ["consts", "slice", "exchange", "sum+peer", "solve"]
             rows = [k for k in range(72) if s[k, 0] != 0]
             for j, slot in enumerate(rows):
                 d = np.diff(s[slot, :6])
