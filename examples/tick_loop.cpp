@@ -58,6 +58,11 @@ int main() {
     voxelmap_manager.StateEstimation(state_propagat);    // :370
     _state = voxelmap_manager.state_;                    // :371
     voxelmap_manager.UpdateVoxelMap();                   // :413-424 in one call: world points, covariances, octree update, refits
+    // :435-443, the world cloud of the coloured scan with the LIO posterior: dense_map_en = true hands over feats_undistort
+    // (here a wall 3 m in front of the camera); dense_map_en = false would be SetWorldCloud() on the scan itself
+    std::vector<PointXYZ> feats_undistort = floor_scan(1600, 0.0f);
+    for (PointXYZ &p : feats_undistort) p.z = 3.0f;
+    voxelmap_manager.SetWorldCloud(&feats_undistort);
     std::printf("tick %d LIO: status %d, effective points %d\n", tick, voxelmap_manager.last_status_, voxelmap_manager.effct_feat_num_);
 
     // ---- VIO tick (LIVMapper::handleVIO -> processFrame -> computeJacobianAndUpdateEKF, vio.cpp:1810)
@@ -81,6 +86,12 @@ int main() {
     state_propagat = _state;
     vio_manager.computeJacobianAndUpdateEKF(img);
     std::printf("tick %d VIO: status %d, patch error %.3f\n", tick, vio_manager.last_status_, submap.errors.empty() ? -1.0f : submap.errors[0]);
+    // publish_frame_world (LIVMapper.cpp:1140-1173): the LIO tick's world cloud coloured from img_rgb at the VIO posterior
+    std::vector<uint8_t> bgr(64 * 48 * 3);
+    for (size_t i = 0; i < bgr.size(); i++) bgr[i] = (uint8_t)(i % 3 == 0 ? 40 : i % 3 == 1 ? 120 : 200);
+    std::vector<PointXYZRGB> laserCloudWorldRGB;
+    vio_manager.ColorizeFrameWorld(BgrImage{bgr.data(), 64, 48}, /*blind_rgb_points*/ 0.01, laserCloudWorldRGB);
+    std::printf("tick %d coloured scan: status %d, %zu points\n", tick, vio_manager.last_status_, laserCloudWorldRGB.size());
   }
   // somebody wants the warp patches of the last selection on the host after all
   vio_manager.MaterializeWarpPatches();

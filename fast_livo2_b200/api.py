@@ -111,6 +111,8 @@ def load_library():
     lib.esikf_vio_warp_affine.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp]
     lib.esikf_vio_set_inverse_refs.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp]
     lib.esikf_vio_select_patches.argtypes = [vp, C.c_int32] + [vp] * 12 + [C.c_double, C.POINTER(VioSelectCfgC), ip, vp, vp, vp, vp, vp]
+    lib.esikf_rgb_set_cloud.argtypes = [vp, vp, C.c_int32, vp]
+    lib.esikf_rgb_colorize.argtypes = [vp, vp, C.c_int32, C.c_int32, vp, C.c_double, C.c_int32, ip, vp, vp, vp]
     lib.esikf_comm_unique_id.argtypes = [C.c_char_p]
     lib.esikf_comm_init.argtypes = [vp, C.c_int32, C.c_int32, C.c_char_p]
     lib.esikf_comm_rank.argtypes = [vp, ip, ip]
@@ -146,7 +148,7 @@ EXPORTED_SYMBOLS = [
     "esikf_set_extrinsics", "esikf_set_lidar_extrinsics", "esikf_map_upload", "esikf_map_patch", "esikf_map_device_init", "esikf_map_device_build", "esikf_map_device_update", "esikf_map_device_update_points", "esikf_map_device_slide", "esikf_map_device_stats", "esikf_map_device_capacity", "esikf_map_device_download", "esikf_map_device_export", "esikf_lio_fetch_normals", "esikf_lio_set_scan", "esikf_lio_run", "esikf_lio_fetch",
     "esikf_lio_update", "esikf_lio_fetch_point_cov", "esikf_vio_set_camera", "esikf_vio_set_image", "esikf_vio_set_patches",
     "esikf_vio_run", "esikf_vio_fetch", "esikf_vio_update", "esikf_vio_get_image_patch", "esikf_vio_set_ref_images",
-    "esikf_vio_warp_patches", "esikf_vio_select_patches", "esikf_vio_warp_affine", "esikf_vio_set_inverse_refs", "esikf_comm_unique_id", "esikf_comm_init", "esikf_comm_rank", "esikf_shard_range", "esikf_peer_export", "esikf_peer_attach", "esikf_profile_kernel", "esikf_set_kernel_timing", "esikf_get_kernel_timing", "esikf_set_phase_stamps", "esikf_get_phase_stamps",
+    "esikf_vio_warp_patches", "esikf_vio_select_patches", "esikf_vio_warp_affine", "esikf_vio_set_inverse_refs", "esikf_rgb_set_cloud", "esikf_rgb_colorize", "esikf_comm_unique_id", "esikf_comm_init", "esikf_comm_rank", "esikf_shard_range", "esikf_peer_export", "esikf_peer_attach", "esikf_profile_kernel", "esikf_set_kernel_timing", "esikf_get_kernel_timing", "esikf_set_phase_stamps", "esikf_get_phase_stamps",
 ]
 
 
@@ -180,6 +182,7 @@ class Context:
         self.n_pts = 0
         self.n_patches = 0
         self.levels = 4
+        self._rgb_n = 0  # points of the last rgb_set_cloud
 
     def close(self):
         if getattr(self, "h", None):
@@ -479,6 +482,32 @@ class Context:
         if want_patches:
             out["warp_patch"] = wp[:k]
         return out
+
+    # ------------------------------------------------------------------ coloured scan (publish_frame_world)
+    def rgb_set_cloud(self, pts=None, state=None):
+        """The world cloud of this LIO tick (esikf_rgb_set_cloud): pts (n, 3) float32 body points, or None for the resident
+        scan of lio_set_scan / lio_update; state: a packed state, or None for the posterior the last LIO update left on the
+        device. Call after the LIO update and before the VIO update."""
+        p = None if pts is None else _c(pts, np.float32).reshape(-1, 3)
+        s = None if state is None else _c(state, np.float64)
+        self._ck(self.lib.esikf_rgb_set_cloud(self.h, _addr(p), 0 if p is None else len(p), _addr(s)))
+        self._rgb_n = self.n_pts if p is None else len(p)
+
+    def rgb_colorize(self, bgr, blind_rgb_points=0.01, state=None, cap=None):
+        """publish_frame_world on the cloud of rgb_set_cloud (esikf_rgb_colorize): bgr (height, width, 3) uint8 B G R of the
+        camera's size; state: a packed state, or None for the posterior the last VIO update left on the device. Returns
+        xyz (k, 3) float32, bgr (k, 3) uint8 (B, G, R) and index (k,) int32 of the kept points in cloud order. cap: room for
+        that many points (default: every point of the cloud); fewer than the kept points raises."""
+        img = _c(bgr, np.uint8)
+        assert img.ndim == 3 and img.shape[2] == 3
+        s = None if state is None else _c(state, np.float64)
+        cap = self._rgb_n if cap is None else int(cap)
+        xyz, col, idx = np.zeros((max(cap, 1), 3), np.float32), np.zeros((max(cap, 1), 3), np.uint8), np.zeros(max(cap, 1), np.int32)
+        n = C.c_int32(0)
+        self._ck(self.lib.esikf_rgb_colorize(self.h, img.ctypes.data, img.shape[1], img.shape[0], _addr(s), float(blind_rgb_points), cap, C.byref(n),
+                                             xyz.ctypes.data, col.ctypes.data, idx.ctypes.data))
+        k = n.value
+        return dict(xyz=xyz[:k], bgr=col[:k], index=idx[:k])
 
     # ------------------------------------------------------------------ multi-GPU / measurement
     def vio_set_inverse_refs(self, ref_img_index, ref_px, ref_f, ref_R, ref_pos):

@@ -22,6 +22,7 @@
 #include "esikf_vio.cu"
 #include "esikf_fused.cu"
 #include "esikf_map.cu"
+#include "esikf_color.cu"
 
 using namespace esikf;
 
@@ -241,6 +242,15 @@ struct esikf_ctx {
   DevBuf<float> sel_warp, sel_err;
   std::vector<double> sel_stage_d;
   std::vector<int32_t> sel_stage_i;
+  // which update's posterior `state` holds: the LIO tick's world cloud (esikf_rgb_set_cloud) and the VIO tick's frame pose
+  // (esikf_rgb_colorize) default to the one their tick left there
+  enum { RESIDENT_NONE, RESIDENT_LIO, RESIDENT_VIO } resident = RESIDENT_NONE;
+
+  // coloured scan (esikf_rgb_*): the world cloud of the last esikf_rgb_set_cloud, the BGR image and the per-point scratch
+  DevBuf<float> rgb_cloud, rgb_xyz;
+  DevBuf<uint8_t> rgb_img, rgb_color, rgb_bgr, rgb_scan_tmp;
+  DevBuf<int32_t> rgb_keep, rgb_dst, rgb_index;
+  int rgb_n = -1;  // points of the cloud, -1 before esikf_rgb_set_cloud
 
   // multi-GPU
   int rank = 0, nranks = 1;
@@ -1074,6 +1084,7 @@ int esikf_lio_run(esikf_ctx *ctx, const double *state_in, const double *state_pr
     int rc = upload_states(ctx, state_in, state_prop);
     if (rc) return rc;
   }
+  ctx->resident = esikf_ctx::RESIDENT_LIO;
   const bool fused_lio = persistent_update(ctx, ctx->coop_lio);
   // the persistent kernel initialises its own loop control / stats / barrier; the per-iteration path needs them zeroed
   if (!fused_lio) CK(cudaMemsetAsync(ctx->lio_stats, 0, sizeof(esikf_lio_stats) + sizeof(Ctrl) + 64, st));
@@ -1304,6 +1315,7 @@ int esikf_vio_run(esikf_ctx *ctx, const double *state_in, const double *state_pr
     int rc = upload_states(ctx, state_in, state_prop);
     if (rc) return rc;
   }
+  ctx->resident = esikf_ctx::RESIDENT_VIO;
   const bool inverse = ctx->vio_cfg.inverse_composition_en != 0;
   if (inverse && ctx->n_patches > 0) {
     if (ctx->n_inv_refs != ctx->n_patches) return fail(ctx, ESIKF_ERR_STATE, "vio_run: inverse_composition_en needs esikf_vio_set_inverse_refs for the %d patches (have %d)", ctx->n_patches, ctx->n_inv_refs);
@@ -1639,6 +1651,101 @@ int esikf_vio_warp_affine(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_inde
   CK(cudaMemcpyAsync(warp_patch_out, ctx->warp_out.p, (size_t)n * 64 * L * sizeof(float), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   CK(cudaGetLastError());
+  return ESIKF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------- coloured scan
+// The device copy of a frame's pose: a packed host state staged into scratch_state, or (state == NULL) the posterior resident on
+// the device, which must be the one an update of kind `want` left there.
+static int rgb_state(esikf_ctx *ctx, const double *state, int want, const char *what, const double **out) {
+  if (!state) {
+    if (ctx->resident != want)
+      return fail(ctx, ESIKF_ERR_STATE, "%s(state = NULL): the device holds no %s posterior", what, want == esikf_ctx::RESIDENT_LIO ? "LIO" : "VIO");
+    *out = ctx->state;
+    return ESIKF_OK;
+  }
+  CK(ctx->scratch_state.reserve(S_N));
+  CK(cudaMemcpyAsync(ctx->scratch_state.p, state, S_N * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  *out = ctx->scratch_state.p;
+  return ESIKF_OK;
+}
+
+int esikf_rgb_set_cloud(esikf_ctx *ctx, const float *pts_xyz, int32_t n, const double *state) {
+  if (!ctx || (pts_xyz && n < 0)) return fail(ctx, ESIKF_ERR_ARG, "rgb_set_cloud: bad argument");
+  if (!ctx->have_ext) return fail(ctx, ESIKF_ERR_STATE, "rgb_set_cloud before set_extrinsics");
+  if (!pts_xyz && !ctx->pts.p) return fail(ctx, ESIKF_ERR_STATE, "rgb_set_cloud(pts_xyz = NULL) without a resident scan (esikf_lio_set_scan)");
+  if (!pts_xyz && !state && ctx->scan_fresh) return fail(ctx, ESIKF_ERR_STATE, "rgb_set_cloud: the resident scan has not been through esikf_lio_run yet");
+  CK(cudaSetDevice(ctx->device));
+  const double *dev_state = nullptr;
+  if (int rc = rgb_state(ctx, state, esikf_ctx::RESIDENT_LIO, "rgb_set_cloud", &dev_state)) return rc;
+  if (!pts_xyz) n = ctx->n_pts;
+  ctx->rgb_n = -1;  // until the new cloud is in place
+  CK(ctx->rgb_cloud.reserve((size_t)n * 3 + 4));
+  cudaStream_t st = ctx->stream;
+  if (pts_xyz && n > 0) CK(cudaMemcpyAsync(ctx->rgb_cloud.p, pts_xyz, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, st));
+  if (pts_xyz || state) CK(cudaStreamSynchronize(st));  // the caller may reuse its buffers on return, pinned ones included
+  if (n > 0) {
+    RgbWorldArgs a;
+    a.body = pts_xyz ? ctx->rgb_cloud.p : ctx->pts.p, a.world = ctx->rgb_cloud.p, a.n = n, a.state = dev_state;
+    memcpy(a.extR, ctx->ext.extR, sizeof(a.extR)), memcpy(a.extT, ctx->ext.extT, sizeof(a.extT));
+    rgb_world_kernel<<<(n + 255) / 256, 256, 0, st>>>(a);
+    ctx->launches++;
+    CK(cudaGetLastError());
+  }
+  ctx->rgb_n = n;
+  return ESIKF_OK;
+}
+
+int esikf_rgb_colorize(esikf_ctx *ctx, const uint8_t *bgr, int32_t width, int32_t height, const double *state, double blind_rgb_points, int32_t cap,
+                       int32_t *n_out, float *xyz_out, uint8_t *bgr_out, int32_t *index_out) {
+  if (!ctx || !bgr || !n_out || cap < 0 || (cap > 0 && (!xyz_out || !bgr_out))) return fail(ctx, ESIKF_ERR_ARG, "rgb_colorize: bad argument");
+  if (ctx->rgb_n < 0) return fail(ctx, ESIKF_ERR_STATE, "rgb_colorize before rgb_set_cloud");
+  if (!ctx->have_cam) return fail(ctx, ESIKF_ERR_STATE, "rgb_colorize before vio_set_camera");
+  if (width != ctx->cam.width || height != ctx->cam.height)
+    return fail(ctx, ESIKF_ERR_ARG, "rgb_colorize: image is %dx%d, camera %dx%d", width, height, ctx->cam.width, ctx->cam.height);
+  CK(cudaSetDevice(ctx->device));
+  const double *dev_state = nullptr;
+  if (int rc = rgb_state(ctx, state, esikf_ctx::RESIDENT_VIO, "rgb_colorize", &dev_state)) return rc;
+  const int n = ctx->rgb_n;
+  cudaStream_t st = ctx->stream;
+  const size_t img_bytes = (size_t)width * height * 3;
+  CK(ctx->rgb_img.reserve(img_bytes));
+  CK(ctx->rgb_keep.reserve((size_t)n + 1));  // keep[n] = 0: the exclusive scan's last entry is the number kept
+  CK(ctx->rgb_dst.reserve((size_t)n + 1));
+  CK(ctx->rgb_color.reserve((size_t)n * 3 + 4));
+  CK(ctx->rgb_xyz.reserve((size_t)n * 3 + 4));
+  CK(ctx->rgb_bgr.reserve((size_t)n * 3 + 4));
+  CK(ctx->rgb_index.reserve((size_t)n + 1));
+  int32_t kept = 0;
+  if (n > 0) {
+    CK(cudaMemcpyAsync(ctx->rgb_img.p, bgr, img_bytes, cudaMemcpyHostToDevice, st));
+    RgbColorArgs a;
+    a.cloud = ctx->rgb_cloud.p, a.n = n, a.bgr = ctx->rgb_img.p, a.state = dev_state, a.blind = blind_rgb_points;
+    cam_dev(ctx, a.cam);
+    double Jdp_dR[9];
+    vio_consts(ctx, a.Rci, a.Pci, Jdp_dR);
+    a.keep = ctx->rgb_keep.p, a.color = ctx->rgb_color.p;
+    rgb_color_kernel<<<(n + 1 + 255) / 256, 256, 0, st>>>(a);
+    // device-wide scan: select_scan_kernel's single CTA took 90 % of the pass at 300 k points (DESIGN.md §8)
+    size_t tmp_bytes = 0;
+    cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, ctx->rgb_keep.p, ctx->rgb_dst.p, n + 1, st);
+    CK(ctx->rgb_scan_tmp.reserve(tmp_bytes + 16));
+    CK(cub::DeviceScan::ExclusiveSum(ctx->rgb_scan_tmp.p, tmp_bytes, ctx->rgb_keep.p, ctx->rgb_dst.p, n + 1, st));
+    rgb_scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(ctx->rgb_keep.p, ctx->rgb_dst.p, n, ctx->rgb_cloud.p, ctx->rgb_color.p, ctx->rgb_xyz.p, ctx->rgb_bgr.p,
+                                                        ctx->rgb_index.p);
+    ctx->launches += 4;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(&kept, ctx->rgb_dst.p + n, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+  }
+  *n_out = kept;
+  if (kept > cap) return fail(ctx, ESIKF_ERR_ARG, "rgb_colorize: %d points kept, room for %d", kept, cap);
+  if (kept > 0) {
+    CK(cudaMemcpyAsync(xyz_out, ctx->rgb_xyz.p, (size_t)kept * 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(bgr_out, ctx->rgb_bgr.p, (size_t)kept * 3, cudaMemcpyDeviceToHost, st));
+    if (index_out) CK(cudaMemcpyAsync(index_out, ctx->rgb_index.p, (size_t)kept * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+  }
   return ESIKF_OK;
 }
 

@@ -554,6 +554,16 @@ __device__ __forceinline__ void p_imu(const double *extR, const double *extT, fl
   pi1 = __dadd_rn(dot3_rn(extR[3], extR[4], extR[5], px, py, pz), extT[1]);
   pi2 = __dadd_rn(dot3_rn(extR[6], extR[7], extR[8], px, py, pz), extT[2]);
 }
+// World point of a body point, rounded to float: R (extR p + extT) + t with the pose (R row-major, t) of a packed state
+// (pointBodyToWorld / RGBpointBodyToWorld, LIVMapper.cpp:645-649, 682-690). No FMA contraction: the float rounding decides
+// the voxel key of the map and is what the coloured scan publishes.
+__device__ __forceinline__ void world_point_f(const double *R, const double *t, const double *extR, const double *extT, float fx, float fy, float fz, float w[3]) {
+  double q0, q1, q2;
+  p_imu(extR, extT, fx, fy, fz, q0, q1, q2);
+  w[0] = (float)__dadd_rn(dot3_rn(R[0], R[1], R[2], q0, q1, q2), t[0]);
+  w[1] = (float)__dadd_rn(dot3_rn(R[3], R[4], R[5], q0, q1, q2), t[1]);
+  w[2] = (float)__dadd_rn(dot3_rn(R[6], R[7], R[8], q0, q1, q2), t[2]);
+}
 // cross-matrix vector of the point (voxel_map.cpp:352-359): extR p + extT with z = 0.001 when the raw z is 0
 __device__ __forceinline__ void cross_vec(const double *extR, const double *extT, float fx, float fy, float fz, double &cx, double &cy, double &cz) {
   p_imu(extR, extT, fx, fy, fz, cx, cy, cz);

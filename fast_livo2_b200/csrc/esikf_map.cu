@@ -71,14 +71,10 @@ __global__ void __launch_bounds__(256) map_points_kernel(const MapArena A, const
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= a.n) return;
   const float fx = a.pts[3 * (size_t)i], fy = a.pts[3 * (size_t)i + 1], fz = a.pts[3 * (size_t)i + 2];
-  // world point: rot * (extR p + extT) + t, stored as float (LIVMapper.cpp:645-649) — no FMA contraction, the float
-  // rounding decides the voxel key
-  double q0, q1, q2;
-  p_imu(a.extR, a.extT, fx, fy, fz, q0, q1, q2);
-  double pw[3];
-  pw[0] = (double)(float)__dadd_rn(dot3_rn(sR[0], sR[1], sR[2], q0, q1, q2), st[0]);
-  pw[1] = (double)(float)__dadd_rn(dot3_rn(sR[3], sR[4], sR[5], q0, q1, q2), st[1]);
-  pw[2] = (double)(float)__dadd_rn(dot3_rn(sR[6], sR[7], sR[8], q0, q1, q2), st[2]);
+  // world point: rot * (extR p + extT) + t, stored as float (LIVMapper.cpp:645-649)
+  float wf[3];
+  world_point_f(sR, st, a.extR, a.extT, fx, fy, fz, wf);
+  const double pw[3] = {wf[0], wf[1], wf[2]};
   // covariance
   double b6[6], cv[3];
   if (a.build) {

@@ -26,28 +26,48 @@ struct CamDev {
   double d[5];
 };
 
+// A double whose every operation is rounded on its own, never contracted into an FMA: what a host compiled without FMA
+// contraction (the reference, the oracle) computes. The camera projection and the frame pose below are written once, over
+// their number type: plain double in the VIO update kernels (which nvcc contracts), Rn where a result must equal the host's
+// bit for bit (the coloured scan, esikf_color.cu).
+struct Rn {
+  double v;
+  __device__ __forceinline__ Rn(double x = 0.0) : v(x) {}
+  __device__ __forceinline__ explicit operator double() const { return v; }
+  friend __device__ __forceinline__ Rn operator+(Rn a, Rn b) { return __dadd_rn(a.v, b.v); }
+  friend __device__ __forceinline__ Rn operator-(Rn a, Rn b) { return __dsub_rn(a.v, b.v); }
+  friend __device__ __forceinline__ Rn operator*(Rn a, Rn b) { return __dmul_rn(a.v, b.v); }
+  friend __device__ __forceinline__ Rn operator/(Rn a, Rn b) { return __ddiv_rn(a.v, b.v); }
+  friend __device__ __forceinline__ Rn operator-(Rn a) { return -a.v; }
+  friend __device__ __forceinline__ Rn &operator+=(Rn &a, Rn b) { return a = a + b; }
+  friend __device__ __forceinline__ bool operator<(Rn a, Rn b) { return a.v < b.v; }
+  friend __device__ __forceinline__ bool operator>(Rn a, Rn b) { return a.v > b.v; }
+  friend __device__ __forceinline__ Rn sqrt(Rn a) { return __dsqrt_rn(a.v); }
+  friend __device__ __forceinline__ Rn atan(Rn a) { return ::atan(a.v); }  // CUDA's atan: within 2 ulp, not always glibc's
+};
+
 // vk::PinholeCamera::world2cam / vk::EquidistantCamera::world2cam (vikit, unpinned; restated from its published algorithm)
-__device__ __forceinline__ void world2cam(const CamDev &cam, double X, double Y, double Z, double &u, double &v) {
-  double x = X / Z, y = Y / Z;
+template <class T> __device__ __forceinline__ void world2cam(const CamDev &cam, T X, T Y, T Z, T &u, T &v) {
+  T x = X / Z, y = Y / Z;
   if (cam.model == 0) {
     if (!(fabs(cam.d[0]) > 0.0000001)) {
       u = cam.fx * x + cam.cx;
       v = cam.fy * y + cam.cy;
     } else {
-      double r2 = x * x + y * y, r4 = r2 * r2, r6 = r4 * r2;
-      double a1 = 2 * x * y, a2 = r2 + 2 * x * x, a3 = r2 + 2 * y * y;
-      double cdist = 1 + cam.d[0] * r2 + cam.d[1] * r4 + cam.d[4] * r6;
-      double xd = x * cdist + cam.d[2] * a1 + cam.d[3] * a2;
-      double yd = y * cdist + cam.d[2] * a3 + cam.d[3] * a1;
+      T r2 = x * x + y * y, r4 = r2 * r2, r6 = r4 * r2;
+      T a1 = 2 * x * y, a2 = r2 + 2 * x * x, a3 = r2 + 2 * y * y;
+      T cdist = 1 + cam.d[0] * r2 + cam.d[1] * r4 + cam.d[4] * r6;
+      T xd = x * cdist + cam.d[2] * a1 + cam.d[3] * a2;
+      T yd = y * cdist + cam.d[2] * a3 + cam.d[3] * a1;
       u = xd * cam.fx + cam.cx;
       v = yd * cam.fy + cam.cy;
     }
   } else {
-    double r = sqrt(x * x + y * y);
-    double theta = atan(r);
-    double t2 = theta * theta, t4 = t2 * t2, t6 = t4 * t2, t8 = t4 * t4;
-    double theta_d = theta * (1 + cam.d[0] * t2 + cam.d[1] * t4 + cam.d[2] * t6 + cam.d[3] * t8);
-    double scaling = (r > 1e-8) ? theta_d / r : 1.0;
+    T r = sqrt(x * x + y * y);
+    T theta = atan(r);
+    T t2 = theta * theta, t4 = t2 * t2, t6 = t4 * t2, t8 = t4 * t4;
+    T theta_d = theta * (1 + cam.d[0] * t2 + cam.d[1] * t4 + cam.d[2] * t6 + cam.d[3] * t8);
+    T scaling = (r > 1e-8) ? theta_d / r : 1.0;
     u = cam.fx * x * scaling + cam.cx;
     v = cam.fy * y * scaling + cam.cy;
   }
@@ -150,25 +170,29 @@ struct __align__(128) VioSmem {
   ReduceSmem<VIO_WARPS> red;
 };
 
+// The frame pose of the packed state `st`, one element per call: Rcw = Rci * Rwi^T (vio.cpp:1542) and, from it,
+// Pcw = -Rci Rwi^T Pwi + Pci (:1543). updateFrameState (:1690-1697) is the same arithmetic. global: `st` lies in global memory,
+// written by an earlier launch, else it is the CTA's resident copy.
+template <class T> __device__ __forceinline__ double frame_rcw(const double *Rci, const double *st, bool global, int e) {
+  const int r = e / 3, c = e % 3;
+  T s = 0.0;
+  for (int k = 0; k < 3; k++) s += T(Rci[r * 3 + k]) * T(ld_state(st + S_R + c * 3 + k, global));
+  return (double)s;
+}
+template <class T> __device__ __forceinline__ double frame_pcw(const double *Rcw, const double *Pci, const double *st, bool global, int r) {
+  T s = 0.0;
+  for (int k = 0; k < 3; k++) s += T(Rcw[r * 3 + k]) * T(ld_state(st + S_P + k, global));
+  return (double)(-s + T(Pci[r]));
+}
+
 // Per-iteration constants of updateState (vio.cpp:1540-1544): Rcw, Pcw, inv_expo_time of the packed state `st` (global: the
 // update's state in global memory, else the CTA's resident copy).
 __device__ __forceinline__ void vio_load_consts(VioSmem &sm, const VioKernelArgs &a, const double *st, bool global) {
   const int tid = threadIdx.x;
-  if (tid < 9) {
-    // Rcw = Rci * Rwi^T  (vio.cpp:1542)
-    const int r = tid / 3, c = tid % 3;
-    double s = 0;
-    for (int k = 0; k < 3; k++) s += a.Rci[r * 3 + k] * ld_state(st + S_R + c * 3 + k, global);
-    sm.Rcw[tid] = s;
-  }
+  if (tid < 9) sm.Rcw[tid] = frame_rcw<double>(a.Rci, st, global, tid);
   if (tid == 0) sm.inv_expo = ld_state(st + S_EXPO, global);
   __syncthreads();
-  if (tid < 3) {
-    // Pcw = -Rci Rwi^T Pwi + Pci  (:1543)
-    double s = 0;
-    for (int k = 0; k < 3; k++) s += sm.Rcw[tid * 3 + k] * ld_state(st + S_P + k, global);
-    sm.Pcw[tid] = -s + a.Pci[tid];
-  }
+  if (tid < 3) sm.Pcw[tid] = frame_pcw<double>(sm.Rcw, a.Pci, st, global, tid);
   __syncthreads();
 }
 

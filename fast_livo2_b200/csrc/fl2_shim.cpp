@@ -328,6 +328,26 @@ void VoxelMapManager::UpdateVoxelMap() {
   UpdateMirror();
 }
 
+void VoxelMapManager::SetWorldCloud(const std::vector<PointXYZ> *dense_scan) {
+  if (!ctx_) {
+    last_status_ = ESIKF_ERR_STATE, last_error_ = "SetWorldCloud: no device context";
+    return;
+  }
+  double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
+  float *pts = dense_scan ? st_pts_.get(dense_scan->size() * 3 + 3) : nullptr;
+  if (!sbuf || (dense_scan && !pts)) {
+    last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
+    return;
+  }
+  state_.pack(sbuf);  // _state == state_ after StateEstimation (LIVMapper.cpp:371)
+  int n = 0;
+  if (dense_scan) {
+    n = (int)dense_scan->size();
+    for (int i = 0; i < n; i++) pts[3 * i] = (*dense_scan)[i].x, pts[3 * i + 1] = (*dense_scan)[i].y, pts[3 * i + 2] = (*dense_scan)[i].z;
+  }
+  if ((last_status_ = esikf_rgb_set_cloud(ctx_, pts, n, sbuf)) != 0) last_error_ = esikf_last_error(ctx_);
+}
+
 // src/voxel_map.cpp:924-948: nothing until the sensor moved sliding_thresh, then roots further than half_map_size voxels go
 void VoxelMapManager::mapSliding() {
   if (!ctx_ || !device_map_) {
@@ -629,6 +649,46 @@ void VIOManager::SetReferenceImages(const GrayImage *imgs, int n) {
   ref_imgs_current_ = last_status_ == 0;
   patch_ref_img_ = nullptr;  // the per-patch warpAffine uploads its own image again
   if (last_status_) last_error_ = n > 0 ? esikf_last_error(ctx_) : "SetReferenceImages: no image";
+}
+
+void VIOManager::ColorizeFrameWorld(const BgrImage &img_rgb, double blind_rgb_points, std::vector<PointXYZRGB> &laserCloudWorldRGB) {
+  laserCloudWorldRGB.clear();
+  if (!ctx_ || !state) {
+    last_status_ = ESIKF_ERR_STATE, last_error_ = "ColorizeFrameWorld: no device context or state";
+    return;
+  }
+  double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
+  if (!sbuf) {
+    last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
+    return;
+  }
+  state->pack(sbuf);
+  int32_t kept = 0;
+  // the staging holds the largest coloured scan seen so far; a larger one is computed again into grown buffers
+  for (int attempt = 0; attempt < 2; attempt++) {
+    float *xyz = st_rgb_xyz_.get((size_t)rgb_cap_ * 3 + 3);
+    uint8_t *bgr = st_rgb_bgr_.get((size_t)rgb_cap_ * 3 + 3);
+    if (!xyz || !bgr) {
+      last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
+      return;
+    }
+    last_status_ = esikf_rgb_colorize(ctx_, img_rgb.data, img_rgb.cols, img_rgb.rows, sbuf, blind_rgb_points, rgb_cap_, &kept, xyz, bgr, nullptr);
+    if (last_status_ == ESIKF_ERR_ARG && kept > rgb_cap_) {
+      rgb_cap_ = kept;
+      continue;
+    }
+    if (last_status_) {
+      last_error_ = esikf_last_error(ctx_);
+      return;
+    }
+    laserCloudWorldRGB.resize(kept);
+    for (int i = 0; i < kept; i++) {
+      PointXYZRGB &p = laserCloudWorldRGB[i];
+      p.x = xyz[3 * i], p.y = xyz[3 * i + 1], p.z = xyz[3 * i + 2];
+      p.b = bgr[3 * i], p.g = bgr[3 * i + 1], p.r = bgr[3 * i + 2];
+    }
+    return;
+  }
 }
 
 void VIOManager::SelectSubSparseMap(const SubMapCandidate *c, int n, const GrayImage &img, const double T_cur_w[12]) {

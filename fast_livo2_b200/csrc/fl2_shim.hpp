@@ -216,6 +216,11 @@ class VoxelMapManager {
   void mapSliding();  // include/voxel_map.h:247 / src/voxel_map.cpp:924-948 (device-resident map); uses position_last_, sliding_thresh, half_map_size
   V3D last_slide_position;
   void MaterializePointLists();                       // fills the four lists from the last StateEstimation (idempotent per call of it)
+  // The world cloud of this LIO tick for the coloured scan VIOManager::ColorizeFrameWorld publishes (LIVMapper.cpp:435-443):
+  // every point of `dense_scan` (feats_undistort, dense_map_en = true) or, with nullptr, of feats_down_body_ as the last
+  // StateEstimation left it on the device (dense_map_en = false), moved to the world frame with state_. Call after
+  // StateEstimation, once per LIO tick.
+  void SetWorldCloud(const std::vector<PointXYZ> *dense_scan = nullptr);
   esikf_ctx *context() { return ctx_; }
 
  private:
@@ -263,6 +268,8 @@ struct SubMapCandidate {
 };
 
 struct GrayImage { const uint8_t *data = nullptr; int cols = 0, rows = 0; };  // cv::Mat CV_8UC1 continuous
+struct BgrImage { const uint8_t *data = nullptr; int cols = 0, rows = 0; };   // cv::Mat CV_8UC3 continuous (img_rgb)
+struct PointXYZRGB { float x, y, z; uint8_t r, g, b; };                          // pcl::PointXYZRGB's fields as published
 
 class VIOManager {
  public:
@@ -311,6 +318,11 @@ class VIOManager {
   void getImagePatch(const GrayImage &img, const double pc[2], float *patch_tmp, int level);
   void warpAffine(const double A_cur_ref[4] /* row-major 2x2 */, const GrayImage &img_ref, const double px_ref[2], int level_ref, int search_level,
                   int pyramid_level, int halfpatch_size, float *patch);
+  // LIVMapper::publish_frame_world (src/LIVMapper.cpp:1140-1173) on the device: the world cloud of the last
+  // VoxelMapManager::SetWorldCloud, coloured from img_rgb (the camera's size) with the frame pose of *state (the VIO
+  // posterior after computeJacobianAndUpdateEKF), the points closer than blind_rgb_points dropped. Fills laserCloudWorldRGB
+  // in the reference's order. Call once per VIO tick, after computeJacobianAndUpdateEKF.
+  void ColorizeFrameWorld(const BgrImage &img_rgb, double blind_rgb_points, std::vector<PointXYZRGB> &laserCloudWorldRGB);
 
  private:
   const uint8_t *patch_img_ = nullptr, *patch_ref_img_ = nullptr;  // what the per-patch helpers uploaded last
@@ -326,6 +338,9 @@ class VIOManager {
   std::vector<int32_t> sel_ref_idx_, sel_sl_;
   std::vector<double> sel_px_, sel_A_;
   std::vector<GrayImage> ref_imgs_;  // SetReferenceImages (the caller keeps the pixels, as Feature::img_ does)
+  PinnedBuf<float> st_rgb_xyz_;      // ColorizeFrameWorld's output staging, grown to the largest coloured scan seen
+  PinnedBuf<uint8_t> st_rgb_bgr_;
+  int32_t rgb_cap_ = 0;
   bool ref_imgs_current_ = false;    // false once the per-patch warpAffine replaced the device's reference images
 };
 

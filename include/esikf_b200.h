@@ -340,6 +340,30 @@ int esikf_vio_warp_affine(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_inde
                           const double *A_cur_ref /* n x 4 */, const int32_t *search_level /* n */,
                           float *warp_patch_out /* n x levels*64 */);
 
+/* ---------------------------------------------------------------- coloured scan (publish_frame_world)
+ * The coloured point cloud LIVMapper publishes after each VIO update (src/LIVMapper.cpp:1140-1173), computed on the device.
+ * One call per tick of each kind:
+ *   LIO tick : esikf_lio_run, then esikf_rgb_set_cloud (before the VIO update overwrites the resident LIO posterior)
+ *   VIO tick : esikf_vio_run, then esikf_rgb_colorize
+ * With several ranks, both calls cover the whole cloud on every rank (the poses are identical on every rank).
+ * The context owns the cloud and image buffers; esikf_destroy frees them. */
+/* The world cloud of this LIO tick (LIVMapper.cpp:435-443, RGBpointBodyToWorld at :682-690):
+ * p_w = rot_end * (extR * p_body + extT) + pos_end in double, stored as float.
+ * pts_xyz == NULL: the resident scan of esikf_lio_set_scan, n ignored (dense_map_en = false); else n body points, host float
+ * xyz (feats_undistort, dense_map_en = true). state == NULL: the posterior the last esikf_lio_run left on the device
+ * (ESIKF_ERR_STATE when no LIO update ran or a VIO update ran since); else a packed host state. The host buffers may be
+ * reused as soon as the call returns. */
+int esikf_rgb_set_cloud(esikf_ctx *ctx, const float *pts_xyz, int32_t n, const double *state);
+/* publish_frame_world on the cloud of esikf_rgb_set_cloud with the image `bgr` (8-bit B G R interleaved, width x height of
+ * the camera, row-major): a point is kept when pf[2] >= 0, isInFrame(pc.cast<int>(), 3) holds and pf.norm() > blind_rgb_points,
+ * with pf = new_frame_->w2f(p_w), pc = w2c(p_w) and the frame pose of updateFrameState (vio.cpp:1690-1697) of `state`
+ * (NULL: the posterior resident after esikf_vio_run; else a packed host state). Its colour is getInterpolatedPixel
+ * (vio.cpp:1742-1760), each channel converted to uint8 as the assignment to PointXYZRGB does (truncation).
+ * The survivors come out in cloud order: xyz_out (3 floats each), bgr_out (B, G, R each), index_out (their cloud index,
+ * nullable). *n_out = the number kept; if it exceeds cap, nothing else is written and the call returns ESIKF_ERR_ARG. */
+int esikf_rgb_colorize(esikf_ctx *ctx, const uint8_t *bgr, int32_t width, int32_t height, const double *state, double blind_rgb_points,
+                       int32_t cap, int32_t *n_out, float *xyz_out, uint8_t *bgr_out, int32_t *index_out);
+
 /* ---------------------------------------------------------------- multi-GPU (one process per GPU)
  * The residual point / patch set is sharded by contiguous blocks; each iteration all-reduces the
  * packed information buffer [HTH upper | HTz | M | sum|d| ...] and every rank solves redundantly.
