@@ -92,6 +92,14 @@ int main() {
     std::vector<PointXYZRGB> laserCloudWorldRGB;
     vio_manager.ColorizeFrameWorld(BgrImage{bgr.data(), 64, 48}, /*blind_rgb_points*/ 0.01, laserCloudWorldRGB);
     std::printf("tick %d coloured scan: status %d, %zu points\n", tick, vio_manager.last_status_, laserCloudWorldRGB.size());
+    // generateVisualMapPoints (vio.cpp:804-906) on the scan the device holds: grid of initializeVIO (vio/grid_size 5,
+    // grid_n_height 17 on a 64 x 48 image: 2-pixel cells, 32 x 24) and border (patch_size_half + 1) << patch_pyrimid_level;
+    // the retrieval marked the candidate's cell TYPE_MAP. The VisualPoint / Feature objects are the caller's (INTEGRATION.md §2).
+    std::vector<uint8_t> grid_num(32 * 24, 0);
+    grid_num[12 * 32 + 16] = 1;
+    std::vector<NewVisualPoint> new_points;
+    vio_manager.GenerateVisualMapPoints(grid_num, 2, 32, 24, 5 << 2, nullptr, nullptr, new_points);
+    std::printf("tick %d new visual map points: status %d, %zu points\n", tick, vio_manager.last_status_, new_points.size());
   }
   // somebody wants the warp patches of the last selection on the host after all
   vio_manager.MaterializeWarpPatches();

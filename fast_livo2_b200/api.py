@@ -113,6 +113,7 @@ def load_library():
     lib.esikf_vio_select_patches.argtypes = [vp, C.c_int32] + [vp] * 12 + [C.c_double, C.POINTER(VioSelectCfgC), ip, vp, vp, vp, vp, vp]
     lib.esikf_rgb_set_cloud.argtypes = [vp, vp, C.c_int32, vp]
     lib.esikf_rgb_colorize.argtypes = [vp, vp, C.c_int32, C.c_int32, vp, C.c_double, C.c_int32, ip, vp, vp, vp]
+    lib.esikf_vio_generate_points.argtypes = [vp, vp, vp, vp, C.c_int32, vp, vp, C.c_int32, vp] + [C.c_int32] * 5 + [vp, C.c_int32, ip] + [vp] * 8
     lib.esikf_comm_unique_id.argtypes = [C.c_char_p]
     lib.esikf_comm_init.argtypes = [vp, C.c_int32, C.c_int32, C.c_char_p]
     lib.esikf_comm_rank.argtypes = [vp, ip, ip]
@@ -130,6 +131,7 @@ def load_library():
 
 TUNE_STAGE_LDG = 1
 TUNE_VIO_TMA = 2  # esikf_set_tuning flag: stage LIO plane records with __ldg copies instead of cp.async.bulk (measurement variant)
+GEN_ADD_FROM = 0x40000000  # esikf_vio_generate_points: the source of a winner from the add_from list
 DEFAULT_LOOP_MODE = 2  # esikf_set_loop_mode: 2 (alias 1) persistent kernel per update, 0 per-iteration launches
 
 class MapCfgC(C.Structure):
@@ -148,7 +150,7 @@ EXPORTED_SYMBOLS = [
     "esikf_set_extrinsics", "esikf_set_lidar_extrinsics", "esikf_map_upload", "esikf_map_patch", "esikf_map_device_init", "esikf_map_device_build", "esikf_map_device_update", "esikf_map_device_update_points", "esikf_map_device_slide", "esikf_map_device_stats", "esikf_map_device_capacity", "esikf_map_device_download", "esikf_map_device_export", "esikf_lio_fetch_normals", "esikf_lio_set_scan", "esikf_lio_run", "esikf_lio_fetch",
     "esikf_lio_update", "esikf_lio_fetch_point_cov", "esikf_vio_set_camera", "esikf_vio_set_image", "esikf_vio_set_patches",
     "esikf_vio_run", "esikf_vio_fetch", "esikf_vio_update", "esikf_vio_get_image_patch", "esikf_vio_set_ref_images",
-    "esikf_vio_warp_patches", "esikf_vio_select_patches", "esikf_vio_warp_affine", "esikf_vio_set_inverse_refs", "esikf_rgb_set_cloud", "esikf_rgb_colorize", "esikf_comm_unique_id", "esikf_comm_init", "esikf_comm_rank", "esikf_shard_range", "esikf_peer_export", "esikf_peer_attach", "esikf_profile_kernel", "esikf_set_kernel_timing", "esikf_get_kernel_timing", "esikf_set_phase_stamps", "esikf_get_phase_stamps",
+    "esikf_vio_warp_patches", "esikf_vio_select_patches", "esikf_vio_warp_affine", "esikf_vio_set_inverse_refs", "esikf_rgb_set_cloud", "esikf_rgb_colorize", "esikf_vio_generate_points", "esikf_comm_unique_id", "esikf_comm_init", "esikf_comm_rank", "esikf_shard_range", "esikf_peer_export", "esikf_peer_attach", "esikf_profile_kernel", "esikf_set_kernel_timing", "esikf_get_kernel_timing", "esikf_set_phase_stamps", "esikf_get_phase_stamps",
 ]
 
 
@@ -508,6 +510,41 @@ class Context:
                                              xyz.ctypes.data, col.ctypes.data, idx.ctypes.data))
         k = n.value
         return dict(xyz=xyz[:k], bgr=col[:k], index=idx[:k])
+
+    # ------------------------------------------------------------------ new visual map points (generateVisualMapPoints)
+    def vio_generate_points(self, type_map, grid_size, grid_n_width, grid_n_height, border, pg=None, add_from=None, state=None, cap=None):
+        """generateVisualMapPoints on the device (esikf_vio_generate_points), after vio_run. type_map: (grid_n_height *
+        grid_n_width,) bool / uint8, True where the retrieval set TYPE_MAP; grid_size .. border as initializeVIO left them.
+        pg: None for the pv list the last map_device_update left on the device, else (point_w (n, 3), normal (n, 3), var (n, 3, 3))
+        float64; add_from: None or (pos (m, 3), normal (m, 3)); state: a packed state, or None for the VIO posterior on the device.
+        Returns the winners in cell order: source (int32: scan index, or api.GEN_ADD_FROM | add_from index), cell, pos (k, 3),
+        pc (k, 2), score (k,) float32, normal (k, 3) (sign-flipped as the reference does), var (k, 3, 3), patch (k, 64) float32.
+        cap: room for that many (default: one per cell); fewer than the winners raises."""
+        mask = _c(type_map, np.uint8).reshape(-1)
+        if pg is None:
+            pw = nv = var = None
+            n = 0
+        else:
+            pw, nv, var = _c(pg[0], np.float64).reshape(-1, 3), _c(pg[1], np.float64).reshape(-1, 3), _c(pg[2], np.float64).reshape(-1, 9)
+            n = len(pw)
+            assert len(nv) == n and len(var) == n
+        if add_from is None:
+            ap = an = None
+            m = 0
+        else:
+            ap, an = _c(add_from[0], np.float64).reshape(-1, 3), _c(add_from[1], np.float64).reshape(-1, 3)
+            m = len(ap)
+            assert len(an) == m
+        s = None if state is None else _c(state, np.float64)
+        cap = len(mask) if cap is None else int(cap)
+        k = max(cap, 1)
+        out = dict(source=np.zeros(k, np.int32), cell=np.zeros(k, np.int32), pos=np.zeros((k, 3)), pc=np.zeros((k, 2)), score=np.zeros(k, np.float32),
+                   normal=np.zeros((k, 3)), var=np.zeros((k, 3, 3)), patch=np.zeros((k, 64), np.float32))
+        cnt = C.c_int32(0)
+        self._ck(self.lib.esikf_vio_generate_points(self.h, _addr(pw), _addr(nv), _addr(var), n, _addr(ap), _addr(an), m, mask.ctypes.data, len(mask),
+                                                    int(grid_size), int(grid_n_width), int(grid_n_height), int(border), _addr(s), cap, C.byref(cnt),
+                                                    *[out[f].ctypes.data for f in ("source", "cell", "pos", "pc", "score", "normal", "var", "patch")]))
+        return {f: v[:cnt.value] for f, v in out.items()}
 
     # ------------------------------------------------------------------ multi-GPU / measurement
     def vio_set_inverse_refs(self, ref_img_index, ref_px, ref_f, ref_R, ref_pos):

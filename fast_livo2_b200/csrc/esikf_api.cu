@@ -23,6 +23,7 @@
 #include "esikf_fused.cu"
 #include "esikf_map.cu"
 #include "esikf_color.cu"
+#include "esikf_generate.cu"
 
 using namespace esikf;
 
@@ -169,6 +170,10 @@ struct esikf_ctx {
   DevBuf<unsigned char> map_sort_tmp;
   int map_pt_n = 0;            // points the normal snapshot / last map step covers
   bool map_normals_valid = false;
+  // points of the pv list (pv_list_ after LIVMapper.cpp:413-424) the last esikf_map_device_update left in map_pt (point_w | var)
+  // and map_pt_normal (pv.normal), which esikf_vio_generate_points(point_w = NULL) reads; -1 when map_pt holds anything else
+  int pv_n = -1;
+  DevBuf<double> fetch_normal;  // esikf_lio_fetch_normals gathering for a later LIO run: map_pt_normal keeps the pv list's normals
   int map_hash_bits = 0;
   esikf_map_stats map_last{};
   // esikf_map_device_export: points of the last applied tick (its touched list is map_touched, its sorted positions 0..n),
@@ -251,6 +256,14 @@ struct esikf_ctx {
   DevBuf<uint8_t> rgb_img, rgb_color, rgb_bgr, rgb_scan_tmp;
   DevBuf<int32_t> rgb_keep, rgb_dst, rgb_index;
   int rgb_n = -1;  // points of the cloud, -1 before esikf_rgb_set_cloud
+
+  // new visual map points (esikf_vio_generate_points): a host scan / add_from list, the TYPE_MAP mask, the per-cell winner keys
+  // and the winners' records
+  DevBuf<double> gen_pt, gen_normal, gen_add, gen_out_d;
+  DevBuf<uint8_t> gen_mask;
+  DevBuf<unsigned long long> gen_key;
+  DevBuf<int32_t> gen_i;
+  DevBuf<float> gen_out_f;
 
   // multi-GPU
   int rank = 0, nranks = 1;
@@ -740,13 +753,14 @@ static int map_apply_exported(esikf_ctx *ctx, int n, bool build) {
 static int map_from_scan(esikf_ctx *ctx, const double *state, bool build) {
   if (!ctx) return ESIKF_ERR_ARG;
   ctx->map_export_points = -1;
+  ctx->pv_n = -1;  // map_pt is rewritten below
   if (!ctx->dev_map) return fail(ctx, ESIKF_ERR_STATE, "map_device_%s before esikf_map_device_init", build ? "build" : "update");
   if (!ctx->have_ext) return fail(ctx, ESIKF_ERR_STATE, "map_device_%s before set_extrinsics", build ? "build" : "update");
   if (!build && ctx->scan_fresh) return fail(ctx, ESIKF_ERR_STATE, "map_device_update: the resident scan has not been through esikf_lio_run yet");
   if (build && ctx->map_last.roots > 0) return fail(ctx, ESIKF_ERR_STATE, "map_device_build needs an empty map (esikf_map_device_init resets it)");
   CK(cudaSetDevice(ctx->device));
   const int n = ctx->n_pts;
-  if (n == 0) return ctx->map_export_points = 0, ESIKF_OK;
+  if (n == 0) return ctx->map_export_points = 0, ctx->pv_n = build ? -1 : 0, ESIKF_OK;
   int rc = map_reserve_tick(ctx, n);
   if (rc) return rc;
   cudaStream_t st = ctx->stream;
@@ -775,7 +789,9 @@ static int map_from_scan(esikf_ctx *ctx, const double *state, bool build) {
   a.pt = ctx->map_pt.p, a.pt_slot = ctx->map_key_in.p, a.pt_idx = ctx->map_idx_in.p, a.invalid_slot = ctx->map.hash_cap;
   map_points_kernel<<<(n + 255) / 256, 256, 0, st>>>(ctx->arena(), a);
   ctx->map_pt_n = n, ctx->map_normals_valid = !build;
-  return map_apply_exported(ctx, n, build);
+  rc = map_apply_exported(ctx, n, build);
+  if (!rc && !build) ctx->pv_n = n;
+  return rc;
 }
 
 int esikf_map_device_build(esikf_ctx *ctx, const double *state) {
@@ -785,7 +801,7 @@ int esikf_map_device_build(esikf_ctx *ctx, const double *state) {
 int esikf_map_device_update(esikf_ctx *ctx, const double *state) { return map_from_scan(ctx, state, false); }
 
 int esikf_map_device_update_points(esikf_ctx *ctx, const double *point_w, const double *var, int32_t n) {
-  if (ctx) ctx->map_export_points = -1;
+  if (ctx) ctx->map_export_points = -1, ctx->pv_n = -1;
   if (!ctx || n < 0 || (n > 0 && (!point_w || !var))) return fail(ctx, ESIKF_ERR_ARG, "map_device_update_points: bad argument");
   if (!ctx->dev_map) return fail(ctx, ESIKF_ERR_STATE, "map_device_update_points before esikf_map_device_init");
   if (n == 0) return ctx->map_export_points = 0, ESIKF_OK;
@@ -944,12 +960,14 @@ int esikf_lio_fetch_normals(esikf_ctx *ctx, double *normals) {
   CK(cudaSetDevice(ctx->device));
   const int n = ctx->n_pts;
   if (n == 0) return ESIKF_OK;
+  const double *src = ctx->map_pt_normal.p;
   if (!(ctx->dev_map && ctx->map_normals_valid && ctx->map_pt_n == n)) {
-    CK(ctx->map_pt_normal.reserve((size_t)n * 3 + 4));
-    gather_normals_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(ctx->normal_plane.p, ctx->map.recs.p, n, ctx->map_pt_normal.p);
+    CK(ctx->fetch_normal.reserve((size_t)n * 3 + 4));
+    gather_normals_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(ctx->normal_plane.p, ctx->map.recs.p, n, ctx->fetch_normal.p);
     ctx->launches++;
+    src = ctx->fetch_normal.p;
   }
-  CK(cudaMemcpyAsync(normals, ctx->map_pt_normal.p, (size_t)n * 3 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(normals, src, (size_t)n * 3 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   return ESIKF_OK;
 }
@@ -1746,6 +1764,99 @@ int esikf_rgb_colorize(esikf_ctx *ctx, const uint8_t *bgr, int32_t width, int32_
     if (index_out) CK(cudaMemcpyAsync(index_out, ctx->rgb_index.p, (size_t)kept * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
   }
+  return ESIKF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------- new visual map points
+int esikf_vio_generate_points(esikf_ctx *ctx, const double *point_w, const double *normal, const double *var, int32_t n, const double *add_pos,
+                              const double *add_normal, int32_t n_add, const uint8_t *type_map, int32_t n_cells, int32_t grid_size, int32_t grid_n_width,
+                              int32_t grid_n_height, int32_t border, const double *state, int32_t cap, int32_t *n_out, int32_t *source_out,
+                              int32_t *cell_out, double *pos_out, double *pc_out, float *score_out, double *normal_out, double *var_out, float *patch_out) {
+  if (!ctx || !n_out || !type_map || cap < 0 || n_add < 0 || (n_add > 0 && (!add_pos || !add_normal)) || (point_w && (n < 0 || !normal || !var)))
+    return fail(ctx, ESIKF_ERR_ARG, "vio_generate_points: bad argument");
+  if (grid_size <= 0 || grid_n_width <= 0 || grid_n_height <= 0 || border < 0)
+    return fail(ctx, ESIKF_ERR_ARG, "vio_generate_points: grid %d px, %d x %d cells, border %d", grid_size, grid_n_width, grid_n_height, border);
+  if ((long long)grid_n_width * grid_n_height != n_cells)
+    return fail(ctx, ESIKF_ERR_ARG, "vio_generate_points: the TYPE_MAP mask has %d cells, the grid %d x %d", n_cells, grid_n_width, grid_n_height);
+  if (!ctx->have_cam) return fail(ctx, ESIKF_ERR_STATE, "vio_generate_points before vio_set_camera");
+  if (ctx->img_w != ctx->cam.width || ctx->img_h != ctx->cam.height) return fail(ctx, ESIKF_ERR_STATE, "vio_generate_points before vio_set_image");
+  if (!point_w && ctx->pv_n < 0)
+    return fail(ctx, ESIKF_ERR_STATE, "vio_generate_points(point_w = NULL): no esikf_map_device_update of the resident scan left its points on the device");
+  if ((long long)(point_w ? n : ctx->pv_n) + n_add >= ESIKF_GEN_ADD_FROM) return fail(ctx, ESIKF_ERR_ARG, "vio_generate_points: too many points");
+  CK(cudaSetDevice(ctx->device));
+  *n_out = 0;
+  const double *dev_state = nullptr;
+  if (int rc = rgb_state(ctx, state, esikf_ctx::RESIDENT_VIO, "vio_generate_points", &dev_state)) return rc;
+  if (!point_w) n = ctx->pv_n;
+  if (n <= 10) return ESIKF_OK;  // :806, add_from included
+  cudaStream_t st = ctx->stream;
+  const int L = n_cells;
+  const size_t N = (size_t)n;
+  GenArgs a;
+  a.img = ctx->img.p;
+  cam_dev(ctx, a.cam);
+  double Jdp_dR[9];
+  vio_consts(ctx, a.Rci, a.Pci, Jdp_dR);
+  a.state = dev_state, a.n = n, a.n_add = n_add, a.pt_stride = MAP_PT_D;
+  a.grid_size = grid_size, a.grid_n_width = grid_n_width, a.length = L, a.border = border;
+  if (point_w) {  // pv_list_ from the host: point_w | var rows as map_pt holds them
+    CK(ctx->gen_pt.reserve(N * MAP_PT_D + 4));
+    CK(ctx->gen_normal.reserve(N * 3 + 4));
+    CK(cudaMemcpy2DAsync(ctx->gen_pt.p, MAP_PT_D * sizeof(double), point_w, 3 * sizeof(double), 3 * sizeof(double), N, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpy2DAsync(ctx->gen_pt.p + 3, MAP_PT_D * sizeof(double), var, 9 * sizeof(double), 9 * sizeof(double), N, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(ctx->gen_normal.p, normal, N * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+    a.pt = ctx->gen_pt.p, a.normal = ctx->gen_normal.p;
+  } else {
+    a.pt = ctx->map_pt.p, a.normal = ctx->map_pt_normal.p;
+  }
+  CK(ctx->gen_add.reserve((size_t)n_add * 6 + 4));
+  if (n_add > 0) {
+    CK(cudaMemcpyAsync(ctx->gen_add.p, add_pos, (size_t)n_add * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(ctx->gen_add.p + 3 * (size_t)n_add, add_normal, (size_t)n_add * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+  }
+  a.add_pos = ctx->gen_add.p, a.add_normal = ctx->gen_add.p + 3 * (size_t)n_add;
+  CK(ctx->gen_mask.reserve(L + 16));
+  CK(ctx->gen_key.reserve(L + 1));
+  CK(ctx->gen_i.reserve(4 * (size_t)L + 2));  // keep | dst | n_kept | source | cell
+  CK(ctx->gen_out_d.reserve(17 * (size_t)L));  // pos 3 | pc 2 | normal 3 | var 9
+  CK(ctx->gen_out_f.reserve(65 * (size_t)L));  // score 1 | patch 64
+  CK(cudaMemcpyAsync(ctx->gen_mask.p, type_map, L, cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(ctx->gen_key.p, 0, (size_t)L * sizeof(unsigned long long), st));
+  a.type_map = ctx->gen_mask.p, a.key = ctx->gen_key.p;
+  int32_t *d_keep = ctx->gen_i.p, *d_dst = d_keep + L, *d_nk = d_dst + L;
+  GenOut o;
+  o.source = d_nk + 1, o.cell = o.source + L;
+  double *od = ctx->gen_out_d.p;
+  o.pos = od, o.pc = od + 3 * (size_t)L, o.normal = od + 5 * (size_t)L, o.var = od + 8 * (size_t)L;
+  o.score = ctx->gen_out_f.p;
+  float *d_patch = ctx->gen_out_f.p + L;
+  gen_score_kernel<<<(n + n_add + GEN_THREADS - 1) / GEN_THREADS, GEN_THREADS, 0, st>>>(a);
+  gen_cells_kernel<<<(L + 255) / 256, 256, 0, st>>>(ctx->gen_key.p, L, d_keep);
+  select_scan_kernel<<<1, SELECT_SCAN_THREADS, 0, st>>>(d_keep, L, d_dst, d_nk);
+  gen_scatter_kernel<<<(L + GEN_THREADS - 1) / GEN_THREADS, GEN_THREADS, 0, st>>>(a, d_keep, d_dst, o);
+  ctx->launches += 4;
+  CK(cudaGetLastError());
+  int32_t nk = 0;
+  CK(cudaMemcpyAsync(&nk, d_nk, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));  // also: the caller may reuse its buffers on return
+  *n_out = nk;
+  if (nk > cap) return fail(ctx, ESIKF_ERR_ARG, "vio_generate_points: %d new points, room for %d", nk, cap);
+  if (nk == 0) return ESIKF_OK;
+  if (patch_out) {
+    image_patch_kernel<<<(nk * 64 + 255) / 256, 256, 0, st>>>(ctx->img.p, ctx->img_w, ctx->img_h, o.pc, nk, 0, d_patch);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(patch_out, d_patch, (size_t)nk * 64 * sizeof(float), cudaMemcpyDeviceToHost, st));
+  }
+  const size_t K = (size_t)nk;
+  if (source_out) CK(cudaMemcpyAsync(source_out, o.source, K * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  if (cell_out) CK(cudaMemcpyAsync(cell_out, o.cell, K * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  if (pos_out) CK(cudaMemcpyAsync(pos_out, o.pos, K * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (pc_out) CK(cudaMemcpyAsync(pc_out, o.pc, K * 2 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (score_out) CK(cudaMemcpyAsync(score_out, o.score, K * sizeof(float), cudaMemcpyDeviceToHost, st));
+  if (normal_out) CK(cudaMemcpyAsync(normal_out, o.normal, K * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (var_out) CK(cudaMemcpyAsync(var_out, o.var, K * 9 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
   return ESIKF_OK;
 }
 

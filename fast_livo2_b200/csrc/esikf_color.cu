@@ -56,9 +56,9 @@ __global__ void __launch_bounds__(256) rgb_color_kernel(const RgbColorArgs a) {
   }
   // V3D p_w(float x, y, z); pf = new_frame_->w2f(p_w) = Rcw p_w + Pcw
   const Rn X = (double)a.cloud[3 * (size_t)i], Y = (double)a.cloud[3 * (size_t)i + 1], Z = (double)a.cloud[3 * (size_t)i + 2];
-  const Rn pf0 = Rn(Rcw[0]) * X + Rn(Rcw[1]) * Y + Rn(Rcw[2]) * Z + Rn(Pcw[0]);
-  const Rn pf1 = Rn(Rcw[3]) * X + Rn(Rcw[4]) * Y + Rn(Rcw[5]) * Z + Rn(Pcw[1]);
-  const Rn pf2 = Rn(Rcw[6]) * X + Rn(Rcw[7]) * Y + Rn(Rcw[8]) * Z + Rn(Pcw[2]);
+  Rn pf[3];
+  frame_point(Rcw, Pcw, X, Y, Z, pf);
+  const Rn pf0 = pf[0], pf1 = pf[1], pf2 = pf[2];
   int keep = 0;
   if (!(pf2 < 0.0)) {
     Rn u, v;

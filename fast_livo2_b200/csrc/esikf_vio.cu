@@ -184,6 +184,11 @@ template <class T> __device__ __forceinline__ double frame_pcw(const double *Rcw
   for (int k = 0; k < 3; k++) s += T(Rcw[r * 3 + k]) * T(ld_state(st + S_P + k, global));
   return (double)(-s + T(Pci[r]));
 }
+// Frame::w2f of a world point with that pose: pf = Rcw p_w + Pcw, each row summed left to right
+template <class T> __device__ __forceinline__ void frame_point(const double *Rcw, const double *Pcw, T X, T Y, T Z, T pf[3]) {
+#pragma unroll
+  for (int r = 0; r < 3; r++) pf[r] = T(Rcw[3 * r]) * X + T(Rcw[3 * r + 1]) * Y + T(Rcw[3 * r + 2]) * Z + T(Pcw[r]);
+}
 
 // Per-iteration constants of updateState (vio.cpp:1540-1544): Rcw, Pcw, inv_expo_time of the packed state `st` (global: the
 // update's state in global memory, else the CTA's resident copy).

@@ -510,6 +510,51 @@ void VoxelMapManager::MaterializePointLists() {
 
 VIOManager::VIOManager(esikf_ctx *shared_ctx) : ctx_(shared_ctx) {}
 
+void VIOManager::GenerateVisualMapPoints(const std::vector<uint8_t> &type_map, int grid_size, int grid_n_width, int grid_n_height, int border,
+                                         const std::vector<pointWithVar> *pg, const std::vector<pointWithVar> *add_from_voxel_map,
+                                         std::vector<NewVisualPoint> &new_points) {
+  new_points.clear();
+  if (!ctx_ || !state) {
+    last_status_ = ESIKF_ERR_STATE, last_error_ = "GenerateVisualMapPoints: no device context or state";
+    return;
+  }
+  double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
+  if (!sbuf) {
+    last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
+    return;
+  }
+  state->pack(sbuf);
+  const size_t n = pg ? pg->size() : 0, m = add_from_voxel_map ? add_from_voxel_map->size() : 0;
+  gen_in_.resize(15 * n + 6 * m + 1);
+  double *pw = gen_in_.data(), *nv = pw + 3 * n, *var = nv + 3 * n, *ap = var + 9 * n, *an = ap + 3 * m;
+  for (size_t i = 0; i < n; i++) {
+    const pointWithVar &p = (*pg)[i];
+    for (int k = 0; k < 3; k++) pw[3 * i + k] = p.point_w[k], nv[3 * i + k] = p.normal[k];
+    memcpy(var + 9 * i, p.var.m, 72);
+  }
+  for (size_t j = 0; j < m; j++)
+    for (int k = 0; k < 3; k++) ap[3 * j + k] = (*add_from_voxel_map)[j].point_w[k], an[3 * j + k] = (*add_from_voxel_map)[j].normal[k];
+  const int cap = (int)type_map.size();  // at most one point per cell
+  gen_src_.resize(cap + 1), gen_cell_.resize(cap + 1), gen_pos_.resize(3 * cap + 3), gen_pc_.resize(2 * cap + 2), gen_normal_.resize(3 * cap + 3);
+  gen_var_.resize(9 * cap + 9), gen_score_.resize(cap + 1), gen_patch_.resize(64 * cap + 64);
+  int32_t k = 0;
+  last_status_ = esikf_vio_generate_points(ctx_, pg ? pw : nullptr, nv, var, (int32_t)n, ap, an, (int32_t)m, type_map.data(), cap, grid_size, grid_n_width,
+                                           grid_n_height, border, sbuf, cap, &k, gen_src_.data(), gen_cell_.data(), gen_pos_.data(), gen_pc_.data(),
+                                           gen_score_.data(), gen_normal_.data(), gen_var_.data(), gen_patch_.data());
+  if (last_status_) {
+    last_error_ = esikf_last_error(ctx_);
+    return;
+  }
+  new_points.resize(k);
+  for (int i = 0; i < k; i++) {
+    NewVisualPoint &q = new_points[i];
+    q.source = gen_src_[i], q.cell = gen_cell_[i], q.score = gen_score_[i];
+    memcpy(q.pos, &gen_pos_[3 * i], sizeof(q.pos)), memcpy(q.pc, &gen_pc_[2 * i], sizeof(q.pc)), memcpy(q.normal, &gen_normal_[3 * i], sizeof(q.normal));
+    memcpy(q.var, &gen_var_[9 * i], sizeof(q.var)), memcpy(q.patch, &gen_patch_[64 * i], sizeof(q.patch));
+  }
+}
+
+
 void VIOManager::initializeVIO() {
   if (!ctx_) return;
   esikf_extrinsics ext;

@@ -270,6 +270,18 @@ struct SubMapCandidate {
 struct GrayImage { const uint8_t *data = nullptr; int cols = 0, rows = 0; };  // cv::Mat CV_8UC1 continuous
 struct BgrImage { const uint8_t *data = nullptr; int cols = 0, rows = 0; };   // cv::Mat CV_8UC3 continuous (img_rgb)
 struct PointXYZRGB { float x, y, z; uint8_t r, g, b; };                          // pcl::PointXYZRGB's fields as published
+// One new visual map point of VIOManager::GenerateVisualMapPoints: what generateVisualMapPoints (src/vio.cpp:864-890) builds
+// its VisualPoint and Feature from. INTEGRATION.md §2 shows the objects made from it.
+struct NewVisualPoint {
+  int32_t source;    // index into pg, or ESIKF_GEN_ADD_FROM | index into add_from_voxel_map
+  int32_t cell;      // grid cell
+  double pos[3];     // VisualPoint::pos_ (pt_var.point_w)
+  double pc[2];      // new_frame_->w2c(pos_): Feature::px_
+  double normal[3];  // VisualPoint::normal_ (pt_var.normal, negated when cos_theta < 0)
+  double var[9];     // VisualPoint::covariance_ (pt_var.var, row-major)
+  float score;       // scan_value of the cell (vk::shiTomasiScore)
+  float patch[64];   // getImagePatch(img, pc, patch, 0): Feature::patch_
+};
 
 class VIOManager {
  public:
@@ -323,6 +335,15 @@ class VIOManager {
   // posterior after computeJacobianAndUpdateEKF), the points closer than blind_rgb_points dropped. Fills laserCloudWorldRGB
   // in the reference's order. Call once per VIO tick, after computeJacobianAndUpdateEKF.
   void ColorizeFrameWorld(const BgrImage &img_rgb, double blind_rgb_points, std::vector<PointXYZRGB> &laserCloudWorldRGB);
+  // generateVisualMapPoints (src/vio.cpp:804-906) on the device, up to the object creation: the new visual map points of this
+  // frame, at most one per grid cell, in cell order. type_map: grid_num after the retrieval, one entry per cell, nonzero
+  // where it is TYPE_MAP; grid_size .. border as initializeVIO left them (vio.cpp:66-80, 154). pg == nullptr: the pv list
+  // the last VoxelMapManager::UpdateVoxelMap() left on the device (_pv_list), else those points (point_w, normal, var).
+  // add_from_voxel_map: visual_submap->add_from_voxel_map (point_w, normal), or nullptr. The frame pose is that of *state
+  // and the image the one of the last computeJacobianAndUpdateEKF. Call once per VIO tick, after it.
+  void GenerateVisualMapPoints(const std::vector<uint8_t> &type_map, int grid_size, int grid_n_width, int grid_n_height, int border,
+                               const std::vector<pointWithVar> *pg, const std::vector<pointWithVar> *add_from_voxel_map,
+                               std::vector<NewVisualPoint> &new_points);
 
  private:
   const uint8_t *patch_img_ = nullptr, *patch_ref_img_ = nullptr;  // what the per-patch helpers uploaded last
@@ -341,6 +362,10 @@ class VIOManager {
   PinnedBuf<float> st_rgb_xyz_;      // ColorizeFrameWorld's output staging, grown to the largest coloured scan seen
   PinnedBuf<uint8_t> st_rgb_bgr_;
   int32_t rgb_cap_ = 0;
+  std::vector<double> gen_in_;       // GenerateVisualMapPoints' host pg / add_from, packed
+  std::vector<int32_t> gen_src_, gen_cell_;
+  std::vector<double> gen_pos_, gen_pc_, gen_normal_, gen_var_;
+  std::vector<float> gen_score_, gen_patch_;
   bool ref_imgs_current_ = false;    // false once the per-patch warpAffine replaced the device's reference images
 };
 

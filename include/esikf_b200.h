@@ -364,6 +364,33 @@ int esikf_rgb_set_cloud(esikf_ctx *ctx, const float *pts_xyz, int32_t n, const d
 int esikf_rgb_colorize(esikf_ctx *ctx, const uint8_t *bgr, int32_t width, int32_t height, const double *state, double blind_rgb_points,
                        int32_t cap, int32_t *n_out, float *xyz_out, uint8_t *bgr_out, int32_t *index_out);
 
+/* ---------------------------------------------------------------- new visual map points (generateVisualMapPoints)
+ * VIOManager::generateVisualMapPoints (src/vio.cpp:804-906) on the device, minus the host-side object creation: the points of
+ * the scan pg, then of add_from_voxel_map, that become new visual map points, at most one per grid cell. Called in the VIO
+ * tick after esikf_vio_run; the image is the one of esikf_vio_set_image (or esikf_vio_update).
+ *   pg      : point_w == NULL: the pv list the last esikf_map_device_update left on the device (pv_list_ after
+ *             LIVMapper.cpp:413-424: the float-narrowed posterior world point, the recomputed var and the LIO normal), n
+ *             ignored; ESIKF_ERR_STATE when there is none (no update yet, or esikf_map_device_build / _update_points since).
+ *             Else n host points: point_w (3 doubles each), normal (3), var (9, row-major).
+ *   add_from: n_add points (position and normal, 3 doubles each; their var is zero), scored after the scan (:834-854).
+ *   type_map: one byte per grid cell (n_cells = grid_n_width * grid_n_height, else ESIKF_ERR_ARG), nonzero where the retrieval
+ *             set grid_num[cell] = TYPE_MAP; those cells get no new point.
+ *   grid_size, grid_n_width, grid_n_height, border: as initializeVIO left them (vio.cpp:66-80, 154).
+ *   state   : NULL: the posterior resident after esikf_vio_run; else a packed host state (the frame pose is updateFrameState's).
+ * A point is scored when its normal is not zero (scan points only), isInFrame(pc.cast<int>(), border) holds and its cell
+ * (int)(pc[1] / grid_size) * grid_n_width + (int)(pc[0] / grid_size) is not TYPE_MAP; the score is vk::shiTomasiScore(img,
+ * (int)pc[0], (int)pc[1]). A cell's winner is the first point with the cell's largest score > 0 (cur_value > scan_value[index],
+ * scan_value reset to 0). Nothing is produced when the scan has 10 points or fewer (:806).
+ * The winners come out in cell order, *n_out of them: source_out (scan index, or ESIKF_GEN_ADD_FROM | add_from index),
+ * cell_out, pos_out (point_w, 3 doubles), pc_out (w2c, 2 doubles), score_out, normal_out (the point's normal, negated when
+ * cos_theta < 0, :867-890), var_out (9 doubles), patch_out (getImagePatch(img, pc, patch, 0), 64 floats). Each output may be
+ * NULL. If *n_out exceeds cap, nothing else is written and the call returns ESIKF_ERR_ARG. */
+#define ESIKF_GEN_ADD_FROM 0x40000000
+int esikf_vio_generate_points(esikf_ctx *ctx, const double *point_w, const double *normal, const double *var, int32_t n, const double *add_pos,
+                              const double *add_normal, int32_t n_add, const uint8_t *type_map, int32_t n_cells, int32_t grid_size, int32_t grid_n_width,
+                              int32_t grid_n_height, int32_t border, const double *state, int32_t cap, int32_t *n_out, int32_t *source_out,
+                              int32_t *cell_out, double *pos_out, double *pc_out, float *score_out, double *normal_out, double *var_out, float *patch_out);
+
 /* ---------------------------------------------------------------- multi-GPU (one process per GPU)
  * The residual point / patch set is sharded by contiguous blocks; each iteration all-reduces the
  * packed information buffer [HTH upper | HTz | M | sum|d| ...] and every rank solves redundantly.
