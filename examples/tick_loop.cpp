@@ -100,6 +100,14 @@ int main() {
     std::vector<NewVisualPoint> new_points;
     vio_manager.GenerateVisualMapPoints(grid_num, 2, 32, 24, 5 << 2, nullptr, nullptr, new_points);
     std::printf("tick %d new visual map points: status %d, %zu points\n", tick, vio_manager.last_status_, new_points.size());
+    // updateVisualMapPoints (vio.cpp:908-967): the sub-map's one entry was last observed from the identity pose at its
+    // reference pixel; whether this frame becomes a new observation of it. The Feature objects and the eviction at 30
+    // observations are the caller's (INTEGRATION.md §2).
+    std::vector<uint8_t> converged(vio_manager.total_points, 0), update_flag;
+    std::vector<LastObservation> last_obs(vio_manager.total_points, LastObservation{{1, 0, 0, 0, 1, 0, 0, 0, 1, 0, 0, 0}, {32.0, 24.0}});
+    std::vector<NewObservation> new_obs;
+    vio_manager.UpdateVisualMapPoints(converged, last_obs, update_flag, new_obs);
+    std::printf("tick %d new observations: status %d, %zu of %d entries\n", tick, vio_manager.last_status_, new_obs.size(), vio_manager.total_points);
   }
   // somebody wants the warp patches of the last selection on the host after all
   vio_manager.MaterializeWarpPatches();

@@ -114,6 +114,7 @@ def load_library():
     lib.esikf_rgb_set_cloud.argtypes = [vp, vp, C.c_int32, vp]
     lib.esikf_rgb_colorize.argtypes = [vp, vp, C.c_int32, C.c_int32, vp, C.c_double, C.c_int32, ip, vp, vp, vp]
     lib.esikf_vio_generate_points.argtypes = [vp, vp, vp, vp, C.c_int32, vp, vp, C.c_int32, vp] + [C.c_int32] * 5 + [vp, C.c_int32, ip] + [vp] * 8
+    lib.esikf_vio_update_points.argtypes = [vp, C.c_int32, vp, vp, vp, vp, C.c_int32, ip, vp, vp, vp, vp]
     lib.esikf_comm_unique_id.argtypes = [C.c_char_p]
     lib.esikf_comm_init.argtypes = [vp, C.c_int32, C.c_int32, C.c_char_p]
     lib.esikf_comm_rank.argtypes = [vp, ip, ip]
@@ -150,7 +151,7 @@ EXPORTED_SYMBOLS = [
     "esikf_set_extrinsics", "esikf_set_lidar_extrinsics", "esikf_map_upload", "esikf_map_patch", "esikf_map_device_init", "esikf_map_device_build", "esikf_map_device_update", "esikf_map_device_update_points", "esikf_map_device_slide", "esikf_map_device_stats", "esikf_map_device_capacity", "esikf_map_device_download", "esikf_map_device_export", "esikf_lio_fetch_normals", "esikf_lio_set_scan", "esikf_lio_run", "esikf_lio_fetch",
     "esikf_lio_update", "esikf_lio_fetch_point_cov", "esikf_vio_set_camera", "esikf_vio_set_image", "esikf_vio_set_patches",
     "esikf_vio_run", "esikf_vio_fetch", "esikf_vio_update", "esikf_vio_get_image_patch", "esikf_vio_set_ref_images",
-    "esikf_vio_warp_patches", "esikf_vio_select_patches", "esikf_vio_warp_affine", "esikf_vio_set_inverse_refs", "esikf_rgb_set_cloud", "esikf_rgb_colorize", "esikf_vio_generate_points", "esikf_comm_unique_id", "esikf_comm_init", "esikf_comm_rank", "esikf_shard_range", "esikf_peer_export", "esikf_peer_attach", "esikf_profile_kernel", "esikf_set_kernel_timing", "esikf_get_kernel_timing", "esikf_set_phase_stamps", "esikf_get_phase_stamps",
+    "esikf_vio_warp_patches", "esikf_vio_select_patches", "esikf_vio_warp_affine", "esikf_vio_set_inverse_refs", "esikf_rgb_set_cloud", "esikf_rgb_colorize", "esikf_vio_generate_points", "esikf_vio_update_points", "esikf_comm_unique_id", "esikf_comm_init", "esikf_comm_rank", "esikf_shard_range", "esikf_peer_export", "esikf_peer_attach", "esikf_profile_kernel", "esikf_set_kernel_timing", "esikf_get_kernel_timing", "esikf_set_phase_stamps", "esikf_get_phase_stamps",
 ]
 
 
@@ -545,6 +546,28 @@ class Context:
                                                     int(grid_size), int(grid_n_width), int(grid_n_height), int(border), _addr(s), cap, C.byref(cnt),
                                                     *[out[f].ctypes.data for f in ("source", "cell", "pos", "pc", "score", "normal", "var", "patch")]))
         return {f: v[:cnt.value] for f, v in out.items()}
+
+    # ------------------------------------------------------------------ new observations of the sub-map (updateVisualMapPoints)
+    def vio_update_points(self, converged, last_T, last_px, state=None, cap=None):
+        """updateVisualMapPoints on the device (esikf_vio_update_points), after vio_run, for the sub-map installed on the device
+        (n entries). converged: (n,) bool / uint8, is_converged_; last_T: (n, 12) float64, obs_.back()->T_f_w_ as R (row-major)
+        then t; last_px: (n, 2) float64, obs_.back()->px_; state: a packed state, or None for the VIO posterior on the device.
+        Returns update_flag (n,) uint8 and, for the added entries in entry order, entry (int32 sub-map index), pc (k, 2) and
+        patch (k, 64) float32. cap: room for that many (default n); fewer than the added entries raises."""
+        conv = _c(converged, np.uint8).reshape(-1)
+        n = len(conv)
+        T = _c(last_T, np.float64).reshape(-1, 12)
+        px = _c(last_px, np.float64).reshape(-1, 2)
+        assert len(T) == n and len(px) == n
+        s = None if state is None else _c(state, np.float64)
+        cap = n if cap is None else int(cap)
+        k = max(cap, 1)
+        flag = np.zeros(max(n, 1), np.uint8)
+        out = dict(entry=np.zeros(k, np.int32), pc=np.zeros((k, 2)), patch=np.zeros((k, 64), np.float32))
+        cnt = C.c_int32(0)
+        self._ck(self.lib.esikf_vio_update_points(self.h, n, conv.ctypes.data, T.ctypes.data, px.ctypes.data, _addr(s), cap, C.byref(cnt),
+                                                  flag.ctypes.data, *[out[f].ctypes.data for f in ("entry", "pc", "patch")]))
+        return dict(update_flag=flag[:n], **{f: v[:cnt.value] for f, v in out.items()})
 
     # ------------------------------------------------------------------ multi-GPU / measurement
     def vio_set_inverse_refs(self, ref_img_index, ref_px, ref_f, ref_R, ref_pos):

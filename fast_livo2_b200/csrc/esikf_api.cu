@@ -24,6 +24,7 @@
 #include "esikf_map.cu"
 #include "esikf_color.cu"
 #include "esikf_generate.cu"
+#include "esikf_observe.cu"
 
 using namespace esikf;
 
@@ -234,6 +235,7 @@ struct esikf_ctx {
   DevBuf<float> warp_out;        // esikf_vio_warp_affine scratch (does not disturb the installed patches)
   DevBuf<int32_t> warp_levels;
   int n_patches = 0;
+  bool have_submap = false;  // a sub-map was installed (set_patches, warp_patches(keep_on_device), select_patches)
   // warp producers
   std::vector<DevBuf<uint8_t>> ref_imgs;
   DevBuf<const uint8_t *> ref_img_ptrs;
@@ -264,6 +266,13 @@ struct esikf_ctx {
   DevBuf<unsigned long long> gen_key;
   DevBuf<int32_t> gen_i;
   DevBuf<float> gen_out_f;
+
+  // new observations of the sub-map (esikf_vio_update_points): the caller's per-entry inputs, the flags, every entry's pc, the
+  // scan offsets and the added entries' records
+  DevBuf<double> obs_in, obs_pc, obs_out_pc;
+  DevBuf<uint8_t> obs_flag;
+  DevBuf<int32_t> obs_i;
+  DevBuf<float> obs_patch;
 
   // multi-GPU
   int rank = 0, nranks = 1;
@@ -1252,6 +1261,7 @@ int esikf_vio_set_patches(esikf_ctx *ctx, const double *pos, const float *warp_p
     CK(cudaMemcpyAsync(ctx->inv_expo.p, inv_expo_list, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, st));
   }
   ctx->n_patches = n;
+  ctx->have_submap = true;
   return ESIKF_OK;
 }
 
@@ -1510,6 +1520,7 @@ int esikf_vio_warp_patches(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_ind
     CK(cudaMemcpyAsync(ctx->inv_expo.p, ones.data(), (size_t)n * sizeof(double), cudaMemcpyHostToDevice, st));
     CK(cudaStreamSynchronize(st));
     ctx->n_patches = n;
+    ctx->have_submap = true;
   }
   CK(cudaStreamSynchronize(st));
   return ESIKF_OK;
@@ -1544,6 +1555,7 @@ int esikf_vio_select_patches(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_i
   *n_kept = 0;
   if (n == 0) {
     ctx->n_patches = 0;
+    ctx->have_submap = true;
     return ESIKF_OK;
   }
   // one staging copy per element type; device layout (doubles): px 2n | ref_f 3n | ref_pos 3n | pos 3n | normal 3n | T_ref 12n |
@@ -1601,6 +1613,7 @@ int esikf_vio_select_patches(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_i
   CK(cudaMemcpyAsync(&nk, d_nk, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   ctx->n_patches = nk;
+  ctx->have_submap = true;
   *n_kept = nk;
   if (nk > 0) {
     CK(cudaMemcpyAsync(kept_index, d_kept, (size_t)nk * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
@@ -1856,6 +1869,84 @@ int esikf_vio_generate_points(esikf_ctx *ctx, const double *point_w, const doubl
   if (score_out) CK(cudaMemcpyAsync(score_out, o.score, K * sizeof(float), cudaMemcpyDeviceToHost, st));
   if (normal_out) CK(cudaMemcpyAsync(normal_out, o.normal, K * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
   if (var_out) CK(cudaMemcpyAsync(var_out, o.var, K * 9 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return ESIKF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------- new observations of the sub-map
+// The largest double x with acos(x) > 0.3 under the host's acos, by bisection over the bit patterns of [0.5, 1] (positive
+// doubles order as their bits; acos(0.5) > 0.3 >= acos(1)). acos is decreasing, so delta_theta > 0.3 (vio.cpp:938-939) holds
+// exactly when -1 <= 0.5 * (trace - 1) <= this bound.
+static double acos_03_bound() {
+  uint64_t lo, hi;
+  const double a = 0.5, b = 1.0;
+  memcpy(&lo, &a, 8), memcpy(&hi, &b, 8);
+  while (hi - lo > 1) {
+    const uint64_t mid = lo + (hi - lo) / 2;
+    double x;
+    memcpy(&x, &mid, 8);
+    (acos(x) > 0.3 ? lo : hi) = mid;
+  }
+  double x;
+  memcpy(&x, &lo, 8);
+  return x;
+}
+
+int esikf_vio_update_points(esikf_ctx *ctx, int32_t n, const uint8_t *converged, const double *last_T_f_w, const double *last_px, const double *state,
+                            int32_t cap, int32_t *n_out, uint8_t *update_flag_out, int32_t *entry_out, double *pc_out, float *patch_out) {
+  if (!ctx || n < 0 || !n_out || cap < 0 || (n > 0 && (!converged || !last_T_f_w || !last_px)))
+    return fail(ctx, ESIKF_ERR_ARG, "vio_update_points: bad argument");
+  if (!ctx->have_cam || !ctx->have_ext) return fail(ctx, ESIKF_ERR_STATE, "vio_update_points before vio_set_camera / set_extrinsics");
+  if (ctx->img_w != ctx->cam.width || ctx->img_h != ctx->cam.height) return fail(ctx, ESIKF_ERR_STATE, "vio_update_points before vio_set_image");
+  if (!ctx->have_submap) return fail(ctx, ESIKF_ERR_STATE, "vio_update_points: no visual sub-map installed (select_patches / set_patches)");
+  if (n != ctx->n_patches) return fail(ctx, ESIKF_ERR_ARG, "vio_update_points: %d entries, the installed sub-map has %d", n, ctx->n_patches);
+  CK(cudaSetDevice(ctx->device));
+  const double *dev_state = nullptr;
+  if (int rc = rgb_state(ctx, state, esikf_ctx::RESIDENT_VIO, "vio_update_points", &dev_state)) return rc;
+  static const double cos_max = acos_03_bound();
+  *n_out = 0;
+  if (n == 0) return ESIKF_OK;  // total_points == 0 (:910)
+  cudaStream_t st = ctx->stream;
+  const size_t N = (size_t)n;
+  CK(ctx->obs_in.reserve(14 * N));    // last_T 12 | last_px 2
+  CK(ctx->obs_flag.reserve(2 * N));   // converged | update_flag
+  CK(ctx->obs_pc.reserve(2 * N));
+  CK(ctx->obs_out_pc.reserve(2 * N));
+  CK(ctx->obs_i.reserve(3 * N + 1));  // keep | dst | n_added | entry
+  CK(ctx->obs_patch.reserve(64 * N));
+  CK(cudaMemcpyAsync(ctx->obs_in.p, last_T_f_w, N * 12 * sizeof(double), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(ctx->obs_in.p + 12 * N, last_px, N * 2 * sizeof(double), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(ctx->obs_flag.p, converged, N, cudaMemcpyHostToDevice, st));
+  ObsArgs a;
+  cam_dev(ctx, a.cam);
+  double Jdp_dR[9];
+  vio_consts(ctx, a.Rci, a.Pci, Jdp_dR);
+  a.state = dev_state, a.pos = ctx->vis_pos.p, a.converged = ctx->obs_flag.p, a.last_T = ctx->obs_in.p, a.last_px = ctx->obs_in.p + 12 * N;
+  a.n = n, a.cos_max = cos_max, a.flag = ctx->obs_flag.p + N, a.pc = ctx->obs_pc.p;
+  int32_t *d_keep = ctx->obs_i.p, *d_dst = d_keep + N, *d_nk = d_dst + N, *d_entry = d_nk + 1;
+  a.keep = d_keep;
+  obs_flag_kernel<<<(n + OBS_THREADS - 1) / OBS_THREADS, OBS_THREADS, 0, st>>>(a);
+  select_scan_kernel<<<1, SELECT_SCAN_THREADS, 0, st>>>(d_keep, n, d_dst, d_nk);
+  obs_scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_keep, d_dst, ctx->obs_pc.p, n, d_entry, ctx->obs_out_pc.p);
+  ctx->launches += 3;
+  CK(cudaGetLastError());
+  int32_t nk = 0;
+  CK(cudaMemcpyAsync(&nk, d_nk, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));  // also: the caller may reuse its buffers on return
+  *n_out = nk;
+  if (nk > cap) return fail(ctx, ESIKF_ERR_ARG, "vio_update_points: %d new observations, room for %d", nk, cap);
+  if (update_flag_out) CK(cudaMemcpyAsync(update_flag_out, a.flag, N, cudaMemcpyDeviceToHost, st));
+  if (nk > 0) {
+    const size_t K = (size_t)nk;
+    if (patch_out) {
+      image_patch_kernel<<<(nk * 64 + 255) / 256, 256, 0, st>>>(ctx->img.p, ctx->img_w, ctx->img_h, ctx->obs_out_pc.p, nk, 0, ctx->obs_patch.p);
+      ctx->launches++;
+      CK(cudaGetLastError());
+      CK(cudaMemcpyAsync(patch_out, ctx->obs_patch.p, K * 64 * sizeof(float), cudaMemcpyDeviceToHost, st));
+    }
+    if (entry_out) CK(cudaMemcpyAsync(entry_out, d_entry, K * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    if (pc_out) CK(cudaMemcpyAsync(pc_out, ctx->obs_out_pc.p, K * 2 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  }
   CK(cudaStreamSynchronize(st));
   return ESIKF_OK;
 }

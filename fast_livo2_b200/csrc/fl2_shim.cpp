@@ -554,6 +554,47 @@ void VIOManager::GenerateVisualMapPoints(const std::vector<uint8_t> &type_map, i
   }
 }
 
+void VIOManager::UpdateVisualMapPoints(const std::vector<uint8_t> &converged, const std::vector<LastObservation> &last_obs, std::vector<uint8_t> &update_flag,
+                                       std::vector<NewObservation> &new_obs) {
+  new_obs.clear();
+  if (!ctx_ || !state) {
+    last_status_ = ESIKF_ERR_STATE, last_error_ = "UpdateVisualMapPoints: no device context or state";
+    return;
+  }
+  update_flag.assign(total_points > 0 ? total_points : 0, 0);
+  if (total_points <= 0) {  // src/vio.cpp:910
+    last_status_ = ESIKF_OK;
+    return;
+  }
+  if (converged.size() != (size_t)total_points || last_obs.size() != (size_t)total_points) {
+    last_status_ = ESIKF_ERR_ARG, last_error_ = "UpdateVisualMapPoints: converged / last_obs must have total_points entries";
+    return;
+  }
+  double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
+  if (!sbuf) {
+    last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
+    return;
+  }
+  state->pack(sbuf);
+  const size_t n = last_obs.size();
+  obs_in_.resize(14 * n + 1);
+  double *T = obs_in_.data(), *px = T + 12 * n;
+  for (size_t i = 0; i < n; i++) memcpy(T + 12 * i, last_obs[i].T_f_w, sizeof(last_obs[i].T_f_w)), memcpy(px + 2 * i, last_obs[i].px, sizeof(last_obs[i].px));
+  obs_entry_.resize(n + 1), obs_pc_.resize(2 * n + 2), obs_patch_.resize(64 * n + 64);
+  int32_t k = 0;
+  last_status_ = esikf_vio_update_points(ctx_, (int32_t)n, converged.data(), T, px, sbuf, (int32_t)n, &k, update_flag.data(), obs_entry_.data(), obs_pc_.data(),
+                                         obs_patch_.data());
+  if (last_status_) {
+    last_error_ = esikf_last_error(ctx_);
+    return;
+  }
+  new_obs.resize(k);
+  for (int i = 0; i < k; i++) {
+    NewObservation &q = new_obs[i];
+    q.entry = obs_entry_[i];
+    memcpy(q.pc, &obs_pc_[2 * i], sizeof(q.pc)), memcpy(q.patch, &obs_patch_[64 * i], sizeof(q.patch));
+  }
+}
 
 void VIOManager::initializeVIO() {
   if (!ctx_) return;

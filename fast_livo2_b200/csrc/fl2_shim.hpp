@@ -282,6 +282,19 @@ struct NewVisualPoint {
   float score;       // scan_value of the cell (vk::shiTomasiScore)
   float patch[64];   // getImagePatch(img, pc, patch, 0): Feature::patch_
 };
+// The oldest observation of a visual sub-map entry, pt->obs_.back() (addFrameRef pushes at the front): what
+// VIOManager::UpdateVisualMapPoints compares the current frame with.
+struct LastObservation {
+  double T_f_w[12];  // Feature::T_f_w_: R row-major, then t
+  double px[2];      // Feature::px_
+};
+// One new observation of VIOManager::UpdateVisualMapPoints: what updateVisualMapPoints (src/vio.cpp:954-964) builds its
+// Feature from. INTEGRATION.md §2 shows the Feature made from it.
+struct NewObservation {
+  int32_t entry;     // index into visual_submap (voxel_points, search_levels)
+  double pc[2];      // new_frame_->w2c(pt->pos_): Feature::px_
+  float patch[64];   // getImagePatch(img, pc, patch, 0): Feature::patch_
+};
 
 class VIOManager {
  public:
@@ -344,6 +357,14 @@ class VIOManager {
   void GenerateVisualMapPoints(const std::vector<uint8_t> &type_map, int grid_size, int grid_n_width, int grid_n_height, int border,
                                const std::vector<pointWithVar> *pg, const std::vector<pointWithVar> *add_from_voxel_map,
                                std::vector<NewVisualPoint> &new_points);
+  // updateVisualMapPoints (src/vio.cpp:908-967) on the device, up to the Feature objects and the eviction at 30 observations:
+  // which entries of the visual sub-map on the device (the last SelectSubSparseMap or computeJacobianAndUpdateEKF, total_points
+  // entries) this frame becomes a new observation of. converged: pt->is_converged_ and last_obs: pt->obs_.back() of every
+  // entry, indexed like visual_submap. Fills update_flag (one per entry, as updateReferencePatch reads it) and new_obs (the
+  // added entries in entry order). The frame pose is that of *state and the image the one of the last
+  // computeJacobianAndUpdateEKF. Call once per VIO tick, after it.
+  void UpdateVisualMapPoints(const std::vector<uint8_t> &converged, const std::vector<LastObservation> &last_obs, std::vector<uint8_t> &update_flag,
+                             std::vector<NewObservation> &new_obs);
 
  private:
   const uint8_t *patch_img_ = nullptr, *patch_ref_img_ = nullptr;  // what the per-patch helpers uploaded last
@@ -366,6 +387,9 @@ class VIOManager {
   std::vector<int32_t> gen_src_, gen_cell_;
   std::vector<double> gen_pos_, gen_pc_, gen_normal_, gen_var_;
   std::vector<float> gen_score_, gen_patch_;
+  std::vector<double> obs_in_, obs_pc_;  // UpdateVisualMapPoints' last observations (T | px) and the added entries' pc
+  std::vector<int32_t> obs_entry_;
+  std::vector<float> obs_patch_;
   bool ref_imgs_current_ = false;    // false once the per-patch warpAffine replaced the device's reference images
 };
 

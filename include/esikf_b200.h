@@ -391,6 +391,31 @@ int esikf_vio_generate_points(esikf_ctx *ctx, const double *point_w, const doubl
                               int32_t grid_n_height, int32_t border, const double *state, int32_t cap, int32_t *n_out, int32_t *source_out,
                               int32_t *cell_out, double *pos_out, double *pc_out, float *score_out, double *normal_out, double *var_out, float *patch_out);
 
+/* ---------------------------------------------------------------- new observations of the visual sub-map (updateVisualMapPoints)
+ * VIOManager::updateVisualMapPoints (src/vio.cpp:908-967) on the device, minus the host-side object management: which entries
+ * of the visual sub-map the current frame becomes a new observation (Feature) of, with that Feature's pixel and patch. Called
+ * in the VIO tick after esikf_vio_run (and esikf_vio_generate_points); the image is the one of esikf_vio_set_image (or
+ * esikf_vio_update).
+ *   sub-map  : the one the last esikf_vio_select_patches, esikf_vio_set_patches, esikf_vio_update or esikf_vio_warp_patches
+ *              (keep_on_device) installed; its pos is read on the device. ESIKF_ERR_STATE when none was installed;
+ *              n must equal its count, else ESIKF_ERR_ARG.
+ *   converged: n bytes, VisualPoint::is_converged_ of each entry.
+ *   last_T_f_w: n x 12 doubles, obs_.back()->T_f_w_ (the oldest observation: addFrameRef pushes at the front) as R
+ *              (row-major) then t.
+ *   last_px  : n x 2 doubles, obs_.back()->px_.
+ *   state    : NULL: the posterior resident after esikf_vio_run; else a packed host state (the frame pose is updateFrameState's).
+ * A converged entry gets flag 0. Any other entry i gets pc = new_frame_->w2c(pos_), delta_pose = pose_ref *
+ * pose_cur.inverse(), delta_p = |t|, delta_theta = 0 when the rotation's trace > 3 - 1e-6, else acos(0.5 * (trace - 1));
+ * it is added (update_flag[i] = 1) when delta_p > 0.5 || delta_theta > 0.3 || |pc - last_px| > 40. The flags do not depend
+ * on the eviction at 30 observations, which stays with the caller.
+ * Outputs: update_flag_out (n bytes), and for the added entries in entry order, *n_out of them: entry_out (sub-map index),
+ * pc_out (2 doubles: the new Feature's px_) and patch_out (getImagePatch(img, pc, patch, 0), 64 floats); the new Feature's
+ * level is search_levels[entry] of the selection. Each output may be NULL. If *n_out exceeds cap, nothing else is written and
+ * the call returns ESIKF_ERR_ARG; a call that fails its argument checks writes nothing. With several ranks every rank
+ * evaluates all n entries. */
+int esikf_vio_update_points(esikf_ctx *ctx, int32_t n, const uint8_t *converged, const double *last_T_f_w, const double *last_px, const double *state,
+                            int32_t cap, int32_t *n_out, uint8_t *update_flag_out, int32_t *entry_out, double *pc_out, float *patch_out);
+
 /* ---------------------------------------------------------------- multi-GPU (one process per GPU)
  * The residual point / patch set is sharded by contiguous blocks; each iteration all-reduces the
  * packed information buffer [HTH upper | HTz | M | sum|d| ...] and every rank solves redundantly.
