@@ -68,8 +68,14 @@ int main() {
     // ---- VIO tick (LIVMapper::handleVIO -> processFrame -> computeJacobianAndUpdateEKF, vio.cpp:1810)
     std::vector<uint8_t> pixels(64 * 48, 128);
     GrayImage img{pixels.data(), 64, 48};
-    // retrieveFromVisualSparseMap (vio.cpp:352-782): the map-side part (depth image, feat_map, grid argmin, depth check) and the
-    // choice of each point's reference feature stay on the host; the per-candidate tail runs in SelectSubSparseMap
+    // retrieveFromVisualSparseMap (vio.cpp:352-782). The scan side runs on the device, from the pv list UpdateVoxelMap left
+    // there: the scan's voxel keys (inserted into the persistent sub_feat_map in the returned order) and the depth image, with
+    // the frame pose of *state; border (patch_size_half + 1) << patch_pyrimid_level as initializeVIO leaves it. The walk over
+    // feat_map, ray casting and the choice of each point's reference feature stay on the host (INTEGRATION.md §2); the depth
+    // check of the retrieved points runs on the device; the per-candidate tail runs in SelectSubSparseMap.
+    std::vector<VOXEL_LOCATION> scan_voxels;
+    vio_manager.RetrieveScanVoxels(5 << 2, nullptr, scan_voxels);
+    std::printf("tick %d scan voxels: status %d, %zu keys\n", tick, vio_manager.last_status_, scan_voxels.size());
     std::vector<uint8_t> ref_pixels(64 * 48, 128);
     GrayImage ref_img{ref_pixels.data(), 64, 48};        // Feature::img_ of the one reference frame
     vio_manager.SetReferenceImages(&ref_img, 1);
@@ -78,6 +84,9 @@ int main() {
     cand.px_ref[0] = 32.0, cand.px_ref[1] = 24.0, cand.ref_f[2] = 1.0, cand.pos_w[2] = 2.0, cand.normal_w[2] = -1.0;
     cand.T_ref_w[0] = cand.T_ref_w[4] = cand.T_ref_w[8] = 1.0, cand.ref_inv_expo = 1.0;
     cand.pc[0] = 32.0, cand.pc[1] = 24.0;                // new_frame_->w2c(pos_), :614
+    std::vector<uint8_t> depth_discontinuous;            // :614-640 for the one retrieved point: 1 drops it
+    vio_manager.CheckDepthContinuity(1, cand.pos_w, cand.pc, depth_discontinuous);
+    std::printf("tick %d depth check: status %d, discontinuous %d\n", tick, vio_manager.last_status_, depth_discontinuous.empty() ? -1 : (int)depth_discontinuous[0]);
     const double T_cur_w[12] = {1, 0, 0, 0, 1, 0, 0, 0, 1, 0, 0, 0};  // new_frame_->T_f_w_
     SubSparseMap submap;
     vio_manager.visual_submap = &submap;

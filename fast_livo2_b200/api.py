@@ -115,6 +115,8 @@ def load_library():
     lib.esikf_rgb_colorize.argtypes = [vp, vp, C.c_int32, C.c_int32, vp, C.c_double, C.c_int32, ip, vp, vp, vp]
     lib.esikf_vio_generate_points.argtypes = [vp, vp, vp, vp, C.c_int32, vp, vp, C.c_int32, vp] + [C.c_int32] * 5 + [vp, C.c_int32, ip] + [vp] * 8
     lib.esikf_vio_update_points.argtypes = [vp, C.c_int32, vp, vp, vp, vp, C.c_int32, ip, vp, vp, vp, vp]
+    lib.esikf_vio_retrieve_scan.argtypes = [vp, vp, C.c_int32, C.c_int32, vp, C.c_int32, ip, vp, vp]
+    lib.esikf_vio_depth_check.argtypes = [vp, C.c_int32, vp, vp, vp]
     lib.esikf_comm_unique_id.argtypes = [C.c_char_p]
     lib.esikf_comm_init.argtypes = [vp, C.c_int32, C.c_int32, C.c_char_p]
     lib.esikf_comm_rank.argtypes = [vp, ip, ip]
@@ -151,7 +153,7 @@ EXPORTED_SYMBOLS = [
     "esikf_set_extrinsics", "esikf_set_lidar_extrinsics", "esikf_map_upload", "esikf_map_patch", "esikf_map_device_init", "esikf_map_device_build", "esikf_map_device_update", "esikf_map_device_update_points", "esikf_map_device_slide", "esikf_map_device_stats", "esikf_map_device_capacity", "esikf_map_device_download", "esikf_map_device_export", "esikf_lio_fetch_normals", "esikf_lio_set_scan", "esikf_lio_run", "esikf_lio_fetch",
     "esikf_lio_update", "esikf_lio_fetch_point_cov", "esikf_vio_set_camera", "esikf_vio_set_image", "esikf_vio_set_patches",
     "esikf_vio_run", "esikf_vio_fetch", "esikf_vio_update", "esikf_vio_get_image_patch", "esikf_vio_set_ref_images",
-    "esikf_vio_warp_patches", "esikf_vio_select_patches", "esikf_vio_warp_affine", "esikf_vio_set_inverse_refs", "esikf_rgb_set_cloud", "esikf_rgb_colorize", "esikf_vio_generate_points", "esikf_vio_update_points", "esikf_comm_unique_id", "esikf_comm_init", "esikf_comm_rank", "esikf_shard_range", "esikf_peer_export", "esikf_peer_attach", "esikf_profile_kernel", "esikf_set_kernel_timing", "esikf_get_kernel_timing", "esikf_set_phase_stamps", "esikf_get_phase_stamps",
+    "esikf_vio_warp_patches", "esikf_vio_select_patches", "esikf_vio_warp_affine", "esikf_vio_set_inverse_refs", "esikf_rgb_set_cloud", "esikf_rgb_colorize", "esikf_vio_generate_points", "esikf_vio_update_points", "esikf_vio_retrieve_scan", "esikf_vio_depth_check", "esikf_comm_unique_id", "esikf_comm_init", "esikf_comm_rank", "esikf_shard_range", "esikf_peer_export", "esikf_peer_attach", "esikf_profile_kernel", "esikf_set_kernel_timing", "esikf_get_kernel_timing", "esikf_set_phase_stamps", "esikf_get_phase_stamps",
 ]
 
 
@@ -392,6 +394,7 @@ class Context:
         v = VioCfgC(vio.img_point_cov, vio.levels, vio.max_iterations, int(vio.exposure_estimate_en), int(getattr(vio, "inverse_composition_en", False)))
         self._ck(self.lib.esikf_vio_set_camera(self.h, C.byref(c), C.byref(v)))
         self.levels = vio.levels
+        self.cam_size = (cam.width, cam.height)
 
     def vio_set_image(self, img):
         h, w = int(img.shape[0]), int(img.shape[1])
@@ -568,6 +571,42 @@ class Context:
         self._ck(self.lib.esikf_vio_update_points(self.h, n, conv.ctypes.data, T.ctypes.data, px.ctypes.data, _addr(s), cap, C.byref(cnt),
                                                   flag.ctypes.data, *[out[f].ctypes.data for f in ("entry", "pc", "patch")]))
         return dict(update_flag=flag[:n], **{f: v[:cnt.value] for f, v in out.items()})
+
+    # ------------------------------------------------------------------ scan side of the retrieval (retrieveFromVisualSparseMap)
+    def vio_retrieve_scan(self, border, pg=None, state=None, depth=False, cap=None):
+        """The scan's voxel keys and depth image (esikf_vio_retrieve_scan, vio.cpp:386-428). pg: (n, 3) float64 world points, or
+        None for the pv list the last map_device_update left on the device; state: the frame's packed state (the VIO prior), or
+        None for the LIO posterior on the device. Returns keys (k, 3) int32 in first-occurrence order and, with depth=True, the
+        depth image (height, width) float32. cap: room for that many keys (fewer raises); by default the scan size, or for the
+        resident scan whatever a first call reports."""
+        p = None if pg is None else _c(pg, np.float64).reshape(-1, 3)
+        s = None if state is None else _c(state, np.float64)
+        n = 0 if p is None else len(p)
+        w, h = self.cam_size
+        img = np.zeros((h, w), np.float32) if depth else None
+        cnt = C.c_int32(-1)
+
+        def call(k):
+            keys = np.zeros((max(k, 1), 3), np.int32)
+            rc = self.lib.esikf_vio_retrieve_scan(self.h, _addr(p), n, int(border), _addr(s), k, C.byref(cnt), keys.ctypes.data, _addr(img))
+            return rc, keys
+
+        rc, keys = call(n if cap is None and p is not None else int(cap or 0))
+        if rc == -3 and cap is None and p is None and cnt.value > 0:  # ESIKF_ERR_ARG with the count of the resident scan's keys
+            rc, keys = call(cnt.value)
+        self._ck(rc)
+        return dict(keys=keys[:cnt.value], depth=img) if depth else dict(keys=keys[:cnt.value])
+
+    def vio_depth_check(self, pos, pc):
+        """The depth-continuity flags of n retrieved points (esikf_vio_depth_check, vio.cpp:614-640) against the depth image of
+        the last vio_retrieve_scan: pos (n, 3) VisualPoint::pos_, pc (n, 2) the caller's w2c(pos_). Returns (n,) uint8, 1 = the
+        point is dropped."""
+        pos = _c(pos, np.float64).reshape(-1, 3)
+        pc = _c(pc, np.float64).reshape(-1, 2)
+        assert len(pos) == len(pc)
+        out = np.zeros(max(len(pos), 1), np.uint8)
+        self._ck(self.lib.esikf_vio_depth_check(self.h, len(pos), pos.ctypes.data, pc.ctypes.data, out.ctypes.data))
+        return out[:len(pos)]
 
     # ------------------------------------------------------------------ multi-GPU / measurement
     def vio_set_inverse_refs(self, ref_img_index, ref_px, ref_f, ref_R, ref_pos):

@@ -25,6 +25,7 @@
 #include "esikf_color.cu"
 #include "esikf_generate.cu"
 #include "esikf_observe.cu"
+#include "esikf_retrieve.cu"
 
 using namespace esikf;
 
@@ -273,6 +274,19 @@ struct esikf_ctx {
   DevBuf<uint8_t> obs_flag;
   DevBuf<int32_t> obs_i;
   DevBuf<float> obs_patch;
+
+  // scan side of the retrieval (esikf_vio_retrieve_scan / esikf_vio_depth_check): a host scan, the per-point keys, scan
+  // indices and depths, the pixel writers, the sort / scan scratch, the depth image and the frame pose it was made with
+  DevBuf<double> ret_pt, ret_state, ret_cand;
+  DevBuf<unsigned long long> ret_key;  // key_in n | key_out n
+  DevBuf<uint32_t> ret_idx;            // idx_in n | idx_out n
+  DevBuf<int32_t> ret_i;               // head n + 1 | dst n + 1 | keys 3n | bad 1
+  DevBuf<int32_t> ret_win;
+  DevBuf<float> ret_depth_pt, ret_depth;
+  DevBuf<uint8_t> ret_tmp, ret_flag;
+  double ret_Rci[9] = {}, ret_Pci[3] = {};
+  int ret_w = 0, ret_h = 0;
+  bool ret_valid = false;  // a depth image and its pose are in place (cleared by esikf_vio_set_camera and by a failed call)
 
   // multi-GPU
   int rank = 0, nranks = 1;
@@ -1229,6 +1243,7 @@ int esikf_vio_set_camera(esikf_ctx *ctx, const esikf_camera *cam, const esikf_vi
   ctx->cam = *cam;
   ctx->vio_cfg = *cfg;
   ctx->have_cam = true;
+  ctx->ret_valid = false;
   return ESIKF_OK;
 }
 
@@ -1947,6 +1962,101 @@ int esikf_vio_update_points(esikf_ctx *ctx, int32_t n, const uint8_t *converged,
     if (entry_out) CK(cudaMemcpyAsync(entry_out, d_entry, K * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     if (pc_out) CK(cudaMemcpyAsync(pc_out, ctx->obs_out_pc.p, K * 2 * sizeof(double), cudaMemcpyDeviceToHost, st));
   }
+  CK(cudaStreamSynchronize(st));
+  return ESIKF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------- scan side of the retrieval
+int esikf_vio_retrieve_scan(esikf_ctx *ctx, const double *point_w, int32_t n, int32_t border, const double *state, int32_t cap, int32_t *n_keys,
+                            int32_t *keys_out, float *depth_out) {
+  if (!ctx || !n_keys || cap < 0 || border < 0 || (point_w && n < 0) || (cap > 0 && !keys_out)) return fail(ctx, ESIKF_ERR_ARG, "vio_retrieve_scan: bad argument");
+  if (!ctx->have_cam || !ctx->have_ext) return fail(ctx, ESIKF_ERR_STATE, "vio_retrieve_scan before vio_set_camera / set_extrinsics");
+  if (!point_w && ctx->pv_n < 0)
+    return fail(ctx, ESIKF_ERR_STATE, "vio_retrieve_scan(point_w = NULL): no esikf_map_device_update of the resident scan left its points on the device");
+  CK(cudaSetDevice(ctx->device));
+  const double *dev_state = nullptr;
+  if (int rc = rgb_state(ctx, state, esikf_ctx::RESIDENT_LIO, "vio_retrieve_scan", &dev_state)) return rc;
+  ctx->ret_valid = false;
+  if (!point_w) n = ctx->pv_n;
+  cudaStream_t st = ctx->stream;
+  const int W = ctx->cam.width, H = ctx->cam.height;
+  const size_t N = (size_t)n, npix = (size_t)W * H;
+  CK(ctx->ret_state.reserve(S_N));
+  CK(ctx->ret_key.reserve(2 * N + 2));
+  CK(ctx->ret_idx.reserve(2 * N + 2));
+  CK(ctx->ret_i.reserve(5 * N + 3));
+  CK(ctx->ret_depth_pt.reserve(N + 1));
+  CK(ctx->ret_win.reserve(npix));
+  CK(ctx->ret_depth.reserve(npix));
+  // the frame pose stays with the depth image for esikf_vio_depth_check, whatever a later update writes to `state`
+  CK(cudaMemcpyAsync(ctx->ret_state.p, dev_state, S_N * sizeof(double), cudaMemcpyDeviceToDevice, st));
+  int32_t *d_head = ctx->ret_i.p, *d_dst = d_head + N + 1, *d_keys = d_dst + N + 1, *d_bad = d_keys + 3 * N;
+  CK(cudaMemsetAsync(ctx->ret_win.p, 0xff, npix * sizeof(int32_t), st));
+  CK(cudaMemsetAsync(d_bad, 0, sizeof(int32_t), st));
+  RetArgs a;
+  cam_dev(ctx, a.cam);
+  double Jdp_dR[9];
+  vio_consts(ctx, a.Rci, a.Pci, Jdp_dR);
+  a.state = ctx->ret_state.p, a.n = n, a.border = border;
+  if (point_w) {
+    CK(ctx->ret_pt.reserve(3 * N + 3));
+    if (n > 0) CK(cudaMemcpyAsync(ctx->ret_pt.p, point_w, 3 * N * sizeof(double), cudaMemcpyHostToDevice, st));
+    a.pt = ctx->ret_pt.p, a.pt_stride = 3;
+  } else {
+    a.pt = ctx->map_pt.p, a.pt_stride = MAP_PT_D;
+  }
+  a.key = ctx->ret_key.p, a.idx = ctx->ret_idx.p, a.depth_pt = ctx->ret_depth_pt.p, a.win = ctx->ret_win.p, a.bad = d_bad;
+  if (n > 0) ret_scan_kernel<<<(n + RET_THREADS - 1) / RET_THREADS, RET_THREADS, 0, st>>>(a);
+  ret_depth_kernel<<<(int)((npix + 255) / 256), 256, 0, st>>>(ctx->ret_win.p, ctx->ret_depth_pt.p, (int)npix, ctx->ret_depth.p);
+  ctx->launches += n > 0 ? 2 : 1;
+  int32_t counts[2] = {0, 0};  // distinct keys, bad
+  if (n > 0) {
+    unsigned long long *k_out = ctx->ret_key.p + N;
+    uint32_t *i_out = ctx->ret_idx.p + N;
+    size_t sort_bytes = 0, scan_bytes = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, ctx->ret_key.p, k_out, ctx->ret_idx.p, i_out, n, 0, 63, st);
+    cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, d_head, d_dst, n + 1, st);
+    CK(ctx->ret_tmp.reserve(std::max(sort_bytes, scan_bytes) + 16));
+    CK(cub::DeviceRadixSort::SortPairs(ctx->ret_tmp.p, sort_bytes, ctx->ret_key.p, k_out, ctx->ret_idx.p, i_out, n, 0, 63, st));
+    ret_head_kernel<<<(n + 1 + 255) / 256, 256, 0, st>>>(k_out, i_out, n, d_head);
+    CK(cub::DeviceScan::ExclusiveSum(ctx->ret_tmp.p, scan_bytes, d_head, d_dst, n + 1, st));
+    ret_keys_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_head, d_dst, ctx->ret_key.p, n, d_keys);
+    ctx->launches += 4;  // sort passes counted as one
+    CK(cudaMemcpyAsync(&counts[0], d_dst + n, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&counts[1], d_bad, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  }
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(st));  // also: the caller may reuse its buffers on return
+  if (counts[1]) return fail(ctx, ESIKF_ERR_ARG, "vio_retrieve_scan: a voxel key leaves [-2^20, 2^20)");
+  *n_keys = counts[0];
+  if (counts[0] > cap) return fail(ctx, ESIKF_ERR_ARG, "vio_retrieve_scan: %d voxel keys, room for %d", counts[0], cap);
+  if (counts[0] > 0) CK(cudaMemcpyAsync(keys_out, d_keys, (size_t)counts[0] * 3 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  if (depth_out) CK(cudaMemcpyAsync(depth_out, ctx->ret_depth.p, npix * sizeof(float), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  memcpy(ctx->ret_Rci, a.Rci, sizeof(a.Rci)), memcpy(ctx->ret_Pci, a.Pci, sizeof(a.Pci));
+  ctx->ret_w = W, ctx->ret_h = H, ctx->ret_valid = true;
+  return ESIKF_OK;
+}
+
+int esikf_vio_depth_check(esikf_ctx *ctx, int32_t n, const double *pos_w, const double *pc, uint8_t *discontinuous_out) {
+  if (!ctx || n < 0 || (n > 0 && (!pos_w || !pc || !discontinuous_out))) return fail(ctx, ESIKF_ERR_ARG, "vio_depth_check: bad argument");
+  if (!ctx->ret_valid) return fail(ctx, ESIKF_ERR_STATE, "vio_depth_check: no esikf_vio_retrieve_scan since the last vio_set_camera");
+  if (n == 0) return ESIKF_OK;
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t N = (size_t)n;
+  CK(ctx->ret_cand.reserve(5 * N));  // pos 3n | pc 2n
+  CK(ctx->ret_flag.reserve(N));
+  CK(cudaMemcpyAsync(ctx->ret_cand.p, pos_w, 3 * N * sizeof(double), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(ctx->ret_cand.p + 3 * N, pc, 2 * N * sizeof(double), cudaMemcpyHostToDevice, st));
+  DepthCheckArgs a;
+  memcpy(a.Rci, ctx->ret_Rci, sizeof(a.Rci)), memcpy(a.Pci, ctx->ret_Pci, sizeof(a.Pci));
+  a.state = ctx->ret_state.p, a.pos = ctx->ret_cand.p, a.pc = ctx->ret_cand.p + 3 * N, a.n = n, a.width = ctx->ret_w, a.height = ctx->ret_h;
+  a.depth = ctx->ret_depth.p, a.flag = ctx->ret_flag.p;
+  ret_depth_check_kernel<<<(n + RET_THREADS - 1) / RET_THREADS, RET_THREADS, 0, st>>>(a);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(discontinuous_out, ctx->ret_flag.p, N, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   return ESIKF_OK;
 }

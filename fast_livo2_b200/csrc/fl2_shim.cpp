@@ -596,6 +596,71 @@ void VIOManager::UpdateVisualMapPoints(const std::vector<uint8_t> &converged, co
   }
 }
 
+void VIOManager::RetrieveScanVoxels(int border, const std::vector<pointWithVar> *pg, std::vector<VOXEL_LOCATION> &keys) {
+  keys.clear();
+  if (!ctx_ || !state) {
+    last_status_ = ESIKF_ERR_STATE, last_error_ = "RetrieveScanVoxels: no device context or state";
+    return;
+  }
+  const size_t n = pg ? pg->size() : 0;
+  double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES), *pw = st_ret_pt_.get(3 * n + 3);
+  if (!sbuf || !pw) {
+    last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
+    return;
+  }
+  state->pack(sbuf);
+  for (size_t i = 0; i < n; i++)
+    for (int k = 0; k < 3; k++) pw[3 * i + k] = (*pg)[i].point_w[k];
+  // room for one key per point of a host scan; for the resident scan a first call reports the count when the room is short
+  int32_t cap = pg ? (int32_t)n : (int32_t)(keys_cap_ > 0 ? keys_cap_ : 1 << 16), k = -1;
+  int32_t *kb = st_ret_keys_.get(3 * (size_t)cap + 3);
+  if (!kb) {
+    last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
+    return;
+  }
+  last_status_ = esikf_vio_retrieve_scan(ctx_, pg ? pw : nullptr, (int32_t)n, border, sbuf, cap, &k, kb, nullptr);
+  if (last_status_ == ESIKF_ERR_ARG && !pg && k > cap) {
+    cap = k, keys_cap_ = k;
+    kb = st_ret_keys_.get(3 * (size_t)cap + 3);
+    if (!kb) {
+      last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
+      return;
+    }
+    last_status_ = esikf_vio_retrieve_scan(ctx_, nullptr, 0, border, sbuf, cap, &k, kb, nullptr);
+  }
+  if (last_status_) {
+    last_error_ = esikf_last_error(ctx_);
+    return;
+  }
+  keys.resize(k);
+  for (int i = 0; i < k; i++) keys[i] = VOXEL_LOCATION(kb[3 * i], kb[3 * i + 1], kb[3 * i + 2]);
+}
+
+void VIOManager::CheckDepthContinuity(int n, const double *pos, const double *pc, std::vector<uint8_t> &discontinuous) {
+  discontinuous.assign(n > 0 ? n : 0, 0);
+  if (!ctx_) {
+    last_status_ = ESIKF_ERR_STATE, last_error_ = "CheckDepthContinuity: no device context";
+    return;
+  }
+  if (n <= 0) {
+    last_status_ = n < 0 ? ESIKF_ERR_ARG : ESIKF_OK;
+    return;
+  }
+  double *cb = st_ret_cand_.get(5 * (size_t)n);
+  uint8_t *fb = st_ret_flag_.get((size_t)n);
+  if (!cb || !fb) {
+    last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
+    return;
+  }
+  memcpy(cb, pos, 3 * (size_t)n * sizeof(double)), memcpy(cb + 3 * (size_t)n, pc, 2 * (size_t)n * sizeof(double));
+  last_status_ = esikf_vio_depth_check(ctx_, n, cb, cb + 3 * (size_t)n, fb);
+  if (last_status_) {
+    last_error_ = esikf_last_error(ctx_);
+    return;
+  }
+  memcpy(discontinuous.data(), fb, (size_t)n);
+}
+
 void VIOManager::initializeVIO() {
   if (!ctx_) return;
   esikf_extrinsics ext;
@@ -1109,6 +1174,41 @@ int fl2_shim_select_run(const esikf_camera *cam, const esikf_vio_cfg *vcfg, cons
         st.pack(state_host);
         for (int j = 0; j < vio.total_points; j++) errors_host[j] = host.errors[j];
       }
+    }
+  }
+  esikf_destroy(ctx);
+  return rc;
+}
+
+// GPU: VIOManager::RetrieveScanVoxels on n host points (pg: n x 3) with the frame pose of `state`, then
+// VIOManager::CheckDepthContinuity on n_cand points (cand_pos: n_cand x 3, cand_pc: n_cand x 2). Outputs: *n_keys, keys (room
+// for n x 3) and flags (n_cand). Returns 0 or the first failing esikf_status.
+int fl2_shim_retrieve_run(const esikf_camera *cam, const esikf_vio_cfg *vcfg, const esikf_extrinsics *ext, const double *state, const double *pg, int n, int border,
+                          const double *cand_pos, const double *cand_pc, int n_cand, int32_t *n_keys, int64_t *keys, uint8_t *flags) {
+  esikf_ctx *ctx = nullptr;
+  int rc = esikf_create(&ctx, 0);
+  if (rc) return rc;
+  {
+    VIOManager vio(ctx);
+    StatesGroup st, stp;
+    st.unpack(state), stp.unpack(state);
+    vio.state = &st, vio.state_propagat = &stp;
+    vio.patch_pyrimid_level = vcfg->patch_pyrimid_level, vio.max_iterations = vcfg->max_iterations, vio.img_point_cov = vcfg->img_point_cov;
+    vio.cam = *cam;
+    memcpy(vio.Rcl.m, ext->Rcl, 72), memcpy(vio.Pcl.v, ext->Pcl, 24), memcpy(vio.extR.m, ext->extR, 72), memcpy(vio.extT.v, ext->extT, 24);
+    vio.initializeVIO();
+    std::vector<pointWithVar> scan(n);
+    for (int i = 0; i < n; i++)
+      for (int k = 0; k < 3; k++) scan[i].point_w[k] = pg[3 * i + k];
+    std::vector<VOXEL_LOCATION> kv;
+    std::vector<uint8_t> fl;
+    if (!vio.last_status_) vio.RetrieveScanVoxels(border, &scan, kv);
+    if (!vio.last_status_) vio.CheckDepthContinuity(n_cand, cand_pos, cand_pc, fl);
+    rc = vio.last_status_;
+    if (!rc) {
+      *n_keys = (int32_t)kv.size();
+      for (size_t i = 0; i < kv.size(); i++) keys[3 * i] = kv[i].x, keys[3 * i + 1] = kv[i].y, keys[3 * i + 2] = kv[i].z;
+      memcpy(flags, fl.data(), fl.size());
     }
   }
   esikf_destroy(ctx);

@@ -365,6 +365,15 @@ class VIOManager {
   // computeJacobianAndUpdateEKF. Call once per VIO tick, after it.
   void UpdateVisualMapPoints(const std::vector<uint8_t> &converged, const std::vector<LastObservation> &last_obs, std::vector<uint8_t> &update_flag,
                              std::vector<NewObservation> &new_obs);
+  // The scan side of retrieveFromVisualSparseMap (src/vio.cpp:386-428) on the device: keys receives the scan's distinct 0.5 m
+  // voxel keys in first-occurrence order (insert them into sub_feat_map in this order: it then iterates as the reference's),
+  // and the device keeps the depth image for CheckDepthContinuity. pg == nullptr: the pv list the last
+  // VoxelMapManager::UpdateVoxelMap() left on the device (_pv_list), else those points. border as initializeVIO left it; the
+  // frame pose is that of *state (the VIO prior). Call at the start of the VIO tick.
+  void RetrieveScanVoxels(int border, const std::vector<pointWithVar> *pg, std::vector<VOXEL_LOCATION> &keys);
+  // The depth-continuity check of :614-640 for n retrieved points (pos: VisualPoint::pos_, pc: the w2c(pos_) the map-side walk
+  // computed, 3 and 2 doubles each) against the depth image of the last RetrieveScanVoxels: discontinuous[i] = depth_continous.
+  void CheckDepthContinuity(int n, const double *pos, const double *pc, std::vector<uint8_t> &discontinuous);
 
  private:
   const uint8_t *patch_img_ = nullptr, *patch_ref_img_ = nullptr;  // what the per-patch helpers uploaded last
@@ -390,6 +399,10 @@ class VIOManager {
   std::vector<double> obs_in_, obs_pc_;  // UpdateVisualMapPoints' last observations (T | px) and the added entries' pc
   std::vector<int32_t> obs_entry_;
   std::vector<float> obs_patch_;
+  PinnedBuf<double> st_ret_pt_, st_ret_cand_;  // RetrieveScanVoxels' host scan, CheckDepthContinuity's pos | pc
+  PinnedBuf<int32_t> st_ret_keys_;
+  PinnedBuf<uint8_t> st_ret_flag_;
+  int32_t keys_cap_ = 0;  // the resident scan's largest key count seen
   bool ref_imgs_current_ = false;    // false once the per-patch warpAffine replaced the device's reference images
 };
 

@@ -416,6 +416,41 @@ int esikf_vio_generate_points(esikf_ctx *ctx, const double *point_w, const doubl
 int esikf_vio_update_points(esikf_ctx *ctx, int32_t n, const uint8_t *converged, const double *last_T_f_w, const double *last_px, const double *state,
                             int32_t cap, int32_t *n_out, uint8_t *update_flag_out, int32_t *entry_out, double *pc_out, float *patch_out);
 
+/* ---------------------------------------------------------------- scan side of the visual sub-map retrieval (retrieveFromVisualSparseMap)
+ * The parts of VIOManager::retrieveFromVisualSparseMap that read the LiDAR scan pg, on the device: the scan's voxel keys and its
+ * depth image (src/vio.cpp:386-428), and the depth-continuity check of the retrieved points (:614-640). The walk over the
+ * host's feat_map, ray casting and the choice of the reference feature stay with the caller (INTEGRATION.md §2). Call
+ * esikf_vio_retrieve_scan at the start of the VIO tick, then esikf_vio_depth_check on the retrieved points, before
+ * esikf_vio_select_patches.
+ *
+ * esikf_vio_retrieve_scan:
+ *   pg      : point_w == NULL: the pv list the last esikf_map_device_update left on the device (the source of
+ *             esikf_vio_generate_points(point_w = NULL)), n ignored; ESIKF_ERR_STATE when there is none. Else n host points
+ *             (point_w, 3 doubles each).
+ *   border  : as initializeVIO left it (vio.cpp:154).
+ *   state   : a packed host state whose frame pose (updateFrameState's) is the frame's: *state at the start of processFrame, the
+ *             VIO prior. NULL: the LIO posterior resident on the device after esikf_lio_run (ESIKF_ERR_STATE when the device
+ *             holds another one); a caller that propagates the state between the LIO and the VIO tick passes it explicitly.
+ * Keys: every scan point's voxel key, loc = floor(c / 0.5) in double, then loc -= 1.0 when negative (the retrieval's own
+ * formula, :392-396, not the map's), including points behind the camera or outside the image. The distinct keys come out in
+ * first-occurrence order (the scan index of each key's first point), *n_keys of them, 3 int32 each: inserted into
+ * sub_feat_map in this order they give the reference's insertion sequence. If *n_keys exceeds cap, nothing else is written and
+ * the call returns ESIKF_ERR_ARG. A key outside [-2^20, 2^20) (the device map's key range): ESIKF_ERR_ARG, nothing written.
+ * Depth image (width x height floats, kept on the device for esikf_vio_depth_check, copied to depth_out when not NULL): a
+ * point with pt_c[2] > 0 and isInFrame(px.cast<int>(), border) writes float(pt_c[2]) at width * int(px[1]) + int(px[0]);
+ * the last such point in scan order wins a pixel; an untouched pixel is 0.
+ *
+ * esikf_vio_depth_check: for n retrieved points (the retrieve_voxel_points[i] of the TYPE_MAP cells, in cell order), pos_w
+ * (VisualPoint::pos_, 3 doubles each) and pc (the caller's w2c(pos_), 2 doubles each, as it computed the cell index at
+ * :466-471), discontinuous_out[i] = 1 when a tap (int(pc[0]) + u, int(pc[1]) + v), u, v in [-4, 4], (u, v) != (0, 0), of the
+ * depth image holds a nonzero depth with |pt_cam[2] - depth| > 0.5 in double, pt_cam = w2f(pos_) with the frame pose of the
+ * last esikf_vio_retrieve_scan; such a point is dropped (:640). A tap outside the image is empty. ESIKF_ERR_STATE when no
+ * esikf_vio_retrieve_scan succeeded since the last esikf_vio_set_camera.
+ * With several ranks every rank evaluates the whole scan and all points. */
+int esikf_vio_retrieve_scan(esikf_ctx *ctx, const double *point_w, int32_t n, int32_t border, const double *state, int32_t cap, int32_t *n_keys,
+                            int32_t *keys_out, float *depth_out);
+int esikf_vio_depth_check(esikf_ctx *ctx, int32_t n, const double *pos_w, const double *pc, uint8_t *discontinuous_out);
+
 /* ---------------------------------------------------------------- multi-GPU (one process per GPU)
  * The residual point / patch set is sharded by contiguous blocks; each iteration all-reduces the
  * packed information buffer [HTH upper | HTz | M | sum|d| ...] and every rank solves redundantly.
