@@ -117,6 +117,14 @@ int main() {
     std::vector<NewObservation> new_obs;
     vio_manager.UpdateVisualMapPoints(converged, last_obs, update_flag, new_obs);
     std::printf("tick %d new observations: status %d, %zu of %d entries\n", tick, vio_manager.last_status_, new_obs.size(), vio_manager.total_points);
+    // updateReferencePatch (vio.cpp:969-1034): the plane under each sub-map entry that passes the four skips, in one lookup
+    // on the device map (no host mirror); the normal refinement and the patch scoring stay the caller's (INTEGRATION.md §3).
+    std::vector<V3D> ref_pos(1);
+    ref_pos[0][0] = 0.3, ref_pos[0][1] = 0.2, ref_pos[0][2] = 0.0;  // the candidate's pos_, on the floor
+    uint8_t found[1];
+    VoxelPlane plane[1];
+    voxelmap_manager.FindCorrespond(1, ref_pos.data(), ESIKF_FIND_RULE_PATCH, found, plane);
+    std::printf("tick %d reference-patch lookup: status %d, answer %d\n", tick, voxelmap_manager.last_status_, (int)found[0]);
   }
   // somebody wants the warp patches of the last selection on the host after all
   vio_manager.MaterializeWarpPatches();

@@ -93,6 +93,7 @@ def load_library():
     lib.esikf_map_device_slide.argtypes = [vp, vp, vp]
     lib.esikf_map_device_download.argtypes = [vp, vp, vp, vp, C.c_int32, vp, C.c_int32, vp, vp]
     lib.esikf_map_device_export.argtypes = [vp, vp, vp, vp, C.c_int32, vp, C.c_int32, vp, vp]
+    lib.esikf_map_device_find.argtypes = [vp, vp, C.c_int32, C.c_int32, vp, vp, vp]
     lib.esikf_lio_fetch_normals.argtypes = [vp, vp]
     lib.esikf_lio_set_scan.argtypes = [vp, vp, C.c_int32]
     lib.esikf_lio_run.argtypes = [vp, vp, vp, C.POINTER(LioCfgC)]
@@ -135,6 +136,8 @@ def load_library():
 TUNE_STAGE_LDG = 1
 TUNE_VIO_TMA = 2  # esikf_set_tuning flag: stage LIO plane records with __ldg copies instead of cp.async.bulk (measurement variant)
 GEN_ADD_FROM = 0x40000000  # esikf_vio_generate_points: the source of a winner from the add_from list
+FIND_RULE_PATCH, FIND_RULE_RAYCAST = 0, 1  # esikf_map_device_find: updateReferencePatch's key, the ray casting's key
+FIND_NO_ROOT, FIND_NODE, FIND_PLANE = 0, 1, 2  # esikf_map_device_find's status per point
 DEFAULT_LOOP_MODE = 2  # esikf_set_loop_mode: 2 (alias 1) persistent kernel per update, 0 per-iteration launches
 
 class MapCfgC(C.Structure):
@@ -150,7 +153,7 @@ class MapStatsC(C.Structure):
 
 EXPORTED_SYMBOLS = [
     "esikf_create", "esikf_destroy", "esikf_last_error", "esikf_stream", "esikf_synchronize", "esikf_host_alloc", "esikf_host_free", "esikf_launch_count", "esikf_set_solve_mode", "esikf_set_loop_mode", "esikf_set_tuning",
-    "esikf_set_extrinsics", "esikf_set_lidar_extrinsics", "esikf_map_upload", "esikf_map_patch", "esikf_map_device_init", "esikf_map_device_build", "esikf_map_device_update", "esikf_map_device_update_points", "esikf_map_device_slide", "esikf_map_device_stats", "esikf_map_device_capacity", "esikf_map_device_download", "esikf_map_device_export", "esikf_lio_fetch_normals", "esikf_lio_set_scan", "esikf_lio_run", "esikf_lio_fetch",
+    "esikf_set_extrinsics", "esikf_set_lidar_extrinsics", "esikf_map_upload", "esikf_map_patch", "esikf_map_device_init", "esikf_map_device_build", "esikf_map_device_update", "esikf_map_device_update_points", "esikf_map_device_slide", "esikf_map_device_stats", "esikf_map_device_capacity", "esikf_map_device_download", "esikf_map_device_export", "esikf_map_device_find", "esikf_lio_fetch_normals", "esikf_lio_set_scan", "esikf_lio_run", "esikf_lio_fetch",
     "esikf_lio_update", "esikf_lio_fetch_point_cov", "esikf_vio_set_camera", "esikf_vio_set_image", "esikf_vio_set_patches",
     "esikf_vio_run", "esikf_vio_fetch", "esikf_vio_update", "esikf_vio_get_image_patch", "esikf_vio_set_ref_images",
     "esikf_vio_warp_patches", "esikf_vio_select_patches", "esikf_vio_warp_affine", "esikf_vio_set_inverse_refs", "esikf_rgb_set_cloud", "esikf_rgb_colorize", "esikf_vio_generate_points", "esikf_vio_update_points", "esikf_vio_retrieve_scan", "esikf_vio_depth_check", "esikf_comm_unique_id", "esikf_comm_init", "esikf_comm_rank", "esikf_shard_range", "esikf_peer_export", "esikf_peer_attach", "esikf_profile_kernel", "esikf_set_kernel_timing", "esikf_get_kernel_timing", "esikf_set_phase_stamps", "esikf_get_phase_stamps",
@@ -312,6 +315,18 @@ class Context:
         self._ck(self.lib.esikf_map_device_export(self.h, keys.ctypes.data, first.ctypes.data, count.ctypes.data, len(first), nodes.ctypes.data, len(nodes),
                                                   C.byref(nr), C.byref(nn)))
         return dict(keys=keys[:nr.value], first=first[:nr.value], count=count[:nr.value], nodes=nodes[:nn.value])
+
+    def map_device_find(self, points, rule):
+        """find_correspond on the device map for world points (n x 3) from the root voxel the call site's key rule gives
+        (FIND_RULE_PATCH / FIND_RULE_RAYCAST): status (FIND_*), key (n x 3, INT64_MIN when out of range) and planes
+        (synthetic.PLANE_DTYPE: the found node's layer, path and plane fields, zero where there is no root)."""
+        from .synthetic import PLANE_DTYPE
+
+        pts = _c(points, np.float64).reshape(-1, 3)
+        n = len(pts)
+        status, keys, rows = np.zeros(n, np.uint8), np.zeros((n, 3), np.int64), np.zeros(n, PLANE_DTYPE)
+        self._ck(self.lib.esikf_map_device_find(self.h, pts.ctypes.data, n, rule, status.ctypes.data, keys.ctypes.data, rows.ctypes.data))
+        return dict(status=status, key=keys, planes=rows)
 
     def lio_fetch_normals(self):
         out = np.zeros((self.n_pts, 3), np.float64)

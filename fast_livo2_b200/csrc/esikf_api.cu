@@ -26,6 +26,7 @@
 #include "esikf_generate.cu"
 #include "esikf_observe.cu"
 #include "esikf_retrieve.cu"
+#include "esikf_find.cu"
 
 using namespace esikf;
 
@@ -288,6 +289,13 @@ struct esikf_ctx {
   int ret_w = 0, ret_h = 0;
   bool ret_valid = false;  // a depth image and its pose are in place (cleared by esikf_vio_set_camera and by a failed call)
 
+  // find_correspond lookups on the device map (esikf_map_device_find): the points, the answers in one block
+  // [rows n x 256 B | keys n x 24 B | status n B] on the device, and its pinned host copy (grow-only)
+  DevBuf<double> find_pt;
+  DevBuf<uint8_t> find_out;
+  uint8_t *find_host = nullptr;
+  size_t find_host_cap = 0;
+
   // multi-GPU
   int rank = 0, nranks = 1;
   ncclComm_t comm = nullptr;
@@ -317,6 +325,7 @@ struct esikf_ctx {
     if (mailbox) cudaFree(mailbox);
     if (stage) cudaFreeHost(stage);
     if (stage_ctrl) cudaFreeHost(stage_ctrl);
+    if (find_host) cudaFreeHost(find_host);
     for (cudaEvent_t e : stage_ev)
       if (e) cudaEventDestroy(e);
     for (cudaEvent_t e : ev) cudaEventDestroy(e);
@@ -965,6 +974,40 @@ int esikf_map_device_export(esikf_ctx *ctx, int64_t *keys, int32_t *first, int32
   CK(cudaMemcpyAsync(count, ctx->map_exp_count.p, (size_t)nr * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(nodes, ctx->map_exp_nodes.p, (size_t)nn * sizeof(esikf_map_node), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
+  return ESIKF_OK;
+}
+
+int esikf_map_device_find(esikf_ctx *ctx, const double *points, int32_t n, int32_t rule, uint8_t *status, int64_t *keys, esikf_plane *rows) {
+  if (!ctx || n < 0 || (rule != ESIKF_FIND_RULE_PATCH && rule != ESIKF_FIND_RULE_RAYCAST) || (n > 0 && (!points || !status || !keys || !rows)))
+    return fail(ctx, ESIKF_ERR_ARG, "map_device_find: bad argument");
+  if (!ctx->dev_map || !ctx->have_map)
+    return fail(ctx, ESIKF_ERR_STATE, "map_device_find: no live device map (esikf_map_device_init first; a failed call or esikf_map_upload voids it)");
+  if (n == 0) return ESIKF_OK;
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t rows_b = (size_t)n * sizeof(esikf_plane), keys_b = (size_t)n * 3 * sizeof(int64_t), bytes = rows_b + keys_b + (size_t)n;
+  CK(ctx->find_pt.reserve((size_t)n * 3));
+  CK(ctx->find_out.reserve(bytes));
+  if (bytes > ctx->find_host_cap) {
+    if (ctx->find_host) cudaFreeHost(ctx->find_host);
+    ctx->find_host = nullptr, ctx->find_host_cap = 0;
+    CK(cudaMallocHost((void **)&ctx->find_host, bytes + bytes / 4));
+    ctx->find_host_cap = bytes + bytes / 4;
+  }
+  CK(cudaMemcpyAsync(ctx->find_pt.p, points, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+  uint8_t *d = ctx->find_out.p;
+  MapFindArgs a;
+  a.pts = ctx->find_pt.p, a.n = n, a.rule = rule;
+  a.rows = (esikf_plane *)d, a.keys = (long long *)(d + rows_b), a.status = d + rows_b + keys_b;
+  map_find_kernel<<<(n + FIND_THREADS - 1) / FIND_THREADS, FIND_THREADS, 0, st>>>(ctx->arena(), a);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  // one copy into pinned staging and one synchronisation; the caller's buffers are written only once everything succeeded
+  CK(cudaMemcpyAsync(ctx->find_host, d, bytes, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  memcpy(rows, ctx->find_host, rows_b);
+  memcpy(keys, ctx->find_host + rows_b, keys_b);
+  memcpy(status, ctx->find_host + rows_b + keys_b, (size_t)n);
   return ESIKF_OK;
 }
 

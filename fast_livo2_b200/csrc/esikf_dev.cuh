@@ -27,6 +27,33 @@ __host__ __device__ inline unsigned long long pack_key(long long x, long long y,
   return ((unsigned long long)(x + ESIKF_KEY_BIAS) << 42) | ((unsigned long long)(y + ESIKF_KEY_BIAS) << 21) |
          (unsigned long long)(z + ESIKF_KEY_BIAS);
 }
+#ifdef __CUDACC__
+// ---- the 0.5 m voxel keys of the VIO front end (reference src/vio.cpp). Both divide by the literal 0.5, not by the map's voxel
+// size. false when the key leaves [-2^20, 2^20) (NaN and infinities included), where the host's conversion would not be defined
+// or the map's packing would wrap; the range is checked before anything is packed.
+//
+// The retrieval and its ray casting (:392-396, :508-514): loc_xyz[j] = floor(c / 0.5); if (loc_xyz[j] < 0) loc_xyz[j] -= 1.0 with
+// an int loc_xyz: the double quotient floored, the int it converts to, and for a negative one the int of (double)loc - 1.0.
+// -0.0 floors to -0.0, whose int is 0.
+__device__ __forceinline__ bool ret_voxel_key(double c, long long &k) {
+  const double f = floor(__ddiv_rn(c, 0.5));
+  if (!(f >= -(double)ESIKF_KEY_BIAS && f < (double)ESIKF_KEY_BIAS)) return false;
+  int loc = (int)f;
+  if (loc < 0) loc = (int)__dsub_rn((double)loc, 1.0);
+  k = loc;
+  return loc >= -ESIKF_KEY_BIAS;
+}
+// updateReferencePatch (:983-989): float loc_xyz[j] = c / 0.5 (the double quotient narrowed to float); if negative, loc -= 1.0
+// (in double, narrowed again); then (int64_t)loc, which truncates. This is map_voxel_key's arithmetic with the divisor 0.5f.
+// trunc(loc) lies in [-2^20, 2^20) exactly when -2^20 - 1 < loc < 2^20 (both bounds are floats).
+__device__ __forceinline__ bool patch_voxel_key(double c, long long &k) {
+  float loc = __double2float_rn(__ddiv_rn(c, 0.5));
+  if (loc < 0) loc = __double2float_rn(__dsub_rn((double)loc, 1.0));
+  if (!(loc > -(float)(ESIKF_KEY_BIAS + 1) && loc < (float)ESIKF_KEY_BIAS)) return false;
+  k = (long long)loc;
+  return true;
+}
+#endif
 __host__ __device__ inline uint32_t hash_key(unsigned long long k) {
   k ^= k >> 33;
   k *= 0xff51afd7ed558ccdull;

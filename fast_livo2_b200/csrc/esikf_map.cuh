@@ -157,6 +157,19 @@ MAP_HD int map_slot_of(const MapArena &A, unsigned long long k) {
   return -1;
 }
 
+// find the slot of a key without inserting it: a pure read of the table. -1: absent. Keys are never removed from a live
+// table (a slide or a growth copies the survivors into a fresh one), so the first empty slot ends the probe. lio_update_kernel's
+// `probe` (esikf_lio.cu) walks the same table the same way with 16-byte slot loads and no probe bound; keep the two in step.
+MAP_HD int map_find_slot(const MapArena &A, unsigned long long k) {
+  uint32_t s = hash_key(k) & A.hash_mask;
+  for (uint32_t probes = 0; probes <= A.hash_mask; probes++, s = (s + 1) & A.hash_mask) {
+    const unsigned long long cur = A.slots[s].key;
+    if (cur == k) return (int)s;
+    if (cur == ESIKF_KEY_EMPTY) return -1;
+  }
+  return -1;
+}
+
 // ---- nodes
 template <class C>
 MAP_HD int map_new_node(const MapArena &A, const C &co, int layer, const double *center, float quarter) {

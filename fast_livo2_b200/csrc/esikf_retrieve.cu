@@ -46,18 +46,6 @@ __device__ __forceinline__ void ret_frame_pose(const double *Rci, const double *
   __syncthreads();
 }
 
-// loc_xyz[j] = floor(pt_w[j] / voxel_size); if (loc_xyz[j] < 0) loc_xyz[j] -= 1.0 (:392-396): the double quotient floored, the
-// int it converts to, and for a negative one the int of (double)loc - 1.0. -0.0 floors to -0.0, whose int is 0. false when the
-// key leaves [-2^20, 2^20) (NaN included), where the host's conversion would not be defined or the map's packing would wrap.
-__device__ __forceinline__ bool ret_voxel_key(double c, long long &k) {
-  const double f = floor(__ddiv_rn(c, 0.5));
-  if (!(f >= -(double)ESIKF_KEY_BIAS && f < (double)ESIKF_KEY_BIAS)) return false;
-  int loc = (int)f;
-  if (loc < 0) loc = (int)__dsub_rn((double)loc, 1.0);
-  k = loc;
-  return loc >= -ESIKF_KEY_BIAS;
-}
-
 __global__ void __launch_bounds__(RET_THREADS) ret_scan_kernel(const RetArgs a) {
   __shared__ double Rcw[9], Pcw[3];
   ret_frame_pose(a.Rci, a.Pci, a.state, Rcw, Pcw);

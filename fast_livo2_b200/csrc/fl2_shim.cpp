@@ -348,6 +348,42 @@ void VoxelMapManager::SetWorldCloud(const std::vector<PointXYZ> *dense_scan) {
   if ((last_status_ = esikf_rgb_set_cloud(ctx_, pts, n, sbuf)) != 0) last_error_ = esikf_last_error(ctx_);
 }
 
+void VoxelMapManager::FindCorrespond(int n, const V3D *pts, int rule, uint8_t *status, VoxelPlane *planes) {
+  if (!ctx_ || !device_map_) {
+    last_status_ = ESIKF_ERR_STATE, last_error_ = "FindCorrespond: EnableDeviceMap first (a host-owned voxel_map_ is read by the reference's own code)";
+    return;
+  }
+  if (n < 0 || (n > 0 && (!pts || !status || !planes))) {
+    last_status_ = ESIKF_ERR_ARG, last_error_ = "FindCorrespond: bad argument";
+    return;
+  }
+  double *p = st_find_pts_.get((size_t)n * 3 + 3);
+  uint8_t *st = st_find_status_.get((size_t)n + 1);
+  int64_t *keys = st_find_keys_.get((size_t)n * 3 + 3);
+  esikf_plane *rows = st_find_rows_.get((size_t)n + 1);
+  if (!p || !st || !keys || !rows) {
+    last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
+    return;
+  }
+  for (int i = 0; i < n; i++)
+    for (int k = 0; k < 3; k++) p[3 * i + k] = pts[i][k];
+  if ((last_status_ = esikf_map_device_find(ctx_, p, n, rule, st, keys, rows)) != 0) {
+    last_error_ = esikf_last_error(ctx_);
+    return;
+  }
+  for (int i = 0; i < n; i++) {
+    status[i] = st[i];
+    VoxelPlane &o = planes[i];
+    o = VoxelPlane();
+    if (st[i] == ESIKF_FIND_NO_ROOT) continue;
+    const esikf_plane &r = rows[i];
+    for (int k = 0; k < 3; k++) o.center_[k] = r.center[k], o.normal_[k] = r.normal[k];
+    for (int a = 0, t = 0; a < 6; a++)
+      for (int b = a; b < 6; b++, t++) o.plane_var_[6 * a + b] = o.plane_var_[6 * b + a] = r.plane_var[t];
+    o.d_ = r.d, o.radius_ = r.radius, o.is_plane_ = st[i] == ESIKF_FIND_PLANE;
+  }
+}
+
 // src/voxel_map.cpp:924-948: nothing until the sensor moved sliding_thresh, then roots further than half_map_size voxels go
 void VoxelMapManager::mapSliding() {
   if (!ctx_ || !device_map_) {
@@ -1500,6 +1536,27 @@ int fl2_shim_session_map_sliding(void *h, const double *position, int half_map_s
   for (int k = 0; k < 3; k++) mgr.position_last_[k] = position[k];
   mgr.mapSliding();
   return mgr.last_status_;
+}
+// VoxelMapManager::FindCorrespond through a session; the answers in esikf_plane rows (plane_var_'s upper triangle; layer and
+// path are not part of a VoxelPlane and stay 0)
+int fl2_shim_session_find_correspond(void *h, const double *pts, int n, int rule, uint8_t *status, esikf_plane *rows) {
+  ShimSession *s = static_cast<ShimSession *>(h);
+  if (!s || n < 0) return ESIKF_ERR_ARG;
+  std::vector<V3D> p(n);
+  for (int i = 0; i < n; i++)
+    for (int k = 0; k < 3; k++) p[i][k] = pts[3 * (size_t)i + k];
+  std::vector<VoxelPlane> planes(n);
+  s->mgr->FindCorrespond(n, p.data(), rule, status, planes.data());
+  if (s->mgr->last_status_) return s->mgr->last_status_;
+  for (int i = 0; i < n; i++) {
+    esikf_plane &r = rows[i];
+    memset(&r, 0, sizeof(r));
+    for (int k = 0; k < 3; k++) r.center[k] = planes[i].center_[k], r.normal[k] = planes[i].normal_[k];
+    for (int a = 0, t = 0; a < 6; a++)
+      for (int b = a; b < 6; b++, t++) r.plane_var[t] = planes[i].plane_var_[6 * a + b];
+    r.d = planes[i].d_, r.radius = planes[i].radius_;
+  }
+  return 0;
 }
 void *fl2_shim_session_context(void *h) { return static_cast<ShimSession *>(h)->mgr->context(); }
 

@@ -221,6 +221,11 @@ class VoxelMapManager {
   // StateEstimation left it on the device (dense_map_en = false), moved to the world frame with state_. Call after
   // StateEstimation, once per LIO tick.
   void SetWorldCloud(const std::vector<PointXYZ> *dense_scan = nullptr);
+  // The VIO front end's find_correspond lookups on the device map, mirror or no mirror (esikf_map_device_find): for the n points
+  // pts, the root voxel by the call site's key rule (ESIKF_FIND_RULE_PATCH: updateReferencePatch, ESIKF_FIND_RULE_RAYCAST: the
+  // retrieval's ray casting), then find_correspond. status[i] = ESIKF_FIND_*; planes[i] = the found node's plane_ptr_ as the
+  // callers read it (center_, normal_, plane_var_ as 6 x 6, d_, radius_, is_plane_), a default VoxelPlane where no root exists.
+  void FindCorrespond(int n, const V3D *pts, int rule, uint8_t *status, VoxelPlane *planes);
   esikf_ctx *context() { return ctx_; }
 
  private:
@@ -237,6 +242,10 @@ class VoxelMapManager {
   PinnedBuf<int64_t> exp_keys_;
   PinnedBuf<int32_t> exp_first_, exp_count_;
   PinnedBuf<esikf_map_node> exp_nodes_;
+  PinnedBuf<double> st_find_pts_;  // FindCorrespond's points and answers
+  PinnedBuf<uint8_t> st_find_status_;
+  PinnedBuf<int64_t> st_find_keys_;
+  PinnedBuf<esikf_plane> st_find_rows_;
   int32_t exp_roots_cap_ = 1024, exp_nodes_cap_ = 4096;  // what the export buffers are requested with (grown from the ticks seen)
 };
 

@@ -241,6 +241,25 @@ typedef struct esikf_map_node {
  * removed with the slide's own bounds). */
 int esikf_map_device_export(esikf_ctx *ctx, int64_t *keys, int32_t *first, int32_t *count, int32_t roots_cap, esikf_map_node *nodes, int32_t nodes_cap,
                             int32_t *n_roots, int32_t *n_nodes);
+/* The VIO front end's octree lookups on the device map, without a host mirror: for each of n world points (host, n x 3), the
+ * root voxel the reference looks up, then VoxelOctoTree::find_correspond (src/voxel_map.cpp:292-305) from that root. The key
+ * rule is the reference's own at the call site, and both divide by the literal 0.5 (not the map's voxel size):
+ *   ESIKF_FIND_RULE_PATCH   updateReferencePatch (src/vio.cpp:983-989): float loc = p / 0.5, loc -= 1.0 when negative, (int64_t)loc
+ *   ESIKF_FIND_RULE_RAYCAST the retrieval's ray casting (:508-514): int loc = floor(p / 0.5), loc -= 1.0 when negative
+ * Outputs per point: status (ESIKF_FIND_*), keys (n x 3, the root looked up; INT64_MIN on every axis when the key leaves
+ * [-2^20, 2^20), NaN and infinities included, which answers ESIKF_FIND_NO_ROOT), and rows (n): for a found node its layer and
+ * path (as esikf_plane.path) and its plane_ptr_ fields center, normal, plane_var, d, radius (the bytes esikf_map_device_export
+ * gives for the node; meaningful for ESIKF_FIND_PLANE); all zero for ESIKF_FIND_NO_ROOT.
+ * A pure read of the map, enqueued on the context's stream after the calls before it; returns when the answers are in. Every
+ * rank answers every point. ESIKF_ERR_STATE when no device map is live (never set up, invalidated by a failed call, or
+ * replaced by esikf_map_upload); ESIKF_ERR_ARG for n < 0, an unknown rule or a NULL buffer with n > 0. A failed call writes
+ * nothing. */
+#define ESIKF_FIND_RULE_PATCH 0
+#define ESIKF_FIND_RULE_RAYCAST 1
+#define ESIKF_FIND_NO_ROOT 0
+#define ESIKF_FIND_NODE 1  /* a node that is not a plane */
+#define ESIKF_FIND_PLANE 2
+int esikf_map_device_find(esikf_ctx *ctx, const double *points, int32_t n, int32_t rule, uint8_t *status, int64_t *keys, esikf_plane *rows);
 
 /* ---------------------------------------------------------------- LIO update (StateEstimation)
  * Staged form (device-resident between calls):
