@@ -6,6 +6,7 @@
 // happen WHEN and who owns what, not a meaningful estimate. Needs an H100 to run; without one the managers report an error.
 //   g++ -std=c++17 -Iinclude examples/tick_loop.cpp -Lfast_livo2_b200 -lfl2_shim -lesikf_b200 -Wl,-rpath,$PWD/fast_livo2_b200 -o tick_loop
 #include <cstdio>
+#include <cstring>
 #include <vector>
 
 #include "../fast_livo2_b200/csrc/fl2_shim.hpp"
@@ -118,13 +119,29 @@ int main() {
     vio_manager.UpdateVisualMapPoints(converged, last_obs, update_flag, new_obs);
     std::printf("tick %d new observations: status %d, %zu of %d entries\n", tick, vio_manager.last_status_, new_obs.size(), vio_manager.total_points);
     // updateReferencePatch (vio.cpp:969-1034): the plane under each sub-map entry that passes the four skips, in one lookup
-    // on the device map (no host mirror); the normal refinement and the patch scoring stay the caller's (INTEGRATION.md §3).
+    // on the device map (no host mirror); the normal refinement stays the caller's (INTEGRATION.md §3).
     std::vector<V3D> ref_pos(1);
     ref_pos[0][0] = 0.3, ref_pos[0][1] = 0.2, ref_pos[0][2] = 0.0;  // the candidate's pos_, on the floor
     uint8_t found[1];
     VoxelPlane plane[1];
     voxelmap_manager.FindCorrespond(1, ref_pos.data(), ESIKF_FIND_RULE_PATCH, found, plane);
     std::printf("tick %d reference-patch lookup: status %d, answer %d\n", tick, voxelmap_manager.last_status_, (int)found[0]);
+    // ... and the patch scoring (vio.cpp:1036-1097) of the same entry in one call: its six observations, seen from the
+    // identity pose and from five poses stepped along x, with the floor's normal; the caller writes score_, mean_ and the
+    // chosen ref_patch back into its Feature / VisualPoint objects (INTEGRATION.md §3).
+    std::vector<ScoredPoint> scored(1, ScoredPoint{{0.3, 0.2, 0.0}, {0.0, 0.0, 1.0}});
+    std::vector<PatchObservation> obs(6);
+    for (int k = 0; k < 6; k++) {
+      PatchObservation &o = obs[k];
+      const double T[12] = {1, 0, 0, 0, 1, 0, 0, 0, 1, 0.1 * k, 0, 2.0};
+      memcpy(o.T_f_w, T, sizeof(T));
+      for (int t = 0; t < 64; t++) o.patch[t] = (float)(100 + (t * (k + 3)) % 17);
+      o.mean = 0.0f, o.id = tick * 10 + k;
+    }
+    std::vector<float> score, mean;
+    std::vector<int32_t> ref;
+    vio_manager.ScoreReferencePatches(std::vector<int32_t>{0, 6}, scored, obs, score, mean, ref);
+    std::printf("tick %d reference patch: status %d, observation %d\n", tick, vio_manager.last_status_, ref.empty() ? -1 : ref[0]);
   }
   // somebody wants the warp patches of the last selection on the host after all
   vio_manager.MaterializeWarpPatches();

@@ -118,6 +118,7 @@ def load_library():
     lib.esikf_vio_update_points.argtypes = [vp, C.c_int32, vp, vp, vp, vp, C.c_int32, ip, vp, vp, vp, vp]
     lib.esikf_vio_retrieve_scan.argtypes = [vp, vp, C.c_int32, C.c_int32, vp, C.c_int32, ip, vp, vp]
     lib.esikf_vio_depth_check.argtypes = [vp, C.c_int32, vp, vp, vp]
+    lib.esikf_vio_score_ref_patches.argtypes = [vp, C.c_int32, vp, C.c_int32] + [vp] * 9
     lib.esikf_comm_unique_id.argtypes = [C.c_char_p]
     lib.esikf_comm_init.argtypes = [vp, C.c_int32, C.c_int32, C.c_char_p]
     lib.esikf_comm_rank.argtypes = [vp, ip, ip]
@@ -156,7 +157,7 @@ EXPORTED_SYMBOLS = [
     "esikf_set_extrinsics", "esikf_set_lidar_extrinsics", "esikf_map_upload", "esikf_map_patch", "esikf_map_device_init", "esikf_map_device_build", "esikf_map_device_update", "esikf_map_device_update_points", "esikf_map_device_slide", "esikf_map_device_stats", "esikf_map_device_capacity", "esikf_map_device_download", "esikf_map_device_export", "esikf_map_device_find", "esikf_lio_fetch_normals", "esikf_lio_set_scan", "esikf_lio_run", "esikf_lio_fetch",
     "esikf_lio_update", "esikf_lio_fetch_point_cov", "esikf_vio_set_camera", "esikf_vio_set_image", "esikf_vio_set_patches",
     "esikf_vio_run", "esikf_vio_fetch", "esikf_vio_update", "esikf_vio_get_image_patch", "esikf_vio_set_ref_images",
-    "esikf_vio_warp_patches", "esikf_vio_select_patches", "esikf_vio_warp_affine", "esikf_vio_set_inverse_refs", "esikf_rgb_set_cloud", "esikf_rgb_colorize", "esikf_vio_generate_points", "esikf_vio_update_points", "esikf_vio_retrieve_scan", "esikf_vio_depth_check", "esikf_comm_unique_id", "esikf_comm_init", "esikf_comm_rank", "esikf_shard_range", "esikf_peer_export", "esikf_peer_attach", "esikf_profile_kernel", "esikf_set_kernel_timing", "esikf_get_kernel_timing", "esikf_set_phase_stamps", "esikf_get_phase_stamps",
+    "esikf_vio_warp_patches", "esikf_vio_select_patches", "esikf_vio_warp_affine", "esikf_vio_set_inverse_refs", "esikf_rgb_set_cloud", "esikf_rgb_colorize", "esikf_vio_generate_points", "esikf_vio_update_points", "esikf_vio_retrieve_scan", "esikf_vio_depth_check", "esikf_vio_score_ref_patches", "esikf_comm_unique_id", "esikf_comm_init", "esikf_comm_rank", "esikf_shard_range", "esikf_peer_export", "esikf_peer_attach", "esikf_profile_kernel", "esikf_set_kernel_timing", "esikf_get_kernel_timing", "esikf_set_phase_stamps", "esikf_get_phase_stamps",
 ]
 
 
@@ -622,6 +623,26 @@ class Context:
         out = np.zeros(max(len(pos), 1), np.uint8)
         self._ck(self.lib.esikf_vio_depth_check(self.h, len(pos), pos.ctypes.data, pc.ctypes.data, out.ctypes.data))
         return out[:len(pos)]
+
+    # ------------------------------------------------------------------ reference patches (updateReferencePatch)
+    def vio_score_ref_patches(self, first, pos, normal, patch, mean, id_, T_f_w):
+        """The patch scoring of updateReferencePatch (esikf_vio_score_ref_patches, vio.cpp:1036-1097) for n visual points:
+        first (n + 1,) int32 offsets of each point's observations in obs_ order; pos, normal (n, 3) float64 (pos_, and normal_
+        after the plane half); per observation patch (m, 64) float32, mean (m,) float32 (mean_), id_ (m,) int32 and T_f_w
+        (m, 12) float64 (R row-major, then t). Returns score (m,) float32 (score_), mean (m,) float32 (mean_ afterwards) and
+        ref (n,) int32, the position of ref_patch within the point's list or -1 when no score beats -1000."""
+        first = _c(first, np.int32).reshape(-1)
+        n = len(first) - 1
+        pos, normal = _c(pos, np.float64).reshape(-1, 3), _c(normal, np.float64).reshape(-1, 3)
+        patch, mean = _c(patch, np.float32).reshape(-1, 64), _c(mean, np.float32).reshape(-1)
+        id_, T = _c(id_, np.int32).reshape(-1), _c(T_f_w, np.float64).reshape(-1, 12)
+        m = len(patch)
+        assert n >= 0 and len(pos) == n and len(normal) == n and len(mean) == m and len(id_) == m and len(T) == m
+        score, mean_out, ref = np.zeros(max(m, 1), np.float32), np.zeros(max(m, 1), np.float32), np.zeros(max(n, 1), np.int32)
+        self._ck(self.lib.esikf_vio_score_ref_patches(self.h, n, first.ctypes.data, m, pos.ctypes.data, normal.ctypes.data, patch.ctypes.data,
+                                                      mean.ctypes.data, id_.ctypes.data, T.ctypes.data, score.ctypes.data, mean_out.ctypes.data,
+                                                      ref.ctypes.data))
+        return dict(score=score[:m], mean=mean_out[:m], ref=ref[:n])
 
     # ------------------------------------------------------------------ multi-GPU / measurement
     def vio_set_inverse_refs(self, ref_img_index, ref_px, ref_f, ref_R, ref_pos):

@@ -27,6 +27,7 @@
 #include "esikf_observe.cu"
 #include "esikf_retrieve.cu"
 #include "esikf_find.cu"
+#include "esikf_refpatch.cu"
 
 using namespace esikf;
 
@@ -296,6 +297,15 @@ struct esikf_ctx {
   uint8_t *find_host = nullptr;
   size_t find_host_cap = 0;
 
+  // reference-patch scoring (esikf_vio_score_ref_patches): the inputs by element type, the answers in one block
+  // [score m | mean m | ref n] on the device, and its pinned host copy (grow-only)
+  DevBuf<double> rp_d;
+  DevBuf<float> rp_f;
+  DevBuf<int32_t> rp_i;
+  DevBuf<uint8_t> rp_out;
+  uint8_t *rp_host = nullptr;
+  size_t rp_host_cap = 0;
+
   // multi-GPU
   int rank = 0, nranks = 1;
   ncclComm_t comm = nullptr;
@@ -326,6 +336,7 @@ struct esikf_ctx {
     if (stage) cudaFreeHost(stage);
     if (stage_ctrl) cudaFreeHost(stage_ctrl);
     if (find_host) cudaFreeHost(find_host);
+    if (rp_host) cudaFreeHost(rp_host);
     for (cudaEvent_t e : stage_ev)
       if (e) cudaEventDestroy(e);
     for (cudaEvent_t e : ev) cudaEventDestroy(e);
@@ -2101,6 +2112,57 @@ int esikf_vio_depth_check(esikf_ctx *ctx, int32_t n, const double *pos_w, const 
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(discontinuous_out, ctx->ret_flag.p, N, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
+  return ESIKF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------- reference patches
+int esikf_vio_score_ref_patches(esikf_ctx *ctx, int32_t n, const int32_t *first, int32_t m, const double *pos, const double *normal, const float *patch,
+                                const float *mean, const int32_t *id, const double *T_f_w, float *score_out, float *mean_out, int32_t *ref_out) {
+  if (!ctx || n < 0 || m < 0 || (n > 0 && (!first || !pos || !normal || !ref_out)) || (m > 0 && (!patch || !mean || !id || !T_f_w || !score_out || !mean_out)))
+    return fail(ctx, ESIKF_ERR_ARG, "vio_score_ref_patches: bad argument");
+  if (n == 0) return ESIKF_OK;
+  if (first[0] != 0 || first[n] != m) return fail(ctx, ESIKF_ERR_ARG, "vio_score_ref_patches: first[0] = %d, first[n] = %d for %d observations", first[0], first[n], m);
+  for (int32_t i = 0; i < n; i++)
+    if (first[i + 1] < first[i]) return fail(ctx, ESIKF_ERR_ARG, "vio_score_ref_patches: first[%d] > first[%d]", i, i + 1);
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t N = (size_t)n, M = (size_t)m;
+  const size_t out_b = 8 * M + 4 * N;  // score m | mean m | ref n
+  CK(ctx->rp_d.reserve(6 * N + 12 * M + 1));  // pos 3n | normal 3n | T_f_w 12m
+  CK(ctx->rp_f.reserve(65 * M + 1));          // patch 64m | mean m
+  CK(ctx->rp_i.reserve(N + 1 + M));           // first n + 1 | id m
+  CK(ctx->rp_out.reserve(out_b));
+  if (out_b > ctx->rp_host_cap) {
+    if (ctx->rp_host) cudaFreeHost(ctx->rp_host);
+    ctx->rp_host = nullptr, ctx->rp_host_cap = 0;
+    CK(cudaMallocHost((void **)&ctx->rp_host, out_b + out_b / 4));
+    ctx->rp_host_cap = out_b + out_b / 4;
+  }
+  double *d = ctx->rp_d.p;
+  float *f = ctx->rp_f.p;
+  int32_t *k = ctx->rp_i.p;
+  CK(cudaMemcpyAsync(d, pos, 3 * N * sizeof(double), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d + 3 * N, normal, 3 * N * sizeof(double), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(k, first, (N + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  if (m > 0) {
+    CK(cudaMemcpyAsync(d + 6 * N, T_f_w, 12 * M * sizeof(double), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(f, patch, 64 * M * sizeof(float), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(f + 64 * M, mean, M * sizeof(float), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(k + N + 1, id, M * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  }
+  uint8_t *o = ctx->rp_out.p;
+  RefPatchArgs a;
+  a.first = k, a.pos = d, a.normal = d + 3 * N, a.T = d + 6 * N, a.patch = f, a.mean = f + 64 * M, a.id = k + N + 1, a.n = n;
+  a.score = (float *)o, a.mean_out = (float *)(o + 4 * M), a.ref = (int32_t *)(o + 8 * M);
+  refpatch_score_kernel<<<(n + RP_WARPS - 1) / RP_WARPS, RP_WARPS * 32, 0, st>>>(a);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  // one copy into pinned staging and one synchronisation; the caller's buffers are written only once everything succeeded
+  CK(cudaMemcpyAsync(ctx->rp_host, o, out_b, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  memcpy(score_out, ctx->rp_host, 4 * M);
+  memcpy(mean_out, ctx->rp_host + 4 * M, 4 * M);
+  memcpy(ref_out, ctx->rp_host + 8 * M, 4 * N);
   return ESIKF_OK;
 }
 

@@ -53,6 +53,16 @@ __device__ __forceinline__ bool patch_voxel_key(double c, long long &k) {
   k = (long long)loc;
   return true;
 }
+// ---- the cosine between a point's viewing ray and its normal in a camera frame (generateVisualMapPoints :867-870,
+// updateReferencePatch :1046-1049): norm_vec = T_f_w_.rotation_matrix() * normal (R row-major); pf = T_f_w_ * pos, already in
+// the camera frame; pf.normalize(); pf.dot(norm_vec). Each sum starts from 0 and runs left to right, as in the stand-in Eigen.
+// T is the single-rounded double Rn of esikf_vio.cu.
+template <class T> __device__ __forceinline__ T view_cos(const double *R, const T pf[3], const double *normal) {
+  T nv[3];
+  for (int r = 0; r < 3; r++) nv[r] = T(0.0) + T(R[3 * r]) * T(normal[0]) + T(R[3 * r + 1]) * T(normal[1]) + T(R[3 * r + 2]) * T(normal[2]);
+  const T len = sqrt(T(0.0) + pf[0] * pf[0] + pf[1] * pf[1] + pf[2] * pf[2]);
+  return T(0.0) + (pf[0] / len) * nv[0] + (pf[1] / len) * nv[1] + (pf[2] / len) * nv[2];
+}
 #endif
 __host__ __device__ inline uint32_t hash_key(unsigned long long k) {
   k ^= k >> 33;

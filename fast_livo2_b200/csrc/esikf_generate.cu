@@ -126,11 +126,7 @@ __global__ void __launch_bounds__(GEN_THREADS) gen_scatter_kernel(const GenArgs 
   Rn pf[3], u, v;
   int cell;
   gen_cell(a, Rcw, Pcw, pw, pf, u, v, cell);  // the winner passed it: pf, pc as when it was scored
-  // norm_vec = T_f_w_.rotation_matrix() * normal; dir = (T_f_w_ * pt).normalized(); cos_theta = dir.dot(norm_vec)
-  Rn nv[3];
-  for (int r = 0; r < 3; r++) nv[r] = Rn(0.0) + Rn(Rcw[3 * r]) * Rn(nw[0]) + Rn(Rcw[3 * r + 1]) * Rn(nw[1]) + Rn(Rcw[3 * r + 2]) * Rn(nw[2]);
-  const Rn len = sqrt(Rn(0.0) + pf[0] * pf[0] + pf[1] * pf[1] + pf[2] * pf[2]);
-  const Rn cos_theta = Rn(0.0) + (pf[0] / len) * nv[0] + (pf[1] / len) * nv[1] + (pf[2] / len) * nv[2];
+  const Rn cos_theta = view_cos(Rcw, pf, nw);
   const bool flip = cos_theta.v < 0.0;
   o.source[p] = s < a.n ? s : (ESIKF_GEN_ADD_FROM | (s - a.n));
   o.cell[p] = c;

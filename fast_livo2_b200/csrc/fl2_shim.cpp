@@ -697,6 +697,40 @@ void VIOManager::CheckDepthContinuity(int n, const double *pos, const double *pc
   memcpy(discontinuous.data(), fb, (size_t)n);
 }
 
+void VIOManager::ScoreReferencePatches(const std::vector<int32_t> &first, const std::vector<ScoredPoint> &pts, const std::vector<PatchObservation> &obs,
+                                       std::vector<float> &score, std::vector<float> &mean, std::vector<int32_t> &ref) {
+  if (!ctx_) {
+    last_status_ = ESIKF_ERR_STATE, last_error_ = "ScoreReferencePatches: no device context";
+    return;
+  }
+  if (first.size() != pts.size() + 1) {
+    last_status_ = ESIKF_ERR_ARG, last_error_ = "ScoreReferencePatches: first must have pts.size() + 1 entries";
+    return;
+  }
+  const size_t n = pts.size(), m = obs.size();
+  double *d = st_rp_d_.get(6 * n + 12 * m + 1);  // pos 3n | normal 3n | T_f_w 12m
+  float *f = st_rp_f_.get(65 * m + 1);           // patch 64m | mean m
+  int32_t *k = st_rp_i_.get(n + 1 + m);          // first n + 1 | id m
+  if (!d || !f || !k) {
+    last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
+    return;
+  }
+  memcpy(k, first.data(), (n + 1) * sizeof(int32_t));
+  for (size_t i = 0; i < n; i++) memcpy(d + 3 * i, pts[i].pos, sizeof(pts[i].pos)), memcpy(d + 3 * n + 3 * i, pts[i].normal, sizeof(pts[i].normal));
+  for (size_t j = 0; j < m; j++) {
+    memcpy(d + 6 * n + 12 * j, obs[j].T_f_w, sizeof(obs[j].T_f_w)), memcpy(f + 64 * j, obs[j].patch, sizeof(obs[j].patch));
+    f[64 * m + j] = obs[j].mean, k[n + 1 + j] = obs[j].id;
+  }
+  std::vector<float> sc(m), mu(m);
+  std::vector<int32_t> rf(n);
+  last_status_ = esikf_vio_score_ref_patches(ctx_, (int32_t)n, k, (int32_t)m, d, d + 3 * n, f, f + 64 * m, k + n + 1, d + 6 * n, sc.data(), mu.data(), rf.data());
+  if (last_status_) {
+    last_error_ = esikf_last_error(ctx_);
+    return;
+  }
+  score.swap(sc), mean.swap(mu), ref.swap(rf);
+}
+
 void VIOManager::initializeVIO() {
   if (!ctx_) return;
   esikf_extrinsics ext;
@@ -1557,6 +1591,36 @@ int fl2_shim_session_find_correspond(void *h, const double *pts, int n, int rule
     r.d = planes[i].d_, r.radius = planes[i].radius_;
   }
   return 0;
+}
+// GPU: VIOManager::ScoreReferencePatches on its own context, with the arrays of esikf_vio_score_ref_patches packed into the
+// shim's records. Returns 0 or the failing esikf_status (the outputs untouched).
+int fl2_shim_score_ref_patches(int n, const int32_t *first, int m, const double *pos, const double *normal, const float *patch, const float *mean,
+                               const int32_t *id, const double *T_f_w, float *score_out, float *mean_out, int32_t *ref_out) {
+  if (n < 0 || m < 0 || !first) return ESIKF_ERR_ARG;
+  esikf_ctx *ctx = nullptr;
+  int rc = esikf_create(&ctx, 0);
+  if (rc) return rc;
+  {
+    VIOManager vio(ctx);
+    std::vector<int32_t> fi(first, first + n + 1);
+    std::vector<ScoredPoint> pts(n);
+    for (int i = 0; i < n; i++) memcpy(pts[i].pos, pos + 3 * i, sizeof(pts[i].pos)), memcpy(pts[i].normal, normal + 3 * i, sizeof(pts[i].normal));
+    std::vector<PatchObservation> obs(m);
+    for (int j = 0; j < m; j++) {
+      memcpy(obs[j].T_f_w, T_f_w + 12 * (size_t)j, sizeof(obs[j].T_f_w)), memcpy(obs[j].patch, patch + 64 * (size_t)j, sizeof(obs[j].patch));
+      obs[j].mean = mean[j], obs[j].id = id[j];
+    }
+    std::vector<float> sc, mu;
+    std::vector<int32_t> rf;
+    vio.ScoreReferencePatches(fi, pts, obs, sc, mu, rf);
+    rc = vio.last_status_;
+    if (!rc) {
+      memcpy(score_out, sc.data(), sc.size() * sizeof(float)), memcpy(mean_out, mu.data(), mu.size() * sizeof(float));
+      memcpy(ref_out, rf.data(), rf.size() * sizeof(int32_t));
+    }
+  }
+  esikf_destroy(ctx);
+  return rc;
 }
 void *fl2_shim_session_context(void *h) { return static_cast<ShimSession *>(h)->mgr->context(); }
 

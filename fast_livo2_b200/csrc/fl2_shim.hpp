@@ -305,6 +305,19 @@ struct NewObservation {
   float patch[64];   // getImagePatch(img, pc, patch, 0): Feature::patch_
 };
 
+// One observation (Feature) of a visual point as updateReferencePatch scores it: VIOManager::ScoreReferencePatches' input.
+struct PatchObservation {
+  double T_f_w[12];  // Feature::T_f_w_: R row-major, then t
+  float patch[64];   // Feature::patch_
+  float mean;        // Feature::mean_
+  int32_t id;        // Feature::id_
+};
+// One visual point whose patches updateReferencePatch scores: pos_ and the normal_ the plane half left.
+struct ScoredPoint {
+  double pos[3];
+  double normal[3];
+};
+
 class VIOManager {
  public:
   StatesGroup *state = nullptr, *state_propagat = nullptr;  // raw pointers into LIVMapper (LIVMapper.cpp:135-136)
@@ -383,6 +396,12 @@ class VIOManager {
   // The depth-continuity check of :614-640 for n retrieved points (pos: VisualPoint::pos_, pc: the w2c(pos_) the map-side walk
   // computed, 3 and 2 doubles each) against the depth image of the last RetrieveScanVoxels: discontinuous[i] = depth_continous.
   void CheckDepthContinuity(int n, const double *pos, const double *pc, std::vector<uint8_t> &discontinuous);
+  // The patch scoring of updateReferencePatch (src/vio.cpp:1036-1097) on the device (esikf_vio_score_ref_patches), after the
+  // plane half: point i of pts owns obs[first[i] .. first[i + 1]), in obs_ order. Fills score (Feature::score_) and mean
+  // (Feature::mean_ afterwards) per observation, and ref per point: the position of the new ref_patch within its list, or -1
+  // when ref_patch and has_ref_patch_ stay as they were. first has pts.size() + 1 entries, first[0] = 0 and the last obs.size().
+  void ScoreReferencePatches(const std::vector<int32_t> &first, const std::vector<ScoredPoint> &pts, const std::vector<PatchObservation> &obs,
+                             std::vector<float> &score, std::vector<float> &mean, std::vector<int32_t> &ref);
 
  private:
   const uint8_t *patch_img_ = nullptr, *patch_ref_img_ = nullptr;  // what the per-patch helpers uploaded last
@@ -412,6 +431,9 @@ class VIOManager {
   PinnedBuf<int32_t> st_ret_keys_;
   PinnedBuf<uint8_t> st_ret_flag_;
   int32_t keys_cap_ = 0;  // the resident scan's largest key count seen
+  PinnedBuf<double> st_rp_d_;  // ScoreReferencePatches' inputs by element type: pos | normal | T_f_w, patch | mean, first | id
+  PinnedBuf<float> st_rp_f_;
+  PinnedBuf<int32_t> st_rp_i_;
   bool ref_imgs_current_ = false;    // false once the per-patch warpAffine replaced the device's reference images
 };
 

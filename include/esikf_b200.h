@@ -470,6 +470,34 @@ int esikf_vio_retrieve_scan(esikf_ctx *ctx, const double *point_w, int32_t n, in
                             int32_t *keys_out, float *depth_out);
 int esikf_vio_depth_check(esikf_ctx *ctx, int32_t n, const double *pos_w, const double *pc, uint8_t *discontinuous_out);
 
+/* ---------------------------------------------------------------- reference patches (updateReferencePatch)
+ * The patch scoring of VIOManager::updateReferencePatch (src/vio.cpp:1036-1097) on the device, for the n visual points that
+ * pass the four skips of :977-980, after the plane half (:981-1034, the caller's, on esikf_map_device_find's answers) has left
+ * their normal_. Point i owns the observations first[i] .. first[i + 1] - 1, in obs_ order (the newest first, as addFrameRef
+ * pushes them); first has n + 1 entries, first[0] = 0 and first[n] = m. Per point (host, 3 doubles each): pos (pos_) and
+ * normal (normal_). Per observation: patch (patch_, 64 floats), mean (mean_), id (id_) and T_f_w (T_f_w_: R row-major, then
+ * t; 12 doubles).
+ * For each observation r of a point, in list order:
+ *   cos_angle = pf.dot(R normal_) with pf = T_f_w_ * pos_ normalised, in double;
+ *   the mean of an observation is its mean_, or when abs(mean_) < 1e-6 the double sum of its 64 taps narrowed to float and
+ *   divided by 64 in float (mean_out: what the reference leaves in mean_);
+ *   over every other observation j with id_ != r's id_, in list order, the float sums up += (a - mean_r)(b - mean_j),
+ *   d1 += (a - mean_r)^2 and d2 += (b - mean_j)^2 over the 64 taps in order, running across all j (they are not reset per j),
+ *   and after each j, ncc += fabs(up / sqrt(d1 * d2)) in float; ncc / count (NaN when no observation has another id_);
+ *   score_out[r] = ncc + cos_angle in double, narrowed to float (the reference's score_).
+ * ref_out[i] = the position within the point's list of the first observation whose score beats the running maximum, which
+ * starts at -1000 (strict >: a tie keeps the earlier one, NaN never wins), or -1 when none does; the caller then sets
+ * ref_patch to it and has_ref_patch_ = true, and leaves both as they were for -1.
+ * The reference declares ref_mean and other_mean (:1054, :1067) without a value and assigns them only when mean_ is below
+ * 1e-6, so a cached mean_ is read as an uninitialised float. Here both are the observation's mean as defined above: the cached
+ * mean_ the code means to use. On inputs where every mean is recomputed at each read the results are the reference's.
+ * One host-to-device copy per input array, one kernel, one copy of the answers into pinned staging; the caller's outputs are
+ * written only after both copies succeeded. ESIKF_ERR_ARG for n < 0, m < 0, a NULL buffer that is needed, first[0] != 0,
+ * first[n] != m or decreasing offsets: a failed call writes nothing. n = 0 succeeds and does nothing. Every observation count
+ * is accepted, 1 included. With several ranks every rank evaluates all points. */
+int esikf_vio_score_ref_patches(esikf_ctx *ctx, int32_t n, const int32_t *first, int32_t m, const double *pos, const double *normal, const float *patch,
+                                const float *mean, const int32_t *id, const double *T_f_w, float *score_out, float *mean_out, int32_t *ref_out);
+
 /* ---------------------------------------------------------------- multi-GPU (one process per GPU)
  * The residual point / patch set is sharded by contiguous blocks; each iteration all-reduces the
  * packed information buffer [HTH upper | HTz | M | sum|d| ...] and every rank solves redundantly.
