@@ -95,6 +95,26 @@ template <typename T> struct DevBuf {
   }
 };
 
+// Pinned host bytes owned by their holder: freed on destruction, grown like DevBuf (n + n / 4); growing discards the contents.
+struct PinnedBlock {
+  uint8_t *p = nullptr;
+  size_t cap = 0;
+  PinnedBlock() = default;
+  PinnedBlock(const PinnedBlock &) = delete;
+  PinnedBlock &operator=(const PinnedBlock &) = delete;
+  ~PinnedBlock() {
+    if (p) cudaFreeHost(p);
+  }
+  cudaError_t reserve(size_t n) {
+    if (n <= cap) return cudaSuccess;
+    if (p) cudaFreeHost(p);
+    p = nullptr, cap = 0;
+    const cudaError_t e = cudaMallocHost((void **)&p, n + n / 4);
+    if (e == cudaSuccess) cap = n + n / 4;
+    return e;
+  }
+};
+
 // The buffers of one device-map arena (MapArena, esikf_map.cuh) and the capacities they were reserved for. The slots,
 // planes and recs buffers of the live arena also hold a host-uploaded map (esikf_map_upload).
 struct MapArenaBufs {
@@ -177,7 +197,6 @@ struct esikf_ctx {
   // points of the pv list (pv_list_ after LIVMapper.cpp:413-424) the last esikf_map_device_update left in map_pt (point_w | var)
   // and map_pt_normal (pv.normal), which esikf_vio_generate_points(point_w = NULL) reads; -1 when map_pt holds anything else
   int pv_n = -1;
-  DevBuf<double> fetch_normal;  // esikf_lio_fetch_normals gathering for a later LIO run: map_pt_normal keeps the pv list's normals
   int map_hash_bits = 0;
   esikf_map_stats map_last{};
   // esikf_map_device_export: points of the last applied tick (its touched list is map_touched, its sorted positions 0..n),
@@ -235,76 +254,32 @@ struct esikf_ctx {
   DevBuf<double> inv_ref_px, inv_ref_f, inv_ref_R, inv_ref_pos, H_sub_inv;  // inverse-compositional variant
   DevBuf<int32_t> inv_ref_idx;
   int n_inv_refs = 0;
-  DevBuf<float> warp_out;        // esikf_vio_warp_affine scratch (does not disturb the installed patches)
-  DevBuf<int32_t> warp_levels;
   int n_patches = 0;
   bool have_submap = false;  // a sub-map was installed (set_patches, warp_patches(keep_on_device), select_patches)
-  // warp producers
+  // reference images of the warp producers
   std::vector<DevBuf<uint8_t>> ref_imgs;
   DevBuf<const uint8_t *> ref_img_ptrs;
   int ref_w = 0, ref_h = 0;
-  DevBuf<int32_t> ref_idx;
-  DevBuf<double> px_ref, pos_w, normal_w, T_ref, T_cur, A_cur_ref, pc_buf;
-  DevBuf<float> patch_buf;
-  // esikf_vio_select_patches scratch (the installed sub-map is only written by its final scatter)
-  DevBuf<double> sel_d, sel_A;
-  DevBuf<int32_t> sel_i;
-  DevBuf<float> sel_warp, sel_err;
-  std::vector<double> sel_stage_d;
-  std::vector<int32_t> sel_stage_i;
   // which update's posterior `state` holds: the LIO tick's world cloud (esikf_rgb_set_cloud) and the VIO tick's frame pose
   // (esikf_rgb_colorize) default to the one their tick left there
   enum { RESIDENT_NONE, RESIDENT_LIO, RESIDENT_VIO } resident = RESIDENT_NONE;
 
-  // coloured scan (esikf_rgb_*): the world cloud of the last esikf_rgb_set_cloud, the BGR image and the per-point scratch
-  DevBuf<float> rgb_cloud, rgb_xyz;
-  DevBuf<uint8_t> rgb_img, rgb_color, rgb_bgr, rgb_scan_tmp;
-  DevBuf<int32_t> rgb_keep, rgb_dst, rgb_index;
+  // coloured scan (esikf_rgb_*): the world cloud of the last esikf_rgb_set_cloud
+  DevBuf<float> rgb_cloud;
   int rgb_n = -1;  // points of the cloud, -1 before esikf_rgb_set_cloud
 
-  // new visual map points (esikf_vio_generate_points): a host scan / add_from list, the TYPE_MAP mask, the per-cell winner keys
-  // and the winners' records
-  DevBuf<double> gen_pt, gen_normal, gen_add, gen_out_d;
-  DevBuf<uint8_t> gen_mask;
-  DevBuf<unsigned long long> gen_key;
-  DevBuf<int32_t> gen_i;
-  DevBuf<float> gen_out_f;
-
-  // new observations of the sub-map (esikf_vio_update_points): the caller's per-entry inputs, the flags, every entry's pc, the
-  // scan offsets and the added entries' records
-  DevBuf<double> obs_in, obs_pc, obs_out_pc;
-  DevBuf<uint8_t> obs_flag;
-  DevBuf<int32_t> obs_i;
-  DevBuf<float> obs_patch;
-
-  // scan side of the retrieval (esikf_vio_retrieve_scan / esikf_vio_depth_check): a host scan, the per-point keys, scan
-  // indices and depths, the pixel writers, the sort / scan scratch, the depth image and the frame pose it was made with
-  DevBuf<double> ret_pt, ret_state, ret_cand;
-  DevBuf<unsigned long long> ret_key;  // key_in n | key_out n
-  DevBuf<uint32_t> ret_idx;            // idx_in n | idx_out n
-  DevBuf<int32_t> ret_i;               // head n + 1 | dst n + 1 | keys 3n | bad 1
-  DevBuf<int32_t> ret_win;
-  DevBuf<float> ret_depth_pt, ret_depth;
-  DevBuf<uint8_t> ret_tmp, ret_flag;
+  // scan side of the retrieval: the depth image of the last esikf_vio_retrieve_scan and the frame pose it was made with, which
+  // esikf_vio_depth_check reads
+  DevBuf<double> ret_state;
+  DevBuf<float> ret_depth;
   double ret_Rci[9] = {}, ret_Pci[3] = {};
   int ret_w = 0, ret_h = 0;
   bool ret_valid = false;  // a depth image and its pose are in place (cleared by esikf_vio_set_camera and by a failed call)
 
-  // find_correspond lookups on the device map (esikf_map_device_find): the points, the answers in one block
-  // [rows n x 256 B | keys n x 24 B | status n B] on the device, and its pinned host copy (grow-only)
-  DevBuf<double> find_pt;
-  DevBuf<uint8_t> find_out;
-  uint8_t *find_host = nullptr;
-  size_t find_host_cap = 0;
-
-  // reference-patch scoring (esikf_vio_score_ref_patches): the inputs by element type, the answers in one block
-  // [score m | mean m | ref n] on the device, and its pinned host copy (grow-only)
-  DevBuf<double> rp_d;
-  DevBuf<float> rp_f;
-  DevBuf<int32_t> rp_i;
-  DevBuf<uint8_t> rp_out;
-  uint8_t *rp_host = nullptr;
-  size_t rp_host_cap = 0;
+  // What the front-end entry points need for the length of one call only (lay_out_scratch). Every such call runs on `stream`
+  // and synchronises it before it returns, so they can share it; nothing a later call reads may be kept here.
+  DevBuf<uint8_t> scratch;
+  PinnedBlock host;  // the same in pinned host memory: select_patches' input staging, find's and score_ref_patches' readback
 
   // multi-GPU
   int rank = 0, nranks = 1;
@@ -335,8 +310,6 @@ struct esikf_ctx {
     if (mailbox) cudaFree(mailbox);
     if (stage) cudaFreeHost(stage);
     if (stage_ctrl) cudaFreeHost(stage_ctrl);
-    if (find_host) cudaFreeHost(find_host);
-    if (rp_host) cudaFreeHost(rp_host);
     for (cudaEvent_t e : stage_ev)
       if (e) cudaEventDestroy(e);
     for (cudaEvent_t e : ev) cudaEventDestroy(e);
@@ -358,6 +331,38 @@ static int fail(esikf_ctx *c, int code, const char *fmt, ...) {
     cudaError_t e__ = (call);                                                                                      \
     if (e__ != cudaSuccess) return fail(ctx, ESIKF_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e__), __FILE__, __LINE__); \
   } while (0)
+
+// One call's scratch block: `lay` takes each sub-array of the call from a ScratchLayout, 256-byte aligned. It runs once with
+// base 0 to size the block and, after the one reserve (which discards the old contents), again to hand out the pointers.
+struct ScratchLayout {
+  uintptr_t base = 0;
+  size_t bytes = 0;
+  template <typename T> T *take(size_t n) {
+    T *p = reinterpret_cast<T *>(base + bytes);
+    bytes += (n * sizeof(T) + 255) & ~(size_t)255;
+    return p;
+  }
+};
+template <typename F> static cudaError_t lay_out_scratch(esikf_ctx *ctx, F &&lay) {
+  ScratchLayout s;
+  lay(s);
+  if (const cudaError_t e = ctx->scratch.reserve(s.bytes)) return e;
+  s = ScratchLayout{(uintptr_t)ctx->scratch.p};
+  lay(s);
+  return cudaSuccess;
+}
+
+// The one readback of answers that lie in scratch between `first` and `end`: a copy into the pinned block and a synchronisation.
+// copy_out then hands them to the caller, whose buffers a failed call thus leaves untouched.
+static cudaError_t read_back(esikf_ctx *ctx, const void *first, const void *end) {
+  const size_t bytes = (const uint8_t *)end - (const uint8_t *)first;
+  cudaError_t e = ctx->host.reserve(bytes);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->host.p, first, bytes, cudaMemcpyDeviceToHost, ctx->stream);
+  return e == cudaSuccess ? cudaStreamSynchronize(ctx->stream) : e;
+}
+static void copy_out(const esikf_ctx *ctx, void *dst, const void *first, const void *src, size_t bytes) {
+  memcpy(dst, ctx->host.p + ((const uint8_t *)src - (const uint8_t *)first), bytes);
+}
 
 static cudaEvent_t *timing_events(esikf_ctx *ctx, int base, int slot) {
   size_t need = (size_t)(base + slot + 1) * 3;
@@ -996,29 +1001,23 @@ int esikf_map_device_find(esikf_ctx *ctx, const double *points, int32_t n, int32
   if (n == 0) return ESIKF_OK;
   CK(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
-  const size_t rows_b = (size_t)n * sizeof(esikf_plane), keys_b = (size_t)n * 3 * sizeof(int64_t), bytes = rows_b + keys_b + (size_t)n;
-  CK(ctx->find_pt.reserve((size_t)n * 3));
-  CK(ctx->find_out.reserve(bytes));
-  if (bytes > ctx->find_host_cap) {
-    if (ctx->find_host) cudaFreeHost(ctx->find_host);
-    ctx->find_host = nullptr, ctx->find_host_cap = 0;
-    CK(cudaMallocHost((void **)&ctx->find_host, bytes + bytes / 4));
-    ctx->find_host_cap = bytes + bytes / 4;
-  }
-  CK(cudaMemcpyAsync(ctx->find_pt.p, points, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
-  uint8_t *d = ctx->find_out.p;
+  const size_t N = (size_t)n;
   MapFindArgs a;
-  a.pts = ctx->find_pt.p, a.n = n, a.rule = rule;
-  a.rows = (esikf_plane *)d, a.keys = (long long *)(d + rows_b), a.status = d + rows_b + keys_b;
+  a.n = n, a.rule = rule;
+  double *pt;
+  auto lay = [&](ScratchLayout &s) {
+    a.pts = pt = s.take<double>(3 * N);
+    a.rows = s.take<esikf_plane>(N), a.keys = s.take<long long>(3 * N), a.status = s.take<uint8_t>(N);  // read back as one span
+  };
+  CK(lay_out_scratch(ctx, lay));
+  CK(cudaMemcpyAsync(pt, points, 3 * N * sizeof(double), cudaMemcpyHostToDevice, st));
   map_find_kernel<<<(n + FIND_THREADS - 1) / FIND_THREADS, FIND_THREADS, 0, st>>>(ctx->arena(), a);
   ctx->launches++;
   CK(cudaGetLastError());
-  // one copy into pinned staging and one synchronisation; the caller's buffers are written only once everything succeeded
-  CK(cudaMemcpyAsync(ctx->find_host, d, bytes, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  memcpy(rows, ctx->find_host, rows_b);
-  memcpy(keys, ctx->find_host + rows_b, keys_b);
-  memcpy(status, ctx->find_host + rows_b + keys_b, (size_t)n);
+  CK(read_back(ctx, a.rows, a.status + N));
+  copy_out(ctx, rows, a.rows, a.rows, N * sizeof(esikf_plane));
+  copy_out(ctx, keys, a.rows, a.keys, 3 * N * sizeof(int64_t));
+  copy_out(ctx, status, a.rows, a.status, N);
   return ESIKF_OK;
 }
 
@@ -1039,10 +1038,12 @@ int esikf_lio_fetch_normals(esikf_ctx *ctx, double *normals) {
   if (n == 0) return ESIKF_OK;
   const double *src = ctx->map_pt_normal.p;
   if (!(ctx->dev_map && ctx->map_normals_valid && ctx->map_pt_n == n)) {
-    CK(ctx->fetch_normal.reserve((size_t)n * 3 + 4));
-    gather_normals_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(ctx->normal_plane.p, ctx->map.recs.p, n, ctx->fetch_normal.p);
+    double *normal;  // not map_pt_normal: it keeps the pv list's normals for a later generate_points
+    auto lay = [&](ScratchLayout &s) { normal = s.take<double>((size_t)n * 3 + 4); };
+    CK(lay_out_scratch(ctx, lay));
+    gather_normals_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(ctx->normal_plane.p, ctx->map.recs.p, n, normal);
     ctx->launches++;
-    src = ctx->fetch_normal.p;
+    src = normal;
   }
   CK(cudaMemcpyAsync(normals, src, (size_t)n * 3 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
@@ -1355,6 +1356,12 @@ static void cam_dev(const esikf_ctx *ctx, CamDev &c) {
   c.fx = ctx->cam.fx, c.fy = ctx->cam.fy, c.cx = ctx->cam.cx, c.cy = ctx->cam.cy;
   for (int i = 0; i < 5; i++) c.d[i] = ctx->cam.d[i];
 }
+// The camera and the camera-from-IMU extrinsics the front-end kernels project with.
+static void frame_consts(const esikf_ctx *ctx, CamDev &cam, double Rci[9], double Pci[3]) {
+  cam_dev(ctx, cam);
+  double Jdp_dR[9];
+  vio_consts(ctx, Rci, Pci, Jdp_dR);
+}
 static void vio_fill_args(esikf_ctx *ctx, VioKernelArgs &ka, double *state_ptr) {
   memset(&ka, 0, sizeof(ka));
   ka.img = ctx->img.p;
@@ -1507,13 +1514,15 @@ int esikf_vio_get_image_patch(esikf_ctx *ctx, const double *pc, int32_t n, int32
   if (ctx->img_w == 0) return fail(ctx, ESIKF_ERR_STATE, "get_image_patch before vio_set_image");
   if (n == 0) return ESIKF_OK;
   CK(cudaSetDevice(ctx->device));
-  CK(ctx->pc_buf.reserve((size_t)n * 2));
-  CK(ctx->patch_buf.reserve((size_t)n * 64));
+  double *pc_d;
+  float *patch;
+  auto lay = [&](ScratchLayout &s) { pc_d = s.take<double>((size_t)n * 2), patch = s.take<float>((size_t)n * 64); };
+  CK(lay_out_scratch(ctx, lay));
   cudaStream_t st = ctx->stream;
-  CK(cudaMemcpyAsync(ctx->pc_buf.p, pc, (size_t)n * 2 * sizeof(double), cudaMemcpyHostToDevice, st));
-  image_patch_kernel<<<(n * 64 + 255) / 256, 256, 0, st>>>(ctx->img.p, ctx->img_w, ctx->img_h, ctx->pc_buf.p, n, level, ctx->patch_buf.p);
+  CK(cudaMemcpyAsync(pc_d, pc, (size_t)n * 2 * sizeof(double), cudaMemcpyHostToDevice, st));
+  image_patch_kernel<<<(n * 64 + 255) / 256, 256, 0, st>>>(ctx->img.p, ctx->img_w, ctx->img_h, pc_d, n, level, patch);
   ctx->launches++;
-  CK(cudaMemcpyAsync(patch_out, ctx->patch_buf.p, (size_t)n * 64 * sizeof(float), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(patch_out, patch, (size_t)n * 64 * sizeof(float), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   return ESIKF_OK;
 }
@@ -1553,30 +1562,30 @@ int esikf_vio_warp_patches(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_ind
   CK(cudaSetDevice(ctx->device));
   const int L = ctx->vio_cfg.patch_pyrimid_level;
   cudaStream_t st = ctx->stream;
-  CK(ctx->ref_idx.reserve(n));
-  CK(ctx->px_ref.reserve((size_t)n * 2));
-  CK(ctx->pos_w.reserve((size_t)n * 3));
-  CK(ctx->normal_w.reserve((size_t)n * 3));
-  CK(ctx->T_ref.reserve((size_t)n * 12));
-  CK(ctx->T_cur.reserve(12));
-  CK(ctx->A_cur_ref.reserve((size_t)n * 4));
+  const size_t N = (size_t)n;
+  int32_t *ref_idx;
+  double *px, *pos, *normal, *T_ref, *T_cur, *A;
+  auto lay = [&](ScratchLayout &s) {
+    ref_idx = s.take<int32_t>(N), px = s.take<double>(2 * N), pos = s.take<double>(3 * N), normal = s.take<double>(3 * N);
+    T_ref = s.take<double>(12 * N), T_cur = s.take<double>(12), A = s.take<double>(4 * N);
+  };
+  CK(lay_out_scratch(ctx, lay));
   CK(ctx->search_levels.reserve(n + 1));
-  CK(ctx->warp_patch.reserve((size_t)n * 64 * L + 64));
-  CK(cudaMemcpyAsync(ctx->ref_idx.p, ref_img_index, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->px_ref.p, px_ref, (size_t)n * 2 * sizeof(double), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->pos_w.p, pos_w, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->normal_w.p, normal_w, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->T_ref.p, T_ref_w, (size_t)n * 12 * sizeof(double), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->T_cur.p, T_cur_w, 12 * sizeof(double), cudaMemcpyHostToDevice, st));
+  CK(ctx->warp_patch.reserve(N * 64 * L + 64));
+  CK(cudaMemcpyAsync(ref_idx, ref_img_index, N * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(px, px_ref, N * 2 * sizeof(double), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(pos, pos_w, N * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(normal, normal_w, N * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(T_ref, T_ref_w, N * 12 * sizeof(double), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(T_cur, T_cur_w, 12 * sizeof(double), cudaMemcpyHostToDevice, st));
   CamDev cam;
   cam_dev(ctx, cam);
-  warp_matrix_kernel<<<(n + 127) / 128, 128, 0, st>>>(cam, n, ctx->px_ref.p, ctx->pos_w.p, ctx->normal_w.p, ctx->T_ref.p, ctx->T_cur.p, ctx->A_cur_ref.p,
-                                                     ctx->search_levels.p);
-  CK(cudaMemsetAsync(ctx->warp_patch.p, 0, (size_t)n * 64 * L * sizeof(float), st));
-  warp_affine_kernel<<<(n * L * 64 + 255) / 256, 256, 0, st>>>(ctx->ref_img_ptrs.p, ctx->ref_idx.p, ctx->ref_w, ctx->ref_h, n, L, ctx->A_cur_ref.p,
-                                                              ctx->px_ref.p, ctx->search_levels.p, ctx->warp_patch.p);
+  warp_matrix_kernel<<<(n + 127) / 128, 128, 0, st>>>(cam, n, px, pos, normal, T_ref, T_cur, A, ctx->search_levels.p);
+  CK(cudaMemsetAsync(ctx->warp_patch.p, 0, N * 64 * L * sizeof(float), st));
+  warp_affine_kernel<<<(n * L * 64 + 255) / 256, 256, 0, st>>>(ctx->ref_img_ptrs.p, ref_idx, ctx->ref_w, ctx->ref_h, n, L, A, px, ctx->search_levels.p,
+                                                              ctx->warp_patch.p);
   ctx->launches += 2;
-  if (A_cur_ref_out) CK(cudaMemcpyAsync(A_cur_ref_out, ctx->A_cur_ref.p, (size_t)n * 4 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (A_cur_ref_out) CK(cudaMemcpyAsync(A_cur_ref_out, A, N * 4 * sizeof(double), cudaMemcpyDeviceToHost, st));
   if (search_level_out) CK(cudaMemcpyAsync(search_level_out, ctx->search_levels.p, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   if (warp_patch_out) CK(cudaMemcpyAsync(warp_patch_out, ctx->warp_patch.p, (size_t)n * 64 * L * sizeof(float), cudaMemcpyDeviceToHost, st));
   if (keep_on_device) {
@@ -1584,7 +1593,7 @@ int esikf_vio_warp_patches(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_ind
     CK(ctx->vis_pos.reserve((size_t)n * 3 + 4));
     CK(ctx->inv_expo.reserve(n + 1));
     CK(ctx->errors.reserve(n + 1));
-    CK(cudaMemcpyAsync(ctx->vis_pos.p, ctx->pos_w.p, (size_t)n * 3 * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(ctx->vis_pos.p, pos, N * 3 * sizeof(double), cudaMemcpyDeviceToDevice, st));
     std::vector<double> ones(n, 1.0);
     CK(cudaMemcpyAsync(ctx->inv_expo.p, ones.data(), (size_t)n * sizeof(double), cudaMemcpyHostToDevice, st));
     CK(cudaStreamSynchronize(st));
@@ -1627,52 +1636,51 @@ int esikf_vio_select_patches(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_i
     ctx->have_submap = true;
     return ESIKF_OK;
   }
-  // one staging copy per element type; device layout (doubles): px 2n | ref_f 3n | ref_pos 3n | pos 3n | normal 3n | T_ref 12n |
-  // inv_expo n | pc 2n | T_cur 12, (ints) ref_idx n | ref_level n | ref_key n | search level n | keep n | dst n | n_kept 1 | kept n
   const size_t N = (size_t)n;
-  const size_t o_px = 0, o_f = 2 * N, o_rp = 5 * N, o_pos = 8 * N, o_nrm = 11 * N, o_T = 14 * N, o_ie = 26 * N, o_pc = 27 * N, o_Tc = 29 * N;
-  std::vector<double> &hd = ctx->sel_stage_d;
-  hd.assign(29 * N + 12, 0.0);
-  auto put = [&](size_t off, const double *src, size_t cnt) {
-    if (src) memcpy(hd.data() + off, src, cnt * sizeof(double));
+  double *d_px, *d_f, *d_rp, *d_pos, *d_nrm, *d_T, *d_ie, *d_pc, *d_Tc, *d_A, *d_Akept;
+  int32_t *d_idx, *d_lvl, *d_key, *d_sl, *d_keep, *d_dst, *d_nk, *d_kept;
+  float *d_warp, *d_err;
+  size_t in_bytes = 0;
+  auto lay = [&](ScratchLayout &s) {
+    // the inputs first: they are staged in the pinned block at the same offsets and uploaded with one copy
+    d_px = s.take<double>(2 * N), d_f = s.take<double>(3 * N), d_rp = s.take<double>(3 * N), d_pos = s.take<double>(3 * N), d_nrm = s.take<double>(3 * N);
+    d_T = s.take<double>(12 * N), d_ie = s.take<double>(N), d_pc = s.take<double>(2 * N), d_Tc = s.take<double>(12);
+    d_idx = s.take<int32_t>(N), d_lvl = s.take<int32_t>(N), d_key = s.take<int32_t>(N);
+    in_bytes = s.bytes;
+    d_sl = s.take<int32_t>(N), d_keep = s.take<int32_t>(N), d_dst = s.take<int32_t>(N), d_nk = s.take<int32_t>(1), d_kept = s.take<int32_t>(N);
+    d_A = s.take<double>(4 * N), d_Akept = s.take<double>(4 * N), d_warp = s.take<float>(N * 64 * L), d_err = s.take<float>(N);
   };
-  put(o_px, px_ref, 2 * N), put(o_f, ref_f, 3 * N), put(o_rp, ref_pos, 3 * N), put(o_pos, pos_w, 3 * N), put(o_nrm, normal_w, 3 * N);
-  put(o_T, T_ref_w, 12 * N), put(o_ie, ref_inv_expo, N), put(o_pc, pc, 2 * N), put(o_Tc, T_cur_w, 12);
-  std::vector<int32_t> &hi = ctx->sel_stage_i;
-  hi.assign(3 * N, 0);
-  memcpy(hi.data(), ref_img_index, N * sizeof(int32_t));
-  if (!homography) memcpy(hi.data() + N, ref_level, N * sizeof(int32_t)), memcpy(hi.data() + 2 * N, ref_key, N * sizeof(int32_t));
-  CK(ctx->sel_d.reserve(hd.size()));
-  CK(ctx->sel_i.reserve(7 * N + 1));
-  CK(ctx->sel_A.reserve(8 * N));
-  CK(ctx->sel_warp.reserve(N * 64 * L));
-  CK(ctx->sel_err.reserve(N));
-  CK(cudaMemcpyAsync(ctx->sel_d.p, hd.data(), hd.size() * sizeof(double), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->sel_i.p, hi.data(), hi.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  const double *d = ctx->sel_d.p;
-  int32_t *iv = ctx->sel_i.p;
-  int32_t *d_idx = iv, *d_lvl = iv + N, *d_key = iv + 2 * N, *d_sl = iv + 3 * N, *d_keep = iv + 4 * N, *d_dst = iv + 5 * N, *d_nk = iv + 6 * N,
-          *d_kept = iv + 6 * N + 1;
-  double *d_A = ctx->sel_A.p, *d_Akept = ctx->sel_A.p + 4 * N;
+  CK(lay_out_scratch(ctx, lay));
+  CK(ctx->host.reserve(in_bytes));
+  memset(ctx->host.p, 0, in_bytes);  // the inputs the chosen warp form does not read stay zero
+  auto put = [&](const void *dst, const void *src, size_t bytes) {
+    if (src) memcpy(ctx->host.p + ((const uint8_t *)dst - ctx->scratch.p), src, bytes);
+  };
+  put(d_px, px_ref, 2 * N * sizeof(double)), put(d_f, ref_f, 3 * N * sizeof(double)), put(d_rp, ref_pos, 3 * N * sizeof(double));
+  put(d_pos, pos_w, 3 * N * sizeof(double)), put(d_nrm, normal_w, 3 * N * sizeof(double)), put(d_T, T_ref_w, 12 * N * sizeof(double));
+  put(d_ie, ref_inv_expo, N * sizeof(double)), put(d_pc, pc, 2 * N * sizeof(double)), put(d_Tc, T_cur_w, 12 * sizeof(double));
+  put(d_idx, ref_img_index, N * sizeof(int32_t));
+  if (!homography) put(d_lvl, ref_level, N * sizeof(int32_t)), put(d_key, ref_key, N * sizeof(int32_t));
+  CK(cudaMemcpyAsync(ctx->scratch.p, ctx->host.p, in_bytes, cudaMemcpyHostToDevice, st));
   CamDev cam;
   cam_dev(ctx, cam);
   if (homography)
-    warp_matrix_kernel<<<(n + 127) / 128, 128, 0, st>>>(cam, n, d + o_px, d + o_pos, d + o_nrm, d + o_T, d + o_Tc, d_A, d_sl);
+    warp_matrix_kernel<<<(n + 127) / 128, 128, 0, st>>>(cam, n, d_px, d_pos, d_nrm, d_T, d_Tc, d_A, d_sl);
   else
-    warp_matrix_depth_kernel<<<(n + 127) / 128, 128, 0, st>>>(cam, n, d + o_px, d + o_f, d + o_rp, d + o_pos, d + o_T, d + o_Tc, d_lvl, d_key, d_A, d_sl);
+    warp_matrix_depth_kernel<<<(n + 127) / 128, 128, 0, st>>>(cam, n, d_px, d_f, d_rp, d_pos, d_T, d_Tc, d_lvl, d_key, d_A, d_sl);
   // patch_wrap is a fresh zero vector per candidate (:646): a NaN inverse leaves it zero (:297-301)
-  CK(cudaMemsetAsync(ctx->sel_warp.p, 0, N * 64 * L * sizeof(float), st));
-  warp_affine_kernel<<<(n * L * 64 + 255) / 256, 256, 0, st>>>(ctx->ref_img_ptrs.p, d_idx, ctx->ref_w, ctx->ref_h, n, L, d_A, d + o_px, d_sl, ctx->sel_warp.p);
+  CK(cudaMemsetAsync(d_warp, 0, N * 64 * L * sizeof(float), st));
+  warp_affine_kernel<<<(n * L * 64 + 255) / 256, 256, 0, st>>>(ctx->ref_img_ptrs.p, d_idx, ctx->ref_w, ctx->ref_h, n, L, d_A, d_px, d_sl, d_warp);
   SelectGateArgs ga;
   ga.img = ctx->img.p, ga.width = ctx->img_w, ga.height = ctx->img_h, ga.n = n, ga.levels = L, ga.ncc_en = cfg->ncc_en != 0;
-  ga.pc = d + o_pc, ga.warp = ctx->sel_warp.p, ga.ref_inv_expo = d + o_ie;
+  ga.pc = d_pc, ga.warp = d_warp, ga.ref_inv_expo = d_ie;
   ga.cur_inv_expo = inv_expo_time, ga.ncc_thre = cfg->ncc_thre, ga.outlier_threshold = cfg->outlier_threshold;
-  ga.error = ctx->sel_err.p, ga.keep = d_keep;
+  ga.error = d_err, ga.keep = d_keep;
   select_gate_kernel<<<(n + SELECT_GATE_WARPS - 1) / SELECT_GATE_WARPS, 32 * SELECT_GATE_WARPS, 0, st>>>(ga);
   select_scan_kernel<<<1, SELECT_SCAN_THREADS, 0, st>>>(d_keep, n, d_dst, d_nk);
   SelectScatterArgs sa;
-  sa.n = n, sa.levels = L, sa.keep = d_keep, sa.dst = d_dst, sa.search_level = d_sl, sa.pos_w = d + o_pos, sa.ref_inv_expo = d + o_ie, sa.A = d_A;
-  sa.warp = ctx->sel_warp.p, sa.error = ctx->sel_err.p;
+  sa.n = n, sa.levels = L, sa.keep = d_keep, sa.dst = d_dst, sa.search_level = d_sl, sa.pos_w = d_pos, sa.ref_inv_expo = d_ie, sa.A = d_A;
+  sa.warp = d_warp, sa.error = d_err;
   sa.vis_pos = ctx->vis_pos.p, sa.inv_expo = ctx->inv_expo.p, sa.A_kept = d_Akept, sa.warp_patch = ctx->warp_patch.p, sa.errors = ctx->errors.p;
   sa.search_levels = ctx->search_levels.p, sa.kept_index = d_kept;
   select_scatter_kernel<<<(n + 7) / 8, 256, 0, st>>>(sa);
@@ -1734,21 +1742,23 @@ int esikf_vio_warp_affine(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_inde
   CK(cudaSetDevice(ctx->device));
   const int L = ctx->vio_cfg.patch_pyrimid_level;
   cudaStream_t st = ctx->stream;
-  CK(ctx->ref_idx.reserve(n));
-  CK(ctx->px_ref.reserve((size_t)n * 2));
-  CK(ctx->A_cur_ref.reserve((size_t)n * 4));
-  CK(ctx->warp_levels.reserve(n + 1));
-  CK(ctx->warp_out.reserve((size_t)n * 64 * L + 64));
-  CK(cudaMemcpyAsync(ctx->ref_idx.p, ref_img_index, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->px_ref.p, px_ref, (size_t)n * 2 * sizeof(double), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->A_cur_ref.p, A_cur_ref, (size_t)n * 4 * sizeof(double), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->warp_levels.p, search_level, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  // separate scratch: the patches / search levels installed by set_patches (or warp_patches with keep_on_device) stay untouched
-  CK(cudaMemsetAsync(ctx->warp_out.p, 0, (size_t)n * 64 * L * sizeof(float), st));
-  warp_affine_kernel<<<(n * L * 64 + 255) / 256, 256, 0, st>>>(ctx->ref_img_ptrs.p, ctx->ref_idx.p, ctx->ref_w, ctx->ref_h, n, L, ctx->A_cur_ref.p,
-                                                              ctx->px_ref.p, ctx->warp_levels.p, ctx->warp_out.p);
+  const size_t N = (size_t)n;
+  // all in scratch: the patches / search levels installed by set_patches (or warp_patches with keep_on_device) stay untouched
+  int32_t *ref_idx, *levels;
+  double *px, *A;
+  float *out;
+  auto lay = [&](ScratchLayout &s) {
+    ref_idx = s.take<int32_t>(N), px = s.take<double>(2 * N), A = s.take<double>(4 * N), levels = s.take<int32_t>(N + 1), out = s.take<float>(N * 64 * L + 64);
+  };
+  CK(lay_out_scratch(ctx, lay));
+  CK(cudaMemcpyAsync(ref_idx, ref_img_index, N * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(px, px_ref, N * 2 * sizeof(double), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(A, A_cur_ref, N * 4 * sizeof(double), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(levels, search_level, N * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(out, 0, N * 64 * L * sizeof(float), st));
+  warp_affine_kernel<<<(n * L * 64 + 255) / 256, 256, 0, st>>>(ctx->ref_img_ptrs.p, ref_idx, ctx->ref_w, ctx->ref_h, n, L, A, px, levels, out);
   ctx->launches += 1;
-  CK(cudaMemcpyAsync(warp_patch_out, ctx->warp_out.p, (size_t)n * 64 * L * sizeof(float), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(warp_patch_out, out, N * 64 * L * sizeof(float), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   CK(cudaGetLastError());
   return ESIKF_OK;
@@ -1808,42 +1818,40 @@ int esikf_rgb_colorize(esikf_ctx *ctx, const uint8_t *bgr, int32_t width, int32_
   if (int rc = rgb_state(ctx, state, esikf_ctx::RESIDENT_VIO, "rgb_colorize", &dev_state)) return rc;
   const int n = ctx->rgb_n;
   cudaStream_t st = ctx->stream;
-  const size_t img_bytes = (size_t)width * height * 3;
-  CK(ctx->rgb_img.reserve(img_bytes));
-  CK(ctx->rgb_keep.reserve((size_t)n + 1));  // keep[n] = 0: the exclusive scan's last entry is the number kept
-  CK(ctx->rgb_dst.reserve((size_t)n + 1));
-  CK(ctx->rgb_color.reserve((size_t)n * 3 + 4));
-  CK(ctx->rgb_xyz.reserve((size_t)n * 3 + 4));
-  CK(ctx->rgb_bgr.reserve((size_t)n * 3 + 4));
-  CK(ctx->rgb_index.reserve((size_t)n + 1));
+  const size_t N = (size_t)n, img_bytes = (size_t)width * height * 3;
+  // device-wide scan: select_scan_kernel's single CTA took 90 % of the pass at 300 k points (DESIGN.md §8)
+  size_t tmp_bytes = 0;
+  if (n > 0) cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, (int32_t *)nullptr, (int32_t *)nullptr, n + 1, st);
+  uint8_t *img, *color, *bgr_kept, *tmp;
+  int32_t *keep, *dst, *index;
+  float *xyz;
+  auto lay = [&](ScratchLayout &s) {
+    img = s.take<uint8_t>(img_bytes), keep = s.take<int32_t>(N + 1), dst = s.take<int32_t>(N + 1);  // keep[n] = 0: dst[n] is the number kept
+    color = s.take<uint8_t>(N * 3 + 4), xyz = s.take<float>(N * 3 + 4), bgr_kept = s.take<uint8_t>(N * 3 + 4), index = s.take<int32_t>(N + 1);
+    tmp = s.take<uint8_t>(tmp_bytes);
+  };
+  CK(lay_out_scratch(ctx, lay));
   int32_t kept = 0;
   if (n > 0) {
-    CK(cudaMemcpyAsync(ctx->rgb_img.p, bgr, img_bytes, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(img, bgr, img_bytes, cudaMemcpyHostToDevice, st));
     RgbColorArgs a;
-    a.cloud = ctx->rgb_cloud.p, a.n = n, a.bgr = ctx->rgb_img.p, a.state = dev_state, a.blind = blind_rgb_points;
-    cam_dev(ctx, a.cam);
-    double Jdp_dR[9];
-    vio_consts(ctx, a.Rci, a.Pci, Jdp_dR);
-    a.keep = ctx->rgb_keep.p, a.color = ctx->rgb_color.p;
+    a.cloud = ctx->rgb_cloud.p, a.n = n, a.bgr = img, a.state = dev_state, a.blind = blind_rgb_points;
+    frame_consts(ctx, a.cam, a.Rci, a.Pci);
+    a.keep = keep, a.color = color;
     rgb_color_kernel<<<(n + 1 + 255) / 256, 256, 0, st>>>(a);
-    // device-wide scan: select_scan_kernel's single CTA took 90 % of the pass at 300 k points (DESIGN.md §8)
-    size_t tmp_bytes = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, ctx->rgb_keep.p, ctx->rgb_dst.p, n + 1, st);
-    CK(ctx->rgb_scan_tmp.reserve(tmp_bytes + 16));
-    CK(cub::DeviceScan::ExclusiveSum(ctx->rgb_scan_tmp.p, tmp_bytes, ctx->rgb_keep.p, ctx->rgb_dst.p, n + 1, st));
-    rgb_scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(ctx->rgb_keep.p, ctx->rgb_dst.p, n, ctx->rgb_cloud.p, ctx->rgb_color.p, ctx->rgb_xyz.p, ctx->rgb_bgr.p,
-                                                        ctx->rgb_index.p);
+    CK(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, keep, dst, n + 1, st));
+    rgb_scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(keep, dst, n, ctx->rgb_cloud.p, color, xyz, bgr_kept, index);
     ctx->launches += 4;
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(&kept, ctx->rgb_dst.p + n, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&kept, dst + n, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
   }
   *n_out = kept;
   if (kept > cap) return fail(ctx, ESIKF_ERR_ARG, "rgb_colorize: %d points kept, room for %d", kept, cap);
   if (kept > 0) {
-    CK(cudaMemcpyAsync(xyz_out, ctx->rgb_xyz.p, (size_t)kept * 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(bgr_out, ctx->rgb_bgr.p, (size_t)kept * 3, cudaMemcpyDeviceToHost, st));
-    if (index_out) CK(cudaMemcpyAsync(index_out, ctx->rgb_index.p, (size_t)kept * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(xyz_out, xyz, (size_t)kept * 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(bgr_out, bgr_kept, (size_t)kept * 3, cudaMemcpyDeviceToHost, st));
+    if (index_out) CK(cudaMemcpyAsync(index_out, index, (size_t)kept * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
   }
   return ESIKF_OK;
@@ -1876,44 +1884,42 @@ int esikf_vio_generate_points(esikf_ctx *ctx, const double *point_w, const doubl
   const size_t N = (size_t)n;
   GenArgs a;
   a.img = ctx->img.p;
-  cam_dev(ctx, a.cam);
-  double Jdp_dR[9];
-  vio_consts(ctx, a.Rci, a.Pci, Jdp_dR);
+  frame_consts(ctx, a.cam, a.Rci, a.Pci);
   a.state = dev_state, a.n = n, a.n_add = n_add, a.pt_stride = MAP_PT_D;
   a.grid_size = grid_size, a.grid_n_width = grid_n_width, a.length = L, a.border = border;
-  if (point_w) {  // pv_list_ from the host: point_w | var rows as map_pt holds them
-    CK(ctx->gen_pt.reserve(N * MAP_PT_D + 4));
-    CK(ctx->gen_normal.reserve(N * 3 + 4));
-    CK(cudaMemcpy2DAsync(ctx->gen_pt.p, MAP_PT_D * sizeof(double), point_w, 3 * sizeof(double), 3 * sizeof(double), N, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpy2DAsync(ctx->gen_pt.p + 3, MAP_PT_D * sizeof(double), var, 9 * sizeof(double), 9 * sizeof(double), N, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(ctx->gen_normal.p, normal, N * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
-    a.pt = ctx->gen_pt.p, a.normal = ctx->gen_normal.p;
+  const size_t M = (size_t)n_add, C = (size_t)L;
+  double *pt = nullptr, *pt_normal = nullptr, *add_pos_d, *add_normal_d;
+  uint8_t *mask;
+  int32_t *d_keep, *d_dst, *d_nk;
+  GenOut o;
+  float *d_patch;
+  auto lay = [&](ScratchLayout &s) {
+    if (point_w) pt = s.take<double>(N * MAP_PT_D + 4), pt_normal = s.take<double>(N * 3 + 4);  // pv_list_ from the host
+    add_pos_d = s.take<double>(3 * M + 4), add_normal_d = s.take<double>(3 * M);
+    mask = s.take<uint8_t>(C + 16), a.key = s.take<unsigned long long>(C + 1);
+    d_keep = s.take<int32_t>(C), d_dst = s.take<int32_t>(C), d_nk = s.take<int32_t>(1), o.source = s.take<int32_t>(C), o.cell = s.take<int32_t>(C);
+    o.pos = s.take<double>(3 * C), o.pc = s.take<double>(2 * C), o.normal = s.take<double>(3 * C), o.var = s.take<double>(9 * C);
+    o.score = s.take<float>(C), d_patch = s.take<float>(64 * C);
+  };
+  CK(lay_out_scratch(ctx, lay));
+  if (point_w) {  // point_w | var rows as map_pt holds them
+    CK(cudaMemcpy2DAsync(pt, MAP_PT_D * sizeof(double), point_w, 3 * sizeof(double), 3 * sizeof(double), N, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpy2DAsync(pt + 3, MAP_PT_D * sizeof(double), var, 9 * sizeof(double), 9 * sizeof(double), N, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(pt_normal, normal, N * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+    a.pt = pt, a.normal = pt_normal;
   } else {
     a.pt = ctx->map_pt.p, a.normal = ctx->map_pt_normal.p;
   }
-  CK(ctx->gen_add.reserve((size_t)n_add * 6 + 4));
   if (n_add > 0) {
-    CK(cudaMemcpyAsync(ctx->gen_add.p, add_pos, (size_t)n_add * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(ctx->gen_add.p + 3 * (size_t)n_add, add_normal, (size_t)n_add * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(add_pos_d, add_pos, M * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(add_normal_d, add_normal, M * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
   }
-  a.add_pos = ctx->gen_add.p, a.add_normal = ctx->gen_add.p + 3 * (size_t)n_add;
-  CK(ctx->gen_mask.reserve(L + 16));
-  CK(ctx->gen_key.reserve(L + 1));
-  CK(ctx->gen_i.reserve(4 * (size_t)L + 2));  // keep | dst | n_kept | source | cell
-  CK(ctx->gen_out_d.reserve(17 * (size_t)L));  // pos 3 | pc 2 | normal 3 | var 9
-  CK(ctx->gen_out_f.reserve(65 * (size_t)L));  // score 1 | patch 64
-  CK(cudaMemcpyAsync(ctx->gen_mask.p, type_map, L, cudaMemcpyHostToDevice, st));
-  CK(cudaMemsetAsync(ctx->gen_key.p, 0, (size_t)L * sizeof(unsigned long long), st));
-  a.type_map = ctx->gen_mask.p, a.key = ctx->gen_key.p;
-  int32_t *d_keep = ctx->gen_i.p, *d_dst = d_keep + L, *d_nk = d_dst + L;
-  GenOut o;
-  o.source = d_nk + 1, o.cell = o.source + L;
-  double *od = ctx->gen_out_d.p;
-  o.pos = od, o.pc = od + 3 * (size_t)L, o.normal = od + 5 * (size_t)L, o.var = od + 8 * (size_t)L;
-  o.score = ctx->gen_out_f.p;
-  float *d_patch = ctx->gen_out_f.p + L;
+  a.add_pos = add_pos_d, a.add_normal = add_normal_d;
+  CK(cudaMemcpyAsync(mask, type_map, L, cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(a.key, 0, C * sizeof(unsigned long long), st));
+  a.type_map = mask;
   gen_score_kernel<<<(n + n_add + GEN_THREADS - 1) / GEN_THREADS, GEN_THREADS, 0, st>>>(a);
-  gen_cells_kernel<<<(L + 255) / 256, 256, 0, st>>>(ctx->gen_key.p, L, d_keep);
+  gen_cells_kernel<<<(L + 255) / 256, 256, 0, st>>>(a.key, L, d_keep);
   select_scan_kernel<<<1, SELECT_SCAN_THREADS, 0, st>>>(d_keep, L, d_dst, d_nk);
   gen_scatter_kernel<<<(L + GEN_THREADS - 1) / GEN_THREADS, GEN_THREADS, 0, st>>>(a, d_keep, d_dst, o);
   ctx->launches += 4;
@@ -1977,26 +1983,26 @@ int esikf_vio_update_points(esikf_ctx *ctx, int32_t n, const uint8_t *converged,
   if (n == 0) return ESIKF_OK;  // total_points == 0 (:910)
   cudaStream_t st = ctx->stream;
   const size_t N = (size_t)n;
-  CK(ctx->obs_in.reserve(14 * N));    // last_T 12 | last_px 2
-  CK(ctx->obs_flag.reserve(2 * N));   // converged | update_flag
-  CK(ctx->obs_pc.reserve(2 * N));
-  CK(ctx->obs_out_pc.reserve(2 * N));
-  CK(ctx->obs_i.reserve(3 * N + 1));  // keep | dst | n_added | entry
-  CK(ctx->obs_patch.reserve(64 * N));
-  CK(cudaMemcpyAsync(ctx->obs_in.p, last_T_f_w, N * 12 * sizeof(double), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->obs_in.p + 12 * N, last_px, N * 2 * sizeof(double), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->obs_flag.p, converged, N, cudaMemcpyHostToDevice, st));
   ObsArgs a;
-  cam_dev(ctx, a.cam);
-  double Jdp_dR[9];
-  vio_consts(ctx, a.Rci, a.Pci, Jdp_dR);
-  a.state = dev_state, a.pos = ctx->vis_pos.p, a.converged = ctx->obs_flag.p, a.last_T = ctx->obs_in.p, a.last_px = ctx->obs_in.p + 12 * N;
-  a.n = n, a.cos_max = cos_max, a.flag = ctx->obs_flag.p + N, a.pc = ctx->obs_pc.p;
-  int32_t *d_keep = ctx->obs_i.p, *d_dst = d_keep + N, *d_nk = d_dst + N, *d_entry = d_nk + 1;
-  a.keep = d_keep;
+  double *last_T, *last_px_d, *out_pc;
+  uint8_t *conv;
+  int32_t *d_keep, *d_dst, *d_nk, *d_entry;
+  float *patch;
+  auto lay = [&](ScratchLayout &s) {
+    last_T = s.take<double>(12 * N), last_px_d = s.take<double>(2 * N), conv = s.take<uint8_t>(N), a.flag = s.take<uint8_t>(N);
+    a.pc = s.take<double>(2 * N), out_pc = s.take<double>(2 * N);
+    d_keep = s.take<int32_t>(N), d_dst = s.take<int32_t>(N), d_nk = s.take<int32_t>(1), d_entry = s.take<int32_t>(N), patch = s.take<float>(64 * N);
+  };
+  CK(lay_out_scratch(ctx, lay));
+  CK(cudaMemcpyAsync(last_T, last_T_f_w, N * 12 * sizeof(double), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(last_px_d, last_px, N * 2 * sizeof(double), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(conv, converged, N, cudaMemcpyHostToDevice, st));
+  frame_consts(ctx, a.cam, a.Rci, a.Pci);
+  a.state = dev_state, a.pos = ctx->vis_pos.p, a.converged = conv, a.last_T = last_T, a.last_px = last_px_d;
+  a.n = n, a.cos_max = cos_max, a.keep = d_keep;
   obs_flag_kernel<<<(n + OBS_THREADS - 1) / OBS_THREADS, OBS_THREADS, 0, st>>>(a);
   select_scan_kernel<<<1, SELECT_SCAN_THREADS, 0, st>>>(d_keep, n, d_dst, d_nk);
-  obs_scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_keep, d_dst, ctx->obs_pc.p, n, d_entry, ctx->obs_out_pc.p);
+  obs_scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_keep, d_dst, a.pc, n, d_entry, out_pc);
   ctx->launches += 3;
   CK(cudaGetLastError());
   int32_t nk = 0;
@@ -2008,13 +2014,13 @@ int esikf_vio_update_points(esikf_ctx *ctx, int32_t n, const uint8_t *converged,
   if (nk > 0) {
     const size_t K = (size_t)nk;
     if (patch_out) {
-      image_patch_kernel<<<(nk * 64 + 255) / 256, 256, 0, st>>>(ctx->img.p, ctx->img_w, ctx->img_h, ctx->obs_out_pc.p, nk, 0, ctx->obs_patch.p);
+      image_patch_kernel<<<(nk * 64 + 255) / 256, 256, 0, st>>>(ctx->img.p, ctx->img_w, ctx->img_h, out_pc, nk, 0, patch);
       ctx->launches++;
       CK(cudaGetLastError());
-      CK(cudaMemcpyAsync(patch_out, ctx->obs_patch.p, K * 64 * sizeof(float), cudaMemcpyDeviceToHost, st));
+      CK(cudaMemcpyAsync(patch_out, patch, K * 64 * sizeof(float), cudaMemcpyDeviceToHost, st));
     }
     if (entry_out) CK(cudaMemcpyAsync(entry_out, d_entry, K * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-    if (pc_out) CK(cudaMemcpyAsync(pc_out, ctx->obs_out_pc.p, K * 2 * sizeof(double), cudaMemcpyDeviceToHost, st));
+    if (pc_out) CK(cudaMemcpyAsync(pc_out, out_pc, K * 2 * sizeof(double), cudaMemcpyDeviceToHost, st));
   }
   CK(cudaStreamSynchronize(st));
   return ESIKF_OK;
@@ -2035,49 +2041,48 @@ int esikf_vio_retrieve_scan(esikf_ctx *ctx, const double *point_w, int32_t n, in
   cudaStream_t st = ctx->stream;
   const int W = ctx->cam.width, H = ctx->cam.height;
   const size_t N = (size_t)n, npix = (size_t)W * H;
+  size_t sort_bytes = 0, scan_bytes = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (unsigned long long *)nullptr, (unsigned long long *)nullptr, (uint32_t *)nullptr, (uint32_t *)nullptr, n, 0, 63, st);
+  cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (int32_t *)nullptr, (int32_t *)nullptr, n + 1, st);
+  double *pt = nullptr;
+  unsigned long long *k_out;
+  uint32_t *i_out;
+  int32_t *d_head, *d_dst, *d_keys;
+  uint8_t *tmp;
+  RetArgs a;
+  auto lay = [&](ScratchLayout &s) {
+    if (point_w) pt = s.take<double>(3 * N + 3);  // a host scan
+    a.key = s.take<unsigned long long>(N + 1), k_out = s.take<unsigned long long>(N + 1), a.idx = s.take<uint32_t>(N + 1), i_out = s.take<uint32_t>(N + 1);
+    d_head = s.take<int32_t>(N + 1), d_dst = s.take<int32_t>(N + 1), d_keys = s.take<int32_t>(3 * N), a.bad = s.take<int32_t>(1);
+    a.depth_pt = s.take<float>(N + 1), a.win = s.take<int32_t>(npix), tmp = s.take<uint8_t>(std::max(sort_bytes, scan_bytes));
+  };
+  CK(lay_out_scratch(ctx, lay));
   CK(ctx->ret_state.reserve(S_N));
-  CK(ctx->ret_key.reserve(2 * N + 2));
-  CK(ctx->ret_idx.reserve(2 * N + 2));
-  CK(ctx->ret_i.reserve(5 * N + 3));
-  CK(ctx->ret_depth_pt.reserve(N + 1));
-  CK(ctx->ret_win.reserve(npix));
   CK(ctx->ret_depth.reserve(npix));
   // the frame pose stays with the depth image for esikf_vio_depth_check, whatever a later update writes to `state`
   CK(cudaMemcpyAsync(ctx->ret_state.p, dev_state, S_N * sizeof(double), cudaMemcpyDeviceToDevice, st));
-  int32_t *d_head = ctx->ret_i.p, *d_dst = d_head + N + 1, *d_keys = d_dst + N + 1, *d_bad = d_keys + 3 * N;
-  CK(cudaMemsetAsync(ctx->ret_win.p, 0xff, npix * sizeof(int32_t), st));
-  CK(cudaMemsetAsync(d_bad, 0, sizeof(int32_t), st));
-  RetArgs a;
-  cam_dev(ctx, a.cam);
-  double Jdp_dR[9];
-  vio_consts(ctx, a.Rci, a.Pci, Jdp_dR);
+  CK(cudaMemsetAsync(a.win, 0xff, npix * sizeof(int32_t), st));
+  CK(cudaMemsetAsync(a.bad, 0, sizeof(int32_t), st));
+  frame_consts(ctx, a.cam, a.Rci, a.Pci);
   a.state = ctx->ret_state.p, a.n = n, a.border = border;
   if (point_w) {
-    CK(ctx->ret_pt.reserve(3 * N + 3));
-    if (n > 0) CK(cudaMemcpyAsync(ctx->ret_pt.p, point_w, 3 * N * sizeof(double), cudaMemcpyHostToDevice, st));
-    a.pt = ctx->ret_pt.p, a.pt_stride = 3;
+    if (n > 0) CK(cudaMemcpyAsync(pt, point_w, 3 * N * sizeof(double), cudaMemcpyHostToDevice, st));
+    a.pt = pt, a.pt_stride = 3;
   } else {
     a.pt = ctx->map_pt.p, a.pt_stride = MAP_PT_D;
   }
-  a.key = ctx->ret_key.p, a.idx = ctx->ret_idx.p, a.depth_pt = ctx->ret_depth_pt.p, a.win = ctx->ret_win.p, a.bad = d_bad;
   if (n > 0) ret_scan_kernel<<<(n + RET_THREADS - 1) / RET_THREADS, RET_THREADS, 0, st>>>(a);
-  ret_depth_kernel<<<(int)((npix + 255) / 256), 256, 0, st>>>(ctx->ret_win.p, ctx->ret_depth_pt.p, (int)npix, ctx->ret_depth.p);
+  ret_depth_kernel<<<(int)((npix + 255) / 256), 256, 0, st>>>(a.win, a.depth_pt, (int)npix, ctx->ret_depth.p);
   ctx->launches += n > 0 ? 2 : 1;
   int32_t counts[2] = {0, 0};  // distinct keys, bad
   if (n > 0) {
-    unsigned long long *k_out = ctx->ret_key.p + N;
-    uint32_t *i_out = ctx->ret_idx.p + N;
-    size_t sort_bytes = 0, scan_bytes = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, ctx->ret_key.p, k_out, ctx->ret_idx.p, i_out, n, 0, 63, st);
-    cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, d_head, d_dst, n + 1, st);
-    CK(ctx->ret_tmp.reserve(std::max(sort_bytes, scan_bytes) + 16));
-    CK(cub::DeviceRadixSort::SortPairs(ctx->ret_tmp.p, sort_bytes, ctx->ret_key.p, k_out, ctx->ret_idx.p, i_out, n, 0, 63, st));
+    CK(cub::DeviceRadixSort::SortPairs(tmp, sort_bytes, a.key, k_out, a.idx, i_out, n, 0, 63, st));
     ret_head_kernel<<<(n + 1 + 255) / 256, 256, 0, st>>>(k_out, i_out, n, d_head);
-    CK(cub::DeviceScan::ExclusiveSum(ctx->ret_tmp.p, scan_bytes, d_head, d_dst, n + 1, st));
-    ret_keys_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_head, d_dst, ctx->ret_key.p, n, d_keys);
+    CK(cub::DeviceScan::ExclusiveSum(tmp, scan_bytes, d_head, d_dst, n + 1, st));
+    ret_keys_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_head, d_dst, a.key, n, d_keys);
     ctx->launches += 4;  // sort passes counted as one
     CK(cudaMemcpyAsync(&counts[0], d_dst + n, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(&counts[1], d_bad, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&counts[1], a.bad, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   }
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(st));  // also: the caller may reuse its buffers on return
@@ -2099,18 +2104,20 @@ int esikf_vio_depth_check(esikf_ctx *ctx, int32_t n, const double *pos_w, const 
   CK(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
   const size_t N = (size_t)n;
-  CK(ctx->ret_cand.reserve(5 * N));  // pos 3n | pc 2n
-  CK(ctx->ret_flag.reserve(N));
-  CK(cudaMemcpyAsync(ctx->ret_cand.p, pos_w, 3 * N * sizeof(double), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->ret_cand.p + 3 * N, pc, 2 * N * sizeof(double), cudaMemcpyHostToDevice, st));
+  double *pos, *pc_d;
+  uint8_t *flag;
+  auto lay = [&](ScratchLayout &s) { pos = s.take<double>(3 * N), pc_d = s.take<double>(2 * N), flag = s.take<uint8_t>(N); };
+  CK(lay_out_scratch(ctx, lay));
+  CK(cudaMemcpyAsync(pos, pos_w, 3 * N * sizeof(double), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(pc_d, pc, 2 * N * sizeof(double), cudaMemcpyHostToDevice, st));
   DepthCheckArgs a;
   memcpy(a.Rci, ctx->ret_Rci, sizeof(a.Rci)), memcpy(a.Pci, ctx->ret_Pci, sizeof(a.Pci));
-  a.state = ctx->ret_state.p, a.pos = ctx->ret_cand.p, a.pc = ctx->ret_cand.p + 3 * N, a.n = n, a.width = ctx->ret_w, a.height = ctx->ret_h;
-  a.depth = ctx->ret_depth.p, a.flag = ctx->ret_flag.p;
+  a.state = ctx->ret_state.p, a.pos = pos, a.pc = pc_d, a.n = n, a.width = ctx->ret_w, a.height = ctx->ret_h;
+  a.depth = ctx->ret_depth.p, a.flag = flag;
   ret_depth_check_kernel<<<(n + RET_THREADS - 1) / RET_THREADS, RET_THREADS, 0, st>>>(a);
   ctx->launches++;
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(discontinuous_out, ctx->ret_flag.p, N, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(discontinuous_out, flag, N, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   return ESIKF_OK;
 }
@@ -2127,42 +2134,34 @@ int esikf_vio_score_ref_patches(esikf_ctx *ctx, int32_t n, const int32_t *first,
   CK(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
   const size_t N = (size_t)n, M = (size_t)m;
-  const size_t out_b = 8 * M + 4 * N;  // score m | mean m | ref n
-  CK(ctx->rp_d.reserve(6 * N + 12 * M + 1));  // pos 3n | normal 3n | T_f_w 12m
-  CK(ctx->rp_f.reserve(65 * M + 1));          // patch 64m | mean m
-  CK(ctx->rp_i.reserve(N + 1 + M));           // first n + 1 | id m
-  CK(ctx->rp_out.reserve(out_b));
-  if (out_b > ctx->rp_host_cap) {
-    if (ctx->rp_host) cudaFreeHost(ctx->rp_host);
-    ctx->rp_host = nullptr, ctx->rp_host_cap = 0;
-    CK(cudaMallocHost((void **)&ctx->rp_host, out_b + out_b / 4));
-    ctx->rp_host_cap = out_b + out_b / 4;
-  }
-  double *d = ctx->rp_d.p;
-  float *f = ctx->rp_f.p;
-  int32_t *k = ctx->rp_i.p;
-  CK(cudaMemcpyAsync(d, pos, 3 * N * sizeof(double), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d + 3 * N, normal, 3 * N * sizeof(double), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(k, first, (N + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  if (m > 0) {
-    CK(cudaMemcpyAsync(d + 6 * N, T_f_w, 12 * M * sizeof(double), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(f, patch, 64 * M * sizeof(float), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(f + 64 * M, mean, M * sizeof(float), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(k + N + 1, id, M * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  }
-  uint8_t *o = ctx->rp_out.p;
+  double *d_pos, *d_normal, *d_T;
+  float *d_patch, *d_mean;
+  int32_t *d_first, *d_id;
   RefPatchArgs a;
-  a.first = k, a.pos = d, a.normal = d + 3 * N, a.T = d + 6 * N, a.patch = f, a.mean = f + 64 * M, a.id = k + N + 1, a.n = n;
-  a.score = (float *)o, a.mean_out = (float *)(o + 4 * M), a.ref = (int32_t *)(o + 8 * M);
+  a.n = n;
+  auto lay = [&](ScratchLayout &s) {
+    d_pos = s.take<double>(3 * N), d_normal = s.take<double>(3 * N), d_T = s.take<double>(12 * M), d_patch = s.take<float>(64 * M), d_mean = s.take<float>(M);
+    d_first = s.take<int32_t>(N + 1), d_id = s.take<int32_t>(M);
+    a.score = s.take<float>(M), a.mean_out = s.take<float>(M), a.ref = s.take<int32_t>(N);  // read back as one span
+  };
+  CK(lay_out_scratch(ctx, lay));
+  CK(cudaMemcpyAsync(d_pos, pos, 3 * N * sizeof(double), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d_normal, normal, 3 * N * sizeof(double), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d_first, first, (N + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  if (m > 0) {
+    CK(cudaMemcpyAsync(d_T, T_f_w, 12 * M * sizeof(double), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_patch, patch, 64 * M * sizeof(float), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_mean, mean, M * sizeof(float), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_id, id, M * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  }
+  a.first = d_first, a.pos = d_pos, a.normal = d_normal, a.T = d_T, a.patch = d_patch, a.mean = d_mean, a.id = d_id;
   refpatch_score_kernel<<<(n + RP_WARPS - 1) / RP_WARPS, RP_WARPS * 32, 0, st>>>(a);
   ctx->launches++;
   CK(cudaGetLastError());
-  // one copy into pinned staging and one synchronisation; the caller's buffers are written only once everything succeeded
-  CK(cudaMemcpyAsync(ctx->rp_host, o, out_b, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  memcpy(score_out, ctx->rp_host, 4 * M);
-  memcpy(mean_out, ctx->rp_host + 4 * M, 4 * M);
-  memcpy(ref_out, ctx->rp_host + 8 * M, 4 * N);
+  CK(read_back(ctx, a.score, a.ref + N));
+  copy_out(ctx, score_out, a.score, a.score, 4 * M);
+  copy_out(ctx, mean_out, a.score, a.mean_out, 4 * M);
+  copy_out(ctx, ref_out, a.score, a.ref, 4 * N);
   return ESIKF_OK;
 }
 

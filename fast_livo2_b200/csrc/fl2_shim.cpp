@@ -216,15 +216,14 @@ void VoxelMapManager::SyncDeviceMap() {
     // same roots and candidate lists as on the device: only the refitted records travel
     std::vector<esikf_plane> recs(ids.size());
     for (size_t k = 0; k < ids.size(); k++) recs[k] = now.planes[ids[k]];
-    last_status_ = ids.empty() ? 0 : esikf_map_patch(ctx_, ids.data(), recs.data(), (int32_t)ids.size());
+    Record(ctx_, ids.empty() ? 0 : esikf_map_patch(ctx_, ids.data(), recs.data(), (int32_t)ids.size()));
     last_sync_patched_ = (int)ids.size();
   } else {
-    last_status_ = esikf_map_upload(ctx_, now.keys.data(), now.first.data(), now.count.data(), (int32_t)now.first.size(), now.planes.data(),
-                                    (int32_t)now.planes.size(), config_setting_.max_voxel_size_);
+    Record(ctx_, esikf_map_upload(ctx_, now.keys.data(), now.first.data(), now.count.data(), (int32_t)now.first.size(), now.planes.data(),
+                                  (int32_t)now.planes.size(), config_setting_.max_voxel_size_));
     last_sync_patched_ = -1;
   }
   if (last_status_) {
-    last_error_ = esikf_last_error(ctx_);
     device_has_map_ = false;  // unknown device state: the next sync uploads everything
   } else {
     flat_.keys.swap(now.keys), flat_.first.swap(now.first), flat_.count.swap(now.count), flat_.planes.swap(now.planes), flat_.plane_src.swap(now.plane_src);
@@ -247,10 +246,7 @@ void VoxelMapManager::EnableDeviceMap() {
   device_map_mirror_ = config_setting_.device_map_mirror_;
   if (device_map_mirror_) ClearVoxelMap(voxel_map_);  // the mirror starts as empty as the device map
   mirror_valid_ = false;
-  if ((last_status_ = esikf_map_device_init(ctx_, &m)) != 0) {
-    last_error_ = esikf_last_error(ctx_);
-    return;
-  }
+  if (Record(ctx_, esikf_map_device_init(ctx_, &m))) return;
   device_map_ = true, map_synced_ = true, device_has_map_ = true;
   mirror_valid_ = device_map_mirror_;
 }
@@ -278,17 +274,14 @@ void VoxelMapManager::UpdateMirror() {
     int32_t *first = exp_first_.get(exp_roots_cap_), *count = exp_count_.get(exp_roots_cap_);
     esikf_map_node *nodes = exp_nodes_.get(exp_nodes_cap_);
     if (!keys || !first || !count || !nodes) {
-      last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
+      StagingFailed();
       return InvalidateMirror();
     }
     last_status_ = esikf_map_device_export(ctx_, keys, first, count, exp_roots_cap_, nodes, exp_nodes_cap_, &nr, &nn);
     if (last_status_ == 0 || (nr <= exp_roots_cap_ && nn <= exp_nodes_cap_)) break;
     exp_roots_cap_ = nr + nr / 4 + 64, exp_nodes_cap_ = nn + nn / 4 + 64;  // too small: grow and export again
   }
-  if (last_status_) {
-    last_error_ = esikf_last_error(ctx_);
-    return InvalidateMirror();
-  }
+  if (Record(ctx_, last_status_)) return InvalidateMirror();
   if (!ApplyMapExport(voxel_map_, config_setting_, exp_keys_.data(), exp_first_.data(), exp_count_.data(), nr, exp_nodes_.data(), nn, &last_error_)) {
     last_status_ = ESIKF_ERR_STATE;
     return InvalidateMirror();
@@ -304,15 +297,12 @@ void VoxelMapManager::BuildVoxelMap() {
   const int n = feats_down_size_;
   float *pts = st_pts_.get((size_t)n * 3 + 4);
   double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
-  if (!pts || !sbuf) {
-    last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
-    return;
-  }
+  if (!pts || !sbuf) return StagingFailed();
   if (n) par_memcpy(pts, &feats_down_body_[0].x, (size_t)n * 12);
   state_.pack(sbuf);
   if ((last_status_ = esikf_set_lidar_extrinsics(ctx_, extR_.m, extT_.v)) == 0 && (last_status_ = esikf_lio_set_scan(ctx_, pts, n)) == 0)
     last_status_ = esikf_map_device_build(ctx_, sbuf);
-  if (last_status_) last_error_ = esikf_last_error(ctx_);
+  Record(ctx_, last_status_);
   UpdateMirror();
 }
 
@@ -324,7 +314,7 @@ void VoxelMapManager::UpdateVoxelMap() {
   }
   double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
   state_.pack(sbuf);  // _state == voxelmap_manager->state_ at this point of the tick (LIVMapper.cpp:371); 3 kB
-  if ((last_status_ = esikf_map_device_update(ctx_, sbuf)) != 0) last_error_ = esikf_last_error(ctx_);
+  Record(ctx_, esikf_map_device_update(ctx_, sbuf));
   UpdateMirror();
 }
 
@@ -335,17 +325,14 @@ void VoxelMapManager::SetWorldCloud(const std::vector<PointXYZ> *dense_scan) {
   }
   double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
   float *pts = dense_scan ? st_pts_.get(dense_scan->size() * 3 + 3) : nullptr;
-  if (!sbuf || (dense_scan && !pts)) {
-    last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
-    return;
-  }
+  if (!sbuf || (dense_scan && !pts)) return StagingFailed();
   state_.pack(sbuf);  // _state == state_ after StateEstimation (LIVMapper.cpp:371)
   int n = 0;
   if (dense_scan) {
     n = (int)dense_scan->size();
     for (int i = 0; i < n; i++) pts[3 * i] = (*dense_scan)[i].x, pts[3 * i + 1] = (*dense_scan)[i].y, pts[3 * i + 2] = (*dense_scan)[i].z;
   }
-  if ((last_status_ = esikf_rgb_set_cloud(ctx_, pts, n, sbuf)) != 0) last_error_ = esikf_last_error(ctx_);
+  Record(ctx_, esikf_rgb_set_cloud(ctx_, pts, n, sbuf));
 }
 
 void VoxelMapManager::FindCorrespond(int n, const V3D *pts, int rule, uint8_t *status, VoxelPlane *planes) {
@@ -361,16 +348,10 @@ void VoxelMapManager::FindCorrespond(int n, const V3D *pts, int rule, uint8_t *s
   uint8_t *st = st_find_status_.get((size_t)n + 1);
   int64_t *keys = st_find_keys_.get((size_t)n * 3 + 3);
   esikf_plane *rows = st_find_rows_.get((size_t)n + 1);
-  if (!p || !st || !keys || !rows) {
-    last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
-    return;
-  }
+  if (!p || !st || !keys || !rows) return StagingFailed();
   for (int i = 0; i < n; i++)
     for (int k = 0; k < 3; k++) p[3 * i + k] = pts[i][k];
-  if ((last_status_ = esikf_map_device_find(ctx_, p, n, rule, st, keys, rows)) != 0) {
-    last_error_ = esikf_last_error(ctx_);
-    return;
-  }
+  if (Record(ctx_, esikf_map_device_find(ctx_, p, n, rule, st, keys, rows))) return;
   for (int i = 0; i < n; i++) {
     status[i] = st[i];
     VoxelPlane &o = planes[i];
@@ -400,7 +381,7 @@ void VoxelMapManager::mapSliding() {
     if (loc < 0) loc -= 1.0;
     lo[j] = (int64_t)loc - config_setting_.half_map_size, hi[j] = (int64_t)loc + config_setting_.half_map_size;
   }
-  if ((last_status_ = esikf_map_device_slide(ctx_, lo, hi)) != 0) last_error_ = esikf_last_error(ctx_);
+  Record(ctx_, esikf_map_device_slide(ctx_, lo, hi));
   if (device_map_mirror_) {
     if (last_status_) {
       InvalidateMirror();
@@ -421,16 +402,13 @@ void VoxelMapManager::UpdateVoxelMap(const std::vector<pointWithVar> &input_poin
   }
   const size_t n = input_points.size();
   double *buf = st_cov_.get(n * 12 + 2);
-  if (!buf) {
-    last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
-    return;
-  }
+  if (!buf) return StagingFailed();
   double *pw = buf, *var = buf + n * 3;
   for (size_t i = 0; i < n; i++) {
     for (int k = 0; k < 3; k++) pw[3 * i + k] = input_points[i].point_w[k];
     memcpy(var + 9 * i, input_points[i].var.m, 72);
   }
-  if ((last_status_ = esikf_map_device_update_points(ctx_, pw, var, (int32_t)n)) != 0) last_error_ = esikf_last_error(ctx_);
+  Record(ctx_, esikf_map_device_update_points(ctx_, pw, var, (int32_t)n));
   UpdateMirror();
 }
 
@@ -440,10 +418,7 @@ void VoxelMapManager::StateEstimation(StatesGroup &state_propagat) {
   if (!map_synced_) SyncDeviceMap();
   if (!map_synced_) return;
   // lidar -> imu extrinsics only: the camera part belongs to the VIOManager sharing this context (it must survive the LIO tick)
-  if ((last_status_ = esikf_set_lidar_extrinsics(ctx_, extR_.m, extT_.v)) != 0) {
-    last_error_ = esikf_last_error(ctx_);
-    return;
-  }
+  if (Record(ctx_, esikf_set_lidar_extrinsics(ctx_, extR_.m, extT_.v))) return;
   const int n = feats_down_size_;
   esikf_lio_cfg cfg;
   cfg.voxel_size = config_setting_.max_voxel_size_, cfg.sigma_num = config_setting_.sigma_num_;
@@ -453,21 +428,14 @@ void VoxelMapManager::StateEstimation(StatesGroup &state_propagat) {
   double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
   float *pts = st_pts_.get((size_t)n * 3 + 4), *dis = st_dis_.get((size_t)n + 1);
   int32_t *match = st_match_.get((size_t)n + 1), *normal = st_normal_.get((size_t)n + 1);
-  if (!sbuf || !pts || !dis || !match || !normal) {
-    last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
-    return;
-  }
+  if (!sbuf || !pts || !dis || !match || !normal) return StagingFailed();
   double *sin = sbuf, *sprop = sbuf + ESIKF_STATE_DOUBLES, *sout = sbuf + 2 * ESIKF_STATE_DOUBLES;
   state_.pack(sin);
   state_propagat.pack(sprop);
   esikf_lio_stats stats;
   static_assert(sizeof(PointXYZ) == 12, "xyz float32");
   if (n) par_memcpy(pts, &feats_down_body_[0].x, (size_t)n * 12);
-  last_status_ = esikf_lio_update(ctx_, n ? pts : nullptr, n, sin, sprop, &cfg, sout, &stats, match, normal, dis);
-  if (last_status_) {
-    last_error_ = esikf_last_error(ctx_);
-    return;
-  }
+  if (Record(ctx_, esikf_lio_update(ctx_, n ? pts : nullptr, n, sin, sprop, &cfg, sout, &stats, match, normal, dis))) return;
   state_.unpack(sout);                 // _state = voxelmap_manager->state_  (LIVMapper.cpp:371)
   position_last_ = state_.pos_end;     // src/voxel_map.cpp:492
   effct_feat_num_ = stats.iters > 0 ? stats.effct_feat_num[stats.iters - 1] : 0;
@@ -484,26 +452,17 @@ void VoxelMapManager::MaterializePointLists() {
   const int32_t *match = st_match_.data(), *normal = st_normal_.data();
   const float *dis = st_dis_.data();
   double *cov = st_cov_.get((size_t)n * 18 + 2);
-  if (!cov) {
-    last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
-    return;
-  }
+  if (!cov) return StagingFailed();
   const double *bc = cov, *cm = cov + (size_t)n * 9;
-  if ((last_status_ = esikf_lio_fetch_point_cov(ctx_, cov, cov + (size_t)n * 9)) != 0) {
-    last_error_ = esikf_last_error(ctx_);
-    return;
-  }
+  if (Record(ctx_, esikf_lio_fetch_point_cov(ctx_, cov, cov + (size_t)n * 9))) return;
   body_cov_list_.resize(n), cross_mat_list_.resize(n);
   pv_list_.resize(n);
   ptpl_list_.clear();
   const double *dev_normals = nullptr;
   if (device_map_) {  // no host VoxelPlane exists: pv.normal comes from the device records
     double *nb = st_normals_.get((size_t)n * 3 + 2);
-    if (!nb || (last_status_ = esikf_lio_fetch_normals(ctx_, nb)) != 0) {
-      last_error_ = nb ? esikf_last_error(ctx_) : "pinned staging allocation failed";
-      if (!nb) last_status_ = ESIKF_ERR_CUDA;
-      return;
-    }
+    if (!nb) return StagingFailed();
+    if (Record(ctx_, esikf_lio_fetch_normals(ctx_, nb))) return;
     dev_normals = nb;
   }
   const double *R = state_.rot_end.m;
@@ -555,10 +514,7 @@ void VIOManager::GenerateVisualMapPoints(const std::vector<uint8_t> &type_map, i
     return;
   }
   double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
-  if (!sbuf) {
-    last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
-    return;
-  }
+  if (!sbuf) return StagingFailed();
   state->pack(sbuf);
   const size_t n = pg ? pg->size() : 0, m = add_from_voxel_map ? add_from_voxel_map->size() : 0;
   gen_in_.resize(15 * n + 6 * m + 1);
@@ -574,13 +530,10 @@ void VIOManager::GenerateVisualMapPoints(const std::vector<uint8_t> &type_map, i
   gen_src_.resize(cap + 1), gen_cell_.resize(cap + 1), gen_pos_.resize(3 * cap + 3), gen_pc_.resize(2 * cap + 2), gen_normal_.resize(3 * cap + 3);
   gen_var_.resize(9 * cap + 9), gen_score_.resize(cap + 1), gen_patch_.resize(64 * cap + 64);
   int32_t k = 0;
-  last_status_ = esikf_vio_generate_points(ctx_, pg ? pw : nullptr, nv, var, (int32_t)n, ap, an, (int32_t)m, type_map.data(), cap, grid_size, grid_n_width,
-                                           grid_n_height, border, sbuf, cap, &k, gen_src_.data(), gen_cell_.data(), gen_pos_.data(), gen_pc_.data(),
-                                           gen_score_.data(), gen_normal_.data(), gen_var_.data(), gen_patch_.data());
-  if (last_status_) {
-    last_error_ = esikf_last_error(ctx_);
+  if (Record(ctx_, esikf_vio_generate_points(ctx_, pg ? pw : nullptr, nv, var, (int32_t)n, ap, an, (int32_t)m, type_map.data(), cap, grid_size, grid_n_width,
+                                             grid_n_height, border, sbuf, cap, &k, gen_src_.data(), gen_cell_.data(), gen_pos_.data(), gen_pc_.data(),
+                                             gen_score_.data(), gen_normal_.data(), gen_var_.data(), gen_patch_.data())))
     return;
-  }
   new_points.resize(k);
   for (int i = 0; i < k; i++) {
     NewVisualPoint &q = new_points[i];
@@ -607,10 +560,7 @@ void VIOManager::UpdateVisualMapPoints(const std::vector<uint8_t> &converged, co
     return;
   }
   double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
-  if (!sbuf) {
-    last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
-    return;
-  }
+  if (!sbuf) return StagingFailed();
   state->pack(sbuf);
   const size_t n = last_obs.size();
   obs_in_.resize(14 * n + 1);
@@ -618,12 +568,9 @@ void VIOManager::UpdateVisualMapPoints(const std::vector<uint8_t> &converged, co
   for (size_t i = 0; i < n; i++) memcpy(T + 12 * i, last_obs[i].T_f_w, sizeof(last_obs[i].T_f_w)), memcpy(px + 2 * i, last_obs[i].px, sizeof(last_obs[i].px));
   obs_entry_.resize(n + 1), obs_pc_.resize(2 * n + 2), obs_patch_.resize(64 * n + 64);
   int32_t k = 0;
-  last_status_ = esikf_vio_update_points(ctx_, (int32_t)n, converged.data(), T, px, sbuf, (int32_t)n, &k, update_flag.data(), obs_entry_.data(), obs_pc_.data(),
-                                         obs_patch_.data());
-  if (last_status_) {
-    last_error_ = esikf_last_error(ctx_);
+  if (Record(ctx_, esikf_vio_update_points(ctx_, (int32_t)n, converged.data(), T, px, sbuf, (int32_t)n, &k, update_flag.data(), obs_entry_.data(),
+                                           obs_pc_.data(), obs_patch_.data())))
     return;
-  }
   new_obs.resize(k);
   for (int i = 0; i < k; i++) {
     NewObservation &q = new_obs[i];
@@ -640,34 +587,22 @@ void VIOManager::RetrieveScanVoxels(int border, const std::vector<pointWithVar> 
   }
   const size_t n = pg ? pg->size() : 0;
   double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES), *pw = st_ret_pt_.get(3 * n + 3);
-  if (!sbuf || !pw) {
-    last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
-    return;
-  }
+  if (!sbuf || !pw) return StagingFailed();
   state->pack(sbuf);
   for (size_t i = 0; i < n; i++)
     for (int k = 0; k < 3; k++) pw[3 * i + k] = (*pg)[i].point_w[k];
   // room for one key per point of a host scan; for the resident scan a first call reports the count when the room is short
   int32_t cap = pg ? (int32_t)n : (int32_t)(keys_cap_ > 0 ? keys_cap_ : 1 << 16), k = -1;
   int32_t *kb = st_ret_keys_.get(3 * (size_t)cap + 3);
-  if (!kb) {
-    last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
-    return;
-  }
+  if (!kb) return StagingFailed();
   last_status_ = esikf_vio_retrieve_scan(ctx_, pg ? pw : nullptr, (int32_t)n, border, sbuf, cap, &k, kb, nullptr);
   if (last_status_ == ESIKF_ERR_ARG && !pg && k > cap) {
     cap = k, keys_cap_ = k;
     kb = st_ret_keys_.get(3 * (size_t)cap + 3);
-    if (!kb) {
-      last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
-      return;
-    }
+    if (!kb) return StagingFailed();
     last_status_ = esikf_vio_retrieve_scan(ctx_, nullptr, 0, border, sbuf, cap, &k, kb, nullptr);
   }
-  if (last_status_) {
-    last_error_ = esikf_last_error(ctx_);
-    return;
-  }
+  if (Record(ctx_, last_status_)) return;
   keys.resize(k);
   for (int i = 0; i < k; i++) keys[i] = VOXEL_LOCATION(kb[3 * i], kb[3 * i + 1], kb[3 * i + 2]);
 }
@@ -684,16 +619,9 @@ void VIOManager::CheckDepthContinuity(int n, const double *pos, const double *pc
   }
   double *cb = st_ret_cand_.get(5 * (size_t)n);
   uint8_t *fb = st_ret_flag_.get((size_t)n);
-  if (!cb || !fb) {
-    last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
-    return;
-  }
+  if (!cb || !fb) return StagingFailed();
   memcpy(cb, pos, 3 * (size_t)n * sizeof(double)), memcpy(cb + 3 * (size_t)n, pc, 2 * (size_t)n * sizeof(double));
-  last_status_ = esikf_vio_depth_check(ctx_, n, cb, cb + 3 * (size_t)n, fb);
-  if (last_status_) {
-    last_error_ = esikf_last_error(ctx_);
-    return;
-  }
+  if (Record(ctx_, esikf_vio_depth_check(ctx_, n, cb, cb + 3 * (size_t)n, fb))) return;
   memcpy(discontinuous.data(), fb, (size_t)n);
 }
 
@@ -711,10 +639,7 @@ void VIOManager::ScoreReferencePatches(const std::vector<int32_t> &first, const 
   double *d = st_rp_d_.get(6 * n + 12 * m + 1);  // pos 3n | normal 3n | T_f_w 12m
   float *f = st_rp_f_.get(65 * m + 1);           // patch 64m | mean m
   int32_t *k = st_rp_i_.get(n + 1 + m);          // first n + 1 | id m
-  if (!d || !f || !k) {
-    last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
-    return;
-  }
+  if (!d || !f || !k) return StagingFailed();
   memcpy(k, first.data(), (n + 1) * sizeof(int32_t));
   for (size_t i = 0; i < n; i++) memcpy(d + 3 * i, pts[i].pos, sizeof(pts[i].pos)), memcpy(d + 3 * n + 3 * i, pts[i].normal, sizeof(pts[i].normal));
   for (size_t j = 0; j < m; j++) {
@@ -723,11 +648,8 @@ void VIOManager::ScoreReferencePatches(const std::vector<int32_t> &first, const 
   }
   std::vector<float> sc(m), mu(m);
   std::vector<int32_t> rf(n);
-  last_status_ = esikf_vio_score_ref_patches(ctx_, (int32_t)n, k, (int32_t)m, d, d + 3 * n, f, f + 64 * m, k + n + 1, d + 6 * n, sc.data(), mu.data(), rf.data());
-  if (last_status_) {
-    last_error_ = esikf_last_error(ctx_);
+  if (Record(ctx_, esikf_vio_score_ref_patches(ctx_, (int32_t)n, k, (int32_t)m, d, d + 3 * n, f, f + 64 * m, k + n + 1, d + 6 * n, sc.data(), mu.data(), rf.data())))
     return;
-  }
   score.swap(sc), mean.swap(mu), ref.swap(rf);
 }
 
@@ -743,7 +665,7 @@ void VIOManager::initializeVIO() {
   cfg.img_point_cov = img_point_cov, cfg.patch_pyrimid_level = patch_pyrimid_level, cfg.max_iterations = max_iterations;
   cfg.exposure_estimate_en = exposure_estimate_en ? 1 : 0, cfg.inverse_composition_en = 0;
   if (!last_status_) last_status_ = esikf_vio_set_camera(ctx_, &cam, &cfg);
-  if (last_status_) last_error_ = esikf_last_error(ctx_);
+  Record(ctx_, last_status_);
 }
 
 // include/vio.h:153 / src/vio.cpp:784-802
@@ -755,10 +677,7 @@ void VIOManager::computeJacobianAndUpdateEKF(const GrayImage &img) {
     // the sub-map SelectSubSparseMap installed is still on the device: image and states only
     double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
     float *err = st_err_.get(n);
-    if (!sbuf || !err) {
-      last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
-      return;
-    }
+    if (!sbuf || !err) return StagingFailed();
     double *sin = sbuf, *sprop = sbuf + ESIKF_STATE_DOUBLES, *sout = sbuf + 2 * ESIKF_STATE_DOUBLES;
     state->pack(sin);
     state_propagat->pack(sprop);
@@ -767,10 +686,7 @@ void VIOManager::computeJacobianAndUpdateEKF(const GrayImage &img) {
     patch_img_ = nullptr;
     if (!last_status_) last_status_ = esikf_vio_run(ctx_, sin, sprop);
     if (!last_status_) last_status_ = esikf_vio_fetch(ctx_, sout, &stats, err);
-    if (last_status_) {
-      last_error_ = esikf_last_error(ctx_);
-      return;
-    }
+    if (Record(ctx_, last_status_)) return;
     visual_submap->errors.assign(err, err + n);
     state->unpack(sout);
     last_total_iters_ = stats.total_iters;
@@ -780,10 +696,7 @@ void VIOManager::computeJacobianAndUpdateEKF(const GrayImage &img) {
   float *wp = st_wp_.get((size_t)n * 64 * L), *err = st_err_.get(n);
   int32_t *sl = st_sl_.get(n);
   uint8_t *im = st_img_.get((size_t)img.cols * img.rows);
-  if (!pos || !ie || !sbuf || !wp || !err || !sl || !im) {
-    last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
-    return;
-  }
+  if (!pos || !ie || !sbuf || !wp || !err || !sl || !im) return StagingFailed();
   const SubSparseMap &sub = *visual_submap;
 #pragma omp parallel for num_threads(FL2_PACK_THREADS) schedule(static) if (n > 256)
   for (int i = 0; i < n; i++) {
@@ -801,10 +714,7 @@ void VIOManager::computeJacobianAndUpdateEKF(const GrayImage &img) {
   last_status_ = esikf_vio_update(ctx_, im, img.cols, img.rows, pos, wp, sl, ie, n, sin, sprop, sout, &stats, err);
   selected_submap_ = nullptr, selected_count_ = -1;  // the device now holds this upload
   submap_uploads_++;
-  if (last_status_) {
-    last_error_ = esikf_last_error(ctx_);
-    return;
-  }
+  if (Record(ctx_, last_status_)) return;
   visual_submap->errors.assign(err, err + n);
   state->unpack(sout);
   last_total_iters_ = stats.total_iters;
@@ -820,10 +730,7 @@ void VIOManager::getImagePatch(const GrayImage &img, const double pc[2], float *
   }
   float out[64];
   if (!last_status_) last_status_ = esikf_vio_get_image_patch(ctx_, pc, 1, level, out);
-  if (last_status_) {
-    last_error_ = esikf_last_error(ctx_);
-    return;
-  }
+  if (Record(ctx_, last_status_)) return;
   memcpy(patch_tmp + 64 * level, out, sizeof(out));
 }
 
@@ -848,10 +755,7 @@ void VIOManager::warpAffine(const double A_cur_ref[4], const GrayImage &img_ref,
   std::vector<float> all((size_t)64 * patch_pyrimid_level);
   const int32_t idx = 0, sl = search_level;
   if (!last_status_) last_status_ = esikf_vio_warp_affine(ctx_, 1, &idx, px_ref, A_cur_ref, &sl, all.data());
-  if (last_status_) {
-    last_error_ = esikf_last_error(ctx_);
-    return;
-  }
+  if (Record(ctx_, last_status_)) return;
   // a singular A leaves the patch untouched in the reference (vio.cpp:297-301); the kernel writes zeros into its own
   // scratch in that case, so only copy when A is invertible
   const double det = A_cur_ref[0] * A_cur_ref[3] - A_cur_ref[1] * A_cur_ref[2];
@@ -879,29 +783,20 @@ void VIOManager::ColorizeFrameWorld(const BgrImage &img_rgb, double blind_rgb_po
     return;
   }
   double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
-  if (!sbuf) {
-    last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
-    return;
-  }
+  if (!sbuf) return StagingFailed();
   state->pack(sbuf);
   int32_t kept = 0;
   // the staging holds the largest coloured scan seen so far; a larger one is computed again into grown buffers
   for (int attempt = 0; attempt < 2; attempt++) {
     float *xyz = st_rgb_xyz_.get((size_t)rgb_cap_ * 3 + 3);
     uint8_t *bgr = st_rgb_bgr_.get((size_t)rgb_cap_ * 3 + 3);
-    if (!xyz || !bgr) {
-      last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed";
-      return;
-    }
+    if (!xyz || !bgr) return StagingFailed();
     last_status_ = esikf_rgb_colorize(ctx_, img_rgb.data, img_rgb.cols, img_rgb.rows, sbuf, blind_rgb_points, rgb_cap_, &kept, xyz, bgr, nullptr);
     if (last_status_ == ESIKF_ERR_ARG && kept > rgb_cap_) {
       rgb_cap_ = kept;
       continue;
     }
-    if (last_status_) {
-      last_error_ = esikf_last_error(ctx_);
-      return;
-    }
+    if (Record(ctx_, last_status_)) return;
     laserCloudWorldRGB.resize(kept);
     for (int i = 0; i < kept; i++) {
       PointXYZRGB &p = laserCloudWorldRGB[i];
@@ -938,10 +833,7 @@ void VIOManager::SelectSubSparseMap(const SubMapCandidate *c, int n, const GrayI
     last_status_ = esikf_vio_select_patches(ctx_, n, idx.data(), px.data(), lvl.data(), f.data(), rp.data(), pw.data(), nw.data(), T.data(), ie.data(),
                                             key.data(), pc.data(), T_cur_w, state->inv_expo_time, &cfg, &nk, kept.data(), err.data(), sl.data(), A.data(),
                                             nullptr);
-  if (last_status_) {
-    last_error_ = esikf_last_error(ctx_);
-    return;
-  }
+  if (Record(ctx_, last_status_)) return;
   SubSparseMap &sub = *visual_submap;  // :765-770, in candidate order
   sub.voxel_points_pos.resize(nk), sub.search_levels.assign(sl.begin(), sl.begin() + nk), sub.errors.assign(err.begin(), err.begin() + nk);
   sub.inv_expo_list.resize(nk), sub.candidate_index.assign(kept.begin(), kept.begin() + nk), sub.warp_patch.clear();
@@ -968,10 +860,7 @@ void VIOManager::MaterializeWarpPatches() {
   // the same kernel on the same matrices, levels and reference pixels as the selection: the patches the device holds
   std::vector<float> wp((size_t)nk * 64 * L);
   if (!last_status_) last_status_ = esikf_vio_warp_affine(ctx_, nk, sel_ref_idx_.data(), sel_px_.data(), sel_A_.data(), sel_sl_.data(), wp.data());
-  if (last_status_) {
-    last_error_ = esikf_last_error(ctx_);
-    return;
-  }
+  if (Record(ctx_, last_status_)) return;
   visual_submap->warp_patch.resize(nk);
   for (int j = 0; j < nk; j++) visual_submap->warp_patch[j].assign(wp.begin() + (size_t)j * 64 * L, wp.begin() + (size_t)(j + 1) * 64 * L);
 }

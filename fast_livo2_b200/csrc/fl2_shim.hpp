@@ -167,7 +167,22 @@ template <typename T> class PinnedBuf {
   size_t cap_ = 0;
 };
 
-class VoxelMapManager {
+// The outcome of a manager's last call (the reference's calls return void): an esikf_status, and the message when it failed.
+struct CallStatus {
+  int last_status_ = 0;
+  std::string last_error_;
+
+ protected:
+  // records the esikf_* return code of a call on ctx, with the context's message when it is an error; returns the code
+  int Record(const esikf_ctx *ctx, int status) {
+    last_status_ = status;
+    if (status) last_error_ = esikf_last_error(ctx);
+    return status;
+  }
+  void StagingFailed() { last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed"; }
+};
+
+class VoxelMapManager : public CallStatus {
  public:
   VoxelMapConfig config_setting_;
   VoxelMap &voxel_map_;
@@ -185,9 +200,7 @@ class VoxelMapManager {
   bool lazy_point_lists_ = false;  // with fill_point_lists_: fill them on MaterializePointLists() instead of inside StateEstimation —
                                    // the 14 MB device->host copy of the per-point covariances and the host loops over the scan
                                    // only happen for callers that read the lists (LIVMapper's host-side UpdateVoxelMap does)
-  int last_status_ = 0;            // esikf_status of the last call (the reference's calls return void)
   int last_iters_ = 0;             // iterations executed by the last StateEstimation
-  std::string last_error_;
 
   VoxelMapManager(VoxelMapConfig &config_setting, VoxelMap &voxel_map, int device = 0);
   ~VoxelMapManager();
@@ -318,7 +331,7 @@ struct ScoredPoint {
   double normal[3];
 };
 
-class VIOManager {
+class VIOManager : public CallStatus {
  public:
   StatesGroup *state = nullptr, *state_propagat = nullptr;  // raw pointers into LIVMapper (LIVMapper.cpp:135-136)
   SubSparseMap *visual_submap = nullptr;
@@ -335,14 +348,12 @@ class VIOManager {
   // reads it and ncc_en stays false); 0 here, which rejects only anti-correlated patches when ncc_en is set.
   bool normal_en = true, ncc_en = false;
   double outlier_threshold = 1000, ncc_thre = 0;
-  int last_status_ = 0;
   int last_total_iters_ = 0;  // iterations executed by the last computeJacobianAndUpdateEKF
   int64_t submap_uploads_ = 0;  // sub-map uploads (esikf_vio_set_patches) made by computeJacobianAndUpdateEKF
   // The per-patch mirrors below are called once per point and level by the reference's retrieval code: the image they are
   // handed is uploaded only when it is not the one of the previous call (same pixel pointer and size). A caller that rewrites
   // the pixels in place calls InvalidatePatchImages().
   void InvalidatePatchImages() { patch_img_ = patch_ref_img_ = nullptr; }
-  std::string last_error_;
 
   explicit VIOManager(esikf_ctx *shared_ctx);  // shares the device context (and stream) of the VoxelMapManager
   void initializeVIO();                         // src/vio.cpp:41-160 (the parts the update needs)
