@@ -15,6 +15,7 @@
 #include <vector>
 
 #include "esikf_dev.cuh"
+#include "scratch_layout.hpp"
 
 // single translation unit: the kernels are included so the whole library builds with one nvcc invocation
 #include "esikf_lio.cu"
@@ -332,17 +333,7 @@ static int fail(esikf_ctx *c, int code, const char *fmt, ...) {
     if (e__ != cudaSuccess) return fail(ctx, ESIKF_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e__), __FILE__, __LINE__); \
   } while (0)
 
-// One call's scratch block: `lay` takes each sub-array of the call from a ScratchLayout, 256-byte aligned. It runs once with
-// base 0 to size the block and, after the one reserve (which discards the old contents), again to hand out the pointers.
-struct ScratchLayout {
-  uintptr_t base = 0;
-  size_t bytes = 0;
-  template <typename T> T *take(size_t n) {
-    T *p = reinterpret_cast<T *>(base + bytes);
-    bytes += (n * sizeof(T) + 255) & ~(size_t)255;
-    return p;
-  }
-};
+// the device scratch of ctx laid out by `lay` (scratch_layout.hpp)
 template <typename F> static cudaError_t lay_out_scratch(esikf_ctx *ctx, F &&lay) {
   ScratchLayout s;
   lay(s);

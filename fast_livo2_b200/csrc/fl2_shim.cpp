@@ -1,6 +1,7 @@
 // fl2_shim.cpp — see fl2_shim.hpp. Host C++ only (no CUDA here): fills the reference-shaped member fields from / into
 // the packed buffers of the C ABI (libesikf_b200.so, resolved at load time through the dynamic linker).
 #include "fl2_shim.hpp"
+#include "scratch_layout.hpp"
 
 #include <omp.h>
 
@@ -28,6 +29,25 @@ static void par_memcpy(void *dst, const void *src, size_t bytes) {
     const size_t off = (size_t)c * chunk;
     memcpy(static_cast<char *>(dst) + off, static_cast<const char *>(src) + off, bytes - off < chunk ? bytes - off : chunk);
   }
+}
+
+// A manager's calls stage their inputs and answers in its one pinned block (scratch_layout.hpp), so no method may return with
+// a copy from it queued. On success each ends in a synchronising call: the fetch of esikf_lio_update / esikf_vio_update /
+// esikf_vio_run, the error check of the map updates, esikf_rgb_set_cloud, the export, or the front-end call itself. The
+// exceptions are the early successful returns of the calls that upload a packed state (rgb_state in esikf_api.cu):
+// GenerateVisualMapPoints at 10 points or fewer and ColorizeFrameWorld of an empty cloud (UpdateVisualMapPoints returns
+// before update_points at no entries). They leave that upload queued into a device copy that every reader rewrites in stream
+// order first, so what the block then holds is never read. esikf_lio_set_scan, esikf_vio_set_image and
+// esikf_vio_set_patches return with their copies queued and a call failing part-way may skip its synchronisation, so Record
+// drains the stream on every error; the first attempt of a grow-and-call-again loop fails only after its call synchronised.
+template <typename F> static bool lay_out_staging(PinnedBuf<uint8_t> &block, F &&lay) {
+  ScratchLayout s;
+  lay(s);
+  uint8_t *p = block.get(s.bytes);
+  if (!p && s.bytes) return false;
+  s = ScratchLayout{(uintptr_t)p};
+  lay(s);
+  return true;
 }
 
 StatesGroup::StatesGroup() {
@@ -267,13 +287,14 @@ void VoxelMapManager::UpdateMirror() {
     last_error_ = "the host mirror of the device map is void since an earlier call failed: EnableDeviceMap() and BuildVoxelMap() rebuild it";
     return;
   }
-  // one export call into grow-only pinned buffers sized by the ticks before; a second one only when they are too small
+  // one export call into room sized by the ticks before; a second one only when that is too small
   int32_t nr = 0, nn = 0;
+  int64_t *keys; int32_t *first, *count; esikf_map_node *nodes;
   for (int attempt = 0; attempt < 2; attempt++) {
-    int64_t *keys = exp_keys_.get(3 * (size_t)exp_roots_cap_);
-    int32_t *first = exp_first_.get(exp_roots_cap_), *count = exp_count_.get(exp_roots_cap_);
-    esikf_map_node *nodes = exp_nodes_.get(exp_nodes_cap_);
-    if (!keys || !first || !count || !nodes) {
+    auto lay = [&](ScratchLayout &s) {
+      keys = s.take<int64_t>(3 * exp_roots_cap_), first = s.take<int32_t>(exp_roots_cap_), count = s.take<int32_t>(exp_roots_cap_), nodes = s.take<esikf_map_node>(exp_nodes_cap_);
+    };
+    if (!lay_out_staging(block_, lay)) {
       StagingFailed();
       return InvalidateMirror();
     }
@@ -282,7 +303,7 @@ void VoxelMapManager::UpdateMirror() {
     exp_roots_cap_ = nr + nr / 4 + 64, exp_nodes_cap_ = nn + nn / 4 + 64;  // too small: grow and export again
   }
   if (Record(ctx_, last_status_)) return InvalidateMirror();
-  if (!ApplyMapExport(voxel_map_, config_setting_, exp_keys_.data(), exp_first_.data(), exp_count_.data(), nr, exp_nodes_.data(), nn, &last_error_)) {
+  if (!ApplyMapExport(voxel_map_, config_setting_, keys, first, count, nr, nodes, nn, &last_error_)) {
     last_status_ = ESIKF_ERR_STATE;
     return InvalidateMirror();
   }
@@ -295,9 +316,8 @@ void VoxelMapManager::BuildVoxelMap() {
     return;
   }
   const int n = feats_down_size_;
-  float *pts = st_pts_.get((size_t)n * 3 + 4);
-  double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
-  if (!pts || !sbuf) return StagingFailed();
+  float *pts; double *sbuf;
+  if (!lay_out_staging(block_, [&](ScratchLayout &s) { pts = s.take<float>((size_t)n * 3 + 4), sbuf = s.take<double>(ESIKF_STATE_DOUBLES); })) return StagingFailed();
   if (n) par_memcpy(pts, &feats_down_body_[0].x, (size_t)n * 12);
   state_.pack(sbuf);
   if ((last_status_ = esikf_set_lidar_extrinsics(ctx_, extR_.m, extT_.v)) == 0 && (last_status_ = esikf_lio_set_scan(ctx_, pts, n)) == 0)
@@ -312,7 +332,8 @@ void VoxelMapManager::UpdateVoxelMap() {
     last_status_ = ESIKF_ERR_STATE, last_error_ = "UpdateVoxelMap(): EnableDeviceMap first";
     return;
   }
-  double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
+  double *sbuf;
+  if (!lay_out_staging(block_, [&](ScratchLayout &s) { sbuf = s.take<double>(ESIKF_STATE_DOUBLES); })) return StagingFailed();
   state_.pack(sbuf);  // _state == voxelmap_manager->state_ at this point of the tick (LIVMapper.cpp:371); 3 kB
   Record(ctx_, esikf_map_device_update(ctx_, sbuf));
   UpdateMirror();
@@ -323,15 +344,12 @@ void VoxelMapManager::SetWorldCloud(const std::vector<PointXYZ> *dense_scan) {
     last_status_ = ESIKF_ERR_STATE, last_error_ = "SetWorldCloud: no device context";
     return;
   }
-  double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
-  float *pts = dense_scan ? st_pts_.get(dense_scan->size() * 3 + 3) : nullptr;
-  if (!sbuf || (dense_scan && !pts)) return StagingFailed();
+  const int n = dense_scan ? (int)dense_scan->size() : 0;
+  double *sbuf; float *pts;
+  if (!lay_out_staging(block_, [&](ScratchLayout &s) { sbuf = s.take<double>(ESIKF_STATE_DOUBLES), pts = dense_scan ? s.take<float>((size_t)n * 3 + 3) : nullptr; }))
+    return StagingFailed();
   state_.pack(sbuf);  // _state == state_ after StateEstimation (LIVMapper.cpp:371)
-  int n = 0;
-  if (dense_scan) {
-    n = (int)dense_scan->size();
-    for (int i = 0; i < n; i++) pts[3 * i] = (*dense_scan)[i].x, pts[3 * i + 1] = (*dense_scan)[i].y, pts[3 * i + 2] = (*dense_scan)[i].z;
-  }
+  for (int i = 0; i < n; i++) pts[3 * i] = (*dense_scan)[i].x, pts[3 * i + 1] = (*dense_scan)[i].y, pts[3 * i + 2] = (*dense_scan)[i].z;
   Record(ctx_, esikf_rgb_set_cloud(ctx_, pts, n, sbuf));
 }
 
@@ -344,11 +362,9 @@ void VoxelMapManager::FindCorrespond(int n, const V3D *pts, int rule, uint8_t *s
     last_status_ = ESIKF_ERR_ARG, last_error_ = "FindCorrespond: bad argument";
     return;
   }
-  double *p = st_find_pts_.get((size_t)n * 3 + 3);
-  uint8_t *st = st_find_status_.get((size_t)n + 1);
-  int64_t *keys = st_find_keys_.get((size_t)n * 3 + 3);
-  esikf_plane *rows = st_find_rows_.get((size_t)n + 1);
-  if (!p || !st || !keys || !rows) return StagingFailed();
+  double *p; int64_t *keys; uint8_t *st; esikf_plane *rows;
+  auto lay = [&](ScratchLayout &s) { p = s.take<double>(3 * n + 3), st = s.take<uint8_t>(n + 1), keys = s.take<int64_t>(3 * n + 3), rows = s.take<esikf_plane>(n + 1); };
+  if (!lay_out_staging(block_, lay)) return StagingFailed();
   for (int i = 0; i < n; i++)
     for (int k = 0; k < 3; k++) p[3 * i + k] = pts[i][k];
   if (Record(ctx_, esikf_map_device_find(ctx_, p, n, rule, st, keys, rows))) return;
@@ -401,9 +417,8 @@ void VoxelMapManager::UpdateVoxelMap(const std::vector<pointWithVar> &input_poin
     return;
   }
   const size_t n = input_points.size();
-  double *buf = st_cov_.get(n * 12 + 2);
-  if (!buf) return StagingFailed();
-  double *pw = buf, *var = buf + n * 3;
+  double *pw, *var;
+  if (!lay_out_staging(block_, [&](ScratchLayout &s) { pw = s.take<double>(n * 3 + 1), var = s.take<double>(n * 9 + 1); })) return StagingFailed();
   for (size_t i = 0; i < n; i++) {
     for (int k = 0; k < 3; k++) pw[3 * i + k] = input_points[i].point_w[k];
     memcpy(var + 9 * i, input_points[i].var.m, 72);
@@ -424,11 +439,11 @@ void VoxelMapManager::StateEstimation(StatesGroup &state_propagat) {
   cfg.voxel_size = config_setting_.max_voxel_size_, cfg.sigma_num = config_setting_.sigma_num_;
   cfg.dept_err = config_setting_.dept_err_, cfg.beam_err = config_setting_.beam_err_;
   cfg.max_layer = config_setting_.max_layer_, cfg.max_iterations = config_setting_.max_iterations_;
-  // every buffer that crosses PCIe is staged in page-locked memory owned by the manager (grow-only, no allocation per tick)
-  double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
-  float *pts = st_pts_.get((size_t)n * 3 + 4), *dis = st_dis_.get((size_t)n + 1);
+  double *sbuf;
+  float *pts, *dis = st_dis_.get((size_t)n + 1);
   int32_t *match = st_match_.get((size_t)n + 1), *normal = st_normal_.get((size_t)n + 1);
-  if (!sbuf || !pts || !dis || !match || !normal) return StagingFailed();
+  auto lay = [&](ScratchLayout &s) { sbuf = s.take<double>(3 * ESIKF_STATE_DOUBLES), pts = s.take<float>((size_t)n * 3 + 4); };
+  if (!dis || !match || !normal || !lay_out_staging(block_, lay)) return StagingFailed();
   double *sin = sbuf, *sprop = sbuf + ESIKF_STATE_DOUBLES, *sout = sbuf + 2 * ESIKF_STATE_DOUBLES;
   state_.pack(sin);
   state_propagat.pack(sprop);
@@ -451,20 +466,15 @@ void VoxelMapManager::MaterializePointLists() {
   const int n = feats_down_size_;
   const int32_t *match = st_match_.data(), *normal = st_normal_.data();
   const float *dis = st_dis_.data();
-  double *cov = st_cov_.get((size_t)n * 18 + 2);
-  if (!cov) return StagingFailed();
-  const double *bc = cov, *cm = cov + (size_t)n * 9;
-  if (Record(ctx_, esikf_lio_fetch_point_cov(ctx_, cov, cov + (size_t)n * 9))) return;
+  double *bc, *cm, *dev_normals = nullptr;
+  // with the device map no host VoxelPlane exists: pv.normal comes from the device records
+  auto lay = [&](ScratchLayout &s) { bc = s.take<double>(9 * n + 1), cm = s.take<double>(9 * n + 1), dev_normals = device_map_ ? s.take<double>(3 * n + 2) : nullptr; };
+  if (!lay_out_staging(block_, lay)) return StagingFailed();
+  if (Record(ctx_, esikf_lio_fetch_point_cov(ctx_, bc, cm))) return;
   body_cov_list_.resize(n), cross_mat_list_.resize(n);
   pv_list_.resize(n);
   ptpl_list_.clear();
-  const double *dev_normals = nullptr;
-  if (device_map_) {  // no host VoxelPlane exists: pv.normal comes from the device records
-    double *nb = st_normals_.get((size_t)n * 3 + 2);
-    if (!nb) return StagingFailed();
-    if (Record(ctx_, esikf_lio_fetch_normals(ctx_, nb))) return;
-    dev_normals = nb;
-  }
+  if (device_map_ && Record(ctx_, esikf_lio_fetch_normals(ctx_, dev_normals))) return;
   const double *R = state_.rot_end.m;
   for (int i = 0; i < n; i++) {
     memcpy(body_cov_list_[i].m, &bc[(size_t)i * 9], 72);
@@ -513,12 +523,19 @@ void VIOManager::GenerateVisualMapPoints(const std::vector<uint8_t> &type_map, i
     last_status_ = ESIKF_ERR_STATE, last_error_ = "GenerateVisualMapPoints: no device context or state";
     return;
   }
-  double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
-  if (!sbuf) return StagingFailed();
-  state->pack(sbuf);
   const size_t n = pg ? pg->size() : 0, m = add_from_voxel_map ? add_from_voxel_map->size() : 0;
-  gen_in_.resize(15 * n + 6 * m + 1);
-  double *pw = gen_in_.data(), *nv = pw + 3 * n, *var = nv + 3 * n, *ap = var + 9 * n, *an = ap + 3 * m;
+  const int cap = (int)type_map.size();  // at most one point per cell
+  double *sbuf, *pw, *nv, *var, *ap, *an, *pos, *pc, *normal, *pvar;
+  int32_t *src, *cell; float *score, *patch; uint8_t *cells;
+  auto lay = [&](ScratchLayout &s) {
+    sbuf = s.take<double>(ESIKF_STATE_DOUBLES), cells = s.take<uint8_t>(cap + 1);
+    pw = s.take<double>(3 * n + 1), nv = s.take<double>(3 * n + 1), var = s.take<double>(9 * n + 1), ap = s.take<double>(3 * m + 1), an = s.take<double>(3 * m + 1);
+    src = s.take<int32_t>(cap + 1), cell = s.take<int32_t>(cap + 1), pos = s.take<double>(3 * cap + 3), pc = s.take<double>(2 * cap + 2);
+    normal = s.take<double>(3 * cap + 3), pvar = s.take<double>(9 * cap + 9), score = s.take<float>(cap + 1), patch = s.take<float>(64 * cap + 64);
+  };
+  if (!lay_out_staging(block_, lay)) return StagingFailed();
+  state->pack(sbuf);
+  memcpy(cells, type_map.data(), cap);
   for (size_t i = 0; i < n; i++) {
     const pointWithVar &p = (*pg)[i];
     for (int k = 0; k < 3; k++) pw[3 * i + k] = p.point_w[k], nv[3 * i + k] = p.normal[k];
@@ -526,20 +543,16 @@ void VIOManager::GenerateVisualMapPoints(const std::vector<uint8_t> &type_map, i
   }
   for (size_t j = 0; j < m; j++)
     for (int k = 0; k < 3; k++) ap[3 * j + k] = (*add_from_voxel_map)[j].point_w[k], an[3 * j + k] = (*add_from_voxel_map)[j].normal[k];
-  const int cap = (int)type_map.size();  // at most one point per cell
-  gen_src_.resize(cap + 1), gen_cell_.resize(cap + 1), gen_pos_.resize(3 * cap + 3), gen_pc_.resize(2 * cap + 2), gen_normal_.resize(3 * cap + 3);
-  gen_var_.resize(9 * cap + 9), gen_score_.resize(cap + 1), gen_patch_.resize(64 * cap + 64);
   int32_t k = 0;
-  if (Record(ctx_, esikf_vio_generate_points(ctx_, pg ? pw : nullptr, nv, var, (int32_t)n, ap, an, (int32_t)m, type_map.data(), cap, grid_size, grid_n_width,
-                                             grid_n_height, border, sbuf, cap, &k, gen_src_.data(), gen_cell_.data(), gen_pos_.data(), gen_pc_.data(),
-                                             gen_score_.data(), gen_normal_.data(), gen_var_.data(), gen_patch_.data())))
+  if (Record(ctx_, esikf_vio_generate_points(ctx_, pg ? pw : nullptr, nv, var, (int32_t)n, ap, an, (int32_t)m, cells, cap, grid_size, grid_n_width, grid_n_height, border,
+                                             sbuf, cap, &k, src, cell, pos, pc, score, normal, pvar, patch)))
     return;
   new_points.resize(k);
   for (int i = 0; i < k; i++) {
     NewVisualPoint &q = new_points[i];
-    q.source = gen_src_[i], q.cell = gen_cell_[i], q.score = gen_score_[i];
-    memcpy(q.pos, &gen_pos_[3 * i], sizeof(q.pos)), memcpy(q.pc, &gen_pc_[2 * i], sizeof(q.pc)), memcpy(q.normal, &gen_normal_[3 * i], sizeof(q.normal));
-    memcpy(q.var, &gen_var_[9 * i], sizeof(q.var)), memcpy(q.patch, &gen_patch_[64 * i], sizeof(q.patch));
+    q.source = src[i], q.cell = cell[i], q.score = score[i];
+    memcpy(q.pos, pos + 3 * i, sizeof(q.pos)), memcpy(q.pc, pc + 2 * i, sizeof(q.pc)), memcpy(q.normal, normal + 3 * i, sizeof(q.normal));
+    memcpy(q.var, pvar + 9 * i, sizeof(q.var)), memcpy(q.patch, patch + 64 * i, sizeof(q.patch));
   }
 }
 
@@ -559,23 +572,24 @@ void VIOManager::UpdateVisualMapPoints(const std::vector<uint8_t> &converged, co
     last_status_ = ESIKF_ERR_ARG, last_error_ = "UpdateVisualMapPoints: converged / last_obs must have total_points entries";
     return;
   }
-  double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
-  if (!sbuf) return StagingFailed();
-  state->pack(sbuf);
   const size_t n = last_obs.size();
-  obs_in_.resize(14 * n + 1);
-  double *T = obs_in_.data(), *px = T + 12 * n;
+  double *sbuf, *T, *px, *pc; uint8_t *conv, *flag; int32_t *entry; float *patch;
+  auto lay = [&](ScratchLayout &s) {
+    sbuf = s.take<double>(ESIKF_STATE_DOUBLES), conv = s.take<uint8_t>(n), T = s.take<double>(12 * n), px = s.take<double>(2 * n);
+    flag = s.take<uint8_t>(n), entry = s.take<int32_t>(n + 1), pc = s.take<double>(2 * n + 2), patch = s.take<float>(64 * n + 64);
+  };
+  if (!lay_out_staging(block_, lay)) return StagingFailed();
+  state->pack(sbuf);
+  memcpy(conv, converged.data(), n);
   for (size_t i = 0; i < n; i++) memcpy(T + 12 * i, last_obs[i].T_f_w, sizeof(last_obs[i].T_f_w)), memcpy(px + 2 * i, last_obs[i].px, sizeof(last_obs[i].px));
-  obs_entry_.resize(n + 1), obs_pc_.resize(2 * n + 2), obs_patch_.resize(64 * n + 64);
   int32_t k = 0;
-  if (Record(ctx_, esikf_vio_update_points(ctx_, (int32_t)n, converged.data(), T, px, sbuf, (int32_t)n, &k, update_flag.data(), obs_entry_.data(),
-                                           obs_pc_.data(), obs_patch_.data())))
-    return;
+  if (Record(ctx_, esikf_vio_update_points(ctx_, (int32_t)n, conv, T, px, sbuf, (int32_t)n, &k, flag, entry, pc, patch))) return;
+  memcpy(update_flag.data(), flag, n);
   new_obs.resize(k);
   for (int i = 0; i < k; i++) {
     NewObservation &q = new_obs[i];
-    q.entry = obs_entry_[i];
-    memcpy(q.pc, &obs_pc_[2 * i], sizeof(q.pc)), memcpy(q.patch, &obs_patch_[64 * i], sizeof(q.patch));
+    q.entry = entry[i];
+    memcpy(q.pc, pc + 2 * i, sizeof(q.pc)), memcpy(q.patch, patch + 64 * i, sizeof(q.patch));
   }
 }
 
@@ -586,20 +600,19 @@ void VIOManager::RetrieveScanVoxels(int border, const std::vector<pointWithVar> 
     return;
   }
   const size_t n = pg ? pg->size() : 0;
-  double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES), *pw = st_ret_pt_.get(3 * n + 3);
-  if (!sbuf || !pw) return StagingFailed();
+  // room for one key per point of a host scan; for the resident scan a first call reports the count when the room is short
+  int32_t cap = pg ? (int32_t)n : (int32_t)(keys_cap_ > 0 ? keys_cap_ : 1 << 16), k = -1;
+  double *sbuf, *pw; int32_t *kb;
+  auto lay = [&](ScratchLayout &s) { sbuf = s.take<double>(ESIKF_STATE_DOUBLES), pw = s.take<double>(3 * n + 3), kb = s.take<int32_t>(3 * (size_t)cap + 3); };
+  if (!lay_out_staging(block_, lay)) return StagingFailed();
   state->pack(sbuf);
   for (size_t i = 0; i < n; i++)
     for (int k = 0; k < 3; k++) pw[3 * i + k] = (*pg)[i].point_w[k];
-  // room for one key per point of a host scan; for the resident scan a first call reports the count when the room is short
-  int32_t cap = pg ? (int32_t)n : (int32_t)(keys_cap_ > 0 ? keys_cap_ : 1 << 16), k = -1;
-  int32_t *kb = st_ret_keys_.get(3 * (size_t)cap + 3);
-  if (!kb) return StagingFailed();
   last_status_ = esikf_vio_retrieve_scan(ctx_, pg ? pw : nullptr, (int32_t)n, border, sbuf, cap, &k, kb, nullptr);
   if (last_status_ == ESIKF_ERR_ARG && !pg && k > cap) {
     cap = k, keys_cap_ = k;
-    kb = st_ret_keys_.get(3 * (size_t)cap + 3);
-    if (!kb) return StagingFailed();
+    if (!lay_out_staging(block_, lay)) return StagingFailed();
+    state->pack(sbuf);
     last_status_ = esikf_vio_retrieve_scan(ctx_, nullptr, 0, border, sbuf, cap, &k, kb, nullptr);
   }
   if (Record(ctx_, last_status_)) return;
@@ -617,9 +630,8 @@ void VIOManager::CheckDepthContinuity(int n, const double *pos, const double *pc
     last_status_ = n < 0 ? ESIKF_ERR_ARG : ESIKF_OK;
     return;
   }
-  double *cb = st_ret_cand_.get(5 * (size_t)n);
-  uint8_t *fb = st_ret_flag_.get((size_t)n);
-  if (!cb || !fb) return StagingFailed();
+  double *cb; uint8_t *fb;
+  if (!lay_out_staging(block_, [&](ScratchLayout &s) { cb = s.take<double>(5 * (size_t)n), fb = s.take<uint8_t>(n); })) return StagingFailed();
   memcpy(cb, pos, 3 * (size_t)n * sizeof(double)), memcpy(cb + 3 * (size_t)n, pc, 2 * (size_t)n * sizeof(double));
   if (Record(ctx_, esikf_vio_depth_check(ctx_, n, cb, cb + 3 * (size_t)n, fb))) return;
   memcpy(discontinuous.data(), fb, (size_t)n);
@@ -636,21 +648,21 @@ void VIOManager::ScoreReferencePatches(const std::vector<int32_t> &first, const 
     return;
   }
   const size_t n = pts.size(), m = obs.size();
-  double *d = st_rp_d_.get(6 * n + 12 * m + 1);  // pos 3n | normal 3n | T_f_w 12m
-  float *f = st_rp_f_.get(65 * m + 1);           // patch 64m | mean m
-  int32_t *k = st_rp_i_.get(n + 1 + m);          // first n + 1 | id m
-  if (!d || !f || !k) return StagingFailed();
+  double *d;  // pos 3n | normal 3n | T_f_w 12m, then by element type patch 64m | mean m | score m | mean_out m and first n + 1 | id m | ref n
+  float *f; int32_t *k;
+  if (!lay_out_staging(block_, [&](ScratchLayout &s) { d = s.take<double>(6 * n + 12 * m), f = s.take<float>(67 * m), k = s.take<int32_t>(2 * n + 1 + m); }))
+    return StagingFailed();
+  float *sc = f + 65 * m, *mu = f + 66 * m;
+  int32_t *rf = k + n + 1 + m;
+  if (n == 0) memset(sc, 0, 2 * m * sizeof(float));  // the call answers nothing: zero scores and means, as many as observations
   memcpy(k, first.data(), (n + 1) * sizeof(int32_t));
   for (size_t i = 0; i < n; i++) memcpy(d + 3 * i, pts[i].pos, sizeof(pts[i].pos)), memcpy(d + 3 * n + 3 * i, pts[i].normal, sizeof(pts[i].normal));
   for (size_t j = 0; j < m; j++) {
     memcpy(d + 6 * n + 12 * j, obs[j].T_f_w, sizeof(obs[j].T_f_w)), memcpy(f + 64 * j, obs[j].patch, sizeof(obs[j].patch));
     f[64 * m + j] = obs[j].mean, k[n + 1 + j] = obs[j].id;
   }
-  std::vector<float> sc(m), mu(m);
-  std::vector<int32_t> rf(n);
-  if (Record(ctx_, esikf_vio_score_ref_patches(ctx_, (int32_t)n, k, (int32_t)m, d, d + 3 * n, f, f + 64 * m, k + n + 1, d + 6 * n, sc.data(), mu.data(), rf.data())))
-    return;
-  score.swap(sc), mean.swap(mu), ref.swap(rf);
+  if (Record(ctx_, esikf_vio_score_ref_patches(ctx_, (int32_t)n, k, (int32_t)m, d, d + 3 * n, f, f + 64 * m, k + n + 1, d + 6 * n, sc, mu, rf))) return;
+  score.assign(sc, sc + m), mean.assign(mu, mu + m), ref.assign(rf, rf + n);
 }
 
 void VIOManager::initializeVIO() {
@@ -675,9 +687,8 @@ void VIOManager::computeJacobianAndUpdateEKF(const GrayImage &img) {
   const int n = total_points, L = patch_pyrimid_level;
   if (visual_submap == selected_submap_ && n == selected_count_) {
     // the sub-map SelectSubSparseMap installed is still on the device: image and states only
-    double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
-    float *err = st_err_.get(n);
-    if (!sbuf || !err) return StagingFailed();
+    double *sbuf; float *err;
+    if (!lay_out_staging(block_, [&](ScratchLayout &s) { sbuf = s.take<double>(3 * ESIKF_STATE_DOUBLES), err = s.take<float>(n); })) return StagingFailed();
     double *sin = sbuf, *sprop = sbuf + ESIKF_STATE_DOUBLES, *sout = sbuf + 2 * ESIKF_STATE_DOUBLES;
     state->pack(sin);
     state_propagat->pack(sprop);
@@ -692,11 +703,12 @@ void VIOManager::computeJacobianAndUpdateEKF(const GrayImage &img) {
     last_total_iters_ = stats.total_iters;
     return;
   }
-  double *pos = st_pos_.get((size_t)n * 3), *ie = st_ie_.get(n), *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
-  float *wp = st_wp_.get((size_t)n * 64 * L), *err = st_err_.get(n);
-  int32_t *sl = st_sl_.get(n);
-  uint8_t *im = st_img_.get((size_t)img.cols * img.rows);
-  if (!pos || !ie || !sbuf || !wp || !err || !sl || !im) return StagingFailed();
+  double *pos, *ie, *sbuf; float *wp, *err; int32_t *sl; uint8_t *im;
+  auto lay = [&](ScratchLayout &s) {
+    pos = s.take<double>((size_t)n * 3), ie = s.take<double>(n), sbuf = s.take<double>(3 * ESIKF_STATE_DOUBLES), wp = s.take<float>((size_t)n * 64 * L);
+    err = s.take<float>(n), sl = s.take<int32_t>(n), im = s.take<uint8_t>((size_t)img.cols * img.rows);
+  };
+  if (!lay_out_staging(block_, lay)) return StagingFailed();
   const SubSparseMap &sub = *visual_submap;
 #pragma omp parallel for num_threads(FL2_PACK_THREADS) schedule(static) if (n > 256)
   for (int i = 0; i < n; i++) {
@@ -752,9 +764,10 @@ void VIOManager::warpAffine(const double A_cur_ref[4], const GrayImage &img_ref,
     patch_ref_img_ = last_status_ ? nullptr : img_ref.data, patch_ref_w_ = img_ref.cols, patch_ref_h_ = img_ref.rows;
     ref_imgs_current_ = false;
   }
-  std::vector<float> all((size_t)64 * patch_pyrimid_level);
+  float *all;
+  if (!lay_out_staging(block_, [&](ScratchLayout &s) { all = s.take<float>(64 * patch_pyrimid_level); })) return StagingFailed();
   const int32_t idx = 0, sl = search_level;
-  if (!last_status_) last_status_ = esikf_vio_warp_affine(ctx_, 1, &idx, px_ref, A_cur_ref, &sl, all.data());
+  if (!last_status_) last_status_ = esikf_vio_warp_affine(ctx_, 1, &idx, px_ref, A_cur_ref, &sl, all);
   if (Record(ctx_, last_status_)) return;
   // a singular A leaves the patch untouched in the reference (vio.cpp:297-301); the kernel writes zeros into its own
   // scratch in that case, so only copy when A is invertible
@@ -762,7 +775,7 @@ void VIOManager::warpAffine(const double A_cur_ref[4], const GrayImage &img_ref,
   const double inv_det = 1.0 / det;
   const float inv00 = (float)(A_cur_ref[3] * inv_det);  // same expression as the kernel's A_ref_cur(0, 0)
   if (inv00 != inv00) return;
-  memcpy(patch + 64 * pyramid_level, all.data() + 64 * pyramid_level, sizeof(float) * 64);
+  memcpy(patch + 64 * pyramid_level, all + 64 * pyramid_level, sizeof(float) * 64);
 }
 
 void VIOManager::SetReferenceImages(const GrayImage *imgs, int n) {
@@ -782,15 +795,13 @@ void VIOManager::ColorizeFrameWorld(const BgrImage &img_rgb, double blind_rgb_po
     last_status_ = ESIKF_ERR_STATE, last_error_ = "ColorizeFrameWorld: no device context or state";
     return;
   }
-  double *sbuf = st_state_.get(3 * ESIKF_STATE_DOUBLES);
-  if (!sbuf) return StagingFailed();
-  state->pack(sbuf);
   int32_t kept = 0;
-  // the staging holds the largest coloured scan seen so far; a larger one is computed again into grown buffers
+  double *sbuf; float *xyz; uint8_t *bgr;
+  // room for the largest coloured scan seen so far; a larger one is computed again with more room
   for (int attempt = 0; attempt < 2; attempt++) {
-    float *xyz = st_rgb_xyz_.get((size_t)rgb_cap_ * 3 + 3);
-    uint8_t *bgr = st_rgb_bgr_.get((size_t)rgb_cap_ * 3 + 3);
-    if (!xyz || !bgr) return StagingFailed();
+    auto lay = [&](ScratchLayout &s) { sbuf = s.take<double>(ESIKF_STATE_DOUBLES), xyz = s.take<float>((size_t)rgb_cap_ * 3 + 3), bgr = s.take<uint8_t>((size_t)rgb_cap_ * 3 + 3); };
+    if (!lay_out_staging(block_, lay)) return StagingFailed();
+    state->pack(sbuf);
     last_status_ = esikf_rgb_colorize(ctx_, img_rgb.data, img_rgb.cols, img_rgb.rows, sbuf, blind_rgb_points, rgb_cap_, &kept, xyz, bgr, nullptr);
     if (last_status_ == ESIKF_ERR_ARG && kept > rgb_cap_) {
       rgb_cap_ = kept;
@@ -818,26 +829,29 @@ void VIOManager::SelectSubSparseMap(const SubMapCandidate *c, int n, const GrayI
   last_status_ = esikf_vio_set_image(ctx_, img.data, img.cols, img.rows);
   patch_img_ = last_status_ ? nullptr : img.data, patch_img_w_ = img.cols, patch_img_h_ = img.rows;
   const size_t N = (size_t)n;
-  std::vector<int32_t> idx(N), lvl(N), key(N), kept(N), sl(N);
-  std::vector<double> px(2 * N), f(3 * N), rp(3 * N), pw(3 * N), nw(3 * N), T(12 * N), ie(N), pc(2 * N), A(4 * N);
-  std::vector<float> err(N);
+  int32_t *idx, *lvl, *key, *kept, *sl;
+  double *px, *f, *rp, *pw, *nw, *T, *ie, *pc, *A; float *err;
+  auto lay = [&](ScratchLayout &s) {
+    idx = s.take<int32_t>(N), lvl = s.take<int32_t>(N), key = s.take<int32_t>(N), kept = s.take<int32_t>(N), sl = s.take<int32_t>(N);
+    px = s.take<double>(2 * N), f = s.take<double>(3 * N), rp = s.take<double>(3 * N), pw = s.take<double>(3 * N), nw = s.take<double>(3 * N);
+    T = s.take<double>(12 * N), ie = s.take<double>(N), pc = s.take<double>(2 * N), A = s.take<double>(4 * N), err = s.take<float>(N);
+  };
+  if (!lay_out_staging(block_, lay)) return StagingFailed();
   for (size_t i = 0; i < N; i++) {
     idx[i] = c[i].ref_img_index, lvl[i] = c[i].ref_level, key[i] = c[i].ref_key, ie[i] = c[i].ref_inv_expo;
-    memcpy(&px[2 * i], c[i].px_ref, 16), memcpy(&pc[2 * i], c[i].pc, 16), memcpy(&T[12 * i], c[i].T_ref_w, 96);
-    memcpy(&f[3 * i], c[i].ref_f, 24), memcpy(&rp[3 * i], c[i].ref_pos, 24), memcpy(&pw[3 * i], c[i].pos_w, 24), memcpy(&nw[3 * i], c[i].normal_w, 24);
+    memcpy(px + 2 * i, c[i].px_ref, 16), memcpy(pc + 2 * i, c[i].pc, 16), memcpy(T + 12 * i, c[i].T_ref_w, 96);
+    memcpy(f + 3 * i, c[i].ref_f, 24), memcpy(rp + 3 * i, c[i].ref_pos, 24), memcpy(pw + 3 * i, c[i].pos_w, 24), memcpy(nw + 3 * i, c[i].normal_w, 24);
   }
   esikf_vio_select_cfg cfg;
   cfg.normal_en = normal_en ? 1 : 0, cfg.ncc_en = ncc_en ? 1 : 0, cfg.ncc_thre = ncc_thre, cfg.outlier_threshold = outlier_threshold;
   int32_t nk = 0;
   if (!last_status_)
-    last_status_ = esikf_vio_select_patches(ctx_, n, idx.data(), px.data(), lvl.data(), f.data(), rp.data(), pw.data(), nw.data(), T.data(), ie.data(),
-                                            key.data(), pc.data(), T_cur_w, state->inv_expo_time, &cfg, &nk, kept.data(), err.data(), sl.data(), A.data(),
-                                            nullptr);
+    last_status_ = esikf_vio_select_patches(ctx_, n, idx, px, lvl, f, rp, pw, nw, T, ie, key, pc, T_cur_w, state->inv_expo_time, &cfg, &nk, kept, err, sl, A, nullptr);
   if (Record(ctx_, last_status_)) return;
   SubSparseMap &sub = *visual_submap;  // :765-770, in candidate order
-  sub.voxel_points_pos.resize(nk), sub.search_levels.assign(sl.begin(), sl.begin() + nk), sub.errors.assign(err.begin(), err.begin() + nk);
-  sub.inv_expo_list.resize(nk), sub.candidate_index.assign(kept.begin(), kept.begin() + nk), sub.warp_patch.clear();
-  sel_ref_idx_.resize(nk), sel_sl_.assign(sl.begin(), sl.begin() + nk), sel_px_.resize(2 * (size_t)nk), sel_A_.assign(A.begin(), A.begin() + 4 * (size_t)nk);
+  sub.voxel_points_pos.resize(nk), sub.search_levels.assign(sl, sl + nk), sub.errors.assign(err, err + nk);
+  sub.inv_expo_list.resize(nk), sub.candidate_index.assign(kept, kept + nk), sub.warp_patch.clear();
+  sel_ref_idx_.resize(nk), sel_sl_.assign(sl, sl + nk), sel_px_.resize(2 * (size_t)nk), sel_A_.assign(A, A + 4 * (size_t)nk);
   for (int j = 0; j < nk; j++) {
     const SubMapCandidate &k = c[kept[j]];
     for (int a = 0; a < 3; a++) sub.voxel_points_pos[j][a] = k.pos_w[a];
@@ -858,11 +872,12 @@ void VIOManager::MaterializeWarpPatches() {
     SetReferenceImages(imgs.data(), (int)imgs.size());
   }
   // the same kernel on the same matrices, levels and reference pixels as the selection: the patches the device holds
-  std::vector<float> wp((size_t)nk * 64 * L);
-  if (!last_status_) last_status_ = esikf_vio_warp_affine(ctx_, nk, sel_ref_idx_.data(), sel_px_.data(), sel_A_.data(), sel_sl_.data(), wp.data());
+  float *wp;
+  if (!lay_out_staging(block_, [&](ScratchLayout &s) { wp = s.take<float>((size_t)nk * 64 * L); })) return StagingFailed();
+  if (!last_status_) last_status_ = esikf_vio_warp_affine(ctx_, nk, sel_ref_idx_.data(), sel_px_.data(), sel_A_.data(), sel_sl_.data(), wp);
   if (Record(ctx_, last_status_)) return;
   visual_submap->warp_patch.resize(nk);
-  for (int j = 0; j < nk; j++) visual_submap->warp_patch[j].assign(wp.begin() + (size_t)j * 64 * L, wp.begin() + (size_t)(j + 1) * 64 * L);
+  for (int j = 0; j < nk; j++) visual_submap->warp_patch[j].assign(wp + (size_t)j * 64 * L, wp + (size_t)(j + 1) * 64 * L);
 }
 
 }  // namespace fl2b200

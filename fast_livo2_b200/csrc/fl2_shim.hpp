@@ -143,8 +143,8 @@ bool ApplyMapExport(VoxelMap &map, const VoxelMapConfig &cfg, const int64_t *key
 void EraseRootsOutside(VoxelMap &map, const int64_t lo[3], const int64_t hi[3]);
 void ClearVoxelMap(VoxelMap &map);
 
-// Grow-only page-locked host buffer (esikf_host_alloc): the staging areas the shim hands to the C ABI, so that every
-// per-tick copy is a DMA from / into pinned memory instead of a driver-staged pageable copy.
+// Grow-only page-locked host buffer (esikf_host_alloc): what the shim hands to the C ABI, so that every per-tick copy is a
+// DMA from / into pinned memory instead of a driver-staged pageable copy. Growing discards the contents.
 template <typename T> class PinnedBuf {
  public:
   PinnedBuf() = default;
@@ -167,19 +167,22 @@ template <typename T> class PinnedBuf {
   size_t cap_ = 0;
 };
 
-// The outcome of a manager's last call (the reference's calls return void): an esikf_status, and the message when it failed.
+// The outcome of a manager's last call (the reference's calls return void): an esikf_status, and the message when it failed;
+// and the pinned block the manager's calls stage through.
 struct CallStatus {
   int last_status_ = 0;
   std::string last_error_;
 
  protected:
-  // records the esikf_* return code of a call on ctx, with the context's message when it is an error; returns the code
-  int Record(const esikf_ctx *ctx, int status) {
+  // records the esikf_* return code of a call on ctx, with the context's message when it is an error; returns the code. A
+  // failed call may leave a copy from the manager's pinned block queued, so an error also drains the stream (fl2_shim.cpp).
+  int Record(esikf_ctx *ctx, int status) {
     last_status_ = status;
-    if (status) last_error_ = esikf_last_error(ctx);
+    if (status) last_error_ = esikf_last_error(ctx), esikf_synchronize(ctx);
     return status;
   }
   void StagingFailed() { last_status_ = ESIKF_ERR_CUDA, last_error_ = "pinned staging allocation failed"; }
+  PinnedBuf<uint8_t> block_;  // every call's inputs and answers, laid out per call (lay_out_staging); nothing is kept across calls
 };
 
 class VoxelMapManager : public CallStatus {
@@ -243,23 +246,16 @@ class VoxelMapManager : public CallStatus {
 
  private:
   esikf_ctx *ctx_ = nullptr;
-  FlatVoxelMap flat_;
+  FlatVoxelMap flat_;  // the host map as the device holds it: SyncDeviceMap diffs against it, MaterializePointLists reads its planes
   bool map_synced_ = false, device_has_map_ = false;
-  PinnedBuf<float> st_pts_, st_dis_;
+  // the association of the last StateEstimation, which a lazy MaterializePointLists reads after the calls in between
   PinnedBuf<int32_t> st_match_, st_normal_;
-  PinnedBuf<double> st_state_, st_cov_, st_normals_;
+  PinnedBuf<float> st_dis_;
   bool lists_pending_ = false;
   // the host mirror: export of the last device build / update applied to voxel_map_ (cleared when either fails)
   void UpdateMirror();
   void InvalidateMirror();
-  PinnedBuf<int64_t> exp_keys_;
-  PinnedBuf<int32_t> exp_first_, exp_count_;
-  PinnedBuf<esikf_map_node> exp_nodes_;
-  PinnedBuf<double> st_find_pts_;  // FindCorrespond's points and answers
-  PinnedBuf<uint8_t> st_find_status_;
-  PinnedBuf<int64_t> st_find_keys_;
-  PinnedBuf<esikf_plane> st_find_rows_;
-  int32_t exp_roots_cap_ = 1024, exp_nodes_cap_ = 4096;  // what the export buffers are requested with (grown from the ticks seen)
+  int32_t exp_roots_cap_ = 1024, exp_nodes_cap_ = 4096;  // what the export is requested with (grown from the ticks seen)
 };
 
 // include/vio.h:26-57 restated over flat storage
@@ -418,33 +414,14 @@ class VIOManager : public CallStatus {
   const uint8_t *patch_img_ = nullptr, *patch_ref_img_ = nullptr;  // what the per-patch helpers uploaded last
   int patch_img_w_ = 0, patch_img_h_ = 0, patch_ref_w_ = 0, patch_ref_h_ = 0;
   esikf_ctx *ctx_ = nullptr;
-  PinnedBuf<double> st_pos_, st_ie_, st_state_;
-  PinnedBuf<float> st_wp_, st_err_;
-  PinnedBuf<int32_t> st_sl_;
-  PinnedBuf<uint8_t> st_img_;
   // the sub-map SelectSubSparseMap left on the device, and what MaterializeWarpPatches needs to rebuild its patches
   const SubSparseMap *selected_submap_ = nullptr;
   int selected_count_ = -1;
   std::vector<int32_t> sel_ref_idx_, sel_sl_;
   std::vector<double> sel_px_, sel_A_;
   std::vector<GrayImage> ref_imgs_;  // SetReferenceImages (the caller keeps the pixels, as Feature::img_ does)
-  PinnedBuf<float> st_rgb_xyz_;      // ColorizeFrameWorld's output staging, grown to the largest coloured scan seen
-  PinnedBuf<uint8_t> st_rgb_bgr_;
-  int32_t rgb_cap_ = 0;
-  std::vector<double> gen_in_;       // GenerateVisualMapPoints' host pg / add_from, packed
-  std::vector<int32_t> gen_src_, gen_cell_;
-  std::vector<double> gen_pos_, gen_pc_, gen_normal_, gen_var_;
-  std::vector<float> gen_score_, gen_patch_;
-  std::vector<double> obs_in_, obs_pc_;  // UpdateVisualMapPoints' last observations (T | px) and the added entries' pc
-  std::vector<int32_t> obs_entry_;
-  std::vector<float> obs_patch_;
-  PinnedBuf<double> st_ret_pt_, st_ret_cand_;  // RetrieveScanVoxels' host scan, CheckDepthContinuity's pos | pc
-  PinnedBuf<int32_t> st_ret_keys_;
-  PinnedBuf<uint8_t> st_ret_flag_;
-  int32_t keys_cap_ = 0;  // the resident scan's largest key count seen
-  PinnedBuf<double> st_rp_d_;  // ScoreReferencePatches' inputs by element type: pos | normal | T_f_w, patch | mean, first | id
-  PinnedBuf<float> st_rp_f_;
-  PinnedBuf<int32_t> st_rp_i_;
+  int32_t rgb_cap_ = 0;              // ColorizeFrameWorld's answers are requested with room for the largest coloured scan seen
+  int32_t keys_cap_ = 0;             // the resident scan's largest key count seen
   bool ref_imgs_current_ = false;    // false once the per-patch warpAffine replaced the device's reference images
 };
 
