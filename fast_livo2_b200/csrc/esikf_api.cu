@@ -167,7 +167,7 @@ struct esikf_ctx {
   DevBuf<unsigned int> barrier;          // LIO kernel: two grid barriers {counter @ +0, release word @ +128 B}, 256 B apart; launches alternate
   DevBuf<unsigned long long> grid_mbox;  // VIO kernel: the grid mailbox (grid_mbox_words), then the exchange counter
   unsigned int *exchange_seq = nullptr;  // device word: exchanges executed so far (the tag of both mailboxes follows it)
-  DevBuf<unsigned long long> stamps;  // 8 per slot: 8 LIO slots then 64 VIO slots
+  DevBuf<unsigned long long> stamps;  // 8 per slot: 8 LIO slots then 64 VIO slots; debug, LIO per-CTA; the VIO chain stamps
   bool want_stamps = false;
   esikf_extrinsics ext{};
   bool have_ext = false, have_ext_dev = false;
@@ -434,7 +434,7 @@ int esikf_create(esikf_ctx **out, int device) {
             ctx->ctl_block.reserve(sizeof(esikf_lio_stats) + sizeof(Ctrl) + 64 + sizeof(esikf_vio_stats)) == cudaSuccess && ctx->ext_dev.reserve(12) == cudaSuccess &&
             ctx->scratch_state.reserve(S_N) == cudaSuccess;
   ctx->partial_blocks = ctx->sm_count < 160 ? ctx->sm_count : 160;  // persistent residual kernels: one CTA per SM
-  ok = ok && ctx->partials.reserve((size_t)2 * ctx->partial_blocks * NE_MAX) == cudaSuccess && ctx->stamps.reserve(8 * 72 + 64 + 160) == cudaSuccess &&
+  ok = ok && ctx->partials.reserve((size_t)2 * ctx->partial_blocks * NE_MAX) == cudaSuccess && ctx->stamps.reserve(800 + ESIKF_VIO_CHAIN_STAMP_WORDS) == cudaSuccess &&
        ctx->barrier.reserve(128) == cudaSuccess && ctx->grid_mbox.reserve(grid_mbox_words(ctx->partial_blocks) + 1) == cudaSuccess &&
        ctx->lio_slot_block.reserve((size_t)ctx->partial_blocks * LIO_L2_WARPS * 32 * SLOT_D) == cudaSuccess;
   if (ok) cudaMemsetAsync(ctx->barrier.p, 0, 128 * sizeof(unsigned int), ctx->stream);
@@ -1446,6 +1446,11 @@ int esikf_vio_run(esikf_ctx *ctx, const double *state_in, const double *state_pr
     }
     const void *fn = inverse ? (const void *)vio_update_kernel<false, true> : (const void *)vio_update_kernel<false, false>;
     const void *fn_peer = inverse ? (const void *)vio_update_kernel<true, true> : (const void *)vio_update_kernel<true, false>;
+    static_assert(VIO_CHAIN_CTA + VIO_CHAIN_MAX_CTAS * 64 == ESIKF_VIO_CHAIN_STAMP_WORDS, "VIO chain stamp layout");
+    if (ctx->want_stamps) {
+      ka.chain = ctx->stamps.p + 800;
+      CK(cudaMemsetAsync(ka.chain, 0, ESIKF_VIO_CHAIN_STAMP_WORDS * sizeof(unsigned long long), ctx->stream));
+    }
     return launch_persistent(ctx, fn, fn_peer, "vio_update_kernel", grid, VIO_THREADS, VIO_PERSIST_SMEM, &ka, sa, 64, 512, ctx->vio_timed, {&iv, tma});
   }
   ctx->vio_timed = ctx->timing;
@@ -2308,6 +2313,14 @@ int esikf_get_phase_stamps(esikf_ctx *ctx, uint64_t *out /* 800 */) {
   if (!ctx || !out) return ESIKF_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
   CK(cudaMemcpyAsync(out, ctx->stamps.p, 800 * sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  return ESIKF_OK;
+}
+
+int esikf_get_vio_chain_stamps(esikf_ctx *ctx, uint64_t *out) {
+  if (!ctx || !out) return ESIKF_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  CK(cudaMemcpyAsync(out, ctx->stamps.p + 800, ESIKF_VIO_CHAIN_STAMP_WORDS * sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   return ESIKF_OK;
 }

@@ -168,6 +168,15 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
 }
+// Measurement only: *p = %globaltimer once `v` has been computed (the clock read is predicated on a test of v, so it cannot
+// issue before v is ready), nothing when p is null.
+__device__ __forceinline__ void stamp_after(unsigned long long *p, double v) {
+  if (!p) return;
+  unsigned long long t;
+  asm volatile(
+      "{\n.reg .pred q;\nsetp.ne.b64 q, %1, 1;\n@q mov.u64 %0, %%globaltimer;\n@!q mov.u64 %0, 0;\n}" : "=l"(t) : "l"(__double_as_longlong(v)));
+  *p = t;
+}
 
 // A value of the update state: in global memory, written by an earlier launch (global), or the CTA's resident copy in shared
 // memory (persistent kernels).

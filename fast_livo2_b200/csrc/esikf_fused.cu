@@ -19,6 +19,12 @@
 namespace esikf {
 
 // Optional phase timestamps (ns, %globaltimer) written by CTA 0 / thread 0 — measurement only.
+// The VIO kernel's finer stamps (builds with ESIKF_VIO_CHAIN_STAMPS; VioKernelArgs::chain, 8 per (level, iteration) slot,
+// 64 slots; tools/vio_chain_timing.py): warp 0's first patch
+// (vio_process_range) at 8 slot + 0..3, every CTA's slice end (its partial summed) at VIO_CHAIN_CTA + VIO_CHAIN_MAX_CTAS slot
+// + blockIdx.x.
+#define VIO_CHAIN_CTA (8 * 64)
+#define VIO_CHAIN_MAX_CTAS 160
 __device__ __forceinline__ void stamp(unsigned long long *stamps, int &k) {
   if (stamps && blockIdx.x == 0 && threadIdx.x == 0) stamps[k] = globaltimer_ns();
   k++;
@@ -240,14 +246,16 @@ __device__ __forceinline__ unsigned int persist_prologue(FusedSolveSmem &fs, Sol
 
 // Exchange step of one iteration: warp 1 evaluates vec = state_propagat (-) state (voxel_map.cpp:470 / vio.cpp:1664) while
 // the CTA waits for the other CTAs; the fixed-order sum lands in fs.io.info and, with peers, is replaced by the rank-ordered
-// sum over the peer mailboxes. Ends with a CTA barrier. Phase stamp: this CTA sees every CTA's contribution.
+// sum over the peer mailboxes. Ends with a CTA barrier. Phase stamp: this CTA sees every CTA's contribution. cta_done
+// (grid mailbox, measurement only): when this CTA's partial was summed, at cta_done[blockIdx.x].
 //   grid mailbox (VIO): the CTA's tagged column, the reduce-scatter of the entries this CTA owns, the all-gather of the
 //                       totals;
 //   grid barrier (LIO): the CTA's column of `partials` (double-buffered by the launch's exchange count `epoch`), the
 //                       barrier, every CTA sums every column.
 template <int WARPS, int M, bool PEER>
 __device__ __forceinline__ void persist_exchange(FusedSolveSmem &fs, ReduceSmem<WARPS> &red, double D0, double D1, double cnt, const GridSync &gs, double *partials,
-                                                 int partial_stride, unsigned int &epoch, const PeerArgs &peer, unsigned int &seq, unsigned long long *stamps, int &sk) {
+                                                 int partial_stride, unsigned int &epoch, const PeerArgs &peer, unsigned int &seq, unsigned long long *stamps, int &sk,
+                                                 unsigned long long *cta_done = nullptr) {
   constexpr int NE = ne_of(M);
   const int tid = threadIdx.x, warp = tid >> 5, nb = gridDim.x;
   if constexpr (uses_grid_mailbox<M>()) {
@@ -255,6 +263,7 @@ __device__ __forceinline__ void persist_exchange(FusedSolveSmem &fs, ReduceSmem<
     unsigned long long *cols = gs.mbox + (seq & 1) * grid_mbox_cols_words(partial_stride);
     unsigned long long *totals = gs.mbox + 2 * grid_mbox_cols_words(partial_stride) + (seq & 1) * NE_MAX * 2;
     const double s = cta_partial<WARPS, M>(red, D0, D1, cnt);
+    if (cta_done && tid == 0) stamp_after(cta_done + blockIdx.x, s);
     if (tid < NE) st_tagged(cols + 2 * ((size_t)tid * partial_stride + blockIdx.x), s, tag);
     if (warp == 1) boxminus_warp(fs.io.pr, fs.io.st, fs.sm.vec, tid & 31);
     for (int e = blockIdx.x + warp * nb; e < NE; e += WARPS * nb) reduce_entry(cols + 2 * (size_t)e * partial_stride, nb, tag, totals + 2 * e, fs.wg);
@@ -374,6 +383,7 @@ __global__ void __launch_bounds__(VIO_THREADS, 1) vio_update_kernel(const VioKer
   for (int level = a.levels - 1; level >= 0; level--) {      // vio.cpp:790
     for (int it = 0; it < sa.max_iterations; it++) {          // :1536
       int sk = 8 * ((a.levels - 1 - level) * sa.max_iterations + it);
+      if (a.chain && threadIdx.x == 0) sm.stamp_slot = sk >> 3;
       stamp(stamps, sk);
       vio_load_consts(sm, a, fs.io.st, false);
       stamp(stamps, sk);
@@ -386,7 +396,12 @@ __global__ void __launch_bounds__(VIO_THREADS, 1) vio_update_kernel(const VioKer
         vio_process_range(a, sm, level, lo, hi, D0, D1, n_meas, cached, tma.enabled ? &tma : nullptr, &tma_phase);
       }
       stamp(stamps, sk);
-      persist_exchange<VIO_WARPS, 7, PEER>(fs, sm.red, D0, D1, n_meas, gs, a.partials, a.partial_stride, epoch, peer, seq, stamps, sk);
+#ifdef ESIKF_VIO_CHAIN_STAMPS
+      unsigned long long *const cta_done = a.chain ? a.chain + VIO_CHAIN_CTA + VIO_CHAIN_MAX_CTAS * (sk >> 3) : nullptr;
+#else
+      unsigned long long *const cta_done = nullptr;
+#endif
+      persist_exchange<VIO_WARPS, 7, PEER>(fs, sm.red, D0, D1, n_meas, gs, a.partials, a.partial_stride, epoch, peer, seq, stamps, sk, cta_done);
       stamp(stamps, sk);
       sa.level = level, sa.slot_iter = it;
       sa.dbg = (stamps && blockIdx.x == 0) ? stamps + sk + 1 : nullptr;  // 6: gain rows done, 7: boxplus done

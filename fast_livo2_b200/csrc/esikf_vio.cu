@@ -120,6 +120,7 @@ struct VioKernelArgs {
   int partial_stride;
   double *info;
   Ctrl *ctrl;
+  unsigned long long *chain;   // measurement only: the VIO chain stamps (esikf_get_vio_chain_stamps), null unless stamping
 };
 
 // raw img.data + offset reads of the reference, with 0 outside the buffer (the reference would read out of bounds there)
@@ -159,14 +160,20 @@ struct VioTma {
   int enabled;
 };
 
+// A warp's 64 rows [JdR Jdt cur res] are staged column by column, rows[warp][j][pixel], with the columns VIO_ROW_LD doubles
+// apart: a lane's two pixels of column j are one 16-byte store into 512 contiguous bytes, and a DMMA operand load (8 columns
+// x 4 pixels) spreads over all 32 banks. Row-major staging (64-byte rows, lanes 128 bytes apart) put every lane's stores on the
+// same four banks.
+#define VIO_ROW_LD 68
 struct __align__(128) VioSmem {
-  double rows[VIO_WARPS][64][8];  // first: double4 stores need 32-byte alignment
+  double rows[VIO_WARPS][8][VIO_ROW_LD];  // first: double2 stores need 16-byte alignment
   alignas(128) unsigned char tile[VIO_WARPS][VIO_TMA_TILE_BYTES];  // TMA landing area of a warp's footprint (u8 rows)
   unsigned long long tma_bar[VIO_WARPS];
   VioPatchCache cache[VIO_WARPS][VIO_KMAX];
   float grid[VIO_WARPS][104];     // 10 x 10 bilinear values: patch pixels plus a one-pixel ring for the central differences
   double Rcw[9], Pcw[3];
   double inv_expo;
+  int stamp_slot;                 // measurement only: the (level, iteration) slot a.chain stamps go to
   ReduceSmem<VIO_WARPS> red;
 };
 
@@ -236,6 +243,9 @@ __device__ __forceinline__ void vio_cache_reset(VioSmem &sm) {
 // Patch lo + warp + 16 k belongs to (warp, k). cached: the CTA's patches fit the per-warp cache (k < VIO_KMAX) and the
 // caller keeps `sm.cache` alive between calls (persistent kernel); otherwise slot 0 is plain scratch, refilled every time.
 // Divisions by the power-of-two tap stride are multiplications with its exact reciprocal (same quotient bit for bit).
+// Built with ESIKF_VIO_CHAIN_STAMPS and a.chain set (measurement only; the stamps cost the kernel registers, so the default
+// build leaves them out), thread 0 of CTA 0 stamps when its first patch finished the projection and tap
+// geometry, the Jacobian constants, the bilinear grid and the rows + DMMA contraction: a.chain[8 sm.stamp_slot + 0..3].
 __device__ __forceinline__ void vio_process_range(const VioKernelArgs &a, VioSmem &sm, int level, int lo, int hi, double &D0, double &D1,
                                                   double &n_meas, bool cached, const VioTma *tma = nullptr, unsigned *tma_phase = nullptr) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -246,6 +256,11 @@ __device__ __forceinline__ void vio_process_range(const VioKernelArgs &a, VioSme
   int k = 0;
   for (int lp = lo + warp; lp < hi; lp += VIO_WARPS, k++) {
     const int i = a.begin + lp;
+    const auto fine = [&](int n, double v) {
+#ifdef ESIKF_VIO_CHAIN_STAMPS
+      if (a.chain && k == 0 && blockIdx.x == 0 && tid == 0) stamp_after(a.chain + 8 * sm.stamp_slot + n, v);
+#endif
+    };
     VioPatchCache &c = sm.cache[warp][cached ? k : 0];
     const bool fill = !cached || !c.have;  // decisions on the shared slot are read first, acted on after a warp barrier
     __syncwarp();
@@ -269,6 +284,7 @@ __device__ __forceinline__ void vio_process_range(const VioKernelArgs &a, VioSme
     double pcu, pcv;
     world2cam(a.cam, pf0, pf1, pf2, pcu, pcv);
     const TapGeom tg = tap_geometry(pcu, pcv, pyramid_level);
+    fine(0, (double)tg.w_br);
 
     // the 11 x 11 tap footprint: tile (r, c) <-> image linear index base0 + r*scale*width + c*scale, where tile (1,1) is the
     // top-left tap of patch pixel (0,0) (:1597). Staged only when the footprint moved.
@@ -323,6 +339,7 @@ __device__ __forceinline__ void vio_process_range(const VioKernelArgs &a, VioSme
       WT[0][cc] = -sc * (J00 * sm.Rcw[cc] + J02 * sm.Rcw[6 + cc]);
       WT[1][cc] = -sc * (J11 * sm.Rcw[3 + cc] + J12 * sm.Rcw[6 + cc]);
     }
+    fine(1, WR[0][2] + WR[1][2] + WT[0][2] + WT[1][2]);
     if (restage) {
       if (by_tma) {
         mbar_wait(&sm.tma_bar[warp], *tma_phase & 1u);
@@ -357,6 +374,8 @@ __device__ __forceinline__ void vio_process_range(const VioKernelArgs &a, VioSme
     }
     __syncwarp();
     const float2 Pv = *reinterpret_cast<const float2 *>(&c.pv[2 * lane]);
+    fine(2, (double)sG[lane]);
+    double row[2][8];
 #pragma unroll
     for (int q = 0; q < 2; q++) {
       const int pix = 2 * lane + q;  // = x*8 + y
@@ -368,11 +387,12 @@ __device__ __forceinline__ void vio_process_range(const VioKernelArgs &a, VioSme
       const double cur_value = (double)gc[0];
       const double res = inv_expo * cur_value - inv_ref_expo * (double)(q == 0 ? Pv.x : Pv.y);
       const double ddu = (double)du, ddv = (double)dv;
-      double4 *dst = reinterpret_cast<double4 *>(&sm.rows[warp][pix][0]);
-      dst[0] = make_double4(ddu * WR[0][0] + ddv * WR[1][0], ddu * WR[0][1] + ddv * WR[1][1], ddu * WR[0][2] + ddv * WR[1][2],
-                            ddu * WT[0][0] + ddv * WT[1][0]);
-      dst[1] = make_double4(ddu * WT[0][1] + ddv * WT[1][1], ddu * WT[0][2] + ddv * WT[1][2], a.exposure_en ? cur_value : 0.0, res);
+#pragma unroll
+      for (int j = 0; j < 3; j++) row[q][j] = ddu * WR[0][j] + ddv * WR[1][j], row[q][3 + j] = ddu * WT[0][j] + ddv * WT[1][j];
+      row[q][6] = a.exposure_en ? cur_value : 0.0, row[q][7] = res;
     }
+#pragma unroll
+    for (int j = 0; j < 8; j++) *reinterpret_cast<double2 *>(&sm.rows[warp][j][2 * lane]) = make_double2(row[0][j], row[1][j]);
     n_meas += 64.0;
     __syncwarp();
     {
@@ -381,7 +401,7 @@ __device__ __forceinline__ void vio_process_range(const VioKernelArgs &a, VioSme
       double A0 = 0.0, A1 = 0.0, B0 = 0.0, B1 = 0.0, C0 = 0.0, C1 = 0.0, E0 = 0.0, E1 = 0.0;
 #pragma unroll
       for (int s = 0; s < 16; s += 4) {
-        const double v0 = sm.rows[warp][4 * s + t][g], v1 = sm.rows[warp][4 * s + 4 + t][g], v2 = sm.rows[warp][4 * s + 8 + t][g], v3 = sm.rows[warp][4 * s + 12 + t][g];
+        const double v0 = sm.rows[warp][g][4 * s + t], v1 = sm.rows[warp][g][4 * s + 4 + t], v2 = sm.rows[warp][g][4 * s + 8 + t], v3 = sm.rows[warp][g][4 * s + 12 + t];
         dmma_m8n8k4(A0, A1, v0, v0);
         dmma_m8n8k4(B0, B1, v1, v1);
         dmma_m8n8k4(C0, C1, v2, v2);
@@ -392,6 +412,7 @@ __device__ __forceinline__ void vio_process_range(const VioKernelArgs &a, VioSme
       // patch error (visual_submap->errors[i], :1632) = sum of the 64 squared residuals = element (7, 7) of the patch's block
       // (lane 31 holds it): fp64 sum narrowed to float, no separate reduction
       if (lane == 31) a.errors[i] = (float)p1;
+      fine(3, p0);
     }
     __syncwarp();
   }
@@ -814,9 +835,8 @@ __device__ __forceinline__ void vio_inverse_process_range(const VioKernelArgs &a
         row[3 + c] = t0 * Rwi[c] + t1 * Rwi[3 + c] + t2 * Rwi[6 + c];
       }
       row[6] = 0.0, row[7] = res;
-      double4 *dst = reinterpret_cast<double4 *>(&sm.rows[warp][pix][0]);
-      dst[0] = make_double4(row[0], row[1], row[2], row[3]);
-      dst[1] = make_double4(row[4], row[5], row[6], row[7]);
+#pragma unroll
+      for (int j = 0; j < 8; j++) sm.rows[warp][j][pix] = row[j];
       sq += res * res;
     }
 #pragma unroll
@@ -828,7 +848,7 @@ __device__ __forceinline__ void vio_inverse_process_range(const VioKernelArgs &a
       const int g = lane >> 2, t = lane & 3;
 #pragma unroll
       for (int s = 0; s < 16; s++) {
-        const double val = sm.rows[warp][4 * s + t][g];
+        const double val = sm.rows[warp][g][4 * s + t];
         dmma_m8n8k4(D0, D1, val, val);
       }
     }

@@ -538,6 +538,12 @@ int esikf_get_kernel_timing(esikf_ctx *ctx, float *lio_residual_ms /* 8 */, floa
  * slots 0..7 = LIO iterations, 8..71 = VIO (levels-1-level)*max_iterations + iteration. 0 = slot not executed. */
 int esikf_set_phase_stamps(esikf_ctx *ctx, int32_t enable);
 int esikf_get_phase_stamps(esikf_ctx *ctx, uint64_t *out /* 800: 576 phase stamps + 64 fine-grained debug stamps + 160 per-CTA slice-end stamps of LIO iteration 3 */);
+// The persistent VIO update's finer stamps of the last stamped update (ns, %globaltimer; 0 = not written: a library built
+// without ESIKF_VIO_CHAIN_STAMPS writes none), per (level,
+// iteration) slot s in the order of the phase stamps: [8 s + 0..3] CTA 0's warp 0, its first patch: projection and tap
+// geometry done, Jacobian constants done, bilinear grid done, rows contracted; [512 + 160 s + b] CTA b's partial summed.
+#define ESIKF_VIO_CHAIN_STAMP_WORDS (8 * 64 + 160 * 64)
+int esikf_get_vio_chain_stamps(esikf_ctx *ctx, uint64_t *out /* ESIKF_VIO_CHAIN_STAMP_WORDS */);
 
 #ifdef __cplusplus
 }
