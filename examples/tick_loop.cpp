@@ -43,6 +43,12 @@ int main() {
   vio_manager.cam.fx = vio_manager.cam.fy = 60.0, vio_manager.cam.cx = 32.0, vio_manager.cam.cy = 24.0;
   vio_manager.patch_pyrimid_level = 2;
   vio_manager.initializeVIO();
+  // the visual map's observations on the device (INTEGRATION.md §3): the sub-map's one entry is store point 0, observed once
+  // from the identity pose at its reference pixel; the host's VisualPoint / Feature objects mirror the store without patch_
+  vio_manager.EnableDeviceObservations(1 << 10);
+  std::vector<int32_t> store_ids;
+  vio_manager.AddVisualPoints({0, 1}, {StoredObservation{{32.0, 24.0}, {1, 0, 0, 0, 1, 0, 0, 0, 1, 0, 0, 0}, {}, 0, 0.0f, 0.0f}}, {-1}, store_ids);
+  std::printf("observation store: status %d, %zu points\n", vio_manager.last_status_, store_ids.size());
 
   // ---- first LiDAR frame (LIVMapper.cpp:356-366): the map is built from the scan at the initial pose
   voxelmap_manager.feats_down_body_ = floor_scan(1600, 1.0f);
@@ -142,6 +148,29 @@ int main() {
     std::vector<int32_t> ref;
     vio_manager.ScoreReferencePatches(std::vector<int32_t>{0, 6}, scored, obs, score, mean, ref);
     std::printf("tick %d reference patch: status %d, observation %d\n", tick, vio_manager.last_status_, ref.empty() ? -1 : ref[0]);
+    // the same three steps on the device's observation store: the new points join it, the sub-map entry's oldest observation
+    // is read and its list edited where it lies, and its patches are scored in place; the retrieval's reference feature of
+    // the entry (getCloseViewObs from the frame's position) is read from it too
+    std::vector<int32_t> first(new_points.size() + 1, 0), none(new_points.size(), -1), ids;
+    std::vector<StoredObservation> born(new_points.size());
+    for (size_t i = 0; i < new_points.size(); i++) {
+      StoredObservation &o = born[i];
+      memcpy(o.px, new_points[i].pc, sizeof(o.px)), memcpy(o.patch, new_points[i].patch, sizeof(o.patch));
+      const double T[12] = {1, 0, 0, 0, 1, 0, 0, 0, 1, 0, 0, 0};
+      memcpy(o.T_f_w, T, sizeof(T));
+      o.id = tick, o.mean = 0.0f, o.score = 0.0f;
+      first[i + 1] = (int32_t)i + 1;
+    }
+    vio_manager.AddVisualPoints(first, born, none, ids);
+    std::printf("tick %d store add: status %d, %zu points\n", tick, vio_manager.last_status_, ids.size());
+    std::vector<int32_t> sub_ids(vio_manager.total_points, store_ids.empty() ? 0 : store_ids[0]), evicted, count;
+    vio_manager.UpdateVisualMapPoints(sub_ids, converged, tick, update_flag, new_obs, evicted, count);
+    std::printf("tick %d store update: status %d, %zu new, count %d\n", tick, vio_manager.last_status_, new_obs.size(), count.empty() ? -1 : count[0]);
+    vio_manager.ScoreReferencePatches(std::vector<int32_t>(1, sub_ids.empty() ? 0 : sub_ids[0]), scored, ref);
+    std::printf("tick %d store reference patch: status %d, observation %d\n", tick, vio_manager.last_status_, ref.empty() ? -1 : ref[0]);
+    const double frame_pos[3] = {0.0, 0.0, 0.0};
+    vio_manager.ChooseReferenceFeatures(std::vector<int32_t>(1, 0), scored[0].pos, frame_pos, false, ref);
+    std::printf("tick %d store reference feature: status %d, observation %d\n", tick, vio_manager.last_status_, ref.empty() ? -1 : ref[0]);
   }
   // somebody wants the warp patches of the last selection on the host after all
   vio_manager.MaterializeWarpPatches();

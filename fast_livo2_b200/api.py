@@ -119,6 +119,13 @@ def load_library():
     lib.esikf_vio_retrieve_scan.argtypes = [vp, vp, C.c_int32, C.c_int32, vp, C.c_int32, ip, vp, vp]
     lib.esikf_vio_depth_check.argtypes = [vp, C.c_int32, vp, vp, vp]
     lib.esikf_vio_score_ref_patches.argtypes = [vp, C.c_int32, vp, C.c_int32] + [vp] * 9
+    lib.esikf_vmap_init.argtypes = [vp, C.c_int64]
+    lib.esikf_vmap_add_points.argtypes = [vp, C.c_int32, vp, C.c_int32] + [vp] * 8
+    lib.esikf_vmap_update_points.argtypes = [vp, C.c_int32, vp, vp, vp, C.c_int32, vp, C.c_int32, ip] + [vp] * 6
+    lib.esikf_vmap_score.argtypes = [vp, C.c_int32] + [vp] * 6
+    lib.esikf_vmap_choose_ref.argtypes = [vp, C.c_int32, vp, vp, vp, C.c_int32, vp]
+    lib.esikf_vmap_download.argtypes = [vp, C.c_int32, vp, C.c_int32] + [vp] * 8
+    lib.esikf_vmap_stats.argtypes = [vp, vp, vp]
     lib.esikf_comm_unique_id.argtypes = [C.c_char_p]
     lib.esikf_comm_init.argtypes = [vp, C.c_int32, C.c_int32, C.c_char_p]
     lib.esikf_comm_rank.argtypes = [vp, ip, ip]
@@ -157,7 +164,8 @@ EXPORTED_SYMBOLS = [
     "esikf_set_extrinsics", "esikf_set_lidar_extrinsics", "esikf_map_upload", "esikf_map_patch", "esikf_map_device_init", "esikf_map_device_build", "esikf_map_device_update", "esikf_map_device_update_points", "esikf_map_device_slide", "esikf_map_device_stats", "esikf_map_device_capacity", "esikf_map_device_download", "esikf_map_device_export", "esikf_map_device_find", "esikf_lio_fetch_normals", "esikf_lio_set_scan", "esikf_lio_run", "esikf_lio_fetch",
     "esikf_lio_update", "esikf_lio_fetch_point_cov", "esikf_vio_set_camera", "esikf_vio_set_image", "esikf_vio_set_patches",
     "esikf_vio_run", "esikf_vio_fetch", "esikf_vio_update", "esikf_vio_get_image_patch", "esikf_vio_set_ref_images",
-    "esikf_vio_warp_patches", "esikf_vio_select_patches", "esikf_vio_warp_affine", "esikf_vio_set_inverse_refs", "esikf_rgb_set_cloud", "esikf_rgb_colorize", "esikf_vio_generate_points", "esikf_vio_update_points", "esikf_vio_retrieve_scan", "esikf_vio_depth_check", "esikf_vio_score_ref_patches", "esikf_comm_unique_id", "esikf_comm_init", "esikf_comm_rank", "esikf_shard_range", "esikf_peer_export", "esikf_peer_attach", "esikf_profile_kernel", "esikf_set_kernel_timing", "esikf_get_kernel_timing", "esikf_set_phase_stamps", "esikf_get_phase_stamps",
+    "esikf_vio_warp_patches", "esikf_vio_select_patches", "esikf_vio_warp_affine", "esikf_vio_set_inverse_refs", "esikf_rgb_set_cloud", "esikf_rgb_colorize", "esikf_vio_generate_points", "esikf_vio_update_points", "esikf_vio_retrieve_scan", "esikf_vio_depth_check", "esikf_vio_score_ref_patches",
+    "esikf_vmap_init", "esikf_vmap_add_points", "esikf_vmap_update_points", "esikf_vmap_score", "esikf_vmap_choose_ref", "esikf_vmap_download", "esikf_vmap_stats", "esikf_comm_unique_id", "esikf_comm_init", "esikf_comm_rank", "esikf_shard_range", "esikf_peer_export", "esikf_peer_attach", "esikf_profile_kernel", "esikf_set_kernel_timing", "esikf_get_kernel_timing", "esikf_set_phase_stamps", "esikf_get_phase_stamps",
 ]
 
 
@@ -643,6 +651,93 @@ class Context:
                                                       mean.ctypes.data, id_.ctypes.data, T.ctypes.data, score.ctypes.data, mean_out.ctypes.data,
                                                       ref.ctypes.data))
         return dict(score=score[:m], mean=mean_out[:m], ref=ref[:n])
+
+    # ------------------------------------------------------------------ the visual map's observations on the device (K14)
+    def vmap_init(self, point_capacity):
+        """An empty observation store with room for point_capacity points (esikf_vmap_init); it grows by doubling."""
+        self._ck(self.lib.esikf_vmap_init(self.h, int(point_capacity)))
+
+    def vmap_stats(self):
+        """(points, capacity) of the observation store."""
+        pts, cap = C.c_int64(0), C.c_int64(0)
+        self._ck(self.lib.esikf_vmap_stats(self.h, C.byref(pts), C.byref(cap)))
+        return pts.value, cap.value
+
+    def vmap_add_points(self, first, px, patch, T_f_w, id, mean, score, ref):  # noqa: A002 (vmap_download's field names)
+        """Append n points (esikf_vmap_add_points): first (n + 1,) int32 offsets of each point's observations in obs_ order;
+        per observation px (m, 2) float64, patch (m, 64) float32, T_f_w (m, 12) float64, id (m,) int32, mean, score (m,)
+        float32; ref (n,) int32, the position of ref_patch or -1. Returns the new points' ids (n,) int32."""
+        first = _c(first, np.int32).reshape(-1)
+        n = len(first) - 1
+        px, patch, T = _c(px, np.float64).reshape(-1, 2), _c(patch, np.float32).reshape(-1, 64), _c(T_f_w, np.float64).reshape(-1, 12)
+        id_, mean, score, ref = _c(id, np.int32).reshape(-1), _c(mean, np.float32).reshape(-1), _c(score, np.float32).reshape(-1), _c(ref, np.int32).reshape(-1)
+        m = len(px)
+        assert n >= 0 and len(ref) == n and len(patch) == m and len(T) == m and len(id_) == m and len(mean) == m and len(score) == m
+        ids = np.zeros(max(n, 1), np.int32)
+        self._ck(self.lib.esikf_vmap_add_points(self.h, n, first.ctypes.data, m, px.ctypes.data, patch.ctypes.data, T.ctypes.data, id_.ctypes.data,
+                                                mean.ctypes.data, score.ctypes.data, ref.ctypes.data, ids.ctypes.data))
+        return ids[:n]
+
+    def vmap_update_points(self, point_id, converged, frame_id, T_f_w=None, state=None, cap=None):
+        """updateVisualMapPoints on the store (esikf_vmap_update_points) for the installed sub-map, entry i being store point
+        point_id[i]. T_f_w (12,): the new observations' T_f_w_, None for the frame pose of the flags; state: a packed state, or
+        None for the VIO posterior on the device. Returns vio_update_points' update_flag, entry, pc and patch, and per entry
+        evicted (the list position removed, or -1) and count (the count afterwards)."""
+        pid = _c(point_id, np.int32).reshape(-1)
+        conv = _c(converged, np.uint8).reshape(-1)
+        n = len(pid)
+        assert len(conv) == n
+        T = None if T_f_w is None else _c(T_f_w, np.float64).reshape(12)
+        s = None if state is None else _c(state, np.float64)
+        cap = n if cap is None else int(cap)
+        k = max(cap, 1)
+        flag, evicted, count = np.zeros(max(n, 1), np.uint8), np.zeros(max(n, 1), np.int32), np.zeros(max(n, 1), np.int32)
+        out = dict(entry=np.zeros(k, np.int32), pc=np.zeros((k, 2)), patch=np.zeros((k, 64), np.float32))
+        cnt = C.c_int32(0)
+        self._ck(self.lib.esikf_vmap_update_points(self.h, n, pid.ctypes.data, conv.ctypes.data, _addr(T), int(frame_id), _addr(s), cap, C.byref(cnt),
+                                                   flag.ctypes.data, *[out[f].ctypes.data for f in ("entry", "pc", "patch")], evicted.ctypes.data,
+                                                   count.ctypes.data))
+        return dict(update_flag=flag[:n], evicted=evicted[:n], count=count[:n], **{f: v[:cnt.value] for f, v in out.items()})
+
+    def vmap_score(self, point_id, pos, normal):
+        """The patch scoring of updateReferencePatch on the store (esikf_vmap_score): pos, normal (n, 3) float64 per entry.
+        Returns ref (n,) int32 (stored where >= 0) and the store's score and mean rows (n, 30) float32 afterwards."""
+        pid = _c(point_id, np.int32).reshape(-1)
+        n = len(pid)
+        pos, normal = _c(pos, np.float64).reshape(-1, 3), _c(normal, np.float64).reshape(-1, 3)
+        assert len(pos) == n and len(normal) == n
+        ref, score, mean = np.zeros(max(n, 1), np.int32), np.zeros((max(n, 1), 30), np.float32), np.zeros((max(n, 1), 30), np.float32)
+        self._ck(self.lib.esikf_vmap_score(self.h, n, pid.ctypes.data, pos.ctypes.data, normal.ctypes.data, ref.ctypes.data, score.ctypes.data,
+                                           mean.ctypes.data))
+        return dict(ref=ref[:n], score=score[:n], mean=mean[:n])
+
+    def vmap_choose_ref(self, point_id, normal_en, pos=None, frame_pos=None):
+        """The reference feature of the retrieval (esikf_vmap_choose_ref, vio.cpp:651-697): normal_en, or getCloseViewObs from
+        frame_pos (3,) with pos (n, 3). Returns ref (n,) int32, -1 where none is chosen."""
+        pid = _c(point_id, np.int32).reshape(-1)
+        n = len(pid)
+        p = None if pos is None else _c(pos, np.float64).reshape(-1, 3)
+        fp = None if frame_pos is None else _c(frame_pos, np.float64).reshape(3)
+        ref = np.zeros(max(n, 1), np.int32)
+        self._ck(self.lib.esikf_vmap_choose_ref(self.h, n, pid.ctypes.data, _addr(p), _addr(fp), int(bool(normal_en)), ref.ctypes.data))
+        return ref[:n]
+
+    def vmap_download(self, point_id):
+        """The lists of the given points (esikf_vmap_download), in vmap_add_points' form: first, px, patch, T_f_w, id, mean,
+        score, ref."""
+        pid = _c(point_id, np.int32).reshape(-1)
+        n = len(pid)
+        first = np.zeros(n + 1, np.int32)
+        rc = self.lib.esikf_vmap_download(self.h, n, pid.ctypes.data, 0, first.ctypes.data, *([None] * 6), np.zeros(max(n, 1), np.int32).ctypes.data)
+        if rc != 0 and first[n] == 0:
+            self._ck(rc)
+        m = int(first[n])
+        out = dict(px=np.zeros((max(m, 1), 2)), patch=np.zeros((max(m, 1), 64), np.float32), T_f_w=np.zeros((max(m, 1), 12)), id=np.zeros(max(m, 1), np.int32),
+                   mean=np.zeros(max(m, 1), np.float32), score=np.zeros(max(m, 1), np.float32))
+        ref = np.zeros(max(n, 1), np.int32)
+        self._ck(self.lib.esikf_vmap_download(self.h, n, pid.ctypes.data, m, first.ctypes.data, *[out[f].ctypes.data for f in ("px", "patch", "T_f_w", "id", "mean", "score")],
+                                              ref.ctypes.data))
+        return dict(first=first, ref=ref[:n], **{f: v[:m] for f, v in out.items()})
 
     # ------------------------------------------------------------------ multi-GPU / measurement
     def vio_set_inverse_refs(self, ref_img_index, ref_px, ref_f, ref_R, ref_pos):

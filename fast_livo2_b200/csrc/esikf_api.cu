@@ -29,6 +29,7 @@
 #include "esikf_retrieve.cu"
 #include "esikf_find.cu"
 #include "esikf_refpatch.cu"
+#include "esikf_vmap.cu"
 
 using namespace esikf;
 
@@ -276,6 +277,13 @@ struct esikf_ctx {
   double ret_Rci[9] = {}, ret_Pci[3] = {};
   int ret_w = 0, ret_h = 0;
   bool ret_valid = false;  // a depth image and its pose are in place (cleared by esikf_vio_set_camera and by a failed call)
+
+  // the visual map's observation store (esikf_vmap_*, esikf_vmap.cu): vmap_cap point records, the first vmap_points in use
+  DevBuf<uint8_t> vmap;
+  int64_t vmap_cap = 0, vmap_points = 0;
+  bool have_vmap = false;
+  std::vector<uint32_t> vmap_seen;  // per point, the last call (vmap_epoch) that named it: the repeated-id check in O(n)
+  uint32_t vmap_epoch = 0;
 
   // What the front-end entry points need for the length of one call only (lay_out_scratch). Every such call runs on `stream`
   // and synchronises it before it returns, so they can share it; nothing a later call reads may be kept here.
@@ -2150,14 +2158,350 @@ int esikf_vio_score_ref_patches(esikf_ctx *ctx, int32_t n, const int32_t *first,
     CK(cudaMemcpyAsync(d_mean, mean, M * sizeof(float), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_id, id, M * sizeof(int32_t), cudaMemcpyHostToDevice, st));
   }
-  a.first = d_first, a.pos = d_pos, a.normal = d_normal, a.T = d_T, a.patch = d_patch, a.mean = d_mean, a.id = d_id;
-  refpatch_score_kernel<<<(n + RP_WARPS - 1) / RP_WARPS, RP_WARPS * 32, 0, st>>>(a);
+  a.pos = d_pos, a.normal = d_normal, a.T = d_T, a.patch = d_patch, a.mean = d_mean, a.id = d_id;
+  refpatch_score_kernel<<<(n + RP_WARPS - 1) / RP_WARPS, RP_WARPS * 32, 0, st>>>(a, RpPacked{d_first});
   ctx->launches++;
   CK(cudaGetLastError());
   CK(read_back(ctx, a.score, a.ref + N));
   copy_out(ctx, score_out, a.score, a.score, 4 * M);
   copy_out(ctx, mean_out, a.score, a.mean_out, 4 * M);
   copy_out(ctx, ref_out, a.score, a.ref, 4 * N);
+  return ESIKF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------- visual map observation store
+static const int64_t VMAP_MAX_POINTS = (int64_t)1 << 26;  // every slot index p * 30 stays below 2^31
+
+static VmapView vmap_of(esikf_ctx *ctx) { return vmap_view(ctx->vmap.p, (size_t)ctx->vmap_cap); }
+
+// exactly `cap` point records into the empty b
+static cudaError_t vmap_alloc(DevBuf<uint8_t> &b, int64_t cap) {
+  uint8_t *p = nullptr;
+  const size_t bytes = vmap_bytes((size_t)cap);
+  const cudaError_t e = cudaMalloc(&p, bytes);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    return e;
+  }
+  b.p = p, b.cap = bytes;
+  return cudaSuccess;
+}
+
+// the point ids of one call: each in [0, points), none twice
+static int vmap_check_ids(esikf_ctx *ctx, int32_t n, const int32_t *point_id, const char *what) {
+  std::vector<uint32_t> &seen = ctx->vmap_seen;
+  if (seen.size() < (size_t)ctx->vmap_points) seen.resize((size_t)ctx->vmap_points, 0);
+  if (++ctx->vmap_epoch == 0) std::fill(seen.begin(), seen.end(), 0), ctx->vmap_epoch = 1;  // the epoch wrapped
+  const uint32_t e = ctx->vmap_epoch;
+  for (int32_t i = 0; i < n; i++) {
+    const int32_t p = point_id[i];
+    if (p < 0 || p >= ctx->vmap_points) return fail(ctx, ESIKF_ERR_ARG, "%s: point id %d outside [0, %lld)", what, p, (long long)ctx->vmap_points);
+    if (seen[p] == e) return fail(ctx, ESIKF_ERR_ARG, "%s: point id %d appears twice", what, p);
+    seen[p] = e;
+  }
+  return ESIKF_OK;
+}
+
+// Host inputs staged in the pinned block at their scratch offsets, then uploaded as the scratch's first in_bytes with one copy.
+struct VmapStage {
+  esikf_ctx *ctx;
+  void put(const void *dst, const void *src, size_t bytes) const {
+    if (bytes) memcpy(ctx->host.p + ((const uint8_t *)dst - ctx->scratch.p), src, bytes);
+  }
+};
+
+int esikf_vmap_init(esikf_ctx *ctx, int64_t point_capacity) {
+  if (!ctx || point_capacity < 1 || point_capacity > VMAP_MAX_POINTS) return fail(ctx, ESIKF_ERR_ARG, "vmap_init: capacity %lld outside [1, 2^26]", (long long)point_capacity);
+  CK(cudaSetDevice(ctx->device));
+  CK(cudaStreamSynchronize(ctx->stream));
+  ctx->have_vmap = false;
+  ctx->vmap = DevBuf<uint8_t>();
+  ctx->vmap_cap = ctx->vmap_points = 0;
+  ctx->vmap_seen.clear(), ctx->vmap_epoch = 0;
+  CK(vmap_alloc(ctx->vmap, point_capacity));
+  ctx->vmap_cap = point_capacity, ctx->have_vmap = true;
+  return ESIKF_OK;
+}
+
+int esikf_vmap_stats(esikf_ctx *ctx, int64_t *points, int64_t *capacity) {
+  if (!ctx || !points || !capacity) return fail(ctx, ESIKF_ERR_ARG, "vmap_stats: bad argument");
+  if (!ctx->have_vmap) return fail(ctx, ESIKF_ERR_STATE, "vmap_stats before esikf_vmap_init");
+  *points = ctx->vmap_points, *capacity = ctx->vmap_cap;
+  return ESIKF_OK;
+}
+
+int esikf_vmap_add_points(esikf_ctx *ctx, int32_t n, const int32_t *first, int32_t m, const double *px, const float *patch, const double *T_f_w,
+                          const int32_t *id, const float *mean, const float *score, const int32_t *ref, int32_t *point_id_out) {
+  if (!ctx) return ESIKF_ERR_ARG;
+  if (!ctx->have_vmap) return fail(ctx, ESIKF_ERR_STATE, "vmap_add_points before esikf_vmap_init");
+  if (n < 0 || m < 0 || (n > 0 && (!first || !ref || !point_id_out)) || (m > 0 && (!px || !patch || !T_f_w || !id || !mean || !score)))
+    return fail(ctx, ESIKF_ERR_ARG, "vmap_add_points: bad argument");
+  if (n == 0) return m == 0 ? ESIKF_OK : fail(ctx, ESIKF_ERR_ARG, "vmap_add_points: %d observations for no point", m);
+  if (first[0] != 0 || first[n] != m) return fail(ctx, ESIKF_ERR_ARG, "vmap_add_points: first[0] = %d, first[n] = %d for %d observations", first[0], first[n], m);
+  for (int32_t i = 0; i < n; i++) {
+    const int32_t c = first[i + 1] - first[i];
+    if (c < 0 || c > VMAP_SLOTS) return fail(ctx, ESIKF_ERR_ARG, "vmap_add_points: point %d has %d observations (0 .. 30)", i, c);
+    if (ref[i] < -1 || ref[i] >= c) return fail(ctx, ESIKF_ERR_ARG, "vmap_add_points: point %d: ref %d of %d observations", i, ref[i], c);
+  }
+  const int64_t base = ctx->vmap_points, need = base + n;
+  if (need > VMAP_MAX_POINTS) return fail(ctx, ESIKF_ERR_ARG, "vmap_add_points: %lld points exceed 2^26", (long long)need);
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  if (need > ctx->vmap_cap) {  // double until the points fit; the old records move over, a failed allocation leaves the store as it was
+    int64_t cap = ctx->vmap_cap;
+    while (cap < need) cap = std::min(2 * cap, VMAP_MAX_POINTS);
+    DevBuf<uint8_t> grown;
+    if (vmap_alloc(grown, cap) != cudaSuccess) return fail(ctx, ESIKF_ERR_CUDA, "vmap_add_points: growing the store to %lld points failed", (long long)cap);
+    const VmapView o = vmap_of(ctx), v = vmap_view(grown.p, (size_t)cap);
+    const size_t P = (size_t)base, S = P * VMAP_SLOTS;
+    CK(cudaMemcpyAsync(v.T, o.T, 12 * S * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(v.px, o.px, 2 * S * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(v.patch, o.patch, 64 * S * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(v.mean, o.mean, S * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(v.score, o.score, S * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(v.id, o.id, S * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(v.count, o.count, P * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(v.ref, o.ref, P * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+    CK(cudaStreamSynchronize(st));
+    ctx->vmap = std::move(grown);  // the old records leave with `grown`
+    ctx->vmap_cap = cap;
+  }
+  const size_t N = (size_t)n, M = (size_t)m;
+  VmapPackArgs a;
+  int32_t *d_pid, *d_first;
+  size_t in_bytes = 0;
+  auto lay = [&](ScratchLayout &s) {
+    a.T = s.take<double>(12 * M), a.px = s.take<double>(2 * M), a.patch = s.take<float>(64 * M), a.mean = s.take<float>(M), a.score = s.take<float>(M);
+    a.id = s.take<int32_t>(M), a.ref = s.take<int32_t>(N), d_pid = s.take<int32_t>(N), d_first = s.take<int32_t>(N + 1);
+    in_bytes = s.bytes;
+  };
+  CK(lay_out_scratch(ctx, lay));
+  CK(ctx->host.reserve(in_bytes));
+  std::vector<int32_t> pid(N);
+  for (size_t i = 0; i < N; i++) pid[i] = (int32_t)(base + (int64_t)i);
+  const VmapStage g{ctx};
+  g.put(a.T, T_f_w, 12 * M * sizeof(double)), g.put(a.px, px, 2 * M * sizeof(double)), g.put(a.patch, patch, 64 * M * sizeof(float));
+  g.put(a.mean, mean, M * sizeof(float)), g.put(a.score, score, M * sizeof(float)), g.put(a.id, id, M * sizeof(int32_t));
+  g.put(a.ref, ref, N * sizeof(int32_t)), g.put(d_pid, pid.data(), N * sizeof(int32_t)), g.put(d_first, first, (N + 1) * sizeof(int32_t));
+  CK(cudaMemcpyAsync(ctx->scratch.p, ctx->host.p, in_bytes, cudaMemcpyHostToDevice, st));
+  a.s = vmap_of(ctx), a.pid = d_pid, a.first = d_first, a.n = n, a.to_store = 1;
+  vmap_pack_kernel<<<(n + VMAP_WARPS - 1) / VMAP_WARPS, VMAP_WARPS * 32, 0, st>>>(a);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(st));
+  ctx->vmap_points = need;
+  memcpy(point_id_out, pid.data(), N * sizeof(int32_t));
+  return ESIKF_OK;
+}
+
+int esikf_vmap_update_points(esikf_ctx *ctx, int32_t n, const int32_t *point_id, const uint8_t *converged, const double *T_f_w, int32_t frame_id,
+                             const double *state, int32_t cap, int32_t *n_out, uint8_t *update_flag_out, int32_t *entry_out, double *pc_out,
+                             float *patch_out, int32_t *evicted_out, int32_t *count_out) {
+  if (!ctx) return ESIKF_ERR_ARG;
+  if (!ctx->have_vmap) return fail(ctx, ESIKF_ERR_STATE, "vmap_update_points before esikf_vmap_init");
+  if (n < 0 || !n_out || cap < 0 || (n > 0 && (!point_id || !converged))) return fail(ctx, ESIKF_ERR_ARG, "vmap_update_points: bad argument");
+  if (!ctx->have_cam || !ctx->have_ext) return fail(ctx, ESIKF_ERR_STATE, "vmap_update_points before vio_set_camera / set_extrinsics");
+  if (ctx->img_w != ctx->cam.width || ctx->img_h != ctx->cam.height) return fail(ctx, ESIKF_ERR_STATE, "vmap_update_points before vio_set_image");
+  if (!ctx->have_submap) return fail(ctx, ESIKF_ERR_STATE, "vmap_update_points: no visual sub-map installed (select_patches / set_patches)");
+  if (n != ctx->n_patches) return fail(ctx, ESIKF_ERR_ARG, "vmap_update_points: %d entries, the installed sub-map has %d", n, ctx->n_patches);
+  if (int rc = vmap_check_ids(ctx, n, point_id, "vmap_update_points")) return rc;
+  CK(cudaSetDevice(ctx->device));
+  const double *dev_state = nullptr;
+  if (int rc = rgb_state(ctx, state, esikf_ctx::RESIDENT_VIO, "vmap_update_points", &dev_state)) return rc;
+  static const double cos_max = acos_03_bound();
+  *n_out = 0;
+  if (n == 0) return ESIKF_OK;  // total_points == 0 (:910)
+  cudaStream_t st = ctx->stream;
+  const size_t N = (size_t)n;
+  VmapEditArgs e;
+  ObsArgs &a = e.obs;
+  int32_t *d_pid, *d_keep, *d_dst, *d_nk, *d_entry, *d_evicted, *d_count;
+  uint8_t *conv;
+  double *last_T, *last_px, *out_pc, *d_Tnew;
+  float *patch;
+  size_t in_bytes = 0;
+  auto lay = [&](ScratchLayout &s) {
+    d_pid = s.take<int32_t>(N), conv = s.take<uint8_t>(N), d_Tnew = s.take<double>(12);
+    in_bytes = s.bytes;
+    last_T = s.take<double>(12 * N), last_px = s.take<double>(2 * N), a.pc = s.take<double>(2 * N), d_keep = s.take<int32_t>(N), d_dst = s.take<int32_t>(N);
+    d_nk = s.take<int32_t>(1);
+    // the answers, read back as one span ending with the k patches
+    a.flag = s.take<uint8_t>(N), d_entry = s.take<int32_t>(N), d_evicted = s.take<int32_t>(N), d_count = s.take<int32_t>(N);
+    out_pc = s.take<double>(2 * N), patch = s.take<float>(64 * N);
+  };
+  CK(lay_out_scratch(ctx, lay));
+  CK(ctx->host.reserve(in_bytes));
+  const VmapStage g{ctx};
+  g.put(d_pid, point_id, N * sizeof(int32_t)), g.put(conv, converged, N);
+  if (T_f_w) g.put(d_Tnew, T_f_w, 12 * sizeof(double));
+  CK(cudaMemcpyAsync(ctx->scratch.p, ctx->host.p, in_bytes, cudaMemcpyHostToDevice, st));
+  e.s = vmap_of(ctx);
+  vmap_last_kernel<<<(n + 255) / 256, 256, 0, st>>>(e.s, d_pid, n, last_T, last_px);
+  frame_consts(ctx, a.cam, a.Rci, a.Pci);
+  a.state = dev_state, a.pos = ctx->vis_pos.p, a.converged = conv, a.last_T = last_T, a.last_px = last_px;
+  a.n = n, a.cos_max = cos_max, a.keep = d_keep;
+  obs_flag_kernel<<<(n + OBS_THREADS - 1) / OBS_THREADS, OBS_THREADS, 0, st>>>(a);
+  select_scan_kernel<<<1, SELECT_SCAN_THREADS, 0, st>>>(d_keep, n, d_dst, d_nk);
+  obs_scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_keep, d_dst, a.pc, n, d_entry, out_pc);
+  ctx->launches += 4;
+  CK(cudaGetLastError());
+  int32_t nk = 0;
+  CK(cudaMemcpyAsync(&nk, d_nk, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  *n_out = nk;
+  // the store is edited only once the answers fit: a call refused here can be repeated with a larger cap
+  if (nk > cap) return fail(ctx, ESIKF_ERR_ARG, "vmap_update_points: %d new observations, room for %d", nk, cap);
+  if (nk > 0) image_patch_kernel<<<(nk * 64 + 255) / 256, 256, 0, st>>>(ctx->img.p, ctx->img_w, ctx->img_h, out_pc, nk, 0, patch);
+  e.pid = d_pid, e.dst = d_dst, e.new_pc = out_pc, e.new_patch = patch, e.T_f_w = T_f_w ? d_Tnew : nullptr, e.frame_id = frame_id;
+  e.evicted = d_evicted, e.count = d_count;
+  vmap_edit_kernel<<<(n + VMAP_WARPS - 1) / VMAP_WARPS, VMAP_WARPS * 32, 0, st>>>(e);
+  ctx->launches += nk > 0 ? 2 : 1;
+  CK(cudaGetLastError());
+  CK(read_back(ctx, a.flag, patch + 64 * (size_t)nk));
+  const void *f0 = a.flag;
+  if (update_flag_out) copy_out(ctx, update_flag_out, f0, a.flag, N);
+  if (evicted_out) copy_out(ctx, evicted_out, f0, d_evicted, N * sizeof(int32_t));
+  if (count_out) copy_out(ctx, count_out, f0, d_count, N * sizeof(int32_t));
+  if (entry_out) copy_out(ctx, entry_out, f0, d_entry, (size_t)nk * sizeof(int32_t));
+  if (pc_out) copy_out(ctx, pc_out, f0, out_pc, (size_t)nk * 2 * sizeof(double));
+  if (patch_out) copy_out(ctx, patch_out, f0, patch, (size_t)nk * 64 * sizeof(float));
+  return ESIKF_OK;
+}
+
+int esikf_vmap_score(esikf_ctx *ctx, int32_t n, const int32_t *point_id, const double *pos, const double *normal, int32_t *ref_out, float *score_out,
+                     float *mean_out) {
+  if (!ctx) return ESIKF_ERR_ARG;
+  if (!ctx->have_vmap) return fail(ctx, ESIKF_ERR_STATE, "vmap_score before esikf_vmap_init");
+  if (n < 0 || (n > 0 && (!point_id || !pos || !normal || !ref_out))) return fail(ctx, ESIKF_ERR_ARG, "vmap_score: bad argument");
+  if (int rc = vmap_check_ids(ctx, n, point_id, "vmap_score")) return rc;
+  if (n == 0) return ESIKF_OK;
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t N = (size_t)n;
+  int32_t *d_pid;
+  double *d_pos, *d_normal;
+  float *d_score = nullptr, *d_mean = nullptr;
+  RefPatchArgs a;
+  size_t in_bytes = 0;
+  auto lay = [&](ScratchLayout &s) {
+    d_pid = s.take<int32_t>(N), d_pos = s.take<double>(3 * N), d_normal = s.take<double>(3 * N);
+    in_bytes = s.bytes;
+    a.ref = s.take<int32_t>(N);  // read back as one span with the rows
+    if (score_out) d_score = s.take<float>(VMAP_SLOTS * N);
+    if (mean_out) d_mean = s.take<float>(VMAP_SLOTS * N);
+  };
+  CK(lay_out_scratch(ctx, lay));
+  CK(ctx->host.reserve(in_bytes));
+  const VmapStage g{ctx};
+  g.put(d_pid, point_id, N * sizeof(int32_t)), g.put(d_pos, pos, 3 * N * sizeof(double)), g.put(d_normal, normal, 3 * N * sizeof(double));
+  CK(cudaMemcpyAsync(ctx->scratch.p, ctx->host.p, in_bytes, cudaMemcpyHostToDevice, st));
+  const VmapView v = vmap_of(ctx);
+  a.pos = d_pos, a.normal = d_normal, a.T = v.T, a.patch = v.patch, a.mean = v.mean, a.id = v.id, a.n = n;
+  a.score = v.score, a.mean_out = v.mean;  // in place
+  refpatch_score_kernel<<<(n + RP_WARPS - 1) / RP_WARPS, RP_WARPS * 32, 0, st>>>(a, RpStore{d_pid, v.count, v.ref});
+  ctx->launches++;
+  if (score_out || mean_out) {
+    vmap_rows_kernel<<<(n * VMAP_SLOTS + 255) / 256, 256, 0, st>>>(v, d_pid, n, nullptr, d_score, d_mean);
+    ctx->launches++;
+  }
+  CK(cudaGetLastError());
+  const float *end = d_mean ? d_mean + VMAP_SLOTS * N : d_score ? d_score + VMAP_SLOTS * N : nullptr;
+  CK(read_back(ctx, a.ref, end ? (const void *)end : (const void *)(a.ref + N)));
+  copy_out(ctx, ref_out, a.ref, a.ref, N * sizeof(int32_t));
+  if (score_out) copy_out(ctx, score_out, a.ref, d_score, VMAP_SLOTS * N * sizeof(float));
+  if (mean_out) copy_out(ctx, mean_out, a.ref, d_mean, VMAP_SLOTS * N * sizeof(float));
+  return ESIKF_OK;
+}
+
+int esikf_vmap_choose_ref(esikf_ctx *ctx, int32_t n, const int32_t *point_id, const double *pos, const double *frame_pos, int32_t normal_en,
+                          int32_t *ref_out) {
+  if (!ctx) return ESIKF_ERR_ARG;
+  if (!ctx->have_vmap) return fail(ctx, ESIKF_ERR_STATE, "vmap_choose_ref before esikf_vmap_init");
+  if (n < 0 || (n > 0 && (!point_id || !ref_out || (!normal_en && (!pos || !frame_pos))))) return fail(ctx, ESIKF_ERR_ARG, "vmap_choose_ref: bad argument");
+  if (int rc = vmap_check_ids(ctx, n, point_id, "vmap_choose_ref")) return rc;
+  if (n == 0) return ESIKF_OK;
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t N = (size_t)n;
+  VmapChooseArgs a;
+  int32_t *d_pid;
+  double *d_pos;
+  size_t in_bytes = 0;
+  auto lay = [&](ScratchLayout &s) {
+    d_pid = s.take<int32_t>(N), d_pos = s.take<double>(3 * N);
+    in_bytes = s.bytes;
+    a.ref = s.take<int32_t>(N);
+  };
+  CK(lay_out_scratch(ctx, lay));
+  CK(ctx->host.reserve(in_bytes));
+  const VmapStage g{ctx};
+  g.put(d_pid, point_id, N * sizeof(int32_t));
+  if (pos) g.put(d_pos, pos, 3 * N * sizeof(double));
+  CK(cudaMemcpyAsync(ctx->scratch.p, ctx->host.p, in_bytes, cudaMemcpyHostToDevice, st));
+  a.s = vmap_of(ctx), a.pid = d_pid, a.pos = d_pos, a.n = n, a.normal_en = normal_en != 0;
+  for (int k = 0; k < 3; k++) a.frame_pos[k] = frame_pos ? frame_pos[k] : 0.0;
+  vmap_choose_kernel<<<(n + VMAP_WARPS - 1) / VMAP_WARPS, VMAP_WARPS * 32, 0, st>>>(a);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  CK(read_back(ctx, a.ref, a.ref + N));
+  copy_out(ctx, ref_out, a.ref, a.ref, N * sizeof(int32_t));
+  return ESIKF_OK;
+}
+
+int esikf_vmap_download(esikf_ctx *ctx, int32_t n, const int32_t *point_id, int32_t cap, int32_t *first_out, double *px, float *patch, double *T_f_w,
+                        int32_t *id, float *mean, float *score, int32_t *ref) {
+  if (!ctx) return ESIKF_ERR_ARG;
+  if (!ctx->have_vmap) return fail(ctx, ESIKF_ERR_STATE, "vmap_download before esikf_vmap_init");
+  if (n < 0 || cap < 0 || !first_out || (n > 0 && (!point_id || !ref)) || (cap > 0 && (!px || !patch || !T_f_w || !id || !mean || !score)))
+    return fail(ctx, ESIKF_ERR_ARG, "vmap_download: bad argument");
+  if (int rc = vmap_check_ids(ctx, n, point_id, "vmap_download")) return rc;
+  if (n == 0) {
+    first_out[0] = 0;
+    return ESIKF_OK;
+  }
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t N = (size_t)n;
+  int32_t *d_pid, *d_count;
+  auto lay1 = [&](ScratchLayout &s) { d_pid = s.take<int32_t>(N), d_count = s.take<int32_t>(N); };
+  CK(lay_out_scratch(ctx, lay1));
+  CK(cudaMemcpyAsync(d_pid, point_id, N * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  const VmapView v = vmap_of(ctx);
+  vmap_rows_kernel<<<(n * VMAP_SLOTS + 255) / 256, 256, 0, st>>>(v, d_pid, n, d_count, nullptr, nullptr);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  CK(read_back(ctx, d_count, d_count + N));
+  std::vector<int32_t> first(N + 1, 0);
+  for (size_t i = 0; i < N; i++) first[i + 1] = first[i] + ((const int32_t *)ctx->host.p)[i];
+  const int32_t m = first[N];
+  if (m > cap) {
+    memcpy(first_out, first.data(), (N + 1) * sizeof(int32_t));
+    return fail(ctx, ESIKF_ERR_ARG, "vmap_download: %d observations, room for %d", m, cap);
+  }
+  const size_t M = (size_t)m;
+  VmapPackArgs a;
+  int32_t *d_first;
+  auto lay2 = [&](ScratchLayout &s) {
+    d_pid = s.take<int32_t>(N), d_first = s.take<int32_t>(N + 1);
+    a.T = s.take<double>(12 * M), a.px = s.take<double>(2 * M), a.patch = s.take<float>(64 * M), a.mean = s.take<float>(M), a.score = s.take<float>(M);
+    a.id = s.take<int32_t>(M), a.ref = s.take<int32_t>(N);  // read back as one span
+  };
+  CK(lay_out_scratch(ctx, lay2));
+  CK(cudaMemcpyAsync(d_pid, point_id, N * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d_first, first.data(), (N + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  a.s = v, a.pid = d_pid, a.first = d_first, a.n = n, a.to_store = 0;
+  vmap_pack_kernel<<<(n + VMAP_WARPS - 1) / VMAP_WARPS, VMAP_WARPS * 32, 0, st>>>(a);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  CK(read_back(ctx, a.T, a.ref + N));
+  const void *f0 = a.T;
+  memcpy(first_out, first.data(), (N + 1) * sizeof(int32_t));
+  if (m > 0) {
+    copy_out(ctx, T_f_w, f0, a.T, 12 * M * sizeof(double)), copy_out(ctx, px, f0, a.px, 2 * M * sizeof(double));
+    copy_out(ctx, patch, f0, a.patch, 64 * M * sizeof(float)), copy_out(ctx, mean, f0, a.mean, M * sizeof(float));
+    copy_out(ctx, score, f0, a.score, M * sizeof(float)), copy_out(ctx, id, f0, a.id, M * sizeof(int32_t));
+  }
+  copy_out(ctx, ref, f0, a.ref, N * sizeof(int32_t));
   return ESIKF_OK;
 }
 

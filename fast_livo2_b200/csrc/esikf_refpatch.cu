@@ -3,7 +3,10 @@
 //
 //   refpatch_score_kernel : one warp per point. Lane q scores the observations q, q + 32, ... of the point's list: the cosine
 //                           between its viewing ray and the point's normal, and the NCC against every observation of another
-//                           frame id; then lane 0 takes the first strict maximum above -1000 in list order.
+//                           frame id; then lane 0 takes the first strict maximum above -1000 in list order. Templated on where a
+//                           point's list lies: packed by first[] offsets (RpPacked, esikf_vio_score_ref_patches) or a slot of
+//                           the visual map's observation store (RpStore in esikf_vmap.cu, esikf_vmap_score), whose mean_ and
+//                           score_ it reads and writes in place.
 //
 // What is computed, per point with observations o_0 .. o_{n-1} in obs_ order (the newest first):
 //   mean(o)   : o.mean_ when abs(mean_) >= 1e-6 (float abs, compared in double), else the double sum of the 64 taps in order,
@@ -32,15 +35,23 @@ namespace esikf {
 #define RP_STRIDE 65
 
 struct RefPatchArgs {
-  const int32_t *first;         // [n + 1] offsets into the observations
   const double *pos, *normal;   // [n][3] VisualPoint::pos_, normal_
   const double *T;              // [m][12] Feature::T_f_w_: R row-major, then t
   const float *patch;           // [m][64] Feature::patch_
   const float *mean;            // [m] Feature::mean_ on entry
   const int32_t *id;            // [m] Feature::id_
   int n;
-  float *score, *mean_out;      // [m]; mean_out is read back by the warp that wrote it
+  float *score, *mean_out;      // [m]; mean_out is read back by the warp that wrote it (it may be `mean`: the lane that reads
+                                // an observation's mean is the one that writes it, and a __syncwarp precedes every other read)
   int32_t *ref;                 // [n]
+};
+
+// point i owns the observations first[i] .. first[i + 1] - 1
+struct RpPacked {
+  const int32_t *first;
+  __device__ __forceinline__ int begin(int i) const { return first[i]; }
+  __device__ __forceinline__ int count(int i) const { return first[i + 1] - first[i]; }
+  __device__ __forceinline__ void set_ref(int, int) const {}
 };
 
 // The mean the scoring uses for an observation whose cached mean_ is `cached` (std::accumulate from 0.0, then float / int)
@@ -81,13 +92,13 @@ template <class Taps> __device__ __forceinline__ float rp_ncc(const Taps &t, con
   return __fdiv_rn(ncc, (float)count);
 }
 
-__global__ void __launch_bounds__(RP_WARPS * 32) refpatch_score_kernel(const RefPatchArgs a) {
+template <class Lists> __global__ void __launch_bounds__(RP_WARPS * 32) refpatch_score_kernel(const RefPatchArgs a, const Lists L) {
   __shared__ float taps[RP_WARPS][RP_CAP * RP_STRIDE];
   __shared__ int32_t ids[RP_WARPS][RP_CAP];
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int i = blockIdx.x * RP_WARPS + w;
   if (i >= a.n) return;
-  const int b = a.first[i], n = a.first[i + 1] - b;
+  const int b = L.begin(i), n = L.count(i);
   const double *pos = a.pos + 3 * (size_t)i, *normal = a.normal + 3 * (size_t)i;
   float *score = a.score + b;
   if (n <= RP_CAP) {
@@ -129,6 +140,7 @@ __global__ void __launch_bounds__(RP_WARPS * 32) refpatch_score_kernel(const Ref
     for (int r = 0; r < n; r++)
       if (score[r] > best) best = score[r], ref = r;
     a.ref[i] = ref;
+    L.set_ref(i, ref);
   }
 }
 

@@ -665,6 +665,115 @@ void VIOManager::ScoreReferencePatches(const std::vector<int32_t> &first, const 
   score.assign(sc, sc + m), mean.assign(mu, mu + m), ref.assign(rf, rf + n);
 }
 
+void VIOManager::EnableDeviceObservations(int64_t capacity) {
+  if (!ctx_) {
+    last_status_ = ESIKF_ERR_STATE, last_error_ = "EnableDeviceObservations: no device context";
+    return;
+  }
+  Record(ctx_, esikf_vmap_init(ctx_, capacity));
+}
+
+void VIOManager::AddVisualPoints(const std::vector<int32_t> &first, const std::vector<StoredObservation> &obs, const std::vector<int32_t> &ref,
+                                 std::vector<int32_t> &point_ids) {
+  point_ids.clear();
+  if (!ctx_) {
+    last_status_ = ESIKF_ERR_STATE, last_error_ = "AddVisualPoints: no device context";
+    return;
+  }
+  if (first.size() != ref.size() + 1) {
+    last_status_ = ESIKF_ERR_ARG, last_error_ = "AddVisualPoints: first must have ref.size() + 1 entries";
+    return;
+  }
+  const size_t n = ref.size(), m = obs.size();
+  double *d;  // px 2m | T_f_w 12m, then patch 64m | mean m | score m, then first n + 1 | id m | ref n | ids n
+  float *f; int32_t *k;
+  if (!lay_out_staging(block_, [&](ScratchLayout &s) { d = s.take<double>(14 * m), f = s.take<float>(66 * m), k = s.take<int32_t>(3 * n + 1 + m); }))
+    return StagingFailed();
+  int32_t *id = k + n + 1, *rf = id + m, *ids = rf + n;
+  memcpy(k, first.data(), (n + 1) * sizeof(int32_t)), memcpy(rf, ref.data(), n * sizeof(int32_t));
+  for (size_t j = 0; j < m; j++) {
+    memcpy(d + 2 * j, obs[j].px, sizeof(obs[j].px)), memcpy(d + 2 * m + 12 * j, obs[j].T_f_w, sizeof(obs[j].T_f_w));
+    memcpy(f + 64 * j, obs[j].patch, sizeof(obs[j].patch));
+    f[64 * m + j] = obs[j].mean, f[65 * m + j] = obs[j].score, id[j] = obs[j].id;
+  }
+  if (Record(ctx_, esikf_vmap_add_points(ctx_, (int32_t)n, k, (int32_t)m, d, f, d + 2 * m, id, f + 64 * m, f + 65 * m, rf, ids))) return;
+  point_ids.assign(ids, ids + n);
+}
+
+void VIOManager::UpdateVisualMapPoints(const std::vector<int32_t> &point_ids, const std::vector<uint8_t> &converged, int32_t frame_id,
+                                       std::vector<uint8_t> &update_flag, std::vector<NewObservation> &new_obs, std::vector<int32_t> &evicted,
+                                       std::vector<int32_t> &count) {
+  new_obs.clear();
+  if (!ctx_ || !state) {
+    last_status_ = ESIKF_ERR_STATE, last_error_ = "UpdateVisualMapPoints: no device context or state";
+    return;
+  }
+  const int n = total_points > 0 ? total_points : 0;
+  update_flag.assign(n, 0), evicted.assign(n, -1), count.assign(n, 0);
+  if (point_ids.size() != (size_t)n || converged.size() != (size_t)n) {
+    last_status_ = ESIKF_ERR_ARG, last_error_ = "UpdateVisualMapPoints: point_ids / converged must have total_points entries";
+    return;
+  }
+  if (n == 0) {  // src/vio.cpp:910
+    last_status_ = ESIKF_OK;
+    return;
+  }
+  const size_t N = (size_t)n;
+  double *sbuf, *pc; uint8_t *conv, *flag; int32_t *pid, *entry, *ev, *cnt; float *patch;
+  auto lay = [&](ScratchLayout &s) {
+    sbuf = s.take<double>(ESIKF_STATE_DOUBLES), pid = s.take<int32_t>(N), conv = s.take<uint8_t>(N), flag = s.take<uint8_t>(N);
+    entry = s.take<int32_t>(N), ev = s.take<int32_t>(N), cnt = s.take<int32_t>(N), pc = s.take<double>(2 * N), patch = s.take<float>(64 * N);
+  };
+  if (!lay_out_staging(block_, lay)) return StagingFailed();
+  state->pack(sbuf);
+  memcpy(pid, point_ids.data(), N * sizeof(int32_t)), memcpy(conv, converged.data(), N);
+  int32_t k = 0;
+  if (Record(ctx_, esikf_vmap_update_points(ctx_, n, pid, conv, nullptr, frame_id, sbuf, n, &k, flag, entry, pc, patch, ev, cnt))) return;
+  memcpy(update_flag.data(), flag, N), memcpy(evicted.data(), ev, N * sizeof(int32_t)), memcpy(count.data(), cnt, N * sizeof(int32_t));
+  new_obs.resize(k);
+  for (int i = 0; i < k; i++) {
+    NewObservation &q = new_obs[i];
+    q.entry = entry[i];
+    memcpy(q.pc, pc + 2 * i, sizeof(q.pc)), memcpy(q.patch, patch + 64 * i, sizeof(q.patch));
+  }
+}
+
+void VIOManager::ScoreReferencePatches(const std::vector<int32_t> &point_ids, const std::vector<ScoredPoint> &pts, std::vector<int32_t> &ref) {
+  ref.clear();
+  if (!ctx_) {
+    last_status_ = ESIKF_ERR_STATE, last_error_ = "ScoreReferencePatches: no device context";
+    return;
+  }
+  if (point_ids.size() != pts.size()) {
+    last_status_ = ESIKF_ERR_ARG, last_error_ = "ScoreReferencePatches: point_ids and pts differ in size";
+    return;
+  }
+  const size_t n = pts.size();
+  double *d; int32_t *k;  // pos 3n | normal 3n, then point_ids n | ref n
+  if (!lay_out_staging(block_, [&](ScratchLayout &s) { d = s.take<double>(6 * n), k = s.take<int32_t>(2 * n); })) return StagingFailed();
+  memcpy(k, point_ids.data(), n * sizeof(int32_t));
+  for (size_t i = 0; i < n; i++) memcpy(d + 3 * i, pts[i].pos, sizeof(pts[i].pos)), memcpy(d + 3 * n + 3 * i, pts[i].normal, sizeof(pts[i].normal));
+  if (Record(ctx_, esikf_vmap_score(ctx_, (int32_t)n, k, d, d + 3 * n, k + n, nullptr, nullptr))) return;
+  ref.assign(k + n, k + 2 * n);
+}
+
+void VIOManager::ChooseReferenceFeatures(const std::vector<int32_t> &point_ids, const double *pos, const double frame_pos[3], bool normal_en,
+                                         std::vector<int32_t> &ref) {
+  ref.clear();
+  if (!ctx_) {
+    last_status_ = ESIKF_ERR_STATE, last_error_ = "ChooseReferenceFeatures: no device context";
+    return;
+  }
+  const size_t n = point_ids.size();
+  double *d; int32_t *k;  // pos 3n | frame_pos 3, then point_ids n | ref n
+  if (!lay_out_staging(block_, [&](ScratchLayout &s) { d = s.take<double>(3 * n + 3), k = s.take<int32_t>(2 * n); })) return StagingFailed();
+  memcpy(k, point_ids.data(), n * sizeof(int32_t));
+  if (pos) memcpy(d, pos, 3 * n * sizeof(double));
+  if (frame_pos) memcpy(d + 3 * n, frame_pos, 3 * sizeof(double));
+  if (Record(ctx_, esikf_vmap_choose_ref(ctx_, (int32_t)n, k, pos ? d : nullptr, frame_pos ? d + 3 * n : nullptr, normal_en ? 1 : 0, k + n))) return;
+  ref.assign(k + n, k + 2 * n);
+}
+
 void VIOManager::initializeVIO() {
   if (!ctx_) return;
   esikf_extrinsics ext;
@@ -1525,6 +1634,62 @@ int fl2_shim_score_ref_patches(int n, const int32_t *first, int m, const double 
   }
   esikf_destroy(ctx);
   return rc;
+}
+// GPU: the observation-store overloads of VIOManager on the caller's context (a VIOManager shares it, as LIVMapper's does),
+// one per C ABI call; the same arguments as esikf_vmap_*. Each returns 0 or the failing esikf_status.
+int fl2_shim_vmap_enable(void *ctx, int64_t capacity) {
+  VIOManager vio((esikf_ctx *)ctx);
+  vio.EnableDeviceObservations(capacity);
+  return vio.last_status_;
+}
+int fl2_shim_vmap_add(void *ctx, int n, const int32_t *first, const double *px, const float *patch, const double *T_f_w, const int32_t *id,
+                      const float *mean, const float *score, const int32_t *ref, int32_t *ids_out) {
+  VIOManager vio((esikf_ctx *)ctx);
+  std::vector<int32_t> fi(first, first + n + 1), rf(ref, ref + n), ids;
+  std::vector<StoredObservation> obs(fi[n]);
+  for (int j = 0; j < fi[n]; j++) {
+    memcpy(obs[j].px, px + 2 * j, sizeof(obs[j].px)), memcpy(obs[j].T_f_w, T_f_w + 12 * (size_t)j, sizeof(obs[j].T_f_w));
+    memcpy(obs[j].patch, patch + 64 * (size_t)j, sizeof(obs[j].patch));
+    obs[j].id = id[j], obs[j].mean = mean[j], obs[j].score = score[j];
+  }
+  vio.AddVisualPoints(fi, obs, rf, ids);
+  if (!vio.last_status_) memcpy(ids_out, ids.data(), ids.size() * sizeof(int32_t));
+  return vio.last_status_;
+}
+int fl2_shim_vmap_update(void *ctx, const double *state, int n, const int32_t *point_id, const uint8_t *converged, int32_t frame_id, int32_t *n_out,
+                         uint8_t *flag_out, int32_t *entry_out, double *pc_out, float *patch_out, int32_t *evicted_out, int32_t *count_out) {
+  VIOManager vio((esikf_ctx *)ctx);
+  StatesGroup st;
+  st.unpack(state);
+  vio.state = &st, vio.total_points = n;
+  std::vector<int32_t> pid(point_id, point_id + n), ev, cnt;
+  std::vector<uint8_t> conv(converged, converged + n), flag;
+  std::vector<NewObservation> obs;
+  vio.UpdateVisualMapPoints(pid, conv, frame_id, flag, obs, ev, cnt);
+  if (vio.last_status_) return vio.last_status_;
+  *n_out = (int32_t)obs.size();
+  memcpy(flag_out, flag.data(), n), memcpy(evicted_out, ev.data(), n * sizeof(int32_t)), memcpy(count_out, cnt.data(), n * sizeof(int32_t));
+  for (size_t i = 0; i < obs.size(); i++) {
+    entry_out[i] = obs[i].entry;
+    memcpy(pc_out + 2 * i, obs[i].pc, sizeof(obs[i].pc)), memcpy(patch_out + 64 * i, obs[i].patch, sizeof(obs[i].patch));
+  }
+  return 0;
+}
+int fl2_shim_vmap_score(void *ctx, int n, const int32_t *point_id, const double *pos, const double *normal, int32_t *ref_out) {
+  VIOManager vio((esikf_ctx *)ctx);
+  std::vector<ScoredPoint> pts(n);
+  for (int i = 0; i < n; i++) memcpy(pts[i].pos, pos + 3 * i, sizeof(pts[i].pos)), memcpy(pts[i].normal, normal + 3 * i, sizeof(pts[i].normal));
+  std::vector<int32_t> ref;
+  vio.ScoreReferencePatches(std::vector<int32_t>(point_id, point_id + n), pts, ref);
+  if (!vio.last_status_) memcpy(ref_out, ref.data(), ref.size() * sizeof(int32_t));
+  return vio.last_status_;
+}
+int fl2_shim_vmap_choose(void *ctx, int n, const int32_t *point_id, const double *pos, const double *frame_pos, int normal_en, int32_t *ref_out) {
+  VIOManager vio((esikf_ctx *)ctx);
+  std::vector<int32_t> ref;
+  vio.ChooseReferenceFeatures(std::vector<int32_t>(point_id, point_id + n), pos, frame_pos, normal_en != 0, ref);
+  if (!vio.last_status_) memcpy(ref_out, ref.data(), ref.size() * sizeof(int32_t));
+  return vio.last_status_;
 }
 void *fl2_shim_session_context(void *h) { return static_cast<ShimSession *>(h)->mgr->context(); }
 

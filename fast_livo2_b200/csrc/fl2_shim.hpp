@@ -326,6 +326,15 @@ struct ScoredPoint {
   double pos[3];
   double normal[3];
 };
+// One observation (Feature) of a visual point as the device's observation store keeps it: VIOManager::AddVisualPoints' input.
+struct StoredObservation {
+  double px[2];      // Feature::px_
+  double T_f_w[12];  // Feature::T_f_w_: R row-major, then t
+  float patch[64];   // Feature::patch_
+  int32_t id;        // Feature::id_
+  float mean;        // Feature::mean_
+  float score;       // Feature::score_
+};
 
 class VIOManager : public CallStatus {
  public:
@@ -409,6 +418,29 @@ class VIOManager : public CallStatus {
   // when ref_patch and has_ref_patch_ stay as they were. first has pts.size() + 1 entries, first[0] = 0 and the last obs.size().
   void ScoreReferencePatches(const std::vector<int32_t> &first, const std::vector<ScoredPoint> &pts, const std::vector<PatchObservation> &obs,
                              std::vector<float> &score, std::vector<float> &mean, std::vector<int32_t> &ref);
+
+  // The visual map's observations kept on the device (esikf_vmap_*, DESIGN.md §3 K14); the host's VisualPoint / Feature objects
+  // mirror them from what these calls return (INTEGRATION.md §3) and need no patch_. EnableDeviceObservations creates an
+  // empty store with room for `capacity` points (it grows by doubling), replacing any store the context held.
+  void EnableDeviceObservations(int64_t capacity);
+  // New points (generateVisualMapPoints' winners, or an existing host map): point i owns obs[first[i] .. first[i + 1]) in obs_
+  // order and ref[i], the position of ref_patch or -1. point_ids receives their store ids.
+  void AddVisualPoints(const std::vector<int32_t> &first, const std::vector<StoredObservation> &obs, const std::vector<int32_t> &ref,
+                       std::vector<int32_t> &point_ids);
+  // updateVisualMapPoints (src/vio.cpp:914-964) on the store: entry i of visual_submap is store point point_ids[i], with
+  // is_converged_ converged[i]; the frame pose is *state's and the new Features' id_ is frame_id. update_flag and new_obs as the
+  // overload above; per entry evicted (the list position deleteFeatureRef removed, -1 none) and count (the count afterwards).
+  void UpdateVisualMapPoints(const std::vector<int32_t> &point_ids, const std::vector<uint8_t> &converged, int32_t frame_id,
+                             std::vector<uint8_t> &update_flag, std::vector<NewObservation> &new_obs, std::vector<int32_t> &evicted,
+                             std::vector<int32_t> &count);
+  // The patch scoring of updateReferencePatch on the store (esikf_vmap_score): score_ and mean_ stay on the device; ref[i] is
+  // the new ref_patch's position, or -1 when ref_patch and has_ref_patch_ stay as they were.
+  void ScoreReferencePatches(const std::vector<int32_t> &point_ids, const std::vector<ScoredPoint> &pts, std::vector<int32_t> &ref);
+  // The reference feature of retrieveFromVisualSparseMap (:651-697) for n retrieved points (pos: pos_, 3 doubles each) seen
+  // from frame_pos (new_frame_->pos()): ref[i] is its position in obs_, -1 where the point is skipped (getCloseViewObs false)
+  // or the reference leaves ref_ftr unset. With normal_en the first two cases of :655-689 set the point's ref on the device.
+  void ChooseReferenceFeatures(const std::vector<int32_t> &point_ids, const double *pos, const double frame_pos[3], bool normal_en,
+                               std::vector<int32_t> &ref);
 
  private:
   const uint8_t *patch_img_ = nullptr, *patch_ref_img_ = nullptr;  // what the per-patch helpers uploaded last

@@ -498,6 +498,74 @@ int esikf_vio_depth_check(esikf_ctx *ctx, int32_t n, const double *pos_w, const 
 int esikf_vio_score_ref_patches(esikf_ctx *ctx, int32_t n, const int32_t *first, int32_t m, const double *pos, const double *normal, const float *patch,
                                 const float *mean, const int32_t *id, const double *T_f_w, float *score_out, float *mean_out, int32_t *ref_out);
 
+/* ---------------------------------------------------------------- the visual map's observations on the device (K14)
+ * A store of every visual point's obs_ list (VisualPoint::obs_), kept on the device so that the per-tick passes over the
+ * observations read and change them in place instead of receiving them from the host. A point id is the slot add_points
+ * handed out, in order from 0. Per point: its observations in obs_ order (the newest first, as addFrameRef pushes them), at
+ * most 30, and ref, the position of ref_patch in the list or -1 (has_ref_patch_ false). Per observation: px_ (2 doubles),
+ * T_f_w_ (12 doubles: R row-major, then t), patch_ (64 floats), id_, mean_ and score_. level_, inv_expo_time_, f_ and img_,
+ * which no device pass reads, stay on the caller's Feature objects, which mirror the store from what each call returns
+ * (INTEGRATION.md §3). A point takes 11,408 bytes of device memory whatever its count: 0.75 GB at 2^16 points.
+ *
+ * esikf_vmap_init      : an empty store with room for point_capacity points (1 .. 2^26), replacing any store the context
+ *                        held. esikf_destroy frees it.
+ * esikf_vmap_add_points: appends n points; point i owns the observations first[i] .. first[i + 1] - 1 of the packed arrays
+ *                        (first[0] = 0, first[n] = m, 0 .. 30 each) and ref[i] (-1 .. count - 1). Its id goes to
+ *                        point_id_out[i]. A new point of generateVisualMapPoints (src/vio.cpp:874-895, esikf_vio_generate_points'
+ *                        winners) has one observation: px_ = pc, the level-0 patch, the frame's T_f_w_ and id_, mean_ 0,
+ *                        score_ 0, ref -1. When the store is full its capacity doubles until the points fit; the old records
+ *                        are copied, and if the larger allocation fails the call returns ESIKF_ERR_CUDA with the store as it
+ *                        was. The capacity never shrinks.
+ * esikf_vmap_update_points: VIOManager::updateVisualMapPoints (:914-964) for the installed sub-map (n must equal its count),
+ *                        entry i being point point_id[i]. The flags, *n_out and the added entries' entry_out, pc_out and
+ *                        patch_out are esikf_vio_update_points' (same rule, same kernels), with each entry's oldest observation
+ *                        (obs_.back(), read before any eviction, as :931 precedes :947) taken from the store. Then per entry:
+ *                          converged: deleteNonRefPatchFeatures, only the ref observation stays (none when ref is -1: the
+ *                                     reference compares with a null or unset ref_patch); evicted_out -1;
+ *                          else, with 30 observations, the first strict minimum of score_ from FLT_MAX goes (the newest when
+ *                                     every score is NaN or >= FLT_MAX; evicted_out = its position, and ref becomes -1 if it was
+ *                                     the ref); then a flagged entry gets the new observation at the front: px_ = pc, the patch,
+ *                                     T_f_w_ = T_f_w (NULL: the frame pose of the flags, updateFrameState's), id_ = frame_id,
+ *                                     mean_ 0, score_ 0.
+ *                        count_out[i] = the count afterwards. With evicted_out and count_out the caller applies the same
+ *                        deleteNonRefPatchFeatures / deleteFeatureRef / addFrameRef to its own objects. An entry without
+ *                        observations (the reference would read obs_.back() of an empty list) is not flagged (DESIGN.md §4).
+ *                        If *n_out exceeds cap, only *n_out is written, the store is left as it was, and the call returns
+ *                        ESIKF_ERR_ARG. Every output but n_out may be NULL.
+ * esikf_vmap_score     : esikf_vio_score_ref_patches (K13, same kernel and arithmetic) on the store for n points that pass the
+ *                        caller's four skips of updateReferencePatch (:977-980); pos and normal (3 doubles each) per entry. The
+ *                        scores and means are written back to the store; a point's ref is set where ref_out[i] >= 0 and left
+ *                        as it was otherwise. score_out and mean_out (NULL or [n][30] floats, 0 past a point's count) receive
+ *                        the store's rows afterwards.
+ * esikf_vmap_choose_ref: the reference feature of retrieveFromVisualSparseMap (:651-697) for retrieved points that passed the
+ *                        depth check and the caller's is_normal_initialized_ skip. normal_en != 0: a point with one observation
+ *                        -> 0; without a ref -> the first strict minimum, from FLT_MAX, of the float sum of the squared patch
+ *                        differences against every observation of another id_, in list order, divided by their count; else
+ *                        its ref. The first two are stored as the point's ref. normal_en == 0: getCloseViewObs(frame_pos),
+ *                        the first strict maximum, from 0, of the cosine between (frame_pos - pos_) and (the observation's
+ *                        camera centre - pos_), both normalised; -1 below 0.5 (the point is skipped). pos (3 doubles per
+ *                        entry) and frame_pos (new_frame_->pos()) are read only then. ref_out[i] = -1 also where the
+ *                        reference leaves ref_ftr unset: no error beats FLT_MAX (every observation has the same id_, 0/0).
+ * esikf_vmap_download  : the inverse of add_points for n points: first_out (n + 1), then the packed observations (cap of them)
+ *                        and ref (n). If there are more than cap, only first_out is written and the call returns ESIKF_ERR_ARG.
+ * esikf_vmap_stats     : points added and capacity.
+ * ESIKF_ERR_ARG, with nothing written, for a point id outside [0, points), an id twice in one call, a count above 30 (add)
+ * or n different from the installed sub-map's count (update_points). ESIKF_ERR_STATE before esikf_vmap_init. With several
+ * ranks every rank holds the whole store and applies every call. */
+int esikf_vmap_init(esikf_ctx *ctx, int64_t point_capacity);
+int esikf_vmap_add_points(esikf_ctx *ctx, int32_t n, const int32_t *first, int32_t m, const double *px, const float *patch, const double *T_f_w,
+                          const int32_t *id, const float *mean, const float *score, const int32_t *ref, int32_t *point_id_out);
+int esikf_vmap_update_points(esikf_ctx *ctx, int32_t n, const int32_t *point_id, const uint8_t *converged, const double *T_f_w, int32_t frame_id,
+                             const double *state, int32_t cap, int32_t *n_out, uint8_t *update_flag_out, int32_t *entry_out, double *pc_out,
+                             float *patch_out, int32_t *evicted_out, int32_t *count_out);
+int esikf_vmap_score(esikf_ctx *ctx, int32_t n, const int32_t *point_id, const double *pos, const double *normal, int32_t *ref_out, float *score_out,
+                     float *mean_out);
+int esikf_vmap_choose_ref(esikf_ctx *ctx, int32_t n, const int32_t *point_id, const double *pos, const double *frame_pos, int32_t normal_en,
+                          int32_t *ref_out);
+int esikf_vmap_download(esikf_ctx *ctx, int32_t n, const int32_t *point_id, int32_t cap, int32_t *first_out, double *px, float *patch, double *T_f_w,
+                        int32_t *id, float *mean, float *score, int32_t *ref);
+int esikf_vmap_stats(esikf_ctx *ctx, int64_t *points, int64_t *capacity);
+
 /* ---------------------------------------------------------------- multi-GPU (one process per GPU)
  * The residual point / patch set is sharded by contiguous blocks; each iteration all-reduces the
  * packed information buffer [HTH upper | HTz | M | sum|d| ...] and every rank solves redundantly.
