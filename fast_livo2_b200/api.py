@@ -126,6 +126,8 @@ def load_library():
     lib.esikf_vmap_choose_ref.argtypes = [vp, C.c_int32, vp, vp, vp, C.c_int32, vp]
     lib.esikf_vmap_download.argtypes = [vp, C.c_int32, vp, C.c_int32] + [vp] * 8
     lib.esikf_vmap_stats.argtypes = [vp, vp, vp]
+    lib.esikf_vmap_place_points.argtypes = [vp, C.c_int32, vp, vp, vp]
+    lib.esikf_vmap_retrieve.argtypes = [vp, C.c_int32, vp] + [C.c_int32] * 6 + [ip] + [vp] * 5
     lib.esikf_comm_unique_id.argtypes = [C.c_char_p]
     lib.esikf_comm_init.argtypes = [vp, C.c_int32, C.c_int32, C.c_char_p]
     lib.esikf_comm_rank.argtypes = [vp, ip, ip]
@@ -146,6 +148,8 @@ TUNE_VIO_TMA = 2  # esikf_set_tuning flag: stage LIO plane records with __ldg co
 GEN_ADD_FROM = 0x40000000  # esikf_vio_generate_points: the source of a winner from the add_from list
 FIND_RULE_PATCH, FIND_RULE_RAYCAST = 0, 1  # esikf_map_device_find: updateReferencePatch's key, the ray casting's key
 FIND_NO_ROOT, FIND_NODE, FIND_PLANE = 0, 1, 2  # esikf_map_device_find's status per point
+# esikf_vmap_retrieve's status per cell: kept, depth-discontinuous, not normal-initialised, no reference feature, no winner
+RETRIEVE_KEPT, RETRIEVE_DEPTH, RETRIEVE_NOT_INIT, RETRIEVE_NO_REF, RETRIEVE_NO_WINNER = 0, 1, 2, 3, 4
 DEFAULT_LOOP_MODE = 2  # esikf_set_loop_mode: 2 (alias 1) persistent kernel per update, 0 per-iteration launches
 
 class MapCfgC(C.Structure):
@@ -165,7 +169,7 @@ EXPORTED_SYMBOLS = [
     "esikf_lio_update", "esikf_lio_fetch_point_cov", "esikf_vio_set_camera", "esikf_vio_set_image", "esikf_vio_set_patches",
     "esikf_vio_run", "esikf_vio_fetch", "esikf_vio_update", "esikf_vio_get_image_patch", "esikf_vio_set_ref_images",
     "esikf_vio_warp_patches", "esikf_vio_select_patches", "esikf_vio_warp_affine", "esikf_vio_set_inverse_refs", "esikf_rgb_set_cloud", "esikf_rgb_colorize", "esikf_vio_generate_points", "esikf_vio_update_points", "esikf_vio_retrieve_scan", "esikf_vio_depth_check", "esikf_vio_score_ref_patches",
-    "esikf_vmap_init", "esikf_vmap_add_points", "esikf_vmap_update_points", "esikf_vmap_score", "esikf_vmap_choose_ref", "esikf_vmap_download", "esikf_vmap_stats", "esikf_comm_unique_id", "esikf_comm_init", "esikf_comm_rank", "esikf_shard_range", "esikf_peer_export", "esikf_peer_attach", "esikf_profile_kernel", "esikf_set_kernel_timing", "esikf_get_kernel_timing", "esikf_set_phase_stamps", "esikf_get_phase_stamps",
+    "esikf_vmap_init", "esikf_vmap_add_points", "esikf_vmap_update_points", "esikf_vmap_score", "esikf_vmap_choose_ref", "esikf_vmap_download", "esikf_vmap_stats", "esikf_vmap_place_points", "esikf_vmap_retrieve", "esikf_comm_unique_id", "esikf_comm_init", "esikf_comm_rank", "esikf_shard_range", "esikf_peer_export", "esikf_peer_attach", "esikf_profile_kernel", "esikf_set_kernel_timing", "esikf_get_kernel_timing", "esikf_set_phase_stamps", "esikf_get_phase_stamps",
 ]
 
 
@@ -721,6 +725,30 @@ class Context:
         ref = np.zeros(max(n, 1), np.int32)
         self._ck(self.lib.esikf_vmap_choose_ref(self.h, n, pid.ctypes.data, _addr(p), _addr(fp), int(bool(normal_en)), ref.ctypes.data))
         return ref[:n]
+
+    def vmap_place_points(self, point_id, pos, normal_init=None):
+        """Place store points in their visual voxels (esikf_vmap_place_points, insertPointIntoVoxelMap): pos (n, 3) float64
+        pos_, normal_init (n,) is_normal_initialized_ (None: all true)."""
+        pid = _c(point_id, np.int32).reshape(-1)
+        n = len(pid)
+        pos = _c(pos, np.float64).reshape(-1, 3)
+        ni = None if normal_init is None else _c(normal_init, np.uint8).reshape(-1)
+        assert len(pos) == n and (ni is None or len(ni) == n)
+        self._ck(self.lib.esikf_vmap_place_points(self.h, n, pid.ctypes.data, pos.ctypes.data, _addr(ni)))
+
+    def vmap_retrieve(self, keys, grid_size, grid_n_width, grid_n_height, border, normal_en, cap=None):
+        """The walk of the retrieval over the placed points, its depth check, skip and reference choice (esikf_vmap_retrieve)
+        for the pose and depth image of the last vio_retrieve_scan: keys (k, 3) in sub_feat_map iteration order. Returns per
+        TYPE_MAP cell, in cell order: cell, point_id (-1 none), pc (m, 2), status (RETRIEVE_*) and ref (-1 unless kept).
+        cap: room for that many cells (fewer raises); by default the grid's length."""
+        keys = _c(keys, np.int32).reshape(-1, 3)
+        cap = int(grid_n_width) * int(grid_n_height) if cap is None else int(cap)
+        k = max(cap, 1)
+        out = dict(cell=np.zeros(k, np.int32), point_id=np.zeros(k, np.int32), pc=np.zeros((k, 2)), status=np.zeros(k, np.int32), ref=np.zeros(k, np.int32))
+        cnt = C.c_int32(0)
+        self._ck(self.lib.esikf_vmap_retrieve(self.h, len(keys), keys.ctypes.data, int(grid_size), int(grid_n_width), int(grid_n_height), int(border),
+                                              int(bool(normal_en)), cap, C.byref(cnt), *[out[f].ctypes.data for f in ("cell", "point_id", "pc", "status", "ref")]))
+        return {f: v[:cnt.value] for f, v in out.items()}
 
     def vmap_download(self, point_id):
         """The lists of the given points (esikf_vmap_download), in vmap_add_points' form: first, px, patch, T_f_w, id, mean,

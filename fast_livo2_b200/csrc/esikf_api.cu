@@ -30,6 +30,7 @@
 #include "esikf_find.cu"
 #include "esikf_refpatch.cu"
 #include "esikf_vmap.cu"
+#include "esikf_vretrieve.cu"
 
 using namespace esikf;
 
@@ -284,6 +285,11 @@ struct esikf_ctx {
   bool have_vmap = false;
   std::vector<uint32_t> vmap_seen;  // per point, the last call (vmap_epoch) that named it: the repeated-id check in O(n)
   uint32_t vmap_epoch = 0;
+  // the device feat_map of the store's points (esikf_vmap_place_points, esikf_vretrieve.cu): vpl_cap point records, ids below
+  // vpl_hi possibly placed, vpl_placed of them placed (the next sequence number); vpl_done mirrors which
+  DevBuf<uint8_t> vpl;
+  int64_t vpl_cap = 0, vpl_hi = 0, vpl_placed = 0;
+  std::vector<uint8_t> vpl_done;
 
   // What the front-end entry points need for the length of one call only (lay_out_scratch). Every such call runs on `stream`
   // and synchronises it before it returns, so they can share it; nothing a later call reads may be kept here.
@@ -2218,6 +2224,9 @@ int esikf_vmap_init(esikf_ctx *ctx, int64_t point_capacity) {
   ctx->vmap = DevBuf<uint8_t>();
   ctx->vmap_cap = ctx->vmap_points = 0;
   ctx->vmap_seen.clear(), ctx->vmap_epoch = 0;
+  ctx->vpl = DevBuf<uint8_t>();
+  ctx->vpl_cap = ctx->vpl_hi = ctx->vpl_placed = 0;
+  ctx->vpl_done.clear();
   CK(vmap_alloc(ctx->vmap, point_capacity));
   ctx->vmap_cap = point_capacity, ctx->have_vmap = true;
   return ESIKF_OK;
@@ -2502,6 +2511,186 @@ int esikf_vmap_download(esikf_ctx *ctx, int32_t n, const int32_t *point_id, int3
     copy_out(ctx, score, f0, a.score, M * sizeof(float)), copy_out(ctx, id, f0, a.id, M * sizeof(int32_t));
   }
   copy_out(ctx, ref, f0, a.ref, N * sizeof(int32_t));
+  return ESIKF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------- the map side of the retrieval
+int esikf_vmap_place_points(esikf_ctx *ctx, int32_t n, const int32_t *point_id, const double *pos, const uint8_t *normal_init) {
+  if (!ctx) return ESIKF_ERR_ARG;
+  if (!ctx->have_vmap) return fail(ctx, ESIKF_ERR_STATE, "vmap_place_points before esikf_vmap_init");
+  if (n < 0 || (n > 0 && (!point_id || !pos))) return fail(ctx, ESIKF_ERR_ARG, "vmap_place_points: bad argument");
+  if (int rc = vmap_check_ids(ctx, n, point_id, "vmap_place_points")) return rc;
+  int64_t hi = ctx->vpl_hi;
+  for (int32_t i = 0; i < n; i++) {
+    const int32_t p = point_id[i];
+    if ((size_t)p < ctx->vpl_done.size() && ctx->vpl_done[p]) return fail(ctx, ESIKF_ERR_ARG, "vmap_place_points: point id %d was placed before", p);
+    hi = std::max(hi, (int64_t)p + 1);
+  }
+  if (n == 0) return ESIKF_OK;
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  if (hi > ctx->vpl_cap) {  // double until the ids fit; a failed allocation leaves everything as it was
+    int64_t cap = std::max<int64_t>(ctx->vpl_cap, 1);
+    while (cap < hi) cap = std::min(2 * cap, VMAP_MAX_POINTS);
+    uint8_t *p = nullptr;
+    if (cudaMalloc(&p, vpl_bytes((size_t)cap)) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(ctx, ESIKF_ERR_CUDA, "vmap_place_points: growing the point arrays to %lld points failed", (long long)cap);
+    }
+    DevBuf<uint8_t> grown;
+    grown.p = p, grown.cap = vpl_bytes((size_t)cap);
+    const VplView v = vpl_view(grown.p, (size_t)cap);
+    CK(cudaMemsetAsync(v.key, 0xff, (size_t)cap * sizeof(unsigned long long), st));  // not placed
+    if (ctx->vpl_hi > 0) {
+      const VplView o = vpl_view(ctx->vpl.p, (size_t)ctx->vpl_cap);
+      const size_t P = (size_t)ctx->vpl_hi;
+      CK(cudaMemcpyAsync(v.pos, o.pos, 3 * P * sizeof(double), cudaMemcpyDeviceToDevice, st));
+      CK(cudaMemcpyAsync(v.key, o.key, P * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, st));
+      CK(cudaMemcpyAsync(v.seq, o.seq, P * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+      CK(cudaMemcpyAsync(v.ninit, o.ninit, P, cudaMemcpyDeviceToDevice, st));
+    }
+    CK(cudaStreamSynchronize(st));
+    ctx->vpl = std::move(grown);  // the old arrays leave with `grown`
+    ctx->vpl_cap = cap;
+  }
+  const size_t N = (size_t)n;
+  VplArgs a;
+  int32_t *d_pid;
+  double *d_pos;
+  uint8_t *d_ninit = nullptr;
+  size_t in_bytes = 0;
+  auto lay = [&](ScratchLayout &s) {
+    d_pid = s.take<int32_t>(N), d_pos = s.take<double>(3 * N);
+    if (normal_init) d_ninit = s.take<uint8_t>(N);
+    in_bytes = s.bytes;
+    a.key = s.take<unsigned long long>(N), a.bad = s.take<int32_t>(1);
+  };
+  CK(lay_out_scratch(ctx, lay));
+  CK(ctx->host.reserve(in_bytes));
+  const VmapStage g{ctx};
+  g.put(d_pid, point_id, N * sizeof(int32_t)), g.put(d_pos, pos, 3 * N * sizeof(double));
+  if (normal_init) g.put(d_ninit, normal_init, N);
+  CK(cudaMemcpyAsync(ctx->scratch.p, ctx->host.p, in_bytes, cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(a.bad, 0, sizeof(int32_t), st));
+  a.v = vpl_view(ctx->vpl.p, (size_t)ctx->vpl_cap), a.pid = d_pid, a.pos = d_pos, a.ninit = d_ninit, a.n = n, a.seq0 = (int32_t)ctx->vpl_placed;
+  vpl_key_kernel<<<(n + 255) / 256, 256, 0, st>>>(a);
+  vpl_commit_kernel<<<(n + 255) / 256, 256, 0, st>>>(a);  // writes nothing when a key was out of range
+  ctx->launches += 2;
+  CK(cudaGetLastError());
+  CK(read_back(ctx, a.bad, a.bad + 1));
+  if (*(const int32_t *)ctx->host.p) return fail(ctx, ESIKF_ERR_ARG, "vmap_place_points: a voxel key leaves [-2^20, 2^20)");
+  ctx->vpl_hi = hi, ctx->vpl_placed += n;
+  if (ctx->vpl_done.size() < (size_t)hi) ctx->vpl_done.resize((size_t)hi, 0);
+  for (int32_t i = 0; i < n; i++) ctx->vpl_done[point_id[i]] = 1;
+  return ESIKF_OK;
+}
+
+int esikf_vmap_retrieve(esikf_ctx *ctx, int32_t n_keys, const int32_t *keys, int32_t grid_size, int32_t grid_n_width, int32_t grid_n_height, int32_t border,
+                        int32_t normal_en, int32_t cap, int32_t *n_cells, int32_t *cell_out, int32_t *point_id_out, double *pc_out, int32_t *status_out,
+                        int32_t *ref_out) {
+  if (!ctx) return ESIKF_ERR_ARG;
+  if (!ctx->have_vmap) return fail(ctx, ESIKF_ERR_STATE, "vmap_retrieve before esikf_vmap_init");
+  if (n_keys < 0 || (n_keys > 0 && !keys) || !n_cells || cap < 0 || border < 0 || (cap > 0 && (!cell_out || !point_id_out || !pc_out || !status_out || !ref_out)))
+    return fail(ctx, ESIKF_ERR_ARG, "vmap_retrieve: bad argument");
+  if (!ctx->ret_valid) return fail(ctx, ESIKF_ERR_STATE, "vmap_retrieve: no esikf_vio_retrieve_scan since the last vio_set_camera");
+  const int W = ctx->ret_w, H = ctx->ret_h;
+  if (grid_size <= 0 || grid_n_width <= 0 || grid_n_height <= 0 || (int64_t)grid_n_width * grid_n_height > (1 << 24) ||
+      (int64_t)grid_n_width * grid_size < W - border || (int64_t)grid_n_height * grid_size < H - border)
+    return fail(ctx, ESIKF_ERR_ARG, "vmap_retrieve: a %d x %d grid of %d px does not cover the %d x %d image inside a border of %d", grid_n_width, grid_n_height,
+                grid_size, W, H, border);
+  {  // the walk keys: in the key range, each once
+    std::vector<unsigned long long> packed((size_t)n_keys);
+    for (int32_t i = 0; i < n_keys; i++) {
+      const int32_t *k = keys + 3 * (size_t)i;
+      if (!key_in_range(k[0], k[1], k[2])) return fail(ctx, ESIKF_ERR_ARG, "vmap_retrieve: walk key %d leaves [-2^20, 2^20)", i);
+      packed[i] = pack_key(k[0], k[1], k[2]);
+    }
+    std::sort(packed.begin(), packed.end());
+    if (std::adjacent_find(packed.begin(), packed.end()) != packed.end()) return fail(ctx, ESIKF_ERR_ARG, "vmap_retrieve: a walk key appears twice");
+  }
+  if (ctx->vpl_placed == 0 || n_keys == 0) {  // feat_map empty (the reference returns at :354), or nothing to walk
+    *n_cells = 0;
+    return ESIKF_OK;
+  }
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const int L = grid_n_width * grid_n_height;
+  const size_t K = (size_t)n_keys, NL = (size_t)L;
+  uint32_t T = 64;
+  while (T < 2 * K) T <<= 1;
+  VrtArgs a;
+  VrtCellArgs c;
+  int32_t *d_keys, *cnt, *ref_tmp;
+  unsigned long long *table;
+  uint8_t *disc;
+  double *fpos;
+  size_t in_bytes = 0;
+  auto lay = [&](ScratchLayout &s) {
+    d_keys = s.take<int32_t>(3 * K);
+    in_bytes = s.bytes;
+    table = s.take<unsigned long long>(T), a.wrank = s.take<int32_t>(T);
+    a.type = s.take<uint8_t>(NL), a.dist = s.take<uint32_t>(NL), a.tie = s.take<unsigned long long>(NL), a.win = s.take<int32_t>(NL);
+    a.pc = s.take<double>(2 * NL), a.wpos = s.take<double>(3 * NL), disc = s.take<uint8_t>(NL);
+    c.keep = s.take<int32_t>(NL), c.dst = s.take<int32_t>(NL), c.skeep = s.take<int32_t>(NL), c.sdst = s.take<int32_t>(NL);
+    c.spid = s.take<int32_t>(NL), c.sat = s.take<int32_t>(NL), c.spos = s.take<double>(3 * NL), ref_tmp = s.take<int32_t>(NL);
+    fpos = s.take<double>(3), cnt = s.take<int32_t>(2);  // read back first: frame_pos, cells, survivors
+    c.pc_out = s.take<double>(2 * NL), c.cell_out = s.take<int32_t>(NL), c.id_out = s.take<int32_t>(NL), c.status_out = s.take<int32_t>(NL);
+    c.ref_out = s.take<int32_t>(NL);  // the answers, read back as one span
+  };
+  CK(lay_out_scratch(ctx, lay));
+  CK(ctx->host.reserve(in_bytes));
+  const VmapStage g{ctx};
+  g.put(d_keys, keys, 3 * K * sizeof(int32_t));
+  CK(cudaMemcpyAsync(ctx->scratch.p, ctx->host.p, in_bytes, cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(table, 0xff, T * sizeof(unsigned long long), st));
+  vrt_hash_kernel<<<(n_keys + 255) / 256, 256, 0, st>>>(d_keys, n_keys, table, (int32_t *)a.wrank, T - 1);
+  CamDev cam;
+  frame_consts(ctx, cam, a.Rci, a.Pci);
+  memcpy(a.Rci, ctx->ret_Rci, sizeof(a.Rci)), memcpy(a.Pci, ctx->ret_Pci, sizeof(a.Pci));  // the scan call's
+  a.cam = cam, a.state = ctx->ret_state.p, a.v = vpl_view(ctx->vpl.p, (size_t)ctx->vpl_cap), a.count = vmap_of(ctx).count, a.n_pts = (int)ctx->vpl_hi;
+  a.wkey = table, a.wmask = T - 1, a.grid_size = grid_size, a.grid_n_width = grid_n_width, a.length = L, a.border = border, a.frame_pos = fpos;
+  vrt_init_kernel<<<(L + 255) / 256, 256, 0, st>>>(a);
+  const int pb = (a.n_pts + VRT_THREADS - 1) / VRT_THREADS;
+  vrt_walk_kernel<0><<<pb, VRT_THREADS, 0, st>>>(a);
+  vrt_walk_kernel<1><<<pb, VRT_THREADS, 0, st>>>(a);
+  vrt_walk_kernel<2><<<pb, VRT_THREADS, 0, st>>>(a);
+  DepthCheckArgs dc;  // K11's check on every cell's winner (a cell without one is not read)
+  memcpy(dc.Rci, ctx->ret_Rci, sizeof(dc.Rci)), memcpy(dc.Pci, ctx->ret_Pci, sizeof(dc.Pci));
+  dc.state = ctx->ret_state.p, dc.pos = a.wpos, dc.pc = a.pc, dc.n = L, dc.width = W, dc.height = H, dc.depth = ctx->ret_depth.p, dc.flag = disc;
+  ret_depth_check_kernel<<<(L + RET_THREADS - 1) / RET_THREADS, RET_THREADS, 0, st>>>(dc);
+  c.length = L, c.type = a.type, c.disc = disc, c.ninit = a.v.ninit, c.win = a.win, c.pc = a.pc, c.wpos = a.wpos;
+  vrt_cells_kernel<true><<<(L + 255) / 256, 256, 0, st>>>(c);
+  select_scan_kernel<<<1, SELECT_SCAN_THREADS, 0, st>>>(c.keep, L, c.dst, cnt);
+  select_scan_kernel<<<1, SELECT_SCAN_THREADS, 0, st>>>(c.skeep, L, c.sdst, cnt + 1);
+  vrt_cells_kernel<false><<<(L + 255) / 256, 256, 0, st>>>(c);
+  ctx->launches += 10;
+  CK(cudaGetLastError());
+  // vmap_choose_kernel takes its count and new_frame_->pos() by value: both come back before it runs, and a call refused for
+  // its cap has not touched the store
+  CK(read_back(ctx, fpos, cnt + 2));
+  double fp[3];
+  int32_t counts[2];
+  copy_out(ctx, fp, fpos, fpos, sizeof(fp)), copy_out(ctx, counts, fpos, cnt, sizeof(counts));
+  *n_cells = counts[0];
+  if (counts[0] > cap) return fail(ctx, ESIKF_ERR_ARG, "vmap_retrieve: %d cells, room for %d", counts[0], cap);
+  const int ns = counts[1];
+  if (ns > 0) {
+    VmapChooseArgs ca;
+    ca.s = vmap_of(ctx), ca.pid = c.spid, ca.pos = c.spos, ca.n = ns, ca.normal_en = normal_en != 0, ca.ref = ref_tmp;
+    for (int k = 0; k < 3; k++) ca.frame_pos[k] = fp[k];
+    vmap_choose_kernel<<<(ns + VMAP_WARPS - 1) / VMAP_WARPS, VMAP_WARPS * 32, 0, st>>>(ca);
+    vrt_refs_kernel<<<(ns + 255) / 256, 256, 0, st>>>(ref_tmp, c.sat, ns, c.ref_out, c.status_out);
+    ctx->launches += 2;
+    CK(cudaGetLastError());
+  }
+  const size_t M = (size_t)counts[0];
+  CK(read_back(ctx, c.pc_out, c.ref_out + M));
+  const void *f0 = c.pc_out;
+  if (M > 0) {
+    copy_out(ctx, pc_out, f0, c.pc_out, 2 * M * sizeof(double)), copy_out(ctx, cell_out, f0, c.cell_out, M * sizeof(int32_t));
+    copy_out(ctx, point_id_out, f0, c.id_out, M * sizeof(int32_t)), copy_out(ctx, status_out, f0, c.status_out, M * sizeof(int32_t));
+    copy_out(ctx, ref_out, f0, c.ref_out, M * sizeof(int32_t));
+  }
   return ESIKF_OK;
 }
 

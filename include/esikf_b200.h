@@ -566,6 +566,47 @@ int esikf_vmap_download(esikf_ctx *ctx, int32_t n, const int32_t *point_id, int3
                         int32_t *id, float *mean, float *score, int32_t *ref);
 int esikf_vmap_stats(esikf_ctx *ctx, int64_t *points, int64_t *capacity);
 
+/* ---------------------------------------------------------------- the map side of the visual sub-map retrieval (K15)
+ * retrieveFromVisualSparseMap's walk over feat_map (src/vio.cpp:438-484, raycast_en off) on a device feat_map of the store's
+ * points, with the depth check (:614-640), the is_normal_initialized_ skip (:651) and the reference-feature choice (:653-697)
+ * chained after it on the device.
+ * esikf_vmap_place_points: places n store points in their visual voxels, as insertPointIntoVoxelMap (:227-250) does: pos
+ *                        (3 doubles per point) is the point's pos_, normal_init its is_normal_initialized_ (NULL: all true).
+ *                        The key of a coordinate c is the insertion rule: float(c / 0.5), minus 1.0 in double and narrowed
+ *                        again when negative, truncated; it is not the scan's floor rule (x = -0.3: insertion key -1, scan
+ *                        key -2), and the walk looks scan keys up in this map, as the reference does. Within a voxel the
+ *                        points keep their placement order (call order, later calls after earlier ones). Positions never
+ *                        change and points are never removed. The point arrays grow by doubling; if that allocation fails the
+ *                        call returns ESIKF_ERR_CUDA with everything as it was.
+ * esikf_vmap_retrieve  : the walk for the frame pose and depth image of the last esikf_vio_retrieve_scan. keys: n_keys scan
+ *                        voxel keys (3 int32 each) in the caller's sub_feat_map iteration order. For each placed point with
+ *                        obs_ count > 0 whose voxel is among them, dir[2] >= 0 and isInFrame(pc.cast<int>(), border): its
+ *                        cell int(pc[1] / grid_size) * grid_n_width + int(pc[0] / grid_size) is TYPE_MAP, and the cell's
+ *                        point is the one of least float distance |new_frame_->pos() - pos_| (<= 10000.0f); of equal
+ *                        distances the one latest in the walk: the later key, then the later place in the voxel's list.
+ *                        The TYPE_MAP cells come out in cell order (at most cap): cell_out, point_id_out (-1: no winner,
+ *                        every point of the cell being beyond 10000 m or NaN; the reference would read a null pointer),
+ *                        pc_out (2 doubles, the winner's w2c(pos_)), status_out (ESIKF_RETRIEVE_*) and ref_out: the
+ *                        position in obs_ of the reference feature esikf_vmap_choose_ref would give the kept point (with
+ *                        normal_en it is stored as the point's ref), -1 for the other statuses. *n_cells = their count.
+ *                        With no placed point, or no key, the call returns 0 cells (the reference returns at :354 when
+ *                        feat_map is empty: the caller then inserts no keys into its sub_feat_map either).
+ * ESIKF_ERR_ARG, with nothing written and the store untouched: an id outside the store or placed before (or twice in one
+ * call), a voxel key outside [-2^20, 2^20) (NaN and inf included), a walk key twice or outside that range, a grid with
+ * grid_n_width * grid_size < width - border (or the same for the height), and more cells than cap (*n_cells is then
+ * written, so that the caller can retry). ESIKF_ERR_STATE before esikf_vmap_init, and for esikf_vmap_retrieve without an
+ * esikf_vio_retrieve_scan since the last esikf_vio_set_camera. esikf_vmap_init forgets every placement. With several ranks
+ * every rank holds the whole visual map and applies every call. */
+#define ESIKF_RETRIEVE_KEPT 0       /* passed every test; ref_out is its reference feature */
+#define ESIKF_RETRIEVE_DEPTH 1      /* depth-discontinuous (:640) */
+#define ESIKF_RETRIEVE_NOT_INIT 2   /* !is_normal_initialized_ (:651) */
+#define ESIKF_RETRIEVE_NO_REF 3     /* no reference feature: getCloseViewObs false, or (normal_en) none below FLT_MAX */
+#define ESIKF_RETRIEVE_NO_WINNER 4  /* a TYPE_MAP cell without a point */
+int esikf_vmap_place_points(esikf_ctx *ctx, int32_t n, const int32_t *point_id, const double *pos, const uint8_t *normal_init);
+int esikf_vmap_retrieve(esikf_ctx *ctx, int32_t n_keys, const int32_t *keys, int32_t grid_size, int32_t grid_n_width, int32_t grid_n_height, int32_t border,
+                        int32_t normal_en, int32_t cap, int32_t *n_cells, int32_t *cell_out, int32_t *point_id_out, double *pc_out, int32_t *status_out,
+                        int32_t *ref_out);
+
 /* ---------------------------------------------------------------- multi-GPU (one process per GPU)
  * The residual point / patch set is sharded by contiguous blocks; each iteration all-reduces the
  * packed information buffer [HTH upper | HTz | M | sum|d| ...] and every rank solves redundantly.
