@@ -4,7 +4,9 @@ retrieve_scan, the world cloud of rgb_set_cloud, the sub-map of warp_patches(kee
 between.
 
 1. Size order: on one context every entry point runs at a large size, a small one and the large one again, in the order
-   of a VIO tick; each answer equals, bit for bit, the same call on a fresh context.
+   of a VIO tick; each answer equals, bit for bit, the same call on a fresh context. On a fresh context the observation
+   store is filled a few points per call, so that vmap_score's rows outgrow both its inputs and the pinned block the
+   earlier calls left.
 2. State that outlives a call: retrieve_scan -> depth_check, rgb_set_cloud -> rgb_colorize and warp_patches(keep_on_device)
    -> vio_run, with larger front-end calls in between, equal the same pairs on a fresh context."""
 import numpy as np
@@ -13,6 +15,7 @@ import pytest
 import color_cases as CC
 import generate_cases as GC
 import map_find as MF
+import map_mirror as MM
 import observe_cases as OC
 import refpatch_cases as RFC
 import retrieve_cases as RC
@@ -99,20 +102,55 @@ def _make(name, large):
     if name == "lio":  # a scan to map and to run the LIO update on
         sc = CC.scene(CAMERA, 60_000 if large else 2000, seed=17 if large else 18)
         return dict(pts=sc["pts"], state=sc["lio_state"], ext=sc["ext"])
+    if name == "patch":  # the lio scan's map in esikf_map_upload's form, and records to patch into it
+        d = inputs("lio", large)
+        m = on_fresh_context(lambda c: (_map_build(c, d), c.map_device_download())[1])
+        rng = np.random.default_rng(19 if large else 20)
+        ids = np.sort(rng.choice(len(m["planes"]), size=len(m["planes"]) // 3, replace=False)).astype(np.int32)
+        return dict(map=m, ids=ids, planes=np.ascontiguousarray(m["planes"][rng.permutation(ids)]))
+    if name == "vmap":  # an observation store of the retrieval scene's visual points, and the inputs of its calls
+        sc = inputs("retrieve", large)["sc"]
+        rng = np.random.default_rng(21 if large else 22)
+        n_obs = np.asarray(sc["n_obs"], np.int32)
+        first = np.concatenate([[0], np.cumsum(n_obs)]).astype(np.int32)
+        m, n = int(first[-1]), len(n_obs)
+        T = np.zeros((m, 12))
+        T[:, [0, 4, 8]] = 1.0
+        T[:, 9:] = rng.normal(0, 2.0, (m, 3))
+        normal = rng.normal(size=(n, 3))
+        return dict(sc=sc, first=first, px=rng.uniform(0, 600, (m, 2)), patch=rng.uniform(0, 255, (m, 64)).astype(np.float32), T=T,
+                    id=rng.integers(0, 5, m).astype(np.int32), mean=rng.uniform(0, 200, m).astype(np.float32), score=rng.uniform(0, 1, m).astype(np.float32),
+                    converged=(rng.random(n) < 0.3).astype(np.uint8), normal=normal / np.linalg.norm(normal, axis=1)[:, None])
     raise KeyError(name)
 
 
 # ------------------------------------------------------------------------------------------------------- entry points
 # Each step sets up what its call reads, makes the call(s) and returns the answers.
-def step_lio_fetch_normals(c, large):
-    d = inputs("lio", large)
-    cfg = S.LioCfg()
+def _map_build(c, d):
     c.set_extrinsics(d["ext"])
-    c.map_device_init(cfg, root_capacity=1 << 16, grow=True)
+    c.map_device_init(S.LioCfg(), root_capacity=1 << 16, grow=True)
     c.lio_set_scan(d["pts"])
     c.map_device_build(d["state"])
-    c.lio_run(d["state"], d["state"], cfg)
-    return dict(normals=c.lio_fetch_normals())
+
+
+def step_lio_tick(c, large):
+    d = inputs("lio", large)
+    _map_build(c, d)
+    c.lio_run(d["state"], d["state"], S.LioCfg())
+    body_cov, cross = c.lio_fetch_point_cov()
+    m, e = c.map_device_download(), c.map_device_export()
+    order = np.lexsort(m["keys"].T[::-1])  # the download lists roots in no fixed order
+    planes = np.concatenate([m["planes"][f:f + k] for f, k in zip(m["first"][order], m["count"][order])])
+    return dict(normals=c.lio_fetch_normals(), body_cov=body_cov, cross=cross, keys=m["keys"][order], planes=planes, export=MM.export_dump(e))
+
+
+def step_map_patch(c, large):
+    d, p = inputs("lio", large), inputs("patch", large)
+    cfg = S.LioCfg()
+    c.set_extrinsics(d["ext"])
+    c.map_upload(p["map"], cfg.voxel_size)
+    c.map_patch(p["ids"], p["planes"])
+    return c.lio_update(d["pts"], d["state"], d["state"], cfg)
 
 
 def step_colorize(c, large):
@@ -194,8 +232,36 @@ def step_score(c, large):
     return c.vio_score_ref_patches(r["first"], r["pos"], r["normal"], r["patch"], r["mean"], r["id"], r["T"])
 
 
-# the order of a VIO tick: the LIO tick's normals and coloured scan, the retrieval, the sub-map, the update's new points
-TICK = [step_lio_fetch_normals, step_colorize, step_retrieve, step_find, step_select, step_warp, step_update_points, step_generate, step_score]
+def step_vmap(c, large):
+    """The observation store through a tick: filled a few points per call, scored, edited by the update's new observations,
+    read back, placed and walked."""
+    v = inputs("vmap", large)
+    sc = v["sc"]
+    first, n = v["first"], len(v["first"]) - 1
+    c.set_extrinsics(sc["ext"])
+    c.vio_set_camera(sc["cam"], RC.VIO_CFG)
+    c.vmap_init(1)
+    ids = []
+    for a in range(0, n, 4):
+        f = first[a:a + 5]
+        o = slice(int(f[0]), int(f[-1]))
+        ids.append(c.vmap_add_points(f - f[0], v["px"][o], v["patch"][o], v["T"][o], v["id"][o], v["mean"][o], v["score"][o], np.full(len(f) - 1, -1, np.int32)))
+    ids = np.concatenate(ids)
+    pos, fp = sc["pos"], -(sc["pos"].mean(axis=0))
+    out = dict(score=c.vmap_score(ids, pos, v["normal"]), choose=c.vmap_choose_ref(ids, False, pos=pos, frame_pos=fp))
+    c.vio_set_image(sc["img"])
+    c.vio_set_patches(pos, np.zeros((n, RC.VIO_CFG.levels * 64), np.float32), np.zeros(n, np.int32), np.ones(n))
+    out["update"] = c.vmap_update_points(ids, v["converged"], 3, state=sc["state"])
+    out["download"] = c.vmap_download(ids)
+    c.vmap_place_points(ids, pos)
+    keys = c.vio_retrieve_scan(sc["border"], pg=sc["pg"], state=sc["state"])["keys"]
+    out["retrieve"] = c.vmap_retrieve(keys, *[int(sc[k]) for k in ("grid_size", "grid_n_width", "grid_n_height", "border")], False)
+    return out
+
+
+# the order of a VIO tick: the LIO tick's normals, point covariances and map mirror, a host map patched in place, the coloured
+# scan, the retrieval, the sub-map, the update's new points, the reference patches and the observation store
+TICK = [step_lio_tick, step_map_patch, step_colorize, step_retrieve, step_find, step_select, step_warp, step_update_points, step_generate, step_score, step_vmap]
 
 
 def test_large_small_large_equals_fresh_contexts(ctx):
