@@ -171,55 +171,87 @@ struct esikf_ctx {
   unsigned int *exchange_seq = nullptr;  // device word: exchanges executed so far (the tag of both mailboxes follows it)
   DevBuf<unsigned long long> stamps;  // 8 per slot: 8 LIO slots then 64 VIO slots; debug, LIO per-CTA; the VIO chain stamps
   bool want_stamps = false;
+  // The inputs the entry points read, one group each with one validity marker: `need` checks them, `void_inputs` voids them.
+  // Besides the input it sets, a call voids:
+  //   esikf_vio_set_camera: the retrieval; the image when width or height changed; the sub-map and its inverse refs when
+  //     patch_pyrimid_level changed (re-setting an identical camera voids neither)
+  //   esikf_vio_set_ref_images: the inverse refs (their indices point into the images it releases); esikf_vmap_init: the placement
+  //   esikf_lio_run, esikf_vio_run: the posterior until their launch has succeeded; esikf_lio_run also the normals
+  //   esikf_map_upload: the normals; esikf_map_device_init: the normals and the export
+  //   esikf_map_device_build / update: the export and the pv list until they succeed
+  //   esikf_map_device_update_points: the export, the pv list and the normals; esikf_map_device_slide: the export and the normals
+  //   a device map call that fails: the map, until esikf_map_device_init
+  //   esikf_rgb_set_cloud, esikf_vio_retrieve_scan: the cloud, the retrieval, until they succeed
+  // extrinsics: as set, and extR | extT on the device (what the LIO precompute reads)
   esikf_extrinsics ext{};
-  bool have_ext = false, have_ext_dev = false;
   double ext_host[12] = {};
+  DevBuf<double> ext_dev;
+  bool have_ext = false;
 
-  // map: map.slots / map.planes (the map as uploaded, 256-byte records) / map.recs (what the residual kernel reads, 144-byte
-  // records derived on the device) serve both the host-uploaded and the device-resident map
-  MapArenaBufs map;
-  uint32_t hash_mask = 0;
-  int n_planes = 0, n_roots = 0;
-  double voxel_size = 0.5;
-  bool have_map = false;
+  // camera and VIO config: cam.width == 0 before the first esikf_vio_set_camera
+  esikf_camera cam{};
+  esikf_vio_cfg vio_cfg{};
 
-  // device-resident map (esikf_map_device_*): octree nodes, point lists and refits stay on the GPU
-  bool dev_map = false;
-  esikf_map_cfg map_cfg{};
-  MapCfg arena_cfg{};
-  MapArenaBufs spare;  // esikf_map_device_slide copies the surviving roots into it, then it and `map` change roles
-  DevBuf<int> map_work, map_survivors;
-  DevBuf<unsigned long long> map_demand;  // map_demand_kernel's sums and defer word (capacity growth)
-  DevBuf<double> map_pt, map_pt_normal;
-  DevBuf<unsigned int> map_key_in, map_key_out, map_idx_in, map_idx_out;
-  DevBuf<MapTouched> map_touched;
-  DevBuf<unsigned char> map_sort_tmp;
-  int map_pt_n = 0;            // points the normal snapshot / last map step covers
-  bool map_normals_valid = false;
-  // points of the pv list (pv_list_ after LIVMapper.cpp:413-424) the last esikf_map_device_update left in map_pt (point_w | var)
-  // and map_pt_normal (pv.normal), which esikf_vio_generate_points(point_w = NULL) reads; -1 when map_pt holds anything else
-  int pv_n = -1;
-  int map_hash_bits = 0;
-  esikf_map_stats map_last{};
-  // esikf_map_device_export: points of the last applied tick (its touched list is map_touched, its sorted positions 0..n),
-  // -1 when there is no tick to export (after init, a slide or a failed build / update)
-  int map_export_points = -1;
+  // current image: img_w == 0 when there is none of the camera's size
+  DevBuf<uint8_t> img;
+  int img_w = 0, img_h = 0;
+  VioTma tma;                      // tensor maps of `img` (ESIKF_TUNE_VIO_TMA), encoded for tma_img / tma_w x tma_h
+  const uint8_t *tma_img = nullptr;
+  int tma_w = 0, tma_h = 0;
 
-  // LIO
+  // installed sub-map (set_patches, warp_patches(keep_on_device), select_patches), laid out for submap_levels levels (0: none
+  // installed), and the inverse-compositional references of its first n_inv_refs patches
+  DevBuf<double> vis_pos, inv_expo;
+  DevBuf<float> warp_patch, errors;
+  DevBuf<int32_t> search_levels;
+  int n_patches = 0, submap_levels = 0;
+  DevBuf<double> inv_ref_px, inv_ref_f, inv_ref_R, inv_ref_pos, H_sub_inv;
+  DevBuf<int32_t> inv_ref_idx;
+  int n_inv_refs = 0;
+
+  // reference images of the warp producers: none while ref_imgs is empty
+  std::vector<DevBuf<uint8_t>> ref_imgs;
+  DevBuf<const uint8_t *> ref_img_ptrs;
+  int ref_w = 0, ref_h = 0;
+
+  // resident scan and its precompute: SCAN_SET until an esikf_lio_run ran it; a fresh context's empty one (SCAN_NONE) needs no run
   DevBuf<float> pts;
   DevBuf<double> pre;
   DevBuf<int32_t> match_plane, normal_plane;
   DevBuf<float> dis;
   int n_pts = 0;
   int pre_stride = 0;
-  bool scan_fresh = false;   // precompute pending
+  enum { SCAN_NONE, SCAN_SET, SCAN_RUN } scan = SCAN_NONE;
   double pre_ext[12] = {};   // the extR extT and dept_err / beam_err the precompute in `pre` was made with
   float pre_dept_err = 0.f, pre_beam_err = 0.f;
   esikf_lio_cfg lio_cfg{};
-  DevBuf<double> ext_dev;    // extR(9) extT(3)
   DevBuf<double> lio_slot_block;  // lane slots of the LIO kernels' L2-slot warps: [partial_blocks][LIO_L2_WARPS * 32][SLOT_D]
 
-  // shared update state
+  // voxel map: map.slots / planes (as uploaded, 256-byte records) / recs (what the residual kernel reads, 144 bytes) serve the
+  // host-uploaded and the device-resident map; MAP_DEVICE_VOID: one a failed call voided (only map_device_* calls reach it)
+  enum { MAP_NONE, MAP_HOST, MAP_DEVICE, MAP_DEVICE_VOID } map_kind = MAP_NONE;
+  MapArenaBufs map;
+  uint32_t hash_mask = 0;
+  int n_planes = 0;  // of the host-uploaded map
+  esikf_map_cfg map_cfg{};  // device-resident map (esikf_map_device_*): octree nodes, point lists and refits stay on the GPU
+  MapCfg arena_cfg{};
+  MapArenaBufs spare;  // esikf_map_device_slide copies the surviving roots into it, then it and `map` change roles
+  DevBuf<int> map_work, map_survivors;
+  DevBuf<unsigned long long> map_demand;  // map_demand_kernel's sums and defer word (capacity growth)
+  DevBuf<unsigned int> map_key_in, map_key_out, map_idx_in, map_idx_out;
+  DevBuf<MapTouched> map_touched;
+  DevBuf<unsigned char> map_sort_tmp;
+  int map_hash_bits = 0;
+  esikf_map_stats map_last{};
+
+  // the last map update's points, -1 for none: map_export_points of its tick (touched list map_touched) for map_device_export;
+  // pv_n of its pv list (pv_list_, LIVMapper.cpp:413-424) in map_pt (point_w | var) and map_pt_normal (pv.normal) for
+  // generate_points / retrieve_scan(point_w = NULL); normals_n whose pv.normal of the current LIO run map_pt_normal holds
+  DevBuf<double> map_pt, map_pt_normal;
+  int map_export_points = -1, pv_n = -1, normals_n = -1;
+
+  // last posterior: which update's posterior `state` holds, what a call's state = NULL stands for (state_or_posterior)
+  enum Resident { RESIDENT_NONE, RESIDENT_LIO, RESIDENT_VIO } resident = RESIDENT_NONE;
   DevBuf<double> state_prop;             // [state 386 | prop 386] contiguous: one H2D copy per update
   double *state = nullptr, *prop = nullptr;
   DevBuf<double> info, partials, old_state, G;
@@ -237,51 +269,23 @@ struct esikf_ctx {
   esikf_vio_stats *vio_stats = nullptr;
   int partial_blocks = 0;
 
-  // VIO
-  esikf_camera cam{};
-  esikf_vio_cfg vio_cfg{};
-  bool have_cam = false;
-  DevBuf<uint8_t> img;
-  int img_w = 0, img_h = 0;
-  VioTma tma;                      // tensor maps of `img` (ESIKF_TUNE_VIO_TMA), encoded for tma_img / tma_w x tma_h
-  const uint8_t *tma_img = nullptr;
-  int tma_w = 0, tma_h = 0;
-  DevBuf<double> vis_pos, inv_expo;
-  DevBuf<float> warp_patch, errors;
-  DevBuf<int32_t> search_levels;
-  DevBuf<double> inv_ref_px, inv_ref_f, inv_ref_R, inv_ref_pos, H_sub_inv;  // inverse-compositional variant
-  DevBuf<int32_t> inv_ref_idx;
-  int n_inv_refs = 0;
-  int n_patches = 0;
-  bool have_submap = false;  // a sub-map was installed (set_patches, warp_patches(keep_on_device), select_patches)
-  // reference images of the warp producers
-  std::vector<DevBuf<uint8_t>> ref_imgs;
-  DevBuf<const uint8_t *> ref_img_ptrs;
-  int ref_w = 0, ref_h = 0;
-  // which update's posterior `state` holds: the LIO tick's world cloud (esikf_rgb_set_cloud) and the VIO tick's frame pose
-  // (esikf_rgb_colorize) default to the one their tick left there
-  enum { RESIDENT_NONE, RESIDENT_LIO, RESIDENT_VIO } resident = RESIDENT_NONE;
-
-  // coloured scan (esikf_rgb_*): the world cloud of the last esikf_rgb_set_cloud
+  // coloured cloud (esikf_rgb_*): the world cloud of the last esikf_rgb_set_cloud, rgb_n == -1 when there is none
   DevBuf<float> rgb_cloud;
-  int rgb_n = -1;  // points of the cloud, -1 before esikf_rgb_set_cloud
+  int rgb_n = -1;
 
-  // scan side of the retrieval: the depth image of the last esikf_vio_retrieve_scan and the frame pose it was made with, which
-  // esikf_vio_depth_check reads
+  // retrieval: the depth image of the last esikf_vio_retrieve_scan (ret_w == 0: none) and the frame pose it was made with
   DevBuf<double> ret_state;
   DevBuf<float> ret_depth;
   double ret_Rci[9] = {}, ret_Pci[3] = {};
   int ret_w = 0, ret_h = 0;
-  bool ret_valid = false;  // a depth image and its pose are in place (cleared by esikf_vio_set_camera and by a failed call)
 
-  // the visual map's observation store (esikf_vmap_*, esikf_vmap.cu): vmap_cap point records, the first vmap_points in use
+  // observation store (esikf_vmap_*, esikf_vmap.cu): vmap_cap point records (0: no store), the first vmap_points in use
   DevBuf<uint8_t> vmap;
   int64_t vmap_cap = 0, vmap_points = 0;
-  bool have_vmap = false;
   std::vector<uint32_t> vmap_seen;  // per point, the last call (vmap_epoch) that named it: the repeated-id check in O(n)
   uint32_t vmap_epoch = 0;
-  // the device feat_map of the store's points (esikf_vmap_place_points, esikf_vretrieve.cu): vpl_cap point records, ids below
-  // vpl_hi possibly placed, vpl_placed of them placed (the next sequence number); vpl_done mirrors which
+  // placement: the device feat_map of the store's points (esikf_vmap_place_points, esikf_vretrieve.cu): vpl_cap point records,
+  // ids below vpl_hi possibly placed, vpl_placed of them placed (the next sequence number); vpl_done mirrors which
   DevBuf<uint8_t> vpl;
   int64_t vpl_cap = 0, vpl_hi = 0, vpl_placed = 0;
   std::vector<uint8_t> vpl_done;
@@ -341,6 +345,53 @@ static int fail(esikf_ctx *c, int code, const char *fmt, ...) {
     cudaError_t e__ = (call);                                                                                      \
     if (e__ != cudaSuccess) return fail(ctx, ESIKF_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e__), __FILE__, __LINE__); \
   } while (0)
+
+// The inputs of the context's groups (esikf_ctx), one bit each.
+enum Input : unsigned {
+  IN_EXT = 1u << 0, IN_CAMERA = 1u << 1, IN_IMAGE = 1u << 2, IN_SUBMAP = 1u << 3, IN_INV_REFS = 1u << 4, IN_REF_IMAGES = 1u << 5,
+  IN_SCAN = 1u << 6, IN_RUN_SCAN = 1u << 7, IN_MAP = 1u << 8, IN_HOST_MAP = 1u << 9, IN_DEVICE_MAP = 1u << 10, IN_EXPORT = 1u << 11,
+  IN_PV_LIST = 1u << 12, IN_NORMALS = 1u << 13, IN_CLOUD = 1u << 14, IN_RETRIEVAL = 1u << 15, IN_STORE = 1u << 16, IN_POSTERIOR = 1u << 17,
+};
+
+// The one check of each input: ESIKF_ERR_STATE naming `call` and the first of `inputs` missing (the posterior: state_or_posterior).
+static int need(esikf_ctx *ctx, const char *call, unsigned inputs) {
+  const esikf_ctx &c = *ctx;
+  const struct { unsigned in; bool ok; const char *missing; } rules[] = {
+      {IN_EXT, c.have_ext, "no extrinsics (set_extrinsics)"},
+      {IN_CAMERA, c.cam.width != 0, "no camera (vio_set_camera)"},
+      {IN_IMAGE, c.img_w != 0, "no image of the camera's size (vio_set_image)"},
+      {IN_SUBMAP, c.submap_levels == c.vio_cfg.patch_pyrimid_level, "no visual sub-map laid out for the camera's level count"},
+      {IN_INV_REFS, c.n_inv_refs == c.n_patches && c.ref_w == c.cam.width && c.ref_h == c.cam.height, "no inverse refs for every patch, or reference images of another size"},
+      {IN_REF_IMAGES, !c.ref_imgs.empty(), "no reference images (set_ref_images)"},
+      {IN_SCAN, c.scan != esikf_ctx::SCAN_NONE, "no resident scan (esikf_lio_set_scan)"},
+      {IN_RUN_SCAN, c.scan != esikf_ctx::SCAN_SET, "the resident scan has not been through esikf_lio_run yet"},
+      {IN_MAP, c.map_kind == esikf_ctx::MAP_HOST || c.map_kind == esikf_ctx::MAP_DEVICE, "no live map (map_upload, esikf_map_device_init)"},
+      {IN_HOST_MAP, c.map_kind == esikf_ctx::MAP_HOST, "no host-uploaded map (map_upload); a device-resident map refits itself"},
+      {IN_DEVICE_MAP, c.map_kind >= esikf_ctx::MAP_DEVICE, "no device-resident map (esikf_map_device_init)"},
+      {IN_EXPORT, c.map_export_points >= 0, "no build / update to export (the map was initialised or slid since, or the last one failed)"},
+      {IN_PV_LIST, c.pv_n >= 0, "no esikf_map_device_update of the resident scan left its points on the device"},
+      {IN_CLOUD, c.rgb_n >= 0, "no cloud (rgb_set_cloud)"},
+      {IN_RETRIEVAL, c.ret_w != 0, "no esikf_vio_retrieve_scan since the last vio_set_camera"},
+      {IN_STORE, c.vmap_cap != 0, "no observation store (esikf_vmap_init)"},
+  };
+  for (const auto &r : rules)
+    if ((inputs & r.in) && !r.ok) return fail(ctx, ESIKF_ERR_STATE, "%s: %s", call, r.missing);
+  return ESIKF_OK;
+}
+
+// The one way to void an input; the table at esikf_ctx says when. A voided device map stays reachable to map_device_* calls.
+static void void_inputs(esikf_ctx *ctx, unsigned inputs) {
+  if (inputs & IN_IMAGE) ctx->img_w = ctx->img_h = 0;
+  if (inputs & IN_SUBMAP) ctx->submap_levels = 0;
+  if (inputs & (IN_SUBMAP | IN_INV_REFS)) ctx->n_inv_refs = 0;
+  if (inputs & IN_MAP) ctx->map_kind = esikf_ctx::MAP_DEVICE_VOID;
+  if (inputs & IN_EXPORT) ctx->map_export_points = -1;
+  if (inputs & IN_PV_LIST) ctx->pv_n = -1;
+  if (inputs & IN_NORMALS) ctx->normals_n = -1;
+  if (inputs & IN_CLOUD) ctx->rgb_n = -1;
+  if (inputs & IN_RETRIEVAL) ctx->ret_w = ctx->ret_h = 0;
+  if (inputs & IN_POSTERIOR) ctx->resident = esikf_ctx::RESIDENT_NONE;
+}
 
 // One call's layout of the scratch: its host inputs first, then its work arrays, then its answers as one span that ends the
 // layout. `lay` marks where the inputs end and where the answers begin.
@@ -570,16 +621,16 @@ int esikf_set_tuning(esikf_ctx *ctx, uint32_t flags) {
 int esikf_set_extrinsics(esikf_ctx *ctx, const esikf_extrinsics *ext) {
   if (!ctx || !ext) return ESIKF_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  ctx->ext = *ext;
-  ctx->have_ext = true;
   double h[12];
   memcpy(h, ext->extR, 9 * sizeof(double));
   memcpy(h + 9, ext->extT, 3 * sizeof(double));
-  if (ctx->have_ext_dev && memcmp(h, ctx->ext_host, sizeof(h)) == 0) return ESIKF_OK;  // unchanged (the shim sets it every tick): nothing to do
-  CK(cudaMemcpyAsync(ctx->ext_dev.p, h, sizeof(h), cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));  // `h` is a stack buffer
-  memcpy(ctx->ext_host, h, sizeof(h));
-  ctx->have_ext_dev = true;
+  if (!ctx->have_ext || memcmp(h, ctx->ext_host, sizeof(h)) != 0) {  // unchanged (the shim sets it every tick): nothing to upload
+    CK(cudaMemcpyAsync(ctx->ext_dev.p, h, sizeof(h), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));  // `h` is a stack buffer
+    memcpy(ctx->ext_host, h, sizeof(h));
+  }
+  ctx->ext = *ext;
+  ctx->have_ext = true;
   return ESIKF_OK;
 }
 
@@ -628,17 +679,15 @@ int esikf_map_upload(esikf_ctx *ctx, const int64_t *keys, const int32_t *first, 
   }
   CK(cudaStreamSynchronize(ctx->stream));
   ctx->hash_mask = cap - 1;
-  ctx->n_planes = n_planes, ctx->n_roots = n_roots;
-  ctx->voxel_size = voxel_size;
-  ctx->have_map = true;
-  ctx->dev_map = false;  // a host-flattened map replaces a device-resident one
+  ctx->n_planes = n_planes;
+  ctx->map_kind = esikf_ctx::MAP_HOST;  // a host-flattened map replaces a device-resident one
+  void_inputs(ctx, IN_NORMALS);
   return ESIKF_OK;
 }
 
 int esikf_map_patch(esikf_ctx *ctx, const int32_t *plane_ids, const esikf_plane *planes, int32_t n) {
   if (!ctx || n < 0 || (n > 0 && (!plane_ids || !planes))) return fail(ctx, ESIKF_ERR_ARG, "map_patch: bad argument");
-  if (!ctx->have_map) return fail(ctx, ESIKF_ERR_STATE, "map_patch before map_upload");
-  if (ctx->dev_map) return fail(ctx, ESIKF_ERR_STATE, "map_patch: the map is device-resident (esikf_map_device_init); it refits itself");
+  if (int rc = need(ctx, "map_patch", IN_HOST_MAP)) return rc;
   CK(cudaSetDevice(ctx->device));
   for (int i = 0; i < n; i++)
     if (plane_ids[i] < 0 || plane_ids[i] >= ctx->n_planes) return fail(ctx, ESIKF_ERR_ARG, "map_patch: plane id %d", plane_ids[i]);
@@ -673,10 +722,8 @@ static int map_check_errors(esikf_ctx *ctx, const char *what) {
   CK(cudaStreamSynchronize(ctx->stream));
   ctx->map_last.nodes = c[0], ctx->map_last.records = c[1], ctx->map_last.errors = c[2], ctx->map_last.roots = c[3];
   ctx->map_last.pool_points = (int64_t)pool_used, ctx->map_last.touched_roots = work[0];
-  ctx->n_planes = c[1] < ctx->map.rec_cap ? c[1] : ctx->map.rec_cap;
-  ctx->n_roots = c[3];
   if (c[2]) {
-    ctx->have_map = false;  // the map is not trustworthy any more: the next lio_run must not use it
+    void_inputs(ctx, IN_MAP);  // the map is not trustworthy any more: the next lio_run must not use it
     return fail(ctx, ESIKF_ERR_STATE, "%s: device map capacity exceeded (flags 0x%x:%s%s%s%s%s%s) — raise the esikf_map_cfg capacities and rebuild", what, c[2],
                 (c[2] & MAP_ERR_NODES) ? " nodes" : "", (c[2] & MAP_ERR_POOL) ? " point-pool" : "", (c[2] & MAP_ERR_RECS) ? " records" : "",
                 (c[2] & MAP_ERR_HASH) ? " hash" : "", (c[2] & MAP_ERR_KEY) ? " key-range" : "", (c[2] & MAP_ERR_STACK) ? " octree-depth" : "");
@@ -712,11 +759,8 @@ int esikf_map_device_init(esikf_ctx *ctx, const esikf_map_cfg *cfg) {
   ctx->map_cfg = *cfg;
   ctx->map_hash_bits = bits;
   ctx->hash_mask = cap - 1;
-  ctx->voxel_size = cfg->voxel_size;
-  ctx->n_planes = 0, ctx->n_roots = 0;
-  ctx->dev_map = true, ctx->have_map = true;  // an empty map is a valid map (nothing matches)
-  ctx->map_normals_valid = false;
-  ctx->map_export_points = -1;
+  ctx->map_kind = esikf_ctx::MAP_DEVICE;  // an empty map is a valid map (nothing matches)
+  void_inputs(ctx, IN_NORMALS | IN_EXPORT);
   memset(&ctx->map_last, 0, sizeof(ctx->map_last));
   return ESIKF_OK;
 }
@@ -745,9 +789,9 @@ static int map_replay_tick(esikf_ctx *ctx, int n, bool build) {
   return ESIKF_OK;
 }
 
-static int map_capacity_error(esikf_ctx *ctx, const char *what, const char *resource, long long need) {
-  ctx->have_map = false;
-  return fail(ctx, ESIKF_ERR_STATE, "%s: the device map cannot grow to %lld %s (the limit is 2^31)", what, need, resource);
+static int map_capacity_error(esikf_ctx *ctx, const char *what, const char *resource, long long want) {
+  void_inputs(ctx, IN_MAP);
+  return fail(ctx, ESIKF_ERR_STATE, "%s: the device map cannot grow to %lld %s (the limit is 2^31)", what, want, resource);
 }
 
 // Capacity growth: copy the live arena into one of the given capacities with the slide's machinery and an unbounded box (the
@@ -765,7 +809,7 @@ static int map_grow(esikf_ctx *ctx, long long hash_cap, long long node_cap, long
   if (e == cudaSuccess) e = ctx->map_survivors.reserve((size_t)(ctx->map_last.roots > 0 ? ctx->map_last.roots : 1) + 1);
   if (e != cudaSuccess) {
     cudaGetLastError();  // a failed allocation is not sticky: later calls must not report it again
-    ctx->have_map = false;
+    void_inputs(ctx, IN_MAP);
     return fail(ctx, ESIKF_ERR_CUDA, "%s: growing the device map to %lld hash slots / %lld nodes / %lld records / %lld points failed: %s", what, hash_cap, node_cap,
                 rec_cap, pool_cap, cudaGetErrorString(e));
   }
@@ -814,7 +858,7 @@ static int map_apply_points(esikf_ctx *ctx, int n, bool build) {
   CK(cudaMemcpyAsync(d, ctx->map_demand.p, sizeof(d), cudaMemcpyDeviceToHost, st));
   if ((rc = map_check_errors(ctx, what))) return rc;
   if (d[5]) {  // the grown arena holds used + demand of every short resource: the bound itself would be broken
-    ctx->have_map = false;
+    void_inputs(ctx, IN_MAP);
     return fail(ctx, ESIKF_ERR_STATE, "%s: the tick was deferred again after the map grew (flags 0x%x)", what, (unsigned)d[5]);
   }
   return ESIKF_OK;
@@ -831,20 +875,11 @@ static int map_reserve_tick(esikf_ctx *ctx, int n) {
   return ESIKF_OK;
 }
 
-// map_apply_points and, when it succeeded, the tick esikf_map_device_export exports
-static int map_apply_exported(esikf_ctx *ctx, int n, bool build) {
-  const int rc = map_apply_points(ctx, n, build);
-  if (!rc) ctx->map_export_points = n;
-  return rc;
-}
-
 static int map_from_scan(esikf_ctx *ctx, const double *state, bool build) {
   if (!ctx) return ESIKF_ERR_ARG;
-  ctx->map_export_points = -1;
-  ctx->pv_n = -1;  // map_pt is rewritten below
-  if (!ctx->dev_map) return fail(ctx, ESIKF_ERR_STATE, "map_device_%s before esikf_map_device_init", build ? "build" : "update");
-  if (!ctx->have_ext) return fail(ctx, ESIKF_ERR_STATE, "map_device_%s before set_extrinsics", build ? "build" : "update");
-  if (!build && ctx->scan_fresh) return fail(ctx, ESIKF_ERR_STATE, "map_device_update: the resident scan has not been through esikf_lio_run yet");
+  const char *what = build ? "map_device_build" : "map_device_update";
+  void_inputs(ctx, IN_EXPORT | IN_PV_LIST);  // map_pt is rewritten below
+  if (int rc = need(ctx, what, IN_DEVICE_MAP | IN_EXT | (build ? 0 : IN_RUN_SCAN))) return rc;
   if (build && ctx->map_last.roots > 0) return fail(ctx, ESIKF_ERR_STATE, "map_device_build needs an empty map (esikf_map_device_init resets it)");
   CK(cudaSetDevice(ctx->device));
   const int n = ctx->n_pts;
@@ -866,7 +901,7 @@ static int map_from_scan(esikf_ctx *ctx, const double *state, bool build) {
       ctx->launches++;
       match_plane = nullptr;
     }
-    if ((rc = map_grow_hash(ctx, n, build ? "map_device_build" : "map_device_update"))) return rc;
+    if ((rc = map_grow_hash(ctx, n, what))) return rc;
   }
   MapPointArgs a;
   memset(&a, 0, sizeof(a));
@@ -876,10 +911,9 @@ static int map_from_scan(esikf_ctx *ctx, const double *state, bool build) {
   a.match_plane = match_plane, a.recs = ctx->map.recs.p, a.pt_normal = ctx->map_pt_normal.p;
   a.pt = ctx->map_pt.p, a.pt_slot = ctx->map_key_in.p, a.pt_idx = ctx->map_idx_in.p, a.invalid_slot = ctx->map.hash_cap;
   map_points_kernel<<<(n + 255) / 256, 256, 0, st>>>(ctx->arena(), a);
-  ctx->map_pt_n = n, ctx->map_normals_valid = !build;
-  rc = map_apply_exported(ctx, n, build);
-  if (!rc && !build) ctx->pv_n = n;
-  return rc;
+  ctx->normals_n = build ? -1 : n;
+  if ((rc = map_apply_points(ctx, n, build))) return rc;
+  return ctx->map_export_points = n, ctx->pv_n = build ? -1 : n, ESIKF_OK;
 }
 
 int esikf_map_device_build(esikf_ctx *ctx, const double *state) {
@@ -889,9 +923,9 @@ int esikf_map_device_build(esikf_ctx *ctx, const double *state) {
 int esikf_map_device_update(esikf_ctx *ctx, const double *state) { return map_from_scan(ctx, state, false); }
 
 int esikf_map_device_update_points(esikf_ctx *ctx, const double *point_w, const double *var, int32_t n) {
-  if (ctx) ctx->map_export_points = -1, ctx->pv_n = -1;
+  if (ctx) void_inputs(ctx, IN_EXPORT | IN_PV_LIST);
   if (!ctx || n < 0 || (n > 0 && (!point_w || !var))) return fail(ctx, ESIKF_ERR_ARG, "map_device_update_points: bad argument");
-  if (!ctx->dev_map) return fail(ctx, ESIKF_ERR_STATE, "map_device_update_points before esikf_map_device_init");
+  if (int rc = need(ctx, "map_device_update_points", IN_DEVICE_MAP)) return rc;
   if (n == 0) return ctx->map_export_points = 0, ESIKF_OK;
   CK(cudaSetDevice(ctx->device));
   int rc = map_reserve_tick(ctx, n);
@@ -903,15 +937,16 @@ int esikf_map_device_update_points(esikf_ctx *ctx, const double *point_w, const 
   if (map_hash_short(ctx, n) && (rc = map_grow_hash(ctx, n, "map_device_update"))) return rc;
   map_keys_kernel<<<(n + 255) / 256, 256, 0, st>>>(ctx->arena(), ctx->map_pt.p, n, ctx->map_key_in.p, ctx->map_idx_in.p, ctx->map.hash_cap);
   ctx->launches++;
-  ctx->map_normals_valid = false;
-  return map_apply_exported(ctx, n, false);
+  void_inputs(ctx, IN_NORMALS);
+  if ((rc = map_apply_points(ctx, n, false))) return rc;
+  return ctx->map_export_points = n, ESIKF_OK;
 }
 
 // mapSliding / clearMemOutOfMap (src/voxel_map.cpp:924-971)
 int esikf_map_device_slide(esikf_ctx *ctx, const int64_t key_min[3], const int64_t key_max[3]) {
   if (!ctx) return ESIKF_ERR_ARG;
-  ctx->map_export_points = -1;
-  if (!ctx->dev_map) return fail(ctx, ESIKF_ERR_STATE, "map_device_slide before esikf_map_device_init");
+  void_inputs(ctx, IN_EXPORT);
+  if (int rc = need(ctx, "map_device_slide", IN_DEVICE_MAP)) return rc;
   CK(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
   const MapArenaBufs &live = ctx->map;
@@ -930,13 +965,13 @@ int esikf_map_device_slide(esikf_ctx *ctx, const int64_t key_min[3], const int64
   CK(cudaGetLastError());
   // the fresh arena becomes the map (also when the copy reports an error: the status says so and the map is invalidated)
   std::swap(ctx->map, ctx->spare);
-  ctx->map_normals_valid = false;  // record positions of the last update are gone
+  void_inputs(ctx, IN_NORMALS);  // record positions of the last update are gone
   return map_check_errors(ctx, "map_device_slide");
 }
 
 int esikf_map_device_capacity(esikf_ctx *ctx, esikf_map_cfg *out) {
   if (!ctx || !out) return fail(ctx, ESIKF_ERR_ARG, "map_device_capacity: bad argument");
-  if (!ctx->dev_map) return fail(ctx, ESIKF_ERR_STATE, "map_device_capacity before esikf_map_device_init");
+  if (int rc = need(ctx, "map_device_capacity", IN_DEVICE_MAP)) return rc;
   out->root_capacity = ctx->map.hash_cap / 2, out->node_capacity = ctx->map.node_cap;
   out->record_capacity = ctx->map.rec_cap, out->point_capacity = ctx->map.pool_cap;
   out->grow = ctx->map_cfg.grow;
@@ -945,7 +980,7 @@ int esikf_map_device_capacity(esikf_ctx *ctx, esikf_map_cfg *out) {
 
 int esikf_map_device_stats(esikf_ctx *ctx, esikf_map_stats *out) {
   if (!ctx || !out) return fail(ctx, ESIKF_ERR_ARG, "map_device_stats: bad argument");
-  if (!ctx->dev_map) return fail(ctx, ESIKF_ERR_STATE, "map_device_stats before esikf_map_device_init");
+  if (int rc = need(ctx, "map_device_stats", IN_DEVICE_MAP)) return rc;
   *out = ctx->map_last;
   return ESIKF_OK;
 }
@@ -953,7 +988,7 @@ int esikf_map_device_stats(esikf_ctx *ctx, esikf_map_stats *out) {
 int esikf_map_device_download(esikf_ctx *ctx, int64_t *keys, int32_t *first, int32_t *count, int32_t roots_cap, esikf_plane *planes, int32_t planes_cap, int32_t *n_roots,
                               int32_t *n_planes) {
   if (!ctx || !n_roots || !n_planes) return fail(ctx, ESIKF_ERR_ARG, "map_device_download: bad argument");
-  if (!ctx->dev_map) return fail(ctx, ESIKF_ERR_STATE, "map_device_download before esikf_map_device_init");
+  if (int rc = need(ctx, "map_device_download", IN_DEVICE_MAP)) return rc;
   CK(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
   const bool fill = keys && first && count && planes && roots_cap > 0;
@@ -987,9 +1022,7 @@ int esikf_map_device_download(esikf_ctx *ctx, int64_t *keys, int32_t *first, int
 int esikf_map_device_export(esikf_ctx *ctx, int64_t *keys, int32_t *first, int32_t *count, int32_t roots_cap, esikf_map_node *nodes, int32_t nodes_cap, int32_t *n_roots,
                             int32_t *n_nodes) {
   if (!ctx || !n_roots || !n_nodes) return fail(ctx, ESIKF_ERR_ARG, "map_device_export: bad argument");
-  if (!ctx->dev_map) return fail(ctx, ESIKF_ERR_STATE, "map_device_export before esikf_map_device_init");
-  if (ctx->map_export_points < 0)
-    return fail(ctx, ESIKF_ERR_STATE, "map_device_export: no build / update to export (the map was initialised or slid since, or the last one failed)");
+  if (int rc = need(ctx, "map_device_export", IN_DEVICE_MAP | IN_EXPORT)) return rc;
   *n_roots = 0, *n_nodes = 0;
   const int n = ctx->map_export_points;
   if (n == 0) return ESIKF_OK;
@@ -1038,8 +1071,7 @@ int esikf_map_device_export(esikf_ctx *ctx, int64_t *keys, int32_t *first, int32
 int esikf_map_device_find(esikf_ctx *ctx, const double *points, int32_t n, int32_t rule, uint8_t *status, int64_t *keys, esikf_plane *rows) {
   if (!ctx || n < 0 || (rule != ESIKF_FIND_RULE_PATCH && rule != ESIKF_FIND_RULE_RAYCAST) || (n > 0 && (!points || !status || !keys || !rows)))
     return fail(ctx, ESIKF_ERR_ARG, "map_device_find: bad argument");
-  if (!ctx->dev_map || !ctx->have_map)
-    return fail(ctx, ESIKF_ERR_STATE, "map_device_find: no live device map (esikf_map_device_init first; a failed call or esikf_map_upload voids it)");
+  if (int rc = need(ctx, "map_device_find", IN_DEVICE_MAP | IN_MAP)) return rc;
   if (n == 0) return ESIKF_OK;
   CK(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
@@ -1073,7 +1105,7 @@ __global__ void gather_normals_kernel(const int32_t *__restrict__ match_plane, c
 }
 int esikf_lio_fetch_normals(esikf_ctx *ctx, double *normals) {
   if (!ctx || !normals) return fail(ctx, ESIKF_ERR_ARG, "lio_fetch_normals: bad argument");
-  if (!ctx->have_map || ctx->scan_fresh) return fail(ctx, ESIKF_ERR_STATE, "lio_fetch_normals before lio_run");
+  if (int rc = need(ctx, "lio_fetch_normals", IN_MAP | IN_RUN_SCAN)) return rc;
   CK(cudaSetDevice(ctx->device));
   const int n = ctx->n_pts;
   if (n == 0) return ESIKF_OK;
@@ -1081,7 +1113,7 @@ int esikf_lio_fetch_normals(esikf_ctx *ctx, double *normals) {
   auto lay = [&](CallLayout &s) { s.begin_answers(), normal = s.take<double>((size_t)n * 3 + 4); };
   CK(lay_out_scratch(ctx, lay));
   const double *src = ctx->map_pt_normal.p;
-  if (!(ctx->dev_map && ctx->map_normals_valid && ctx->map_pt_n == n)) {
+  if (ctx->normals_n != n) {
     gather_normals_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(ctx->normal_plane.p, ctx->map.recs.p, n, normal);
     ctx->launches++;
     src = normal;
@@ -1102,7 +1134,7 @@ int esikf_lio_set_scan(esikf_ctx *ctx, const float *pts_xyz, int32_t n) {
   CK(ctx->dis.reserve(n + 1));
   if (n) CK(cudaMemcpyAsync(ctx->pts.p, pts_xyz, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
   ctx->n_pts = n;
-  ctx->scan_fresh = true;
+  ctx->scan = esikf_ctx::SCAN_SET;
   return ESIKF_OK;
 }
 
@@ -1115,7 +1147,7 @@ static void lio_precompute(esikf_ctx *ctx, float dept_err, float beam_err) {
   ctx->pre_dept_err = dept_err, ctx->pre_beam_err = beam_err;
 }
 static bool lio_precompute_current(const esikf_ctx *ctx, float dept_err, float beam_err) {
-  return !ctx->scan_fresh && memcmp(ctx->pre_ext, ctx->ext_host, sizeof(ctx->pre_ext)) == 0 && ctx->pre_dept_err == dept_err && ctx->pre_beam_err == beam_err;
+  return ctx->scan != esikf_ctx::SCAN_SET && memcmp(ctx->pre_ext, ctx->ext_host, sizeof(ctx->pre_ext)) == 0 && ctx->pre_dept_err == dept_err && ctx->pre_beam_err == beam_err;
 }
 
 static int lio_fill_args(esikf_ctx *ctx, LioKernelArgs &ka, double *state_ptr) {
@@ -1150,6 +1182,7 @@ static int lio_grid(const esikf_ctx *ctx, int count) {
 }
 // Stage the two packed states of an update in pinned memory and upload them with ONE copy ([state | prop] is contiguous).
 static int upload_states(esikf_ctx *ctx, const double *state_in, const double *state_prop) {
+  void_inputs(ctx, IN_POSTERIOR);  // until the update's launch has succeeded
   const unsigned slot = ctx->stage_idx++ % esikf_ctx::STAGE_SLOTS;
   CK(cudaEventSynchronize(ctx->stage_ev[slot]));  // the copy that last used this slot has been consumed
   double *h = ctx->stage + (size_t)slot * 2 * S_N;
@@ -1187,7 +1220,7 @@ static bool persistent_update(const esikf_ctx *ctx, int coop_blocks) {
 // VioKernelArgs, `tail` the VIO-only arguments. Both instantiations get the same argument list, so the single-GPU
 // launch passes exactly what the peer launch does. `stamp_off` / `stamp_words`: this kernel's slice of the phase stamps.
 static int launch_persistent(esikf_ctx *ctx, const void *fn, const void *fn_peer, const char *name, int grid, int threads, size_t smem, void *ka, SolveArgs &sa,
-                             size_t stamp_off, size_t stamp_words, bool &timed, std::initializer_list<void *> tail) {
+                             size_t stamp_off, size_t stamp_words, bool &timed, std::initializer_list<void *> tail, esikf_ctx::Resident posterior) {
   const unsigned par = ctx->launch_parity & 1;
   GridSync gs;
   gs.barrier = ctx->barrier.p + 64 * par, gs.barrier_next = ctx->barrier.p + 64 * (par ^ 1);  // this launch's barrier / the next launch's (zeroed by the kernel)
@@ -1203,24 +1236,20 @@ static int launch_persistent(esikf_ctx *ctx, const void *fn, const void *fn_peer
   if (le != cudaSuccess) return fail(ctx, ESIKF_ERR_CUDA, "cooperative launch of %s failed: %s", name, cudaGetErrorString(le));
   ctx->launch_parity++;  // only a launch that happened consumes its barrier counter (the kernel zeroes the other one)
   ctx->launches += 1;
+  ctx->resident = posterior;  // what `state` holds once the launch has happened
   timed = false;
   return ESIKF_OK;
 }
 
 int esikf_lio_run(esikf_ctx *ctx, const double *state_in, const double *state_prop, const esikf_lio_cfg *cfg) {
   if (!ctx || !state_in || !state_prop || !cfg) return fail(ctx, ESIKF_ERR_ARG, "lio_run: null argument");
-  if (!ctx->have_map) return fail(ctx, ESIKF_ERR_STATE, "lio_run before map_upload");
-  if (!ctx->have_ext) return fail(ctx, ESIKF_ERR_STATE, "lio_run before set_extrinsics");
-  ctx->map_normals_valid = false;  // a snapshot of pv.normal belongs to the update it was taken after
+  if (int rc = need(ctx, "lio_run", IN_MAP | IN_EXT)) return rc;
+  void_inputs(ctx, IN_NORMALS);  // a snapshot of pv.normal belongs to the update it was taken after
   if (cfg->max_iterations < 1 || cfg->max_iterations > 8) return fail(ctx, ESIKF_ERR_ARG, "lio_run: max_iterations must be in [1,8]");
   CK(cudaSetDevice(ctx->device));
   ctx->lio_cfg = *cfg;
   cudaStream_t st = ctx->stream;
-  {
-    int rc = upload_states(ctx, state_in, state_prop);
-    if (rc) return rc;
-  }
-  ctx->resident = esikf_ctx::RESIDENT_LIO;
+  if (int rc = upload_states(ctx, state_in, state_prop)) return rc;
   const bool fused_lio = persistent_update(ctx, ctx->coop_lio);
   // the persistent kernel initialises its own loop control / stats / barrier; the per-iteration path needs them zeroed
   if (!fused_lio) CK(cudaMemsetAsync(ctx->lio_stats, 0, sizeof(esikf_lio_stats) + sizeof(Ctrl) + 64, st));
@@ -1231,7 +1260,7 @@ int esikf_lio_run(esikf_ctx *ctx, const double *state_in, const double *state_pr
       lio_precompute(ctx, dept_err, beam_err);
       ctx->launches++;
     }
-    ctx->scan_fresh = false;
+    if (ctx->scan == esikf_ctx::SCAN_SET) ctx->scan = esikf_ctx::SCAN_RUN;
   }
   LioKernelArgs ka;
   lio_fill_args(ctx, ka, ctx->state);
@@ -1241,10 +1270,10 @@ int esikf_lio_run(esikf_ctx *ctx, const double *state_in, const double *state_pr
   const bool l2_slots = lio_use_l2_slots(ka.count, grid);
   if (fused_lio && l2_slots)
     return launch_persistent(ctx, (const void *)lio_update_kernel<false, LIO_L2_WARPS>, (const void *)lio_update_kernel<true, LIO_L2_WARPS>, "lio_update_kernel", grid,
-                             LioSmem<LIO_L2_WARPS>::THREADS, sizeof(LioSmem<LIO_L2_WARPS>), &ka, sa, 0, 64, ctx->lio_timed, {});
+                             LioSmem<LIO_L2_WARPS>::THREADS, sizeof(LioSmem<LIO_L2_WARPS>), &ka, sa, 0, 64, ctx->lio_timed, {}, esikf_ctx::RESIDENT_LIO);
   if (fused_lio)
     return launch_persistent(ctx, (const void *)lio_update_kernel<false, 0>, (const void *)lio_update_kernel<true, 0>, "lio_update_kernel", grid, LioSmem<0>::THREADS,
-                             sizeof(LioSmem<0>), &ka, sa, 0, 64, ctx->lio_timed, {});
+                             sizeof(LioSmem<0>), &ka, sa, 0, 64, ctx->lio_timed, {}, esikf_ctx::RESIDENT_LIO);
   ctx->lio_timed = ctx->timing;
   ctx->lio_slots = cfg->max_iterations;
   for (int it = 0; it < cfg->max_iterations; it++) {
@@ -1260,6 +1289,7 @@ int esikf_lio_run(esikf_ctx *ctx, const double *state_in, const double *state_pr
     ctx->launches += 2;
   }
   CK(cudaGetLastError());
+  ctx->resident = esikf_ctx::RESIDENT_LIO;
   return ESIKF_OK;
 }
 
@@ -1315,7 +1345,7 @@ __global__ void expand_point_cov_kernel(const double *__restrict__ pre, int pre_
 
 int esikf_lio_fetch_point_cov(esikf_ctx *ctx, double *body_cov9, double *cross_mat9) {
   if (!ctx) return ESIKF_ERR_ARG;
-  if (ctx->scan_fresh) return fail(ctx, ESIKF_ERR_STATE, "fetch_point_cov before lio_run");
+  if (int rc = need(ctx, "fetch_point_cov", IN_RUN_SCAN)) return rc;
   CK(cudaSetDevice(ctx->device));
   const int n = ctx->n_pts;
   if (n == 0) return ESIKF_OK;
@@ -1338,16 +1368,16 @@ int esikf_vio_set_camera(esikf_ctx *ctx, const esikf_camera *cam, const esikf_vi
   if (cam->model < 0 || cam->model > 1 || cam->width <= 0 || cam->height <= 0) return fail(ctx, ESIKF_ERR_ARG, "vio_set_camera: bad camera");
   if (cfg->patch_pyrimid_level < 1 || cfg->patch_pyrimid_level > 8 || cfg->max_iterations < 1 || cfg->max_iterations > 8 || !(cfg->img_point_cov > 0))
     return fail(ctx, ESIKF_ERR_ARG, "vio_set_camera: bad vio cfg");
+  const bool resized = cam->width != ctx->cam.width || cam->height != ctx->cam.height;  // a first camera voids no sub-map
+  void_inputs(ctx, IN_RETRIEVAL | (resized ? IN_IMAGE : 0) | (ctx->cam.width && cfg->patch_pyrimid_level != ctx->vio_cfg.patch_pyrimid_level ? IN_SUBMAP : 0));
   ctx->cam = *cam;
   ctx->vio_cfg = *cfg;
-  ctx->have_cam = true;
-  ctx->ret_valid = false;
   return ESIKF_OK;
 }
 
 int esikf_vio_set_image(esikf_ctx *ctx, const uint8_t *img, int32_t width, int32_t height) {
   if (!ctx || !img || width <= 0 || height <= 0) return fail(ctx, ESIKF_ERR_ARG, "vio_set_image: bad argument");
-  if (!ctx->have_cam) return fail(ctx, ESIKF_ERR_STATE, "vio_set_image before vio_set_camera");
+  if (int rc = need(ctx, "vio_set_image", IN_CAMERA)) return rc;
   if (width != ctx->cam.width || height != ctx->cam.height) return fail(ctx, ESIKF_ERR_ARG, "vio_set_image: image is %dx%d, camera %dx%d", width, height, ctx->cam.width, ctx->cam.height);
   CK(cudaSetDevice(ctx->device));
   CK(ctx->img.reserve((size_t)width * height + 64));
@@ -1358,7 +1388,7 @@ int esikf_vio_set_image(esikf_ctx *ctx, const uint8_t *img, int32_t width, int32
 
 int esikf_vio_set_patches(esikf_ctx *ctx, const double *pos, const float *warp_patch, const int32_t *search_levels, const double *inv_expo_list, int32_t n) {
   if (!ctx || n < 0 || (n > 0 && (!pos || !warp_patch || !search_levels || !inv_expo_list))) return fail(ctx, ESIKF_ERR_ARG, "vio_set_patches: bad argument");
-  if (!ctx->have_cam) return fail(ctx, ESIKF_ERR_STATE, "vio_set_patches before vio_set_camera");
+  if (int rc = need(ctx, "vio_set_patches", IN_CAMERA)) return rc;
   CK(cudaSetDevice(ctx->device));
   const int L = ctx->vio_cfg.patch_pyrimid_level;
   CK(ctx->vis_pos.reserve((size_t)n * 3 + 4));
@@ -1373,8 +1403,7 @@ int esikf_vio_set_patches(esikf_ctx *ctx, const double *pos, const float *warp_p
     CK(cudaMemcpyAsync(ctx->search_levels.p, search_levels, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(ctx->inv_expo.p, inv_expo_list, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, st));
   }
-  ctx->n_patches = n;
-  ctx->have_submap = true;
+  ctx->n_patches = n, ctx->submap_levels = L;
   return ESIKF_OK;
 }
 
@@ -1454,26 +1483,17 @@ static int vio_encode_tma(esikf_ctx *ctx) {
 
 int esikf_vio_run(esikf_ctx *ctx, const double *state_in, const double *state_prop) {
   if (!ctx || !state_in || !state_prop) return fail(ctx, ESIKF_ERR_ARG, "vio_run: null argument");
-  if (!ctx->have_cam || !ctx->have_ext) return fail(ctx, ESIKF_ERR_STATE, "vio_run before vio_set_camera / set_extrinsics");
-  if (ctx->img_w == 0) return fail(ctx, ESIKF_ERR_STATE, "vio_run before vio_set_image");
+  const bool inverse = ctx->vio_cfg.inverse_composition_en != 0;
+  if (int rc = need(ctx, "vio_run", IN_CAMERA | IN_EXT | IN_IMAGE | (ctx->n_patches > 0 ? IN_SUBMAP | (inverse ? IN_INV_REFS : 0) : 0))) return rc;
   CK(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
-  {
-    int rc = upload_states(ctx, state_in, state_prop);
-    if (rc) return rc;
-  }
-  ctx->resident = esikf_ctx::RESIDENT_VIO;
-  const bool inverse = ctx->vio_cfg.inverse_composition_en != 0;
-  if (inverse && ctx->n_patches > 0) {
-    if (ctx->n_inv_refs != ctx->n_patches) return fail(ctx, ESIKF_ERR_STATE, "vio_run: inverse_composition_en needs esikf_vio_set_inverse_refs for the %d patches (have %d)", ctx->n_patches, ctx->n_inv_refs);
-    if (ctx->ref_w != ctx->cam.width || ctx->ref_h != ctx->cam.height) return fail(ctx, ESIKF_ERR_STATE, "vio_run: reference images must have the camera's size");
-  }
+  if (int rc = upload_states(ctx, state_in, state_prop)) return rc;
   const bool fused_vio = ctx->n_patches > 0 && persistent_update(ctx, ctx->coop_vio);
   if (!fused_vio) {
     CK(cudaMemsetAsync(ctx->ctrl, 0, sizeof(Ctrl), st));
     CK(cudaMemsetAsync(ctx->vio_stats, 0, sizeof(esikf_vio_stats), st));
   }
-  if (ctx->n_patches == 0) return ESIKF_OK;  // total_points == 0: early return (vio.cpp:786)
+  if (ctx->n_patches == 0) return ctx->resident = esikf_ctx::RESIDENT_VIO, ESIKF_OK;  // total_points == 0: early return (vio.cpp:786)
   VioKernelArgs ka;
   vio_fill_args(ctx, ka, ctx->state);
   SolveArgs sa = solve_args(ctx, ctx->state, ctx->vio_cfg.max_iterations);
@@ -1503,7 +1523,7 @@ int esikf_vio_run(esikf_ctx *ctx, const double *state_in, const double *state_pr
       ka.chain = ctx->stamps.p + 800;
       CK(cudaMemsetAsync(ka.chain, 0, ESIKF_VIO_CHAIN_STAMP_WORDS * sizeof(unsigned long long), ctx->stream));
     }
-    return launch_persistent(ctx, fn, fn_peer, "vio_update_kernel", grid, VIO_THREADS, VIO_PERSIST_SMEM, &ka, sa, 64, 512, ctx->vio_timed, {&iv, tma});
+    return launch_persistent(ctx, fn, fn_peer, "vio_update_kernel", grid, VIO_THREADS, VIO_PERSIST_SMEM, &ka, sa, 64, 512, ctx->vio_timed, {&iv, tma}, esikf_ctx::RESIDENT_VIO);
   }
   ctx->vio_timed = ctx->timing;
   ctx->vio_slots = ctx->vio_cfg.patch_pyrimid_level * ctx->vio_cfg.max_iterations;
@@ -1531,6 +1551,7 @@ int esikf_vio_run(esikf_ctx *ctx, const double *state_in, const double *state_pr
     }
   }
   CK(cudaGetLastError());
+  ctx->resident = esikf_ctx::RESIDENT_VIO;
   return ESIKF_OK;
 }
 
@@ -1559,7 +1580,7 @@ int esikf_vio_update(esikf_ctx *ctx, const uint8_t *img, int32_t width, int32_t 
 // ---------------------------------------------------------------------------------------------------------------- patch producers
 int esikf_vio_get_image_patch(esikf_ctx *ctx, const double *pc, int32_t n, int32_t level, float *patch_out) {
   if (!ctx || n < 0 || level < 0 || level > 12 || (n > 0 && (!pc || !patch_out))) return fail(ctx, ESIKF_ERR_ARG, "get_image_patch: bad argument");
-  if (ctx->img_w == 0) return fail(ctx, ESIKF_ERR_STATE, "get_image_patch before vio_set_image");
+  if (int rc = need(ctx, "get_image_patch", IN_IMAGE)) return rc;
   if (n == 0) return ESIKF_OK;
   CK(cudaSetDevice(ctx->device));
   const size_t N = (size_t)n;
@@ -1579,7 +1600,7 @@ int esikf_vio_set_ref_images(esikf_ctx *ctx, const uint8_t *const *imgs, int32_t
   CK(cudaSetDevice(ctx->device));
   CK(cudaStreamSynchronize(ctx->stream));
   ctx->ref_imgs.clear();
-  ctx->n_inv_refs = 0;  // the inverse-compositional reference indices pointed into the images just released
+  void_inputs(ctx, IN_INV_REFS);  // their indices pointed into the images just released
   std::vector<const uint8_t *> ptrs;
   for (int i = 0; i < n_imgs; i++) {
     DevBuf<uint8_t> d;
@@ -1601,8 +1622,7 @@ int esikf_vio_warp_patches(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_ind
                            int32_t keep_on_device) {
   if (!ctx || n < 0 || (n > 0 && (!ref_img_index || !px_ref || !pos_w || !normal_w || !T_ref_w || !T_cur_w)))
     return fail(ctx, ESIKF_ERR_ARG, "warp_patches: bad argument");
-  if (!ctx->have_cam) return fail(ctx, ESIKF_ERR_STATE, "warp_patches before vio_set_camera");
-  if (ctx->ref_imgs.empty()) return fail(ctx, ESIKF_ERR_STATE, "warp_patches before set_ref_images");
+  if (int rc = need(ctx, "warp_patches", IN_CAMERA | IN_REF_IMAGES)) return rc;
   for (int i = 0; i < n; i++)
     if (ref_img_index[i] < 0 || ref_img_index[i] >= (int)ctx->ref_imgs.size()) return fail(ctx, ESIKF_ERR_ARG, "warp_patches: ref image index %d", ref_img_index[i]);
   if (n == 0) return ESIKF_OK;
@@ -1644,7 +1664,7 @@ int esikf_vio_warp_patches(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_ind
     CK(cudaMemcpyAsync(ctx->inv_expo.p, ones, N * sizeof(double), cudaMemcpyDeviceToDevice, st));
   }
   CK(read_back(ctx, A, warp_patch_out ? (const void *)(warp + N * 64 * L) : search_level_out ? (const void *)(levels + N) : (const void *)(A + 4 * N)));
-  if (keep_on_device) ctx->n_patches = n, ctx->have_submap = true;
+  if (keep_on_device) ctx->n_patches = n, ctx->submap_levels = L;
   if (A_cur_ref_out) copy_out(ctx, A_cur_ref_out, A, A, N * 4 * sizeof(double));
   if (search_level_out) copy_out(ctx, search_level_out, A, levels, N * sizeof(int32_t));
   if (warp_patch_out) copy_out(ctx, warp_patch_out, A, warp, N * 64 * L * sizeof(float));
@@ -1661,9 +1681,7 @@ int esikf_vio_select_patches(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_i
   if (n > 0 && (!ref_img_index || !px_ref || !pos_w || !T_ref_w || !ref_inv_expo || !pc || !T_cur_w || !kept_index ||
                 (homography ? !normal_w : (!ref_f || !ref_pos || !ref_level || !ref_key))))
     return fail(ctx, ESIKF_ERR_ARG, "select_patches: null argument");
-  if (!ctx->have_cam) return fail(ctx, ESIKF_ERR_STATE, "select_patches before vio_set_camera");
-  if (ctx->img_w == 0) return fail(ctx, ESIKF_ERR_STATE, "select_patches before vio_set_image");
-  if (n > 0 && ctx->ref_imgs.empty()) return fail(ctx, ESIKF_ERR_STATE, "select_patches before set_ref_images");
+  if (int rc = need(ctx, "select_patches", IN_CAMERA | IN_IMAGE | (n > 0 ? IN_REF_IMAGES : 0))) return rc;
   for (int i = 0; i < n; i++) {
     if (ref_img_index[i] < 0 || ref_img_index[i] >= (int)ctx->ref_imgs.size()) return fail(ctx, ESIKF_ERR_ARG, "select_patches: ref image index %d", ref_img_index[i]);
     if (!homography && (ref_level[i] < 0 || ref_level[i] > 8)) return fail(ctx, ESIKF_ERR_ARG, "select_patches: ref level %d", ref_level[i]);
@@ -1678,11 +1696,7 @@ int esikf_vio_select_patches(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_i
   CK(ctx->inv_expo.reserve(n + 1));
   CK(ctx->errors.reserve(n + 1));
   *n_kept = 0;
-  if (n == 0) {
-    ctx->n_patches = 0;
-    ctx->have_submap = true;
-    return ESIKF_OK;
-  }
+  if (n == 0) return ctx->n_patches = 0, ctx->submap_levels = L, ESIKF_OK;
   const size_t N = (size_t)n;
   double *d_px, *d_f, *d_rp, *d_pos, *d_nrm, *d_T, *d_ie, *d_pc, *d_Tc, *d_A, *d_Akept;
   int32_t *d_idx, *d_lvl, *d_key, *d_sl, *d_keep, *d_dst, *d_nk, *d_kept, *d_sl_out;
@@ -1731,8 +1745,7 @@ int esikf_vio_select_patches(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_i
   CK(cudaGetLastError());
   int32_t nk;
   CK(read_back_to(ctx, d_nk, &nk));
-  ctx->n_patches = nk;
-  ctx->have_submap = true;
+  ctx->n_patches = nk, ctx->submap_levels = L;
   *n_kept = nk;
   if (nk > 0) {
     const size_t K = (size_t)nk;
@@ -1752,7 +1765,7 @@ int esikf_vio_select_patches(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_i
 int esikf_vio_set_inverse_refs(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_index, const double *ref_px, const double *ref_f, const double *ref_R,
                                const double *ref_pos) {
   if (!ctx || n < 0 || (n > 0 && (!ref_img_index || !ref_px || !ref_f || !ref_R || !ref_pos))) return fail(ctx, ESIKF_ERR_ARG, "set_inverse_refs: bad argument");
-  if (ctx->ref_imgs.empty() && n > 0) return fail(ctx, ESIKF_ERR_STATE, "set_inverse_refs before set_ref_images");
+  if (int rc = need(ctx, "set_inverse_refs", n > 0 ? IN_REF_IMAGES : 0)) return rc;
   for (int i = 0; i < n; i++)
     if (ref_img_index[i] < 0 || ref_img_index[i] >= (int)ctx->ref_imgs.size()) return fail(ctx, ESIKF_ERR_ARG, "set_inverse_refs: ref image index %d", ref_img_index[i]);
   CK(cudaSetDevice(ctx->device));
@@ -1778,8 +1791,7 @@ int esikf_vio_warp_affine(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_inde
                           const int32_t *search_level, float *warp_patch_out) {
   if (!ctx || n < 0 || (n > 0 && (!ref_img_index || !px_ref || !A_cur_ref || !search_level || !warp_patch_out)))
     return fail(ctx, ESIKF_ERR_ARG, "warp_affine: bad argument");
-  if (!ctx->have_cam) return fail(ctx, ESIKF_ERR_STATE, "warp_affine before vio_set_camera");
-  if (ctx->ref_imgs.empty()) return fail(ctx, ESIKF_ERR_STATE, "warp_affine before set_ref_images");
+  if (int rc = need(ctx, "warp_affine", IN_CAMERA | IN_REF_IMAGES)) return rc;
   for (int i = 0; i < n; i++) {
     if (ref_img_index[i] < 0 || ref_img_index[i] >= (int)ctx->ref_imgs.size()) return fail(ctx, ESIKF_ERR_ARG, "warp_affine: ref image index %d", ref_img_index[i]);
     if (search_level[i] < 0 || search_level[i] > 8) return fail(ctx, ESIKF_ERR_ARG, "warp_affine: search level %d", search_level[i]);
@@ -1809,15 +1821,12 @@ int esikf_vio_warp_affine(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_inde
 }
 
 // ---------------------------------------------------------------------------------------------------------------- coloured scan
-// The device copy of a frame's pose: a packed host state staged into scratch_state, or (state == NULL) the posterior resident on
-// the device, which must be the one an update of kind `want` left there.
-static int rgb_state(esikf_ctx *ctx, const double *state, int want, const char *what, const double **out) {
-  if (!state) {
-    if (ctx->resident != want)
-      return fail(ctx, ESIKF_ERR_STATE, "%s(state = NULL): the device holds no %s posterior", what, want == esikf_ctx::RESIDENT_LIO ? "LIO" : "VIO");
-    *out = ctx->state;
-    return ESIKF_OK;
-  }
+// The device copy of the state a call projects with: a packed host state staged into scratch_state, or (state == NULL) the
+// posterior resident on the device, which must be the one an update of kind `want` left there.
+static int state_or_posterior(esikf_ctx *ctx, const double *state, esikf_ctx::Resident want, const char *what, const double **out) {
+  if (!state && ctx->resident != want)
+    return fail(ctx, ESIKF_ERR_STATE, "%s(state = NULL): the device holds no %s posterior", what, want == esikf_ctx::RESIDENT_LIO ? "LIO" : "VIO");
+  if (!state) return *out = ctx->state, ESIKF_OK;
   CK(ctx->scratch_state.reserve(S_N));
   CK(cudaMemcpyAsync(ctx->scratch_state.p, state, S_N * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
   *out = ctx->scratch_state.p;
@@ -1826,14 +1835,12 @@ static int rgb_state(esikf_ctx *ctx, const double *state, int want, const char *
 
 int esikf_rgb_set_cloud(esikf_ctx *ctx, const float *pts_xyz, int32_t n, const double *state) {
   if (!ctx || (pts_xyz && n < 0)) return fail(ctx, ESIKF_ERR_ARG, "rgb_set_cloud: bad argument");
-  if (!ctx->have_ext) return fail(ctx, ESIKF_ERR_STATE, "rgb_set_cloud before set_extrinsics");
-  if (!pts_xyz && !ctx->pts.p) return fail(ctx, ESIKF_ERR_STATE, "rgb_set_cloud(pts_xyz = NULL) without a resident scan (esikf_lio_set_scan)");
-  if (!pts_xyz && !state && ctx->scan_fresh) return fail(ctx, ESIKF_ERR_STATE, "rgb_set_cloud: the resident scan has not been through esikf_lio_run yet");
+  if (int rc = need(ctx, "rgb_set_cloud", IN_EXT | (pts_xyz ? 0 : IN_SCAN | (state ? 0 : IN_RUN_SCAN)))) return rc;
   CK(cudaSetDevice(ctx->device));
   const double *dev_state = nullptr;
-  if (int rc = rgb_state(ctx, state, esikf_ctx::RESIDENT_LIO, "rgb_set_cloud", &dev_state)) return rc;
+  if (int rc = state_or_posterior(ctx, state, esikf_ctx::RESIDENT_LIO, "rgb_set_cloud", &dev_state)) return rc;
   if (!pts_xyz) n = ctx->n_pts;
-  ctx->rgb_n = -1;  // until the new cloud is in place
+  void_inputs(ctx, IN_CLOUD);  // until the new cloud is in place
   CK(ctx->rgb_cloud.reserve((size_t)n * 3 + 4));
   cudaStream_t st = ctx->stream;
   if (pts_xyz && n > 0) CK(cudaMemcpyAsync(ctx->rgb_cloud.p, pts_xyz, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, st));
@@ -1853,13 +1860,12 @@ int esikf_rgb_set_cloud(esikf_ctx *ctx, const float *pts_xyz, int32_t n, const d
 int esikf_rgb_colorize(esikf_ctx *ctx, const uint8_t *bgr, int32_t width, int32_t height, const double *state, double blind_rgb_points, int32_t cap,
                        int32_t *n_out, float *xyz_out, uint8_t *bgr_out, int32_t *index_out) {
   if (!ctx || !bgr || !n_out || cap < 0 || (cap > 0 && (!xyz_out || !bgr_out))) return fail(ctx, ESIKF_ERR_ARG, "rgb_colorize: bad argument");
-  if (ctx->rgb_n < 0) return fail(ctx, ESIKF_ERR_STATE, "rgb_colorize before rgb_set_cloud");
-  if (!ctx->have_cam) return fail(ctx, ESIKF_ERR_STATE, "rgb_colorize before vio_set_camera");
+  if (int rc = need(ctx, "rgb_colorize", IN_CLOUD | IN_CAMERA)) return rc;
   if (width != ctx->cam.width || height != ctx->cam.height)
     return fail(ctx, ESIKF_ERR_ARG, "rgb_colorize: image is %dx%d, camera %dx%d", width, height, ctx->cam.width, ctx->cam.height);
   CK(cudaSetDevice(ctx->device));
   const double *dev_state = nullptr;
-  if (int rc = rgb_state(ctx, state, esikf_ctx::RESIDENT_VIO, "rgb_colorize", &dev_state)) return rc;
+  if (int rc = state_or_posterior(ctx, state, esikf_ctx::RESIDENT_VIO, "rgb_colorize", &dev_state)) return rc;
   const int n = ctx->rgb_n;
   cudaStream_t st = ctx->stream;
   const size_t N = (size_t)n, img_bytes = (size_t)width * height * 3;
@@ -1912,15 +1918,12 @@ int esikf_vio_generate_points(esikf_ctx *ctx, const double *point_w, const doubl
     return fail(ctx, ESIKF_ERR_ARG, "vio_generate_points: grid %d px, %d x %d cells, border %d", grid_size, grid_n_width, grid_n_height, border);
   if ((long long)grid_n_width * grid_n_height != n_cells)
     return fail(ctx, ESIKF_ERR_ARG, "vio_generate_points: the TYPE_MAP mask has %d cells, the grid %d x %d", n_cells, grid_n_width, grid_n_height);
-  if (!ctx->have_cam) return fail(ctx, ESIKF_ERR_STATE, "vio_generate_points before vio_set_camera");
-  if (ctx->img_w != ctx->cam.width || ctx->img_h != ctx->cam.height) return fail(ctx, ESIKF_ERR_STATE, "vio_generate_points before vio_set_image");
-  if (!point_w && ctx->pv_n < 0)
-    return fail(ctx, ESIKF_ERR_STATE, "vio_generate_points(point_w = NULL): no esikf_map_device_update of the resident scan left its points on the device");
+  if (int rc = need(ctx, "vio_generate_points", IN_CAMERA | IN_IMAGE | (point_w ? 0 : IN_PV_LIST))) return rc;
   if ((long long)(point_w ? n : ctx->pv_n) + n_add >= ESIKF_GEN_ADD_FROM) return fail(ctx, ESIKF_ERR_ARG, "vio_generate_points: too many points");
   CK(cudaSetDevice(ctx->device));
   *n_out = 0;
   const double *dev_state = nullptr;
-  if (int rc = rgb_state(ctx, state, esikf_ctx::RESIDENT_VIO, "vio_generate_points", &dev_state)) return rc;
+  if (int rc = state_or_posterior(ctx, state, esikf_ctx::RESIDENT_VIO, "vio_generate_points", &dev_state)) return rc;
   if (!point_w) n = ctx->pv_n;
   if (n <= 10) return ESIKF_OK;  // :806, add_from included
   cudaStream_t st = ctx->stream;
@@ -2016,13 +2019,11 @@ int esikf_vio_update_points(esikf_ctx *ctx, int32_t n, const uint8_t *converged,
                             int32_t cap, int32_t *n_out, uint8_t *update_flag_out, int32_t *entry_out, double *pc_out, float *patch_out) {
   if (!ctx || n < 0 || !n_out || cap < 0 || (n > 0 && (!converged || !last_T_f_w || !last_px)))
     return fail(ctx, ESIKF_ERR_ARG, "vio_update_points: bad argument");
-  if (!ctx->have_cam || !ctx->have_ext) return fail(ctx, ESIKF_ERR_STATE, "vio_update_points before vio_set_camera / set_extrinsics");
-  if (ctx->img_w != ctx->cam.width || ctx->img_h != ctx->cam.height) return fail(ctx, ESIKF_ERR_STATE, "vio_update_points before vio_set_image");
-  if (!ctx->have_submap) return fail(ctx, ESIKF_ERR_STATE, "vio_update_points: no visual sub-map installed (select_patches / set_patches)");
+  if (int rc = need(ctx, "vio_update_points", IN_CAMERA | IN_EXT | IN_IMAGE | IN_SUBMAP)) return rc;
   if (n != ctx->n_patches) return fail(ctx, ESIKF_ERR_ARG, "vio_update_points: %d entries, the installed sub-map has %d", n, ctx->n_patches);
   CK(cudaSetDevice(ctx->device));
   const double *dev_state = nullptr;
-  if (int rc = rgb_state(ctx, state, esikf_ctx::RESIDENT_VIO, "vio_update_points", &dev_state)) return rc;
+  if (int rc = state_or_posterior(ctx, state, esikf_ctx::RESIDENT_VIO, "vio_update_points", &dev_state)) return rc;
   static const double cos_max = acos_03_bound();
   *n_out = 0;
   if (n == 0) return ESIKF_OK;  // total_points == 0 (:910)
@@ -2072,13 +2073,11 @@ int esikf_vio_update_points(esikf_ctx *ctx, int32_t n, const uint8_t *converged,
 int esikf_vio_retrieve_scan(esikf_ctx *ctx, const double *point_w, int32_t n, int32_t border, const double *state, int32_t cap, int32_t *n_keys,
                             int32_t *keys_out, float *depth_out) {
   if (!ctx || !n_keys || cap < 0 || border < 0 || (point_w && n < 0) || (cap > 0 && !keys_out)) return fail(ctx, ESIKF_ERR_ARG, "vio_retrieve_scan: bad argument");
-  if (!ctx->have_cam || !ctx->have_ext) return fail(ctx, ESIKF_ERR_STATE, "vio_retrieve_scan before vio_set_camera / set_extrinsics");
-  if (!point_w && ctx->pv_n < 0)
-    return fail(ctx, ESIKF_ERR_STATE, "vio_retrieve_scan(point_w = NULL): no esikf_map_device_update of the resident scan left its points on the device");
+  if (int rc = need(ctx, "vio_retrieve_scan", IN_CAMERA | IN_EXT | (point_w ? 0 : IN_PV_LIST))) return rc;
   CK(cudaSetDevice(ctx->device));
   const double *dev_state = nullptr;
-  if (int rc = rgb_state(ctx, state, esikf_ctx::RESIDENT_LIO, "vio_retrieve_scan", &dev_state)) return rc;
-  ctx->ret_valid = false;
+  if (int rc = state_or_posterior(ctx, state, esikf_ctx::RESIDENT_LIO, "vio_retrieve_scan", &dev_state)) return rc;
+  void_inputs(ctx, IN_RETRIEVAL);
   if (!point_w) n = ctx->pv_n;
   cudaStream_t st = ctx->stream;
   const int W = ctx->cam.width, H = ctx->cam.height;
@@ -2139,13 +2138,13 @@ int esikf_vio_retrieve_scan(esikf_ctx *ctx, const double *point_w, int32_t n, in
   if (K > 0) copy_out(ctx, keys_out, d_keys, d_keys, K * 3 * sizeof(int32_t));
   if (depth_out) copy_out(ctx, depth_out, d_keys, depth, npix * sizeof(float));
   memcpy(ctx->ret_Rci, a.Rci, sizeof(a.Rci)), memcpy(ctx->ret_Pci, a.Pci, sizeof(a.Pci));
-  ctx->ret_w = W, ctx->ret_h = H, ctx->ret_valid = true;
+  ctx->ret_w = W, ctx->ret_h = H;
   return ESIKF_OK;
 }
 
 int esikf_vio_depth_check(esikf_ctx *ctx, int32_t n, const double *pos_w, const double *pc, uint8_t *discontinuous_out) {
   if (!ctx || n < 0 || (n > 0 && (!pos_w || !pc || !discontinuous_out))) return fail(ctx, ESIKF_ERR_ARG, "vio_depth_check: bad argument");
-  if (!ctx->ret_valid) return fail(ctx, ESIKF_ERR_STATE, "vio_depth_check: no esikf_vio_retrieve_scan since the last vio_set_camera");
+  if (int rc = need(ctx, "vio_depth_check", IN_RETRIEVAL)) return rc;
   if (n == 0) return ESIKF_OK;
   CK(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
@@ -2247,7 +2246,6 @@ int esikf_vmap_init(esikf_ctx *ctx, int64_t point_capacity) {
   if (!ctx || point_capacity < 1 || point_capacity > VMAP_MAX_POINTS) return fail(ctx, ESIKF_ERR_ARG, "vmap_init: capacity %lld outside [1, 2^26]", (long long)point_capacity);
   CK(cudaSetDevice(ctx->device));
   CK(cudaStreamSynchronize(ctx->stream));
-  ctx->have_vmap = false;
   ctx->vmap = DevBuf<uint8_t>();
   ctx->vmap_cap = ctx->vmap_points = 0;
   ctx->vmap_seen.clear(), ctx->vmap_epoch = 0;
@@ -2255,13 +2253,13 @@ int esikf_vmap_init(esikf_ctx *ctx, int64_t point_capacity) {
   ctx->vpl_cap = ctx->vpl_hi = ctx->vpl_placed = 0;
   ctx->vpl_done.clear();
   CK(vmap_alloc(ctx->vmap, point_capacity));
-  ctx->vmap_cap = point_capacity, ctx->have_vmap = true;
+  ctx->vmap_cap = point_capacity;
   return ESIKF_OK;
 }
 
 int esikf_vmap_stats(esikf_ctx *ctx, int64_t *points, int64_t *capacity) {
   if (!ctx || !points || !capacity) return fail(ctx, ESIKF_ERR_ARG, "vmap_stats: bad argument");
-  if (!ctx->have_vmap) return fail(ctx, ESIKF_ERR_STATE, "vmap_stats before esikf_vmap_init");
+  if (int rc = need(ctx, "vmap_stats", IN_STORE)) return rc;
   *points = ctx->vmap_points, *capacity = ctx->vmap_cap;
   return ESIKF_OK;
 }
@@ -2269,7 +2267,7 @@ int esikf_vmap_stats(esikf_ctx *ctx, int64_t *points, int64_t *capacity) {
 int esikf_vmap_add_points(esikf_ctx *ctx, int32_t n, const int32_t *first, int32_t m, const double *px, const float *patch, const double *T_f_w,
                           const int32_t *id, const float *mean, const float *score, const int32_t *ref, int32_t *point_id_out) {
   if (!ctx) return ESIKF_ERR_ARG;
-  if (!ctx->have_vmap) return fail(ctx, ESIKF_ERR_STATE, "vmap_add_points before esikf_vmap_init");
+  if (int rc = need(ctx, "vmap_add_points", IN_STORE)) return rc;
   if (n < 0 || m < 0 || (n > 0 && (!first || !ref || !point_id_out)) || (m > 0 && (!px || !patch || !T_f_w || !id || !mean || !score)))
     return fail(ctx, ESIKF_ERR_ARG, "vmap_add_points: bad argument");
   if (n == 0) return m == 0 ? ESIKF_OK : fail(ctx, ESIKF_ERR_ARG, "vmap_add_points: %d observations for no point", m);
@@ -2330,16 +2328,14 @@ int esikf_vmap_update_points(esikf_ctx *ctx, int32_t n, const int32_t *point_id,
                              const double *state, int32_t cap, int32_t *n_out, uint8_t *update_flag_out, int32_t *entry_out, double *pc_out,
                              float *patch_out, int32_t *evicted_out, int32_t *count_out) {
   if (!ctx) return ESIKF_ERR_ARG;
-  if (!ctx->have_vmap) return fail(ctx, ESIKF_ERR_STATE, "vmap_update_points before esikf_vmap_init");
+  if (int rc = need(ctx, "vmap_update_points", IN_STORE)) return rc;
   if (n < 0 || !n_out || cap < 0 || (n > 0 && (!point_id || !converged))) return fail(ctx, ESIKF_ERR_ARG, "vmap_update_points: bad argument");
-  if (!ctx->have_cam || !ctx->have_ext) return fail(ctx, ESIKF_ERR_STATE, "vmap_update_points before vio_set_camera / set_extrinsics");
-  if (ctx->img_w != ctx->cam.width || ctx->img_h != ctx->cam.height) return fail(ctx, ESIKF_ERR_STATE, "vmap_update_points before vio_set_image");
-  if (!ctx->have_submap) return fail(ctx, ESIKF_ERR_STATE, "vmap_update_points: no visual sub-map installed (select_patches / set_patches)");
+  if (int rc = need(ctx, "vmap_update_points", IN_CAMERA | IN_EXT | IN_IMAGE | IN_SUBMAP)) return rc;
   if (n != ctx->n_patches) return fail(ctx, ESIKF_ERR_ARG, "vmap_update_points: %d entries, the installed sub-map has %d", n, ctx->n_patches);
   if (int rc = vmap_check_ids(ctx, n, point_id, "vmap_update_points")) return rc;
   CK(cudaSetDevice(ctx->device));
   const double *dev_state = nullptr;
-  if (int rc = rgb_state(ctx, state, esikf_ctx::RESIDENT_VIO, "vmap_update_points", &dev_state)) return rc;
+  if (int rc = state_or_posterior(ctx, state, esikf_ctx::RESIDENT_VIO, "vmap_update_points", &dev_state)) return rc;
   static const double cos_max = acos_03_bound();
   *n_out = 0;
   if (n == 0) return ESIKF_OK;  // total_points == 0 (:910)
@@ -2396,7 +2392,7 @@ int esikf_vmap_update_points(esikf_ctx *ctx, int32_t n, const int32_t *point_id,
 int esikf_vmap_score(esikf_ctx *ctx, int32_t n, const int32_t *point_id, const double *pos, const double *normal, int32_t *ref_out, float *score_out,
                      float *mean_out) {
   if (!ctx) return ESIKF_ERR_ARG;
-  if (!ctx->have_vmap) return fail(ctx, ESIKF_ERR_STATE, "vmap_score before esikf_vmap_init");
+  if (int rc = need(ctx, "vmap_score", IN_STORE)) return rc;
   if (n < 0 || (n > 0 && (!point_id || !pos || !normal || !ref_out))) return fail(ctx, ESIKF_ERR_ARG, "vmap_score: bad argument");
   if (int rc = vmap_check_ids(ctx, n, point_id, "vmap_score")) return rc;
   if (n == 0) return ESIKF_OK;
@@ -2437,7 +2433,7 @@ int esikf_vmap_score(esikf_ctx *ctx, int32_t n, const int32_t *point_id, const d
 int esikf_vmap_choose_ref(esikf_ctx *ctx, int32_t n, const int32_t *point_id, const double *pos, const double *frame_pos, int32_t normal_en,
                           int32_t *ref_out) {
   if (!ctx) return ESIKF_ERR_ARG;
-  if (!ctx->have_vmap) return fail(ctx, ESIKF_ERR_STATE, "vmap_choose_ref before esikf_vmap_init");
+  if (int rc = need(ctx, "vmap_choose_ref", IN_STORE)) return rc;
   if (n < 0 || (n > 0 && (!point_id || !ref_out || (!normal_en && (!pos || !frame_pos))))) return fail(ctx, ESIKF_ERR_ARG, "vmap_choose_ref: bad argument");
   if (int rc = vmap_check_ids(ctx, n, point_id, "vmap_choose_ref")) return rc;
   if (n == 0) return ESIKF_OK;
@@ -2462,7 +2458,7 @@ int esikf_vmap_choose_ref(esikf_ctx *ctx, int32_t n, const int32_t *point_id, co
 int esikf_vmap_download(esikf_ctx *ctx, int32_t n, const int32_t *point_id, int32_t cap, int32_t *first_out, double *px, float *patch, double *T_f_w,
                         int32_t *id, float *mean, float *score, int32_t *ref) {
   if (!ctx) return ESIKF_ERR_ARG;
-  if (!ctx->have_vmap) return fail(ctx, ESIKF_ERR_STATE, "vmap_download before esikf_vmap_init");
+  if (int rc = need(ctx, "vmap_download", IN_STORE)) return rc;
   if (n < 0 || cap < 0 || !first_out || (n > 0 && (!point_id || !ref)) || (cap > 0 && (!px || !patch || !T_f_w || !id || !mean || !score)))
     return fail(ctx, ESIKF_ERR_ARG, "vmap_download: bad argument");
   if (int rc = vmap_check_ids(ctx, n, point_id, "vmap_download")) return rc;
@@ -2520,7 +2516,7 @@ int esikf_vmap_download(esikf_ctx *ctx, int32_t n, const int32_t *point_id, int3
 // ---------------------------------------------------------------------------------------------------------------- the map side of the retrieval
 int esikf_vmap_place_points(esikf_ctx *ctx, int32_t n, const int32_t *point_id, const double *pos, const uint8_t *normal_init) {
   if (!ctx) return ESIKF_ERR_ARG;
-  if (!ctx->have_vmap) return fail(ctx, ESIKF_ERR_STATE, "vmap_place_points before esikf_vmap_init");
+  if (int rc = need(ctx, "vmap_place_points", IN_STORE)) return rc;
   if (n < 0 || (n > 0 && (!point_id || !pos))) return fail(ctx, ESIKF_ERR_ARG, "vmap_place_points: bad argument");
   if (int rc = vmap_check_ids(ctx, n, point_id, "vmap_place_points")) return rc;
   int64_t hi = ctx->vpl_hi;
@@ -2588,10 +2584,10 @@ int esikf_vmap_retrieve(esikf_ctx *ctx, int32_t n_keys, const int32_t *keys, int
                         int32_t normal_en, int32_t cap, int32_t *n_cells, int32_t *cell_out, int32_t *point_id_out, double *pc_out, int32_t *status_out,
                         int32_t *ref_out) {
   if (!ctx) return ESIKF_ERR_ARG;
-  if (!ctx->have_vmap) return fail(ctx, ESIKF_ERR_STATE, "vmap_retrieve before esikf_vmap_init");
+  if (int rc = need(ctx, "vmap_retrieve", IN_STORE)) return rc;
   if (n_keys < 0 || (n_keys > 0 && !keys) || !n_cells || cap < 0 || border < 0 || (cap > 0 && (!cell_out || !point_id_out || !pc_out || !status_out || !ref_out)))
     return fail(ctx, ESIKF_ERR_ARG, "vmap_retrieve: bad argument");
-  if (!ctx->ret_valid) return fail(ctx, ESIKF_ERR_STATE, "vmap_retrieve: no esikf_vio_retrieve_scan since the last vio_set_camera");
+  if (int rc = need(ctx, "vmap_retrieve", IN_RETRIEVAL)) return rc;
   const int W = ctx->ret_w, H = ctx->ret_h;
   if (grid_size <= 0 || grid_n_width <= 0 || grid_n_height <= 0 || (int64_t)grid_n_width * grid_n_height > (1 << 24) ||
       (int64_t)grid_n_width * grid_size < W - border || (int64_t)grid_n_height * grid_size < H - border)
@@ -2787,12 +2783,15 @@ int esikf_profile_kernel(esikf_ctx *ctx, int32_t which, int32_t arg, int32_t rep
   memset(&sa, 0, sizeof(sa));
   int grid = 1;
   if (which == 0 || which == 1 || which == 3) {
-    if (!ctx->have_map || ctx->n_pts == 0 || ctx->scan_fresh) return fail(ctx, ESIKF_ERR_STATE, "profile_kernel: no resident LIO frame (run lio once)");
+    if (int rc = need(ctx, "profile_kernel: no resident LIO frame", IN_MAP | IN_RUN_SCAN)) return rc;
+    if (ctx->n_pts == 0) return fail(ctx, ESIKF_ERR_STATE, "profile_kernel: no resident LIO frame (run lio once)");
     lio_fill_args(ctx, la, ctx->scratch_state.p);
     grid = lio_grid(ctx, la.count);
     sa = solve_args(ctx, ctx->scratch_state.p, 1 << 20);
   } else if (which == 2) {
-    if (ctx->n_patches == 0 || ctx->img_w == 0) return fail(ctx, ESIKF_ERR_STATE, "profile_kernel: no resident VIO frame");
+    if (int rc = need(ctx, "profile_kernel: no resident VIO frame", IN_IMAGE | IN_SUBMAP)) return rc;
+    if (ctx->n_patches == 0) return fail(ctx, ESIKF_ERR_STATE, "profile_kernel: no resident VIO frame (an empty sub-map)");
+    if (arg < 0 || arg >= ctx->vio_cfg.patch_pyrimid_level) return fail(ctx, ESIKF_ERR_ARG, "profile_kernel: level %d outside [0, %d)", arg, ctx->vio_cfg.patch_pyrimid_level);
     vio_fill_args(ctx, va, ctx->scratch_state.p);
     va.level = arg, va.slot_iter = 0;
     grid = vio_grid(ctx, va.count);

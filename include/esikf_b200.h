@@ -286,7 +286,10 @@ int esikf_lio_fetch_normals(esikf_ctx *ctx, double *normals);
 int esikf_lio_fetch_point_cov(esikf_ctx *ctx, double *body_cov9 /* nullable */, double *cross_mat9 /* nullable */);
 
 /* ---------------------------------------------------------------- VIO update (computeJacobianAndUpdateEKF)
- * set_camera    : vk camera + vio/ parameters.
+ * set_camera    : vk camera + vio/ parameters. It voids the retrieval (esikf_vio_retrieve_scan); a new width or height voids
+ *                 the current image, and a new patch_pyrimid_level the installed sub-map and its inverse-compositional refs.
+ *                 Calls that read a voided input return ESIKF_ERR_STATE until it is set again. Re-setting an identical
+ *                 camera voids only the retrieval.
  * set_image     : the current 8-bit grey image, width x height of the camera.
  * set_patches   : visual_submap (include/vio.h:26-57): voxel_points[i]->pos_ (n x 3 f64), warp_patch
  *                 (n x levels*64 f32, [level][row][col]), search_levels (n), inv_expo_list (n).
@@ -630,7 +633,7 @@ int esikf_shard_range(int32_t n, int32_t rank, int32_t nranks, int32_t *begin, i
 /* ---------------------------------------------------------------- measurement hooks (bench.py)
  * Average device time (ms, CUDA events on esikf_stream) of `reps` back-to-back launches of one
  * kernel on the resident inputs: which = 0 LIO residual kernel, 1 solve kernel, 2 VIO patch kernel
- * (level given by `arg`), 3 per-frame LIO precompute. flush_l2 != 0 writes a >L2 buffer between launches
+ * (level given by `arg`, in [0, patch_pyrimid_level)), 3 per-frame LIO precompute. flush_l2 != 0 writes a >L2 buffer between launches
  * (excluded from the timing). */
 int esikf_profile_kernel(esikf_ctx *ctx, int32_t which, int32_t arg, int32_t reps, int32_t flush_l2, float *avg_ms);
 
