@@ -57,28 +57,6 @@ def test_vio_persistent_kernel_is_bit_identical_to_per_iteration_launches(gpu_ct
         bits_equal(ref, r, VIO_KEYS)
 
 
-@pytest.mark.parametrize("n_patches", [4000, 6000])
-def test_vio_patch_cache_with_two_and_more_patches_per_warp_and_search_levels(gpu_ctx, n_patches):
-    """4 k patches: two per warp, both cached across iterations. 6 k: more than the cache holds, slot 0 is refilled every
-    time. Non-zero search levels (tap strides up to 32) and five levels; against the cold per-iteration path."""
-    from fast_livo2_b200 import synthetic as S
-
-    cam = S.CamCfg(width=612, height=512, fx=612.0 * 0.72, fy=612.0 * 0.72, cx=306.0, cy=256.0)
-    vcfg = S.VioCfg(levels=5, img_point_cov=1000.0)
-    fr = get_frame(seed=13, n_pts=1000, n_map=300_000, n_patches=4000, scene_scale=0.7, cam=cam, vio=vcfg)
-    vio_setup(gpu_ctx, fr)
-    prior = vio_prior(fr, 13)
-    w = vio_warp(gpu_ctx, fr, prior)
-    n = len(fr["vis_pos"])
-    rep = (np.arange(n_patches) % n)
-    sl = (np.arange(n_patches) % 2).astype(np.int32)  # exercise search_level 1 as well
-    args = (fr["img"], fr["vis_pos"][rep], w["warp_patch"][rep], sl, fr["inv_ref_expo"][rep], prior, prior)
-    a, b, b2 = sweep(gpu_ctx, lambda: gpu_ctx.vio_update(*args), [dict(loop_mode=0), dict(loop_mode=2), dict(loop_mode=2)])
-    assert a["total_iters"] == b["total_iters"] == b2["total_iters"]
-    bits_equal(a, b, VIO_KEYS)
-    bits_equal(a, b2, VIO_KEYS)
-
-
 def test_vio_tap_footprints_through_tma_are_bit_identical(gpu_ctx):
     """ESIKF_TUNE_VIO_TMA: the 11 x 11 tap footprint arrives by one tiled TMA load (cp.async.bulk.tensor.2d, elementStrides
     {1, s}) instead of per-lane byte loads. BASELINE config-2 image (640 x 512, pitch a multiple of 16) with search levels
