@@ -56,7 +56,7 @@ __device__ __forceinline__ bool patch_voxel_key(double c, long long &k) {
 // ---- the cosine between a point's viewing ray and its normal in a camera frame (generateVisualMapPoints :867-870,
 // updateReferencePatch :1046-1049): norm_vec = T_f_w_.rotation_matrix() * normal (R row-major); pf = T_f_w_ * pos, already in
 // the camera frame; pf.normalize(); pf.dot(norm_vec). Each sum starts from 0 and runs left to right, as in the stand-in Eigen.
-// T is the single-rounded double Rn of esikf_vio.cu.
+// T is the single-rounded double Rn of esikf_vio.cuh.
 template <class T> __device__ __forceinline__ T view_cos(const double *R, const T pf[3], const double *normal) {
   T nv[3];
   for (int r = 0; r < 3; r++) nv[r] = T(0.0) + T(R[3 * r]) * T(normal[0]) + T(R[3 * r + 1]) * T(normal[1]) + T(R[3 * r + 2]) * T(normal[2]);
@@ -119,6 +119,27 @@ __host__ __device__ __forceinline__ double m_dot3(double a0, double b0, double a
 // inverse). Contracted into an FMA it can land on the other side of getBestSearchLevel's thresholds 3 / 12 when it lies
 // within an ulp of one, and it gives a different float inverse when the products cancel.
 __device__ __forceinline__ double det2_rn(double a00, double a11, double a01, double a10) { return __dsub_rn(__dmul_rn(a00, a11), __dmul_rn(a01, a10)); }
+__device__ __forceinline__ double dot3_rn(double a0, double a1, double a2, double b0, double b1, double b2) {
+  return __dadd_rn(__dadd_rn(__dmul_rn(a0, b0), __dmul_rn(a1, b1)), __dmul_rn(a2, b2));
+}
+// p_imu = extR p + extT (TransformLidar, voxel_map.cpp:524). No FMA contraction: the chain ends in the float rounding of p_w,
+// which decides the voxel key.
+__device__ __forceinline__ void p_imu(const double *extR, const double *extT, float fx, float fy, float fz, double &pi0, double &pi1, double &pi2) {
+  const double px = fx, py = fy, pz = fz;
+  pi0 = __dadd_rn(dot3_rn(extR[0], extR[1], extR[2], px, py, pz), extT[0]);
+  pi1 = __dadd_rn(dot3_rn(extR[3], extR[4], extR[5], px, py, pz), extT[1]);
+  pi2 = __dadd_rn(dot3_rn(extR[6], extR[7], extR[8], px, py, pz), extT[2]);
+}
+// World point of a body point, rounded to float: R (extR p + extT) + t with the pose (R row-major, t) of a packed state
+// (pointBodyToWorld / RGBpointBodyToWorld, LIVMapper.cpp:645-649, 682-690). No FMA contraction: the float rounding decides
+// the voxel key of the map and is what the coloured scan publishes.
+__device__ __forceinline__ void world_point_f(const double *R, const double *t, const double *extR, const double *extT, float fx, float fy, float fz, float w[3]) {
+  double q0, q1, q2;
+  p_imu(extR, extT, fx, fy, fz, q0, q1, q2);
+  w[0] = (float)__dadd_rn(dot3_rn(R[0], R[1], R[2], q0, q1, q2), t[0]);
+  w[1] = (float)__dadd_rn(dot3_rn(R[3], R[4], R[5], q0, q1, q2), t[1]);
+  w[2] = (float)__dadd_rn(dot3_rn(R[6], R[7], R[8], q0, q1, q2), t[2]);
+}
 
 // 256-byte map plane -> the 144-byte record (one definition for the upload / patch kernel and the device-resident map, evaluated
 // without FMA contraction: both paths hand the residual kernel bit-identical records for the same plane)
@@ -147,6 +168,9 @@ __host__ __device__ __forceinline__ void compact_plane(const esikf_plane &p, Pla
 #define NE_MAX 40
 __host__ __device__ constexpr int ne_of(int m) { return m * (m + 1) / 2 + m + 2; }
 __host__ __device__ constexpr int tri_of(int m, int i, int j) { return i * m - (i * (i - 1)) / 2 + (j - i); }  // i <= j
+// the peer mailbox of the persistent kernels (esikf_fused.cu): [2 parities][PEER_MAX_RANKS][PEER_SLOT_WORDS] u64 words
+#define PEER_SLOT_WORDS (NE_MAX * 2)  // u64 words per (parity, rank) slot
+#define PEER_MAX_RANKS 8
 
 // ---- loop-control block shared by the kernels of one update (device memory)
 struct Ctrl {

@@ -60,8 +60,6 @@ __device__ __forceinline__ bool wait_expired(WaitGuard &w, unsigned long long t0
 // early: a per-launch formula would reuse a parity). Two parities suffice because exchanges strictly alternate: a rank's
 // CTA 0 writes exchange k + 2 only after it received every peer's k + 1, which a peer's CTA 0 sends after its own grid
 // exchange k + 1 — and every CTA of that peer completes that grid exchange only after it finished pulling exchange k.
-#define PEER_SLOT_WORDS (NE_MAX * 2)  // u64 words per (parity, rank) slot
-#define PEER_MAX_RANKS 8
 struct PeerArgs {
   unsigned long long *const *mbox;  // device array: mailbox base of every rank (own entry = local memory)
   unsigned int *seq;                // device word: exchanges executed so far (same on every rank); set without peers too

@@ -36,7 +36,7 @@ namespace esikf {
 #ifndef LIO_FULL_REC
 #define LIO_FULL_REC 0  // cold candidates: head first, covariance part after the range gate (0, default) or the whole record in one round trip (1). The one-trip form saves an L2 round trip but keeps 18 more registers live
 #endif
-// One CTA per SM, in one of two geometries chosen per launch (lio_use_l2_slots in esikf_api.cu). Warps [0, LIO_SMEM_WARPS)
+// One CTA per SM, in one of two geometries chosen per launch (lio_use_l2_slots in esikf_api_update.cu). Warps [0, LIO_SMEM_WARPS)
 // keep their lane slots in shared memory; 22 x 32 slots of 304 B is what fits next to the rest of LioSmem. The 768-lane
 // kernel adds LIO_L2_WARPS warps ("L2-slot warps") that keep theirs in a per-CTA block of global memory, which stays in L2
 // for the whole update: 132 x 768 = 101 k points resident on H100. It runs only where it makes a slice resident that the
@@ -88,9 +88,6 @@ struct LioCold {
   double extR[9], extT[3];
 };
 
-__device__ __forceinline__ double dot3_rn(double a0, double a1, double a2, double b0, double b1, double b2) {
-  return __dadd_rn(__dadd_rn(__dmul_rn(a0, b0), __dmul_rn(a1, b1)), __dmul_rn(a2, b2));
-}
 // index of (i,j) in the row-major upper triangle of a 6x6
 __host__ __device__ constexpr int tri6(int i, int j) { return (i <= j) ? (i * 6 - (i * (i - 1)) / 2 + (j - i)) : (j * 6 - (j * (j - 1)) / 2 + (i - j)); }
 
@@ -546,24 +543,6 @@ __device__ LIO_COLD void resolve_voxel(const LioCold &a, const LioSmemCore &sm, 
 // Cold part of the association, out of line: the extras of sub-divided home voxels, then one neighbour voxel for the lanes
 // whose home voxel gave nothing (voxel_map.cpp:680-691). loc is in voxel units, centre / quarter length in metres:
 // reproduced literally. Called by the whole warp.
-// p_imu = extR p + extT (TransformLidar, voxel_map.cpp:524). No FMA contraction: the chain ends in the float rounding of p_w,
-// which decides the voxel key.
-__device__ __forceinline__ void p_imu(const double *extR, const double *extT, float fx, float fy, float fz, double &pi0, double &pi1, double &pi2) {
-  const double px = fx, py = fy, pz = fz;
-  pi0 = __dadd_rn(dot3_rn(extR[0], extR[1], extR[2], px, py, pz), extT[0]);
-  pi1 = __dadd_rn(dot3_rn(extR[3], extR[4], extR[5], px, py, pz), extT[1]);
-  pi2 = __dadd_rn(dot3_rn(extR[6], extR[7], extR[8], px, py, pz), extT[2]);
-}
-// World point of a body point, rounded to float: R (extR p + extT) + t with the pose (R row-major, t) of a packed state
-// (pointBodyToWorld / RGBpointBodyToWorld, LIVMapper.cpp:645-649, 682-690). No FMA contraction: the float rounding decides
-// the voxel key of the map and is what the coloured scan publishes.
-__device__ __forceinline__ void world_point_f(const double *R, const double *t, const double *extR, const double *extT, float fx, float fy, float fz, float w[3]) {
-  double q0, q1, q2;
-  p_imu(extR, extT, fx, fy, fz, q0, q1, q2);
-  w[0] = (float)__dadd_rn(dot3_rn(R[0], R[1], R[2], q0, q1, q2), t[0]);
-  w[1] = (float)__dadd_rn(dot3_rn(R[3], R[4], R[5], q0, q1, q2), t[1]);
-  w[2] = (float)__dadd_rn(dot3_rn(R[6], R[7], R[8], q0, q1, q2), t[2]);
-}
 // cross-matrix vector of the point (voxel_map.cpp:352-359): extR p + extT with z = 0.001 when the raw z is 0
 __device__ __forceinline__ void cross_vec(const double *extR, const double *extT, float fx, float fy, float fz, double &cx, double &cy, double &cz) {
   p_imu(extR, extT, fx, fy, fz, cx, cy, cz);

@@ -146,11 +146,6 @@ __global__ void __launch_bounds__(256) map_keys_kernel(const MapArena A, const d
   pt_slot[i] = slot, pt_idx[i] = (unsigned int)i;
 }
 
-struct MapTouched {
-  unsigned int slot;
-  int start, count;
-};
-
 // work[0] = touched roots, work[1] = next root to hand out
 __global__ void __launch_bounds__(256) map_heads_kernel(const unsigned int *__restrict__ sorted_slot, int n, unsigned int invalid_slot, MapTouched *touched, int *work) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;

@@ -76,6 +76,11 @@ struct MapArena {
   MapCfg cfg;
 };
 
+struct MapTouched {
+  unsigned int slot;
+  int start, count;
+};
+
 // ---- atomics that degrade to plain operations on the host (single thread there)
 MAP_HD int map_atomic_add(int *p, int v) {
 #ifdef __CUDA_ARCH__

@@ -34,7 +34,7 @@ static void par_memcpy(void *dst, const void *src, size_t bytes) {
 // A manager's calls stage their inputs and answers in its one pinned block (scratch_layout.hpp), so no method may return with
 // a copy from it queued. On success each ends in a synchronising call: the fetch of esikf_lio_update / esikf_vio_update /
 // esikf_vio_run, the error check of the map updates, esikf_rgb_set_cloud, the export, or the front-end call itself. The
-// exceptions are the early successful returns of the calls that upload a packed state (rgb_state in esikf_api.cu):
+// exceptions are the early successful returns of the calls that upload a packed state (state_or_posterior in esikf_api_ctx.cu):
 // GenerateVisualMapPoints at 10 points or fewer and ColorizeFrameWorld of an empty cloud (UpdateVisualMapPoints returns
 // before update_points at no entries). They leave that upload queued into a device copy that every reader rewrites in stream
 // order first, so what the block then holds is never read. esikf_lio_set_scan, esikf_vio_set_image and

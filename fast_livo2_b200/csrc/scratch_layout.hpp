@@ -1,5 +1,5 @@
 // scratch_layout.hpp — how one call's sub-arrays are laid out in a shared per-call block: the device scratch of esikf_ctx
-// (esikf_api.cu) and the pinned host blocks of the shim managers (fl2_shim.cpp).
+// (esikf_api.cuh) and the pinned host blocks of the shim managers (fl2_shim.cpp).
 #pragma once
 #include <cstddef>
 #include <cstdint>

@@ -1,6 +1,6 @@
 """GPU: the persistent update kernels at every grid and slice geometry their launches can take.
 
-How a launch deals its work (csrc/esikf_api.cu vio_grid / lio_grid, esikf_vio.cu vio_block_range, esikf_lio.cu
+How a launch deals its work (csrc/esikf_api_update.cu vio_grid / lio_grid, esikf_vio.cu vio_block_range, esikf_lio.cu
 lio_block_range, esikf_fused.cu persist_exchange / reduce_entry), with PB = min(SMs, 160) partial columns:
   VIO  G = min(ceil(n / 16), PB) CTAs of per = ceil(n / G) patches; patch lo + warp + 16 k goes to (warp, k) and the
        per-warp patch cache holds a CTA's patches while per <= 32 (above it slot 0 is refilled for every patch); trailing

@@ -38,7 +38,7 @@ def build_new(out_dir):
     import __graft_entry__ as G
 
     lib = os.path.join(out_dir, "libesikf_b200.so")
-    subprocess.run([G.nvcc_path(), *G.NVCC_FLAGS, "-o", lib, G.SRC[0], "-ldl"], cwd=ROOT, check=True)
+    G.build_library(lib, force=True)
     return lib
 
 

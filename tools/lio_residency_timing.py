@@ -34,17 +34,14 @@ def card():
 
 
 def build_all(out_dir):
-    """Both libraries, compiled in parallel with the flags of __graft_entry__.build()."""
+    """Both libraries, compiled with the flags of __graft_entry__.build()."""
     import __graft_entry__ as G
 
-    procs, libs = [], {}
+    libs = {}
     for name, w in BUILDS.items():
         os.makedirs(os.path.join(out_dir, name), exist_ok=True)
         libs[name] = os.path.join(out_dir, name, "libesikf_b200.so")
-        procs.append(subprocess.Popen([G.nvcc_path(), *G.NVCC_FLAGS, f"-DLIO_L2_WARPS={w}", "-o", libs[name], G.SRC[0], "-ldl"], cwd=ROOT))
-    for p in procs:
-        if p.wait() != 0:
-            raise SystemExit("lio_residency_timing: build failed")
+        G.build_library(libs[name], [f"-DLIO_L2_WARPS={w}"], force=True)
     return libs
 
 
