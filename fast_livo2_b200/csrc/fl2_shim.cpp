@@ -6,6 +6,7 @@
 #include <omp.h>
 
 #include <chrono>
+#include <memory>
 
 #include <cmath>
 #include <cstring>
@@ -50,6 +51,24 @@ template <typename F> static bool lay_out_staging(PinnedBuf<uint8_t> &block, F &
   return true;
 }
 
+// The guards of the managers' calls: false when the call has what it needs, else true with ESIKF_ERR_STATE and the call's
+// message recorded. Every guarded call needs the device context; some also a state (VIOManager::state) or the device map.
+static bool missing(CallStatus &c, const char *call, const esikf_ctx *ctx) {
+  if (ctx) return false;
+  c.last_status_ = ESIKF_ERR_STATE, c.last_error_ = std::string(call) + ": no device context";
+  return true;
+}
+static bool missing(CallStatus &c, const char *call, const esikf_ctx *ctx, const StatesGroup *state) {
+  if (ctx && state) return false;
+  c.last_status_ = ESIKF_ERR_STATE, c.last_error_ = std::string(call) + ": no device context or state";
+  return true;
+}
+static bool no_device_map(CallStatus &c, bool device_map, const char *error) {
+  if (device_map) return false;
+  c.last_status_ = ESIKF_ERR_STATE, c.last_error_ = error;
+  return true;
+}
+
 StatesGroup::StatesGroup() {
   for (int i = 0; i < 361; i++) cov[i] = 0.0;
   for (int i = 0; i < 19; i++) cov[i * 19 + i] = 0.01;   // INIT_COV, include/common_lib.h:31,137
@@ -79,6 +98,21 @@ void StatesGroup::unpack(const double *s) {
 
 pointWithVar::pointWithVar() {
   for (int i = 0; i < 9; i++) var_nostate.m[i] = body_var.m[i] = var.m[i] = point_crossmat.m[i] = 0.0;
+}
+
+// The plane fields a C ABI row (esikf_plane, esikf_map_node) shares with a VoxelPlane. The row holds plane_var_'s upper
+// triangle, row by row (DESIGN.md §4): the layout the device map, its export and the oracle all read.
+template <typename Row> static void plane_from_row(const Row &r, VoxelPlane &p) {
+  for (int k = 0; k < 3; k++) p.center_[k] = r.center[k], p.normal_[k] = r.normal[k];
+  for (int a = 0, t = 0; a < 6; a++)
+    for (int b = a; b < 6; b++, t++) p.plane_var_[6 * a + b] = p.plane_var_[6 * b + a] = r.plane_var[t];
+  p.d_ = r.d, p.radius_ = r.radius;
+}
+static void row_from_plane(const VoxelPlane &p, esikf_plane &r) {
+  for (int k = 0; k < 3; k++) r.center[k] = p.center_[k], r.normal[k] = p.normal_[k];
+  for (int a = 0, t = 0; a < 6; a++)
+    for (int b = a; b < 6; b++, t++) r.plane_var[t] = p.plane_var_[6 * a + b];
+  r.d = p.d_, r.radius = p.radius_;
 }
 
 VoxelOctoTree::~VoxelOctoTree() {
@@ -131,11 +165,8 @@ bool ApplyMapExport(VoxelMap &map, const VoxelMapConfig &cfg, const int64_t *key
       t->init_octo_ = e.init_octo != 0, t->octo_state_ = e.octo_state, t->update_enable_ = e.update_enable != 0;
       t->new_points_ = e.new_points, t->temp_points_size_ = e.temp_points;
       VoxelPlane &p = *t->plane_ptr_;
-      for (int k = 0; k < 3; k++) p.center_[k] = e.center[k], p.normal_[k] = e.normal[k];
-      int q = 0;
-      for (int a = 0; a < 6; a++)
-        for (int b = a; b < 6; b++) p.plane_var_[a * 6 + b] = p.plane_var_[b * 6 + a] = e.plane_var[q++];  // symmetric (DESIGN.md §4)
-      p.d_ = e.d, p.radius_ = e.radius, p.points_size_ = e.points_size;
+      plane_from_row(e, p);
+      p.points_size_ = e.points_size;
       p.is_plane_ = e.is_plane != 0, p.is_init_ = e.points_size > 0;
     }
   }
@@ -165,12 +196,7 @@ static void flatten_node(const VoxelOctoTree *node, int layer, int max_layer, in
     const VoxelPlane &p = *node->plane_ptr_;
     esikf_plane f;
     memset(&f, 0, sizeof(f));
-    for (int k = 0; k < 3; k++) f.center[k] = p.center_[k], f.normal[k] = p.normal_[k];
-    int t = 0;
-    for (int i = 0; i < 6; i++)
-      for (int j = i; j < 6; j++) f.plane_var[t++] = p.plane_var_[i * 6 + j];
-    f.d = p.d_;
-    f.radius = p.radius_;
+    row_from_plane(p, f);
     f.layer = layer;
     f.path = path;
     out.planes.push_back(f);
@@ -311,10 +337,7 @@ void VoxelMapManager::UpdateMirror() {
 
 // include/voxel_map.h:231 / src/voxel_map.cpp:532-591 with feats_down_world_ = transformLidar(state_) (LIVMapper.cpp:360)
 void VoxelMapManager::BuildVoxelMap() {
-  if (!ctx_ || !device_map_) {
-    last_status_ = ESIKF_ERR_STATE, last_error_ = "BuildVoxelMap: EnableDeviceMap first (a host-owned voxel_map_ is built by the reference's own code)";
-    return;
-  }
+  if (no_device_map(*this, ctx_ && device_map_, "BuildVoxelMap: EnableDeviceMap first (a host-owned voxel_map_ is built by the reference's own code)")) return;
   const int n = feats_down_size_;
   float *pts; double *sbuf;
   if (!lay_out_staging(block_, [&](ScratchLayout &s) { pts = s.take<float>((size_t)n * 3 + 4), sbuf = s.take<double>(ESIKF_STATE_DOUBLES); })) return StagingFailed();
@@ -328,10 +351,7 @@ void VoxelMapManager::BuildVoxelMap() {
 
 // LIVMapper.cpp:413-424: pv_list_[i].point_w / .var with the posterior, then UpdateVoxelMap(pv_list_) — on the device
 void VoxelMapManager::UpdateVoxelMap() {
-  if (!ctx_ || !device_map_) {
-    last_status_ = ESIKF_ERR_STATE, last_error_ = "UpdateVoxelMap(): EnableDeviceMap first";
-    return;
-  }
+  if (no_device_map(*this, ctx_ && device_map_, "UpdateVoxelMap(): EnableDeviceMap first")) return;
   double *sbuf;
   if (!lay_out_staging(block_, [&](ScratchLayout &s) { sbuf = s.take<double>(ESIKF_STATE_DOUBLES); })) return StagingFailed();
   state_.pack(sbuf);  // _state == voxelmap_manager->state_ at this point of the tick (LIVMapper.cpp:371); 3 kB
@@ -340,10 +360,7 @@ void VoxelMapManager::UpdateVoxelMap() {
 }
 
 void VoxelMapManager::SetWorldCloud(const std::vector<PointXYZ> *dense_scan) {
-  if (!ctx_) {
-    last_status_ = ESIKF_ERR_STATE, last_error_ = "SetWorldCloud: no device context";
-    return;
-  }
+  if (missing(*this, "SetWorldCloud", ctx_)) return;
   const int n = dense_scan ? (int)dense_scan->size() : 0;
   double *sbuf; float *pts;
   if (!lay_out_staging(block_, [&](ScratchLayout &s) { sbuf = s.take<double>(ESIKF_STATE_DOUBLES), pts = dense_scan ? s.take<float>((size_t)n * 3 + 3) : nullptr; }))
@@ -354,10 +371,7 @@ void VoxelMapManager::SetWorldCloud(const std::vector<PointXYZ> *dense_scan) {
 }
 
 void VoxelMapManager::FindCorrespond(int n, const V3D *pts, int rule, uint8_t *status, VoxelPlane *planes) {
-  if (!ctx_ || !device_map_) {
-    last_status_ = ESIKF_ERR_STATE, last_error_ = "FindCorrespond: EnableDeviceMap first (a host-owned voxel_map_ is read by the reference's own code)";
-    return;
-  }
+  if (no_device_map(*this, ctx_ && device_map_, "FindCorrespond: EnableDeviceMap first (a host-owned voxel_map_ is read by the reference's own code)")) return;
   if (n < 0 || (n > 0 && (!pts || !status || !planes))) {
     last_status_ = ESIKF_ERR_ARG, last_error_ = "FindCorrespond: bad argument";
     return;
@@ -373,20 +387,14 @@ void VoxelMapManager::FindCorrespond(int n, const V3D *pts, int rule, uint8_t *s
     VoxelPlane &o = planes[i];
     o = VoxelPlane();
     if (st[i] == ESIKF_FIND_NO_ROOT) continue;
-    const esikf_plane &r = rows[i];
-    for (int k = 0; k < 3; k++) o.center_[k] = r.center[k], o.normal_[k] = r.normal[k];
-    for (int a = 0, t = 0; a < 6; a++)
-      for (int b = a; b < 6; b++, t++) o.plane_var_[6 * a + b] = o.plane_var_[6 * b + a] = r.plane_var[t];
-    o.d_ = r.d, o.radius_ = r.radius, o.is_plane_ = st[i] == ESIKF_FIND_PLANE;
+    plane_from_row(rows[i], o);
+    o.is_plane_ = st[i] == ESIKF_FIND_PLANE;
   }
 }
 
 // src/voxel_map.cpp:924-948: nothing until the sensor moved sliding_thresh, then roots further than half_map_size voxels go
 void VoxelMapManager::mapSliding() {
-  if (!ctx_ || !device_map_) {
-    last_status_ = ESIKF_ERR_STATE, last_error_ = "mapSliding: EnableDeviceMap first (a host-owned voxel_map_ slides in the reference's own code)";
-    return;
-  }
+  if (no_device_map(*this, ctx_ && device_map_, "mapSliding: EnableDeviceMap first (a host-owned voxel_map_ slides in the reference's own code)")) return;
   double d2 = 0;
   for (int k = 0; k < 3; k++) d2 += (position_last_[k] - last_slide_position[k]) * (position_last_[k] - last_slide_position[k]);
   if (sqrt(d2) < config_setting_.sliding_thresh) return;
@@ -412,10 +420,7 @@ void VoxelMapManager::mapSliding() {
 
 // include/voxel_map.h:232 / src/voxel_map.cpp:609-641
 void VoxelMapManager::UpdateVoxelMap(const std::vector<pointWithVar> &input_points) {
-  if (!ctx_ || !device_map_) {
-    last_status_ = ESIKF_ERR_STATE, last_error_ = "UpdateVoxelMap: EnableDeviceMap first";
-    return;
-  }
+  if (no_device_map(*this, ctx_ && device_map_, "UpdateVoxelMap: EnableDeviceMap first")) return;
   const size_t n = input_points.size();
   double *pw, *var;
   if (!lay_out_staging(block_, [&](ScratchLayout &s) { pw = s.take<double>(n * 3 + 1), var = s.take<double>(n * 9 + 1); })) return StagingFailed();
@@ -519,10 +524,7 @@ void VIOManager::GenerateVisualMapPoints(const std::vector<uint8_t> &type_map, i
                                          const std::vector<pointWithVar> *pg, const std::vector<pointWithVar> *add_from_voxel_map,
                                          std::vector<NewVisualPoint> &new_points) {
   new_points.clear();
-  if (!ctx_ || !state) {
-    last_status_ = ESIKF_ERR_STATE, last_error_ = "GenerateVisualMapPoints: no device context or state";
-    return;
-  }
+  if (missing(*this, "GenerateVisualMapPoints", ctx_, state)) return;
   const size_t n = pg ? pg->size() : 0, m = add_from_voxel_map ? add_from_voxel_map->size() : 0;
   const int cap = (int)type_map.size();  // at most one point per cell
   double *sbuf, *pw, *nv, *var, *ap, *an, *pos, *pc, *normal, *pvar;
@@ -559,10 +561,7 @@ void VIOManager::GenerateVisualMapPoints(const std::vector<uint8_t> &type_map, i
 void VIOManager::UpdateVisualMapPoints(const std::vector<uint8_t> &converged, const std::vector<LastObservation> &last_obs, std::vector<uint8_t> &update_flag,
                                        std::vector<NewObservation> &new_obs) {
   new_obs.clear();
-  if (!ctx_ || !state) {
-    last_status_ = ESIKF_ERR_STATE, last_error_ = "UpdateVisualMapPoints: no device context or state";
-    return;
-  }
+  if (missing(*this, "UpdateVisualMapPoints", ctx_, state)) return;
   update_flag.assign(total_points > 0 ? total_points : 0, 0);
   if (total_points <= 0) {  // src/vio.cpp:910
     last_status_ = ESIKF_OK;
@@ -595,10 +594,7 @@ void VIOManager::UpdateVisualMapPoints(const std::vector<uint8_t> &converged, co
 
 void VIOManager::RetrieveScanVoxels(int border, const std::vector<pointWithVar> *pg, std::vector<VOXEL_LOCATION> &keys) {
   keys.clear();
-  if (!ctx_ || !state) {
-    last_status_ = ESIKF_ERR_STATE, last_error_ = "RetrieveScanVoxels: no device context or state";
-    return;
-  }
+  if (missing(*this, "RetrieveScanVoxels", ctx_, state)) return;
   const size_t n = pg ? pg->size() : 0;
   // room for one key per point of a host scan; for the resident scan a first call reports the count when the room is short
   int32_t cap = pg ? (int32_t)n : (int32_t)(keys_cap_ > 0 ? keys_cap_ : 1 << 16), k = -1;
@@ -622,10 +618,7 @@ void VIOManager::RetrieveScanVoxels(int border, const std::vector<pointWithVar> 
 
 void VIOManager::CheckDepthContinuity(int n, const double *pos, const double *pc, std::vector<uint8_t> &discontinuous) {
   discontinuous.assign(n > 0 ? n : 0, 0);
-  if (!ctx_) {
-    last_status_ = ESIKF_ERR_STATE, last_error_ = "CheckDepthContinuity: no device context";
-    return;
-  }
+  if (missing(*this, "CheckDepthContinuity", ctx_)) return;
   if (n <= 0) {
     last_status_ = n < 0 ? ESIKF_ERR_ARG : ESIKF_OK;
     return;
@@ -639,10 +632,7 @@ void VIOManager::CheckDepthContinuity(int n, const double *pos, const double *pc
 
 void VIOManager::ScoreReferencePatches(const std::vector<int32_t> &first, const std::vector<ScoredPoint> &pts, const std::vector<PatchObservation> &obs,
                                        std::vector<float> &score, std::vector<float> &mean, std::vector<int32_t> &ref) {
-  if (!ctx_) {
-    last_status_ = ESIKF_ERR_STATE, last_error_ = "ScoreReferencePatches: no device context";
-    return;
-  }
+  if (missing(*this, "ScoreReferencePatches", ctx_)) return;
   if (first.size() != pts.size() + 1) {
     last_status_ = ESIKF_ERR_ARG, last_error_ = "ScoreReferencePatches: first must have pts.size() + 1 entries";
     return;
@@ -666,20 +656,14 @@ void VIOManager::ScoreReferencePatches(const std::vector<int32_t> &first, const 
 }
 
 void VIOManager::EnableDeviceObservations(int64_t capacity) {
-  if (!ctx_) {
-    last_status_ = ESIKF_ERR_STATE, last_error_ = "EnableDeviceObservations: no device context";
-    return;
-  }
+  if (missing(*this, "EnableDeviceObservations", ctx_)) return;
   Record(ctx_, esikf_vmap_init(ctx_, capacity));
 }
 
 void VIOManager::AddVisualPoints(const std::vector<int32_t> &first, const std::vector<StoredObservation> &obs, const std::vector<int32_t> &ref,
                                  std::vector<int32_t> &point_ids) {
   point_ids.clear();
-  if (!ctx_) {
-    last_status_ = ESIKF_ERR_STATE, last_error_ = "AddVisualPoints: no device context";
-    return;
-  }
+  if (missing(*this, "AddVisualPoints", ctx_)) return;
   if (first.size() != ref.size() + 1) {
     last_status_ = ESIKF_ERR_ARG, last_error_ = "AddVisualPoints: first must have ref.size() + 1 entries";
     return;
@@ -704,10 +688,7 @@ void VIOManager::UpdateVisualMapPoints(const std::vector<int32_t> &point_ids, co
                                        std::vector<uint8_t> &update_flag, std::vector<NewObservation> &new_obs, std::vector<int32_t> &evicted,
                                        std::vector<int32_t> &count) {
   new_obs.clear();
-  if (!ctx_ || !state) {
-    last_status_ = ESIKF_ERR_STATE, last_error_ = "UpdateVisualMapPoints: no device context or state";
-    return;
-  }
+  if (missing(*this, "UpdateVisualMapPoints", ctx_, state)) return;
   const int n = total_points > 0 ? total_points : 0;
   update_flag.assign(n, 0), evicted.assign(n, -1), count.assign(n, 0);
   if (point_ids.size() != (size_t)n || converged.size() != (size_t)n) {
@@ -740,10 +721,7 @@ void VIOManager::UpdateVisualMapPoints(const std::vector<int32_t> &point_ids, co
 
 void VIOManager::ScoreReferencePatches(const std::vector<int32_t> &point_ids, const std::vector<ScoredPoint> &pts, std::vector<int32_t> &ref) {
   ref.clear();
-  if (!ctx_) {
-    last_status_ = ESIKF_ERR_STATE, last_error_ = "ScoreReferencePatches: no device context";
-    return;
-  }
+  if (missing(*this, "ScoreReferencePatches", ctx_)) return;
   if (point_ids.size() != pts.size()) {
     last_status_ = ESIKF_ERR_ARG, last_error_ = "ScoreReferencePatches: point_ids and pts differ in size";
     return;
@@ -760,10 +738,7 @@ void VIOManager::ScoreReferencePatches(const std::vector<int32_t> &point_ids, co
 void VIOManager::ChooseReferenceFeatures(const std::vector<int32_t> &point_ids, const double *pos, const double frame_pos[3], bool normal_en,
                                          std::vector<int32_t> &ref) {
   ref.clear();
-  if (!ctx_) {
-    last_status_ = ESIKF_ERR_STATE, last_error_ = "ChooseReferenceFeatures: no device context";
-    return;
-  }
+  if (missing(*this, "ChooseReferenceFeatures", ctx_)) return;
   const size_t n = point_ids.size();
   double *d; int32_t *k;  // pos 3n | frame_pos 3, then point_ids n | ref n
   if (!lay_out_staging(block_, [&](ScratchLayout &s) { d = s.take<double>(3 * n + 3), k = s.take<int32_t>(2 * n); })) return StagingFailed();
@@ -900,10 +875,7 @@ void VIOManager::SetReferenceImages(const GrayImage *imgs, int n) {
 
 void VIOManager::ColorizeFrameWorld(const BgrImage &img_rgb, double blind_rgb_points, std::vector<PointXYZRGB> &laserCloudWorldRGB) {
   laserCloudWorldRGB.clear();
-  if (!ctx_ || !state) {
-    last_status_ = ESIKF_ERR_STATE, last_error_ = "ColorizeFrameWorld: no device context or state";
-    return;
-  }
+  if (missing(*this, "ColorizeFrameWorld", ctx_, state)) return;
   int32_t kept = 0;
   double *sbuf; float *xyz; uint8_t *bgr;
   // room for the largest coloured scan seen so far; a larger one is computed again with more room
@@ -1024,14 +996,78 @@ static void build_tree(VoxelMap &map, const VoxelMapConfig &cfg, const int64_t *
         node = node->leaves_[leaf];
       }
       VoxelPlane &p = *node->plane_ptr_;
-      for (int k = 0; k < 3; k++) p.center_[k] = f.center[k], p.normal_[k] = f.normal[k];
-      int t = 0;
-      for (int i = 0; i < 6; i++)
-        for (int j = i; j < 6; j++) p.plane_var_[i * 6 + j] = p.plane_var_[j * 6 + i] = f.plane_var[t++];
-      p.d_ = f.d, p.radius_ = f.radius, p.is_plane_ = true, p.is_init_ = true;
+      plane_from_row(f, p);
+      p.is_plane_ = true, p.is_init_ = true;
     }
   }
 }
+
+// VoxelMapConfig from the C ABI's LIO settings; the map-building part keeps its defaults
+static VoxelMapConfig map_config(const esikf_lio_cfg &l) {
+  VoxelMapConfig cfg;
+  cfg.max_voxel_size_ = l.voxel_size, cfg.max_layer_ = l.max_layer, cfg.max_iterations_ = l.max_iterations;
+  cfg.beam_err_ = l.beam_err, cfg.dept_err_ = l.dept_err, cfg.sigma_num_ = l.sigma_num;
+  return cfg;
+}
+
+// A VIOManager set up from the C ABI's camera and VIO settings, then initializeVIO. A null ext keeps the manager's default
+// extrinsics.
+static void configure_vio(VIOManager &vio, const esikf_camera &cam, const esikf_vio_cfg &vcfg, const esikf_extrinsics *ext) {
+  vio.cam = cam;
+  vio.patch_pyrimid_level = vcfg.patch_pyrimid_level, vio.max_iterations = vcfg.max_iterations, vio.img_point_cov = vcfg.img_point_cov;
+  vio.exposure_estimate_en = vcfg.exposure_estimate_en != 0;
+  if (ext) memcpy(vio.Rcl.m, ext->Rcl, 72), memcpy(vio.Pcl.v, ext->Pcl, 24), memcpy(vio.extR.m, ext->extR, 72), memcpy(vio.extT.v, ext->extT, 24);
+  vio.initializeVIO();
+}
+
+namespace {
+// The managers a hook runs on, held as LIVMapper holds them: the host octree, the VoxelMapManager on it (whose constructor
+// creates the device context) and a VIOManager sharing that context, on the session's states and visual sub-map. The
+// session hooks keep one across ticks (bench.py e2e_shim); the one-shot GPU hooks open one per call. A mirror handle
+// (fl2_shim_mirror_create) is a session without managers.
+struct ShimSession {
+  VoxelMapConfig cfg;
+  VoxelMap map;
+  std::unique_ptr<VoxelMapManager> mgr;
+  std::unique_ptr<VIOManager> vio;
+  SubSparseMap sub;
+  StatesGroup st, stp;
+  bool has_vio = false;
+  esikf_camera cam{};
+  esikf_vio_cfg vcfg{};
+  long long manager_ns = 0;
+  ~ShimSession() {
+    vio.reset(), mgr.reset();
+    ClearVoxelMap(map);
+  }
+  // A VoxelMapManager on the session's map and a new device context: all the hooks that need no map open. Returns its status.
+  int open(int device = 0) {
+    mgr.reset(new VoxelMapManager(cfg, map, device));
+    return mgr->last_status_;
+  }
+  // The LIO half: the octree of the flat map, its manager set up from lcfg and the LiDAR extrinsics of ext, and the map's
+  // first upload. Returns the first failing esikf_status.
+  int open_map(const esikf_lio_cfg &lcfg, const int64_t *keys, const int32_t *first, const int32_t *count, int n_roots, const esikf_plane *planes,
+               const esikf_extrinsics &ext, int device) {
+    cfg = map_config(lcfg);
+    build_tree(map, cfg, keys, first, count, n_roots, planes);
+    if (int rc = open(device)) return rc;
+    memcpy(mgr->extR_.m, ext.extR, 72), memcpy(mgr->extT_.v, ext.extT, 24);
+    mgr->SyncDeviceMap();
+    return mgr->last_status_;
+  }
+  // The VIO half: a VIOManager on the context, st, stp and sub; with cam (and vcfg) configured by configure_vio, without left
+  // as constructed. Returns its status.
+  int open_vio(const esikf_camera *c, const esikf_vio_cfg *v, const esikf_extrinsics *ext) {
+    vio.reset(new VIOManager(mgr->context()));
+    vio->state = &st, vio->state_propagat = &stp, vio->visual_submap = &sub;
+    if (c) has_vio = true, cam = *c, vcfg = *v, configure_vio(*vio, *c, *v, ext);
+    return vio->last_status_;
+  }
+};
+}  // namespace
+
+static ShimSession *session_of(void *h) { return static_cast<ShimSession *>(h); }
 
 extern "C" {
 
@@ -1062,65 +1098,49 @@ int fl2_shim_run(const int64_t *keys, const int32_t *first, const int32_t *count
                  const esikf_vio_cfg *vcfg, const uint8_t *img, int n_patches, const double *pos, const float *warp_patch, const int32_t *search_levels,
                  const double *inv_expo, double *vio_state_out, float *errors_out) {
   (void)n_planes;
-  VoxelMapConfig cfg;
-  cfg.max_voxel_size_ = lcfg->voxel_size, cfg.max_layer_ = lcfg->max_layer, cfg.max_iterations_ = lcfg->max_iterations;
-  cfg.beam_err_ = lcfg->beam_err, cfg.dept_err_ = lcfg->dept_err, cfg.sigma_num_ = lcfg->sigma_num;
-  VoxelMap map;
-  build_tree(map, cfg, keys, first, count, n_roots, planes);
-  int rc = 0;
-  {
-    VoxelMapManager mgr(cfg, map, 0);
-    if (mgr.last_status_) rc = mgr.last_status_;
-    memcpy(mgr.extR_.m, ext->extR, 72);
-    memcpy(mgr.extT_.v, ext->extT, 24);
-    mgr.feats_down_body_.resize(n);
-    memcpy(mgr.feats_down_body_.data(), pts, (size_t)n * 12);
-    mgr.feats_down_size_ = n;
-    mgr.state_.unpack(state_in);              // voxelmap_manager->state_ = _state  (LIVMapper.cpp:257)
-    StatesGroup prop;
-    prop.unpack(state_prop);
-    if (!rc) {
-      mgr.SyncDeviceMap();
-      mgr.StateEstimation(prop);              // LIVMapper.cpp:370
-      rc = mgr.last_status_;
+  ShimSession s;
+  int rc = s.open_map(*lcfg, keys, first, count, n_roots, planes, *ext, 0);
+  VoxelMapManager &mgr = *s.mgr;
+  mgr.feats_down_body_.resize(n);
+  memcpy(mgr.feats_down_body_.data(), pts, (size_t)n * 12);
+  mgr.feats_down_size_ = n;
+  mgr.state_.unpack(state_in);              // voxelmap_manager->state_ = _state  (LIVMapper.cpp:257)
+  StatesGroup prop;
+  prop.unpack(state_prop);
+  if (!rc) {
+    mgr.StateEstimation(prop);              // LIVMapper.cpp:370
+    rc = mgr.last_status_;
+  }
+  if (!rc) {
+    mgr.state_.pack(lio_state_out);
+    *n_effective = mgr.effct_feat_num_;
+    *n_ptpl = (int32_t)mgr.ptpl_list_.size();
+    for (int i = 0; i < n; i++)
+      for (int k = 0; k < 3; k++) normals_out[3 * i + k] = mgr.pv_list_[i].normal[k];
+  }
+  if (!rc && cam && n_patches > 0) {
+    s.st = mgr.state_, s.stp = mgr.state_;
+    SubSparseMap &sub = s.sub;
+    const int L = vcfg->patch_pyrimid_level;
+    for (int i = 0; i < n_patches; i++) {
+      V3D p;
+      for (int k = 0; k < 3; k++) p[k] = pos[3 * i + k];
+      sub.voxel_points_pos.push_back(p);
+      sub.warp_patch.emplace_back(warp_patch + (size_t)i * 64 * L, warp_patch + (size_t)(i + 1) * 64 * L);
+      sub.search_levels.push_back(search_levels[i]);
+      sub.inv_expo_list.push_back(inv_expo[i]);
     }
+    rc = s.open_vio(cam, vcfg, ext);
+    s.vio->total_points = n_patches;
+    GrayImage im;
+    im.data = img, im.cols = cam->width, im.rows = cam->height;
+    if (!rc) s.vio->computeJacobianAndUpdateEKF(im);
+    rc = s.vio->last_status_;
     if (!rc) {
-      mgr.state_.pack(lio_state_out);
-      *n_effective = mgr.effct_feat_num_;
-      *n_ptpl = (int32_t)mgr.ptpl_list_.size();
-      for (int i = 0; i < n; i++)
-        for (int k = 0; k < 3; k++) normals_out[3 * i + k] = mgr.pv_list_[i].normal[k];
-    }
-    if (!rc && cam && n_patches > 0) {
-      VIOManager vio(mgr.context());
-      StatesGroup st = mgr.state_, stp = mgr.state_;
-      SubSparseMap sub;
-      const int L = vcfg->patch_pyrimid_level;
-      for (int i = 0; i < n_patches; i++) {
-        V3D p;
-        for (int k = 0; k < 3; k++) p[k] = pos[3 * i + k];
-        sub.voxel_points_pos.push_back(p);
-        sub.warp_patch.emplace_back(warp_patch + (size_t)i * 64 * L, warp_patch + (size_t)(i + 1) * 64 * L);
-        sub.search_levels.push_back(search_levels[i]);
-        sub.inv_expo_list.push_back(inv_expo[i]);
-      }
-      vio.state = &st, vio.state_propagat = &stp, vio.visual_submap = &sub, vio.total_points = n_patches;
-      vio.patch_pyrimid_level = L, vio.max_iterations = vcfg->max_iterations, vio.img_point_cov = vcfg->img_point_cov;
-      vio.exposure_estimate_en = vcfg->exposure_estimate_en != 0;
-      vio.cam = *cam;
-      memcpy(vio.Rcl.m, ext->Rcl, 72), memcpy(vio.Pcl.v, ext->Pcl, 24), memcpy(vio.extR.m, ext->extR, 72), memcpy(vio.extT.v, ext->extT, 24);
-      vio.initializeVIO();
-      GrayImage im;
-      im.data = img, im.cols = cam->width, im.rows = cam->height;
-      if (!vio.last_status_) vio.computeJacobianAndUpdateEKF(im);
-      rc = vio.last_status_;
-      if (!rc) {
-        st.pack(vio_state_out);
-        for (int i = 0; i < n_patches; i++) errors_out[i] = sub.errors[i];
-      }
+      s.st.pack(vio_state_out);
+      for (int i = 0; i < n_patches; i++) errors_out[i] = sub.errors[i];
     }
   }
-  for (auto &kv : map) delete kv.second;
   return rc;
 }
 
@@ -1147,56 +1167,37 @@ int fl2_shim_resync_run(const int64_t *keys, const int32_t *first, const int32_t
                         int n_planes, const esikf_lio_cfg *lcfg, const esikf_extrinsics *ext, const float *pts, int n, const double *state_in,
                         double *state_out, int32_t *n_patched) {
   (void)n_planes;
-  VoxelMapConfig cfg;
-  cfg.max_voxel_size_ = lcfg->voxel_size, cfg.max_layer_ = lcfg->max_layer, cfg.max_iterations_ = lcfg->max_iterations;
-  cfg.beam_err_ = lcfg->beam_err, cfg.dept_err_ = lcfg->dept_err, cfg.sigma_num_ = lcfg->sigma_num;
-  VoxelMap map;
-  build_tree(map, cfg, keys, first, count, n_roots, planes_a);
-  int rc = 0;
-  {
-    VoxelMapManager mgr(cfg, map, 0);
-    rc = mgr.last_status_;
-    memcpy(mgr.extR_.m, ext->extR, 72);
-    memcpy(mgr.extT_.v, ext->extT, 24);
-    if (!rc) {
-      mgr.SyncDeviceMap();
-      rc = mgr.last_status_;
-    }
-    if (!rc) {
-      // the host map changes under the manager: same octree, new plane fits
-      for (int r = 0; r < n_roots; r++) {
-        VOXEL_LOCATION loc(keys[3 * r], keys[3 * r + 1], keys[3 * r + 2]);
-        for (int c = 0; c < count[r]; c++) {
-          const esikf_plane &f = planes_b[first[r] + c];
-          VoxelOctoTree *node = map[loc];
-          for (int l = 0; l < f.layer; l++) node = node->leaves_[(f.path >> (3 * l)) & 7];
-          VoxelPlane &p = *node->plane_ptr_;
-          for (int k = 0; k < 3; k++) p.center_[k] = f.center[k], p.normal_[k] = f.normal[k];
-          int t = 0;
-          for (int i = 0; i < 6; i++)
-            for (int j = i; j < 6; j++) p.plane_var_[i * 6 + j] = p.plane_var_[j * 6 + i] = f.plane_var[t++];
-          p.d_ = f.d, p.radius_ = f.radius;
-        }
+  ShimSession s;
+  int rc = s.open_map(*lcfg, keys, first, count, n_roots, planes_a, *ext, 0);
+  VoxelMapManager &mgr = *s.mgr;
+  if (!rc) {
+    // the host map changes under the manager: same octree, new plane fits
+    for (int r = 0; r < n_roots; r++) {
+      VOXEL_LOCATION loc(keys[3 * r], keys[3 * r + 1], keys[3 * r + 2]);
+      for (int c = 0; c < count[r]; c++) {
+        const esikf_plane &f = planes_b[first[r] + c];
+        VoxelOctoTree *node = s.map[loc];
+        for (int l = 0; l < f.layer; l++) node = node->leaves_[(f.path >> (3 * l)) & 7];
+        plane_from_row(f, *node->plane_ptr_);
       }
-      mgr.MarkMapDirty();
-      mgr.SyncDeviceMap();
-      rc = mgr.last_status_;
-      *n_patched = mgr.last_sync_patched_;
     }
-    if (!rc) {
-      mgr.feats_down_body_.resize(n);
-      memcpy(mgr.feats_down_body_.data(), pts, (size_t)n * 12);
-      mgr.feats_down_size_ = n;
-      mgr.fill_point_lists_ = false;
-      mgr.state_.unpack(state_in);
-      StatesGroup prop;
-      prop.unpack(state_in);
-      mgr.StateEstimation(prop);
-      rc = mgr.last_status_;
-      if (!rc) mgr.state_.pack(state_out);
-    }
+    mgr.MarkMapDirty();
+    mgr.SyncDeviceMap();
+    rc = mgr.last_status_;
+    *n_patched = mgr.last_sync_patched_;
   }
-  for (auto &kv : map) delete kv.second;
+  if (!rc) {
+    mgr.feats_down_body_.resize(n);
+    memcpy(mgr.feats_down_body_.data(), pts, (size_t)n * 12);
+    mgr.feats_down_size_ = n;
+    mgr.fill_point_lists_ = false;
+    mgr.state_.unpack(state_in);
+    StatesGroup prop;
+    prop.unpack(state_in);
+    mgr.StateEstimation(prop);
+    rc = mgr.last_status_;
+    if (!rc) mgr.state_.pack(state_out);
+  }
   return rc;
 }
 
@@ -1207,59 +1208,52 @@ int fl2_shim_resync_run(const int64_t *keys, const int32_t *first, const int32_t
 int fl2_shim_select_run(const esikf_camera *cam, const esikf_vio_cfg *vcfg, const esikf_extrinsics *ext, const uint8_t *img, const uint8_t *const *ref_imgs,
                         int n_imgs, const SubMapCandidate *cands, int n, const double *T_cur_w, const double *state_in, const double *gate, int32_t *n_kept,
                         int32_t *kept, double *state_sel, float *errors_sel, double *state_host, float *errors_host, float *warp_out, int64_t *counts) {
-  esikf_ctx *ctx = nullptr;
-  int rc = esikf_create(&ctx, 0);
+  ShimSession s;
+  int rc = s.open();
   if (rc) return rc;
-  {
-    VIOManager vio(ctx);
-    StatesGroup st, stp;
-    st.unpack(state_in), stp.unpack(state_in);
-    SubSparseMap sub;
-    vio.state = &st, vio.state_propagat = &stp, vio.visual_submap = &sub;
-    vio.patch_pyrimid_level = vcfg->patch_pyrimid_level, vio.max_iterations = vcfg->max_iterations, vio.img_point_cov = vcfg->img_point_cov;
-    vio.exposure_estimate_en = vcfg->exposure_estimate_en != 0;
-    vio.cam = *cam;
-    memcpy(vio.Rcl.m, ext->Rcl, 72), memcpy(vio.Pcl.v, ext->Pcl, 24), memcpy(vio.extR.m, ext->extR, 72), memcpy(vio.extT.v, ext->extT, 24);
-    vio.normal_en = gate[0] != 0, vio.ncc_en = gate[1] != 0, vio.ncc_thre = gate[2], vio.outlier_threshold = gate[3];
-    vio.initializeVIO();
-    GrayImage im;
-    im.data = img, im.cols = cam->width, im.rows = cam->height;
-    std::vector<GrayImage> refs(n_imgs);
-    for (int k = 0; k < n_imgs; k++) refs[k].data = ref_imgs[k], refs[k].cols = cam->width, refs[k].rows = cam->height;
-    if (!vio.last_status_) vio.SetReferenceImages(refs.data(), n_imgs);
-    if (!vio.last_status_) vio.SelectSubSparseMap(cands, n, im, T_cur_w);
+  esikf_ctx *ctx = s.mgr->context();
+  StatesGroup &st = s.st;
+  SubSparseMap &sub = s.sub;
+  st.unpack(state_in), s.stp.unpack(state_in);
+  s.open_vio(cam, vcfg, ext);
+  VIOManager &vio = *s.vio;
+  vio.normal_en = gate[0] != 0, vio.ncc_en = gate[1] != 0, vio.ncc_thre = gate[2], vio.outlier_threshold = gate[3];
+  GrayImage im;
+  im.data = img, im.cols = cam->width, im.rows = cam->height;
+  std::vector<GrayImage> refs(n_imgs);
+  for (int k = 0; k < n_imgs; k++) refs[k].data = ref_imgs[k], refs[k].cols = cam->width, refs[k].rows = cam->height;
+  if (!vio.last_status_) vio.SetReferenceImages(refs.data(), n_imgs);
+  if (!vio.last_status_) vio.SelectSubSparseMap(cands, n, im, T_cur_w);
+  rc = vio.last_status_;
+  if (!rc) {
+    *n_kept = vio.total_points;
+    for (int j = 0; j < vio.total_points; j++) kept[j] = sub.candidate_index[j];
+    int64_t l0 = esikf_launch_count(ctx);
+    vio.computeJacobianAndUpdateEKF(im);
+    counts[0] = esikf_launch_count(ctx) - l0, counts[1] = vio.submap_uploads_;
+    rc = vio.last_status_;
+  }
+  if (!rc) {
+    st.pack(state_sel);
+    for (int j = 0; j < vio.total_points; j++) errors_sel[j] = sub.errors[j];
+    vio.MaterializeWarpPatches();
+    rc = vio.last_status_;
+  }
+  if (!rc) {
+    const int L = vio.patch_pyrimid_level;
+    for (int j = 0; j < vio.total_points; j++) memcpy(warp_out + (size_t)j * 64 * L, sub.warp_patch[j].data(), sizeof(float) * 64 * L);
+    SubSparseMap host = sub;  // the sub-map as a host-side retrieval would have assembled it
+    vio.visual_submap = &host;
+    st.unpack(state_in);
+    int64_t l0 = esikf_launch_count(ctx);
+    vio.computeJacobianAndUpdateEKF(im);
+    counts[2] = esikf_launch_count(ctx) - l0, counts[3] = vio.submap_uploads_;
     rc = vio.last_status_;
     if (!rc) {
-      *n_kept = vio.total_points;
-      for (int j = 0; j < vio.total_points; j++) kept[j] = sub.candidate_index[j];
-      int64_t l0 = esikf_launch_count(ctx);
-      vio.computeJacobianAndUpdateEKF(im);
-      counts[0] = esikf_launch_count(ctx) - l0, counts[1] = vio.submap_uploads_;
-      rc = vio.last_status_;
-    }
-    if (!rc) {
-      st.pack(state_sel);
-      for (int j = 0; j < vio.total_points; j++) errors_sel[j] = sub.errors[j];
-      vio.MaterializeWarpPatches();
-      rc = vio.last_status_;
-    }
-    if (!rc) {
-      const int L = vio.patch_pyrimid_level;
-      for (int j = 0; j < vio.total_points; j++) memcpy(warp_out + (size_t)j * 64 * L, sub.warp_patch[j].data(), sizeof(float) * 64 * L);
-      SubSparseMap host = sub;  // the sub-map as a host-side retrieval would have assembled it
-      vio.visual_submap = &host;
-      st.unpack(state_in);
-      int64_t l0 = esikf_launch_count(ctx);
-      vio.computeJacobianAndUpdateEKF(im);
-      counts[2] = esikf_launch_count(ctx) - l0, counts[3] = vio.submap_uploads_;
-      rc = vio.last_status_;
-      if (!rc) {
-        st.pack(state_host);
-        for (int j = 0; j < vio.total_points; j++) errors_host[j] = host.errors[j];
-      }
+      st.pack(state_host);
+      for (int j = 0; j < vio.total_points; j++) errors_host[j] = host.errors[j];
     }
   }
-  esikf_destroy(ctx);
   return rc;
 }
 
@@ -1268,33 +1262,25 @@ int fl2_shim_select_run(const esikf_camera *cam, const esikf_vio_cfg *vcfg, cons
 // for n x 3) and flags (n_cand). Returns 0 or the first failing esikf_status.
 int fl2_shim_retrieve_run(const esikf_camera *cam, const esikf_vio_cfg *vcfg, const esikf_extrinsics *ext, const double *state, const double *pg, int n, int border,
                           const double *cand_pos, const double *cand_pc, int n_cand, int32_t *n_keys, int64_t *keys, uint8_t *flags) {
-  esikf_ctx *ctx = nullptr;
-  int rc = esikf_create(&ctx, 0);
+  ShimSession s;
+  int rc = s.open();
   if (rc) return rc;
-  {
-    VIOManager vio(ctx);
-    StatesGroup st, stp;
-    st.unpack(state), stp.unpack(state);
-    vio.state = &st, vio.state_propagat = &stp;
-    vio.patch_pyrimid_level = vcfg->patch_pyrimid_level, vio.max_iterations = vcfg->max_iterations, vio.img_point_cov = vcfg->img_point_cov;
-    vio.cam = *cam;
-    memcpy(vio.Rcl.m, ext->Rcl, 72), memcpy(vio.Pcl.v, ext->Pcl, 24), memcpy(vio.extR.m, ext->extR, 72), memcpy(vio.extT.v, ext->extT, 24);
-    vio.initializeVIO();
-    std::vector<pointWithVar> scan(n);
-    for (int i = 0; i < n; i++)
-      for (int k = 0; k < 3; k++) scan[i].point_w[k] = pg[3 * i + k];
-    std::vector<VOXEL_LOCATION> kv;
-    std::vector<uint8_t> fl;
-    if (!vio.last_status_) vio.RetrieveScanVoxels(border, &scan, kv);
-    if (!vio.last_status_) vio.CheckDepthContinuity(n_cand, cand_pos, cand_pc, fl);
-    rc = vio.last_status_;
-    if (!rc) {
-      *n_keys = (int32_t)kv.size();
-      for (size_t i = 0; i < kv.size(); i++) keys[3 * i] = kv[i].x, keys[3 * i + 1] = kv[i].y, keys[3 * i + 2] = kv[i].z;
-      memcpy(flags, fl.data(), fl.size());
-    }
+  s.st.unpack(state), s.stp.unpack(state);
+  s.open_vio(cam, vcfg, ext);
+  VIOManager &vio = *s.vio;
+  std::vector<pointWithVar> scan(n);
+  for (int i = 0; i < n; i++)
+    for (int k = 0; k < 3; k++) scan[i].point_w[k] = pg[3 * i + k];
+  std::vector<VOXEL_LOCATION> kv;
+  std::vector<uint8_t> fl;
+  if (!vio.last_status_) vio.RetrieveScanVoxels(border, &scan, kv);
+  if (!vio.last_status_) vio.CheckDepthContinuity(n_cand, cand_pos, cand_pc, fl);
+  rc = vio.last_status_;
+  if (!rc) {
+    *n_keys = (int32_t)kv.size();
+    for (size_t i = 0; i < kv.size(); i++) keys[3 * i] = kv[i].x, keys[3 * i + 1] = kv[i].y, keys[3 * i + 2] = kv[i].z;
+    memcpy(flags, fl.data(), fl.size());
   }
-  esikf_destroy(ctx);
   return rc;
 }
 
@@ -1302,83 +1288,33 @@ int fl2_shim_retrieve_run(const esikf_camera *cam, const esikf_vio_cfg *vcfg, co
 int fl2_shim_patch_helpers(const esikf_camera *cam, const esikf_vio_cfg *vcfg, const uint8_t *img, int cols, int rows, const double *pc, int level,
                            float *patch_tmp /* levels*64, only `level` written */, const double *A_cur_ref, const uint8_t *img_ref, const double *px_ref,
                            int search_level, int pyramid_level, float *warp_patch /* levels*64, only `pyramid_level` written */) {
-  esikf_ctx *ctx = nullptr;
-  int rc = esikf_create(&ctx, 0);
+  ShimSession s;
+  int rc = s.open();
   if (rc) return rc;
-  {
-    VIOManager vio(ctx);
-    vio.cam = *cam;
-    vio.patch_pyrimid_level = vcfg->patch_pyrimid_level, vio.max_iterations = vcfg->max_iterations, vio.img_point_cov = vcfg->img_point_cov;
-    vio.exposure_estimate_en = vcfg->exposure_estimate_en != 0;
-    vio.initializeVIO();
+  // no extrinsics: both helpers sample images at the pixel coordinates they are given
+  rc = s.open_vio(cam, vcfg, nullptr);
+  VIOManager &vio = *s.vio;
+  GrayImage g{img, cols, rows}, gr{img_ref, cols, rows};
+  if (!rc) {
+    vio.getImagePatch(g, pc, patch_tmp, level);
     rc = vio.last_status_;
-    GrayImage g{img, cols, rows}, gr{img_ref, cols, rows};
-    if (!rc) {
-      vio.getImagePatch(g, pc, patch_tmp, level);
-      rc = vio.last_status_;
-    }
-    if (!rc) {
-      vio.warpAffine(A_cur_ref, gr, px_ref, 0, search_level, pyramid_level, 4, warp_patch);
-      rc = vio.last_status_;
-    }
   }
-  esikf_destroy(ctx);
+  if (!rc) {
+    vio.warpAffine(A_cur_ref, gr, px_ref, 0, search_level, pyramid_level, 4, warp_patch);
+    rc = vio.last_status_;
+  }
   return rc;
 }
 
 // ---- persistent session for the end-to-end measurement through the drop-in classes (bench.py e2e_shim): the managers,
 // the host octree and the visual sub-map live across ticks like they do inside LIVMapper.
-struct ShimSession {
-  VoxelMapConfig cfg;
-  VoxelMap map;
-  VoxelMapManager *mgr = nullptr;
-  VIOManager *vio = nullptr;
-  SubSparseMap sub;
-  StatesGroup st, stp;
-  bool has_vio = false;
-  esikf_camera cam{};
-  esikf_vio_cfg vcfg{};
-  long long manager_ns = 0;
-  ~ShimSession() {
-    delete vio;
-    delete mgr;
-    for (auto &kv : map) delete kv.second;
-  }
-};
-
 void *fl2_shim_session_create(const int64_t *keys, const int32_t *first, const int32_t *count, int n_roots, const esikf_plane *planes, int n_planes,
                               const esikf_lio_cfg *lcfg, const esikf_extrinsics *ext, const esikf_camera *cam, const esikf_vio_cfg *vcfg, int device) {
   (void)n_planes;
   ShimSession *s = new ShimSession;
-  s->cfg.max_voxel_size_ = lcfg->voxel_size, s->cfg.max_layer_ = lcfg->max_layer, s->cfg.max_iterations_ = lcfg->max_iterations;
-  s->cfg.beam_err_ = lcfg->beam_err, s->cfg.dept_err_ = lcfg->dept_err, s->cfg.sigma_num_ = lcfg->sigma_num;
-  build_tree(s->map, s->cfg, keys, first, count, n_roots, planes);
-  s->mgr = new VoxelMapManager(s->cfg, s->map, device);
-  if (s->mgr->last_status_) {
+  if (s->open_map(*lcfg, keys, first, count, n_roots, planes, *ext, device) || (cam && vcfg && s->open_vio(cam, vcfg, ext))) {
     delete s;
     return nullptr;
-  }
-  memcpy(s->mgr->extR_.m, ext->extR, 72);
-  memcpy(s->mgr->extT_.v, ext->extT, 24);
-  s->mgr->SyncDeviceMap();
-  if (s->mgr->last_status_) {
-    delete s;
-    return nullptr;
-  }
-  if (cam && vcfg) {
-    s->has_vio = true, s->cam = *cam, s->vcfg = *vcfg;
-    s->vio = new VIOManager(s->mgr->context());
-    VIOManager &vio = *s->vio;
-    vio.state = &s->st, vio.state_propagat = &s->stp, vio.visual_submap = &s->sub;
-    vio.patch_pyrimid_level = vcfg->patch_pyrimid_level, vio.max_iterations = vcfg->max_iterations, vio.img_point_cov = vcfg->img_point_cov;
-    vio.exposure_estimate_en = vcfg->exposure_estimate_en != 0;
-    vio.cam = *cam;
-    memcpy(vio.Rcl.m, ext->Rcl, 72), memcpy(vio.Pcl.v, ext->Pcl, 24), memcpy(vio.extR.m, ext->extR, 72), memcpy(vio.extT.v, ext->extT, 24);
-    vio.initializeVIO();
-    if (vio.last_status_) {
-      delete s;
-      return nullptr;
-    }
   }
   return s;
 }
@@ -1387,7 +1323,7 @@ void *fl2_shim_session_create(const int64_t *keys, const int32_t *first, const i
 // iterations, [1] = VIO iterations.
 int fl2_shim_session_step(void *h, const float *pts, int n, const double *state_in, const double *state_prop, const uint8_t *img, int n_patches, const double *pos,
                           const float *warp_patch, const int32_t *search_levels, const double *inv_expo, double *lio_state_out, double *vio_state_out, int32_t *iters_out) {
-  ShimSession *s = static_cast<ShimSession *>(h);
+  ShimSession *s = session_of(h);
   if (!s) return ESIKF_ERR_ARG;
   VoxelMapManager &mgr = *s->mgr;
   mgr.feats_down_body_.resize(n);
@@ -1432,14 +1368,14 @@ int fl2_shim_session_step(void *h, const float *pts, int n, const double *state_
 // mode 0: pv_list_ / ptpl_list_ / body_cov_list_ / cross_mat_list_ filled inside every StateEstimation (the reference's member
 // contract); 1: filled lazily (MaterializePointLists — never, in the timed loop of a caller that does not read them); 2: off.
 void fl2_shim_session_point_lists(void *h, int mode) {
-  ShimSession *s = static_cast<ShimSession *>(h);
+  ShimSession *s = session_of(h);
   if (!s) return;
   s->mgr->fill_point_lists_ = (mode != 2);
   s->mgr->lazy_point_lists_ = (mode == 1);
 }
 // number of entries the lists hold after materialising them (checks the lazy path in the tests)
 int fl2_shim_session_materialize(void *h, int32_t *n_pv, int32_t *n_ptpl) {
-  ShimSession *s = static_cast<ShimSession *>(h);
+  ShimSession *s = session_of(h);
   if (!s) return ESIKF_ERR_ARG;
   s->mgr->MaterializePointLists();
   if (n_pv) *n_pv = (int32_t)s->mgr->pv_list_.size();
@@ -1450,7 +1386,7 @@ int fl2_shim_session_materialize(void *h, int32_t *n_pv, int32_t *n_ptpl) {
 // Device-resident map for the session: the map the session was created with is dropped, an empty device map takes its place and
 // absorbs `pts` at `state` through BuildVoxelMap (first LiDAR frame, LIVMapper.cpp:356-366).
 int fl2_shim_session_device_map(void *h, const float *pts, int n, const double *state, double min_eigen_value, int max_points_num, long long root_capacity) {
-  ShimSession *s = static_cast<ShimSession *>(h);
+  ShimSession *s = session_of(h);
   if (!s) return ESIKF_ERR_ARG;
   VoxelMapManager &mgr = *s->mgr;
   mgr.config_setting_.planner_threshold_ = min_eigen_value, mgr.config_setting_.max_points_num_ = max_points_num;
@@ -1466,7 +1402,7 @@ int fl2_shim_session_device_map(void *h, const float *pts, int n, const double *
 }
 // LIVMapper.cpp:413-424 after the LIO half of a tick: the device map absorbs the scan with the LIO posterior.
 int fl2_shim_session_update_map(void *h) {
-  ShimSession *s = static_cast<ShimSession *>(h);
+  ShimSession *s = session_of(h);
   if (!s) return ESIKF_ERR_ARG;
   s->mgr->UpdateVoxelMap();
   return s->mgr->last_status_;
@@ -1475,11 +1411,11 @@ int fl2_shim_session_update_map(void *h) {
 // nanoseconds the last step spent inside StateEstimation + computeJacobianAndUpdateEKF (the two calls LIVMapper makes; filling
 // the managers' members from the harness' flat buffers — which LIVMapper already holds in that shape — is outside)
 long long fl2_shim_session_manager_ns(void *h) {
-  ShimSession *s = static_cast<ShimSession *>(h);
+  ShimSession *s = session_of(h);
   return s ? s->manager_ns : 0;
 }
 
-void fl2_shim_session_destroy(void *h) { delete static_cast<ShimSession *>(h); }
+void fl2_shim_session_destroy(void *h) { delete session_of(h); }
 
 // ---- the host mirror of a device map (VoxelMapConfig::device_map_mirror_). A mirror handle is a session without managers:
 // the apply code runs on the CPU there. The dump / flatten / find hooks take either kind of handle.
@@ -1489,11 +1425,11 @@ void *fl2_shim_mirror_create(double voxel_size, int max_layer) {
   return s;
 }
 int fl2_shim_mirror_apply(void *h, const int64_t *keys, const int32_t *first, const int32_t *count, int n_roots, const esikf_map_node *nodes, int n_nodes) {
-  ShimSession *s = static_cast<ShimSession *>(h);
+  ShimSession *s = session_of(h);
   if (!s) return ESIKF_ERR_ARG;
   return ApplyMapExport(s->map, s->cfg, keys, first, count, n_roots, nodes, n_nodes, nullptr) ? 0 : ESIKF_ERR_ARG;
 }
-void fl2_shim_mirror_erase(void *h, const int64_t *lo, const int64_t *hi) { EraseRootsOutside(static_cast<ShimSession *>(h)->map, lo, hi); }
+void fl2_shim_mirror_erase(void *h, const int64_t *lo, const int64_t *hi) { EraseRootsOutside(session_of(h)->map, lo, hi); }
 // The mirror's nodes as oracle_bind.NODE_COLS rows (DFS pre-order, leaves 0..7, roots in map order). Returns the number of
 // nodes; rows beyond cap are counted, not written.
 static void mirror_dump_node(const VoxelOctoTree *t, int64_t path, const VOXEL_LOCATION &key, int64_t *out, int cap, int *n) {
@@ -1509,12 +1445,12 @@ static void mirror_dump_node(const VoxelOctoTree *t, int64_t path, const VOXEL_L
 }
 int fl2_shim_mirror_dump(void *h, int64_t *out, int cap) {
   int n = 0;
-  for (const auto &kv : static_cast<ShimSession *>(h)->map) mirror_dump_node(kv.second, 0, kv.first, out, cap, &n);
+  for (const auto &kv : session_of(h)->map) mirror_dump_node(kv.second, 0, kv.first, out, cap, &n);
   return n;
 }
 // FlattenVoxelMap of the mirror, two calls: planes == NULL returns the sizes
 int fl2_shim_mirror_flatten(void *h, int *n_roots, int *n_planes, int64_t *keys, int32_t *first, int32_t *count, esikf_plane *planes) {
-  ShimSession *s = static_cast<ShimSession *>(h);
+  ShimSession *s = session_of(h);
   FlatVoxelMap flat;
   std::string err;
   if (!FlattenVoxelMap(s->map, s->cfg, flat, &err)) return ESIKF_ERR_ARG;
@@ -1530,7 +1466,7 @@ int fl2_shim_mirror_flatten(void *h, int *n_roots, int *n_planes, int64_t *keys,
 // updateReferencePatch's lookup (src/vio.cpp:983-993) per point: the root voxel by the float quotient (with the map's voxel
 // size), then find_correspond. out: n x 4 = found, layer, path, is_plane of the node it returns.
 void fl2_shim_mirror_find(void *h, const double *pts, int n, int64_t *out) {
-  ShimSession *s = static_cast<ShimSession *>(h);
+  ShimSession *s = session_of(h);
   for (int i = 0; i < n; i++) {
     const double *p = pts + 3 * (size_t)i;
     float loc_xyz[3];
@@ -1557,14 +1493,14 @@ void fl2_shim_mirror_find(void *h, const double *pts, int n, int64_t *out) {
 // fl2_shim_session_device_map with the growth and mirror switches of VoxelMapConfig
 int fl2_shim_session_device_map_mirror(void *h, const float *pts, int n, const double *state, double min_eigen_value, int max_points_num, long long root_capacity, int grow,
                                        int mirror) {
-  ShimSession *s = static_cast<ShimSession *>(h);
+  ShimSession *s = session_of(h);
   if (!s) return ESIKF_ERR_ARG;
   s->mgr->config_setting_.device_map_grow_ = grow != 0, s->mgr->config_setting_.device_map_mirror_ = mirror != 0;
   return fl2_shim_session_device_map(h, pts, n, state, min_eigen_value, max_points_num, root_capacity);
 }
 // UpdateVoxelMap(input_points) (include/voxel_map.h:232) with point_w [n][3] and var [n][9]
 int fl2_shim_session_update_points(void *h, const double *pw, const double *var, int n) {
-  ShimSession *s = static_cast<ShimSession *>(h);
+  ShimSession *s = session_of(h);
   if (!s) return ESIKF_ERR_ARG;
   std::vector<pointWithVar> pts(n);
   for (int i = 0; i < n; i++) {
@@ -1576,7 +1512,7 @@ int fl2_shim_session_update_points(void *h, const double *pw, const double *var,
 }
 // mapSliding (src/voxel_map.cpp:924-948) with the sensor at `position`
 int fl2_shim_session_map_sliding(void *h, const double *position, int half_map_size, double sliding_thresh) {
-  ShimSession *s = static_cast<ShimSession *>(h);
+  ShimSession *s = session_of(h);
   if (!s) return ESIKF_ERR_ARG;
   VoxelMapManager &mgr = *s->mgr;
   mgr.config_setting_.half_map_size = half_map_size, mgr.config_setting_.sliding_thresh = sliding_thresh;
@@ -1587,7 +1523,7 @@ int fl2_shim_session_map_sliding(void *h, const double *position, int half_map_s
 // VoxelMapManager::FindCorrespond through a session; the answers in esikf_plane rows (plane_var_'s upper triangle; layer and
 // path are not part of a VoxelPlane and stay 0)
 int fl2_shim_session_find_correspond(void *h, const double *pts, int n, int rule, uint8_t *status, esikf_plane *rows) {
-  ShimSession *s = static_cast<ShimSession *>(h);
+  ShimSession *s = session_of(h);
   if (!s || n < 0) return ESIKF_ERR_ARG;
   std::vector<V3D> p(n);
   for (int i = 0; i < n; i++)
@@ -1596,12 +1532,8 @@ int fl2_shim_session_find_correspond(void *h, const double *pts, int n, int rule
   s->mgr->FindCorrespond(n, p.data(), rule, status, planes.data());
   if (s->mgr->last_status_) return s->mgr->last_status_;
   for (int i = 0; i < n; i++) {
-    esikf_plane &r = rows[i];
-    memset(&r, 0, sizeof(r));
-    for (int k = 0; k < 3; k++) r.center[k] = planes[i].center_[k], r.normal[k] = planes[i].normal_[k];
-    for (int a = 0, t = 0; a < 6; a++)
-      for (int b = a; b < 6; b++, t++) r.plane_var[t] = planes[i].plane_var_[6 * a + b];
-    r.d = planes[i].d_, r.radius = planes[i].radius_;
+    memset(&rows[i], 0, sizeof(rows[i]));
+    row_from_plane(planes[i], rows[i]);
   }
   return 0;
 }
@@ -1610,29 +1542,27 @@ int fl2_shim_session_find_correspond(void *h, const double *pts, int n, int rule
 int fl2_shim_score_ref_patches(int n, const int32_t *first, int m, const double *pos, const double *normal, const float *patch, const float *mean,
                                const int32_t *id, const double *T_f_w, float *score_out, float *mean_out, int32_t *ref_out) {
   if (n < 0 || m < 0 || !first) return ESIKF_ERR_ARG;
-  esikf_ctx *ctx = nullptr;
-  int rc = esikf_create(&ctx, 0);
+  ShimSession s;
+  int rc = s.open();
   if (rc) return rc;
-  {
-    VIOManager vio(ctx);
-    std::vector<int32_t> fi(first, first + n + 1);
-    std::vector<ScoredPoint> pts(n);
-    for (int i = 0; i < n; i++) memcpy(pts[i].pos, pos + 3 * i, sizeof(pts[i].pos)), memcpy(pts[i].normal, normal + 3 * i, sizeof(pts[i].normal));
-    std::vector<PatchObservation> obs(m);
-    for (int j = 0; j < m; j++) {
-      memcpy(obs[j].T_f_w, T_f_w + 12 * (size_t)j, sizeof(obs[j].T_f_w)), memcpy(obs[j].patch, patch + 64 * (size_t)j, sizeof(obs[j].patch));
-      obs[j].mean = mean[j], obs[j].id = id[j];
-    }
-    std::vector<float> sc, mu;
-    std::vector<int32_t> rf;
-    vio.ScoreReferencePatches(fi, pts, obs, sc, mu, rf);
-    rc = vio.last_status_;
-    if (!rc) {
-      memcpy(score_out, sc.data(), sc.size() * sizeof(float)), memcpy(mean_out, mu.data(), mu.size() * sizeof(float));
-      memcpy(ref_out, rf.data(), rf.size() * sizeof(int32_t));
-    }
+  s.open_vio(nullptr, nullptr, nullptr);  // the scoring reads no camera, VIO settings or extrinsics
+  VIOManager &vio = *s.vio;
+  std::vector<int32_t> fi(first, first + n + 1);
+  std::vector<ScoredPoint> pts(n);
+  for (int i = 0; i < n; i++) memcpy(pts[i].pos, pos + 3 * i, sizeof(pts[i].pos)), memcpy(pts[i].normal, normal + 3 * i, sizeof(pts[i].normal));
+  std::vector<PatchObservation> obs(m);
+  for (int j = 0; j < m; j++) {
+    memcpy(obs[j].T_f_w, T_f_w + 12 * (size_t)j, sizeof(obs[j].T_f_w)), memcpy(obs[j].patch, patch + 64 * (size_t)j, sizeof(obs[j].patch));
+    obs[j].mean = mean[j], obs[j].id = id[j];
   }
-  esikf_destroy(ctx);
+  std::vector<float> sc, mu;
+  std::vector<int32_t> rf;
+  vio.ScoreReferencePatches(fi, pts, obs, sc, mu, rf);
+  rc = vio.last_status_;
+  if (!rc) {
+    memcpy(score_out, sc.data(), sc.size() * sizeof(float)), memcpy(mean_out, mu.data(), mu.size() * sizeof(float));
+    memcpy(ref_out, rf.data(), rf.size() * sizeof(int32_t));
+  }
   return rc;
 }
 // GPU: the observation-store overloads of VIOManager on the caller's context (a VIOManager shares it, as LIVMapper's does),
@@ -1691,6 +1621,6 @@ int fl2_shim_vmap_choose(void *ctx, int n, const int32_t *point_id, const double
   if (!vio.last_status_) memcpy(ref_out, ref.data(), ref.size() * sizeof(int32_t));
   return vio.last_status_;
 }
-void *fl2_shim_session_context(void *h) { return static_cast<ShimSession *>(h)->mgr->context(); }
+void *fl2_shim_session_context(void *h) { return session_of(h)->mgr->context(); }
 
 }  // extern "C"

@@ -9,6 +9,7 @@ import numpy as np
 import __graft_entry__
 import map_bind as MB
 import oracle_bind as O
+import shim_bind as SB
 from fast_livo2_b200.synthetic import NODE_DTYPE, PLANE_DTYPE
 
 REF_FIND_SO = os.path.join(O.ORACLE_DIR, "_ref", "libfl2_ref_find.so")
@@ -99,24 +100,11 @@ def flat_of(flat, keys):
     return dict(keys=np.asarray(keys, np.int64).reshape(-1, 3), first=first, count=count, planes=np.concatenate(planes) if planes else np.zeros(0, PLANE_DTYPE))
 
 
-def _shim():
-    lib = C.CDLL(__graft_entry__.SHIM_LIB)
-    lib.fl2_shim_mirror_create.restype = C.c_void_p
-    lib.fl2_shim_mirror_create.argtypes = [C.c_double, C.c_int]
-    lib.fl2_shim_mirror_apply.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
-    lib.fl2_shim_mirror_erase.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.fl2_shim_mirror_dump.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-    lib.fl2_shim_mirror_flatten.argtypes = [C.c_void_p] * 7
-    lib.fl2_shim_mirror_find.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
-    lib.fl2_shim_session_destroy.argtypes = [C.c_void_p]
-    return lib
-
-
 class MirrorView:
     """The shim's mirror behind a handle (a standalone mirror, or a session's voxel_map_): node dump, flatten, find_correspond."""
 
     def __init__(self, h, lib=None):
-        self.lib, self.h = lib or _shim(), h
+        self.lib, self.h = lib or SB.load(), h
 
     def dump_nodes(self):
         return O._dump_nodes(lambda out, cap: self.lib.fl2_shim_mirror_dump(self.h, out.ctypes.data, cap))
@@ -140,7 +128,7 @@ class Mirror(MirrorView):
     """A mirror built on the CPU from exports (ApplyMapExport) and slide bounds (EraseRootsOutside)."""
 
     def __init__(self, cfg):
-        lib = _shim()
+        lib = SB.load()
         super().__init__(lib.fl2_shim_mirror_create(cfg.voxel_size, cfg.max_layer), lib)
 
     def __del__(self):
@@ -218,19 +206,8 @@ def vp(a):
 
 
 def shim_sessions():
-    """The shim library with the session entry points the mirror tests and tools/map_mirror_timing.py call."""
-    lib = _shim()
-    lib.fl2_shim_session_create.restype = C.c_void_p
-    lib.fl2_shim_session_create.argtypes = [C.c_void_p] * 3 + [C.c_int, C.c_void_p, C.c_int] + [C.c_void_p] * 4 + [C.c_int]
-    lib.fl2_shim_session_step.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 7
-    lib.fl2_shim_session_device_map_mirror.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_double, C.c_int, C.c_longlong, C.c_int, C.c_int]
-    lib.fl2_shim_session_update_map.argtypes = [C.c_void_p]
-    lib.fl2_shim_session_point_lists.argtypes = [C.c_void_p, C.c_int]
-    lib.fl2_shim_session_update_points.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
-    lib.fl2_shim_session_map_sliding.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_double]
-    lib.fl2_shim_session_context.restype = C.c_void_p
-    lib.fl2_shim_session_context.argtypes = [C.c_void_p]
-    return lib
+    """The shim library (shim_bind.load()), whose session entry points the mirror tests and tools/map_mirror_timing.py call."""
+    return SB.load()
 
 
 def session(lib, cfg, ext, vmap=None):

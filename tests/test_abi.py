@@ -8,6 +8,7 @@ import re
 import numpy as np
 import pytest
 
+import shim_bind as SB
 from fast_livo2_b200 import api
 from fast_livo2_b200 import synthetic as S
 
@@ -48,11 +49,10 @@ def test_no_cpu_fallback_without_device():
 
 def test_shim_flattener_roundtrip(small_frame):
     """fl2_shim: flat arrays -> pointer octree (VoxelOctoTree mirrors) -> FlattenVoxelMap -> identical candidate lists."""
-    path = os.path.join(ROOT, "fast_livo2_b200", "libfl2_shim.so")
-    if not os.path.exists(path):
+    if not os.path.exists(SB.PATH):
         pytest.skip("shim not built")
     api.load_library()
-    shim = C.CDLL(path)
+    shim = SB.load()
     m = small_frame["map"]
     k, f, c, p = (np.ascontiguousarray(m["keys"]), np.ascontiguousarray(m["first"]), np.ascontiguousarray(m["count"]), np.ascontiguousarray(m["planes"]))
     ko, fo, co, po = np.zeros_like(k), np.zeros_like(f), np.zeros_like(c), np.zeros_like(p)
@@ -74,8 +74,7 @@ def test_shim_flattener_roundtrip(small_frame):
 def test_shim_map_diff_finds_refitted_planes_and_structure_changes(small_frame):
     """fl2_shim DiffFlatVoxelMaps: what VoxelMapManager::SyncDeviceMap uses to choose between esikf_map_patch (same roots and
     candidate lists, some refitted plane records) and a full esikf_map_upload."""
-    path = os.path.join(ROOT, "fast_livo2_b200", "libfl2_shim.so")
-    shim = C.CDLL(path)
+    shim = SB.load()
     m = small_frame["map"]
     k, f, c = (np.ascontiguousarray(m["keys"], dtype=np.int64), np.ascontiguousarray(m["first"], dtype=np.int32), np.ascontiguousarray(m["count"], dtype=np.int32))
     pa = np.ascontiguousarray(m["planes"]).copy()

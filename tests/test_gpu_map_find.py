@@ -2,7 +2,6 @@
 retrieval's ray casting (rule B) on the device-resident voxel map, against the oracle's keyed restatement
 (oracle/orc_find_keyed.cpp) and the device map's own export; the map left untouched by queries; the call's refusals; and the
 shim's VoxelMapManager::FindCorrespond against the host mirror's find_correspond."""
-import ctypes as C
 
 import numpy as np
 import pytest
@@ -219,7 +218,6 @@ def test_find_refusals_write_nothing():
 
 
 def _shim_find(lib, h, q, rule):
-    lib.fl2_shim_session_find_correspond.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     q = np.ascontiguousarray(q, np.float64)
     st, rows = np.zeros(len(q), np.uint8), np.zeros(len(q), PLANE_DTYPE)
     assert lib.fl2_shim_session_find_correspond(h, q.ctypes.data, len(q), rule, st.ctypes.data, rows.ctypes.data) == 0

@@ -3,17 +3,15 @@ oracle's restatement (oracle/orc_refpatch.cpp) bit for bit: on the hand-built ca
 realistic observation sets (the visual points of a keyframe_cases frame, each observed in 6 to 30 keyframe images through
 image_patch_kernel with those keyframes' poses), with cached means the patches do not have, twice in a row, through the
 shim's VIOManager::ScoreReferencePatches, and on the refusals, which write nothing."""
-import ctypes as C
-import os
 
 import numpy as np
 import pytest
 
 import refpatch_cases as RC
+import shim_bind as SB
 from fast_livo2_b200 import api
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ERR_ARG = -3  # ESIKF_ERR_ARG
 
 
@@ -128,10 +126,7 @@ def test_refusals_write_nothing_and_empty_calls_succeed(ctx):
 
 
 def test_shim_score_reference_patches_is_the_c_abi(ctx):
-    shim = C.CDLL(os.path.join(ROOT, "fast_livo2_b200", "libfl2_shim.so"))
-    vp = C.c_void_p
-    shim.fl2_shim_score_ref_patches.argtypes = [C.c_int, vp, C.c_int] + [vp] * 9
-    shim.fl2_shim_score_ref_patches.restype = C.c_int
+    shim = SB.load()
     for c in (RC.pin_case(), RC.realistic_case(ctx, 2000, seed=5)):
         n, m = len(c["first"]) - 1, len(c["patch"])
         out = dict(score=np.zeros(m, np.float32), mean=np.zeros(m, np.float32), ref=np.zeros(n, np.int32))

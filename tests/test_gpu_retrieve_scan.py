@@ -7,18 +7,17 @@ depth-check flags are the oracle's bit for bit. Fisheye (config 3's camera and e
 CUDA's and glibc's may differ in the last ulp, so a point whose int(px) straddles an integer can land one pixel over; the
 differing pixels are counted and printed, and each must come from such a point."""
 import ctypes as C
-import os
 
 import numpy as np
 import pytest
 
 import oracle_bind as O
 import retrieve_cases as RC
+import shim_bind as SB
 from fast_livo2_b200 import api
 from fast_livo2_b200 import synthetic as S
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _setup(ctx, sc):
@@ -248,9 +247,8 @@ def test_errors():
 
 def test_shim_gives_the_c_abi_results(gpu_ctx):
     """VIOManager::RetrieveScanVoxels / CheckDepthContinuity (fl2_shim) against the C ABI on the same scan and points."""
-    path = os.path.join(ROOT, "fast_livo2_b200", "libfl2_shim.so")
     api.load_library()
-    shim = C.CDLL(path)
+    shim = SB.load()
     sc = RC.scene("radtan", 50_000, seed=12)
     _setup(gpu_ctx, sc)
     want = gpu_ctx.vio_retrieve_scan(sc["border"], pg=sc["pg"], state=sc["state"])

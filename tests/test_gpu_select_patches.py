@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 import select_cases as SC
+import shim_bind as SB
 from fast_livo2_b200 import api
 from fast_livo2_b200 import synthetic as S
 from harness import VIO_KEYS, bits_equal, variant
@@ -171,7 +172,7 @@ def test_shim_select_then_update_equals_host_sub_map(gpu_ctx, normal_en):
     kept, e_sel, e_host = np.zeros(n, np.int32), np.zeros(n, np.float32), np.zeros(n, np.float32)
     s_sel, s_host, wp, counts = np.zeros(386), np.zeros(386), np.zeros((n, 256), np.float32), np.zeros(4, np.int64)
     img, T_cur = np.ascontiguousarray(c["img"]), np.ascontiguousarray(c["T_cur"])
-    shim = C.CDLL(os.path.join(SC.ROOT, "fast_livo2_b200", "libfl2_shim.so"))
+    shim = SB.load()
     vp = lambda a: a.ctypes.data_as(C.c_void_p)
     rc = shim.fl2_shim_select_run(C.byref(cc), C.byref(vc), C.byref(ec), vp(img), C.cast(arr, C.c_void_p), len(imgs), vp(cand), n, vp(T_cur), vp(prior),
                                   vp(gate), C.byref(nk), vp(kept), vp(s_sel), vp(e_sel), vp(s_host), vp(e_host), vp(wp), vp(counts))

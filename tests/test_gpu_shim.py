@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 import oracle_bind as O
+import shim_bind as SB
 from fast_livo2_b200 import api
 from fast_livo2_b200 import synthetic as S
 from parity_util import assert_state_close
@@ -17,7 +18,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 def test_shim_lio_and_vio_match_oracle(gpu_ctx, small_vio_frame):
     fr = small_vio_frame
-    shim = C.CDLL(os.path.join(ROOT, "fast_livo2_b200", "libfl2_shim.so"))
+    shim = SB.load()
     m = fr["map"]
     k, f, c, p = (np.ascontiguousarray(m["keys"]), np.ascontiguousarray(m["first"]), np.ascontiguousarray(m["count"]), np.ascontiguousarray(m["planes"]))
     lcfg = api.lio_cfg_c(fr["lio_cfg"])
@@ -66,15 +67,7 @@ def test_shim_session_with_device_resident_map_equals_the_c_abi_tick_loop(small_
     pv_list_ / ptpl_list_ materialise from device data (no host VoxelPlane exists in this mode)."""
     fr = small_vio_frame
     cfg, ext = fr["lio_cfg"], fr["ext"]
-    shim = C.CDLL(os.path.join(ROOT, "fast_livo2_b200", "libfl2_shim.so"))
-    shim.fl2_shim_session_create.restype = C.c_void_p
-    shim.fl2_shim_session_create.argtypes = [C.c_void_p] * 3 + [C.c_int, C.c_void_p, C.c_int] + [C.c_void_p] * 4 + [C.c_int]
-    shim.fl2_shim_session_step.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 7
-    shim.fl2_shim_session_device_map.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_double, C.c_int, C.c_longlong]
-    shim.fl2_shim_session_update_map.argtypes = [C.c_void_p]
-    shim.fl2_shim_session_point_lists.argtypes = [C.c_void_p, C.c_int]
-    shim.fl2_shim_session_materialize.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-    shim.fl2_shim_session_destroy.argtypes = [C.c_void_p]
+    shim = SB.load()
     m = fr["map"]
     k, f, c, p = (np.ascontiguousarray(m["keys"]), np.ascontiguousarray(m["first"]), np.ascontiguousarray(m["count"]), np.ascontiguousarray(m["planes"]))
     lcfg = api.lio_cfg_c(cfg)

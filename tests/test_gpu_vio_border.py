@@ -7,12 +7,12 @@ warp_affine_kernel's in-frame test. Every test below places patches there (tests
 footprints actually leave the image, so the border cases cannot silently disappear."""
 import ctypes as C
 import dataclasses
-import os
 
 import numpy as np
 import pytest
 
 import oracle_bind as O
+import shim_bind as SB
 import vio_border as VB
 from conftest import get_frame
 from fast_livo2_b200 import api
@@ -21,7 +21,6 @@ from harness import VIO_KEYS, bits_equal, compare_vio, sm_count, sweep, vio_prio
 from ref_pin_cases import BORDER_FRAME, warp_affine_border_cases
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 FISHEYE = dict(seed=9, n_pts=1000, n_map=100_000, n_patches=100, scene_scale=0.5, vio=S.VioCfg(img_point_cov=1000.0), ext=S.hilti_extrinsics(),
                cam=S.CamCfg(model=1, width=720, height=540, fx=351.31400364193297, fy=351.4911744656785, cx=367.8522793375995, cy=253.8402144980996,
                             d=(-0.03696737352869157, -0.008917880497032812, 0.008912969593422046, -0.0037685977496087313, 0.0)))
@@ -68,7 +67,7 @@ def test_shim_image_patch_and_warp_at_a_border_pixel(border):
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")
     fr, _, _ = border
-    shim = C.CDLL(os.path.join(ROOT, "fast_livo2_b200", "libfl2_shim.so"))
+    shim = SB.load()
     cc, L = fr["cam_cfg"], fr["vio_cfg"].levels
     cam = api.CameraC(cc.model, cc.width, cc.height, 0, cc.fx, cc.fy, cc.cx, cc.cy)
     cam.d[:] = list(cc.d)

@@ -4,6 +4,7 @@ against the packed entry points (esikf_vio_score_ref_patches, esikf_vio_update_p
 import numpy as np
 import pytest
 
+import shim_bind as SB
 import vmap_cases as VC
 from fast_livo2_b200 import api
 from fast_livo2_b200 import synthetic as S
@@ -226,15 +227,8 @@ def test_shim_overloads_equal_the_c_abi(gpu_ctx):
     """VIOManager::EnableDeviceObservations / AddVisualPoints / UpdateVisualMapPoints / ScoreReferencePatches /
     ChooseReferenceFeatures on one context equal esikf_vmap_* on another over 12 ticks: every output and every list."""
     import ctypes as C
-    import os
 
-    vp = C.c_void_p
-    shim = C.CDLL(os.path.join(os.path.dirname(api.__file__), "libfl2_shim.so"))
-    shim.fl2_shim_vmap_enable.argtypes = [vp, C.c_int64]
-    shim.fl2_shim_vmap_add.argtypes = [vp, C.c_int] + [vp] * 9
-    shim.fl2_shim_vmap_update.argtypes = [vp, vp, C.c_int, vp, vp, C.c_int32] + [vp] * 7
-    shim.fl2_shim_vmap_score.argtypes = [vp, C.c_int] + [vp] * 4
-    shim.fl2_shim_vmap_choose.argtypes = [vp, C.c_int, vp, vp, vp, C.c_int, vp]
+    shim = SB.load()
     cam, ext, ticks = VC.sequence(ticks=12)
     other = api.Context(0)
     try:

@@ -2,19 +2,18 @@
 VIO update over 6 to 8 pyramid levels with 8 iterations each."""
 import ctypes as C
 import dataclasses
-import os
 
 import numpy as np
 import pytest
 
 import oracle_bind as O
+import shim_bind as SB
 import warp_cases as W
 from fast_livo2_b200 import api
 from fast_livo2_b200 import synthetic as S
 from harness import VIO_KEYS, bits_equal, compare_vio, sweep, variant, vio_setup
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _ref_image(cam, seed=0):
@@ -102,7 +101,7 @@ def test_warp_affine_on_cancelling_matrices(gpu_ctx):
     A, px, sl, img = W.caller_matrices()
     n = len(A)
     cam = dataclasses.replace(W.CAMERAS["pinhole"], width=img.shape[1], height=img.shape[0])
-    shim = C.CDLL(os.path.join(ROOT, "fast_livo2_b200", "libfl2_shim.so"))
+    shim = SB.load()
     vp = lambda a: a.ctypes.data_as(C.c_void_p)
     cc = api.CameraC(cam.model, cam.width, cam.height, 0, cam.fx, cam.fy, cam.cx, cam.cy)
     cc.d[:] = list(cam.d)

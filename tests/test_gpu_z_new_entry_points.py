@@ -1,17 +1,16 @@
 """GPU: entry points added (or first tested) at the end of round 1 — esikf_vio_warp_affine, the shim's per-patch
 getImagePatch / warpAffine mirrors, esikf_map_patch and the shim's incremental map refresh."""
 import ctypes as C
-import os
 
 import numpy as np
 import pytest
 
 import oracle_bind as O
+import shim_bind as SB
 from fast_livo2_b200 import api
 from harness import compare_lio, lio_gpu, lio_oracle, vio_prior, vio_setup, vio_warp
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def test_warp_affine_alone_with_caller_matrices(gpu_ctx, small_vio_frame):
@@ -50,7 +49,7 @@ def test_shim_patch_helpers_match_oracle(small_vio_frame):
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")
     fr = small_vio_frame
-    shim = C.CDLL(os.path.join(ROOT, "fast_livo2_b200", "libfl2_shim.so"))
+    shim = SB.load()
     L = fr["vio_cfg"].levels
     cam = api.CameraC(fr["cam_cfg"].model, fr["cam_cfg"].width, fr["cam_cfg"].height, 0, fr["cam_cfg"].fx, fr["cam_cfg"].fy, fr["cam_cfg"].cx, fr["cam_cfg"].cy)
     cam.d[:] = list(fr["cam_cfg"].d)
@@ -123,7 +122,7 @@ def test_shim_incremental_map_sync_equals_fresh_upload(small_frame):
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")
     fr = small_frame
-    shim = C.CDLL(os.path.join(ROOT, "fast_livo2_b200", "libfl2_shim.so"))
+    shim = SB.load()
     m = fr["map"]
     k, f, c = (np.ascontiguousarray(m["keys"], dtype=np.int64), np.ascontiguousarray(m["first"], dtype=np.int32), np.ascontiguousarray(m["count"], dtype=np.int32))
     pa = np.ascontiguousarray(m["planes"])
