@@ -138,6 +138,7 @@ def load_library():
     lib.esikf_set_kernel_timing.argtypes = [vp, C.c_int32]
     lib.esikf_set_phase_stamps.argtypes = [vp, C.c_int32]
     lib.esikf_get_phase_stamps.argtypes = [vp, C.POINTER(C.c_uint64)]
+    lib.esikf_get_vio_chain_stamps.argtypes = [vp, C.POINTER(C.c_uint64)]
     lib.esikf_get_kernel_timing.argtypes = [vp, fp, fp, fp, fp]
     _lib = lib
     return lib
@@ -150,6 +151,10 @@ FIND_RULE_PATCH, FIND_RULE_RAYCAST = 0, 1  # esikf_map_device_find: updateRefere
 FIND_NO_ROOT, FIND_NODE, FIND_PLANE = 0, 1, 2  # esikf_map_device_find's status per point
 # esikf_vmap_retrieve's status per cell: kept, depth-discontinuous, not normal-initialised, no reference feature, no winner
 RETRIEVE_KEPT, RETRIEVE_DEPTH, RETRIEVE_NOT_INIT, RETRIEVE_NO_REF, RETRIEVE_NO_WINNER = 0, 1, 2, 3, 4
+# esikf_get_vio_chain_stamps (csrc/esikf_fused.cu): 8 words per (level, iteration) slot, then from VIO_CHAIN_CTA on
+# VIO_CHAIN_MAX_CTAS words per slot, one per CTA
+VIO_CHAIN_CTA, VIO_CHAIN_MAX_CTAS = 8 * 64, 160
+VIO_CHAIN_STAMP_WORDS = VIO_CHAIN_CTA + VIO_CHAIN_MAX_CTAS * 64  # ESIKF_VIO_CHAIN_STAMP_WORDS
 DEFAULT_LOOP_MODE = 2  # esikf_set_loop_mode: 2 (alias 1) persistent kernel per update, 0 per-iteration launches
 
 class MapCfgC(C.Structure):
@@ -170,6 +175,7 @@ EXPORTED_SYMBOLS = [
     "esikf_vio_run", "esikf_vio_fetch", "esikf_vio_update", "esikf_vio_get_image_patch", "esikf_vio_set_ref_images",
     "esikf_vio_warp_patches", "esikf_vio_select_patches", "esikf_vio_warp_affine", "esikf_vio_set_inverse_refs", "esikf_rgb_set_cloud", "esikf_rgb_colorize", "esikf_vio_generate_points", "esikf_vio_update_points", "esikf_vio_retrieve_scan", "esikf_vio_depth_check", "esikf_vio_score_ref_patches",
     "esikf_vmap_init", "esikf_vmap_add_points", "esikf_vmap_update_points", "esikf_vmap_score", "esikf_vmap_choose_ref", "esikf_vmap_download", "esikf_vmap_stats", "esikf_vmap_place_points", "esikf_vmap_retrieve", "esikf_comm_unique_id", "esikf_comm_init", "esikf_comm_rank", "esikf_shard_range", "esikf_peer_export", "esikf_peer_attach", "esikf_profile_kernel", "esikf_set_kernel_timing", "esikf_get_kernel_timing", "esikf_set_phase_stamps", "esikf_get_phase_stamps",
+    "esikf_get_vio_chain_stamps",
 ]
 
 
@@ -796,6 +802,13 @@ class Context:
         self.debug_stamps = out[576:640].copy()
         self.cta_stamps = out[640:].copy()
         return out[:576].reshape(72, 8)
+
+    def get_vio_chain_stamps(self):
+        """The VIO kernel's chain stamps (esikf_get_vio_chain_stamps): written only by a library built with
+        -DESIKF_VIO_CHAIN_STAMPS, by a persistent update run while phase stamps are on."""
+        out = np.zeros(VIO_CHAIN_STAMP_WORDS, np.uint64)
+        self._ck(self.lib.esikf_get_vio_chain_stamps(self.h, out.ctypes.data_as(C.POINTER(C.c_uint64))))
+        return out
 
     def set_kernel_timing(self, enable):
         self._ck(self.lib.esikf_set_kernel_timing(self.h, int(enable)))

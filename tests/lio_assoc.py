@@ -742,6 +742,22 @@ def case(name):
     return _cases[name]
 
 
+SMEM_LANES, LANES = 704, 768  # lanes per CTA of the LIO kernels in shared-memory slots / in all (csrc/esikf_lio.cu)
+
+
+def l2_lane_layout(fr, G, start):
+    """A scan of G * 768 points (every CTA exactly 24 chunks of 32) built from the case's designed warps: CTA b runs the
+    case's warps start + 2b and start + 2b + 1 in its L2-slot warps and the 22 warps after them in its shared-slot warps."""
+    pts, tags = fr["pts"], np.asarray(fr["tags"])
+    W = len(pts) // 32
+    order = []
+    for b in range(G):
+        ws = [(start + 2 * b + 2 + j) % W for j in range(SMEM_LANES // 32)] + [(start + 2 * b) % W, (start + 2 * b + 1) % W]
+        order += [np.arange(32 * w, 32 * w + 32) for w in ws]
+    order = np.concatenate(order)
+    return dict(fr, pts=np.ascontiguousarray(pts[order]), tags=tags[order])
+
+
 def tiled(fr, n):
     """The case's scan repeated warp by warp to n points (the designed warps keep their lanes)."""
     pts = fr["pts"]

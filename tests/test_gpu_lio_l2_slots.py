@@ -8,12 +8,12 @@ import numpy as np
 import pytest
 
 import lio_assoc as A
+from lio_assoc import LANES, SMEM_LANES
 from fast_livo2_b200 import api
 from harness import LIO_KEYS, bits_equal, compare_lio, lio_gpu, lio_oracle, sm_count, sweep
 
 pytestmark = pytest.mark.gpu
 
-SMEM_LANES, LANES = 704, 768  # lanes per CTA in shared-memory slots / in all
 VARIANTS = [dict(loop_mode=2), dict(loop_mode=0), dict(loop_mode=2, tuning=api.TUNE_STAGE_LDG), dict(loop_mode=0, tuning=api.TUNE_STAGE_LDG)]
 
 
@@ -41,19 +41,6 @@ def test_slices_at_the_768_lane_boundaries(gpu_ctx, name):
         check_all_variants(gpu_ctx, A.tiled(fr, n))
 
 
-def l2_lane_layout(fr, G, start):
-    """A scan of G * 768 points (every CTA exactly 24 chunks of 32) built from the case's designed warps: CTA b runs the
-    case's warps start + 2b and start + 2b + 1 in its L2-slot warps and the 22 warps after them in its shared-slot warps."""
-    pts, tags = fr["pts"], np.asarray(fr["tags"])
-    W = len(pts) // 32
-    order = []
-    for b in range(G):
-        ws = [(start + 2 * b + 2 + j) % W for j in range(SMEM_LANES // 32)] + [(start + 2 * b) % W, (start + 2 * b + 1) % W]
-        order += [np.arange(32 * w, 32 * w + 32) for w in ws]
-    order = np.concatenate(order)
-    return dict(fr, pts=np.ascontiguousarray(pts[order]), tags=tags[order])
-
-
 @pytest.mark.parametrize("name", A.CASES)
 def test_designed_warps_in_l2_slot_lanes(gpu_ctx, name):
     """Every designed warp of the case, in turn, in lanes 704-767 of some CTA: the association of those lanes against the
@@ -63,7 +50,7 @@ def test_designed_warps_in_l2_slot_lanes(gpu_ctx, name):
     W = len(fr["pts"]) // 32
     matched_l2 = 0
     for start in range(0, W, 2 * G):
-        f = l2_lane_layout(fr, G, start)
+        f = A.l2_lane_layout(fr, G, start)
         g, o = check_all_variants(gpu_ctx, f)
         in_l2 = (np.arange(len(f["pts"])) % LANES) >= SMEM_LANES
         assert np.array_equal(g["match_plane"][in_l2], o["match_plane"][in_l2])
