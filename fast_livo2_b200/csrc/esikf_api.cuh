@@ -131,7 +131,8 @@ struct MapArenaBufs {
   uint32_t hash_cap = 0;
   int node_cap = 0, rec_cap = 0;
   long long pool_cap = 0;  // points
-  cudaError_t reserve(uint32_t hash_cap_, int node_cap_, int rec_cap_, long long pool_cap_) {
+  // hidden: where the compiler does not inline it, the copy it emits stays out of the library's export table
+  ESIKF_HIDDEN cudaError_t reserve(uint32_t hash_cap_, int node_cap_, int rec_cap_, long long pool_cap_) {
     cudaError_t e;
     if ((e = slots.reserve(hash_cap_)) || (e = slot_root.reserve(hash_cap_)) || (e = slot_cap.reserve(hash_cap_)) || (e = nodes.reserve((size_t)node_cap_)) ||
         (e = pool.reserve((size_t)pool_cap_ * MAP_PT_D)) || (e = recs.reserve((size_t)rec_cap_)) || (e = planes.reserve((size_t)rec_cap_)) ||
@@ -334,6 +335,20 @@ ESIKF_HIDDEN int fail(esikf_ctx *c, int code, const char *fmt, ...);
     cudaError_t e__ = (call);                                                                                      \
     if (e__ != cudaSuccess) return fail(ctx, ESIKF_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e__), __FILE__, __LINE__); \
   } while (0)
+
+// The one launch path of the entry points' kernels: `kernel` on the context's stream, its launch error returned, and one
+// launch added to esikf_launch_count once it is enqueued. Only launch_persistent's cooperative launch goes another way.
+// cudaGetLastError() also returns an error an earlier runtime call left, so every runtime call on an entry point's path is
+// checked (CK) or has its error cleared where it is handled: the error returned here is this launch's.
+template <typename... P, typename... A>
+static cudaError_t launch(esikf_ctx *ctx, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, A &&...args) {
+  kernel<<<grid, block, smem, ctx->stream>>>(std::forward<A>(args)...);
+  const cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) ctx->launches++;
+  return e;
+}
+// A CUB device-wide call: whatever number of kernels it runs, it counts as one launch.
+static inline cudaError_t counted(esikf_ctx *ctx, cudaError_t e) { return e == cudaSuccess ? (ctx->launches++, e) : e; }
 
 // The inputs of the context's groups (esikf_ctx), one bit each.
 enum Input : unsigned {

@@ -34,9 +34,7 @@ int esikf_rgb_set_cloud(esikf_ctx *ctx, const float *pts_xyz, int32_t n, const d
     RgbWorldArgs a;
     a.body = pts_xyz ? ctx->rgb_cloud.p : ctx->pts.p, a.world = ctx->rgb_cloud.p, a.n = n, a.state = dev_state;
     memcpy(a.extR, ctx->ext.extR, sizeof(a.extR)), memcpy(a.extT, ctx->ext.extT, sizeof(a.extT));
-    rgb_world_kernel<<<(n + 255) / 256, 256, 0, st>>>(a);
-    ctx->launches++;
-    CK(cudaGetLastError());
+    CK(launch(ctx, rgb_world_kernel, (n + 255) / 256, 256, 0, a));
   }
   ctx->rgb_n = n;
   return ESIKF_OK;
@@ -56,7 +54,7 @@ int esikf_rgb_colorize(esikf_ctx *ctx, const uint8_t *bgr, int32_t width, int32_
   const size_t N = (size_t)n, img_bytes = (size_t)width * height * 3;
   // device-wide scan: select_scan_kernel's single CTA took 90 % of the pass at 300 k points (DESIGN.md §8)
   size_t tmp_bytes = 0;
-  if (n > 0) cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, (int32_t *)nullptr, (int32_t *)nullptr, n + 1, st);
+  if (n > 0) CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, (int32_t *)nullptr, (int32_t *)nullptr, n + 1, st));
   uint8_t *img, *color, *bgr_kept, *tmp;
   int32_t *keep, *dst, *index;
   float *xyz;
@@ -74,11 +72,9 @@ int esikf_rgb_colorize(esikf_ctx *ctx, const uint8_t *bgr, int32_t width, int32_
     a.cloud = ctx->rgb_cloud.p, a.n = n, a.bgr = img, a.state = dev_state, a.blind = blind_rgb_points;
     frame_consts(ctx, a.cam, a.Rci, a.Pci);
     a.keep = keep, a.color = color;
-    rgb_color_kernel<<<(n + 1 + 255) / 256, 256, 0, st>>>(a);
-    CK(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, keep, dst, n + 1, st));
-    rgb_scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(keep, dst, n, ctx->rgb_cloud.p, color, xyz, bgr_kept, index);
-    ctx->launches += 4;
-    CK(cudaGetLastError());
+    CK(launch(ctx, rgb_color_kernel, (n + 1 + 255) / 256, 256, 0, a));
+    CK(counted(ctx, cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, keep, dst, n + 1, st)));
+    CK(launch(ctx, rgb_scatter_kernel, (n + 255) / 256, 256, 0, keep, dst, n, ctx->rgb_cloud.p, color, xyz, bgr_kept, index));
     CK(read_back_to(ctx, dst + n, &kept));
   }
   *n_out = kept;
@@ -151,12 +147,10 @@ int esikf_vio_generate_points(esikf_ctx *ctx, const double *point_w, const doubl
   CK(cudaMemcpyAsync(mask, type_map, L, cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(a.key, 0, C * sizeof(unsigned long long), st));
   a.type_map = mask;
-  gen_score_kernel<<<(n + n_add + GEN_THREADS - 1) / GEN_THREADS, GEN_THREADS, 0, st>>>(a);
-  gen_cells_kernel<<<(L + 255) / 256, 256, 0, st>>>(a.key, L, d_keep);
-  select_scan_kernel<<<1, SELECT_SCAN_THREADS, 0, st>>>(d_keep, L, d_dst, d_nk);
-  gen_scatter_kernel<<<(L + GEN_THREADS - 1) / GEN_THREADS, GEN_THREADS, 0, st>>>(a, d_keep, d_dst, o);
-  ctx->launches += 4;
-  CK(cudaGetLastError());
+  CK(launch(ctx, gen_score_kernel, (n + n_add + GEN_THREADS - 1) / GEN_THREADS, GEN_THREADS, 0, a));
+  CK(launch(ctx, gen_cells_kernel, (L + 255) / 256, 256, 0, a.key, L, d_keep));
+  CK(launch(ctx, select_scan_kernel, 1, SELECT_SCAN_THREADS, 0, d_keep, L, d_dst, d_nk));
+  CK(launch(ctx, gen_scatter_kernel, (L + GEN_THREADS - 1) / GEN_THREADS, GEN_THREADS, 0, a, d_keep, d_dst, o));
   int32_t nk = 0;
   CK(cudaMemcpyAsync(&nk, d_nk, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));  // also: the caller may reuse its buffers on return
@@ -164,9 +158,7 @@ int esikf_vio_generate_points(esikf_ctx *ctx, const double *point_w, const doubl
   if (nk > cap) return fail(ctx, ESIKF_ERR_ARG, "vio_generate_points: %d new points, room for %d", nk, cap);
   if (nk == 0) return ESIKF_OK;
   if (patch_out) {
-    image_patch_kernel<<<(nk * 64 + 255) / 256, 256, 0, st>>>(ctx->img.p, ctx->img_w, ctx->img_h, o.pc, nk, 0, d_patch);
-    ctx->launches++;
-    CK(cudaGetLastError());
+    CK(launch(ctx, image_patch_kernel, (nk * 64 + 255) / 256, 256, 0, ctx->img.p, ctx->img_w, ctx->img_h, o.pc, nk, 0, d_patch));
     CK(cudaMemcpyAsync(patch_out, d_patch, (size_t)nk * 64 * sizeof(float), cudaMemcpyDeviceToHost, st));
   }
   const size_t K = (size_t)nk;
@@ -212,7 +204,6 @@ int esikf_vio_update_points(esikf_ctx *ctx, int32_t n, const uint8_t *converged,
   static const double cos_max = acos_03_bound();
   *n_out = 0;
   if (n == 0) return ESIKF_OK;  // total_points == 0 (:910)
-  cudaStream_t st = ctx->stream;
   const size_t N = (size_t)n;
   ObsArgs a;
   double *last_T, *last_px_d, *out_pc;
@@ -230,21 +221,15 @@ int esikf_vio_update_points(esikf_ctx *ctx, int32_t n, const uint8_t *converged,
   frame_consts(ctx, a.cam, a.Rci, a.Pci);
   a.state = dev_state, a.pos = ctx->vis_pos.p, a.converged = conv, a.last_T = last_T, a.last_px = last_px_d;
   a.n = n, a.cos_max = cos_max, a.keep = d_keep;
-  obs_flag_kernel<<<(n + OBS_THREADS - 1) / OBS_THREADS, OBS_THREADS, 0, st>>>(a);
-  select_scan_kernel<<<1, SELECT_SCAN_THREADS, 0, st>>>(d_keep, n, d_dst, d_nk);
-  obs_scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_keep, d_dst, a.pc, n, d_entry, out_pc);
-  ctx->launches += 3;
-  CK(cudaGetLastError());
+  CK(launch(ctx, obs_flag_kernel, (n + OBS_THREADS - 1) / OBS_THREADS, OBS_THREADS, 0, a));
+  CK(launch(ctx, select_scan_kernel, 1, SELECT_SCAN_THREADS, 0, d_keep, n, d_dst, d_nk));
+  CK(launch(ctx, obs_scatter_kernel, (n + 255) / 256, 256, 0, d_keep, d_dst, a.pc, n, d_entry, out_pc));
   int32_t nk;
   CK(read_back_to(ctx, d_nk, &nk));
   *n_out = nk;
   if (nk > cap) return fail(ctx, ESIKF_ERR_ARG, "vio_update_points: %d new observations, room for %d", nk, cap);
   const size_t K = (size_t)nk;
-  if (nk > 0 && patch_out) {
-    image_patch_kernel<<<(nk * 64 + 255) / 256, 256, 0, st>>>(ctx->img.p, ctx->img_w, ctx->img_h, out_pc, nk, 0, patch);
-    ctx->launches++;
-    CK(cudaGetLastError());
-  }
+  if (nk > 0 && patch_out) CK(launch(ctx, image_patch_kernel, (nk * 64 + 255) / 256, 256, 0, ctx->img.p, ctx->img_w, ctx->img_h, out_pc, nk, 0, patch));
   const void *f0 = a.flag;
   CK(read_back(ctx, f0, patch_out ? (const void *)(patch + 64 * K) : (const void *)(out_pc + 2 * K)));
   if (update_flag_out) copy_out(ctx, update_flag_out, f0, a.flag, N);
@@ -268,8 +253,9 @@ int esikf_vio_retrieve_scan(esikf_ctx *ctx, const double *point_w, int32_t n, in
   const int W = ctx->cam.width, H = ctx->cam.height;
   const size_t N = (size_t)n, npix = (size_t)W * H;
   size_t sort_bytes = 0, scan_bytes = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (unsigned long long *)nullptr, (unsigned long long *)nullptr, (uint32_t *)nullptr, (uint32_t *)nullptr, n, 0, 63, st);
-  cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (int32_t *)nullptr, (int32_t *)nullptr, n + 1, st);
+  CK(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (unsigned long long *)nullptr, (unsigned long long *)nullptr, (uint32_t *)nullptr, (uint32_t *)nullptr, n, 0, 63,
+                                     st));
+  CK(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (int32_t *)nullptr, (int32_t *)nullptr, n + 1, st));
   double *pt = nullptr;
   unsigned long long *k_out;
   uint32_t *i_out;
@@ -300,18 +286,15 @@ int esikf_vio_retrieve_scan(esikf_ctx *ctx, const double *point_w, int32_t n, in
   } else {
     a.pt = ctx->map_pt.p, a.pt_stride = MAP_PT_D;
   }
-  if (n > 0) ret_scan_kernel<<<(n + RET_THREADS - 1) / RET_THREADS, RET_THREADS, 0, st>>>(a);
-  ret_depth_kernel<<<(int)((npix + 255) / 256), 256, 0, st>>>(a.win, a.depth_pt, (int)npix, ctx->ret_depth.p);
-  ctx->launches += n > 0 ? 2 : 1;
+  if (n > 0) CK(launch(ctx, ret_scan_kernel, (n + RET_THREADS - 1) / RET_THREADS, RET_THREADS, 0, a));
+  CK(launch(ctx, ret_depth_kernel, (int)((npix + 255) / 256), 256, 0, a.win, a.depth_pt, (int)npix, ctx->ret_depth.p));
   int32_t counts[2] = {0, 0};  // distinct keys, bad
   if (n > 0) {
-    CK(cub::DeviceRadixSort::SortPairs(tmp, sort_bytes, a.key, k_out, a.idx, i_out, n, 0, 63, st));
-    ret_head_kernel<<<(n + 1 + 255) / 256, 256, 0, st>>>(k_out, i_out, n, d_head);
-    CK(cub::DeviceScan::ExclusiveSum(tmp, scan_bytes, d_head, d_dst, n + 1, st));
-    ret_keys_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_head, d_dst, a.key, n, d_keys);
-    ctx->launches += 4;  // sort passes counted as one
+    CK(counted(ctx, cub::DeviceRadixSort::SortPairs(tmp, sort_bytes, a.key, k_out, a.idx, i_out, n, 0, 63, st)));
+    CK(launch(ctx, ret_head_kernel, (n + 1 + 255) / 256, 256, 0, k_out, i_out, n, d_head));
+    CK(counted(ctx, cub::DeviceScan::ExclusiveSum(tmp, scan_bytes, d_head, d_dst, n + 1, st)));
+    CK(launch(ctx, ret_keys_kernel, (n + 255) / 256, 256, 0, d_head, d_dst, a.key, n, d_keys));
   }
-  CK(cudaGetLastError());
   CK(read_back(ctx, d_dst + n, a.bad + 1));  // also: the caller may reuse its buffers on return
   if (n > 0) copy_out(ctx, &counts[0], d_dst + n, d_dst + n, sizeof(int32_t)), copy_out(ctx, &counts[1], d_dst + n, a.bad, sizeof(int32_t));
   if (counts[1]) return fail(ctx, ESIKF_ERR_ARG, "vio_retrieve_scan: a voxel key leaves [-2^20, 2^20)");
@@ -332,7 +315,6 @@ int esikf_vio_depth_check(esikf_ctx *ctx, int32_t n, const double *pos_w, const 
   if (int rc = need(ctx, "vio_depth_check", IN_RETRIEVAL)) return rc;
   if (n == 0) return ESIKF_OK;
   CK(cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
   const size_t N = (size_t)n;
   double *pos, *pc_d;
   uint8_t *flag;
@@ -343,9 +325,7 @@ int esikf_vio_depth_check(esikf_ctx *ctx, int32_t n, const double *pos_w, const 
   memcpy(a.Rci, ctx->ret_Rci, sizeof(a.Rci)), memcpy(a.Pci, ctx->ret_Pci, sizeof(a.Pci));
   a.state = ctx->ret_state.p, a.pos = pos, a.pc = pc_d, a.n = n, a.width = ctx->ret_w, a.height = ctx->ret_h;
   a.depth = ctx->ret_depth.p, a.flag = flag;
-  ret_depth_check_kernel<<<(n + RET_THREADS - 1) / RET_THREADS, RET_THREADS, 0, st>>>(a);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, ret_depth_check_kernel, (n + RET_THREADS - 1) / RET_THREADS, RET_THREADS, 0, a));
   CK(read_back_to(ctx, flag, discontinuous_out, N));
   return ESIKF_OK;
 }
@@ -384,9 +364,7 @@ int esikf_vio_score_ref_patches(esikf_ctx *ctx, int32_t n, const int32_t *first,
     CK(cudaMemcpyAsync(d_id, id, M * sizeof(int32_t), cudaMemcpyHostToDevice, st));
   }
   a.pos = d_pos, a.normal = d_normal, a.T = d_T, a.patch = d_patch, a.mean = d_mean, a.id = d_id;
-  refpatch_score_kernel<<<(n + RP_WARPS - 1) / RP_WARPS, RP_WARPS * 32, 0, st>>>(a, RpPacked{d_first});
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, refpatch_score_kernel<RpPacked>, (n + RP_WARPS - 1) / RP_WARPS, RP_WARPS * 32, 0, a, RpPacked{d_first}));
   CK(read_back(ctx, a.score, a.ref + N));
   copy_out(ctx, score_out, a.score, a.score, 4 * M);
   copy_out(ctx, mean_out, a.score, a.mean_out, 4 * M);
@@ -500,9 +478,7 @@ int esikf_vmap_add_points(esikf_ctx *ctx, int32_t n, const int32_t *first, int32
                   {a.mean, mean, M * sizeof(float)}, {a.score, score, M * sizeof(float)}, {a.id, id, M * sizeof(int32_t)},
                   {a.ref, ref, N * sizeof(int32_t)}, {d_pid, pid.data(), N * sizeof(int32_t)}, {d_first, first, (N + 1) * sizeof(int32_t)}}));
   a.s = vmap_of(ctx), a.pid = d_pid, a.first = d_first, a.n = n, a.to_store = 1;
-  vmap_pack_kernel<<<(n + VMAP_WARPS - 1) / VMAP_WARPS, VMAP_WARPS * 32, 0, st>>>(a);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, vmap_pack_kernel, (n + VMAP_WARPS - 1) / VMAP_WARPS, VMAP_WARPS * 32, 0, a));
   CK(cudaStreamSynchronize(st));
   ctx->vmap_points = need;
   memcpy(point_id_out, pid.data(), N * sizeof(int32_t));
@@ -524,7 +500,6 @@ int esikf_vmap_update_points(esikf_ctx *ctx, int32_t n, const int32_t *point_id,
   static const double cos_max = acos_03_bound();
   *n_out = 0;
   if (n == 0) return ESIKF_OK;  // total_points == 0 (:910)
-  cudaStream_t st = ctx->stream;
   const size_t N = (size_t)n;
   VmapEditArgs e;
   ObsArgs &a = e.obs;
@@ -543,26 +518,22 @@ int esikf_vmap_update_points(esikf_ctx *ctx, int32_t n, const int32_t *point_id,
   CK(lay_out_scratch(ctx, lay));
   CK(upload(ctx, {{d_pid, point_id, N * sizeof(int32_t)}, {conv, converged, N}, {d_Tnew, T_f_w, 12 * sizeof(double)}}));
   e.s = vmap_of(ctx);
-  vmap_last_kernel<<<(n + 255) / 256, 256, 0, st>>>(e.s, d_pid, n, last_T, last_px);
+  CK(launch(ctx, vmap_last_kernel, (n + 255) / 256, 256, 0, e.s, d_pid, n, last_T, last_px));
   frame_consts(ctx, a.cam, a.Rci, a.Pci);
   a.state = dev_state, a.pos = ctx->vis_pos.p, a.converged = conv, a.last_T = last_T, a.last_px = last_px;
   a.n = n, a.cos_max = cos_max, a.keep = d_keep;
-  obs_flag_kernel<<<(n + OBS_THREADS - 1) / OBS_THREADS, OBS_THREADS, 0, st>>>(a);
-  select_scan_kernel<<<1, SELECT_SCAN_THREADS, 0, st>>>(d_keep, n, d_dst, d_nk);
-  obs_scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_keep, d_dst, a.pc, n, d_entry, out_pc);
-  ctx->launches += 4;
-  CK(cudaGetLastError());
+  CK(launch(ctx, obs_flag_kernel, (n + OBS_THREADS - 1) / OBS_THREADS, OBS_THREADS, 0, a));
+  CK(launch(ctx, select_scan_kernel, 1, SELECT_SCAN_THREADS, 0, d_keep, n, d_dst, d_nk));
+  CK(launch(ctx, obs_scatter_kernel, (n + 255) / 256, 256, 0, d_keep, d_dst, a.pc, n, d_entry, out_pc));
   int32_t nk;
   CK(read_back_to(ctx, d_nk, &nk));
   *n_out = nk;
   // the store is edited only once the answers fit: a call refused here can be repeated with a larger cap
   if (nk > cap) return fail(ctx, ESIKF_ERR_ARG, "vmap_update_points: %d new observations, room for %d", nk, cap);
-  if (nk > 0) image_patch_kernel<<<(nk * 64 + 255) / 256, 256, 0, st>>>(ctx->img.p, ctx->img_w, ctx->img_h, out_pc, nk, 0, patch);
+  if (nk > 0) CK(launch(ctx, image_patch_kernel, (nk * 64 + 255) / 256, 256, 0, ctx->img.p, ctx->img_w, ctx->img_h, out_pc, nk, 0, patch));
   e.pid = d_pid, e.dst = d_dst, e.new_pc = out_pc, e.new_patch = patch, e.T_f_w = T_f_w ? d_Tnew : nullptr, e.frame_id = frame_id;
   e.evicted = d_evicted, e.count = d_count;
-  vmap_edit_kernel<<<(n + VMAP_WARPS - 1) / VMAP_WARPS, VMAP_WARPS * 32, 0, st>>>(e);
-  ctx->launches += nk > 0 ? 2 : 1;
-  CK(cudaGetLastError());
+  CK(launch(ctx, vmap_edit_kernel, (n + VMAP_WARPS - 1) / VMAP_WARPS, VMAP_WARPS * 32, 0, e));
   CK(read_back(ctx, a.flag, patch + 64 * (size_t)nk));
   const void *f0 = a.flag;
   if (update_flag_out) copy_out(ctx, update_flag_out, f0, a.flag, N);
@@ -582,7 +553,6 @@ int esikf_vmap_score(esikf_ctx *ctx, int32_t n, const int32_t *point_id, const d
   if (int rc = vmap_check_ids(ctx, n, point_id, "vmap_score")) return rc;
   if (n == 0) return ESIKF_OK;
   CK(cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
   const size_t N = (size_t)n;
   int32_t *d_pid;
   double *d_pos, *d_normal;
@@ -600,13 +570,8 @@ int esikf_vmap_score(esikf_ctx *ctx, int32_t n, const int32_t *point_id, const d
   const VmapView v = vmap_of(ctx);
   a.pos = d_pos, a.normal = d_normal, a.T = v.T, a.patch = v.patch, a.mean = v.mean, a.id = v.id, a.n = n;
   a.score = v.score, a.mean_out = v.mean;  // in place
-  refpatch_score_kernel<<<(n + RP_WARPS - 1) / RP_WARPS, RP_WARPS * 32, 0, st>>>(a, RpStore{d_pid, v.count, v.ref});
-  ctx->launches++;
-  if (score_out || mean_out) {
-    vmap_rows_kernel<<<(n * VMAP_SLOTS + 255) / 256, 256, 0, st>>>(v, d_pid, n, nullptr, d_score, d_mean);
-    ctx->launches++;
-  }
-  CK(cudaGetLastError());
+  CK(launch(ctx, refpatch_score_kernel<RpStore>, (n + RP_WARPS - 1) / RP_WARPS, RP_WARPS * 32, 0, a, RpStore{d_pid, v.count, v.ref}));
+  if (score_out || mean_out) CK(launch(ctx, vmap_rows_kernel, (n * VMAP_SLOTS + 255) / 256, 256, 0, v, d_pid, n, nullptr, d_score, d_mean));
   const float *end = d_mean ? d_mean + VMAP_SLOTS * N : d_score ? d_score + VMAP_SLOTS * N : nullptr;
   CK(read_back(ctx, a.ref, end ? (const void *)end : (const void *)(a.ref + N)));
   copy_out(ctx, ref_out, a.ref, a.ref, N * sizeof(int32_t));
@@ -623,7 +588,6 @@ int esikf_vmap_choose_ref(esikf_ctx *ctx, int32_t n, const int32_t *point_id, co
   if (int rc = vmap_check_ids(ctx, n, point_id, "vmap_choose_ref")) return rc;
   if (n == 0) return ESIKF_OK;
   CK(cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
   const size_t N = (size_t)n;
   VmapChooseArgs a;
   int32_t *d_pid;
@@ -633,9 +597,7 @@ int esikf_vmap_choose_ref(esikf_ctx *ctx, int32_t n, const int32_t *point_id, co
   CK(upload(ctx, {{d_pid, point_id, N * sizeof(int32_t)}, {d_pos, pos, 3 * N * sizeof(double)}}));
   a.s = vmap_of(ctx), a.pid = d_pid, a.pos = d_pos, a.n = n, a.normal_en = normal_en != 0;
   for (int k = 0; k < 3; k++) a.frame_pos[k] = frame_pos ? frame_pos[k] : 0.0;
-  vmap_choose_kernel<<<(n + VMAP_WARPS - 1) / VMAP_WARPS, VMAP_WARPS * 32, 0, st>>>(a);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, vmap_choose_kernel, (n + VMAP_WARPS - 1) / VMAP_WARPS, VMAP_WARPS * 32, 0, a));
   CK(read_back_to(ctx, a.ref, ref_out, N));
   return ESIKF_OK;
 }
@@ -652,16 +614,13 @@ int esikf_vmap_download(esikf_ctx *ctx, int32_t n, const int32_t *point_id, int3
     return ESIKF_OK;
   }
   CK(cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
   const size_t N = (size_t)n;
   int32_t *d_pid, *d_count;
   auto lay1 = [&](CallLayout &s) { d_pid = s.take<int32_t>(N), s.end_inputs(), s.begin_answers(), d_count = s.take<int32_t>(N); };
   CK(lay_out_scratch(ctx, lay1));
   CK(upload(ctx, {{d_pid, point_id, N * sizeof(int32_t)}}));
   const VmapView v = vmap_of(ctx);
-  vmap_rows_kernel<<<(n * VMAP_SLOTS + 255) / 256, 256, 0, st>>>(v, d_pid, n, d_count, nullptr, nullptr);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, vmap_rows_kernel, (n * VMAP_SLOTS + 255) / 256, 256, 0, v, d_pid, n, d_count, nullptr, nullptr));
   CK(read_back(ctx, d_count, d_count + N));
   std::vector<int32_t> first(N + 1, 0);
   copy_out(ctx, first.data() + 1, d_count, d_count, N * sizeof(int32_t));
@@ -683,9 +642,7 @@ int esikf_vmap_download(esikf_ctx *ctx, int32_t n, const int32_t *point_id, int3
   CK(lay_out_scratch(ctx, lay2));
   CK(upload(ctx, {{d_pid, point_id, N * sizeof(int32_t)}, {d_first, first.data(), (N + 1) * sizeof(int32_t)}}));
   a.s = v, a.pid = d_pid, a.first = d_first, a.n = n, a.to_store = 0;
-  vmap_pack_kernel<<<(n + VMAP_WARPS - 1) / VMAP_WARPS, VMAP_WARPS * 32, 0, st>>>(a);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, vmap_pack_kernel, (n + VMAP_WARPS - 1) / VMAP_WARPS, VMAP_WARPS * 32, 0, a));
   CK(read_back(ctx, a.T, a.ref + N));
   const void *f0 = a.T;
   memcpy(first_out, first.data(), (N + 1) * sizeof(int32_t));
@@ -752,10 +709,8 @@ int esikf_vmap_place_points(esikf_ctx *ctx, int32_t n, const int32_t *point_id, 
   CK(upload(ctx, {{d_pid, point_id, N * sizeof(int32_t)}, {d_pos, pos, 3 * N * sizeof(double)}, {d_ninit, normal_init, normal_init ? N : 0}}));
   CK(cudaMemsetAsync(a.bad, 0, sizeof(int32_t), st));
   a.v = vpl_view(ctx->vpl.p, (size_t)ctx->vpl_cap), a.pid = d_pid, a.pos = d_pos, a.ninit = d_ninit, a.n = n, a.seq0 = (int32_t)ctx->vpl_placed;
-  vpl_key_kernel<<<(n + 255) / 256, 256, 0, st>>>(a);
-  vpl_commit_kernel<<<(n + 255) / 256, 256, 0, st>>>(a);  // writes nothing when a key was out of range
-  ctx->launches += 2;
-  CK(cudaGetLastError());
+  CK(launch(ctx, vpl_key_kernel, (n + 255) / 256, 256, 0, a));
+  CK(launch(ctx, vpl_commit_kernel, (n + 255) / 256, 256, 0, a));  // writes nothing when a key was out of range
   int32_t bad;
   CK(read_back_to(ctx, a.bad, &bad));
   if (bad) return fail(ctx, ESIKF_ERR_ARG, "vmap_place_points: a voxel key leaves [-2^20, 2^20)");
@@ -820,28 +775,26 @@ int esikf_vmap_retrieve(esikf_ctx *ctx, int32_t n_keys, const int32_t *keys, int
   CK(lay_out_scratch(ctx, lay));
   CK(upload(ctx, {{d_keys, keys, 3 * K * sizeof(int32_t)}}));
   CK(cudaMemsetAsync(table, 0xff, T * sizeof(unsigned long long), st));
-  vrt_hash_kernel<<<(n_keys + 255) / 256, 256, 0, st>>>(d_keys, n_keys, table, (int32_t *)a.wrank, T - 1);
+  CK(launch(ctx, vrt_hash_kernel, (n_keys + 255) / 256, 256, 0, d_keys, n_keys, table, (int32_t *)a.wrank, T - 1));
   CamDev cam;
   frame_consts(ctx, cam, a.Rci, a.Pci);
   memcpy(a.Rci, ctx->ret_Rci, sizeof(a.Rci)), memcpy(a.Pci, ctx->ret_Pci, sizeof(a.Pci));  // the scan call's
   a.cam = cam, a.state = ctx->ret_state.p, a.v = vpl_view(ctx->vpl.p, (size_t)ctx->vpl_cap), a.count = vmap_of(ctx).count, a.n_pts = (int)ctx->vpl_hi;
   a.wkey = table, a.wmask = T - 1, a.grid_size = grid_size, a.grid_n_width = grid_n_width, a.length = L, a.border = border, a.frame_pos = fpos;
-  vrt_init_kernel<<<(L + 255) / 256, 256, 0, st>>>(a);
+  CK(launch(ctx, vrt_init_kernel, (L + 255) / 256, 256, 0, a));
   const int pb = (a.n_pts + VRT_THREADS - 1) / VRT_THREADS;
-  vrt_walk_kernel<0><<<pb, VRT_THREADS, 0, st>>>(a);
-  vrt_walk_kernel<1><<<pb, VRT_THREADS, 0, st>>>(a);
-  vrt_walk_kernel<2><<<pb, VRT_THREADS, 0, st>>>(a);
+  CK(launch(ctx, vrt_walk_kernel<0>, pb, VRT_THREADS, 0, a));
+  CK(launch(ctx, vrt_walk_kernel<1>, pb, VRT_THREADS, 0, a));
+  CK(launch(ctx, vrt_walk_kernel<2>, pb, VRT_THREADS, 0, a));
   DepthCheckArgs dc;  // K11's check on every cell's winner (a cell without one is not read)
   memcpy(dc.Rci, ctx->ret_Rci, sizeof(dc.Rci)), memcpy(dc.Pci, ctx->ret_Pci, sizeof(dc.Pci));
   dc.state = ctx->ret_state.p, dc.pos = a.wpos, dc.pc = a.pc, dc.n = L, dc.width = W, dc.height = H, dc.depth = ctx->ret_depth.p, dc.flag = disc;
-  ret_depth_check_kernel<<<(L + RET_THREADS - 1) / RET_THREADS, RET_THREADS, 0, st>>>(dc);
+  CK(launch(ctx, ret_depth_check_kernel, (L + RET_THREADS - 1) / RET_THREADS, RET_THREADS, 0, dc));
   c.length = L, c.type = a.type, c.disc = disc, c.ninit = a.v.ninit, c.win = a.win, c.pc = a.pc, c.wpos = a.wpos;
-  vrt_cells_kernel<true><<<(L + 255) / 256, 256, 0, st>>>(c);
-  select_scan_kernel<<<1, SELECT_SCAN_THREADS, 0, st>>>(c.keep, L, c.dst, cnt);
-  select_scan_kernel<<<1, SELECT_SCAN_THREADS, 0, st>>>(c.skeep, L, c.sdst, cnt + 1);
-  vrt_cells_kernel<false><<<(L + 255) / 256, 256, 0, st>>>(c);
-  ctx->launches += 10;
-  CK(cudaGetLastError());
+  CK(launch(ctx, vrt_cells_kernel<true>, (L + 255) / 256, 256, 0, c));
+  CK(launch(ctx, select_scan_kernel, 1, SELECT_SCAN_THREADS, 0, c.keep, L, c.dst, cnt));
+  CK(launch(ctx, select_scan_kernel, 1, SELECT_SCAN_THREADS, 0, c.skeep, L, c.sdst, cnt + 1));
+  CK(launch(ctx, vrt_cells_kernel<false>, (L + 255) / 256, 256, 0, c));
   // vmap_choose_kernel takes its count and new_frame_->pos() by value: both come back before it runs, and a call refused for
   // its cap has not touched the store
   CK(read_back(ctx, fpos, cnt + 2));
@@ -855,10 +808,8 @@ int esikf_vmap_retrieve(esikf_ctx *ctx, int32_t n_keys, const int32_t *keys, int
     VmapChooseArgs ca;
     ca.s = vmap_of(ctx), ca.pid = c.spid, ca.pos = c.spos, ca.n = ns, ca.normal_en = normal_en != 0, ca.ref = ref_tmp;
     for (int k = 0; k < 3; k++) ca.frame_pos[k] = fp[k];
-    vmap_choose_kernel<<<(ns + VMAP_WARPS - 1) / VMAP_WARPS, VMAP_WARPS * 32, 0, st>>>(ca);
-    vrt_refs_kernel<<<(ns + 255) / 256, 256, 0, st>>>(ref_tmp, c.sat, ns, c.ref_out, c.status_out);
-    ctx->launches += 2;
-    CK(cudaGetLastError());
+    CK(launch(ctx, vmap_choose_kernel, (ns + VMAP_WARPS - 1) / VMAP_WARPS, VMAP_WARPS * 32, 0, ca));
+    CK(launch(ctx, vrt_refs_kernel, (ns + 255) / 256, 256, 0, ref_tmp, c.sat, ns, c.ref_out, c.status_out));
   }
   const size_t M = (size_t)counts[0];
   CK(read_back(ctx, c.pc_out, c.ref_out + M));

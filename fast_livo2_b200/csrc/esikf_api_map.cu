@@ -35,8 +35,7 @@ int esikf_map_upload(esikf_ctx *ctx, const int64_t *keys, const int32_t *first, 
   CK(cudaMemcpyAsync(ctx->map.slots.p, table.data(), cap * sizeof(HashSlot), cudaMemcpyHostToDevice, ctx->stream));
   if (n_planes) {
     CK(cudaMemcpyAsync(ctx->map.planes.p, planes, (size_t)n_planes * sizeof(esikf_plane), cudaMemcpyHostToDevice, ctx->stream));
-    plane_compact_kernel<<<(n_planes + 127) / 128, 128, 0, ctx->stream>>>(ctx->map.planes.p, nullptr, n_planes, ctx->map.recs.p);
-    ctx->launches++;
+    CK(launch(ctx, plane_compact_kernel, (n_planes + 127) / 128, 128, 0, ctx->map.planes.p, nullptr, n_planes, ctx->map.recs.p));
   }
   CK(cudaStreamSynchronize(ctx->stream));
   ctx->hash_mask = cap - 1;
@@ -63,8 +62,7 @@ int esikf_map_patch(esikf_ctx *ctx, const int32_t *plane_ids, const esikf_plane 
     auto lay = [&](CallLayout &s) { ids = s.take<int32_t>(n), s.end_inputs(); };
     CK(lay_out_scratch(ctx, lay));
     CK(upload(ctx, {{ids, plane_ids, (size_t)n * sizeof(int32_t)}}));
-    plane_compact_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(ctx->map.planes.p, ids, n, ctx->map.recs.p);
-    ctx->launches++;
+    CK(launch(ctx, plane_compact_kernel, (n + 127) / 128, 128, 0, ctx->map.planes.p, ids, n, ctx->map.recs.p));
   }
   CK(cudaStreamSynchronize(ctx->stream));
   return ESIKF_OK;
@@ -121,10 +119,9 @@ int esikf_map_device_init(esikf_ctx *ctx, const esikf_map_cfg *cfg) {
   mc.voxel_size = (float)cfg->voxel_size, mc.planer_threshold = (float)cfg->min_eigen_value;
   mc.max_layer = cfg->max_layer, mc.max_points_num = cfg->max_points_num;
   for (int k = 0; k < MAP_MAX_LAYERS; k++) mc.layer_init_num[k] = cfg->layer_init_num[k <= cfg->max_layer ? k : cfg->max_layer];
-  map_reset_kernel<<<(cap + 255) / 256, 256, 0, ctx->stream>>>(ctx->arena());
+  CK(launch(ctx, map_reset_kernel, (cap + 255) / 256, 256, 0, ctx->arena()));
   CK(cudaMemsetAsync(ctx->map_work.p, 0, 4 * sizeof(int), ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  ctx->launches++;
   ctx->map_cfg = *cfg;
   ctx->map_hash_bits = bits;
   ctx->hash_mask = cap - 1;
@@ -139,22 +136,20 @@ static int map_replay_tick(esikf_ctx *ctx, int n, bool build) {
   cudaStream_t st = ctx->stream;
   const unsigned int invalid = ctx->map.hash_cap;
   size_t tmp_bytes = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, ctx->map_key_in.p, ctx->map_key_out.p, ctx->map_idx_in.p, ctx->map_idx_out.p, n, 0, ctx->map_hash_bits + 1, st);
+  CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, ctx->map_key_in.p, ctx->map_key_out.p, ctx->map_idx_in.p, ctx->map_idx_out.p, n, 0, ctx->map_hash_bits + 1,
+                                     st));
   CK(ctx->map_sort_tmp.reserve(tmp_bytes + 16));
-  CK(cub::DeviceRadixSort::SortPairs(ctx->map_sort_tmp.p, tmp_bytes, ctx->map_key_in.p, ctx->map_key_out.p, ctx->map_idx_in.p, ctx->map_idx_out.p, n, 0,
-                                     ctx->map_hash_bits + 1, st));
+  CK(counted(ctx, cub::DeviceRadixSort::SortPairs(ctx->map_sort_tmp.p, tmp_bytes, ctx->map_key_in.p, ctx->map_key_out.p, ctx->map_idx_in.p, ctx->map_idx_out.p, n,
+                                                  0, ctx->map_hash_bits + 1, st)));
   CK(cudaMemsetAsync(ctx->map_work.p, 0, 2 * sizeof(int), st));
-  map_heads_kernel<<<(n + 255) / 256, 256, 0, st>>>(ctx->map_key_out.p, n, invalid, ctx->map_touched.p, ctx->map_work.p);
+  CK(launch(ctx, map_heads_kernel, (n + 255) / 256, 256, 0, ctx->map_key_out.p, n, invalid, ctx->map_touched.p, ctx->map_work.p));
   const unsigned long long *defer = nullptr;
   if (ctx->map_cfg.grow) {
     CK(cudaMemsetAsync(ctx->map_demand.p, 0, MAP_DEMAND_WORDS * sizeof(unsigned long long), st));
-    map_demand_kernel<<<ctx->sm_count * 4, 128, 0, st>>>(ctx->arena(), ctx->map_touched.p, ctx->map_work.p, ctx->map_demand.p, build ? 1 : 0);
+    CK(launch(ctx, map_demand_kernel, ctx->sm_count * 4, 128, 0, ctx->arena(), ctx->map_touched.p, ctx->map_work.p, ctx->map_demand.p, build ? 1 : 0));
     defer = ctx->map_demand.p + 5;
-    ctx->launches++;
   }
-  map_replay_kernel<<<ctx->sm_count * 4, 128, 0, st>>>(ctx->arena(), ctx->map_touched.p, ctx->map_work.p, ctx->map_idx_out.p, ctx->map_pt.p, build ? 1 : 0, defer);
-  ctx->launches += 4;
-  CK(cudaGetLastError());
+  CK(launch(ctx, map_replay_kernel, ctx->sm_count * 4, 128, 0, ctx->arena(), ctx->map_touched.p, ctx->map_work.p, ctx->map_idx_out.p, ctx->map_pt.p, build ? 1 : 0, defer));
   return ESIKF_OK;
 }
 
@@ -184,12 +179,10 @@ static int map_grow(esikf_ctx *ctx, long long hash_cap, long long node_cap, long
   }
   const MapArena S = ctx->arena(), D = fresh.view(ctx->arena_cfg);
   const long long big = 1ll << 40;
-  map_reset_kernel<<<(unsigned)((hash_cap + 255) / 256), 256, 0, st>>>(D);
+  CK(launch(ctx, map_reset_kernel, (unsigned)((hash_cap + 255) / 256), 256, 0, D));
   CK(cudaMemsetAsync(ctx->map_work.p, 0, 2 * sizeof(int), st));
-  map_survivors_kernel<<<(ctx->map.hash_cap + 255) / 256, 256, 0, st>>>(S, -big, -big, -big, big, big, big, ctx->map_survivors.p, ctx->map_work.p);
-  map_copy_kernel<<<ctx->sm_count * 4, 128, 0, st>>>(S, D, ctx->map_survivors.p, ctx->map_work.p);
-  ctx->launches += 3;
-  CK(cudaGetLastError());
+  CK(launch(ctx, map_survivors_kernel, (ctx->map.hash_cap + 255) / 256, 256, 0, S, -big, -big, -big, big, big, big, ctx->map_survivors.p, ctx->map_work.p));
+  CK(launch(ctx, map_copy_kernel, ctx->sm_count * 4, 128, 0, S, D, ctx->map_survivors.p, ctx->map_work.p));
   std::swap(ctx->map, fresh);
   int bits = 0;
   while ((1ll << bits) < hash_cap) bits++;
@@ -221,8 +214,7 @@ static int map_apply_points(esikf_ctx *ctx, int n, bool build) {
   const long long pool_cap = (d[5] & MAP_ERR_POOL) ? map_grown_capacity(m.pool_cap, u.pool_points, (long long)d[1]) : m.pool_cap;
   const long long rec_cap = (d[5] & MAP_ERR_RECS) ? map_grown_capacity(m.rec_cap, u.records, (long long)d[2]) : m.rec_cap;
   if ((rc = map_grow(ctx, m.hash_cap, node_cap, rec_cap, pool_cap, what))) return rc;
-  map_keys_kernel<<<(n + 255) / 256, 256, 0, st>>>(ctx->arena(), ctx->map_pt.p, n, ctx->map_key_in.p, ctx->map_idx_in.p, ctx->map.hash_cap);
-  ctx->launches++;
+  CK(launch(ctx, map_keys_kernel, (n + 255) / 256, 256, 0, ctx->arena(), ctx->map_pt.p, n, ctx->map_key_in.p, ctx->map_idx_in.p, ctx->map.hash_cap));
   if ((rc = map_replay_tick(ctx, n, build))) return rc;
   CK(cudaMemcpyAsync(d, ctx->map_demand.p, sizeof(d), cudaMemcpyDeviceToHost, st));
   if ((rc = map_check_errors(ctx, what))) return rc;
@@ -266,8 +258,7 @@ static int map_from_scan(esikf_ctx *ctx, const double *state, bool build) {
   if (map_hash_short(ctx, n)) {
     // pv.normal refers to the records of the last LIO run: snapshot it before the copy moves them
     if (match_plane) {
-      gather_normals_kernel<<<(n + 255) / 256, 256, 0, st>>>(match_plane, ctx->map.recs.p, n, ctx->map_pt_normal.p);
-      ctx->launches++;
+      CK(launch(ctx, gather_normals_kernel, (n + 255) / 256, 256, 0, match_plane, ctx->map.recs.p, n, ctx->map_pt_normal.p));
       match_plane = nullptr;
     }
     if ((rc = map_grow_hash(ctx, n, what))) return rc;
@@ -279,7 +270,7 @@ static int map_from_scan(esikf_ctx *ctx, const double *state, bool build) {
   a.build = build ? 1 : 0, a.dept_err = (float)ctx->map_cfg.dept_err, a.beam_err = (float)ctx->map_cfg.beam_err;
   a.match_plane = match_plane, a.recs = ctx->map.recs.p, a.pt_normal = ctx->map_pt_normal.p;
   a.pt = ctx->map_pt.p, a.pt_slot = ctx->map_key_in.p, a.pt_idx = ctx->map_idx_in.p, a.invalid_slot = ctx->map.hash_cap;
-  map_points_kernel<<<(n + 255) / 256, 256, 0, st>>>(ctx->arena(), a);
+  CK(launch(ctx, map_points_kernel, (n + 255) / 256, 256, 0, ctx->arena(), a));
   ctx->normals_n = build ? -1 : n;
   if ((rc = map_apply_points(ctx, n, build))) return rc;
   return ctx->map_export_points = n, ctx->pv_n = build ? -1 : n, ESIKF_OK;
@@ -304,8 +295,7 @@ int esikf_map_device_update_points(esikf_ctx *ctx, const double *point_w, const 
   CK(cudaMemcpy2DAsync(ctx->map_pt.p, MAP_PT_D * sizeof(double), point_w, 3 * sizeof(double), 3 * sizeof(double), n, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpy2DAsync(ctx->map_pt.p + 3, MAP_PT_D * sizeof(double), var, 9 * sizeof(double), 9 * sizeof(double), n, cudaMemcpyHostToDevice, st));
   if (map_hash_short(ctx, n) && (rc = map_grow_hash(ctx, n, "map_device_update"))) return rc;
-  map_keys_kernel<<<(n + 255) / 256, 256, 0, st>>>(ctx->arena(), ctx->map_pt.p, n, ctx->map_key_in.p, ctx->map_idx_in.p, ctx->map.hash_cap);
-  ctx->launches++;
+  CK(launch(ctx, map_keys_kernel, (n + 255) / 256, 256, 0, ctx->arena(), ctx->map_pt.p, n, ctx->map_key_in.p, ctx->map_idx_in.p, ctx->map.hash_cap));
   void_inputs(ctx, IN_NORMALS);
   if ((rc = map_apply_points(ctx, n, false))) return rc;
   return ctx->map_export_points = n, ESIKF_OK;
@@ -326,12 +316,10 @@ int esikf_map_device_slide(esikf_ctx *ctx, const int64_t key_min[3], const int64
   const long long big = 1ll << 40;
   const long long lo[3] = {key_min ? key_min[0] : -big, key_min ? key_min[1] : -big, key_min ? key_min[2] : -big};
   const long long hi[3] = {key_max ? key_max[0] : big, key_max ? key_max[1] : big, key_max ? key_max[2] : big};
-  map_reset_kernel<<<(cap + 255) / 256, 256, 0, st>>>(D);
+  CK(launch(ctx, map_reset_kernel, (cap + 255) / 256, 256, 0, D));
   CK(cudaMemsetAsync(ctx->map_work.p, 0, 2 * sizeof(int), st));
-  map_survivors_kernel<<<(cap + 255) / 256, 256, 0, st>>>(S, lo[0], lo[1], lo[2], hi[0], hi[1], hi[2], ctx->map_survivors.p, ctx->map_work.p);
-  map_copy_kernel<<<ctx->sm_count * 4, 128, 0, st>>>(S, D, ctx->map_survivors.p, ctx->map_work.p);
-  ctx->launches += 3;
-  CK(cudaGetLastError());
+  CK(launch(ctx, map_survivors_kernel, (cap + 255) / 256, 256, 0, S, lo[0], lo[1], lo[2], hi[0], hi[1], hi[2], ctx->map_survivors.p, ctx->map_work.p));
+  CK(launch(ctx, map_copy_kernel, ctx->sm_count * 4, 128, 0, S, D, ctx->map_survivors.p, ctx->map_work.p));
   // the fresh arena becomes the map (also when the copy reports an error: the status says so and the map is invalidated)
   std::swap(ctx->map, ctx->spare);
   void_inputs(ctx, IN_NORMALS);  // record positions of the last update are gone
@@ -373,8 +361,8 @@ int esikf_map_device_download(esikf_ctx *ctx, int64_t *keys, int32_t *first, int
   CK(lay_out_scratch(ctx, lay));
   CK(cudaMemsetAsync(d_out, 0, 2 * sizeof(int), st));
   const unsigned cap = ctx->map.hash_cap;
-  map_download_kernel<<<(cap + 255) / 256, 256, 0, st>>>(ctx->arena(), fill ? d_keys : nullptr, d_first, d_count, d_planes, fill ? roots_cap : 0, fill ? planes_cap : 0, d_out);
-  ctx->launches++;
+  CK(launch(ctx, map_download_kernel, (cap + 255) / 256, 256, 0, ctx->arena(), fill ? d_keys : nullptr, d_first, d_count, d_planes, fill ? roots_cap : 0,
+            fill ? planes_cap : 0, d_out));
   int out[2];
   CK(read_back_to(ctx, d_out, out, 2));
   *n_roots = out[0], *n_planes = out[1];
@@ -412,12 +400,11 @@ int esikf_map_device_export(esikf_ctx *ctx, int64_t *keys, int32_t *first, int32
   CK(lay_out_scratch(ctx, lay));
   // position n stays 0: the exclusive scan leaves the totals there
   CK(cudaMemsetAsync(packed, 0, ((size_t)n + 1) * sizeof(unsigned long long), st));
-  map_export_count_kernel<<<ctx->sm_count * 4, 128, 0, st>>>(ctx->arena(), ctx->map_touched.p, ctx->map_work.p, packed);
+  CK(launch(ctx, map_export_count_kernel, ctx->sm_count * 4, 128, 0, ctx->arena(), ctx->map_touched.p, ctx->map_work.p, packed));
   size_t tmp_bytes = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, packed, offs, n + 1, st);
+  CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, packed, offs, n + 1, st));
   CK(ctx->map_sort_tmp.reserve(tmp_bytes + 16));
-  CK(cub::DeviceScan::ExclusiveSum(ctx->map_sort_tmp.p, tmp_bytes, packed, offs, n + 1, st));
-  ctx->launches += 2;
+  CK(counted(ctx, cub::DeviceScan::ExclusiveSum(ctx->map_sort_tmp.p, tmp_bytes, packed, offs, n + 1, st)));
   unsigned long long total;
   CK(read_back_to(ctx, offs + n, &total));
   const int nr = (int)(total >> 32), nn = (int)(total & 0xffffffffull);
@@ -425,9 +412,7 @@ int esikf_map_device_export(esikf_ctx *ctx, int64_t *keys, int32_t *first, int32
   if (!fill) return ESIKF_OK;
   if (nr > roots_cap || nn > nodes_cap)
     return fail(ctx, ESIKF_ERR_ARG, "map_device_export: %d roots / %d nodes do not fit the buffers (%d / %d)", nr, nn, roots_cap, nodes_cap);
-  map_export_kernel<<<ctx->sm_count * 4, 128, 0, st>>>(ctx->arena(), ctx->map_touched.p, ctx->map_work.p, offs, d_keys, d_first, d_count, d_nodes, d_rows);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, map_export_kernel, ctx->sm_count * 4, 128, 0, ctx->arena(), ctx->map_touched.p, ctx->map_work.p, offs, d_keys, d_first, d_count, d_nodes, d_rows));
   // direct copies: read back through the pinned block, config 2's export (6.5 MB) took 2.0-2.1 ms a call against 1.75 ms (H100, 700 W)
   CK(cudaMemcpyAsync(keys, d_keys, (size_t)nr * 3 * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(first, d_first, (size_t)nr * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
@@ -443,7 +428,6 @@ int esikf_map_device_find(esikf_ctx *ctx, const double *points, int32_t n, int32
   if (int rc = need(ctx, "map_device_find", IN_DEVICE_MAP | IN_MAP)) return rc;
   if (n == 0) return ESIKF_OK;
   CK(cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
   const size_t N = (size_t)n;
   MapFindArgs a;
   a.n = n, a.rule = rule;
@@ -453,9 +437,7 @@ int esikf_map_device_find(esikf_ctx *ctx, const double *points, int32_t n, int32
   };
   CK(lay_out_scratch(ctx, lay));
   CK(upload(ctx, {{a.pts, points, 3 * N * sizeof(double)}}));
-  map_find_kernel<<<(n + FIND_THREADS - 1) / FIND_THREADS, FIND_THREADS, 0, st>>>(ctx->arena(), a);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, map_find_kernel, (n + FIND_THREADS - 1) / FIND_THREADS, FIND_THREADS, 0, ctx->arena(), a));
   CK(read_back(ctx, a.rows, a.status + N));
   copy_out(ctx, rows, a.rows, a.rows, N * sizeof(esikf_plane));
   copy_out(ctx, keys, a.rows, a.keys, 3 * N * sizeof(int64_t));
@@ -474,8 +456,7 @@ int esikf_lio_fetch_normals(esikf_ctx *ctx, double *normals) {
   CK(lay_out_scratch(ctx, lay));
   const double *src = ctx->map_pt_normal.p;
   if (ctx->normals_n != n) {
-    gather_normals_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(ctx->normal_plane.p, ctx->map.recs.p, n, normal);
-    ctx->launches++;
+    CK(launch(ctx, gather_normals_kernel, (n + 255) / 256, 256, 0, ctx->normal_plane.p, ctx->map.recs.p, n, normal));
     src = normal;
   }
   CK(read_back_to(ctx, src, normals, (size_t)n * 3));

@@ -18,7 +18,7 @@ static cudaEvent_t *timing_events(esikf_ctx *ctx, int base, int slot) {
   size_t need = (size_t)(base + slot + 1) * 3;
   while (ctx->ev.size() < need) {
     cudaEvent_t e;
-    if (cudaEventCreate(&e) != cudaSuccess) return nullptr;
+    if (cudaEventCreate(&e) != cudaSuccess) return cudaGetLastError(), nullptr;  // the run goes on untimed; no later launch reports this
     ctx->ev.push_back(e);
   }
   return &ctx->ev[(size_t)(base + slot) * 3];
@@ -53,12 +53,9 @@ static bool lio_use_l2_slots(int count, int grid) {
   const int chunks = (count + 31) / 32, per_cta = (chunks + grid - 1) / grid;
   return LIO_L2_WARPS > 0 && per_cta > LIO_SMEM_WARPS && per_cta <= LIO_SMEM_WARPS + LIO_L2_WARPS;
 }
-template <int L2W> static void launch_lio_residual(int grid, cudaStream_t st, const LioKernelArgs &ka) {
-  lio_residual_kernel<L2W><<<grid, LioSmem<L2W>::THREADS, sizeof(LioSmem<L2W>), st>>>(ka);
-}
-static void launch_lio_residual(bool l2_slots, int grid, cudaStream_t st, const LioKernelArgs &ka) {
-  if (l2_slots) launch_lio_residual<LIO_L2_WARPS>(grid, st, ka);
-  else launch_lio_residual<0>(grid, st, ka);
+static cudaError_t launch_lio_residual(esikf_ctx *ctx, bool l2_slots, int grid, const LioKernelArgs &ka) {
+  if (l2_slots) return launch(ctx, lio_residual_kernel<LIO_L2_WARPS>, grid, LioSmem<LIO_L2_WARPS>::THREADS, sizeof(LioSmem<LIO_L2_WARPS>), ka);
+  return launch(ctx, lio_residual_kernel<0>, grid, LioSmem<0>::THREADS, sizeof(LioSmem<0>), ka);
 }
 
 cudaError_t update_kernels_setup(esikf_ctx *ctx) {
@@ -111,10 +108,13 @@ int esikf_lio_set_scan(esikf_ctx *ctx, const float *pts_xyz, int32_t n) {
 // calcBodyCov and the cross-matrix vector of every point of the resident scan (voxel_map.cpp:349-360). StateEstimation
 // recomputes both every call; here they are kept with what they were made from and redone only when the scan, the lidar
 // extrinsics or the noise model changed.
-static void lio_precompute(esikf_ctx *ctx, float dept_err, float beam_err) {
-  lio_precompute_kernel<<<(ctx->n_pts + 255) / 256, 256, 0, ctx->stream>>>(ctx->pts.p, ctx->n_pts, ctx->pre.p, ctx->pre_stride, ctx->ext_dev.p, dept_err, beam_err);
+static cudaError_t lio_precompute(esikf_ctx *ctx, float dept_err, float beam_err) {
+  const cudaError_t e = launch(ctx, lio_precompute_kernel, (ctx->n_pts + 255) / 256, 256, 0, ctx->pts.p, ctx->n_pts, ctx->pre.p, ctx->pre_stride, ctx->ext_dev.p,
+                               dept_err, beam_err);
+  if (e) return e;
   memcpy(ctx->pre_ext, ctx->ext_host, sizeof(ctx->pre_ext));
   ctx->pre_dept_err = dept_err, ctx->pre_beam_err = beam_err;
+  return cudaSuccess;
 }
 static bool lio_precompute_current(const esikf_ctx *ctx, float dept_err, float beam_err) {
   return ctx->scan != esikf_ctx::SCAN_SET && memcmp(ctx->pre_ext, ctx->ext_host, sizeof(ctx->pre_ext)) == 0 && ctx->pre_dept_err == dept_err && ctx->pre_beam_err == beam_err;
@@ -226,10 +226,7 @@ int esikf_lio_run(esikf_ctx *ctx, const double *state_in, const double *state_pr
   const int n = ctx->n_pts;
   const float dept_err = (float)cfg->dept_err, beam_err = (float)cfg->beam_err;
   if (!lio_precompute_current(ctx, dept_err, beam_err)) {
-    if (n > 0) {
-      lio_precompute(ctx, dept_err, beam_err);
-      ctx->launches++;
-    }
+    if (n > 0) CK(lio_precompute(ctx, dept_err, beam_err));
     if (ctx->scan == esikf_ctx::SCAN_SET) ctx->scan = esikf_ctx::SCAN_RUN;
   }
   LioKernelArgs ka;
@@ -248,17 +245,15 @@ int esikf_lio_run(esikf_ctx *ctx, const double *state_in, const double *state_pr
   ctx->lio_slots = cfg->max_iterations;
   for (int it = 0; it < cfg->max_iterations; it++) {
     cudaEvent_t *e = ctx->timing ? timing_events(ctx, EV_LIO_BASE, it) : nullptr;
-    if (e) cudaEventRecord(e[0], st);
+    if (e) CK(cudaEventRecord(e[0], st));
     ka.init_normal = (it == 0);
-    launch_lio_residual(l2_slots, grid, st, ka);
-    if (e) cudaEventRecord(e[1], st);
+    CK(launch_lio_residual(ctx, l2_slots, grid, ka));
+    if (e) CK(cudaEventRecord(e[1], st));
     int rc = allreduce_info(ctx);
     if (rc) return rc;
-    lio_solve_kernel<<<1, SOLVE_THREADS, 0, st>>>(sa);
-    if (e) cudaEventRecord(e[2], st);
-    ctx->launches += 2;
+    CK(launch(ctx, lio_solve_kernel, 1, SOLVE_THREADS, 0, sa));
+    if (e) CK(cudaEventRecord(e[2], st));
   }
-  CK(cudaGetLastError());
   ctx->resident = esikf_ctx::RESIDENT_LIO;
   return ESIKF_OK;
 }
@@ -270,7 +265,7 @@ static int finish_fetch(esikf_ctx *ctx) {
   CK(cudaMemcpyAsync(h, ctx->ctrl, sizeof(Ctrl), cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   if (h->comm_error) {
-    cudaMemsetAsync(&ctx->ctrl->comm_error, 0, sizeof(int), ctx->stream);
+    CK(cudaMemsetAsync(&ctx->ctrl->comm_error, 0, sizeof(int), ctx->stream));
     return fail(ctx, ESIKF_ERR_COMM, "a bounded in-kernel wait expired (grid barrier, grid or peer mailbox): a rank did not take part in the update");
   }
   return ESIKF_OK;
@@ -323,8 +318,7 @@ int esikf_lio_fetch_point_cov(esikf_ctx *ctx, double *body_cov9, double *cross_m
   double *body, *cross;
   auto lay = [&](CallLayout &s) { s.begin_answers(), body = s.take<double>(N9), cross = s.take<double>(N9); };
   CK(lay_out_scratch(ctx, lay));
-  expand_point_cov_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(ctx->pre.p, ctx->pre_stride, n, body_cov9 ? body : nullptr, cross_mat9 ? cross : nullptr);
-  ctx->launches++;
+  CK(launch(ctx, expand_point_cov_kernel, (n + 255) / 256, 256, 0, ctx->pre.p, ctx->pre_stride, n, body_cov9 ? body : nullptr, cross_mat9 ? cross : nullptr));
   const double *f0 = body_cov9 ? body : cross;
   CK(read_back(ctx, f0, cross_mat9 ? cross + N9 : body_cov9 ? body + N9 : f0));
   if (body_cov9) copy_out(ctx, body_cov9, f0, body, N9 * sizeof(double));
@@ -486,28 +480,24 @@ int esikf_vio_run(esikf_ctx *ctx, const double *state_in, const double *state_pr
   ctx->vio_slots = ctx->vio_cfg.patch_pyrimid_level * ctx->vio_cfg.max_iterations;
   int slot = 0;
   for (int level = ctx->vio_cfg.patch_pyrimid_level - 1; level >= 0; level--) {
-    if (inverse) {  // has_ref_patch_cache = false at every level (vio.cpp:794): H_sub_inv of this level's tap stride
-      vio_inverse_precompute_kernel<<<(ka.count + 7) / 8, 256, 0, st>>>(ka, iv, level);
-      ctx->launches++;
-    }
+    if (inverse)  // has_ref_patch_cache = false at every level (vio.cpp:794): H_sub_inv of this level's tap stride
+      CK(launch(ctx, vio_inverse_precompute_kernel, (ka.count + 7) / 8, 256, 0, ka, iv, level));
     for (int it = 0; it < ctx->vio_cfg.max_iterations; it++, slot++) {
       ka.level = level, ka.slot_iter = it;
       cudaEvent_t *e = ctx->timing ? timing_events(ctx, EV_VIO_BASE, slot) : nullptr;
-      if (e) cudaEventRecord(e[0], st);
+      if (e) CK(cudaEventRecord(e[0], st));
       if (inverse)
-        vio_inverse_patch_kernel<<<grid, VIO_THREADS, sizeof(VioSmem), st>>>(ka, iv);
+        CK(launch(ctx, vio_inverse_patch_kernel, grid, VIO_THREADS, sizeof(VioSmem), ka, iv));
       else
-        vio_patch_kernel<<<grid, VIO_THREADS, sizeof(VioSmem), st>>>(ka);
-      if (e) cudaEventRecord(e[1], st);
+        CK(launch(ctx, vio_patch_kernel, grid, VIO_THREADS, sizeof(VioSmem), ka));
+      if (e) CK(cudaEventRecord(e[1], st));
       int rc = allreduce_info(ctx);
       if (rc) return rc;
       sa.level = level, sa.slot_iter = it, sa.last_slot = (level == 0 && it == ctx->vio_cfg.max_iterations - 1);
-      vio_solve_kernel<<<1, SOLVE_THREADS, 0, st>>>(sa);
-      if (e) cudaEventRecord(e[2], st);
-      ctx->launches += 2;
+      CK(launch(ctx, vio_solve_kernel, 1, SOLVE_THREADS, 0, sa));
+      if (e) CK(cudaEventRecord(e[2], st));
     }
   }
-  CK(cudaGetLastError());
   ctx->resident = esikf_ctx::RESIDENT_VIO;
   return ESIKF_OK;
 }
@@ -546,8 +536,7 @@ int esikf_vio_get_image_patch(esikf_ctx *ctx, const double *pc, int32_t n, int32
   auto lay = [&](CallLayout &s) { pc_d = s.take<double>(N * 2), s.end_inputs(), s.begin_answers(), patch = s.take<float>(N * 64); };
   CK(lay_out_scratch(ctx, lay));
   CK(upload(ctx, {{pc_d, pc, N * 2 * sizeof(double)}}));
-  image_patch_kernel<<<(n * 64 + 255) / 256, 256, 0, ctx->stream>>>(ctx->img.p, ctx->img_w, ctx->img_h, pc_d, n, level, patch);
-  ctx->launches++;
+  CK(launch(ctx, image_patch_kernel, (n * 64 + 255) / 256, 256, 0, ctx->img.p, ctx->img_w, ctx->img_h, pc_d, n, level, patch));
   CK(read_back_to(ctx, patch, patch_out, N * 64));
   return ESIKF_OK;
 }
@@ -609,11 +598,10 @@ int esikf_vio_warp_patches(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_ind
                   {T_cur, T_cur_w, 12 * sizeof(double)}}));
   CamDev cam;
   cam_dev(ctx, cam);
-  warp_matrix_kernel<<<(n + 127) / 128, 128, 0, st>>>(cam, n, px, pos, normal, T_ref, T_cur, A, ctx->search_levels.p);
+  CK(launch(ctx, warp_matrix_kernel, (n + 127) / 128, 128, 0, cam, n, px, pos, normal, T_ref, T_cur, A, ctx->search_levels.p));
   CK(cudaMemsetAsync(ctx->warp_patch.p, 0, N * 64 * L * sizeof(float), st));
-  warp_affine_kernel<<<(n * L * 64 + 255) / 256, 256, 0, st>>>(ctx->ref_img_ptrs.p, ref_idx, ctx->ref_w, ctx->ref_h, n, L, A, px, ctx->search_levels.p,
-                                                              ctx->warp_patch.p);
-  ctx->launches += 2;
+  CK(launch(ctx, warp_affine_kernel, (n * L * 64 + 255) / 256, 256, 0, ctx->ref_img_ptrs.p, ref_idx, ctx->ref_w, ctx->ref_h, n, L, A, px, ctx->search_levels.p,
+            ctx->warp_patch.p));
   if (search_level_out) CK(cudaMemcpyAsync(levels, ctx->search_levels.p, N * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
   if (warp_patch_out) CK(cudaMemcpyAsync(warp, ctx->warp_patch.p, N * 64 * L * sizeof(float), cudaMemcpyDeviceToDevice, st));
   if (keep_on_device) {
@@ -676,27 +664,25 @@ int esikf_vio_select_patches(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_i
   CamDev cam;
   cam_dev(ctx, cam);
   if (homography)
-    warp_matrix_kernel<<<(n + 127) / 128, 128, 0, st>>>(cam, n, d_px, d_pos, d_nrm, d_T, d_Tc, d_A, d_sl);
+    CK(launch(ctx, warp_matrix_kernel, (n + 127) / 128, 128, 0, cam, n, d_px, d_pos, d_nrm, d_T, d_Tc, d_A, d_sl));
   else
-    warp_matrix_depth_kernel<<<(n + 127) / 128, 128, 0, st>>>(cam, n, d_px, d_f, d_rp, d_pos, d_T, d_Tc, d_lvl, d_key, d_A, d_sl);
+    CK(launch(ctx, warp_matrix_depth_kernel, (n + 127) / 128, 128, 0, cam, n, d_px, d_f, d_rp, d_pos, d_T, d_Tc, d_lvl, d_key, d_A, d_sl));
   // patch_wrap is a fresh zero vector per candidate (:646): a NaN inverse leaves it zero (:297-301)
   CK(cudaMemsetAsync(d_warp, 0, N * 64 * L * sizeof(float), st));
-  warp_affine_kernel<<<(n * L * 64 + 255) / 256, 256, 0, st>>>(ctx->ref_img_ptrs.p, d_idx, ctx->ref_w, ctx->ref_h, n, L, d_A, d_px, d_sl, d_warp);
+  CK(launch(ctx, warp_affine_kernel, (n * L * 64 + 255) / 256, 256, 0, ctx->ref_img_ptrs.p, d_idx, ctx->ref_w, ctx->ref_h, n, L, d_A, d_px, d_sl, d_warp));
   SelectGateArgs ga;
   ga.img = ctx->img.p, ga.width = ctx->img_w, ga.height = ctx->img_h, ga.n = n, ga.levels = L, ga.ncc_en = cfg->ncc_en != 0;
   ga.pc = d_pc, ga.warp = d_warp, ga.ref_inv_expo = d_ie;
   ga.cur_inv_expo = inv_expo_time, ga.ncc_thre = cfg->ncc_thre, ga.outlier_threshold = cfg->outlier_threshold;
   ga.error = d_err, ga.keep = d_keep;
-  select_gate_kernel<<<(n + SELECT_GATE_WARPS - 1) / SELECT_GATE_WARPS, 32 * SELECT_GATE_WARPS, 0, st>>>(ga);
-  select_scan_kernel<<<1, SELECT_SCAN_THREADS, 0, st>>>(d_keep, n, d_dst, d_nk);
+  CK(launch(ctx, select_gate_kernel, (n + SELECT_GATE_WARPS - 1) / SELECT_GATE_WARPS, 32 * SELECT_GATE_WARPS, 0, ga));
+  CK(launch(ctx, select_scan_kernel, 1, SELECT_SCAN_THREADS, 0, d_keep, n, d_dst, d_nk));
   SelectScatterArgs sa;
   sa.n = n, sa.levels = L, sa.keep = d_keep, sa.dst = d_dst, sa.search_level = d_sl, sa.pos_w = d_pos, sa.ref_inv_expo = d_ie, sa.A = d_A;
   sa.warp = d_warp, sa.error = d_err;
   sa.vis_pos = ctx->vis_pos.p, sa.inv_expo = ctx->inv_expo.p, sa.A_kept = d_Akept, sa.warp_patch = ctx->warp_patch.p, sa.errors = ctx->errors.p;
   sa.search_levels = ctx->search_levels.p, sa.kept_index = d_kept;
-  select_scatter_kernel<<<(n + 7) / 8, 256, 0, st>>>(sa);
-  ctx->launches += 5;
-  CK(cudaGetLastError());
+  CK(launch(ctx, select_scatter_kernel, (n + 7) / 8, 256, 0, sa));
   int32_t nk;
   CK(read_back_to(ctx, d_nk, &nk));
   commit_submap(ctx, nk, L);
@@ -767,9 +753,7 @@ int esikf_vio_warp_affine(esikf_ctx *ctx, int32_t n, const int32_t *ref_img_inde
   CK(upload(ctx, {{ref_idx, ref_img_index, N * sizeof(int32_t)}, {px, px_ref, N * 2 * sizeof(double)}, {A, A_cur_ref, N * 4 * sizeof(double)},
                   {levels, search_level, N * sizeof(int32_t)}}));
   CK(cudaMemsetAsync(out, 0, N * 64 * L * sizeof(float), st));
-  warp_affine_kernel<<<(n * L * 64 + 255) / 256, 256, 0, st>>>(ctx->ref_img_ptrs.p, ref_idx, ctx->ref_w, ctx->ref_h, n, L, A, px, levels, out);
-  ctx->launches += 1;
-  CK(cudaGetLastError());
+  CK(launch(ctx, warp_affine_kernel, (n * L * 64 + 255) / 256, 256, 0, ctx->ref_img_ptrs.p, ref_idx, ctx->ref_w, ctx->ref_h, n, L, A, px, levels, out));
   CK(read_back_to(ctx, out, warp_patch_out, N * 64 * L));
   return ESIKF_OK;
 }
@@ -823,18 +807,16 @@ int esikf_profile_kernel(esikf_ctx *ctx, int32_t which, int32_t arg, int32_t rep
       CK(cudaMemsetAsync(ctx->ctrl, 0, sizeof(Ctrl), st));
     }
     CK(cudaEventRecord(e0, st));
-    if (which == 0) launch_lio_residual(lio_use_l2_slots(la.count, grid), grid, st, la);
-    else if (which == 1) lio_solve_kernel<<<1, SOLVE_THREADS, 0, st>>>(sa);
-    else if (which == 2) vio_patch_kernel<<<grid, VIO_THREADS, sizeof(VioSmem), st>>>(va);
-    else lio_precompute(ctx, (float)ctx->lio_cfg.dept_err, (float)ctx->lio_cfg.beam_err);
+    if (which == 0) CK(launch_lio_residual(ctx, lio_use_l2_slots(la.count, grid), grid, la));
+    else if (which == 1) CK(launch(ctx, lio_solve_kernel, 1, SOLVE_THREADS, 0, sa));
+    else if (which == 2) CK(launch(ctx, vio_patch_kernel, grid, VIO_THREADS, sizeof(VioSmem), va));
+    else CK(lio_precompute(ctx, (float)ctx->lio_cfg.dept_err, (float)ctx->lio_cfg.beam_err));
     CK(cudaEventRecord(e1, st));
     CK(cudaEventSynchronize(e1));
-    ctx->launches++;
     float ms = 0;
     CK(cudaEventElapsedTime(&ms, e0, e1));
     if (r >= 3) total += ms;
   }
-  CK(cudaGetLastError());
   *avg_ms = (float)(total / reps);
   return ESIKF_OK;
 }

@@ -126,7 +126,9 @@ int esikf_synchronize(esikf_ctx *ctx);
  * it are DMA transfers instead of driver-staged pageable copies. NULL on failure; free(NULL) is a no-op. */
 void *esikf_host_alloc(size_t bytes);
 void esikf_host_free(void *p);
-/* Number of kernels launched by this context since creation (bench.py "gpu_launches"). */
+/* Number of launches this context has enqueued since creation (bench.py "gpu_launches"). Each kernel launch counts one,
+ * the persistent update kernel's single cooperative launch included, and each CUB device-wide call (a sort or a scan)
+ * counts one, however many kernels it runs. A launch that fails to enqueue is not counted. */
 int64_t esikf_launch_count(const esikf_ctx *ctx);
 /* solve_mode: 0 = Woodbury 6x6/7x7 form of (H^T H + P^-1)^-1 (default), 1 = literal two 19x19
  * partial-pivot inversions as at src/voxel_map.cpp:468 / src/vio.cpp:1661. */
