@@ -20,7 +20,7 @@ namespace esikf {
 
 // Optional phase timestamps (ns, %globaltimer) written by CTA 0 / thread 0 — measurement only.
 // The VIO kernel's finer stamps (builds with ESIKF_VIO_CHAIN_STAMPS; VioKernelArgs::chain, 8 per (level, iteration) slot,
-// 64 slots; tools/vio_chain_timing.py): warp 0's first patch
+// 64 slots; tools/ab_timing.py): warp 0's first patch
 // (vio_process_range) at 8 slot + 0..3, every CTA's slice end (its partial summed) at VIO_CHAIN_CTA + VIO_CHAIN_MAX_CTAS slot
 // + blockIdx.x.
 #define VIO_CHAIN_CTA (8 * 64)

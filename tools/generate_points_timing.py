@@ -9,20 +9,21 @@ host loop of the oracle's restatement (oracle/orc_generate.cpp, the reference's 
               torch.profiler run of its own, per tick
   host loop : orc_generate_points, one thread
 
-The winners of the device and the oracle are checked to be equal. The card's name and power limit are printed in the same
+The winners of the device and the oracle are checked to be equal. The card's name, power limit and maximum SM clock are printed in the same
 run. Writes nothing; needs a GPU.
 
   python tools/generate_points_timing.py [--reps 30]"""
 import argparse
+import json
 import os
-import subprocess
 import sys
 import time
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests"), os.path.join(ROOT, "tools")]
+import timing as T  # noqa: E402
 import torch  # noqa: E402
 
 import generate_cases as GC  # noqa: E402
@@ -37,10 +38,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=30)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("needs a CUDA device")
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    print(f"device: {q.splitlines()[0] if q else torch.cuda.get_device_name(0)}")
+    T.require_gpu("generate_points_timing")
+    print(f"device: {json.dumps(T.card())}")
     ctx = api.Context(0)
     stream = torch.cuda.ExternalStream(ctx.stream)
     for n in (100_000, 300_000):
@@ -56,36 +55,12 @@ def main():
         for _ in range(5):
             got = once()
         ctx.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        t0 = time.perf_counter()
-        e0.record(stream)
-        for _ in range(args.reps):
-            once()
-        e1.record(stream)
-        ctx.synchronize()
-        e1.synchronize()
-        wall = (time.perf_counter() - t0) / args.reps * 1e3
-        print(f"n={n} api (H2D scan + mask, D2H winners)  events {e0.elapsed_time(e1) / args.reps:.3f} ms/tick  host {wall:.3f} ms/tick  "
+        ev, wall = T.window_ms(stream, once, args.reps)
+        print(f"n={n} api (H2D scan + mask, D2H winners)  events {ev:.3f} ms/tick  host {wall:.3f} ms/tick  "
               f"new points={len(got['cell'])}")
 
-        from torch.profiler import ProfilerActivity, profile
-
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            for _ in range(args.reps):
-                once()
-            ctx.synchronize()
-        per = {k: [] for k in KERNELS}
-        for ev in prof.events():
-            for k in KERNELS:
-                if k in ev.name and ev.device_type == torch.autograd.DeviceType.CUDA:
-                    per[k].append(ev.device_time if hasattr(ev, "device_time") else ev.cuda_time)
-        tot = 0.0
-        parts = []
-        for k in KERNELS:
-            us = float(np.sum(per[k])) / args.reps if per[k] else float("nan")  # per tick
-            tot += us
-            parts.append(f"{k} {us:.1f} us")
-        print(f"n={n} kernels {tot / 1e3:.3f} ms/tick: " + ", ".join(parts))
+        us = {k: float(np.sum(v)) / args.reps if v else float("nan") for k, v in T.kernel_us(once, args.reps, KERNELS).items()}  # per tick
+        print(f"n={n} kernels {sum(us.values()) / 1e3:.3f} ms/tick: " + ", ".join(f"{k} {v:.1f} us" for k, v in us.items()))
 
         o = GC.OracleGenerate(sc)
         t0 = time.perf_counter()

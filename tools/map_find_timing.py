@@ -10,7 +10,7 @@ tick a LIO update and UpdateVoxelMap), after --warmup such ticks.
            UpdateVoxelMap(); and for the same query points the host find_correspond on the mirror (fl2_shim_mirror_find) and
            FindCorrespond through the mirror-off session.
 
-Prints one JSON line with the card's name and power limit read in the same run.
+Prints one JSON line with the card's name, power limit and maximum SM clock read in the same run.
 
     python tools/map_find_timing.py [--warmup 10] [--ticks 20] [--reps 50] [--out result.json]
 """
@@ -24,22 +24,14 @@ import time
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests"), os.path.join(ROOT, "tools")]
+import timing as T  # noqa: E402
 
 SIZES = (2000, 5000, 20000)
 
 
-def _profiled_kernel_ms(ctx, q, torch):
-    from torch.profiler import ProfilerActivity, profile
-
-    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
-        for _ in range(10):
-            ctx.map_device_find(q, 0)
-        torch.cuda.synchronize()
-    us = [e.device_time if hasattr(e, "device_time") else e.cuda_time for e in prof.events()
-          if e.device_type == torch.autograd.DeviceType.CUDA and "map_find_kernel" in e.name]
+def _profiled_kernel_ms(ctx, q):
+    us = T.kernel_us(lambda: ctx.map_device_find(q, 0), 10, ("map_find_kernel",))["map_find_kernel"]
     assert us, "no map_find_kernel in the trace"
     return statistics.median(us) / 1e3
 
@@ -53,13 +45,10 @@ def main():
     args = ap.parse_args()
     import ctypes as C
 
+    T.require_gpu("map_find_timing")
     import torch
-
-    if not torch.cuda.is_available():
-        raise SystemExit("map_find_timing: no CUDA device (the numbers are GPU timings; there is no CPU fallback)")
     from fast_livo2_b200 import api, workloads
     from fast_livo2_b200.synthetic import PLANE_DTYPE
-    from map_growth_timing import card
     from map_mirror import MirrorView, session, shim_sessions, vp
 
     fr = workloads.frame("cfg2")
@@ -70,7 +59,7 @@ def main():
     lib = shim_sessions()
     lib.fl2_shim_session_find_correspond.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     hs = {"mirror": session(lib, cfg, ext, fr["map"]), "plain": session(lib, cfg, ext, fr["map"])}
-    res = dict(what=f"cfg2 frame ({len(pts)} points), bench.py's map-leg sequence after {args.warmup} warm-up ticks; lookups with updateReferencePatch's key rule", **card(),
+    res = dict(what=f"cfg2 frame ({len(pts)} points), bench.py's map-leg sequence after {args.warmup} warm-up ticks; lookups with updateReferencePatch's key rule", **T.card(),
                voxel_size=cfg.voxel_size)
     try:
         ctx.set_extrinsics(ext)
@@ -103,16 +92,7 @@ def main():
             got = ctx.map_device_find(q, 0)
             for _ in range(5):
                 ctx.map_device_find(q, 0)
-            ev_ms, wall_ms = [], []
-            for _ in range(args.reps):
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record(stream)
-                t0 = time.perf_counter()
-                ctx.map_device_find(q, 0)
-                wall_ms.append((time.perf_counter() - t0) * 1e3)
-                e1.record(stream)
-                e1.synchronize()
-                ev_ms.append(e0.elapsed_time(e1))
+            ev_ms, wall_ms = T.per_call_ms(stream, lambda: ctx.map_device_find(q, 0), args.reps)
             mirror_ms, shim_ms = [], []
             st, rows = np.zeros(n, np.uint8), np.zeros(n, PLANE_DTYPE)
             for _ in range(max(5, args.reps // 5)):
@@ -122,7 +102,7 @@ def main():
                 t0 = time.perf_counter()
                 assert lib.fl2_shim_session_find_correspond(hs["plain"], q.ctypes.data, n, 0, st.ctypes.data, rows.ctypes.data) == 0
                 shim_ms.append((time.perf_counter() - t0) * 1e3)
-            res["sizes"][n] = dict(planes_found=int((got["status"] == 2).sum()), kernel_ms=_profiled_kernel_ms(ctx, q, torch), call_events_ms=statistics.median(ev_ms),
+            res["sizes"][n] = dict(planes_found=int((got["status"] == 2).sum()), kernel_ms=_profiled_kernel_ms(ctx, q), call_events_ms=statistics.median(ev_ms),
                                    call_wall_ms=statistics.median(wall_ms), mirror_host_find_ms=statistics.median(mirror_ms),
                                    shim_find_correspond_ms=statistics.median(shim_ms))
     finally:

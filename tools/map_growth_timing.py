@@ -7,7 +7,7 @@ contexts, tick by tick in turn:
 
 CUDA events on each context's stream around esikf_map_device_update. Reports the steady-state tick time of both (B's extra
 cost there is the demand kernel), the time of every tick on which B grew, both final capacities and the bytes they take
-(computed from the capacities and the struct sizes, without the allocator's headroom), and the card's name and power limit
+(computed from the capacities and the struct sizes, without the allocator's headroom), and the card's name, power limit and maximum SM clock
 read in the same run. The two maps are compared bit for bit at the end.
 
     python tools/map_growth_timing.py [--ticks 30] [--out result.json]
@@ -16,14 +16,13 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests"), os.path.join(ROOT, "tools")]
+import timing as T  # noqa: E402
 
 # bytes per unit of each capacity: a hash slot (HashSlot + slot_root + slot_cap), a MapNode, a stored point (12 doubles),
 # a record (PlaneRec + esikf_plane + rec_node)
@@ -35,28 +34,14 @@ def footprint(cap):
     return int(sum(cap[k] * BYTES[k] for k in CAPS))
 
 
-def card():
-    import torch
-
-    name = torch.cuda.get_device_name(0)
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True, timeout=30)
-        power = q.stdout.strip() or "not available"
-    except (OSError, subprocess.SubprocessError):
-        power = "not available"
-    return dict(gpu=name, power_limit=power)
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--ticks", type=int, default=30)
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
-    import torch
-
-    if not torch.cuda.is_available():
-        raise SystemExit("map_growth_timing: no CUDA device (the numbers are GPU timings; there is no CPU fallback)")
+    T.require_gpu("map_growth_timing")
     import map_bind as MB
+    import torch
     from fast_livo2_b200 import api, workloads
 
     fr = workloads.frame("cfg2")
@@ -80,12 +65,7 @@ def main():
             for name, c in ctxs.items():  # A then B, every tick
                 c.lio_update(pts, fr["state_prior"], fr["state_prior"], cfg)
                 before = c.map_device_capacity()
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record(streams[name])
-                c.map_device_update()
-                e1.record(streams[name])
-                e1.synchronize()
-                ms[name].append(e0.elapsed_time(e1))
+                ms[name] += T.per_call_ms(streams[name], c.map_device_update, 1)[0]
                 now = c.map_device_capacity()
                 if name == "B" and any(now[q] != before[q] for q in CAPS):
                     grew.append(dict(tick=k, ms=ms["B"][-1], grown={q: [before[q], now[q]] for q in CAPS if now[q] != before[q]}))
@@ -96,7 +76,7 @@ def main():
         res = dict(
             what="esikf_map_device_update on the cfg2 frame (100k points, bench.py's map-leg sequence), A fixed at 2^19 roots, B growing from 2^12 roots, "
                  "alternating tick by tick; CUDA events on each context's stream",
-            **card(), ticks=args.ticks, n_pts=int(len(pts)),
+            **T.card(), ticks=args.ticks, n_pts=int(len(pts)),
             steady_ms_median={name: statistics.median([ms[name][k] for k in steady]) for name in ms} if steady else "not measured",
             steady_ms_min={name: min(ms[name][k] for k in steady) for name in ms} if steady else "not measured",
             steady_ticks=len(steady), growth_ticks=grew, b_grew_at_build={q: [start["B"][q], after_build[q]] for q in CAPS if after_build[q] != start["B"][q]},

@@ -8,7 +8,7 @@ bench.py's map-leg call sequence (BuildVoxelMap from the scan at the true pose, 
   shim   : two fl2b200::VoxelMapManager sessions, mirror on and off, tick by tick in turn: the host wall time of
            UpdateVoxelMap() (it returns after the device synchronised; with the mirror, export + apply are inside).
 
-Prints one JSON line with the card's name and power limit read in the same run.
+Prints one JSON line with the card's name, power limit and maximum SM clock read in the same run.
 
     python tools/map_mirror_timing.py [--ticks 30] [--out result.json]
 """
@@ -22,28 +22,14 @@ import time
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests"), os.path.join(ROOT, "tools")]
+import timing as T  # noqa: E402
 
 
-def _profiled_export(ctx, torch):
+def _profiled_export(ctx):
     """Kernel and device-to-host copy time (ms) of one esikf_map_device_export call, from torch.profiler's CUDA activity."""
-    from torch.profiler import ProfilerActivity, profile
-
-    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
-        ctx.map_device_export()
-        torch.cuda.synchronize()
-    kern = copy = 0.0
-    for e in prof.events():
-        if e.device_type != torch.autograd.DeviceType.CUDA:
-            continue
-        us = e.device_time if hasattr(e, "device_time") else e.cuda_time
-        if "memcpy" in e.name.lower() and "dtoh" in e.name.lower().replace(" ", ""):
-            copy += us
-        elif "map_export" in e.name or "DeviceScan" in e.name:
-            kern += us
-    return kern / 1e3, copy / 1e3
+    us = T.kernel_us(ctx.map_device_export, 1, ("Memcpy DtoH", "map_export", "DeviceScan"))
+    return (sum(us["map_export"]) + sum(us["DeviceScan"])) / 1e3, sum(us["Memcpy DtoH"]) / 1e3
 
 
 def main():
@@ -51,12 +37,9 @@ def main():
     ap.add_argument("--ticks", type=int, default=30)
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
+    T.require_gpu("map_mirror_timing")
     import torch
-
-    if not torch.cuda.is_available():
-        raise SystemExit("map_mirror_timing: no CUDA device (the numbers are GPU timings; there is no CPU fallback)")
     from fast_livo2_b200 import api, workloads
-    from map_growth_timing import card
     from map_mirror import session, shim_sessions, vp
 
     fr = workloads.frame("cfg2")
@@ -80,14 +63,12 @@ def main():
         for k in range(args.ticks):
             ctx.lio_update(pts, prior, prior, cfg)
             ctx.map_device_update()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record(stream)
-            exp = ctx.map_device_export()
-            e1.record(stream)
-            e1.synchronize()
-            kern_ms, d2h_ms = _profiled_export(ctx, torch)
+            got = []
+            (export_ms,), _ = T.per_call_ms(stream, lambda: got.append(ctx.map_device_export()), 1)
+            exp = got[0]
+            kern_ms, d2h_ms = _profiled_export(ctx)
             row = dict(tick=k, touched_roots=int(len(exp["keys"])), nodes=int(len(exp["nodes"])),
-                       bytes=int(exp["nodes"].nbytes + exp["keys"].nbytes + exp["first"].nbytes + exp["count"].nbytes), export_call_ms=e0.elapsed_time(e1),
+                       bytes=int(exp["nodes"].nbytes + exp["keys"].nbytes + exp["first"].nbytes + exp["count"].nbytes), export_call_ms=export_ms,
                        export_kernels_ms=kern_ms, export_d2h_ms=d2h_ms)
             for name, h in hs.items():  # mirror then plain, every tick
                 lio_out, vio_out, iters = np.zeros(386), np.zeros(386), np.zeros(2, np.int32)
@@ -104,7 +85,7 @@ def main():
     med = lambda key: statistics.median(r[key] for r in steady)
     res = dict(what="cfg2 frame (100k points), bench.py's map-leg sequence; export on a C-ABI context, UpdateVoxelMap() through two shim sessions "
                     "(mirror on / off) alternating tick by tick; medians over ticks 3..",
-               **card(), ticks=args.ticks, n_pts=int(len(pts)),
+               **T.card(), ticks=args.ticks, n_pts=int(len(pts)),
                median={k: med(k) for k in ("touched_roots", "nodes", "bytes", "export_call_ms", "export_kernels_ms", "export_d2h_ms", "update_voxel_map_mirror_ms",
                                            "update_voxel_map_plain_ms")},
                per_tick=rows)

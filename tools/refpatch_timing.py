@@ -11,7 +11,7 @@ For 2 k and 4 k points with k = 6, 15 and 30 observations:
             the same points (medians over --host-reps runs);
   upload  : the bytes the call copies to the device.
 
-Prints one JSON line with the card's name and power limit read in the same run.
+Prints one JSON line with the card's name, power limit and maximum SM clock read in the same run.
 
     python tools/refpatch_timing.py [--reps 50] [--host-reps 5] [--out result.json]
 """
@@ -26,9 +26,8 @@ import time
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests"), os.path.join(ROOT, "tools")]
+import timing as T  # noqa: E402
 
 SIZES = (2000, 4000)
 OBS = (6, 15, 30)
@@ -38,15 +37,8 @@ def _call(ctx, c):
     return ctx.vio_score_ref_patches(c["first"], c["pos"], c["normal"], c["patch"], c["mean"], c["id"], c["T"])
 
 
-def _kernel_ms(ctx, c, reps, torch):
-    from torch.profiler import ProfilerActivity, profile
-
-    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
-        for _ in range(reps):
-            _call(ctx, c)
-        torch.cuda.synchronize()
-    us = [e.device_time if hasattr(e, "device_time") else e.cuda_time for e in prof.events()
-          if e.device_type == torch.autograd.DeviceType.CUDA and "refpatch_score_kernel" in e.name]
+def _kernel_ms(ctx, c, reps):
+    us = T.kernel_us(lambda: _call(ctx, c), reps, ("refpatch_score_kernel",))["refpatch_score_kernel"]
     assert us, "no refpatch_score_kernel in the trace"
     return statistics.median(us) / 1e3
 
@@ -70,35 +62,23 @@ def main():
     ap.add_argument("--host-reps", type=int, default=5)
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
-    import torch
-
-    if not torch.cuda.is_available():
-        raise SystemExit("refpatch_timing: no CUDA device (the numbers are GPU timings; there is no CPU fallback)")
+    T.require_gpu("refpatch_timing")
     import refpatch_cases as RC
+    import torch
     from fast_livo2_b200 import api
     from fast_livo2_b200 import synthetic as S
-    from map_growth_timing import card
 
     ctx = api.Context(0)
     stream = torch.cuda.ExternalStream(ctx.stream)
-    res = dict(what="realistic observation sets (tests/refpatch_cases.realistic_case), k observations per point", **card(), rows=[])
+    res = dict(what="realistic observation sets (tests/refpatch_cases.realistic_case), k observations per point", **T.card(), rows=[])
     for n in SIZES:
         for k in OBS:
             c = RC.realistic_case(ctx, n, seed=n + k, lo=k, hi=k)
             m = len(c["patch"])
             for _ in range(5):
                 _call(ctx, c)
-            ev_ms, wall_ms = [], []
-            for _ in range(args.reps):
-                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                a.record(stream)
-                t0 = time.perf_counter()
-                _call(ctx, c)
-                wall_ms.append((time.perf_counter() - t0) * 1e3)
-                b.record(stream)
-                b.synchronize()
-                ev_ms.append(a.elapsed_time(b))
-            row = dict(points=n, obs_per_point=k, observations=m, kernel_ms=round(_kernel_ms(ctx, c, args.reps, torch), 4),
+            ev_ms, wall_ms = T.per_call_ms(stream, lambda: _call(ctx, c), args.reps)
+            row = dict(points=n, obs_per_point=k, observations=m, kernel_ms=round(_kernel_ms(ctx, c, args.reps), 4),
                        call_event_ms=round(statistics.median(ev_ms), 4), call_wall_ms=round(statistics.median(wall_ms), 4),
                        upload_bytes=int(m * (64 * 4 + 4 + 4 + 12 * 8) + n * (6 * 8 + 4) + 4),
                        orc_host_ms=round(statistics.median(_orc_ms(c) for _ in range(args.host_reps)), 3))

@@ -8,20 +8,21 @@ restatement of vio.cpp:386-428 + 605-640 (oracle/orc_retrieve.cpp, the reference
   kernels      : the device time of the kernels alone, from a torch.profiler run of its own, per tick
   host loop    : orc_retrieve_scan + orc_depth_check, one thread
 
-The device's keys, depth image and flags are checked against the oracle's. The card's name and power limit are printed in the
+The device's keys, depth image and flags are checked against the oracle's. The card's name, power limit and maximum SM clock are printed in the
 same run. Writes nothing; needs a GPU.
 
   python tools/retrieve_scan_timing.py [--reps 30]"""
 import argparse
+import json
 import os
-import subprocess
 import sys
 import time
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests"), os.path.join(ROOT, "tools")]
+import timing as T  # noqa: E402
 import torch  # noqa: E402
 
 import retrieve_cases as RC  # noqa: E402
@@ -35,15 +36,7 @@ def timed(ctx, stream, fn, reps):
     for _ in range(3):
         fn()
     ctx.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    t0 = time.perf_counter()
-    e0.record(stream)
-    for _ in range(reps):
-        fn()
-    e1.record(stream)
-    ctx.synchronize()
-    e1.synchronize()
-    return e0.elapsed_time(e1) / reps, (time.perf_counter() - t0) / reps * 1e3
+    return T.window_ms(stream, fn, reps)
 
 
 def resident_scan(ctx, sc):
@@ -65,10 +58,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=30)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("needs a CUDA device")
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    print(f"device: {q.splitlines()[0] if q else torch.cuda.get_device_name(0)}")
+    T.require_gpu("retrieve_scan_timing")
+    print(f"device: {json.dumps(T.card())}")
     ctx = api.Context(0)
     stream = torch.cuda.ExternalStream(ctx.stream)
     for n in (100_000, 300_000):
@@ -90,20 +81,7 @@ def main():
         ev, wall = timed(ctx, stream, host_call, args.reps)
         print(f"n={n} api host buffers (retrieve_scan + depth_check of {len(pos)} points)  events {ev:.3f} ms/tick  host {wall:.3f} ms/tick  keys={len(want['keys'])}")
 
-        from torch.profiler import ProfilerActivity, profile
-
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            for _ in range(args.reps):
-                host_call()
-            ctx.synchronize()
-        per = {k: 0.0 for k in KERNELS}
-        for e in prof.events():
-            if e.device_type != torch.autograd.DeviceType.CUDA:
-                continue
-            for k in KERNELS:
-                if k in e.name:
-                    per[k] += e.device_time if hasattr(e, "device_time") else e.cuda_time
-                    break
+        per = {k: sum(v) for k, v in T.kernel_us(host_call, args.reps, KERNELS).items()}
         tot = sum(per.values()) / args.reps
         print(f"n={n} kernels {tot / 1e3:.4f} ms/tick: " + ", ".join(f"{k} {v / args.reps:.1f} us" for k, v in per.items()))
 

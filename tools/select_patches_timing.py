@@ -7,19 +7,19 @@
              and gate loop on the host (numpy, the reference's per-candidate arithmetic) and esikf_vio_set_patches of the survivors
 
 Both are timed with CUDA events on the context's stream and with the host clock, around calls that end in a device
-synchronise, and the kept sets of the two paths are checked to be equal. The card's name and power limit are printed in the same run. Writes nothing; needs a GPU.
+synchronise, and the kept sets of the two paths are checked to be equal. The card's name, power limit and maximum SM clock are printed in the same run. Writes nothing; needs a GPU.
 
   python tools/select_patches_timing.py [--reps 50]"""
 import argparse
+import json
 import os
-import subprocess
 import sys
-import time
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests"), os.path.join(ROOT, "tools")]
+import timing as T  # noqa: E402
 import torch  # noqa: E402
 
 import select_cases as SC  # noqa: E402
@@ -41,10 +41,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=50)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("needs a CUDA device")
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    print(f"device: {q.splitlines()[0] if q else torch.cuda.get_device_name(0)}")
+    T.require_gpu("select_patches_timing")
+    print(f"device: {json.dumps(T.card())}")
     ctx = api.Context(0)
     stream = torch.cuda.ExternalStream(ctx.stream)
     for n in (2000, 4000):
@@ -68,19 +66,11 @@ def main():
 
         for name, fn in (("select", lambda: sel(thr)), ("replaced", replaced)):
             for _ in range(5):
-                fn()
-            ctx.synchronize()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            t0 = time.perf_counter()
-            e0.record(stream)
-            for _ in range(args.reps):
                 r = fn()
-            e1.record(stream)
             ctx.synchronize()
-            e1.synchronize()
-            wall = (time.perf_counter() - t0) / args.reps * 1e3
+            ev, wall = T.window_ms(stream, fn, args.reps)
             kept = len(r["kept"]) if isinstance(r, dict) else len(r)
-            print(f"n={n} {name:8s} kept={kept:5d}  events {e0.elapsed_time(e1) / args.reps:.3f} ms/call  host {wall:.3f} ms/call")
+            print(f"n={n} {name:8s} kept={kept:5d}  events {ev:.3f} ms/call  host {wall:.3f} ms/call")
         # both paths select the same sub-map (same warps, same current patches, the reference's error arithmetic)
         assert np.array_equal(sel(thr)["kept"], replaced()), "the two timed paths kept different candidates"
     ctx.close()

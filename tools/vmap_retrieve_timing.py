@@ -9,20 +9,21 @@ and the scan keys of one frame, against host walks on the same frames:
   reference   : the reference source's own retrieveFromVisualSparseMap (oracle/_ref/libfl2_ref_vretrieve.so, where it was
                 built), the whole retrieval with its scan side and the per-point warps after the choice
 
-The device's cells are checked against the restatement first. The card's name and power limit are printed in the same run.
+The device's cells are checked against the restatement first. The card's name, power limit and maximum SM clock are printed in the same run.
 Writes nothing; needs a GPU.
 
   python tools/vmap_retrieve_timing.py [--reps 30]"""
 import argparse
+import json
 import os
-import subprocess
 import sys
 import time
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests"), os.path.join(ROOT, "tools")]
+import timing as T  # noqa: E402
 import torch  # noqa: E402
 
 import retrieve_cases as RC  # noqa: E402
@@ -37,8 +38,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=30)
     args = ap.parse_args()
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    print("card:", q)
+    T.require_gpu("vmap_retrieve_timing")
+    print("card:", json.dumps(T.card()))
     for n_vis in (20_000, 100_000, 400_000):
         sc = RC.scene("pinhole", max(n_vis, 100_000), seed=11, n_vis=n_vis)
         n = len(sc["pos"])
@@ -50,10 +51,10 @@ def main():
             ctx.vmap_init(n)
             first = np.concatenate([[0], np.cumsum(sc["n_obs"])]).astype(np.int32)
             m = int(first[-1])
-            T = np.zeros((m, 12))
-            T[:, [0, 4, 8]] = 1.0
+            T_f_w = np.zeros((m, 12))
+            T_f_w[:, [0, 4, 8]] = 1.0
             rng = np.random.default_rng(2)
-            ctx.vmap_add_points(first, np.zeros((m, 2)), rng.uniform(0, 255, (m, 64)).astype(np.float32), T, (np.arange(m) % 3).astype(np.int32),
+            ctx.vmap_add_points(first, np.zeros((m, 2)), rng.uniform(0, 255, (m, 64)).astype(np.float32), T_f_w, (np.arange(m) % 3).astype(np.int32),
                                 np.zeros(m, np.float32), np.zeros(m, np.float32), np.full(n, -1, np.int32))
             ctx.vmap_place_points(order, sc["pos"][order])
             dev = ctx.vio_retrieve_scan(sc["border"], pg=sc["pg"], state=sc["state"], depth=True)
@@ -68,29 +69,9 @@ def main():
             stream = torch.cuda.ExternalStream(ctx.stream)
             for _ in range(3):
                 call()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            t0 = time.perf_counter()
-            e0.record(stream)
-            for _ in range(args.reps):
-                call()
-            e1.record(stream)
-            e1.synchronize()
-            wall = (time.perf_counter() - t0) / args.reps * 1e3
-            print(f"points={n} keys={len(walk)} cells={len(got['cell'])}  call: events {e0.elapsed_time(e1) / args.reps:.3f} ms  host {wall:.3f} ms")
-            from torch.profiler import ProfilerActivity, profile
-
-            with profile(activities=[ProfilerActivity.CUDA]) as prof:
-                for _ in range(args.reps):
-                    call()
-                ctx.synchronize()
-            per = {k: 0.0 for k in KERNELS}
-            for e in prof.events():
-                if e.device_type != torch.autograd.DeviceType.CUDA:
-                    continue
-                for k in KERNELS:
-                    if k in e.name:
-                        per[k] += e.device_time if hasattr(e, "device_time") else e.cuda_time
-                        break
+            ev, wall = T.window_ms(stream, call, args.reps)
+            print(f"points={n} keys={len(walk)} cells={len(got['cell'])}  call: events {ev:.3f} ms  host {wall:.3f} ms")
+            per = {k: sum(v) for k, v in T.kernel_us(call, args.reps, KERNELS).items()}
             print(f"points={n} kernels {sum(per.values()) / args.reps / 1e3:.4f} ms/call: " + ", ".join(f"{k} {v / args.reps:.1f} us" for k, v in per.items()))
             s2 = dict(sc, **vis)
             t0 = time.perf_counter()
@@ -100,7 +81,7 @@ def main():
             if VR.ref_vretrieve_available():
                 ref = VR.RefVretrieve(sc)
                 tk = dict(order=order, ids=np.arange(n, dtype=np.int32), first=first, pos=sc["pos"], normal=sc["normal"], ninit=np.ones(n, np.uint8),
-                          patch=np.zeros((m, 64), np.float32), fid=(np.arange(m) % 3).astype(np.int32), T=T)
+                          patch=np.zeros((m, 64), np.float32), fid=(np.arange(m) % 3).astype(np.int32), T=T_f_w)
                 ref.place(tk)
                 ref.retrieve(sc, True)
                 t0 = time.perf_counter()

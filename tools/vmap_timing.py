@@ -5,30 +5,25 @@
 
 Call times: CUDA events on the context's stream around the call (median of `reps`); the call enqueues its uploads, kernels
 and readback there and synchronises before it returns. Kernel times:
-torch.profiler with CUDA activities in a separate pass (sum of the call's kernels, averaged per call). The card's name and
-power limit are read in the same run.
+torch.profiler with CUDA activities in a separate pass (sum of the call's kernels, averaged per call). The card's name,
+power limit and maximum SM clock are read in the same run.
 
   python tools/vmap_timing.py [--reps 30] [--out results.json]
 """
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests"), os.path.join(ROOT, "tools")]
+import timing as T  # noqa: E402
 
 import observe_cases as OC  # noqa: E402
 from fast_livo2_b200 import api  # noqa: E402
 from fast_livo2_b200 import synthetic as S  # noqa: E402
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    return q.splitlines()[0] if q else "unknown"
 
 
 def lists(rng, n, k):
@@ -44,31 +39,16 @@ def lists(rng, n, k):
 def call_ms(ctx, f, reps):
     import torch
 
-    st = torch.cuda.ExternalStream(ctx.stream)
     f()
-    ts = []
-    for _ in range(reps):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record(st)
-        f()
-        b.record(st)
-        b.synchronize()
-        ts.append(a.elapsed_time(b))
-    return float(np.median(ts))
+    return float(np.median(T.per_call_ms(torch.cuda.ExternalStream(ctx.stream), f, reps)[0]))
 
 
 def kernel_ms(f, reps):
     import torch
-    from torch.profiler import ProfilerActivity, profile
 
     f()
     torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for _ in range(reps):
-            f()
-        torch.cuda.synchronize()
-    us = sum(e.device_time_total for e in prof.key_averages() if e.device_type.name == "CUDA" and "Memcpy" not in e.key and "Memset" not in e.key)
-    return us / reps / 1e3
+    return sum(sum(us) for us in T.kernel_us(f, reps).values()) / reps / 1e3
 
 
 def main():
@@ -76,13 +56,10 @@ def main():
     ap.add_argument("--reps", type=int, default=30)
     ap.add_argument("--out", default=None, help="also write the results as JSON here")
     a = ap.parse_args()
-    import torch
-
-    if not torch.cuda.is_available():
-        sys.exit("no CUDA device: these are GPU timings")
+    T.require_gpu("vmap_timing")
     ctx = api.Context(0)
     rng = np.random.default_rng(0)
-    out = dict(card=card(), score=[], update=[])
+    out = dict(card=T.card(), score=[], update=[])
     for n in (2000, 4000):
         for k in (6, 15, 30):
             L = lists(rng, n, k)
